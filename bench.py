@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — events/sec through EventBus.Publish on B200 (BASELINE.json metric).
+"""bench.py — events/sec through EventBus.Publish on H100 (BASELINE.json metric).
 
 A "step" is one pass of the hot path over one batch: `batch` published events fanned out to every subscriber mailbox of
 every GPU's shard (one fan-out kernel launch per GPU).  Headline unit (BASELINE.md §3): deliveries/s = 32-byte records
@@ -7,13 +7,14 @@ landed in mailboxes per second, whole job; publishes/s is reported beside it.
 
   python bench.py [--gpus N --steps K --warmup W] [--workload default|config2|config3|config5]
   python bench.py --impl reference ...      # the reference's CPU path (restated Go bus) on the host cores
+  python bench.py ... --dump-outputs DIR     # also write what the last timed step computed, as DIR/<name>.npy
 
 Default: the headline is BASELINE config 3 — the configuration north_star's target is quoted on (1,048,576 subscribers
 per GPU, 1 kHz timer per subscriber; at --gpus 8 this IS config 4: 8,388,608 subscribers sharded evenly) — and configs 2
 and 5 are measured in the same run and printed under "extra_configs", each with its own roofline / e2e / parity check.
 Every configuration is verified after its timed regions (sampled subscribers bit-exact against a 1-subscriber oracle over
 the exact trace the bench issued, the shard's total count in closed form, the digest fold across ranks); a mismatch
-fails the run (rc != 0).  One JSON line on stdout (rank 0).  Nothing here reads /root/reference.
+fails the run (rc != 0).  One JSON line on stdout (rank 0).  Nothing here reads the reference project.
 """
 from __future__ import annotations
 
@@ -34,10 +35,10 @@ METRIC = "events/sec through Bus.Publish (deliveries/s = 32-byte records landed 
 WORKLOADS = {
     # BASELINE.json configs[1]
     "config2": dict(subs=65_536, events=10_000_000, timers=0, zipf=None, scaling="weak",
-                    desc="1xB200: 65,536 subscribers, 10M-event synthetic trace, 32-byte records, all-ones masks"),
+                    desc="1xH100: 65,536 subscribers, 10M-event synthetic trace, 32-byte records, all-ones masks"),
     # configs[2] (and configs[3] = the same shard on each of 8 GPUs): the configuration north_star's target is quoted on
     "config3": dict(subs=1_048_576, events=100_000_000, timers=1, zipf=None, scaling="weak",
-                    desc="1xB200: 1,048,576 subscribers, 100M events (prefix timed), Timer ticks interleaved at 1 kHz"),
+                    desc="1xH100: 1,048,576 subscribers, 100M events (prefix timed), Timer ticks interleaved at 1 kHz"),
     # configs[4]: Zipf-skewed masks over 16 codes, TOTAL subscriber count fixed as GPUs are added (strong scaling)
     "config5": dict(subs=1_048_576, events=10_000_000, timers=0, zipf=1.0, scaling="strong",
                     desc="filter sweep: 1,048,576 subscribers in total, 16 event codes, Zipf(s=1.0) masks and codes"),
@@ -49,11 +50,12 @@ TICK_NS = 1_000_000       # 1 kHz
 def parse():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=0, help="batches to time (0 = the workload's whole trace, capped)")
+    ap.add_argument("--steps", type=int, default=0,
+                    help="batches to time in every timed leg (0 = the workload's whole trace, capped; the e2e leg then times 4000)")
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--impl", default="cpbus", choices=["cpbus", "reference"])
     ap.add_argument("--workload", default="default", choices=["default"] + sorted(WORKLOADS))
-    ap.add_argument("--batch", type=int, default=512, help="events per step (<= ring/2); 512 measured best: config 2 +1.5 %, config 3 +8 % over 256")
+    ap.add_argument("--batch", type=int, default=512, help="events per step (<= ring/2)")
     ap.add_argument("--ring", type=int, default=1024)
     ap.add_argument("--subs", type=int, default=0, help="override subscribers per GPU")
     ap.add_argument("--store", type=int, default=0, help="0 auto, 1 v4, 2 v8, 3 TMA bulk")
@@ -64,6 +66,9 @@ def parse():
     ap.add_argument("--no-extras", action="store_true", help="default workload: headline only")
     ap.add_argument("--no-verify", action="store_true", help="skip the in-bench oracle check (diagnostics only; the line says so)")
     ap.add_argument("--max-steps", type=int, default=40_000)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps of each throughput configuration, write what the last one computed (seeded sample of "
+                         "mailboxes, at most 64 MB in all) as DIR/<name>.npy; the lossless and bridge legs are not dumped")
     return ap.parse_args()
 
 
@@ -304,16 +309,13 @@ def run_config(cx, name: str, headline: bool):
     sampler = ClockSampler(local)
     sampler.start()                                            # started early so NVML is warm before the timed region
     run_steps(warmup)
-    # settle: a fresh box pages in driver/library code lazily; keep warming (untimed) for ~0.3 s of wall clock
-    settle, t_settle = 0, time.perf_counter()
+    # settle: a fresh box pages in driver/library code lazily; keep warming (untimed) for ~1 TiB of record writes (about
+    # 0.3 s on one H100).  A fixed step count, not a wall-clock budget: the same arguments then give the same inputs to
+    # every timed step on every run and every build, so that --dump-outputs can be compared output for output.
     settle_chunk = 100 if n_subs <= 131_072 else 10
-    while settle < 20_000:
-        run_steps(settle_chunk); torch.cuda.synchronize(); settle += settle_chunk
-        done = time.perf_counter() - t_settle >= 0.3
-        if world > 1:                                          # every rank issues the same number of steps: rank 0's clock decides
-            t_ = torch.tensor([1 if done else 0], device=dev); dist.broadcast(t_, src=0); done = bool(int(t_.item()))
-        if done:
-            break
+    settle = min(20_000, -(-(1 << 40) // (n_subs * B * 32)))
+    for done in range(0, settle, settle_chunk):
+        run_steps(min(settle_chunk, settle - done)); torch.cuda.synchronize()
     # if the timed region would straddle the end of the trace, start it at the next cycle instead (re-stamp outside the timing)
     pos = state["step"] % n_trace_batches
     if steps <= n_trace_batches and pos + steps > n_trace_batches:
@@ -331,6 +333,9 @@ def run_config(cx, name: str, headline: bool):
     sampler.stop_flag = True
     ms_local = e0.elapsed_time(e1)
     st1 = bus.stats()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, name if world == 1 else f"{name}_rank{rank}", bus, first, n_subs, state["step"] - 1, B,
+                     n_dumps=cx.n_configs * world)
     t = torch.tensor([ms_local], dtype=torch.float64, device=dev)
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -348,7 +353,7 @@ def run_config(cx, name: str, headline: bool):
     if os.path.exists(peaks_path):
         peak, peak_src = float(json.load(open(peaks_path))["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (of measured)"
     else:
-        peak, peak_src = 6650.0, "B200_PROFILING.md fallback (of fallback)"
+        peak, peak_src = 3350.0, "NVIDIA H100 SXM data sheet, 3.35 TB/s HBM3 (not measured)"
     d_local = (st1["deliveries"] - st0["deliveries"]) / steps        # records per launch on this GPU
     # algorithmic bytes per launch (DESIGN.md §4.1): every delivered record is one 32-byte sector; every mailbox's 32-byte
     # control block is read once and written once; an armed timer slot costs its 16-byte hot half read plus, when it fires,
@@ -357,24 +362,16 @@ def run_config(cx, name: str, headline: bool):
     alg_bytes = 32.0 * d_local + n_subs * per_sub_state + B * 32
     kernel_ms = float(ms_local) / steps                              # this rank's launches are back to back on the stream
     achieved = alg_bytes / (kernel_ms * 1e-3) / 1e9
-    traffic = None
-    tp = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(tp):
-        try:
-            traffic = (json.load(open(tp)).get(name) or {}).get(str(B))
-        except Exception:
-            traffic = None
     roofline = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                "traffic": traffic, "kernel": "cpbus_dev::fanout_kernel", "alg_bytes_per_launch": alg_bytes,
+                "kernel": "cpbus_dev::fanout_kernel", "alg_bytes_per_launch": alg_bytes,
                 "record_bytes_per_launch": 32.0 * d_local, "state_bytes_per_launch": float(n_subs * per_sub_state + B * 32),
                 "kernel_ms": kernel_ms, "peak_source": peak_src}
 
     # ---- end to end through the public C-ABI with HOST buffers: `e2e` ----
     e2e, launches_e2e = None, 0
     if not args.no_e2e:
-        k2 = min(steps, 4000)
+        k2 = steps if args.steps else min(steps, 4000)         # --steps sets this leg's timed steps too
         jump_to_next_cycle()                                   # the host leg starts on a fresh trace cycle (clock keeps increasing)
-        k2 = min(k2, n_trace_batches - 8)
         host = base                                            # events as a caller holds them (host memory): code + source are read
         nxt = state["step"]
         tickets = []                                           # result reads are pipelined two steps deep
@@ -475,13 +472,48 @@ def run_config(cx, name: str, headline: bool):
                    "digest": not args.no_digest, "timers_per_sub": K_timers, "warmup_settle_steps": settle, "store_path": args.store,
                    "parallelism": f"subscriber shards x{world}" + (f", ingest: {ingest_mode}" if world > 1 else ""),
                    "l2": f"inputs larger than L2: {n_subs * R * 32 / 2**30:.1f} GiB of rings per GPU, "
-                         f"{d_local * 32 / 2**20:.0f} MiB written per step vs 126 MB L2",
+                         f"{d_local * 32 / 2**20:.0f} MiB written per step vs {torch.cuda.get_device_properties(dev).L2_cache_size / 1e6:.0f} MB L2",
                    "trace": f"splitmix-seeded {'Zipf' if wl['zipf'] else 'uniform'} codes 1..16, 4096 sources, {n_trace_batches} batches cycled with re-stamped seq/ts"},
         "roofline": roofline, "e2e": e2e, "cpu_baseline": cpu, "gpu_launches": int(launches), "gpu_launches_e2e": int(launches_e2e),
         "clocks": sampler.summary(), "parity_checked": bool(parity and parity["ok"]) if parity is not None else False,
         "parity": parity if parity is not None else {"skipped": "--no-verify"},
     }
     return res
+
+
+DUMP_SUBS = 128                 # mailboxes sampled by --dump-outputs (fixed seed), fewer where the 64 MB budget needs it
+DUMP_BUDGET = 60_000_000       # bytes of .npy files over all configurations and ranks (the cap is 64 MB)
+
+
+def dump_outputs(out_dir: str, name: str, bus, first: int, n_subs: int, last_step: int, B: int, n_dumps: int):
+    """What the timed path handed its caller for the last timed step, as float64 .npy files (32-bit halves where a value
+    needs 64 bits): the step result of the launch (<name>_step_result: deliveries, ticks, digest-sum hi/lo, launch
+    ordinal) and, for a seeded sample of mailboxes, the records that step appended (<name>_records: subscriber, position
+    in the step, seq hi/lo, ts hi/lo, code, source_id, target, flags) and the control blocks after it (<name>_mailboxes:
+    subscriber, count hi/lo, digest hi/lo)."""
+    os.makedirs(out_dir, exist_ok=True)
+    res = bus.step_result_end(bus.step_result_begin())
+    rng = np.random.default_rng(0xD0B5 + first)
+    # a step appends at most B events + 32 timer firings to a mailbox: 10 float64 columns each, plus 5 per mailbox row
+    per_sub = (B + 32) * 10 * 8 + 5 * 8
+    n_pick = max(2, min(DUMP_SUBS, DUMP_BUDGET // (n_dumps * per_sub)))
+    subs = np.unique(np.concatenate([[0, n_subs - 1], rng.integers(0, n_subs, n_pick - 2)])) + first
+    wm_prev = last_step * B * DT_NS                               # records due/stamped after the previous watermark
+    recs, boxes = [], []
+    for s in subs:
+        w = bus.peek_window(int(s))
+        w = w[w["ts_ns"] > wm_prev]
+        cols = [np.full(len(w), s), np.arange(len(w)), w["seq"] >> 32, w["seq"] & 0xFFFFFFFF, w["ts_ns"] >> 32,
+                w["ts_ns"] & 0xFFFFFFFF, w["code"], w["source_id"], w["target"], w["flags"]]
+        recs.append(np.stack([np.asarray(c, dtype=np.float64) for c in cols], axis=1))
+        d = bus.digests(int(s), 1)[0]
+        c, g = int(d["count"]), int(d["digest"])
+        boxes.append([s, c >> 32, c & 0xFFFFFFFF, g >> 32, g & 0xFFFFFFFF])
+    split = lambda x: [int(x) >> 32, int(x) & 0xFFFFFFFF]
+    np.save(os.path.join(out_dir, f"{name}_step_result.npy"),
+            np.array([res[0], res[1], *split(res[2]), res[3]], dtype=np.float64))
+    np.save(os.path.join(out_dir, f"{name}_records.npy"), np.concatenate(recs))
+    np.save(os.path.join(out_dir, f"{name}_mailboxes.npy"), np.array(boxes, dtype=np.float64))
 
 
 def run_lossless_and_bridge(cx):
@@ -651,6 +683,7 @@ def main():
     names = ["config3", "config2", "config5"] if args.workload == "default" else [args.workload]
     if args.no_extras:
         names = names[:1]
+    cx.n_configs = len(names)
     results = [run_config(cx, n, headline=(i == 0)) for i, n in enumerate(names)]
     ok = all(r["parity_checked"] for r in results) or args.no_verify
     side = []

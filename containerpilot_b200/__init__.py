@@ -1,7 +1,7 @@
-"""cpbus — a B200-native event bus behind ContainerPilot's `events` API.
+"""cpbus — an H100-native event bus behind ContainerPilot's `events` API.
 
 Package layout (only what the hot path needs):
-  csrc/cpbus_kernels.cuh   sm_100a kernels (fan-out, admission, digest fold)
+  csrc/cpbus_kernels.cuh   sm_90a kernels (fan-out, admission, digest fold)
   csrc/cpbus.cu            C-ABI implementation (include/cpbus.h) -> libcpbus.so
   _native.py               ctypes binding of the C-ABI (no fallback)
   bus.py                   numpy-friendly `Bus` wrapper, 1:1 with cpbus_*

@@ -140,7 +140,7 @@ def load() -> C.CDLL:
         if not os.path.exists(LIB_PATH):
             raise ImportError(
                 f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a). There is no CPU fallback.")
+                "(nvcc, sm_90a). There is no CPU fallback.")
         lib = C.CDLL(LIB_PATH)
         for name, (res, args) in SYMBOLS.items():
             fn = getattr(lib, name)   # AttributeError if the .so does not export a declared symbol

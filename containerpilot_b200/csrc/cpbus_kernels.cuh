@@ -1,4 +1,4 @@
-// cpbus_kernels.cuh — sm_100a kernels of the event bus hot path.
+// cpbus_kernels.cuh — sm_90a (H100) kernels of the event bus hot path.
 //
 // Replaces the inner loop of EventBus.Publish (reference events/bus.go:134-138:
 // `for subscriber := range bus.registry { subscriber.Receive(event) }`, one
@@ -10,8 +10,8 @@
 // cores.  One warp owns one subscriber (mailbox) at a time; the batch of 32-byte
 // records is staged once per CTA into shared memory with a 1-D TMA bulk copy
 // (cp.async.bulk + mbarrier); matches are found with warp ballots; every record
-// is written as one full, aligned 32-byte sector (st.global.v8.b32 or a v4 pair)
-// or, for dense runs, by TMA bulk stores straight out of the staged batch.
+// is written as one full, aligned 32-byte sector (two 16-byte stores from one lane, or
+// a lane pair) or, for dense runs, by TMA bulk stores straight out of the staged batch.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -22,45 +22,43 @@ namespace cpbus_dev {
 
 constexpr int kWarpsPerCta = 8;
 constexpr int kThreads = kWarpsPerCta * 32;
-// Every variant of the fan-out kernel is held to 64 registers with zero spills => 4 CTAs (32 warps) per SM.
-// Occupancy was the biggest single lever (DESIGN.md §4.1); the macro exists for A/B builds.
+// Every variant of the fan-out kernel is held to 64 registers => 4 CTAs (32 warps) per SM.  ptxas (CUDA 12.9, sm_90a) spills
+// nothing in the dense, ORDERED and no-digest timers variants, 4-14 bytes in the timers + digest variants and 52-140 bytes
+// in the PAIRS variants.  Occupancy is the biggest single lever (DESIGN.md §4.1); the macro exists for A/B builds.
 #ifndef CPBUS_CTAS_PER_SM
 #define CPBUS_CTAS_PER_SM 4
 #endif
-// A/B build switches (scripts/gpu_ab.sh builds variants with -D...=0/1 and times them on one box; defaults = best measured)
+// A/B build switches (build variants with -D...=0/1 and time them on one GPU; the defaults are the chosen variants)
 #ifndef CPBUS_SWIZZLE
 #define CPBUS_SWIZZLE 2      // shared-memory record reads with lanes 4-7 of each quarter warp fetching their halves in swapped order:
-                             // 0 = never, 1 = every path, 2 = only the gathered reads of the filtered path in the ORDERED build.
-                             // Measured (profiles/r02_ab_kernel_variants.md): the swizzle removes the bank conflicts everywhere, but on
-                             // the dense paths the two extra live registers per record cost more than the conflicts did
-                             // (config 2: 154 -> 166 us per launch, config 3: 2741 -> 2836); on the gathered reads it gains 1 %.
+                             // 0 = never, 1 = every path, 2 = only gathered reads.  Only lds_record uses it, i.e. the per-lane
+                             // reads of the CPBUS_ORD_RUNS variant; every other path copies records with copy_record_pairs.
+                             // The swizzle removes the bank conflicts everywhere, but on the dense paths the two extra live
+                             // registers per record cost more than the conflicts do.
 #endif
 #ifndef CPBUS_TICKS_REG
 #define CPBUS_TICKS_REG 1    // dense+ticks copy loop: tick positions in registers (ballots) instead of shared-memory loads
 #endif
 #ifndef CPBUS_COLD_EARLY
-#define CPBUS_COLD_EARLY 1   // (+1 % on config 3 once the loop is not unrolled) cold half of the timer slot loaded before the copy loop instead of after it
+#define CPBUS_COLD_EARLY 1   // cold half of the timer slot loaded before the copy loop instead of after it
 #endif
 #ifndef CPBUS_UNROLL2
-#define CPBUS_UNROLL2 1      // dense+ticks loop: two 32-event chunks per iteration (with planar staging: config 3 2647 -> 2640 us, r2v)
+#define CPBUS_UNROLL2 1      // dense+ticks loop: two 32-event chunks per iteration
 #endif
 #ifndef CPBUS_EARLY_PF
-#define CPBUS_EARLY_PF 0     // (measured: neutral) prefetch.L2 of the warp's first control block / timer slot at kernel entry
+#define CPBUS_EARLY_PF 0     // prefetch.L2 of the warp's first control block / timer slot at kernel entry
 #endif
 #ifndef CPBUS_ORD_PF
-#define CPBUS_ORD_PF 0       // (measured: -1.3 % on config 5) ORDERED build: prefetch.L2 of the whole block's control blocks once the ids are known
-#endif
-#ifndef CPBUS_IDX_PF
-#define CPBUS_IDX_PF 1       // filtered path, pass 2: read the index list one iteration ahead (measured: -0.35 % on config 5)
+#define CPBUS_ORD_PF 0       // ORDERED build: prefetch.L2 of the whole block's control blocks once the ids are known
 #endif
 #ifndef CPBUS_PLANAR
 #define CPBUS_PLANAR 1       // the staged batch is re-laid in shared memory as two 16-byte planes (lo[i] = bytes 0-15 of record i, hi[i] =
 #endif                       // bytes 16-31) before the copy loops: a lane's two LDS.128 are then conflict-free on the dense paths with no
-                             // select and no extra register (VERDICT round 1 item 4; the lane-swapped reads of CPBUS_SWIZZLE cost registers)
+                             // select and no extra register (the lane-swapped reads of CPBUS_SWIZZLE cost registers)
 #ifndef CPBUS_ORD_RUNS
 #define CPBUS_ORD_RUNS 0     // ORDERED build: process runs of equal masks as a unit (records read once, stored to every ring of the run).
-                             // Measured (profiles/r02_ab_kernel_variants.md, table 5): bit-exact, but 5.7 % SLOWER on config 5 — the rings then
-                             // receive 1-2 KiB per visit instead of one contiguous 7.7 KiB append, and that costs more than the saved gathers.
+                             // Bit-exact, but off by default: the rings then receive 1-2 KiB per visit instead of one contiguous
+                             // multi-KiB append, which can cost more than the saved gathers.
 #endif
 constexpr uint32_t kActiveBit = 0x80000000u;   // mask word: subscriber is subscribed
 constexpr int kTimerHintShift = 24;            // mask word bits 24..27: #timer slots to look at
@@ -92,7 +90,7 @@ struct __align__(32) DevTimer {
 constexpr uint64_t kTimerIdle = ~0ull;
 
 // Statistics are spread over kStatSlots sector-sized slots: same-address REDs serialise at
-// L2 (~2.7 ns each, measured: 65,536 warps -> +180 us per launch), distinct sectors do not.
+// L2, distinct sectors do not.
 constexpr int kStatSlots = 256;
 struct __align__(32) DevStatSlot { unsigned long long deliveries, ticks, pad[2]; };
 struct DevStats {
@@ -225,19 +223,32 @@ __device__ __forceinline__ uint64_t warp_sum64(uint64_t v) {
   }
   return v;
 }
-// one full 32-byte sector per instruction (SASS: STG.E.ENL2.256)
-__device__ __forceinline__ void st_v8(void* dst, const uint4& a, const uint4& b) {
-  asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(dst), "r"(a.x), "r"(a.y), "r"(a.z),
-               "r"(a.w), "r"(b.x), "r"(b.y), "r"(b.z), "r"(b.w)
-               : "memory");
-}
 __device__ __forceinline__ void st_v4(void* dst, const uint4& a) {
   asm volatile("st.global.v4.b32 [%0], {%1,%2,%3,%4};" ::"l"(dst), "r"(a.x), "r"(a.y), "r"(a.z), "r"(a.w) : "memory");
 }
-template <int STORE>
-__device__ __forceinline__ void st_record(cpbus_event* dst, const uint4& a, const uint4& b) {
-  if (STORE == CPBUS_STORE_V8) st_v8(dst, a, b);
-  else { st_v4(dst, a); st_v4(reinterpret_cast<unsigned char*>(dst) + 16, b); }
+// one full 32-byte sector per lane.  sm_90 has no 256-bit global store: the sector is written as two back-to-back
+// 16-byte stores from the same lane, which L2 merges into one full-sector write (no read-for-ownership).
+__device__ __forceinline__ void st_v8(void* dst, const uint4& a, const uint4& b) {
+  st_v4(dst, a);
+  st_v4(reinterpret_cast<unsigned char*>(dst) + 16, b);
+}
+// Warp-cooperative copy of staged records into a ring: lane l copies staged record i to ring slot (tail + out) & Rm if
+// `valid`.  Every lane of the warp must call it.  One lane storing both 16-byte halves of its record leaves each store
+// instruction with 32 half-filled sectors, and H100 then sustains about half of the lane-pair rate.  So the two lanes of
+// a pair copy one record per instruction together, each lane loading from shared memory the half it stores: each of the
+// two store instructions fills 16 whole 32-byte sectors.  Staged layout: planar (PL: half h of record i at s4[h * hi + i])
+// or record-major (s4[2 * i + h]).
+template <bool PL>
+__device__ __forceinline__ void copy_record_pairs(const uint4* s4, uint32_t hi, cpbus_event* ring, uint32_t tail, uint32_t Rm,
+                                                  uint32_t i, uint32_t out, bool valid) {
+  const uint32_t h = threadIdx.x & 1u, ev = (threadIdx.x & 31u) & ~1u;
+  const uint32_t pi = __shfl_xor_sync(0xffffffffu, i, 1), po = __shfl_xor_sync(0xffffffffu, out, 1);
+  const uint32_t vm = __ballot_sync(0xffffffffu, valid);
+  const uint32_t ie = h ? pi : i, oe = h ? po : out, io = h ? i : pi, oo = h ? out : po;   // the even / odd lane's record
+  if ((vm >> ev) & 1u)
+    st_v4(reinterpret_cast<unsigned char*>(ring + ((tail + oe) & Rm)) + 16u * h, PL ? s4[h * hi + ie] : s4[2u * ie + h]);
+  if ((vm >> (ev + 1u)) & 1u)
+    st_v4(reinterpret_cast<unsigned char*>(ring + ((tail + oo) & Rm)) + 16u * h, PL ? s4[h * hi + io] : s4[2u * io + h]);
 }
 // 32-byte sector / 16-byte half load/store with an L2 evict_last hint: control blocks and timer slots are
 // re-read every launch, ring records are write-once streams
@@ -246,24 +257,16 @@ __device__ __forceinline__ uint64_t keep_policy() {
   asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
   return pol;
 }
+__device__ __forceinline__ void ld_half(const void* src, uint4& a, bool hinted);
+__device__ __forceinline__ void st_half(void* dst, const uint4& a, bool hinted);
+// a whole 32-byte sector as two 16-byte accesses from one lane (sm_90 has no 256-bit global load/store)
 __device__ __forceinline__ void ld_sector(const void* src, uint4& a, uint4& b, bool hinted) {
-  const uint64_t pol = hinted ? keep_policy() : 0ull;
-  if (hinted)
-    asm volatile("ld.global.L2::cache_hint.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8], %9;"
-                 : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w), "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w)
-                 : "l"(src), "l"(pol));
-  else
-    asm volatile("ld.global.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w), "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w)
-                 : "l"(src));
+  ld_half(src, a, hinted);
+  ld_half(reinterpret_cast<const unsigned char*>(src) + 16, b, hinted);
 }
 __device__ __forceinline__ void st_sector(void* dst, const uint4& a, const uint4& b, bool hinted) {
-  const uint64_t pol = hinted ? keep_policy() : 0ull;
-  if (hinted)
-    asm volatile("st.global.L2::cache_hint.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8}, %9;" ::"l"(dst), "r"(a.x), "r"(a.y),
-                 "r"(a.z), "r"(a.w), "r"(b.x), "r"(b.y), "r"(b.z), "r"(b.w), "l"(pol)
-                 : "memory");
-  else st_v8(dst, a, b);
+  st_half(dst, a, hinted);
+  st_half(reinterpret_cast<unsigned char*>(dst) + 16, b, hinted);
 }
 __device__ __forceinline__ void ld_half(const void* src, uint4& a, bool hinted) {
   const uint64_t pol = hinted ? keep_policy() : 0ull;
@@ -279,8 +282,7 @@ __device__ __forceinline__ void st_half(void* dst, const uint4& a, bool hinted) 
   else st_v4(dst, a);
 }
 // One lane reads one staged 32-byte record as two 16-byte shared-memory loads.  At a 32-byte lane stride the eight lanes
-// of a quarter warp (one LDS.128 wavefront) touch only four distinct 16-byte bank groups: a 2-way conflict on every read
-// (round 1 ncu: l1tex__data_bank_conflicts_pipe_lsu_mem_shared_op_ld = 0.74 per record, 44 % of stall samples short_sb).
+// of a quarter warp (one LDS.128 wavefront) touch only four distinct 16-byte bank groups: a 2-way conflict on every read.
 // Lanes 4-7 of each quarter therefore fetch their two halves in the opposite order: each wavefront then covers all 32
 // banks, and two selects per register put the halves back in place.  No re-layout of the TMA-staged batch is needed.
 template <bool GATHER = false, bool PL = false>
@@ -574,11 +576,11 @@ __global__ void __launch_bounds__(kThreads, CPBUS_CTAS_PER_SM) fanout_kernel(con
   }
   // ---- planar re-layout of the staged batch (in place): record i = {lo[i], hi[i]}, lo at s4[i], hi at s4[cap + i] ----
   // At a 32-byte lane stride the eight lanes of an LDS.128 wavefront touch only four of the eight 16-byte bank groups
-  // (2-way conflict on every record read: round 1 ncu, 0.74 conflicts per record); at a 16-byte stride they touch all
+  // (2-way conflict on every record read); at a 16-byte stride they touch all
   // eight.  All 2n chunks are read into registers (n <= 1024: at most 8 per thread), barrier, then written to their
   // plane: two barriers and 8 shared-memory instructions per thread per CTA, against ~2000 record reads per thread.
-  // Not in the ORDERED build: its gathered reads do no better on planes than with the lane-swapped halves (same box, r2v:
-  // 1353 vs 1349 us), and not with the bulk store path, which copies whole records out of shared memory.
+  // Not in the ORDERED build: its gathered reads do no better on planes than with the lane-swapped halves, and not with
+  // the bulk store path, which copies whole records out of shared memory.
   constexpr bool PLANAR = CPBUS_PLANAR && STORE != CPBUS_STORE_BULK && !ORDERED;
   const uint32_t hi_off = cap;                                         // in 16-byte units
   if (PLANAR && n) {
@@ -617,7 +619,6 @@ __global__ void __launch_bounds__(kThreads, CPBUS_CTAS_PER_SM) fanout_kernel(con
   // (its id is in my_ids, its control block in registers: ONE load instruction brings the block's control blocks in).
   // A run of L mailboxes with the same mask word shares the filter pass AND the record reads: each gathered record is
   // stored to all L rings back to back, so the index-list -> gather -> select chain is paid once per run, not per mailbox
-  // (round 2 ncu: that chain held 29 % of config 5's stall samples; DRAM throughput 70 % against 79 % for the dense paths).
   bool runs_done = false;
   if constexpr (ORDERED && !TIMERS && !PAIRS && CPBUS_ORD_RUNS) {
     if (!s_dsum[1]) {   // CTA-uniform: no unicast record in this batch
@@ -681,8 +682,8 @@ __global__ void __launch_bounds__(kThreads, CPBUS_CTAS_PER_SM) fanout_kernel(con
             const uint32_t tl = __shfl_sync(0xffffffffu, ma.x, t);                        // low word of the tail: all the ring index needs
             const uint32_t id = __shfl_sync(0xffffffffu, my_ids, t);
             cpbus_event* ring = p.ring + (size_t)id * p.ring_cap;
-            if (v0) st_record<STORE>(ring + ((tl + o) & Rm_r), a0, b0);
-            if (v1) st_record<STORE>(ring + ((tl + o + 32) & Rm_r), a1, b1);
+            if (v0) st_v8(ring + ((tl + o) & Rm_r), a0, b0);
+            if (v1) st_v8(ring + ((tl + o + 32) & Rm_r), a1, b1);
           }
         }
         uint64_t dsum = 0;
@@ -722,8 +723,8 @@ __global__ void __launch_bounds__(kThreads, CPBUS_CTAS_PER_SM) fanout_kernel(con
   const bool has_unicast = s_dsum[1] != 0;
   // PAIRS build: TRIAGE.  A fleet of pair-filtered subscribers (jobs/jobs.go:188-231: every consumer listens for a dozen exact
   // events) takes almost nothing from a given batch, so walking the mailboxes one per warp-iteration — control block, then
-  // pair table, then 16 probes, each a dependent load — is all latency (round 2 ncu: 46 us per launch for 32,768 mailboxes
-  // and 55 deliveries).  Instead lane l decides for mailbox 32*blk + l: one control-block load per lane, and only when the
+  // pair table, then 16 probes, each a dependent load — is all latency.
+  // Instead lane l decides for mailbox 32*blk + l: one control-block load per lane, and only when the
   // code mask misses, its timer slots' due times and its pair row's probes into the presence filter.  The ballot of the
   // survivors drives the ordinary per-mailbox path below (control block handed over by shuffles); exactness is unchanged —
   // a survivor may still turn out to receive nothing.
@@ -778,7 +779,6 @@ __global__ void __launch_bounds__(kThreads, CPBUS_CTAS_PER_SM) fanout_kernel(con
   }
   const uint32_t Rm = p.ring_cap - 1;
   const uint4* s4 = reinterpret_cast<const uint4*>(s_batch);
-  const uint32_t sw = ((uint32_t)lane >> 2) & 1u;                      // which half this lane fetches first (lds_record)
   const uint32_t scratch_words = max(32u, cap / 2u);                   // per warp: 32 tick positions or cap u16 event indices
   uint32_t* my_tick = s_tick + warp * scratch_words;
 
@@ -877,11 +877,8 @@ __global__ void __launch_bounds__(kThreads, CPBUS_CTAS_PER_SM) fanout_kernel(con
         }
         bulk_pending = true;
       } else if (STORE == CPBUS_STORE_V8) {
-        for (uint32_t i = lane; i < n; i += 32) {
-          uint4 a, b;
-          lds_record<false, PLANAR>(s4, i, sw, a, b, hi_off);
-          st_v8(ring + (((uint32_t)tail + i) & Rm), a, b);
-        }
+        for (uint32_t c0 = 0; c0 < n; c0 += 32)   // warp-uniform trip count (copy_record_pairs needs every lane)
+          copy_record_pairs<PLANAR>(s4, hi_off, ring, (uint32_t)tail, Rm, c0 + lane, c0 + lane, c0 + lane < n);
       } else {
         for (uint32_t q = lane; q < 2 * n; q += 32) {   // lane pair per record: 512 contiguous bytes per instruction
           const uint4 v = PLANAR ? s4[(q & 1u) * hi_off + (q >> 1)] : s4[q];
@@ -893,16 +890,16 @@ __global__ void __launch_bounds__(kThreads, CPBUS_CTAS_PER_SM) fanout_kernel(con
     } else if (dense) {
       // ================= dense run with interleaved ticks: O(#ticks) bookkeeping =================
       if (CPBUS_COLD_EARLY && TIMERS && tk_slot < nslots) {   // cold half of the timer slot {source_id, fired}: needed only for the tick records after the
-        uint4 cold;                        // copy loop, but issued HERE so that its DRAM round trip hides under the copy (round 2 ncu:
-        ld_half(reinterpret_cast<const unsigned char*>(p.timers + (size_t)s * K + tk_slot) + 16, cold, keep);   // 13 % of stalls sat on it)
+        uint4 cold;                        // copy loop, but issued HERE so that its DRAM round trip hides under the copy
+        ld_half(reinterpret_cast<const unsigned char*>(p.timers + (size_t)s * K + tk_slot) + 16, cold, keep);
         tk_src = cold.x; tk_fired = cold.y;
       }
       if (tk_valid) my_tick[tk_rank] = tk_pos;
       __syncwarp();
       k = n + n_ticks;
       // event i lands at i + #{ticks with pos <= i}.  Lane r keeps the r-th smallest tick position in a register, so per
-      // 32-event chunk the count is two ballots and a bit mask — no shared-memory round trip in the copy loop (round 1:
-      // 34 % of this path's stall samples sat on the my_tick[] loads feeding these compares).
+      // 32-event chunk the count is two ballots and a bit mask — no shared-memory round trip in the copy loop (the my_tick[]
+      // loads feeding these compares would otherwise stall it).
 #if CPBUS_TICKS_REG
       const uint32_t T = (uint32_t)lane < n_ticks ? my_tick[lane] : 0xFFFFFFFFu;
       // destination of event i = c0 + lane of the chunk starting at c0
@@ -925,21 +922,14 @@ __global__ void __launch_bounds__(kThreads, CPBUS_CTAS_PER_SM) fanout_kernel(con
 #pragma unroll 1
       for (; c0 + 64 <= n; c0 += 64) {   // two chunks per iteration: both records' shared-memory loads are in flight before the selects
         const uint32_t o0 = slot_of(c0), o1 = slot_of(c0 + 32);
-        uint4 a0, b0, a1, b1;
-        lds_record<false, PLANAR>(s4, c0 + lane, sw, a0, b0, hi_off);
-        lds_record<false, PLANAR>(s4, c0 + 32 + lane, sw, a1, b1, hi_off);
-        st_record<STORE>(ring + (((uint32_t)tail + o0) & Rm), a0, b0);
-        st_record<STORE>(ring + (((uint32_t)tail + o1) & Rm), a1, b1);
+        copy_record_pairs<PLANAR>(s4, hi_off, ring, (uint32_t)tail, Rm, c0 + lane, o0, true);
+        copy_record_pairs<PLANAR>(s4, hi_off, ring, (uint32_t)tail, Rm, c0 + 32 + lane, o1, true);
       }
 #endif
 #pragma unroll 1
       for (; c0 < n; c0 += 32) {
         const uint32_t out = slot_of(c0);
-        if (c0 + lane < n) {
-          uint4 a, b;
-          lds_record<false, PLANAR>(s4, c0 + lane, sw, a, b, hi_off);
-          st_record<STORE>(ring + (((uint32_t)tail + out) & Rm), a, b);
-        }
+        copy_record_pairs<PLANAR>(s4, hi_off, ring, (uint32_t)tail, Rm, c0 + lane, out, c0 + lane < n);
       }
 #else
       // Tick positions are sorted, so the count is warp-uniform for a whole 32-event chunk unless a tick falls strictly inside it
@@ -950,11 +940,7 @@ __global__ void __launch_bounds__(kThreads, CPBUS_CTAS_PER_SM) fanout_kernel(con
         const uint32_t i = c0 + lane;
         uint32_t out = i + t_idx;
         for (uint32_t t = t_idx; t < n_ticks && my_tick[t] < c0 + 32; t++) out += (my_tick[t] <= i) ? 1u : 0u;
-        if (i < n) {
-          uint4 a, b;
-          lds_record<false, PLANAR>(s4, i, sw, a, b, hi_off);
-          st_record<STORE>(ring + (((uint32_t)tail + out) & Rm), a, b);
-        }
+        copy_record_pairs<PLANAR>(s4, hi_off, ring, (uint32_t)tail, Rm, i, out, i < n);
       }
 #endif
       if (!CPBUS_COLD_EARLY && TIMERS && tk_slot < nslots) {
@@ -969,7 +955,7 @@ __global__ void __launch_bounds__(kThreads, CPBUS_CTAS_PER_SM) fanout_kernel(con
         const uint64_t w3 = (uint64_t)gid | ((uint64_t)CPBUS_F_TICK << 32);
         const uint4 a = make_uint4((uint32_t)w0, (uint32_t)(w0 >> 32), (uint32_t)w1, (uint32_t)(w1 >> 32));
         const uint4 b = make_uint4((uint32_t)w2, (uint32_t)(w2 >> 32), (uint32_t)w3, (uint32_t)(w3 >> 32));
-        st_record<STORE>(ring + (((uint32_t)tail + out) & Rm), a, b);
+        st_v8(ring + (((uint32_t)tail + out) & Rm), a, b);
         if (DIGEST) {
           // the run of events in front of this tick keeps its internal weights and is shifted by the
           // ticks still to come: (Q[pos_r] - Q[pos_{r-1}]) * P^(n_ticks - r)
@@ -990,7 +976,7 @@ __global__ void __launch_bounds__(kThreads, CPBUS_CTAS_PER_SM) fanout_kernel(con
           uint32_t base = 0;
           const uint32_t nchunks = (n + 31) >> 5;
           // code bits of 4 chunks are fetched up front: 4 independent shared-memory loads in flight instead of a
-          // load -> test -> ballot chain per chunk (46 % of this path's stall samples were short-scoreboard on that load)
+          // load -> test -> ballot chain per chunk
           for (uint32_t c0 = 0; c0 < nchunks; c0 += 4) {
             uint32_t cbit[4];
 #pragma unroll
@@ -1015,50 +1001,27 @@ __global__ void __launch_bounds__(kThreads, CPBUS_CTAS_PER_SM) fanout_kernel(con
         uint64_t acc = 0;
         const uint64_t p32 = s_pow[32];
         const bool hashing = DIGEST && !reuse;
-        uint32_t o = lane;
-#if CPBUS_IDX_PF
-        // the index list is read one iteration ahead: the records' shared-memory addresses are then ready when the loop turns
-        uint32_t i0 = o < k ? my_idx[o] : 0u, i1 = o + 32 < k ? my_idx[o + 32] : 0u;
-        for (; o + 32 < k; o += 64) {
+        // warp-uniform trip count (copy_record_pairs needs every lane); the index list is read one iteration ahead, so the
+        // records' shared-memory addresses are ready when the loop turns
+        uint32_t i0 = (uint32_t)lane < k ? my_idx[lane] : 0u, i1 = lane + 32u < k ? my_idx[lane + 32] : 0u;
+        for (uint32_t o0 = 0; o0 < k; o0 += 64) {
+          const uint32_t o = o0 + lane;
+          const bool v0 = o < k, v1 = o + 32 < k;
           const uint32_t n0 = o + 64 < k ? my_idx[o + 64] : 0u, n1 = o + 96 < k ? my_idx[o + 96] : 0u;
-          uint4 a0, b0, a1, b1;
-          lds_record<ORDERED, PLANAR>(s4, i0, sw, a0, b0, hi_off);
-          lds_record<ORDERED, PLANAR>(s4, i1, sw, a1, b1, hi_off);
-          st_record<STORE>(ring + (((uint32_t)tail + o) & Rm), a0, b0);
-          st_record<STORE>(ring + (((uint32_t)tail + o + 32) & Rm), a1, b1);
-          if (hashing) acc = (acc * p32 + s_rhash[i0]) * p32 + s_rhash[i1];
+          copy_record_pairs<PLANAR>(s4, hi_off, ring, (uint32_t)tail, Rm, i0, o, v0);
+          copy_record_pairs<PLANAR>(s4, hi_off, ring, (uint32_t)tail, Rm, i1, o + 32, v1);
+          if (hashing) {
+            if (v0) acc = acc * p32 + s_rhash[i0];
+            if (v1) acc = acc * p32 + s_rhash[i1];
+          }
           i0 = n0; i1 = n1;
         }
-        if (o < k) {
-          uint4 a, b;
-          lds_record<ORDERED, PLANAR>(s4, i0, sw, a, b, hi_off);
-          st_record<STORE>(ring + (((uint32_t)tail + o) & Rm), a, b);
-          if (hashing) acc = acc * p32 + s_rhash[i0];
-          o += 32;
-        }
-#else
-        for (; o + 32 < k; o += 64) {   // two outputs per lane per iteration: their index/record/hash loads are independent
-          const uint32_t i0 = my_idx[o], i1 = my_idx[o + 32];
-          uint4 a0, b0, a1, b1;
-          lds_record<ORDERED, PLANAR>(s4, i0, sw, a0, b0, hi_off);
-          lds_record<ORDERED, PLANAR>(s4, i1, sw, a1, b1, hi_off);
-          st_record<STORE>(ring + (((uint32_t)tail + o) & Rm), a0, b0);
-          st_record<STORE>(ring + (((uint32_t)tail + o + 32) & Rm), a1, b1);
-          if (hashing) acc = (acc * p32 + s_rhash[i0]) * p32 + s_rhash[i1];
-        }
-        for (; o < k; o += 32) {
-          const uint32_t i = my_idx[o];
-          uint4 a, b;
-          lds_record<ORDERED, PLANAR>(s4, i, sw, a, b, hi_off);
-          st_record<STORE>(ring + (((uint32_t)tail + o) & Rm), a, b);
-          if (hashing) acc = acc * p32 + s_rhash[i];
-        }
-#endif
         if (DIGEST) {
           if (reuse) dsum = run_sum;
           else {
-            // o is now the first index this lane did NOT write; its last one was o-32 (if any)
-            dsum = (o >= 32 && o - 32 < k) ? acc * s_pow[k - 1 - (o - 32)] : 0ull;
+            // lane l wrote outputs l, l+32, ...: cnt of them, the last one at l + 32 (cnt - 1)
+            const uint32_t cnt = k > (uint32_t)lane ? (k - lane + 31u) / 32u : 0u;
+            dsum = cnt ? acc * s_pow[k - 1 - (lane + 32u * (cnt - 1u))] : 0ull;
             dsum = warp_sum64(dsum);
             if (ORDERED) run_sum = dsum;
           }
@@ -1076,13 +1039,9 @@ __global__ void __launch_bounds__(kThreads, CPBUS_CTAS_PER_SM) fanout_kernel(con
           const uint32_t i = c * 32 + lane;
           const bool match = i < n && (m & s_meta[i].x) != 0;
           const uint32_t w = __ballot_sync(0xffffffffu, match);
-          if (match) {
-            const uint32_t out = base + __popc(w & ((1u << lane) - 1u));
-            uint4 a, b;
-            lds_record<false, PLANAR>(s4, i, sw, a, b, hi_off);
-            st_record<STORE>(ring + (((uint32_t)tail + out) & Rm), a, b);
-            if (DIGEST) dsum += s_rhash[i] * s_pow[k - 1 - out];
-          }
+          const uint32_t out = base + __popc(w & ((1u << lane) - 1u));
+          if (DIGEST && match) dsum += s_rhash[i] * s_pow[k - 1 - out];
+          copy_record_pairs<PLANAR>(s4, hi_off, ring, (uint32_t)tail, Rm, i, out, match);
           base += __popc(w);
         }
         if (DIGEST) dsum = warp_sum64(dsum);
@@ -1139,16 +1098,17 @@ __global__ void __launch_bounds__(kThreads, CPBUS_CTAS_PER_SM) fanout_kernel(con
       for (uint32_t c = 0; c < nchunks; c++) {   // pass B
         const uint32_t w = __shfl_sync(0xffffffffu, myword, c);
         const uint32_t wp = __shfl_sync(0xffffffffu, wprefix, c);
-        if ((w >> lane) & 1u) {
-          const uint32_t i = c * 32 + lane;
+        if (!w) continue;                          // warp-uniform
+        const bool mine = (w >> lane) & 1u;
+        const uint32_t i = c * 32 + lane;
+        uint32_t out = 0;
+        if (mine) {
           const uint32_t mrank = wp + __popc(w & ((1u << lane) - 1u));
-          uint32_t out = mrank;
+          out = mrank;
           for (uint32_t t = 0; t < n_ticks; t++) out += (my_tick[t] <= mrank) ? 1u : 0u;
-          uint4 a, b;
-          lds_record<false, PLANAR>(s4, i, sw, a, b, hi_off);
-          st_record<STORE>(ring + (((uint32_t)tail + out) & Rm), a, b);
           if (DIGEST) dsum += s_rhash[i] * s_pow[k - 1 - out];
         }
+        copy_record_pairs<PLANAR>(s4, hi_off, ring, (uint32_t)tail, Rm, i, out, mine);
       }
       if (n_ticks) {
         if (TIMERS && tk_slot < nslots) {   // cold half of the timer slot {source_id, fired}: loaded late, only when something fires
@@ -1164,7 +1124,7 @@ __global__ void __launch_bounds__(kThreads, CPBUS_CTAS_PER_SM) fanout_kernel(con
         const uint64_t w3 = (uint64_t)gid | ((uint64_t)CPBUS_F_TICK << 32);
         const uint4 a = make_uint4((uint32_t)w0, (uint32_t)(w0 >> 32), (uint32_t)w1, (uint32_t)(w1 >> 32));
         const uint4 b = make_uint4((uint32_t)w2, (uint32_t)(w2 >> 32), (uint32_t)w3, (uint32_t)(w3 >> 32));
-        st_record<STORE>(ring + (((uint32_t)tail + out) & Rm), a, b);
+        st_v8(ring + (((uint32_t)tail + out) & Rm), a, b);
         if (DIGEST) dsum += record_hash_words(w0, w1, w2, w3) * s_pow[k - 1 - out];
       }
       if (DIGEST) dsum = warp_sum64(dsum);

@@ -1,6 +1,6 @@
 /*
- * cpbus.h — C-ABI of libcpbus, the B200-native event bus that sits behind
- * ContainerPilot's `events` package (reference: /root/reference/events/).
+ * cpbus.h — C-ABI of libcpbus, the H100-native event bus that sits behind
+ * ContainerPilot's `events` package (reference: TritonDataCenter/containerpilot, events/).
  *
  * This header is the drop-in boundary (SURVEY.md §8b).  It is what a cgo shim
  * for package `events` binds (see INTEGRATION.md for the Go side).  Everything
@@ -90,8 +90,8 @@ enum {
 /* cpbus_config.store_path: how records reach the rings (all are bit-identical) */
 enum {
   CPBUS_STORE_AUTO = 0, /* library default = best measured (see DESIGN.md)       */
-  CPBUS_STORE_V4   = 1, /* st.global.v4.b32: lane pair per record, 16 B / lane   */
-  CPBUS_STORE_V8   = 2, /* st.global.v8.b32: one lane per record, 32 B / lane    */
+  CPBUS_STORE_V4   = 1, /* lane pair per record, 16 B / lane, half-indexed loop  */
+  CPBUS_STORE_V8   = 2, /* lane pair per record, record-indexed loop (default)   */
   CPBUS_STORE_BULK = 3  /* cp.async.bulk smem->global (TMA) for dense segments   */
 };
 

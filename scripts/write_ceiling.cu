@@ -1,7 +1,7 @@
-// write_ceiling.cu — calibration: what does a B200 sustain for PURE HBM writes, and which
+// write_ceiling.cu — calibration: what does the GPU sustain for PURE HBM writes, and which
 // store flavour / layout / occupancy gets the mailbox-append pattern closest to it?
-// (MEASURED_PEAKS.json's 6575 GB/s is a copy: half reads, half writes.)
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o write_ceiling write_ceiling.cu
+// (A copy peak counts half reads, half writes.)  sm_90 has no 256-bit store: a "v8" sector is two 16-byte stores.
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o write_ceiling write_ceiling.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -9,11 +9,11 @@
 
 enum { PLAIN = 0, CS = 1, WT = 2, NOALLOC = 3, EVICT_FIRST = 4 };
 template <int F> __device__ __forceinline__ void st_v8(void* dst, uint32_t v, uint64_t pol) {
-  if (F == PLAIN) asm volatile("st.global.v8.b32 [%0], {%1,%1,%1,%1,%1,%1,%1,%1};" ::"l"(dst), "r"(v) : "memory");
+  if (F == PLAIN) { asm volatile("st.global.v4.b32 [%0], {%1,%1,%1,%1};" ::"l"(dst), "r"(v) : "memory"); asm volatile("st.global.v4.b32 [%0+16], {%1,%1,%1,%1};" ::"l"(dst), "r"(v) : "memory"); }
   if (F == CS) { asm volatile("st.global.cs.v4.b32 [%0], {%1,%1,%1,%1};" ::"l"(dst), "r"(v) : "memory"); asm volatile("st.global.cs.v4.b32 [%0+16], {%1,%1,%1,%1};" ::"l"(dst), "r"(v) : "memory"); }
   if (F == WT) { asm volatile("st.global.wt.v4.b32 [%0], {%1,%1,%1,%1};" ::"l"(dst), "r"(v) : "memory"); asm volatile("st.global.wt.v4.b32 [%0+16], {%1,%1,%1,%1};" ::"l"(dst), "r"(v) : "memory"); }
-  if (F == NOALLOC) asm volatile("st.global.L1::no_allocate.v8.b32 [%0], {%1,%1,%1,%1,%1,%1,%1,%1};" ::"l"(dst), "r"(v) : "memory");
-  if (F == EVICT_FIRST) asm volatile("st.global.L2::cache_hint.v8.b32 [%0], {%1,%1,%1,%1,%1,%1,%1,%1}, %2;" ::"l"(dst), "r"(v), "l"(pol) : "memory");
+  if (F == NOALLOC) { asm volatile("st.global.L1::no_allocate.v4.b32 [%0], {%1,%1,%1,%1};" ::"l"(dst), "r"(v) : "memory"); asm volatile("st.global.L1::no_allocate.v4.b32 [%0+16], {%1,%1,%1,%1};" ::"l"(dst), "r"(v) : "memory"); }
+  if (F == EVICT_FIRST) { asm volatile("st.global.L2::cache_hint.v4.b32 [%0], {%1,%1,%1,%1}, %2;" ::"l"(dst), "r"(v), "l"(pol) : "memory"); asm volatile("st.global.L2::cache_hint.v4.b32 [%0+16], {%1,%1,%1,%1}, %2;" ::"l"(dst), "r"(v), "l"(pol) : "memory"); }
 }
 __device__ __forceinline__ void st_v4(void* dst, uint32_t v) {
   asm volatile("st.global.v4.b32 [%0], {%1,%1,%1,%1};" ::"l"(dst), "r"(v) : "memory");
@@ -102,6 +102,8 @@ __global__ void chunked_fenced(unsigned char* p, size_t n_chunks, uint32_t chunk
   }
 }
 int main() {
+  int sms = 0;
+  CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0));
   const size_t bytes = (size_t)4 << 30;
   unsigned char* d; CK(cudaMalloc(&d, bytes));
   cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
@@ -112,7 +114,7 @@ int main() {
     cudaEventElapsedTime(&ms, e0, e1);
   }
   report("cudaMemset 4 GiB", bytes, 10);
-  for (int g : {148 * 4, 148 * 8, 148 * 16, 148 * 64}) {
+  for (int g : {sms * 4, sms * 8, sms * 16, sms * 64}) {
     cudaEventRecord(e0); for (int r = 0; r < 10; r++) linear_v4<<<g, 256>>>((uint4*)d, bytes / 16, r); cudaEventRecord(e1); cudaEventSynchronize(e1);
     cudaEventElapsedTime(&ms, e0, e1); char nm[64]; snprintf(nm, 64, "linear st.v4 grid=%d", g); report(nm, bytes, 10);
   }
@@ -128,12 +130,12 @@ int main() {
     cudaEventRecord(e1); cudaEventSynchronize(e1); cudaEventElapsedTime(&ms, e0, e1);
     char nm[96]; snprintf(nm, 96, "chunk=%5u stride=%5u grid=%4d %s", chunk, stride, g, flav); report(nm, b, 40);
   };
-  for (uint32_t chunk : {8192u}) for (uint32_t stride : {32768u, chunk}) for (int g : {148 * 3, 148 * 4, 148 * 8, 148 * 16, 148 * 32, 148 * 64, 8192}) {
+  for (uint32_t chunk : {8192u}) for (uint32_t stride : {32768u, chunk}) for (int g : {sms * 3, sms * 4, sms * 8, sms * 16, sms * 32, sms * 64, 8192}) {
     run(chunked_v8<PLAIN>, "plain", chunk, stride, g);
-    if (g <= 148 * 4) run(chunked_v8<EVICT_FIRST>, "L2::evict_first", chunk, stride, g);
+    if (g <= sms * 4) run(chunked_v8<EVICT_FIRST>, "L2::evict_first", chunk, stride, g);
   }
   // fewer threads per CTA, more CTAs (128-thread CTAs)
-  for (uint32_t stride : {32768u, 8192u}) for (int g : {148 * 16, 148 * 64, 16384}) {
+  for (uint32_t stride : {32768u, 8192u}) for (int g : {sms * 16, sms * 64, 16384}) {
     const size_t b = n_chunks * 8192;
     cudaEventRecord(e0);
     for (int r = 0; r < 40; r++) chunked_v8<PLAIN><<<g, 128>>>(stride == 32768 ? d + (size_t)(r % 4) * 8192 : d + (size_t)(r % 4) * n_chunks * 8192, n_chunks, 8192, stride, r);
@@ -142,7 +144,7 @@ int main() {
   }
   {
     unsigned long long* ctr; CK(cudaMalloc(&ctr, 8 * 64));
-    for (uint32_t stride : {32768u, 8192u}) for (uint32_t T : {1u, 4u, 16u}) for (int g : {148 * 3, 148 * 4, 148 * 8}) {
+    for (uint32_t stride : {32768u, 8192u}) for (uint32_t T : {1u, 4u, 16u}) for (int g : {sms * 3, sms * 4, sms * 8}) {
       const size_t b = n_chunks * 8192;
       cudaEventRecord(e0);
       for (int r = 0; r < 40; r++) {
@@ -155,14 +157,14 @@ int main() {
   }
   {
     unsigned long long* ctr; CK(cudaMalloc(&ctr, 8 * 64));
-    for (uint32_t T : {2u, 4u, 8u}) for (int g : {148 * 3, 148 * 4, 148 * 8}) {
+    for (uint32_t T : {2u, 4u, 8u}) for (int g : {sms * 3, sms * 4, sms * 8}) {
       const size_t b = n_chunks * 8192;
       cudaEventRecord(e0);
       for (int r = 0; r < 40; r++) { CK(cudaMemsetAsync(ctr, 0, 8)); chunked_dyn_pf<<<g, 256>>>(d + (size_t)(r % 4) * 8192, n_chunks, 8192, 32768, r, ctr, T); }
       cudaEventRecord(e1); cudaEventSynchronize(e1); cudaEventElapsedTime(&ms, e0, e1);
       char nm[96]; snprintf(nm, 96, "DYN+PREFETCH chunk=8192 stride=32768 grid=%4d claim=%u", g, T); report(nm, b, 40);
     }
-    for (size_t nch : {(size_t)65536, (size_t)(444 * 8 * 18), (size_t)(444 * 8 * 19)}) for (int g : {148 * 3}) {
+    for (size_t nch : {(size_t)65536, (size_t)((sms * 3) * 8 * 18), (size_t)((sms * 3) * 8 * 19)}) for (int g : {sms * 3}) {
       const size_t b = nch * 8192;
       cudaEventRecord(e0);
       for (int r = 0; r < 40; r++) chunked_v8<PLAIN><<<g, 256>>>(d + (size_t)(r % 4) * 8192, nch, 8192, 32768, r);
@@ -174,7 +176,7 @@ int main() {
       snprintf(nm, 96, "STATIC blocked n_chunks=%zu grid=%d", nch, g); report(nm, b, 40);
     }
   }
-  for (int g : {148 * 3, 148 * 4, 148 * 8}) {
+  for (int g : {sms * 3, sms * 4, sms * 8}) {
     const size_t b = n_chunks * 8192;
     auto go = [&](auto kern, const char* nm0) {
       cudaEventRecord(e0);
@@ -191,7 +193,7 @@ int main() {
     cudaEventRecord(e1); cudaEventSynchronize(e1); cudaEventElapsedTime(&ms, e0, e1);
     char nm[96]; snprintf(nm, 96, "SKEW grid=%4d skew=%5u rot=%u", g, skew, rot); report(nm, b, 40);
   }
-  for (uint32_t chunk : {32768u}) for (int g : {148 * 4, 148 * 8}) { run(chunked_v8<PLAIN>, "plain", chunk, 32768, g); run(chunked_v8<EVICT_FIRST>, "L2::evict_first", chunk, 32768, g); }
+  for (uint32_t chunk : {32768u}) for (int g : {sms * 4, sms * 8}) { run(chunked_v8<PLAIN>, "plain", chunk, 32768, g); run(chunked_v8<EVICT_FIRST>, "L2::evict_first", chunk, 32768, g); }
   CK(cudaGetLastError());
   return 0;
 }
