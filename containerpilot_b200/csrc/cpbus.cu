@@ -76,6 +76,7 @@ struct cpbus_stream;
 struct cpbus {
   cpbus_config cfg{};
   int device = 0, sm_count = 132;
+  size_t smem_per_sm = 228 * 1024, smem_reserved = 1024;   // shared memory per SM, and what the system keeps per CTA
   cudaStream_t stream = nullptr;
   bool own_stream = false;
   uint32_t N = 0, R = 0, B = 0, K = 0;
@@ -279,27 +280,15 @@ int rebuild_order(cpbus* b) {
   return CPBUS_OK;
 }
 
+constexpr int kFanoutMaxSmem = 200 * 1024;
+
 template <int STORE, bool TIMERS, bool DIGEST, bool ORDERED, bool PAIRS = false>
 int launch_fanout_t(cpbus* b, const FanoutParams& p, uint32_t grid, size_t smem) {
   static bool attr_done[64] = {};   // per instantiation AND per device: function attributes are per-device state
   const int dev = b->device & 63;
   if (!attr_done[dev]) {
-    CK(cudaFuncSetAttribute(fanout_kernel<STORE, TIMERS, DIGEST, ORDERED, PAIRS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    CK(cudaFuncSetAttribute(fanout_kernel<STORE, TIMERS, DIGEST, ORDERED, PAIRS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kFanoutMaxSmem));
     attr_done[dev] = true;
-  }
-  if (!grid) {
-    // Several waves of short-lived CTAs rather than one persistent wave: the hardware CTA scheduler balances the
-    // SM speed spread for free.  Per-CTA setup here is a descriptor copy + TMA wait, so the grid aims at 2-16
-    // mailboxes per warp, scaled with the SM count.
-    const uint32_t need = (p.n_subs + kWarpsPerCta - 1) / kWarpsPerCta;
-    uint32_t spw = b->subs_per_warp;
-    if (!spw) {
-      // ~constant bytes per warp: the counts above are for 256-event batches; a 512-event batch halves them
-      const uint32_t scale = std::max(1u, (p.n_ev + 128u) / 256u);
-      const uint32_t cap = std::max(1u, 16u / scale);
-      spw = std::max(1u, std::min(cap, (need + (uint32_t)b->sm_count * 7 * scale) / ((uint32_t)b->sm_count * 14 * scale)));
-    }
-    grid = std::max(1u, std::min((need + spw - 1) / spw, need));
   }
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = smem; cfg.stream = b->stream;
@@ -345,7 +334,7 @@ int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, in
   const size_t hot_bytes = (size_t)b->n_next * (sizeof(SubCtl) + (p.timers_on ? b->K * sizeof(DevTimer) : 0));
   p.hints = b->hints >= 0 ? (uint32_t)b->hints : (hot_bytes <= (64u << 20) ? 1u : 0u);
   const uint32_t need = (b->n_next + kWarpsPerCta - 1) / kWarpsPerCta;
-  uint32_t grid = b->cfg.grid_ctas ? std::max(1u, std::min(b->cfg.grid_ctas, need)) : 0u;   // 0: sized from occupancy
+  uint32_t grid = b->cfg.grid_ctas ? std::max(1u, std::min(b->cfg.grid_ctas, need)) : 0u;
   int rc;
   // ORDERED build (no timers armed, at least one filtered subscriber): walk the mailboxes in code-mask order so that
   // equal masks are neighbours and share one filter pass (cost ~ deliveries + distinct masks, not subscribers x events)
@@ -353,7 +342,7 @@ int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, in
   // general path; subscribers without a pair table take the same paths as before
   const bool pairs_on = b->n_paired > 0 && b->d_pairs;
   p.pairs = pairs_on ? b->d_pairs : nullptr;
-  const size_t smem = fanout_smem_bytes(p.smem_cap) + (pairs_on ? kPairFilterBytes : 0);   // + the batch's {code, source} presence filter
+  size_t smem = fanout_smem_bytes(p.smem_cap) + (pairs_on ? kPairFilterBytes : 0);   // + the batch's {code, source} presence filter
   if (!pairs_on && !p.timers_on && (b->use_order == 2 || (b->use_order == 1 && b->n_filtered > 0))) {
     if (b->order_dirty) { const int rc_order = rebuild_order(b); if (rc_order) return rc_order; }
     if (b->n_order) {
@@ -369,6 +358,33 @@ int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, in
   if (pairs_on && !b->cfg.grid_ctas) {   // PAIRS build: lane-parallel triage over blocks of 32 mailboxes per warp turn
     const uint32_t blocks = (b->n_next + 31u) / 32u;
     grid = std::max(1u, std::min((blocks + kWarpsPerCta - 1) / kWarpsPerCta, (uint32_t)b->sm_count * 16u));
+  }
+  if (!pairs_on && !p.order) {
+    // Plain build: CTA b owns subscribers [8 spw b, 8 spw (b + 1)).  Several waves of short-lived CTAs rather than one
+    // persistent wave: the hardware CTA scheduler balances the SM speed spread for free.  Per-CTA setup here is a
+    // descriptor copy + TMA wait, so the grid aims at 2-16 mailboxes per warp, scaled with the SM count.
+    // (need == 0: a stream batch on a bus without subscribers still takes one CTA, which acknowledges it)
+    uint32_t spw = b->subs_per_warp;
+    if (grid) spw = std::max(1u, (need + grid - 1) / grid);   // a fixed grid: ranges cover every subscriber
+    else if (!spw) {
+      // ~constant bytes per warp: the counts above are for 256-event batches; a 512-event batch halves them
+      const uint32_t scale = std::max(1u, (p.n_ev + 128u) / 256u);
+      const uint32_t cap = std::max(1u, 16u / scale);
+      spw = std::max(1u, std::min(cap, (need + (uint32_t)b->sm_count * 7 * scale) / ((uint32_t)b->sm_count * 14 * scale)));
+    }
+    p.spw = spw;
+    grid = std::max(1u, (need + spw - 1) / spw);
+    // The range's control blocks (and timer slots) are staged in shared memory stage_subs at a time, in what the batch
+    // leaves of the shared memory at the residency that the batch plus the smallest round (one subscriber per warp)
+    // allows, at most CPBUS_CTAS_PER_SM CTAs per SM.  Staging can therefore cost a resident CTA only where the batch
+    // leaves less than that smallest round.
+    const size_t off = fanout_stage_off(p.smem_cap);
+    const size_t per_sub = sizeof(SubCtl) + (p.timers_on ? (size_t)b->K * sizeof(DevTimer) : 0);
+    const size_t min_round = (size_t)kWarpsPerCta * per_sub;
+    const size_t ctas = std::max<size_t>(1, std::min<size_t>(CPBUS_CTAS_PER_SM, b->smem_per_sm / (off + min_round + b->smem_reserved)));
+    const size_t room = std::min<size_t>(kFanoutMaxSmem, b->smem_per_sm / ctas - b->smem_reserved) - off;   // >= min_round
+    p.stage_subs = std::max<uint32_t>(kWarpsPerCta, (uint32_t)std::min<size_t>((size_t)kWarpsPerCta * spw, room / per_sub) & ~7u);
+    smem = off + p.stage_subs * per_sub;
   }
   const int variant = pairs_on ? (p.use_digest ? 7 : 6) : (p.timers_on ? 2 : 0) | (p.use_digest ? 1 : 0) | (p.order ? 4 : 0);
 #define CPBUS_DISPATCH(ST)                                                                \
@@ -636,7 +652,10 @@ int cpbus_create(const cpbus_config* cfg, cpbus_t** out) try {
   if (b->device >= ndev) return fail(CPBUS_EINVAL);
   if ((rc = dev_guard(b))) return fail(rc);
   cudaDeviceProp prop{};
-  if (cudaGetDeviceProperties(&prop, b->device) == cudaSuccess) b->sm_count = prop.multiProcessorCount;
+  if (cudaGetDeviceProperties(&prop, b->device) == cudaSuccess) {
+    b->sm_count = prop.multiProcessorCount;
+    b->smem_per_sm = prop.sharedMemPerMultiprocessor; b->smem_reserved = prop.reservedSharedMemPerBlock;
+  }
   if (cfg->stream) b->stream = (cudaStream_t)cfg->stream;
   else {
     if (cudaStreamCreateWithFlags(&b->stream, cudaStreamNonBlocking) != cudaSuccess) return fail(CPBUS_ECUDA);

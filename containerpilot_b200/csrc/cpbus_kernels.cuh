@@ -23,8 +23,8 @@ namespace cpbus_dev {
 constexpr int kWarpsPerCta = 8;
 constexpr int kThreads = kWarpsPerCta * 32;
 // Every variant of the fan-out kernel is held to 64 registers => 4 CTAs (32 warps) per SM.  ptxas (CUDA 12.9, sm_90a) spills
-// nothing in the dense, ORDERED and no-digest timers variants, 4-14 bytes in the timers + digest variants and 52-140 bytes
-// in the PAIRS variants.  Occupancy is the biggest single lever (DESIGN.md §4.1); the macro exists for A/B builds.
+// nothing in the plain (dense and timers, with or without digest) and ORDERED variants, and 40-76 bytes in the PAIRS
+// variants.  Occupancy is the biggest single lever (DESIGN.md §4.1); the macro exists for A/B builds.
 #ifndef CPBUS_CTAS_PER_SM
 #define CPBUS_CTAS_PER_SM 4
 #endif
@@ -40,13 +40,10 @@ constexpr int kThreads = kWarpsPerCta * 32;
 #define CPBUS_TICKS_REG 1    // dense+ticks copy loop: tick positions in registers (ballots) instead of shared-memory loads
 #endif
 #ifndef CPBUS_COLD_EARLY
-#define CPBUS_COLD_EARLY 1   // cold half of the timer slot loaded before the copy loop instead of after it
-#endif
+#define CPBUS_COLD_EARLY 1   // PAIRS build: cold half of the timer slot loaded before the copy loop instead of after it (the plain
+#endif                       // build reads it from its shared-memory staging)
 #ifndef CPBUS_UNROLL2
 #define CPBUS_UNROLL2 1      // dense+ticks loop: two 32-event chunks per iteration
-#endif
-#ifndef CPBUS_EARLY_PF
-#define CPBUS_EARLY_PF 0     // prefetch.L2 of the warp's first control block / timer slot at kernel entry
 #endif
 #ifndef CPBUS_ORD_PF
 #define CPBUS_ORD_PF 0       // ORDERED build: prefetch.L2 of the whole block's control blocks once the ids are known
@@ -78,8 +75,8 @@ constexpr uint64_t kDigestP = 0x9E3779B97F4A7C15ull;
 constexpr uint32_t kPowTableLen = 2048 + 65 + 7;   // batch_cap <= 2048
 
 // One timer slot (events/timer.go: one goroutine + ticker).  The first 16 bytes are all the fan-out kernel
-// needs to decide whether anything fires (and are what it prefetches); the second half is touched only
-// when a tick is actually emitted.  Disarmed slot: next_due == kTimerIdle.  One-shot: period == 0.
+// needs to decide whether anything fires; the second half is read only when a tick is actually emitted.
+// Disarmed slot: next_due == kTimerIdle.  One-shot: period == 0.
 struct __align__(32) DevTimer {
   uint64_t next_due;
   uint64_t period;
@@ -168,7 +165,9 @@ struct FanoutParams {
   uint32_t prefetch_n;
   uint32_t batch_dep;         // 1: `batch` was produced by the previous launch (prefetch buffer): wait for it before staging
   const uint32_t* order;      // ORDERED build: active subscribers sorted by code mask (equal masks are neighbours)
-  uint32_t n_order, spw;      // ... how many, and how many consecutive positions each warp takes (<= 32)
+  uint32_t n_order, spw;      // ... how many, and how many consecutive positions each warp takes (<= 32).  Plain build: CTA b
+                              // owns subscribers [8 spw b, 8 spw (b + 1))
+  uint32_t stage_subs;        // plain build: subscribers whose control blocks and timer slots are staged in shared memory at a time
   uint64_t w_now;             // watermark: timers due <= w_now fire in this launch
   uint32_t n_ev, n_subs, ring_cap, K, sub_base;
   uint32_t use_digest, lossless, timers_on;
@@ -303,6 +302,14 @@ __device__ __forceinline__ void bulk_g2s(void* sdst, const void* gsrc, uint32_t 
                "l"(gsrc), "r"(bytes), "r"(smem_u32(mbar))
                : "memory");
 }
+// ... and with the evict_last L2 policy when `hinted`
+__device__ __forceinline__ void bulk_g2s_hint(void* sdst, const void* gsrc, uint32_t bytes, uint64_t* mbar, bool hinted) {
+  if (!hinted) { bulk_g2s(sdst, gsrc, bytes, mbar); return; }
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(
+                   smem_u32(sdst)),
+               "l"(gsrc), "r"(bytes), "r"(smem_u32(mbar)), "l"(keep_policy())
+               : "memory");
+}
 __device__ __forceinline__ void bulk_s2g(void* gdst, const void* ssrc, uint32_t bytes) {
   asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst), "r"(smem_u32(ssrc)),
                "r"(bytes)
@@ -336,9 +343,11 @@ __device__ __forceinline__ void mbar_wait(uint64_t* mbar, uint32_t parity) {
 //   [.., +160)            descriptor summary {present, has_unicast, hist[32]} (lands with the descriptor's bulk copy)
 //   [.., +4096)           PAIRS build only: presence filter of the batch's {code, source} keys (same bulk copy)
 //   then                  powers P^0 .. P^(cap+64), BatchSummary (mbarriers, per-CTA accumulators), per-warp tick scratch
+//   [fanout_stage_off, ..) plain build: control blocks [stage_subs], then timer slots [stage_subs][K] of the current round
 struct BatchSummary {
   uint64_t mbar;
   uint64_t mbar_desc;      // the descriptor's bulk copy (CTAs other than the one that built it)
+  uint64_t mbar_state;     // plain build: one phase per staging round of control blocks and timer slots
   uint32_t acc_deliv, acc_ticks, acc_pad[2];   // per-CTA statistics (flushed once at exit)
   uint32_t acc_dig_lo, acc_dig_hi;                     // sum of fold32(new digest), as two 16-bit-limb sums (native 32-bit atomics)
   uint32_t stream_local;   // stream mode: this batch was prefetched into local HBM by an earlier launch
@@ -354,6 +363,7 @@ __host__ __device__ inline size_t fanout_smem_bytes(uint32_t cap) {
   const size_t scratch = (cap / 2u > 32u ? cap / 2u : 32u) * sizeof(uint32_t);
   return (size_t)cap * 56 + 16 + 160 + (size_t)(cap + 66) * 8 + sizeof(BatchSummary) + kWarpsPerCta * scratch + 128;
 }
+__host__ __device__ inline size_t fanout_stage_off(uint32_t cap) { return (fanout_smem_bytes(cap) + 127) & ~(size_t)127; }
 
 // TIMERS=false compiles every timer/tick path out (the host knows when no timer is armed): fewer registers,
 // one more resident CTA per SM.
@@ -362,8 +372,12 @@ __host__ __device__ inline size_t fanout_smem_bytes(uint32_t cap) {
 // plus one filter pass per DISTINCT mask in the warp's block, instead of a filter pass per mailbox.
 // PAIRS (second-level filter, jobs/jobs.go:188-231): a subscriber whose mask word carries kPairBit also takes the broadcast
 // events that equal one of its exact {code, source} cases.  Such mailboxes go through the general two-pass path.
+// Plain build (neither ORDERED nor PAIRS): CTA b owns one contiguous range of subscribers.  Their control blocks and timer
+// slots arrive in shared memory by bulk copies, stage_subs subscribers per round, instead of as one scattered DRAM read per
+// mailbox in the middle of the ring write stream.
 template <int STORE, bool TIMERS, bool DIGEST, bool ORDERED, bool PAIRS = false>
 __global__ void __launch_bounds__(kThreads, CPBUS_CTAS_PER_SM) fanout_kernel(const FanoutParams p) {
+  constexpr bool STAGED = !ORDERED && !PAIRS;
   extern __shared__ __align__(128) unsigned char smem[];
   const uint32_t cap = p.smem_cap;
   cpbus_event* s_batch = reinterpret_cast<cpbus_event*>(smem);
@@ -375,6 +389,8 @@ __global__ void __launch_bounds__(kThreads, CPBUS_CTAS_PER_SM) fanout_kernel(con
   uint64_t* s_pow = s_q + cap + 2 + 20 + (PAIRS ? kPairFilterWords / 2 : 0);   // 16-byte aligned (TMA destination)
   BatchSummary* s_sum = reinterpret_cast<BatchSummary*>(s_pow + cap + 66);
   uint32_t* s_tick = reinterpret_cast<uint32_t*>(s_sum + 1);
+  const uint4* s_ctl4 = reinterpret_cast<const uint4*>(smem + fanout_stage_off(cap));   // STAGED: 2 halves per control block
+  const uint4* s_tim4 = s_ctl4 + 2u * p.stage_subs;                                      // ... and per timer slot
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const uint32_t n = p.n_ev;
@@ -386,20 +402,14 @@ __global__ void __launch_bounds__(kThreads, CPBUS_CTAS_PER_SM) fanout_kernel(con
   if (p.batch_dep) asm volatile("griddepcontrol.wait;" ::: "memory");
   const bool stream = p.staged == 2u;
   const uint32_t pf_slot = stream ? (uint32_t)(p.stream_seq % kStreamPrefetch) : 0u;
-  // position space: plain build = subscriber index, strided over the grid; ORDERED build = index into p.order, one
-  // contiguous block of p.spw positions per warp (lane l keeps the id at block position l: one coalesced load)
-  uint32_t pos = ORDERED ? (blockIdx.x * kWarpsPerCta + warp) * p.spw : blockIdx.x * kWarpsPerCta + warp;
+  // position space: plain build = subscriber index, set per staging round; PAIRS build = subscriber index, set per triage
+  // survivor; ORDERED build = index into p.order, one contiguous block of p.spw positions per warp (lane l keeps the id at
+  // block position l: one coalesced load)
+  uint32_t pos = ORDERED ? (blockIdx.x * kWarpsPerCta + warp) * p.spw : 0u;
   uint32_t my_ids = 0;
   if (ORDERED && pos + lane < min(pos + p.spw, p.n_order)) my_ids = __ldg(p.order + pos + lane);   // static data: safe before the wait
-  if (CPBUS_EARLY_PF && !ORDERED && pos < p.n_subs && lane == 0) {
-    // the first control block (and timer slot) of this warp: pull it towards L2 now, so that the load after the prologue
-    // does not pay a DRAM round trip behind the write stream.  L2 is the point of coherence: a prefetch can never make
-    // the later load see stale data, so this is safe before griddepcontrol.wait.
-    asm volatile("prefetch.global.L2 [%0];" ::"l"(p.ctl + pos));
-    if (TIMERS && p.timers_on && p.K) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.timers + (size_t)pos * p.K));
-  }
   if (tid == 0) {
-    mbar_init(&s_sum->mbar, 1); mbar_init(&s_sum->mbar_desc, 1);
+    mbar_init(&s_sum->mbar, 1); mbar_init(&s_sum->mbar_desc, 1); mbar_init(&s_sum->mbar_state, 1);
     s_sum->acc_deliv = 0; s_sum->acc_ticks = 0; s_sum->acc_dig_lo = 0; s_sum->acc_dig_hi = 0;
     // stream mode: an earlier launch (two back, so it is complete and visible) may already hold this batch locally
     s_sum->stream_local = (stream && __ldcg(p.pf_state + pf_slot) == p.stream_seq) ? 1u : 0u;
@@ -606,14 +616,27 @@ __global__ void __launch_bounds__(kThreads, CPBUS_CTAS_PER_SM) fanout_kernel(con
   const uint32_t tk_slot = lane / J, tk_j = lane % J;
   const bool timers_on = TIMERS && p.timers_on && K;
   const uint32_t wstride = gridDim.x * kWarpsPerCta;
-  uint32_t pos_end = aborted ? 0u : (ORDERED ? min(pos + p.spw, p.n_order) : p.n_subs);
-  const uint32_t pos_step = ORDERED ? 1u : wstride;
+  uint32_t pos_end = (aborted || !ORDERED) ? 0u : min(pos + p.spw, p.n_order);
+  const uint32_t pos_step = ORDERED ? 1u : kWarpsPerCta;   // (PAIRS: one position per triage turn)
   const uint32_t pos0 = pos;
   uint32_t s = ORDERED ? __shfl_sync(0xffffffffu, my_ids, 0) : pos;
   // ---- from here on the previous launch's results are needed: wait for it, then let the NEXT launch start its prologue
   // (the trigger comes after the wait so that a launch can never overlap its grand-parent: two descriptor buffers suffice)
   if (!p.batch_dep) asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("griddepcontrol.launch_dependents;");
+  // STAGED: this CTA's range is [rng_first, rng_end).  Thread 0 stages one round of it at a time (control blocks, then timer
+  // slots) on mbar_state.
+  const uint32_t rng_first = blockIdx.x * kWarpsPerCta * p.spw, rng_end = min(rng_first + kWarpsPerCta * p.spw, p.n_subs);
+  auto stage_round = [&](uint32_t first) {
+    if (!STAGED || tid != 0 || aborted || first >= rng_end) return;
+    const uint32_t rn = min(p.stage_subs, rng_end - first);
+    // the previous round's generic-proxy reads of the staging area are complete (barrier at the end of the turn)
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    const uint32_t tim_bytes = timers_on ? rn * K * (uint32_t)sizeof(DevTimer) : 0u;
+    mbar_expect_tx(&s_sum->mbar_state, rn * (uint32_t)sizeof(SubCtl) + tim_bytes);
+    bulk_g2s_hint(const_cast<uint4*>(s_ctl4), p.ctl + first, rn * (uint32_t)sizeof(SubCtl), &s_sum->mbar_state, keep);
+    if (tim_bytes) bulk_g2s_hint(const_cast<uint4*>(s_tim4), p.timers + (size_t)first * K, tim_bytes, &s_sum->mbar_state, keep);
+  };
   // ================= ORDERED build, no unicast in the batch: whole RUNS of equal masks at a time =================
   // The warp's block is <= 32 consecutive positions of the mask order; lane l owns position pos + l for the whole block
   // (its id is in my_ids, its control block in registers: ONE load instruction brings the block's control blocks in).
@@ -715,10 +738,7 @@ __global__ void __launch_bounds__(kThreads, CPBUS_CTAS_PER_SM) fanout_kernel(con
   }
   if (runs_done) pos = pos_end;   // nothing left for the per-mailbox loop below
   uint4 ca = make_uint4(0, 0, 0, 0), cb = ca, ta = ca;
-  if (!PAIRS && pos < pos_end) {   // software pipeline, stage 0: first subscriber's control block (and timer slot)
-    ld_sector(p.ctl + s, ca, cb, keep);
-    if (timers_on && tk_slot < K) ld_half(p.timers + (size_t)s * K + tk_slot, ta, keep);
-  }
+  if (ORDERED && pos < pos_end) ld_sector(p.ctl + s, ca, cb, keep);   // software pipeline, stage 0: first control block
   const uint32_t present = s_dsum[0];
   const bool has_unicast = s_dsum[1] != 0;
   // PAIRS build: TRIAGE.  A fleet of pair-filtered subscribers (jobs/jobs.go:188-231: every consumer listens for a dozen exact
@@ -731,7 +751,15 @@ __global__ void __launch_bounds__(kThreads, CPBUS_CTAS_PER_SM) fanout_kernel(con
   bool bulk_pending = false;
   uint32_t tri_blk = blockIdx.x * kWarpsPerCta + warp, tri_base = 0, tri_live = 0;
   uint4 tri_a = make_uint4(0, 0, 0, 0), tri_b = tri_a;
-  for (;;) {   // PAIRS: one surviving mailbox per turn; every other build: exactly one turn
+  uint32_t rnd_first = rng_first, rnd_phase = 0;   // STAGED: the current round starts at rnd_first
+  for (;;) {   // PAIRS: one surviving mailbox per turn; plain build: one staging round per turn; ORDERED: exactly one turn
+  if constexpr (STAGED) {
+    if (aborted || rnd_first >= rng_end) break;   // CTA-uniform
+    stage_round(rnd_first);
+    mbar_wait(&s_sum->mbar_state, rnd_phase);
+    rnd_phase ^= 1u;
+    pos = rnd_first + warp; pos_end = rnd_first + min(p.stage_subs, rng_end - rnd_first);
+  }
   if constexpr (PAIRS) {
     bool exhausted = aborted;
     while (!tri_live && !exhausted) {
@@ -782,28 +810,32 @@ __global__ void __launch_bounds__(kThreads, CPBUS_CTAS_PER_SM) fanout_kernel(con
   const uint32_t scratch_words = max(32u, cap / 2u);                   // per warp: 32 tick positions or cap u16 event indices
   uint32_t* my_tick = s_tick + warp * scratch_words;
 
-  // software pipeline: the control block (and timer slot) of the NEXT subscriber is in flight
-  // while the current one is being written, so no DRAM round trip is exposed per subscriber
+  // ORDERED: software pipeline, the control block of the NEXT subscriber is in flight while the current one is being
+  // written, so no DRAM round trip is exposed per subscriber.  STAGED: the round's state is in shared memory; halves are
+  // re-read where they are needed rather than kept in registers across the copy loops.
   uint32_t run_mask = 0xffffffffu, run_k = 0;   // ORDERED: the filter pass of the previous mailbox, reusable while the mask repeats
   uint64_t run_sum = 0;
   for (; pos < pos_end; pos += pos_step) {
-    const uint4 cur_a = ca, cur_b = cb, cur_ta = ta;
+    const uint32_t si = pos - rnd_first;   // STAGED: staging index
+    uint4 cur_a = ca, cur_b = cb;
+    // half h of this subscriber's control block / of its timer slot tk_slot
+    auto ctl_half = [&](uint32_t h) -> uint4 { return STAGED ? s_ctl4[2u * si + h] : (h ? cur_b : cur_a); };
+    auto tim_half = [&](uint32_t h) -> uint4 {
+      if (STAGED) return s_tim4[2u * (si * K + tk_slot) + h];
+      if (!h) return ta;
+      uint4 cold;
+      ld_half(reinterpret_cast<const unsigned char*>(p.timers + (size_t)s * K + tk_slot) + 16, cold, keep);
+      return cold;
+    };
+    if (STAGED) { cur_a = ctl_half(0); cur_b = ctl_half(1); }
     if (ORDERED) s = __shfl_sync(0xffffffffu, my_ids, (pos - pos0) & 31); else s = pos;
-    {
+    if (ORDERED) {
       const uint32_t pn = pos + pos_step;
-      if (pn < pos_end) {
-        const uint32_t sn = ORDERED ? __shfl_sync(0xffffffffu, my_ids, (pn - pos0) & 31) : pn;
-        ld_sector(p.ctl + sn, ca, cb, keep);
-        if (timers_on && tk_slot < K) ld_half(p.timers + (size_t)sn * K + tk_slot, ta, keep);
-        // fleets are homogeneous: if this mailbox has a pair table, the next one most likely has one too
-        if (PAIRS && (cur_b.z & kPairBit) && lane == 0)
-          asm volatile("prefetch.global.L2 [%0];" ::"l"(p.pairs + (size_t)sn * CPBUS_MAX_PAIRS));
-      }
+      if (pn < pos_end) ld_sector(p.ctl + __shfl_sync(0xffffffffu, my_ids, (pn - pos0) & 31), ca, cb, keep);
     }
     const uint32_t m = cur_b.z;
     if (!(m & kActiveBit)) continue;
     const uint64_t tail = ((uint64_t)cur_a.y << 32) | cur_a.x;
-    const uint64_t dig = ((uint64_t)cur_b.y << 32) | cur_b.x;
     cpbus_event* ring = p.ring + (size_t)s * p.ring_cap;
     const uint32_t gid = p.sub_base + s;
     const uint32_t nslots = timers_on ? min((m >> kTimerHintShift) & 0xFu, K) : 0u;
@@ -816,7 +848,8 @@ __global__ void __launch_bounds__(kThreads, CPBUS_CTAS_PER_SM) fanout_kernel(con
     if (nslots) {
       uint64_t tk_due0 = kTimerIdle;
       if (TIMERS && tk_slot < nslots) {
-        tk_due0 = ((uint64_t)cur_ta.y << 32) | cur_ta.x; tk_period = ((uint64_t)cur_ta.w << 32) | cur_ta.z;
+        const uint4 hot = tim_half(0);
+        tk_due0 = ((uint64_t)hot.y << 32) | hot.x; tk_period = ((uint64_t)hot.w << 32) | hot.z;
       }
       tk_due = tk_due0 + (uint64_t)tk_j * tk_period;
       tk_valid = tk_due0 != kTimerIdle && tk_due <= p.w_now && (tk_j == 0 || tk_period != 0);
@@ -889,9 +922,9 @@ __global__ void __launch_bounds__(kThreads, CPBUS_CTAS_PER_SM) fanout_kernel(con
       if (DIGEST) dsum = s_q[n];
     } else if (dense) {
       // ================= dense run with interleaved ticks: O(#ticks) bookkeeping =================
-      if (CPBUS_COLD_EARLY && TIMERS && tk_slot < nslots) {   // cold half of the timer slot {source_id, fired}: needed only for the tick records after the
-        uint4 cold;                        // copy loop, but issued HERE so that its DRAM round trip hides under the copy
-        ld_half(reinterpret_cast<const unsigned char*>(p.timers + (size_t)s * K + tk_slot) + 16, cold, keep);
+      constexpr bool cold_early = CPBUS_COLD_EARLY && !STAGED;
+      if (cold_early && TIMERS && tk_slot < nslots) {   // cold half of the timer slot {source_id, fired}: needed only for the tick records
+        const uint4 cold = tim_half(1);                 // after the copy loop, but loaded HERE so that its DRAM round trip hides under the copy
         tk_src = cold.x; tk_fired = cold.y;
       }
       if (tk_valid) my_tick[tk_rank] = tk_pos;
@@ -943,9 +976,8 @@ __global__ void __launch_bounds__(kThreads, CPBUS_CTAS_PER_SM) fanout_kernel(con
         copy_record_pairs<PLANAR>(s4, hi_off, ring, (uint32_t)tail, Rm, i, out, i < n);
       }
 #endif
-      if (!CPBUS_COLD_EARLY && TIMERS && tk_slot < nslots) {
-        uint4 cold;
-        ld_half(reinterpret_cast<const unsigned char*>(p.timers + (size_t)s * K + tk_slot) + 16, cold, keep);
+      if (!cold_early && TIMERS && tk_slot < nslots) {
+        const uint4 cold = tim_half(1);
         tk_src = cold.x; tk_fired = cold.y;
       }
       if (tk_valid) {
@@ -1111,9 +1143,8 @@ __global__ void __launch_bounds__(kThreads, CPBUS_CTAS_PER_SM) fanout_kernel(con
         copy_record_pairs<PLANAR>(s4, hi_off, ring, (uint32_t)tail, Rm, i, out, mine);
       }
       if (n_ticks) {
-        if (TIMERS && tk_slot < nslots) {   // cold half of the timer slot {source_id, fired}: loaded late, only when something fires
-          uint4 cold;
-          ld_half(reinterpret_cast<const unsigned char*>(p.timers + (size_t)s * K + tk_slot) + 16, cold, keep);
+        if (TIMERS && tk_slot < nslots) {   // cold half of the timer slot {source_id, fired}: read late, only when something fires
+          const uint4 cold = tim_half(1);
           tk_src = cold.x; tk_fired = cold.y;
         }
       }
@@ -1143,9 +1174,11 @@ __global__ void __launch_bounds__(kThreads, CPBUS_CTAS_PER_SM) fanout_kernel(con
       }
     }
     if (lane == 0 && k) {   // one full-sector write of the control block
+      const uint4 c0 = ctl_half(0), c1 = ctl_half(1);
+      const uint64_t dig = ((uint64_t)c1.y << 32) | c1.x;
       const uint64_t nt = tail + k;
       const uint64_t nd = DIGEST ? dig * s_pow[k] + dsum : dig;
-      st_sector(p.ctl + s, make_uint4((uint32_t)nt, (uint32_t)(nt >> 32), cur_a.z, cur_a.w),   // head: consumer-owned, passed through
+      st_sector(p.ctl + s, make_uint4((uint32_t)nt, (uint32_t)(nt >> 32), c0.z, c0.w),   // head: consumer-owned, passed through
                 make_uint4((uint32_t)nd, (uint32_t)(nd >> 32), m, 0u), keep);
       atomicAdd(&s_sum->acc_deliv, k);
       if (DIGEST) {
@@ -1157,8 +1190,12 @@ __global__ void __launch_bounds__(kThreads, CPBUS_CTAS_PER_SM) fanout_kernel(con
     }
   }
 
-  if constexpr (!PAIRS) break;
-  }   // triage turns
+  if constexpr (ORDERED) break;
+  if constexpr (STAGED) {
+    __syncthreads();   // every warp is done with this round's staging before the next round overwrites it
+    rnd_first += p.stage_subs;
+  }
+  }   // triage turns / staging rounds
   if (STORE == CPBUS_STORE_BULK && bulk_pending && lane == 0)
     asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // the staged batch must outlive the TMA reads
   __syncthreads();
