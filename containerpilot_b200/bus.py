@@ -185,6 +185,17 @@ class Bus:
     def stream_fanout(self, st, n: int, now_ns: int) -> int:
         return self._lib.cpbus_stream_fanout(st, n, now_ns)
 
+    def stream_admit(self, st, n: int, now_ns: int) -> int:
+        """lossless stream: how many of the current batch's undelivered records this shard can take.  Raises on an error,
+        CPBUS_EAGAIN included (an empty remainder whose ticks do not fit, or this bus's own staged events are blocked)."""
+        prefix = C.c_size_t()
+        nat.check(self._lib.cpbus_stream_admit(st, n, now_ns, C.byref(prefix)), "cpbus_stream_admit")
+        return prefix.value
+
+    def stream_fanout_prefix(self, st, n: int, now_ns: int, m: int) -> int:
+        """lossless stream: fan out the next m undelivered records; OK = batch complete, EAGAIN = records remain"""
+        return self._lib.cpbus_stream_fanout_prefix(st, n, now_ns, m)
+
     def stream_poll(self, st):
         """(n, now_ns) of the next batch if the publisher has released it, else None — for consumers that are not told"""
         ready, n, now = C.c_int(), C.c_size_t(), C.c_uint64()

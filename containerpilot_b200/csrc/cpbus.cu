@@ -93,6 +93,7 @@ struct cpbus {
   unsigned long long* d_desc_ready = nullptr;
   unsigned long long launch_seq = 0;
   cpbus_event* d_batch_local = nullptr;    // staged ingest: CTA 0's local copy of a peer batch
+  cpbus_event* d_admit_batch = nullptr;    // lossless stream: local copy of a slot's undelivered records for the admission pass
   static constexpr int kPrefetch = 3;      // fused ingest: later batches pulled over NVLink by earlier launches
   cpbus_event* d_prefetch[kPrefetch] = {};
   const void* pf_ptr[kPrefetch] = {};      // which peer batch sits in d_prefetch[i] ...
@@ -302,9 +303,10 @@ int launch_fanout_t(cpbus* b, const FanoutParams& p, uint32_t grid, size_t smem)
 }
 
 // fan out `n` records at d_src with watermark w (all checks done by the caller)
-struct StreamArgs {   // stream mode (cpbus_stream_fanout): where this batch's header / ack words live
+struct StreamArgs {   // stream mode (cpbus_stream_fanout_prefix): where this batch's header / ack words live
   const StreamHdr* hdr = nullptr; unsigned long long* ack = nullptr; unsigned long long seq = 0;
   const StreamHdr* next_hdr = nullptr;
+  uint32_t off = 0; bool final = true;   // records delivered before this launch; whether it completes the batch
 };
 
 int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, int staged = 0,
@@ -321,7 +323,10 @@ int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, in
   p.batch_local = b->d_batch_local; p.staged = (uint32_t)staged;
   p.err_word = b->d_err; p.acct = account ? b->d_acct : nullptr;
   p.pf_state = b->d_pf_state; p.pf_buf = b->d_pf_buf; p.pf_stride = b->B; p.spin_us = b->stream_spin_us;
-  if (sa) { p.stream_hdr = sa->hdr; p.stream_ack = sa->ack; p.stream_seq = sa->seq; p.stream_next_hdr = sa->next_hdr; }
+  if (sa) {
+    p.stream_hdr = sa->hdr; p.stream_ack = sa->ack; p.stream_seq = sa->seq; p.stream_next_hdr = sa->next_hdr;
+    p.stream_off = sa->off; p.stream_final = sa->final ? 1u : 0u;
+  }
   p.prefetch_src = prefetch_src; p.prefetch_dst = prefetch_dst; p.prefetch_n = prefetch_n;
   p.batch_dep = batch_dep ? 1u : 0u; p.n_ev = n;
   p.n_subs = b->n_next; p.ring_cap = b->R; p.K = b->K; p.sub_base = b->cfg.sub_id_base;
@@ -412,17 +417,21 @@ int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, in
 }
 
 // lossless admission (reference: the sender blocks on a full channel, events/subscriber.go:30-32)
-int admit(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, bool* ok, uint32_t* prefix = nullptr) {
-  *ok = true;
-  if (prefix) *prefix = n;
-  if (!b->lossless || b->n_next == 0) return CPBUS_OK;
+// Fast path: true when n records with watermark w provably fit (or nothing has to be admitted) — no kernel, no sync.
+bool admit_fits(cpbus* b, uint32_t n, uint64_t w) {
+  if (!b->lossless || b->n_next == 0) return true;
   // the most this launch can append to ONE mailbox: every event of the batch + every firing of its timer slots in the window
   uint64_t need = n;
   if (b->n_timers && b->K) {
     const uint64_t per_slot = (b->min_period != UINT64_MAX && w > b->last_watermark) ? (w - b->last_watermark) / b->min_period + 2 : 2;
     need += (uint64_t)b->K * per_slot;
   }
-  if (b->room_lb >= need) { b->room_lb -= need; b->st.admit_skipped++; return CPBUS_OK; }   // provably fits: no kernel, no sync
+  if (b->room_lb >= need) { b->room_lb -= need; b->st.admit_skipped++; return true; }
+  return false;
+}
+
+// The admission pass (after admit_fits said no): one kernel over every mailbox of the shard, then a host sync.
+int admit_pass(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, bool* ok, uint32_t* prefix) {
   CK(cudaMemsetAsync(&b->d_stats->admit_overflow, 0, 4 * sizeof(unsigned long long), b->stream));   // overflow, overwritten, max_used, deficit
   const uint32_t threads = 256, grid = (b->n_next + threads - 1) / threads;
   admit_kernel<<<grid, threads, 0, b->stream>>>(d_src, n, w, b->d_ctl, b->d_timers, b->n_next, b->R, b->K,
@@ -440,6 +449,13 @@ int admit(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, bool* ok, 
   // keep the conservative figure either way
   b->room_lb = used >= b->R ? 0 : b->R - used;
   return CPBUS_OK;
+}
+
+int admit(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, bool* ok, uint32_t* prefix = nullptr) {
+  *ok = true;
+  if (prefix) *prefix = n;
+  if (admit_fits(b, n, w)) return CPBUS_OK;
+  return admit_pass(b, d_src, n, w, ok, prefix);
 }
 
 // host mirror of one-shot timers that have fired on the device (events/timer.go:19-33):
@@ -685,6 +701,7 @@ int cpbus_create(const cpbus_config* cfg, cpbus_t** out) try {
     if (cudaEventCreateWithFlags(&b->consumed[i], cudaEventDisableTiming) != cudaSuccess) return fail(CPBUS_ECUDA);
   }
   ALLOC(b->d_batch_local, (size_t)B * sizeof(cpbus_event));
+  if (b->lossless) ALLOC(b->d_admit_batch, (size_t)B * sizeof(cpbus_event));
   ALLOC(b->d_pf_buf, (size_t)kStreamPrefetch * B * sizeof(cpbus_event)); ALLOC(b->d_pf_state, 64);
   ALLOC(b->d_acct, sizeof(DevPubAcct));
   if (cudaMemsetAsync(b->d_pf_state, 0, 64, b->stream) != cudaSuccess ||
@@ -744,7 +761,7 @@ int cpbus_destroy(cpbus_t* b) try {
   if (b->copy_stream) cudaStreamDestroy(b->copy_stream);
   if (b->launched) cudaEventDestroy(b->launched);
   cudaFree(b->d_drain); cudaFree(b->d_drain_idx);
-  cudaFree(b->d_result); cudaFree(b->d_batch_local); cudaFree(b->d_pf_buf); cudaFree(b->d_pf_state); cudaFree(b->d_acct);
+  cudaFree(b->d_result); cudaFree(b->d_batch_local); cudaFree(b->d_admit_batch); cudaFree(b->d_pf_buf); cudaFree(b->d_pf_state); cudaFree(b->d_acct);
   if (b->h_err) cudaFreeHost(b->h_err);
   if (b->h_acct) cudaFreeHost(b->h_acct);
   for (int i = 0; i < cpbus::kPrefetch; i++) cudaFree(b->d_prefetch[i]);
@@ -1274,6 +1291,8 @@ struct cpbus_stream {
   unsigned long long* ack = nullptr;         // consumer c's word is ack[4 * c] (one sector each)
   cpbus_event* payload = nullptr;
   unsigned long long put_seq = 0, get_seq = 0;   // batches released / fanned out so far (ordinals are 1-based)
+  uint32_t get_off = 0;                      // lossless mode: records of batch get_seq + 1 already delivered
+  unsigned long long seen_seq = 0;           // highest batch whose release this consumer has seen from the host
   unsigned long long pub_seq = 0;            // publisher: publish ordinal stamped into the next record (CPBUS_PUT_STAMP)
   unsigned long long min_ack = 0;            // publisher: cached min over the consumers' acks
   // publisher staging: pinned payload + header buffers, copies on their own stream
@@ -1294,7 +1313,6 @@ static int stream_bind(cpbus_stream* st) {
 
 int cpbus_stream_create(cpbus_t* b, uint32_t n_slots, uint32_t n_consumers, cpbus_stream_t** out, unsigned char handle[64]) try {
   if (!b || !out || !handle || n_slots < 4 || n_consumers == 0 || n_consumers > kStreamMaxConsumers) return CPBUS_EINVAL;
-  if (b->lossless) return CPBUS_EINVAL;   // admission would have to see every shard: throughput mode only
   *out = nullptr;
   int rc = dev_guard(b); if (rc) return rc;
   cpbus_stream* st = new (std::nothrow) cpbus_stream();
@@ -1325,7 +1343,6 @@ int cpbus_stream_create(cpbus_t* b, uint32_t n_slots, uint32_t n_consumers, cpbu
 
 int cpbus_stream_open(cpbus_t* b, const unsigned char handle[64], uint32_t consumer_index, cpbus_stream_t** out) try {
   if (!b || !out || !handle || consumer_index == 0 || consumer_index >= kStreamMaxConsumers) return CPBUS_EINVAL;
-  if (b->lossless) return CPBUS_EINVAL;
   *out = nullptr;
   int rc = dev_guard(b); if (rc) return rc;      // the IMPORTING device must be current: the mapping is made for it
   cpbus_stream* st = new (std::nothrow) cpbus_stream();
@@ -1353,7 +1370,7 @@ int cpbus_stream_open(cpbus_t* b, const unsigned char handle[64], uint32_t consu
 // pointer is used directly, with peer access enabled when the consumer's bus lives on another GPU.
 int cpbus_stream_attach(cpbus_t* b, cpbus_stream_t* owner, uint32_t consumer_index, cpbus_stream_t** out) try {
   if (!b || !owner || !owner->owner || !out || consumer_index == 0 || consumer_index >= owner->n_consumers) return CPBUS_EINVAL;
-  if (b->lossless || b->B != owner->B) return CPBUS_EINVAL;
+  if (b->B != owner->B) return CPBUS_EINVAL;
   *out = nullptr;
   int rc = dev_guard(b); if (rc) return rc;
   if (b->device != owner->bus->device) {
@@ -1466,27 +1483,118 @@ int cpbus_stream_poll(cpbus_stream_t* st, int* ready, size_t* n, uint64_t* now_n
   return CPBUS_OK;
 } CPBUS_CATCH
 
-// Every rank (the publisher's included): fan out the next batch of the stream to this GPU's shard.
-int cpbus_stream_fanout(cpbus_stream_t* st, size_t n, uint64_t now_ns) try {
-  if (!st || n > st->B) return CPBUS_EINVAL;
+// Lossless stream, slow path only: before the host copies or reads records of batch q outside the fan-out kernel (which
+// acquires the slot header itself), it waits until the publisher has released the batch — the payload lands before the
+// header.  Bounded by the stream timeout; once per batch.
+static int stream_wait_released(cpbus_stream* st, unsigned long long q, size_t n) {
+  if (st->seen_seq >= q) return CPBUS_OK;
+  cpbus* b = st->bus;
+  const auto t0 = std::chrono::steady_clock::now();
+  const auto budget = std::chrono::microseconds(b->stream_spin_us ? b->stream_spin_us : 2000000u);
+  for (;;) {
+    StreamHdr h{};
+    CK(cudaMemcpyAsync(&h, &st->hdr[q % st->n_slots], sizeof(h), cudaMemcpyDeviceToHost, b->result_stream));
+    CK(cudaStreamSynchronize(b->result_stream));
+    if (h.seq == q) {
+      if (h.n != n) return CPBUS_EINVAL;   // the caller's shape is not the released batch's
+      st->seen_seq = q;
+      return CPBUS_OK;
+    }
+    if (std::chrono::steady_clock::now() - t0 > budget) return CPBUS_ETIMEDOUT;
+    std::this_thread::sleep_for(std::chrono::microseconds(20));
+  }
+}
+
+// The checks every stream call makes before it admits or launches anything (clock, window, this bus's own staged events).
+static int stream_enter(cpbus_stream* st, uint64_t now_ns) {
   cpbus* b = st->bus;
   int rc = dev_guard(b); if (rc) return rc;
   if (*(volatile unsigned int*)b->h_err) return CPBUS_ETIMEDOUT;
   if ((rc = flush_staged(b, b->now))) return rc;
   if (now_ns < b->now) return CPBUS_EORDER;
   if (now_ns - b->last_watermark > max_window(b)) return CPBUS_EORDER;
-  b->now = now_ns;
+  return CPBUS_OK;
+}
+
+int cpbus_stream_admit(cpbus_stream_t* st, size_t n, uint64_t now_ns, size_t* prefix) try {
+  if (!st || !prefix || n > st->B || st->get_off > n) return CPBUS_EINVAL;
+  *prefix = 0;
+  cpbus* b = st->bus;
+  int rc = stream_enter(st, now_ns); if (rc) return rc;
+  const uint32_t rem = (uint32_t)n - st->get_off;
+  if (admit_fits(b, rem, now_ns)) { *prefix = rem; return CPBUS_OK; }   // no kernel, no sync
+  // Slow path: the admission kernel reads the whole remainder from every CTA, so it runs on a local copy of it (one peer
+  // copy on the bus stream) rather than over the link.  (Not d_batch_local: the fan-out kernel writes that one.)
+  const unsigned long long q = st->get_seq + 1;
+  if ((rc = stream_wait_released(st, q, n))) return rc;
+  if (rem)
+    CK(cudaMemcpyAsync(b->d_admit_batch, st->payload + (size_t)(q % st->n_slots) * st->B + st->get_off,
+                       (size_t)rem * sizeof(cpbus_event), cudaMemcpyDefault, b->stream));
+  bool ok = true;
+  uint32_t m = rem;
+  if ((rc = admit_pass(b, b->d_admit_batch, rem, now_ns, &ok, &m))) return rc;
+  if (!ok && m == rem) {
+    // Every record fits, but not the ticks due after the last of them (records older than now_ns, or none at all): the
+    // batch cannot complete yet.  Hold back its last record, or report the stall when there is none.
+    if (rem == 0) return CPBUS_EAGAIN;
+    m = rem - 1;
+  }
+  *prefix = m;
+  return CPBUS_OK;
+} CPBUS_CATCH
+
+// Fan out the next m undelivered records of the current batch (throughput mode: m = the whole batch, in one launch).
+static int stream_fanout_prefix(cpbus_stream* st, size_t n, uint64_t now_ns, size_t m) {
+  cpbus* b = st->bus;
+  int rc = stream_enter(st, now_ns); if (rc) return rc;
+  const bool final = m == n - st->get_off;
+  if (m == 0 && !final) return CPBUS_EAGAIN;
   const unsigned long long q = st->get_seq + 1;
   StreamArgs sa;
   const uint32_t slot = (uint32_t)(q % st->n_slots), slot2 = (uint32_t)((q + 2) % st->n_slots);
-  sa.hdr = &st->hdr[slot]; sa.ack = &st->ack[4 * st->consumer]; sa.seq = q; sa.next_hdr = &st->hdr[slot2];
-  rc = launch_fanout(b, st->payload + (size_t)slot * st->B, (uint32_t)n, now_ns, /*staged=*/2,
-                     st->payload + (size_t)slot2 * st->B, b->d_pf_buf + (size_t)((q + 2) % kStreamPrefetch) * b->B, 0,
-                     /*batch_dep=*/false, /*account=*/true, &sa);
+  sa.hdr = &st->hdr[slot]; sa.ack = &st->ack[4 * st->consumer]; sa.seq = q; sa.off = st->get_off; sa.final = final;
+  const cpbus_event* src = st->payload + (size_t)slot * st->B + st->get_off;
+  uint64_t w = now_ns;
+  if (!final) {
+    // Like a partial cpbus_flush: the watermark is the last delivered record's timestamp, so the ticks due after it go with
+    // the remainder.  Read from the slot (8 bytes) rather than assumed to be now_ns: RAW records may be older.
+    if ((rc = stream_wait_released(st, q, n))) return rc;
+    uint64_t ts = 0;
+    CK(cudaMemcpyAsync(&ts, &src[m - 1].ts_ns, sizeof(ts), cudaMemcpyDefault, b->result_stream));
+    CK(cudaStreamSynchronize(b->result_stream));
+    w = std::min(now_ns, std::max(ts, b->last_watermark));
+  }
+  // The clock follows the launched watermark.  Were it set to now_ns before the batch completes, the next call's flush of
+  // this bus's own staged events would fire the ticks due by now_ns on their own, in front of the undelivered records and
+  // without their admission.
+  b->now = w;
+  if (b->lossless) {   // no device-managed prefetch: a batch may take several launches, each reads its part of the slot
+    rc = launch_fanout(b, src, (uint32_t)m, w, /*staged=*/2, nullptr, nullptr, 0, /*batch_dep=*/false, /*account=*/true, &sa);
+  } else {
+    sa.next_hdr = &st->hdr[slot2];
+    rc = launch_fanout(b, src, (uint32_t)m, w, /*staged=*/2,
+                       st->payload + (size_t)slot2 * st->B, b->d_pf_buf + (size_t)((q + 2) % kStreamPrefetch) * b->B, 0,
+                       /*batch_dep=*/false, /*account=*/true, &sa);
+  }
   if (rc) return rc;
-  st->get_seq = q;
-  b->st.publishes += n; b->seq += n;
-  return CPBUS_OK;
+  b->st.publishes += m; b->seq += m;
+  if (final) { st->get_seq = q; st->get_off = 0; return CPBUS_OK; }
+  st->get_off += (uint32_t)m;
+  b->room_lb = 0;
+  b->st.admit_partial++;
+  return CPBUS_EAGAIN;
+}
+
+int cpbus_stream_fanout_prefix(cpbus_stream_t* st, size_t n, uint64_t now_ns, size_t m) try {
+  if (!st || n > st->B || st->get_off > n || m > n - st->get_off) return CPBUS_EINVAL;
+  return stream_fanout_prefix(st, n, now_ns, m);
+} CPBUS_CATCH
+
+// Every rank (the publisher's included): fan out the next batch of the stream to this GPU's shard.
+int cpbus_stream_fanout(cpbus_stream_t* st, size_t n, uint64_t now_ns) try {
+  if (!st || n > st->B || st->get_off > n) return CPBUS_EINVAL;
+  if (st->bus->lossless) return CPBUS_EINVAL;   // without admission this shard could deliver more than another one does
+  return stream_fanout_prefix(st, n, now_ns, n - st->get_off);
 } CPBUS_CATCH
 
 static int read_cursors(cpbus* b, uint32_t l, uint64_t* tail, uint64_t* head, uint64_t* lost = nullptr) {

@@ -180,6 +180,8 @@ struct FanoutParams {
   unsigned long long* stream_ack;    // this consumer's ack word in the publisher's HBM
   unsigned long long stream_seq;     // 1-based ordinal of the batch this launch fans out
   const StreamHdr* stream_next_hdr;  // header of batch stream_seq + 2 (prefetch_src = its payload), or nullptr
+  uint32_t stream_off;               // records of this batch delivered by earlier launches (`batch` = slot payload + stream_off)
+  uint32_t stream_final;             // 1: this launch completes the batch (header n == stream_off + n_ev) and acknowledges the slot
   unsigned long long* pf_state;      // [kStreamPrefetch] local: pf_state[q % 3] == q  <=>  batch q sits in pf_buf slot q % 3
   cpbus_event* pf_buf;               // kStreamPrefetch local buffers of pf_stride records
   uint32_t pf_stride;
@@ -411,8 +413,9 @@ __global__ void __launch_bounds__(kThreads, CPBUS_CTAS_PER_SM) fanout_kernel(con
   if (tid == 0) {
     mbar_init(&s_sum->mbar, 1); mbar_init(&s_sum->mbar_desc, 1); mbar_init(&s_sum->mbar_state, 1);
     s_sum->acc_deliv = 0; s_sum->acc_ticks = 0; s_sum->acc_dig_lo = 0; s_sum->acc_dig_hi = 0;
-    // stream mode: an earlier launch (two back, so it is complete and visible) may already hold this batch locally
-    s_sum->stream_local = (stream && __ldcg(p.pf_state + pf_slot) == p.stream_seq) ? 1u : 0u;
+    // stream mode: an earlier launch (two back, so it is complete and visible) may already hold this batch locally.  Not in
+    // lossless mode (no launch prefetches there) and not for a resumed batch (stream_off > 0): those always read the slot
+    s_sum->stream_local = (stream && !p.lossless && p.stream_off == 0 && __ldcg(p.pf_state + pf_slot) == p.stream_seq) ? 1u : 0u;
     s_sum->own_desc = blockIdx.x == 0 ? 1u : 0u; s_sum->abort_launch = 0;
   }
   __syncthreads();
@@ -497,7 +500,8 @@ __global__ void __launch_bounds__(kThreads, CPBUS_CTAS_PER_SM) fanout_kernel(con
         else {
           uint32_t hn;
           asm volatile("ld.relaxed.sys.global.u32 %0, [%1];" : "=r"(hn) : "l"(&p.stream_hdr->n) : "memory");
-          if (hn != n) err = kErrStreamShape;
+          // a final launch takes the batch's last records; a partial one (lossless mode) leaves some behind
+          if (p.stream_final ? hn != p.stream_off + n : hn <= p.stream_off + n) err = kErrStreamShape;
         }
         if (err) {
           s_sum->abort_launch = 1u;
@@ -520,7 +524,7 @@ __global__ void __launch_bounds__(kThreads, CPBUS_CTAS_PER_SM) fanout_kernel(con
     }
     mbar_wait(&s_sum->mbar, 0);
     __syncthreads();
-    if (lead && stream && tid == 0 && !ab)   // the batch is out of the shared ring: the publisher may reuse the slot
+    if (lead && stream && tid == 0 && !ab && p.stream_final)   // the batch is out of the shared ring: the publisher may reuse the slot
       asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(p.stream_ack), "l"(p.stream_seq) : "memory");
     const uint32_t nd = ab ? 0u : n;
     {

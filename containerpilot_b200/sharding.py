@@ -9,7 +9,8 @@ Two drivers over the same C-ABI:
 * `ShardedBus`      — one process per GPU (`torch.distributed.run`); torch.distributed (NCCL or gloo) is used ONLY for the
                       construction handshake (the 64-byte CUDA-IPC handle) and for reducing statistics.
 * `LocalShardedBus` — one process driving G buses (what a cgo shim inside the single ContainerPilot process does):
-                      `cpbus_stream_attach`, peer access instead of IPC; also runs with all shards on ONE GPU.
+                      `cpbus_stream_attach`, peer access instead of IPC; also runs with all shards on ONE GPU.  Also in
+                      lossless mode (`cpbus_stream_admit` on every shard, then `cpbus_stream_fanout_prefix` of the minimum).
 """
 from __future__ import annotations
 
@@ -233,16 +234,18 @@ class ShardedBus(_ShardOps):
 
 class LocalShardedBus:
     """G shards driven by ONE process (shard g on `devices[g]`; all on one GPU is allowed): what a cgo shim inside the
-    single ContainerPilot process does.  Same stream protocol as `ShardedBus`, attached in-process."""
+    single ContainerPilot process does.  Same stream protocol as `ShardedBus`, attached in-process.  `lossless=True` gives every
+    shard the reference's blocking semantics: a publish stops at the event the Go bus would block on, on every shard."""
 
     def __init__(self, n_subs_total: int, devices, ring_cap: int = 1024, batch_cap: int = 512, timers_per_sub: int = 0,
-                 digest: bool = True, stream_slots: int = 64):
+                 digest: bool = True, stream_slots: int = 64, lossless: bool = False):
         self.world = len(devices)
+        self.lossless = lossless
         self.shards = []
         for g, dev in enumerate(devices):
             first, count = shard_range(n_subs_total, self.world, g)
             self.shards.append((first, count, Bus(max(count, 1), ring_cap=ring_cap, batch_cap=batch_cap, timers_per_sub=timers_per_sub,
-                                                  digest=digest, device=dev, sub_id_base=first)))
+                                                  lossless=lossless, digest=digest, device=dev, sub_id_base=first)))
         pub = self.shards[0][2]
         st0, _ = pub.stream_create(stream_slots, self.world)
         self._st = [st0] + [self.shards[g][2].stream_attach(st0, g) for g in range(1, self.world)]
@@ -265,19 +268,51 @@ class LocalShardedBus:
             if count:
                 bus.timer_add_many(first, count, period_ns, source_id0=source_id0 + first)
 
-    def publish(self, events: np.ndarray, now_ns: int, raw: bool = False):
-        """One batch to every shard: put once, fan out on each GPU (never ahead of its own fan-outs, so it may wait)."""
+    def publish(self, events: np.ndarray, now_ns: int, raw: bool = False) -> int:
+        """One batch to every shard: put once, fan out on each GPU (never ahead of its own fan-outs, so it may wait).
+        Lossless mode: returns what `fanout` returns (EAGAIN: drain, then call `fanout` with the same shape)."""
         nat.check(self.shards[0][2].stream_put(self._st[0], events, now_ns, raw), "cpbus_stream_put")
-        self.fanout(len(events), now_ns)
+        return self.fanout(len(events), now_ns)
 
     def put(self, events: np.ndarray, now_ns: int, raw: bool = False) -> int:
         """Run ahead of the fan-outs.  One thread drives publisher and consumers here, so this never waits: EAGAIN means
         "fan out (or sync) first" — the slot's previous batch has not been pulled by every shard yet."""
         return self.shards[0][2].stream_put(self._st[0], events, now_ns, raw, nowait=True)
 
-    def fanout(self, n: int, now_ns: int):
+    def fanout(self, n: int, now_ns: int) -> int:
+        """Fan the next batch out to every shard.  Lossless mode: every shard admits what its mailboxes can take and every
+        shard delivers the shortest of those prefixes, so a stalled publish stops at the same event everywhere.  Returns
+        nat.OK (batch complete) or nat.EAGAIN (records remain: let the consumers drain, then call again with the same
+        n and now_ns — the batch resumes at its first undelivered record)."""
+        if not self.lossless:
+            for g, (_, _, bus) in enumerate(self.shards):
+                nat.check(bus.stream_fanout(self._st[g], n, now_ns), "cpbus_stream_fanout")
+            return nat.OK
+        m = None
         for g, (_, _, bus) in enumerate(self.shards):
-            nat.check(bus.stream_fanout(self._st[g], n, now_ns), "cpbus_stream_fanout")
+            try:
+                p = bus.stream_admit(self._st[g], n, now_ns)
+            except nat.CpbusError as ex:
+                if ex.status != nat.EAGAIN:
+                    raise
+                return nat.EAGAIN                   # nothing can go out on this shard, so nothing goes out anywhere
+            m = p if m is None else min(m, p)
+        rc = nat.OK
+        for g, (_, _, bus) in enumerate(self.shards):
+            r = bus.stream_fanout_prefix(self._st[g], n, now_ns, m)
+            if r not in (nat.OK, nat.EAGAIN):
+                nat.check(r, "cpbus_stream_fanout_prefix")
+            rc = r
+        return rc
+
+    def drain(self, sub_id: int, cap: int | None = None) -> np.ndarray:
+        """Consumer side: up to `cap` records of global subscriber `sub_id`, from the shard that owns it."""
+        return self.bus_of(sub_id).drain(sub_id, cap)
+
+    def consume_all(self):
+        """Device-side consumer on every shard: every mailbox read to the end, records discarded."""
+        for _, _, bus in self.shards:
+            bus.consume_all()
 
     def sync(self):
         for _, _, bus in self.shards:

@@ -244,11 +244,21 @@ int cpbus_publish_device_staged(cpbus_t* bus, const void* d_events, size_t n, ui
  * broadcast is fused into the fan-out launch; there is no collective, no copy-engine op and no cross-stream wait on the
  * consumers' data path.  When the publisher runs >= 2 batches ahead, the lead CTA of batch q also pulls batch q+2 while
  * its own stores are in flight, so later launches start from local memory and keep their prologue overlapped with the
- * previous launch (programmatic dependent launch).  Throughput (overwrite-oldest) mode only.
+ * previous launch (programmatic dependent launch).
  *   publisher rank : cpbus_stream_create(bus, n_slots, n_consumers, &st, handle); send `handle` to the other ranks
  *   other ranks    : cpbus_stream_open(bus, handle, consumer_index (1..n_consumers-1), &st)
  *   every step     : [publisher] cpbus_stream_put(st, events, n, now_ns, flags)   (may run ahead by < n_slots batches)
  *                    [all ranks] cpbus_stream_fanout(st, n, now_ns)
+ * Lossless mode (CPBUS_CFG_LOSSLESS): a stalled publish must stop at the same event on every shard — the shortest of the
+ * prefixes the shards can take — so the fan-out is split in two and the driver takes the minimum in between:
+ *   every step     : [publisher] cpbus_stream_put(st, events, n, now_ns, flags)
+ *                    [all shards] cpbus_stream_admit(st, n, now_ns, &p_g)      m = min over the shards of p_g
+ *                    [all shards] cpbus_stream_fanout_prefix(st, n, now_ns, m)
+ *                    CPBUS_EAGAIN (from an admit, or from fanout_prefix: records remain): let the consumers drain, then admit
+ *                    and fan out again with the same (n, now_ns); the batch resumes at its first undelivered record.
+ * While the mailboxes provably have room, admission costs no kernel and no host sync (as for cpbus_flush).  A batch's slot
+ * is acknowledged only when its last record has been fanned out, so the publisher cannot run more than n_slots batches
+ * ahead of the slowest shard.  Plain cpbus_stream_fanout returns CPBUS_EINVAL on a lossless bus.
  * The consumers must be told n and now_ns of every batch by the caller: SPMD drivers know them; others ask cpbus_stream_poll,
  * which reads them from the slot header (the kernel cross-checks n either way).  CPBUS_EAGAIN from _put: the slot's previous batch is still not acknowledged by every
  * consumer after the stream timeout (or at once with CPBUS_PUT_NOWAIT) — call again after the consumers have advanced.  CPBUS_ETIMEDOUT from _fanout/_status: an earlier stream
@@ -269,6 +279,22 @@ int cpbus_stream_open(cpbus_t* bus, const unsigned char handle[64], uint32_t con
 int cpbus_stream_attach(cpbus_t* bus, cpbus_stream_t* owner, uint32_t consumer_index, cpbus_stream_t** out);
 int cpbus_stream_put(cpbus_stream_t* st, const cpbus_event* events, size_t n, uint64_t now_ns, uint32_t flags);
 int cpbus_stream_fanout(cpbus_stream_t* st, size_t n, uint64_t now_ns);
+/* Lossless stream.  *prefix = how many of the current batch's undelivered records this shard's mailboxes can take (every
+ * record of the batch up to then, plus the ticks due by the last of them); the whole remainder means the batch can complete,
+ * the ticks due by now_ns included.  Where only those trailing ticks do not fit (records older than now_ns), the last record
+ * is held back; an empty remainder whose ticks do not fit gives CPBUS_EAGAIN.  First flushes the bus's own staged events
+ * (CPBUS_EAGAIN propagates) and checks the clock like cpbus_stream_fanout (CPBUS_EORDER).  The admission kernel runs, on a
+ * local copy of the remainder, only when the fast path cannot prove the fit.  On a throughput-mode bus it is the whole
+ * remainder, with no kernel. */
+int cpbus_stream_admit(cpbus_stream_t* st, size_t n, uint64_t now_ns, size_t* prefix);
+/* Fan out the next m undelivered records of the current batch (n, now_ns = the batch's full shape, as for
+ * cpbus_stream_fanout).  Returns CPBUS_OK when the batch is complete: the slot is acknowledged and the stream moves to the
+ * next batch.  Returns CPBUS_EAGAIN when records remain (m == 0: nothing is launched): the caller lets consumers drain, then
+ * admits and fans out again.  A partial launch's watermark is its last record's ts_ns, and the bus clock moves only that far
+ * until the batch completes, so the ticks due after it go with the remainder.  m beyond the remainder: CPBUS_EINVAL (m is
+ * the minimum of the shards' admitted prefixes; more than this shard admitted would overfill a mailbox).  An empty batch
+ * has a remainder of 0: m = 0 completes it. */
+int cpbus_stream_fanout_prefix(cpbus_stream_t* st, size_t n, uint64_t now_ns, size_t m);
 /* For a consumer whose driver does not know the batches' shapes: *ready = 1 and {n, now_ns} of the NEXT batch if the publisher
  * has released it, *ready = 0 otherwise (one 32-byte read of the slot header, synchronous).  Then cpbus_stream_fanout(st, n, now_ns). */
 int cpbus_stream_poll(cpbus_stream_t* st, int* ready, size_t* n, uint64_t* now_ns);
