@@ -99,6 +99,8 @@ SYMBOLS = {
     "cpbus_shared_close": (C.c_int, [C.c_void_p, C.c_void_p]),
     "cpbus_drain": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t, _P(C.c_size_t), _P(C.c_uint64)]),
     "cpbus_drain_many": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, _P(C.c_size_t)]),
+    "cpbus_drain_ready": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p,
+                                    C.c_size_t, _P(C.c_size_t), _P(C.c_size_t), _P(C.c_uint32)]),
     "cpbus_consume_all": (C.c_int, [C.c_void_p]),
     "cpbus_peek_window": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t, _P(C.c_size_t)]),
     "cpbus_digest": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]),

@@ -14,6 +14,9 @@ from . import _native as nat
 EVENT_DTYPE = np.dtype([("seq", "<u8"), ("ts_ns", "<u8"), ("code", "<u4"), ("source_id", "<u4"),
                         ("target", "<u4"), ("flags", "<u4")])
 assert EVENT_DTYPE.itemsize == 32
+# cpbus_ready: one entry of cpbus_drain_ready's ready list
+READY_DTYPE = np.dtype([("sub_id", "<u4"), ("count", "<u4"), ("offset", "<u4"), ("pad", "<u4"), ("lost", "<u8")])
+assert READY_DTYPE.itemsize == 24
 
 
 class Bus:
@@ -247,6 +250,22 @@ class Bus:
         nat.check(self._lib.cpbus_drain_many(self._h, first_sub, n, out.ctypes.data, cap, offs.ctypes.data, cnts.ctypes.data,
                                              C.byref(total)), "cpbus_drain_many")
         return out, offs, cnts
+
+    def drain_ready(self, first_sub: int, n: int, start_sub: int, cap: int, ready_cap: int, out=None):
+        """Sparse drain of mailboxes [first_sub, first_sub+n) in cyclic order from start_sub: returns (records, ready,
+        next_sub).  ready is a READY_DTYPE array with one entry per mailbox taken; entry i's FIFO run is
+        records[ready[i].offset : ready[i].offset + ready[i].count].  Pass next_sub back as start_sub to continue.
+        `out`: a preallocated EVENT_DTYPE array of at least `cap` records; records is a view of it."""
+        if out is None:
+            out = np.zeros(cap, dtype=EVENT_DTYPE)
+        if len(out) < cap:
+            raise ValueError("out holds fewer than cap records")
+        ready = np.zeros(min(ready_cap, n), dtype=READY_DTYPE)
+        n_ready, total, next_sub = C.c_size_t(), C.c_size_t(), C.c_uint32()
+        nat.check(self._lib.cpbus_drain_ready(self._h, first_sub, n, start_sub, out.ctypes.data, cap, ready.ctypes.data,
+                                              ready_cap, C.byref(n_ready), C.byref(total), C.byref(next_sub)),
+                  "cpbus_drain_ready")
+        return out[: total.value], ready[: n_ready.value], next_sub.value
 
     def peek_window(self, sub_id: int, cap: int | None = None) -> np.ndarray:
         cap = cap or self.ring_cap

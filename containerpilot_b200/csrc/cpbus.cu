@@ -114,6 +114,11 @@ struct cpbus {
   PairCounter pub_pairs;                              // host publishes by (code << 32 | source_id), Metric excluded (bus.go:130-132)
   cpbus_event* d_drain = nullptr; size_t drain_cap = 0;        // cpbus_drain_many staging
   uint2* d_drain_idx = nullptr; size_t drain_idx_cap = 0;
+  // cpbus_drain_ready staging (records go to d_drain): header + tile counter + tile status, ready list, ring slot of each run
+  unsigned long long* d_ready_lb = nullptr; size_t ready_lb_tiles = 0;
+  cpbus_ready* d_ready = nullptr; uint32_t* d_ready_slot = nullptr; size_t ready_stage_cap = 0;
+  unsigned long long* h_ready_hdr = nullptr;   // pinned + mapped: the header the gather kernel hands to the host
+  unsigned long long* d_ready_hdr = nullptr;   // device alias of h_ready_hdr
   uint32_t subs_per_warp = 0;             // 0 = auto
   uint32_t order_block = 0;               // mask order is built per block of this many consecutive subscribers (0 = one global order)
   bool order_heavy_first = true;          // within a block: masks with more codes first (CPBUS_ORDER_HEAVY=0: plain mask order)
@@ -761,6 +766,8 @@ int cpbus_destroy(cpbus_t* b) try {
   if (b->copy_stream) cudaStreamDestroy(b->copy_stream);
   if (b->launched) cudaEventDestroy(b->launched);
   cudaFree(b->d_drain); cudaFree(b->d_drain_idx);
+  cudaFree(b->d_ready_lb); cudaFree(b->d_ready); cudaFree(b->d_ready_slot);
+  if (b->h_ready_hdr) cudaFreeHost(b->h_ready_hdr);
   cudaFree(b->d_result); cudaFree(b->d_batch_local); cudaFree(b->d_admit_batch); cudaFree(b->d_pf_buf); cudaFree(b->d_pf_state); cudaFree(b->d_acct);
   if (b->h_err) cudaFreeHost(b->h_err);
   if (b->h_acct) cudaFreeHost(b->h_acct);
@@ -1668,6 +1675,66 @@ int cpbus_drain_many(cpbus_t* b, uint32_t first_sub, uint32_t n, cpbus_event* ou
   if (hi) CK(cudaMemcpyAsync(out, b->d_drain, hi * sizeof(cpbus_event), cudaMemcpyDeviceToHost, b->stream));
   CK(cudaStreamSynchronize(b->stream));
   *total = tot;
+  return CPBUS_OK;
+} CPBUS_CATCH
+
+// Sparse drain: only the mailboxes that hold records.  The scan kernel reads each control block of the range once and
+// writes the ready list of the taken prefix; the gather kernel copies their runs and hands the 3-word header to the host
+// through mapped pinned memory.  One sync reads the header; a second one follows the two copies sized by it.
+int cpbus_drain_ready(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start_sub, cpbus_event* out, size_t cap,
+                      cpbus_ready* ready, size_t ready_cap, size_t* n_ready, size_t* total, uint32_t* next_sub) try {
+  if (!b || !out || !ready || !n_ready || !total || !next_sub || !n || !ready_cap) return CPBUS_EINVAL;
+  if (cap < b->R || cap > 0xFFFFFFFFull) return CPBUS_EINVAL;   // cap >= ring_cap: a ready mailbox always fits an empty call
+  if (start_sub < first_sub || start_sub - first_sub >= n) return CPBUS_EINVAL;
+  const uint32_t l = first_sub - b->cfg.sub_id_base;
+  if (first_sub < b->cfg.sub_id_base || (uint64_t)l + n > b->n_next) return CPBUS_ENOENT;
+  std::lock_guard<std::mutex> g(b->mu);
+  int rc = dev_guard(b); if (rc) return rc;
+  const size_t rcap = std::min<size_t>(ready_cap, n);   // never more entries than mailboxes
+  const uint32_t tiles = (n + kReadyTile - 1) / kReadyTile;
+  // device staging grows on demand and is kept (the records share cpbus_drain_many's buffer)
+  if (b->drain_cap < cap) {
+    cudaFree(b->d_drain); b->d_drain = nullptr; b->drain_cap = 0;
+    CK(cudaMalloc((void**)&b->d_drain, cap * sizeof(cpbus_event))); b->drain_cap = cap;
+  }
+  if (b->ready_stage_cap < rcap) {
+    cudaFree(b->d_ready); cudaFree(b->d_ready_slot); b->d_ready = nullptr; b->d_ready_slot = nullptr; b->ready_stage_cap = 0;
+    CK(cudaMalloc((void**)&b->d_ready, rcap * sizeof(cpbus_ready)));
+    CK(cudaMalloc((void**)&b->d_ready_slot, rcap * sizeof(uint32_t)));
+    b->ready_stage_cap = rcap;
+  }
+  if (b->ready_lb_tiles < tiles) {
+    cudaFree(b->d_ready_lb); b->d_ready_lb = nullptr; b->ready_lb_tiles = 0;
+    CK(cudaMalloc((void**)&b->d_ready_lb, (kReadyLbOffset + (size_t)tiles) * sizeof(unsigned long long)));
+    b->ready_lb_tiles = tiles;
+  }
+  if (!b->h_ready_hdr) {
+    unsigned long long *h = nullptr, *d = nullptr;
+    CK(cudaHostAlloc((void**)&h, 64, cudaHostAllocMapped));
+    if (cudaHostGetDevicePointer((void**)&d, h, 0) != cudaSuccess) { cudaFreeHost(h); CK(cudaGetLastError()); return CPBUS_ECUDA; }
+    b->h_ready_hdr = h; b->d_ready_hdr = d;
+  }
+  CK(cudaMemsetAsync(b->d_ready_lb + kReadyHdrWords, 0, (kReadyLbOffset - kReadyHdrWords + (size_t)tiles) * sizeof(unsigned long long),
+                     b->stream));
+  const uint32_t rot = start_sub - first_sub;
+  drain_ready_scan_kernel<<<tiles, kThreads, 0, b->stream>>>(b->d_ctl, l, n, rot, b->R, b->lossless ? 1u : 0u, b->cfg.sub_id_base,
+                                                              cap, rcap, b->d_ready_lb, b->d_ready, b->d_ready_slot);
+  CK(cudaGetLastError());
+  const uint32_t gather_grid = (uint32_t)std::min<size_t>((size_t)b->sm_count * 4, (rcap + kWarpsPerCta - 1) / kWarpsPerCta);
+  drain_ready_gather_kernel<<<gather_grid, kThreads, 0, b->stream>>>(b->d_ring, b->R, b->cfg.sub_id_base, b->d_ready,
+                                                                      b->d_ready_slot, b->d_ready_lb, b->d_drain, b->d_ready_hdr);
+  CK(cudaGetLastError());
+  b->st.kernel_launches += 2;
+  CK(cudaStreamSynchronize(b->stream));
+  const size_t nr = (size_t)b->h_ready_hdr[0], tot = (size_t)b->h_ready_hdr[1];
+  const uint64_t cut = b->h_ready_hdr[2];
+  if (nr) {
+    CK(cudaMemcpyAsync(ready, b->d_ready, nr * sizeof(cpbus_ready), cudaMemcpyDeviceToHost, b->stream));
+    CK(cudaMemcpyAsync(out, b->d_drain, tot * sizeof(cpbus_event), cudaMemcpyDeviceToHost, b->stream));
+    CK(cudaStreamSynchronize(b->stream));
+  }
+  *n_ready = nr; *total = tot;
+  *next_sub = cut >= n ? start_sub : first_sub + (uint32_t)((rot + cut) % n);
   return CPBUS_OK;
 } CPBUS_CATCH
 

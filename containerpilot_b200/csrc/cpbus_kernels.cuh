@@ -1428,6 +1428,151 @@ __global__ void drain_many_kernel(SubCtl* ctl, const cpbus_event* ring, uint32_t
   }
 }
 
+// ---- sparse drain (cpbus_drain_ready) ----------------------------------------------------------------------------------
+// Position p in [0, n) is mailbox first + (rot + p) mod n: the range in cyclic order from start_sub.  One single-pass scan
+// kernel reads each control block once, numbers the ready mailboxes and their records in position order (decoupled
+// look-back over tiles of kReadyTile positions), takes the prefix that fits and writes the ready list; a gather kernel
+// then copies the taken runs.  A tile's status word: flag (bits 62-63: 1 = tile aggregate, 2 = inclusive prefix) | ready
+// mailboxes (bits 33-61) | records (bits 0-32, saturating).  A shard has fewer than 2^29 mailboxes (each ring is at least
+// 2 KiB), and a saturated record count exceeds every allowed cap (< 2^32), so neither field can mislead the cut.
+constexpr uint32_t kReadyItems = 4, kReadyTile = kThreads * kReadyItems;
+static_assert(kReadyItems * kWarpsPerCta == 32, "one lane per (item, warp) chunk of a tile");
+constexpr unsigned long long kLbAgg = 1ull << 62, kLbIncl = 2ull << 62, kLbRecMax = (1ull << 33) - 1;
+constexpr uint32_t kReadyHdrWords = 4, kReadyLbOffset = 8;   // lb buffer: [0..3] header, [4] tile counter, [8..] tile status
+
+__device__ __forceinline__ unsigned long long lb_pack(unsigned long long flag, unsigned long long ready, unsigned long long rec) {
+  return flag | (ready << 33) | (rec < kLbRecMax ? rec : kLbRecMax);
+}
+
+// hdr[0..2] = {mailboxes taken, records taken, position of the first ready mailbox that did not fit (n: none)}; exactly one
+// thread writes it: the one holding that mailbox, or the last tile when everything fits.
+__global__ void __launch_bounds__(kThreads) drain_ready_scan_kernel(SubCtl* __restrict__ ctl, uint32_t first, uint32_t n,
+                                                                    uint32_t rot, uint32_t ring_cap, uint32_t lossless,
+                                                                    uint32_t sub_base, unsigned long long cap,
+                                                                    unsigned long long ready_cap, unsigned long long* lb,
+                                                                    cpbus_ready* __restrict__ ready, uint32_t* __restrict__ slot) {
+  __shared__ uint32_t s_tile;
+  __shared__ uint32_t s_wr[32];              // per (item, warp) chunk: ready mailboxes, then their exclusive prefix in the tile
+  __shared__ unsigned long long s_wc[32];    // ... and records
+  __shared__ unsigned long long s_base_r, s_base_c;
+  unsigned long long* hdr = lb;
+  unsigned long long* status = lb + kReadyLbOffset;
+  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  // tiles are numbered in the order the CTAs start, so every predecessor a tile waits for is running or done
+  if (threadIdx.x == 0) s_tile = atomicAdd(reinterpret_cast<unsigned int*>(lb + kReadyHdrWords), 1u);
+  __syncthreads();
+  const uint32_t tile = s_tile;
+  uint32_t loc[kReadyItems], r_in[kReadyItems];
+  unsigned long long tl[kReadyItems], cur[kReadyItems], hd[kReadyItems], c_in[kReadyItems];
+#pragma unroll
+  for (uint32_t k = 0; k < kReadyItems; k++) {   // item k of the tile = positions k*kThreads .. +kThreads: coalesced loads
+    const uint32_t p = tile * kReadyTile + k * kThreads + threadIdx.x;
+    unsigned long long t = 0, h = 0, c = 0;
+    uint32_t l = 0;
+    if (p < n) {
+      unsigned long long q = (unsigned long long)rot + p;
+      if (q >= n) q -= n;
+      l = first + (uint32_t)q;
+      const ulonglong2 th = *reinterpret_cast<const ulonglong2*>(ctl + l);   // {tail, head}
+      t = th.x; h = th.y; c = h;
+      if (!lossless && t > ring_cap && t - ring_cap > c) c = t - ring_cap;   // overwritten before being taken
+    }
+    loc[k] = l; tl[k] = t; hd[k] = h; cur[k] = c;
+    uint32_t r = t != c ? 1u : 0u;
+    unsigned long long s = t - c;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const uint32_t ro = __shfl_up_sync(0xffffffffu, r, o);
+      const unsigned long long so = shfl64(s, (int)lane - o);
+      if ((int)lane >= o) { r += ro; s += so; }
+    }
+    r_in[k] = r; c_in[k] = s;
+    if (lane == 31) { s_wr[k * kWarpsPerCta + warp] = r; s_wc[k * kWarpsPerCta + warp] = s; }
+  }
+  __syncthreads();
+  if (warp == 0) {
+    const uint32_t r0 = s_wr[lane];
+    const unsigned long long c0 = s_wc[lane];
+    uint32_t r = r0;
+    unsigned long long c = c0;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const uint32_t ro = __shfl_up_sync(0xffffffffu, r, o);
+      const unsigned long long co = shfl64(c, (int)lane - o);
+      if ((int)lane >= o) { r += ro; c += co; }
+    }
+    s_wr[lane] = r - r0; s_wc[lane] = c - c0;
+    const unsigned long long agg_r = __shfl_sync(0xffffffffu, r, 31), agg_c = shfl64(c, 31);
+    unsigned long long ex_r = 0, ex_c = 0;
+    if (tile == 0) {
+      if (lane == 0) *reinterpret_cast<volatile unsigned long long*>(status) = lb_pack(kLbIncl, agg_r, agg_c);
+    } else {
+      if (lane == 0) *reinterpret_cast<volatile unsigned long long*>(status + tile) = lb_pack(kLbAgg, agg_r, agg_c);
+      // look back over windows of 32 predecessors until one has published its inclusive prefix (tile 0 always does)
+      for (int pred = (int)tile - 1;; pred -= 32) {
+        const int j = pred - (int)lane;
+        unsigned long long v = kLbIncl;   // before tile 0: an empty inclusive prefix (never summed, tile 0 stops the walk)
+        do {
+          if (j >= 0) v = *reinterpret_cast<volatile unsigned long long*>(status + j);
+        } while (__any_sync(0xffffffffu, (v >> 62) == 0));
+        const uint32_t incl = __ballot_sync(0xffffffffu, (v >> 62) == 2);
+        const uint32_t stop = incl ? (uint32_t)(__ffs(incl) - 1) : 31u;   // the nearest inclusive predecessor ends the walk
+        ex_r += warp_sum64(lane <= stop ? (v >> 33) & ((1ull << 29) - 1) : 0ull);
+        ex_c += warp_sum64(lane <= stop ? v & kLbRecMax : 0ull);
+        ex_c = ex_c < kLbRecMax ? ex_c : kLbRecMax;
+        if (incl) break;
+      }
+      if (lane == 0) *reinterpret_cast<volatile unsigned long long*>(status + tile) = lb_pack(kLbIncl, ex_r + agg_r, ex_c + agg_c);
+    }
+    if (lane == 0) {
+      s_base_r = ex_r; s_base_c = ex_c;
+      const unsigned long long all_r = ex_r + agg_r, all_c = ex_c + agg_c;
+      if (tile == gridDim.x - 1 && all_r <= ready_cap && all_c <= cap) { hdr[0] = all_r; hdr[1] = all_c; hdr[2] = n; }
+    }
+  }
+  __syncthreads();
+#pragma unroll
+  for (uint32_t k = 0; k < kReadyItems; k++) {
+    const unsigned long long cnt = tl[k] - cur[k];
+    if (!cnt) continue;
+    const uint32_t chunk = k * kWarpsPerCta + warp;
+    const unsigned long long r = s_base_r + s_wr[chunk] + r_in[k] - 1;        // entry index among the ready mailboxes
+    const unsigned long long o = s_base_c + s_wc[chunk] + c_in[k] - cnt;      // first record of the run in `out`
+    if (r < ready_cap && o + cnt <= cap) {
+      ready[r] = cpbus_ready{sub_base + loc[k], (uint32_t)cnt, (uint32_t)o, 0u, cur[k] - hd[k]};
+      slot[r] = (uint32_t)(cur[k] & (ring_cap - 1));
+      ctl[loc[k]].head = tl[k];
+    } else if (r == 0 || (r - 1 < ready_cap && o <= cap)) {   // its predecessor was taken: this one ends the call
+      hdr[0] = r; hdr[1] = o; hdr[2] = tile * kReadyTile + k * kThreads + threadIdx.x;
+    }
+  }
+}
+
+// Copies the taken runs: one warp per ready entry, lane pairs per record (each pair writes one whole 32-byte sector), and
+// hands the header to the host through mapped pinned memory.
+__global__ void __launch_bounds__(kThreads) drain_ready_gather_kernel(const cpbus_event* __restrict__ ring, uint32_t ring_cap,
+                                                                      uint32_t sub_base, const cpbus_ready* __restrict__ ready,
+                                                                      const uint32_t* __restrict__ slot,
+                                                                      const unsigned long long* __restrict__ hdr,
+                                                                      cpbus_event* __restrict__ out, unsigned long long* h_hdr) {
+  const unsigned long long n_ready = hdr[0];
+  if (blockIdx.x == 0 && threadIdx.x < 3) h_hdr[threadIdx.x] = hdr[threadIdx.x];
+  const uint32_t lane = threadIdx.x & 31, half = lane & 1;
+  const unsigned long long nw = (gridDim.x * blockDim.x) >> 5;
+  for (unsigned long long e = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; e < n_ready; e += nw) {
+    const cpbus_ready rd = ready[e];
+    const uint32_t s0 = slot[e];
+    const uint4* src = reinterpret_cast<const uint4*>(ring + (size_t)(rd.sub_id - sub_base) * ring_cap);
+    uint4* dst = reinterpret_cast<uint4*>(out + rd.offset);
+    uint32_t j = lane >> 1;
+    for (; j + 16 < rd.count; j += 32) {   // two records per pair in flight
+      const uint4 a = src[2 * ((s0 + j) & (ring_cap - 1)) + half], b = src[2 * ((s0 + j + 16) & (ring_cap - 1)) + half];
+      dst[2 * j + half] = a; dst[2 * (j + 16) + half] = b;
+    }
+    if (j < rd.count) dst[2 * j + half] = src[2 * ((s0 + j) & (ring_cap - 1)) + half];
+  }
+}
+
 // (count, digest) folds over a range of mailboxes: one 32-byte result instead of 16 B per subscriber
 __global__ void digest_fold_kernel(const SubCtl* ctl, uint32_t first, uint32_t n, uint32_t sub_base,
                                    unsigned long long* out4) {

@@ -22,6 +22,7 @@
 #include <map>
 #include <memory>
 #include <mutex>
+#include <set>
 #include <stdexcept>
 #include <string>
 #include <thread>
@@ -194,6 +195,7 @@ class EventBus {   // events/bus.go:12-22
     cfg.n_max_subs = n_max_subs; cfg.ring_cap = mailbox_cap; cfg.batch_cap = mailbox_cap >= 512 ? 256 : mailbox_cap / 2;
     cfg.timers_per_sub = 4; cfg.flags = CPBUS_CFG_LOSSLESS | CPBUS_CFG_DIGEST; cfg.device = -1;
     batch_cap_ = cfg.batch_cap;
+    drain_cap_ = std::max<size_t>(kDrainCap, mailbox_cap);
     int rc = cpbus_create(&cfg, &h_);
     if (rc) throw std::runtime_error(std::string("cpbus_create: ") + cpbus_strerror(rc) + " " + cpbus_last_cuda_error());
     start_ = std::chrono::steady_clock::now();
@@ -240,6 +242,8 @@ class EventBus {   // events/bus.go:12-22
       id = old->id_;
       Retry([&] { return cpbus_set_mask(h_, id, mask); }, "cpbus_set_mask");
       sub->pending_ = std::move(old->pending_);
+      pending_subs_.erase(old);
+      if (!sub->pending_.empty()) pending_subs_.insert(sub);
       registry_.erase(old);
       implicit_.erase(imp);
     } else {
@@ -247,6 +251,7 @@ class EventBus {   // events/bus.go:12-22
     }
     sub->id_ = id;
     registry_[sub] = id;
+    by_id_[id] = sub;
     if (sub->Rx) detail::RxRegistry()[sub->Rx.get()] = {this, sub};
     done_.Add(1);
   }
@@ -260,6 +265,8 @@ class EventBus {   // events/bus.go:12-22
       FlushLocked();
       DrainOne(sub, /*blocking=*/false);   // what was published before the unsubscribe still reaches Rx
       Retry([&] { return cpbus_unsubscribe(h_, it->second); }, "cpbus_unsubscribe");
+      by_id_.erase(it->second);
+      pending_subs_.erase(sub);
       registry_.erase(it);
       if (sub->Rx) detail::RxRegistry().erase(sub->Rx.get());
       sub->id_ = UINT32_MAX;
@@ -372,6 +379,7 @@ class EventBus {   // events/bus.go:12-22
     Retry([&] { return cpbus_subscribe(h_, 0u, &id); }, "cpbus_subscribe");
     sub->id_ = id;
     registry_[sub.get()] = id;
+    by_id_[id] = sub.get();
     detail::RxRegistry()[rx.get()] = {this, sub.get()};
     Subscriber* raw = sub.get();
     implicit_[rx.get()] = std::move(sub);
@@ -381,6 +389,8 @@ class EventBus {   // events/bus.go:12-22
   // (events/timer.go:26-30,50-54) — release the mailbox and with it the timers
   void ReleaseImplicit(Subscriber* sub) {
     cpbus_unsubscribe(h_, sub->id_);
+    by_id_.erase(sub->id_);
+    pending_subs_.erase(sub);
     registry_.erase(sub);
     detail::RxRegistry().erase(sub->Rx.get());
     implicit_.erase(sub->Rx.get());
@@ -424,30 +434,35 @@ class EventBus {   // events/bus.go:12-22
       else if (!sub->Rx->TrySend(sub->pending_.front())) break;
       sub->pending_.pop_front();
     }
+    if (sub->pending_.empty()) pending_subs_.erase(sub);
+    else pending_subs_.insert(sub);
   }
-  // All mailboxes at once: one gather kernel + two D2H copies (cpbus_drain_many) instead of a round trip per subscriber.
+  // Only the mailboxes that hold records (cpbus_drain_ready), then only the subscribers with pending records: the pump's
+  // cost follows what was delivered, not how many subscribers there are.
   void DrainAll(bool blocking) {
-    if (registry_.empty()) return;
-    uint32_t lo = UINT32_MAX, hi = 0;
-    for (auto& kv : registry_) { lo = std::min(lo, kv.second); hi = std::max(hi, kv.second); }
-    const uint32_t n = hi - lo + 1;
-    if (drain_buf_.size() < kDrainCap) drain_buf_.resize(kDrainCap);
-    drain_off_.resize(n); drain_cnt_.resize(n);
-    std::vector<Subscriber*> by_id(n, nullptr);
-    for (auto& kv : registry_) by_id[kv.second - lo] = kv.first;
-    for (;;) {
-      size_t total = 0;
-      Check(cpbus_drain_many(h_, lo, n, drain_buf_.data(), kDrainCap, drain_off_.data(), drain_cnt_.data(), &total), "cpbus_drain_many");
-      if (!total) break;
-      for (uint32_t i = 0; i < n; i++) {
-        if (!drain_cnt_[i] || !by_id[i]) continue;
-        const cpbus_event* r = drain_buf_.data() + drain_off_[i];
-        for (uint32_t j = 0; j < drain_cnt_[i]; j++) by_id[i]->pending_.push_back(Event{(EventCode)r[j].code, Source(r[j].source_id)});
+    if (by_id_.empty()) return;
+    const uint32_t lo = by_id_.begin()->first, n = by_id_.rbegin()->first - lo + 1;
+    if (drain_buf_.size() < drain_cap_) drain_buf_.resize(drain_cap_);
+    if (drain_ready_.size() < kReadyCap) drain_ready_.resize(kReadyCap);
+    for (uint32_t start = lo;;) {   // resume at the first mailbox that did not fit: every mailbox gets its turn
+      size_t n_ready = 0, total = 0;
+      uint32_t next = lo;
+      Check(cpbus_drain_ready(h_, lo, n, start, drain_buf_.data(), drain_cap_, drain_ready_.data(), kReadyCap, &n_ready, &total, &next),
+            "cpbus_drain_ready");
+      for (size_t i = 0; i < n_ready; i++) {
+        const cpbus_ready& e = drain_ready_[i];
+        auto it = by_id_.find(e.sub_id);
+        if (it == by_id_.end()) continue;   // an id in the range that is no longer subscribed
+        const cpbus_event* r = drain_buf_.data() + e.offset;
+        for (uint32_t j = 0; j < e.count; j++) it->second->pending_.push_back(Event{(EventCode)r[j].code, Source(r[j].source_id)});
+        pending_subs_.insert(it->second);
       }
+      if (!n_ready || next == start) break;   // next == start: everything that was ready has been taken
+      start = next;
     }
     std::vector<Subscriber*> dead;
-    for (auto& kv : registry_) {
-      Subscriber* sub = kv.first;
+    for (auto it = pending_subs_.begin(); it != pending_subs_.end();) {
+      Subscriber* sub = *it;
       try {
         while (!sub->pending_.empty() && sub->Rx) {
           if (blocking) sub->Rx->Send(sub->pending_.front());
@@ -458,6 +473,7 @@ class EventBus {   // events/bus.go:12-22
         if (!sub->implicit_) throw;          // bus.go:135-137: publishing into a closed subscriber channel is a panic
         dead.push_back(sub);                 // timer.go:50-54: the timer goroutine recovers and exits
       }
+      it = sub->pending_.empty() ? pending_subs_.erase(it) : std::next(it);
     }
     for (Subscriber* sub : dead) ReleaseImplicit(sub);
   }
@@ -473,9 +489,10 @@ class EventBus {   // events/bus.go:12-22
     }
   }
 
-  static constexpr size_t kDrainCap = 1 << 16;
+  static constexpr size_t kDrainCap = 1 << 16, kReadyCap = 4096;
+  size_t drain_cap_ = kDrainCap;               // records per cpbus_drain_ready call (at least one mailbox's capacity)
   std::vector<cpbus_event> drain_buf_;
-  std::vector<uint32_t> drain_off_, drain_cnt_;
+  std::vector<cpbus_ready> drain_ready_;
   cpbus_t* h_ = nullptr;
   std::shared_ptr<Life> life_ = std::make_shared<Life>();
   std::recursive_mutex& lock_ = life_->m;   // bus.lock (bus.go:14): serialises publishers and membership changes
@@ -483,6 +500,8 @@ class EventBus {   // events/bus.go:12-22
   bool reload_ = false;
   WaitGroup done_;
   std::map<Subscriber*, uint32_t> registry_;   // bus.go:13
+  std::map<uint32_t, Subscriber*> by_id_;      // the same, by mailbox id: DrainAll's id range and lookups
+  std::set<Subscriber*> pending_subs_;         // subscribers whose pending_ is not empty (in registry_ order)
   uint32_t batch_cap_ = 32;                    // events per cpbus_publish batch (PublishMany)
   std::map<std::pair<std::string, std::string>, uint64_t> counter_;   // containerpilot_events{code,source}
   Clock clock_;

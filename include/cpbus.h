@@ -317,9 +317,31 @@ int cpbus_drain(cpbus_t* bus, uint32_t sub_id, cpbus_event* out, size_t cap, siz
 /* Bulk drain of mailboxes [first_sub, first_sub+n): one kernel gathers every undrained record into a staging
  * buffer (one atomic per mailbox), two D2H copies bring them back.  out[offsets[i] .. offsets[i]+counts[i]) is mailbox
  * i's run, FIFO.  A mailbox whose run does not fit into `cap` is left untouched (counts[i] = 0) for the next call;
- * *total = records returned.  This is what the `chan Event` pump of a shim with many subscribers calls. */
+ * *total = records returned.  Its index traffic is sized by n; a pump on a large fleet calls cpbus_drain_ready. */
 int cpbus_drain_many(cpbus_t* bus, uint32_t first_sub, uint32_t n, cpbus_event* out, size_t cap,
                      uint32_t* offsets, uint32_t* counts, size_t* total);
+/* Sparse drain: only the mailboxes that hold records.  Mailboxes [first_sub, first_sub+n) are examined in cyclic id order
+ * starting at start_sub; a mailbox is ready when it has undrained records (throughput mode: from max(head, tail - ring_cap),
+ * as cpbus_drain).  Ready mailboxes are taken in that order while their whole run still fits into `cap` records and
+ * `ready_cap` entries; the first one that does not fit ends the call (a run is never split).  Entry i of ready[0 .. *n_ready)
+ * is the i-th mailbox taken; its records are out[offset .. offset+count), FIFO, runs packed back to back (*total records).
+ * Taken mailboxes are left empty (head = tail); nothing else changes.  *next_sub = the first mailbox not taken (the one
+ * that did not fit), or start_sub when everything was taken: a pump passing it back as start_sub visits every mailbox.
+ * The same state and arguments give byte-identical out and ready.  Cost: one read of the range's control blocks on the
+ * device plus the records taken; host<->device traffic is 24*n_ready + 32*total bytes plus a constant; at most two stream
+ * synchronisations (one, and no copy, when nothing is ready).  Runs on the bus stream behind every earlier fan-out.
+ * CPBUS_EINVAL: a NULL pointer, n == 0, cap < ring_cap, cap > 0xFFFFFFFF, ready_cap == 0, or start_sub outside the range.
+ * CPBUS_ENOENT: the range is not within this shard's subscribers. */
+typedef struct cpbus_ready {
+  uint32_t sub_id;   /* global id (sub_id_base applied)                                                  */
+  uint32_t count;    /* records of this mailbox in out[offset .. offset+count), FIFO                      */
+  uint32_t offset;   /* offsets increase with the entry index; runs are packed back to back                */
+  uint32_t pad;      /* 0 */
+  uint64_t lost;     /* throughput mode: records overwritten since the stored cursor (as cpbus_drain); 0 in lossless mode */
+} cpbus_ready;       /* sizeof == 24 */
+int cpbus_drain_ready(cpbus_t* bus, uint32_t first_sub, uint32_t n, uint32_t start_sub,
+                      cpbus_event* out, size_t cap, cpbus_ready* ready, size_t ready_cap,
+                      size_t* n_ready, size_t* total, uint32_t* next_sub);
 /* Device-side consumer: every mailbox is read to the end and its records are discarded (head = tail), ordered behind
  * every earlier fan-out on the bus stream.  For subscribers nobody reads, and for measuring the lossless mode with
  * consumers that keep up. */
