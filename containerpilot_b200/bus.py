@@ -199,6 +199,17 @@ class Bus:
         """lossless stream: fan out the next m undelivered records; OK = batch complete, EAGAIN = records remain"""
         return self._lib.cpbus_stream_fanout_prefix(st, n, now_ns, m)
 
+    def stream_offer(self, st, prefix: int, stalled: bool = False):
+        """lossless stream across processes: post this shard's admitted prefix for the current round (async)"""
+        nat.check(self._lib.cpbus_stream_offer(st, prefix, 1 if stalled else 0), "cpbus_stream_offer")
+
+    def stream_agree(self, st) -> int:
+        """lossless stream across processes: the minimum of every shard's offer of this round.  Raises on an error,
+        CPBUS_EAGAIN included (some shard stalled: drain, then run the round again)."""
+        m = C.c_size_t()
+        nat.check(self._lib.cpbus_stream_agree(st, C.byref(m)), "cpbus_stream_agree")
+        return m.value
+
     def stream_poll(self, st):
         """(n, now_ns) of the next batch if the publisher has released it, else None — for consumers that are not told"""
         ready, n, now = C.c_int(), C.c_size_t(), C.c_uint64()

@@ -1309,6 +1309,14 @@ struct cpbus_stream {
   unsigned long long* h_ack = nullptr;       // kStreamMaxConsumers x 4 words
   cudaEvent_t staged_done[kStage] = {};
   cudaStream_t put_stream = nullptr;
+  // lossless across processes (cpbus_stream_offer / _agree): admission rounds agreed so far, and this round's state
+  unsigned long long agree_round = 0;
+  bool offered = false;
+  unsigned long long admit_q = 0;            // batch ordinal and shape of the latest cpbus_stream_admit (bounds an offer)
+  size_t admit_n = 0;
+  StreamAgreeResult* h_agree = nullptr;      // pinned + mapped: written by the agree kernel
+  StreamAgreeResult* d_agree = nullptr;      // device alias of h_agree
+  cudaEvent_t agree_done = nullptr;
 };
 
 static int stream_bind(cpbus_stream* st) {
@@ -1410,6 +1418,8 @@ int cpbus_stream_close(cpbus_stream_t* st) try {
   }
   if (st->h_hdr) cudaFreeHost(st->h_hdr);
   if (st->h_ack) cudaFreeHost(st->h_ack);
+  if (st->h_agree) cudaFreeHost(st->h_agree);
+  if (st->agree_done) cudaEventDestroy(st->agree_done);
   if (st->base) { if (st->owner) cudaFree(st->base); else if (!st->attached) cudaIpcCloseMemHandle(st->base); }
   b->streams.erase(std::remove(b->streams.begin(), b->streams.end(), st), b->streams.end());
   delete st;
@@ -1526,6 +1536,7 @@ static int stream_enter(cpbus_stream* st, uint64_t now_ns) {
 int cpbus_stream_admit(cpbus_stream_t* st, size_t n, uint64_t now_ns, size_t* prefix) try {
   if (!st || !prefix || n > st->B || st->get_off > n) return CPBUS_EINVAL;
   *prefix = 0;
+  st->admit_q = st->get_seq + 1; st->admit_n = n;
   cpbus* b = st->bus;
   int rc = stream_enter(st, now_ns); if (rc) return rc;
   const uint32_t rem = (uint32_t)n - st->get_off;
@@ -1602,6 +1613,55 @@ int cpbus_stream_fanout(cpbus_stream_t* st, size_t n, uint64_t now_ns) try {
   if (!st || n > st->B || st->get_off > n) return CPBUS_EINVAL;
   if (st->bus->lossless) return CPBUS_EINVAL;   // without admission this shard could deliver more than another one does
   return stream_fanout_prefix(st, n, now_ns, n - st->get_off);
+} CPBUS_CATCH
+
+// Lossless stream across processes, step 1 of the exchange: post this shard's admitted prefix for the current round.
+// One-thread kernel on the bus stream (behind the admission pass when it ran); no host sync.
+int cpbus_stream_offer(cpbus_stream_t* st, size_t prefix, int stalled) try {
+  if (!st) return CPBUS_EINVAL;
+  cpbus* b = st->bus;
+  if (!b->lossless || st->offered) return CPBUS_EINVAL;   // throughput mode needs no agreement; one offer per round
+  const size_t n = st->admit_q == st->get_seq + 1 ? st->admit_n : st->B;   // the batch's shape when this shard admitted it
+  if (prefix > n - st->get_off || (stalled && prefix)) return CPBUS_EINVAL;
+  int rc = dev_guard(b); if (rc) return rc;
+  if (*(volatile unsigned int*)b->h_err) return CPBUS_ETIMEDOUT;
+  const unsigned long long r = st->agree_round + 1;
+  stream_offer_kernel<<<1, 1, 0, b->stream>>>(st->ack + stream_offer_word_index(st->consumer, r),
+                                              stream_offer_word(r, stalled ? 1u : 0u, (uint32_t)prefix));
+  CK(cudaGetLastError());
+  b->st.kernel_launches++;
+  st->offered = true;
+  return CPBUS_OK;
+} CPBUS_CATCH
+
+// Step 2: wait (in a one-CTA kernel, bounded by the stream timeout) for every shard's offer of this round; *m = the minimum.
+// The host waits for that kernel only.  Every call completes the round, whatever it returns.
+int cpbus_stream_agree(cpbus_stream_t* st, size_t* m) try {
+  if (!st || !m) return CPBUS_EINVAL;
+  *m = 0;
+  cpbus* b = st->bus;
+  if (!b->lossless || !st->offered) return CPBUS_EINVAL;
+  int rc = dev_guard(b); if (rc) return rc;
+  if (*(volatile unsigned int*)b->h_err) return CPBUS_ETIMEDOUT;
+  if (!st->h_agree) {
+    StreamAgreeResult *h = nullptr, *d = nullptr;
+    CK(cudaHostAlloc((void**)&h, sizeof(StreamAgreeResult), cudaHostAllocMapped));
+    if (cudaHostGetDevicePointer((void**)&d, h, 0) != cudaSuccess) { cudaFreeHost(h); CK(cudaGetLastError()); return CPBUS_ECUDA; }
+    st->h_agree = h; st->d_agree = d;
+  }
+  if (!st->agree_done) CK(cudaEventCreateWithFlags(&st->agree_done, cudaEventDisableTiming));
+  const unsigned long long r = st->agree_round + 1;
+  stream_agree_kernel<<<1, kStreamMaxConsumers, 0, b->stream>>>(st->ack, st->n_consumers, r, b->stream_spin_us, st->d_agree, b->d_err);
+  CK(cudaGetLastError());
+  b->st.kernel_launches++;
+  st->agree_round = r; st->offered = false;
+  CK(cudaEventRecord(st->agree_done, b->stream));
+  CK(cudaEventSynchronize(st->agree_done));
+  const volatile StreamAgreeResult* res = st->h_agree;
+  if (res->status) return CPBUS_ETIMEDOUT;   // a shard never offered: the sticky error word is set, nothing goes out
+  if (res->stalled) return CPBUS_EAGAIN;
+  *m = res->m;
+  return CPBUS_OK;
 } CPBUS_CATCH
 
 static int read_cursors(cpbus* b, uint32_t l, uint64_t* tail, uint64_t* head, uint64_t* lost = nullptr) {

@@ -146,6 +146,20 @@ __host__ __device__ inline size_t stream_ack_off(uint32_t n_slots) { return stre
 __host__ __device__ inline size_t stream_payload_off(uint32_t n_slots) { return stream_ack_off(n_slots) + (size_t)kStreamMaxConsumers * 32; }
 __host__ __device__ inline size_t stream_bytes(uint32_t n_slots, uint32_t batch_cap) { return stream_payload_off(n_slots) + (size_t)n_slots * batch_cap * 32; }
 
+// Lossless stream across processes (cpbus_stream_offer / _agree): consumer c posts its admitted prefix for admission round
+// r as one word of its ack sector, word 1 + (r & 1).  Two words alternate because a shard that has finished round r may post
+// its round r + 1 offer while a slower shard's agree kernel has not read the round r one yet; it cannot get to round r + 2
+// before every shard has posted (hence finished agreeing on) round r + 1.  Word: r (31 bits) << 33 | stalled << 32 | prefix.
+constexpr unsigned long long kOfferRoundMask = (1ull << 31) - 1;
+__host__ __device__ inline uint32_t stream_offer_word_index(uint32_t consumer, unsigned long long round) {
+  return 4u * consumer + 1u + (uint32_t)(round & 1ull);
+}
+__host__ __device__ inline unsigned long long stream_offer_word(unsigned long long round, uint32_t stalled, uint32_t prefix) {
+  return ((round & kOfferRoundMask) << 33) | ((unsigned long long)(stalled ? 1u : 0u) << 32) | prefix;
+}
+// agree kernel -> host (pinned, mapped): the agreed prefix, the OR of the stall bits, 0 / kErrStreamTimeout
+struct __align__(16) StreamAgreeResult { uint32_t m, stalled, status, pad; };
+
 struct FanoutParams {
   const cpbus_event* batch;   // n_ev records, sorted by ts (HBM)
   cpbus_event* ring;          // [n_subs][R]
@@ -1590,6 +1604,50 @@ __global__ void digest_fold_kernel(const SubCtl* ctl, uint32_t first, uint32_t n
   }
   if ((threadIdx.x & 31) == 0) { atomicAdd(&out4[0], c); atomicAdd(&out4[1], d); atomicXor(&out4[2], x); }
   if (blockIdx.x == 0 && threadIdx.x == 0) out4[3] = n;
+}
+
+// Lossless stream across processes: post this shard's offer word into the publisher's memory (peer mapping elsewhere).
+// Stream-ordered behind the admission pass; the release orders nothing else, it makes the word itself visible system-wide.
+__global__ void stream_offer_kernel(unsigned long long* word, unsigned long long value) {
+  asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(word), "l"(value) : "memory");
+}
+
+// One CTA of kStreamMaxConsumers threads, lane c = consumer c: acquire every shard's offer of round `round` (bounded by the
+// stream timeout), then the minimum prefix and the OR of the stall bits.  A missing offer sets the sticky error word.
+__global__ void __launch_bounds__(kStreamMaxConsumers) stream_agree_kernel(const unsigned long long* ack, uint32_t n_consumers,
+                                                                          unsigned long long round, uint32_t spin_us,
+                                                                          StreamAgreeResult* out, unsigned int* err_word) {
+  __shared__ uint32_t s_min[kStreamMaxConsumers / 32], s_flags[kStreamMaxConsumers / 32];
+  const uint32_t c = threadIdx.x, lane = c & 31u, w = c >> 5;
+  const unsigned long long tag = round & kOfferRoundMask;
+  uint32_t prefix = 0xFFFFFFFFu, flags = 0;   // flags: bit 0 stalled, bit 1 missing
+  if (c < n_consumers) {
+    const unsigned long long* word = ack + stream_offer_word_index(c, round);
+    const unsigned long long budget = (spin_us ? (unsigned long long)spin_us : 2000000ull) * 1000ull;
+    unsigned long long v, t0, t1;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
+    for (;;) {
+      asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(word) : "memory");
+      if ((v >> 33) == tag) break;
+      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1));
+      if (t1 - t0 > budget) break;
+      __nanosleep(128);
+    }
+    if ((v >> 33) == tag) { prefix = (uint32_t)v; flags = (uint32_t)(v >> 32) & 1u; }
+    else flags = 2u;
+  }
+  prefix = __reduce_min_sync(0xFFFFFFFFu, prefix);
+  flags = __reduce_or_sync(0xFFFFFFFFu, flags);
+  if (lane == 0) { s_min[w] = prefix; s_flags[w] = flags; }
+  __syncthreads();
+  if (c == 0) {
+    for (uint32_t i = 1; i < blockDim.x / 32; i++) { prefix = min(prefix, s_min[i]); flags |= s_flags[i]; }
+    const uint32_t status = (flags & 2u) ? kErrStreamTimeout : 0u;
+    if (status) asm volatile("st.relaxed.sys.global.u32 [%0], %1;" ::"l"(err_word), "r"(status) : "memory");   // host-mapped, sticky
+    out->m = flags ? 0u : prefix;
+    out->stalled = flags & 1u;
+    out->status = status;
+  }
 }
 #endif  // __CUDACC__
 

@@ -7,7 +7,9 @@ subscriber ids (`cpbus_config.sub_id_base`), a subscriber's sequence and digest 
 Two drivers over the same C-ABI:
 
 * `ShardedBus`      — one process per GPU (`torch.distributed.run`); torch.distributed (NCCL or gloo) is used ONLY for the
-                      construction handshake (the 64-byte CUDA-IPC handle) and for reducing statistics.
+                      construction handshake (the 64-byte CUDA-IPC handle) and for reducing statistics.  Also in lossless
+                      mode: the ranks agree on the minimum admitted prefix through offer words in the publisher's memory
+                      (`cpbus_stream_offer` / `cpbus_stream_agree`).
 * `LocalShardedBus` — one process driving G buses (what a cgo shim inside the single ContainerPilot process does):
                       `cpbus_stream_attach`, peer access instead of IPC; also runs with all shards on ONE GPU.  Also in
                       lossless mode (`cpbus_stream_admit` on every shard, then `cpbus_stream_fanout_prefix` of the minimum).
@@ -53,6 +55,26 @@ def broadcast_events(dist, events_u8, src: int = 0):
     return events_u8
 
 
+def _admit_or_stall(bus, st, n: int, now_ns: int) -> tuple[int, bool]:
+    """(prefix, stalled) this shard offers: what cpbus_stream_admit admits, or (0, True) when it reports a stall."""
+    try:
+        return bus.stream_admit(st, n, now_ns), False
+    except nat.CpbusError as ex:
+        if ex.status != nat.EAGAIN:
+            raise
+        return 0, True
+
+
+def _agree(bus, st) -> int | None:
+    """the agreed prefix of this round, or None when some shard stalled"""
+    try:
+        return bus.stream_agree(st)
+    except nat.CpbusError as ex:
+        if ex.status != nat.EAGAIN:
+            raise
+        return None
+
+
 class _ShardOps:
     """What both drivers share: a shard is a `Bus` plus its end of the publisher's stream."""
 
@@ -79,19 +101,27 @@ class ShardedBus(_ShardOps):
         rank 0       : put(events, now_ns)            host batch -> the stream ring (H2D + release), may run ahead
         every rank   : fanout(n, now_ns)              one fan-out launch; the batch is pulled inside the kernel
     Device-resident traces (the publisher's events already in its HBM): attach_trace / fanout_trace.
+
+    `lossless=True` gives every shard the reference's blocking semantics (a publish stops at the event the Go bus would
+    block on, on every rank): `fanout` runs one admission round — admit, offer, agree, fan out the agreed prefix — and
+    returns nat.OK (batch complete) or nat.EAGAIN (drain, then every rank calls `fanout` again with the same n, now_ns).
+    The ranks agree through offer words in the publisher's memory, with no collective.  Device-batch paths
+    (fanout_trace, fanout_broadcast) stay throughput-only.
     """
 
     def __init__(self, n_subs_total: int, dist=None, rank: int = 0, world: int = 1, device: int = -1, ring_cap: int = 1024,
                  batch_cap: int = 512, timers_per_sub: int = 0, digest: bool = True, stream_slots: int = 64,
                  stream=None, store_path: int = nat.STORE_AUTO, grid_ctas: int = 0, subs_per_rank: int | None = None,
-                 bus_factory=Bus):
+                 bus_factory=Bus, lossless: bool = False):
         self.dist, self.rank, self.world = dist, rank, world
+        self.lossless = lossless
         if subs_per_rank is not None:               # weak scaling: fixed shard size
             self.first, self.count = rank * subs_per_rank, subs_per_rank
         else:
             self.first, self.count = shard_range(n_subs_total, world, rank)
         self.bus = bus_factory(max(self.count, 1), ring_cap=ring_cap, batch_cap=batch_cap, timers_per_sub=timers_per_sub, digest=digest,
-                       device=device, sub_id_base=self.first, store_path=store_path, stream=stream, grid_ctas=grid_ctas)
+                       device=device, sub_id_base=self.first, store_path=store_path, stream=stream, grid_ctas=grid_ctas,
+                       lossless=lossless)
         self.batch_cap = batch_cap
         self._st = None
         self._peer_trace = None      # (mapped pointer, owner?) of the attached device trace
@@ -142,10 +172,22 @@ class ShardedBus(_ShardOps):
         return self.bus.stream_put(self._st, events, now_ns, raw)
 
     def fanout(self, n: int, now_ns: int) -> int:
-        return self.bus.stream_fanout(self._st, n, now_ns)
+        if not self.lossless:
+            return self.bus.stream_fanout(self._st, n, now_ns)
+        # one admission round; every rank runs it, so every rank's round ordinal advances together
+        prefix, stalled = _admit_or_stall(self.bus, self._st, n, now_ns)
+        self.bus.stream_offer(self._st, prefix, stalled)
+        m = _agree(self.bus, self._st)
+        if m is None:
+            return nat.EAGAIN                       # some rank stalled: nothing goes out anywhere
+        rc = self.bus.stream_fanout_prefix(self._st, n, now_ns, m)
+        if rc not in (nat.OK, nat.EAGAIN):
+            nat.check(rc, "cpbus_stream_fanout_prefix")
+        return rc
 
     def publish(self, events: np.ndarray, now_ns: int) -> int:
-        """put + fanout for callers that do not pipeline."""
+        """put + fanout for callers that do not pipeline.  Lossless mode: one round, no retry (EAGAIN: drain, then
+        `fanout` again)."""
         rc = self.put(events, now_ns)
         return rc if rc else self.fanout(len(events), now_ns)
 
@@ -178,6 +220,11 @@ class ShardedBus(_ShardOps):
             self.ingest = "nvlink-peer-pull (fused into the fan-out kernel)"
         return ptr
 
+    def _no_device_batches_in_lossless(self):
+        if self.lossless:
+            raise RuntimeError("device-resident batches are all-or-nothing per shard: a lossless ShardedBus takes its "
+                               "batches through put / fanout only")
+
     def use_local_trace(self, ptr: int):
         """The trace already sits in THIS GPU's memory at `ptr` (single GPU, or a replicated / NCCL-broadcast copy)."""
         self._trace_ptr, self._trace_local = ptr, True
@@ -185,6 +232,7 @@ class ShardedBus(_ShardOps):
     def fanout_trace(self, offset_bytes: int, n: int, watermark_ns: int, next_offset_bytes: int | None = None, next_n: int = 0) -> int:
         """Fan out records [offset, offset + 32 n) of the attached trace; `next_offset_bytes` names a LATER batch (best: the
         one after next) that this launch pulls across the link while its stores are in flight."""
+        self._no_device_batches_in_lossless()
         base = self._trace_ptr
         if self.world == 1 or self._trace_local:
             return self.bus.publish_device(base + offset_bytes, n, watermark_ns)
@@ -194,6 +242,7 @@ class ShardedBus(_ShardOps):
     def fanout_broadcast(self, batch_u8, n: int, watermark_ns: int) -> int:
         """Fallback (no peer mapping): `batch_u8` is a [n, 32] uint8 CUDA tensor, valid on rank 0; NCCL broadcast, then a
         local fan-out.  One collective per call — the caller batches several steps per call to amortise it."""
+        self._no_device_batches_in_lossless()
         if self.world > 1:
             broadcast_events(self.dist, batch_u8, src=0)
         return self.bus.publish_device(batch_u8.data_ptr(), n, watermark_ns)
@@ -235,12 +284,17 @@ class ShardedBus(_ShardOps):
 class LocalShardedBus:
     """G shards driven by ONE process (shard g on `devices[g]`; all on one GPU is allowed): what a cgo shim inside the
     single ContainerPilot process does.  Same stream protocol as `ShardedBus`, attached in-process.  `lossless=True` gives every
-    shard the reference's blocking semantics: a publish stops at the event the Go bus would block on, on every shard."""
+    shard the reference's blocking semantics: a publish stops at the event the Go bus would block on, on every shard.
+    The shards' minimum prefix is taken on the host (`agree="host"`) or, with `agree="device"`, through the offer words
+    in the publisher's memory and the agree kernel — the protocol `ShardedBus(lossless=True)` runs across processes."""
 
     def __init__(self, n_subs_total: int, devices, ring_cap: int = 1024, batch_cap: int = 512, timers_per_sub: int = 0,
-                 digest: bool = True, stream_slots: int = 64, lossless: bool = False):
+                 digest: bool = True, stream_slots: int = 64, lossless: bool = False, agree: str = "host"):
+        if agree not in ("host", "device"):
+            raise ValueError(f"agree must be 'host' or 'device', not {agree!r}")
         self.world = len(devices)
-        self.lossless = lossless
+        self.lossless, self.agree = lossless, agree
+        self.last_round = None                      # agree="device": ([(prefix, stalled)], [agreed m or None]) per shard
         self.shards = []
         for g, dev in enumerate(devices):
             first, count = shard_range(n_subs_total, self.world, g)
@@ -288,6 +342,8 @@ class LocalShardedBus:
             for g, (_, _, bus) in enumerate(self.shards):
                 nat.check(bus.stream_fanout(self._st[g], n, now_ns), "cpbus_stream_fanout")
             return nat.OK
+        if self.agree == "device":
+            return self._fanout_device_agree(n, now_ns)
         m = None
         for g, (_, _, bus) in enumerate(self.shards):
             try:
@@ -300,6 +356,29 @@ class LocalShardedBus:
         rc = nat.OK
         for g, (_, _, bus) in enumerate(self.shards):
             r = bus.stream_fanout_prefix(self._st[g], n, now_ns, m)
+            if r not in (nat.OK, nat.EAGAIN):
+                nat.check(r, "cpbus_stream_fanout_prefix")
+            rc = r
+        return rc
+
+    def _fanout_device_agree(self, n: int, now_ns: int) -> int:
+        """One admission round through the publisher's memory (what `ShardedBus(lossless=True)` does on each rank): every
+        shard offers before any shard waits, and every shard agrees, so the round advances in lockstep."""
+        offers = []
+        for g, (_, _, bus) in enumerate(self.shards):
+            offers.append(_admit_or_stall(bus, self._st[g], n, now_ns))
+            bus.stream_offer(self._st[g], *offers[-1])
+        agreed = []
+        for g, (_, _, bus) in enumerate(self.shards):
+            agreed.append(_agree(bus, self._st[g]))
+        self.last_round = (offers, agreed)
+        if len(set(agreed)) != 1:                   # every agree kernel read the same words
+            raise RuntimeError(f"shards agreed on different prefixes: {agreed}")
+        if agreed[0] is None:
+            return nat.EAGAIN
+        rc = nat.OK
+        for g, (_, _, bus) in enumerate(self.shards):
+            r = bus.stream_fanout_prefix(self._st[g], n, now_ns, agreed[g])
             if r not in (nat.OK, nat.EAGAIN):
                 nat.check(r, "cpbus_stream_fanout_prefix")
             rc = r

@@ -256,6 +256,17 @@ int cpbus_publish_device_staged(cpbus_t* bus, const void* d_events, size_t n, ui
  *                    [all shards] cpbus_stream_fanout_prefix(st, n, now_ns, m)
  *                    CPBUS_EAGAIN (from an admit, or from fanout_prefix: records remain): let the consumers drain, then admit
  *                    and fan out again with the same (n, now_ns); the batch resumes at its first undelivered record.
+ * Where no one thread can take that minimum (one process per GPU), the shards agree on it through the publisher's memory:
+ *   every step     : [publisher] cpbus_stream_put(st, events, n, now_ns, flags)
+ *                    [all shards] cpbus_stream_admit(st, n, now_ns, &p)        CPBUS_EAGAIN: p = 0, stalled = 1
+ *                    [all shards] cpbus_stream_offer(st, p, stalled)
+ *                    [all shards] cpbus_stream_agree(st, &m)                  CPBUS_EAGAIN: some shard stalled, m = 0
+ *                    [all shards] cpbus_stream_fanout_prefix(st, n, now_ns, m)   (skipped after CPBUS_EAGAIN from _agree)
+ * An offer is one 64-bit word {round, stalled, prefix} stored (st.release.sys) into a spare word of the shard's ack sector;
+ * the agree kernel acquires every shard's word of the current round (ld.acquire.sys, bounded by the stream timeout) and
+ * the host waits for that one kernel.  Each stream counts its admission rounds (one per _agree, on every shard alike), so
+ * a retry of the same batch never reads the previous round's offer.  Offers are split from the wait so that one thread
+ * driving several attached shards can post every offer before it waits on any.
  * While the mailboxes provably have room, admission costs no kernel and no host sync (as for cpbus_flush).  A batch's slot
  * is acknowledged only when its last record has been fanned out, so the publisher cannot run more than n_slots batches
  * ahead of the slowest shard.  Plain cpbus_stream_fanout returns CPBUS_EINVAL on a lossless bus.
@@ -295,6 +306,15 @@ int cpbus_stream_admit(cpbus_stream_t* st, size_t n, uint64_t now_ns, size_t* pr
  * the minimum of the shards' admitted prefixes; more than this shard admitted would overfill a mailbox).  An empty batch
  * has a remainder of 0: m = 0 completes it. */
 int cpbus_stream_fanout_prefix(cpbus_stream_t* st, size_t n, uint64_t now_ns, size_t m);
+/* Lossless stream across processes: post this shard's admitted prefix, then learn the minimum over all shards.
+ * _offer is asynchronous (a one-thread kernel on the bus stream).  CPBUS_EINVAL: a throughput-mode bus, a second offer in
+ * one round, a prefix beyond the remainder of the batch last admitted, or stalled != 0 with a prefix.
+ * _agree waits for every shard's offer of this round and sets *m to the minimum prefix.  CPBUS_EAGAIN (*m = 0): some
+ * shard stalled — let the consumers drain, then run the round again with the same (n, now_ns).  CPBUS_ETIMEDOUT: a shard
+ * did not offer within the stream timeout; sticky, as for a batch that never arrives.  CPBUS_EINVAL: no offer this round,
+ * or a throughput-mode bus. */
+int cpbus_stream_offer(cpbus_stream_t* st, size_t prefix, int stalled);   /* async, stream-ordered */
+int cpbus_stream_agree(cpbus_stream_t* st, size_t* m);                   /* waits for every shard's offer */
 /* For a consumer whose driver does not know the batches' shapes: *ready = 1 and {n, now_ns} of the NEXT batch if the publisher
  * has released it, *ready = 0 otherwise (one 32-byte read of the slot header, synchronous).  Then cpbus_stream_fanout(st, n, now_ns). */
 int cpbus_stream_poll(cpbus_stream_t* st, int* ready, size_t* n, uint64_t* now_ns);
