@@ -216,6 +216,12 @@ class Bus:
         nat.check(self._lib.cpbus_stream_poll(st, C.byref(ready), C.byref(n), C.byref(now)), "cpbus_stream_poll")
         return (n.value, now.value) if ready.value else None
 
+    def stream_fanout_next(self, st) -> int:
+        """follower: enqueue the fan-out of the stream's next batch without knowing its shape (n and the watermark come
+        from the slot header inside the kernel); returns at once.  Outstanding followers are resolved by the next call
+        that reads or changes this bus's host state."""
+        return self._lib.cpbus_stream_fanout_next(st)
+
     def stream_status(self, st) -> int:
         return self._lib.cpbus_stream_status(st)
 

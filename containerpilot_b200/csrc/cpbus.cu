@@ -107,6 +107,16 @@ struct cpbus {
   unsigned int* h_err = nullptr;              // pinned + mapped: kErr* bits written by the fan-out kernel
   unsigned int* d_err = nullptr;              // device alias of h_err
   uint32_t stream_spin_us = 0;                // bound of the in-kernel wait for a stream batch (0 = 2 s)
+  // follower launches (cpbus_stream_fanout_next): enqueued without the batch's shape, resolved lazily (follow_resolve)
+  static constexpr int kFollowMax = 8;        // outstanding at most; the next one resolves first
+  struct FollowPending { cpbus_stream* st; unsigned long long launch_seq; int rec; };
+  std::vector<FollowPending> follow_q;        // outstanding, in launch order
+  FollowRec* h_follow = nullptr;              // pinned + mapped: kFollowMax records written by the lead CTAs
+  FollowRec* d_follow = nullptr;              // device alias of h_follow
+  unsigned long long* d_follow_clock = nullptr;   // 4 words: {watermark, launch ordinal} by launch parity
+  int follow_next = 0;
+  cudaEvent_t follow_done = nullptr;
+  std::recursive_mutex follow_mu;              // the queue, when stats or drains on another thread resolve it
   // accounting of device-published batches (cpbus_publish_device*, cpbus_stream_fanout): done by the kernel's lead CTA
   DevPubAcct* d_acct = nullptr;
   DevPubAcct* h_acct = nullptr;               // pinned staging for cpbus_stats / cpbus_debug_events / cpbus_publish_counts
@@ -205,6 +215,13 @@ int dev_guard(cpbus* b) {
   return CPBUS_OK;
 }
 
+// The sticky stream error of this bus: a followed batch out of order (CPBUS_EORDER), otherwise a batch that never arrived or
+// did not match its header (CPBUS_ETIMEDOUT).
+int stream_error(const cpbus* b) {
+  const unsigned int e = *(volatile const unsigned int*)b->h_err;
+  return (e & kErrFollowOrder) ? CPBUS_EORDER : (e ? CPBUS_ETIMEDOUT : CPBUS_OK);
+}
+
 uint32_t mask_word(const cpbus* b, uint32_t local) {
   uint32_t hint = 0;
   if (b->K && !b->h_timers.empty())
@@ -289,12 +306,14 @@ int rebuild_order(cpbus* b) {
 constexpr int kFanoutMaxSmem = 200 * 1024;
 
 template <int STORE, bool TIMERS, bool DIGEST, bool ORDERED, bool PAIRS = false>
-int launch_fanout_t(cpbus* b, const FanoutParams& p, uint32_t grid, size_t smem) {
-  static bool attr_done[64] = {};   // per instantiation AND per device: function attributes are per-device state
+int launch_fanout_t(cpbus* b, const FanoutParams& p, uint32_t grid, size_t smem, bool follow) {
+  static bool attr_done[2][64] = {};   // per instantiation AND per device: function attributes are per-device state
+  void (*kernel)(FanoutParams) = follow ? fanout_follow_kernel<STORE, TIMERS, DIGEST, ORDERED, PAIRS>
+                                        : fanout_kernel<STORE, TIMERS, DIGEST, ORDERED, PAIRS>;
   const int dev = b->device & 63;
-  if (!attr_done[dev]) {
-    CK(cudaFuncSetAttribute(fanout_kernel<STORE, TIMERS, DIGEST, ORDERED, PAIRS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kFanoutMaxSmem));
-    attr_done[dev] = true;
+  if (!attr_done[follow][dev]) {
+    CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kFanoutMaxSmem));
+    attr_done[follow][dev] = true;
   }
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = smem; cfg.stream = b->stream;
@@ -302,16 +321,20 @@ int launch_fanout_t(cpbus* b, const FanoutParams& p, uint32_t grid, size_t smem)
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;   // PDL: the next fan-out's prologue overlaps this one's tail
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr; cfg.numAttrs = b->pdl ? 1 : 0;
-  CK(cudaLaunchKernelEx(&cfg, fanout_kernel<STORE, TIMERS, DIGEST, ORDERED, PAIRS>, p));
+  CK(cudaLaunchKernelEx(&cfg, kernel, p));
   CK(cudaGetLastError());
   return CPBUS_OK;
 }
+
+uint64_t max_window(const cpbus* b);
 
 // fan out `n` records at d_src with watermark w (all checks done by the caller)
 struct StreamArgs {   // stream mode (cpbus_stream_fanout_prefix): where this batch's header / ack words live
   const StreamHdr* hdr = nullptr; unsigned long long* ack = nullptr; unsigned long long seq = 0;
   const StreamHdr* next_hdr = nullptr;
   uint32_t off = 0; bool final = true;   // records delivered before this launch; whether it completes the batch
+  FollowRec* follow_rec = nullptr;       // follower launch (cpbus_stream_fanout_next): n and the watermark come from the header
+  bool follow_from_host = false;         // ... and the previous watermark is the host clock rather than the clock words
 };
 
 int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, int staged = 0,
@@ -331,6 +354,11 @@ int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, in
   if (sa) {
     p.stream_hdr = sa->hdr; p.stream_ack = sa->ack; p.stream_seq = sa->seq; p.stream_next_hdr = sa->next_hdr;
     p.stream_off = sa->off; p.stream_final = sa->final ? 1u : 0u;
+  }
+  const bool follow = sa && sa->follow_rec;
+  if (follow) {   // n = batch_cap sizes the launch; the kernel takes the batch's own n and watermark from the header
+    p.follow_clock = b->d_follow_clock; p.follow_rec = sa->follow_rec; p.follow_window = max_window(b);
+    p.follow_from_host = sa->follow_from_host ? 1u : 0u;
   }
   p.prefetch_src = prefetch_src; p.prefetch_dst = prefetch_dst; p.prefetch_n = prefetch_n;
   p.batch_dep = batch_dep ? 1u : 0u; p.n_ev = n;
@@ -399,14 +427,14 @@ int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, in
   const int variant = pairs_on ? (p.use_digest ? 7 : 6) : (p.timers_on ? 2 : 0) | (p.use_digest ? 1 : 0) | (p.order ? 4 : 0);
 #define CPBUS_DISPATCH(ST)                                                                \
   switch (variant) {                                                                     \
-    case 0: rc = launch_fanout_t<ST, false, false, false>(b, p, grid, smem); break;      \
-    case 1: rc = launch_fanout_t<ST, false, true, false>(b, p, grid, smem); break;       \
-    case 2: rc = launch_fanout_t<ST, true, false, false>(b, p, grid, smem); break;       \
-    case 3: rc = launch_fanout_t<ST, true, true, false>(b, p, grid, smem); break;        \
-    case 4: rc = launch_fanout_t<ST, false, false, true>(b, p, grid, smem); break;       \
-    case 5: rc = launch_fanout_t<ST, false, true, true>(b, p, grid, smem); break;        \
-    case 6: rc = launch_fanout_t<ST, true, false, false, true>(b, p, grid, smem); break; \
-    default: rc = launch_fanout_t<ST, true, true, false, true>(b, p, grid, smem); break; \
+    case 0: rc = launch_fanout_t<ST, false, false, false>(b, p, grid, smem, follow); break;      \
+    case 1: rc = launch_fanout_t<ST, false, true, false>(b, p, grid, smem, follow); break;       \
+    case 2: rc = launch_fanout_t<ST, true, false, false>(b, p, grid, smem, follow); break;       \
+    case 3: rc = launch_fanout_t<ST, true, true, false>(b, p, grid, smem, follow); break;        \
+    case 4: rc = launch_fanout_t<ST, false, false, true>(b, p, grid, smem, follow); break;       \
+    case 5: rc = launch_fanout_t<ST, false, true, true>(b, p, grid, smem, follow); break;        \
+    case 6: rc = launch_fanout_t<ST, true, false, false, true>(b, p, grid, smem, follow); break; \
+    default: rc = launch_fanout_t<ST, true, true, false, true>(b, p, grid, smem, follow); break; \
   }
   switch (b->store) {
     case CPBUS_STORE_V4: CPBUS_DISPATCH(CPBUS_STORE_V4); break;
@@ -416,6 +444,7 @@ int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, in
 #undef CPBUS_DISPATCH
   if (rc) return rc;
   b->st.batches++; b->st.kernel_launches++;
+  if (follow) return CPBUS_OK;   // clock and debug-ring marker: when the launch is resolved (follow_resolve)
   b->last_watermark = w;
   if (account && n) dbg_mark_device_batch(b, p.launch_seq);
   return CPBUS_OK;
@@ -561,6 +590,7 @@ bool is_pow2(uint32_t x) { return x && !(x & (x - 1)); }
 }  // namespace
 
 extern "C" {
+static int follow_resolve(cpbus* b);
 // Nothing may unwind through the C boundary (cgo, ctypes): every status-returning entry point is a function-try-block.
 #define CPBUS_CATCH                                                                                   \
   catch (const std::bad_alloc&) { return CPBUS_ENOMEM; }                                              \
@@ -749,9 +779,13 @@ int cpbus_create(const cpbus_config* cfg, cpbus_t** out) try {
 
 int cpbus_destroy(cpbus_t* b) try {
   if (!b) return CPBUS_EINVAL;
+  follow_resolve(b);
   cudaSetDevice(b->device);
   if (b->stream) cudaStreamSynchronize(b->stream);
   while (!b->streams.empty()) cpbus_stream_close(b->streams.back());
+  if (b->h_follow) cudaFreeHost(b->h_follow);
+  cudaFree(b->d_follow_clock);
+  if (b->follow_done) cudaEventDestroy(b->follow_done);
   cudaFree(b->d_ring); cudaFree(b->d_ctl); cudaFree(b->d_order); cudaFree(b->d_pairs);
   cudaFree(b->d_timers); cudaFree(b->d_stats); cudaFree(b->d_fold); cudaFree(b->d_pow); cudaFree(b->d_desc); cudaFree(b->d_desc_ready);
   if (b->copy_stream) cudaStreamSynchronize(b->copy_stream);
@@ -844,6 +878,7 @@ int cpbus_subscribe_many(cpbus_t* b, const uint32_t* masks, uint32_t n, uint32_t
   if (!b || !n) return CPBUS_EINVAL;
   if ((uint64_t)b->n_next + n > b->N) return CPBUS_ENOSPC;
   int rc = dev_guard(b); if (rc) return rc;
+  if ((rc = follow_resolve(b))) return rc;
   if ((rc = flush_staged(b, b->now))) return rc;   // ordered with publishes (events/bus.go:105-107 takes the same lock)
   const uint32_t first = b->n_next;
   std::vector<SubCtl> blocks(n);
@@ -875,6 +910,7 @@ int cpbus_subscribe_pairs(cpbus_t* b, uint32_t mask, const cpbus_pair* pairs, ui
     if (!((mask >> pairs[j].code) & 1u)) row[used++] = make_uint2(pairs[j].code, pairs[j].source_id);
   if (used == 0) return cpbus_subscribe_many(b, &mask, 1, sub_id);
   int rc = dev_guard(b); if (rc) return rc;
+  if ((rc = follow_resolve(b))) return rc;
   if (!b->d_pairs) {
     if (cudaMalloc((void**)&b->d_pairs, (size_t)b->N * CPBUS_MAX_PAIRS * sizeof(uint2)) != cudaSuccess) {
       snprintf(g_cuda_err, sizeof(g_cuda_err), "cudaMalloc(pair tables) failed");
@@ -904,6 +940,7 @@ int cpbus_subscribe_pairs_many(cpbus_t* b, const uint32_t* masks, const cpbus_pa
   }
   if ((uint64_t)b->n_next + n > b->N) return CPBUS_ENOSPC;
   int rc = dev_guard(b); if (rc) return rc;
+  if ((rc = follow_resolve(b))) return rc;
   if (!b->d_pairs) {
     if (cudaMalloc((void**)&b->d_pairs, (size_t)b->N * CPBUS_MAX_PAIRS * sizeof(uint2)) != cudaSuccess) {
       snprintf(g_cuda_err, sizeof(g_cuda_err), "cudaMalloc(pair tables) failed");
@@ -940,6 +977,7 @@ int cpbus_unsubscribe(cpbus_t* b, uint32_t sub_id) try {
   const uint32_t l = sub_id - b->cfg.sub_id_base;
   if (sub_id < b->cfg.sub_id_base || l >= b->n_next) return CPBUS_ENOENT;
   int rc = dev_guard(b); if (rc) return rc;
+  if ((rc = follow_resolve(b))) return rc;
   if ((rc = flush_staged(b, b->now))) return rc;
   // second Unsubscribe drives the WaitGroup negative in Go (events/bus.go:121) => panic
   if (!b->h_active[l]) return CPBUS_ECLOSED;
@@ -970,6 +1008,7 @@ int cpbus_set_mask(cpbus_t* b, uint32_t sub_id, uint32_t mask) try {
   if (sub_id < b->cfg.sub_id_base || l >= b->n_next) return CPBUS_ENOENT;
   if (!b->h_active[l]) return CPBUS_ECLOSED;
   int rc = dev_guard(b); if (rc) return rc;
+  if ((rc = follow_resolve(b))) return rc;
   if ((rc = flush_staged(b, b->now))) return rc;
   mask &= CPBUS_MASK_ALL;
   if (b->h_mask[l] != CPBUS_MASK_ALL) b->n_filtered--;
@@ -992,6 +1031,7 @@ int cpbus_timer_add(cpbus_t* b, uint32_t sub_id, uint64_t period_ns, uint32_t so
   const uint32_t l = sub_id - b->cfg.sub_id_base;
   if (sub_id < b->cfg.sub_id_base || l >= b->n_next) return CPBUS_ENOENT;
   int rc = dev_guard(b); if (rc) return rc;
+  if ((rc = follow_resolve(b))) return rc;
   if ((rc = flush_staged(b, b->now))) return rc;
   if (b->h_timers.empty()) b->h_timers.resize((size_t)b->N * b->K);
   retire_oneshots(b, b->last_watermark);
@@ -1020,6 +1060,7 @@ int cpbus_timer_add_many(cpbus_t* b, uint32_t first_sub, uint32_t n, uint64_t pe
   const uint32_t l0 = first_sub - b->cfg.sub_id_base;
   if (first_sub < b->cfg.sub_id_base || (uint64_t)l0 + n > b->n_next) return CPBUS_ENOENT;
   int rc = dev_guard(b); if (rc) return rc;
+  if ((rc = follow_resolve(b))) return rc;
   if ((rc = flush_staged(b, b->now))) return rc;
   if (b->h_timers.empty()) b->h_timers.resize((size_t)b->N * b->K);
   // bulk arm: uses slot 0 of each subscriber (must be free)
@@ -1054,6 +1095,7 @@ int cpbus_timer_cancel(cpbus_t* b, uint32_t timer_id) try {
   const uint32_t l = slot_index / b->K, k = slot_index % b->K;
   if (l >= b->n_next) return CPBUS_ENOENT;
   int rc = dev_guard(b); if (rc) return rc;
+  if ((rc = follow_resolve(b))) return rc;
   if ((rc = flush_staged(b, b->now))) return rc;   // firings due before the cancel still happen
   retire_oneshots(b, b->last_watermark);
   HostTimer& t = b->h_timers[(size_t)l * b->K + k];
@@ -1068,6 +1110,7 @@ int cpbus_timer_cancel(cpbus_t* b, uint32_t timer_id) try {
 int cpbus_publish(cpbus_t* b, const cpbus_event* ev, size_t n) try {
   if (!b || (!ev && n)) return CPBUS_EINVAL;
   int rc = dev_guard(b); if (rc) return rc;
+  if ((rc = follow_resolve(b))) return rc;
   for (size_t i = 0; i < n; i++) {   // counter slots of the whole burst: requested up front, touched in the loop below
     if (ev[i].code < CPBUS_N_CODES && ev[i].code != CPBUS_METRIC) b->pub_pairs.prefetch(((uint64_t)ev[i].code << 32) | ev[i].source_id);
   }
@@ -1100,6 +1143,7 @@ int cpbus_send(cpbus_t* b, uint32_t sub_id, const cpbus_event* ev) try {
   if (sub_id < b->cfg.sub_id_base || l >= b->n_next) return CPBUS_ENOENT;
   if (!b->h_active[l]) return CPBUS_ECLOSED;   // the mailbox is gone (Go: send on a closed channel panics)
   int rc = dev_guard(b); if (rc) return rc;
+  if ((rc = follow_resolve(b))) return rc;
   if ((rc = stage_one(b, ev->code, ev->source_id, sub_id, CPBUS_F_UNICAST))) return rc;
   b->st.publishes++;
   return CPBUS_OK;
@@ -1107,9 +1151,10 @@ int cpbus_send(cpbus_t* b, uint32_t sub_id, const cpbus_event* ev) try {
 
 int cpbus_advance(cpbus_t* b, uint64_t now_ns) try {
   if (!b) return CPBUS_EINVAL;
+  int rc = follow_resolve(b); if (rc) return rc;   // the clock moves with the batches that followers fanned out
   if (now_ns < b->now) return CPBUS_EORDER;
   if (now_ns == b->now) return CPBUS_OK;
-  int rc = dev_guard(b); if (rc) return rc;
+  if ((rc = dev_guard(b))) return rc;
   // the kernel looks at <= 32/K candidate firings per timer slot per launch: keep every
   // flush window within that many periods of the fastest periodic timer
   const uint64_t win = max_window(b);
@@ -1124,12 +1169,14 @@ int cpbus_advance(cpbus_t* b, uint64_t now_ns) try {
 int cpbus_flush(cpbus_t* b) try {
   if (!b) return CPBUS_EINVAL;
   int rc = dev_guard(b); if (rc) return rc;
+  if ((rc = follow_resolve(b))) return rc;
   return flush_staged(b, b->now);
 } CPBUS_CATCH
 
 int cpbus_sync(cpbus_t* b) try {
   if (!b) return CPBUS_EINVAL;
   int rc = dev_guard(b); if (rc) return rc;
+  if ((rc = follow_resolve(b))) return rc;
   CK(cudaStreamSynchronize(b->stream));
   return CPBUS_OK;
 } CPBUS_CATCH
@@ -1193,6 +1240,7 @@ static int publish_device_impl(cpbus_t* b, const void* d_events, size_t n, uint6
                                const void* d_next, size_t n_next) {
   if (!b || (!d_events && n) || ((uintptr_t)d_events & 31u) || n_next > b->B || ((uintptr_t)d_next & 31u)) return CPBUS_EINVAL;
   int rc = dev_guard(b); if (rc) return rc;
+  if ((rc = follow_resolve(b))) return rc;
   if ((rc = flush_staged(b, b->now))) return rc;
   if (watermark_ns < b->now) return CPBUS_EORDER;
   if (staged && b->lossless) return CPBUS_EINVAL;   // admission would have to read the peer batch: not supported
@@ -1299,6 +1347,7 @@ struct cpbus_stream {
   cpbus_event* payload = nullptr;
   unsigned long long put_seq = 0, get_seq = 0;   // batches released / fanned out so far (ordinals are 1-based)
   uint32_t get_off = 0;                      // lossless mode: records of batch get_seq + 1 already delivered
+  uint32_t follow_out = 0;                   // follower launches of batches get_seq + 1 .. not yet resolved
   unsigned long long seen_seq = 0;           // highest batch whose release this consumer has seen from the host
   unsigned long long pub_seq = 0;            // publisher: publish ordinal stamped into the next record (CPBUS_PUT_STAMP)
   unsigned long long min_ack = 0;            // publisher: cached min over the consumers' acks
@@ -1409,6 +1458,7 @@ int cpbus_stream_attach(cpbus_t* b, cpbus_stream_t* owner, uint32_t consumer_ind
 int cpbus_stream_close(cpbus_stream_t* st) try {
   if (!st) return CPBUS_EINVAL;
   cpbus* b = st->bus;
+  follow_resolve(b);   // (teardown: the records of outstanding followers are folded in before the stream goes)
   cudaSetDevice(b->device);
   cudaStreamSynchronize(b->stream);
   if (st->put_stream) { cudaStreamSynchronize(st->put_stream); cudaStreamDestroy(st->put_stream); }
@@ -1434,7 +1484,8 @@ int cpbus_stream_set_timeout(cpbus_stream_t* st, uint32_t microseconds) try {
 
 int cpbus_stream_status(cpbus_stream_t* st) try {
   if (!st) return CPBUS_EINVAL;
-  return (*(volatile unsigned int*)st->bus->h_err) ? CPBUS_ETIMEDOUT : CPBUS_OK;
+  const int rc = follow_resolve(st->bus); if (rc) return rc;
+  return stream_error(st->bus);
 } CPBUS_CATCH
 
 // Publisher: copy the batch into the next slot, then release it (header after payload, same stream).
@@ -1490,7 +1541,8 @@ int cpbus_stream_poll(cpbus_stream_t* st, int* ready, size_t* n, uint64_t* now_n
   if (!st || !ready) return CPBUS_EINVAL;
   cpbus* b = st->bus;
   int rc = dev_guard(b); if (rc) return rc;
-  if (*(volatile unsigned int*)b->h_err) return CPBUS_ETIMEDOUT;
+  if ((rc = follow_resolve(b))) return rc;
+  if ((rc = stream_error(b))) return rc;
   const unsigned long long q = st->get_seq + 1;
   StreamHdr h{};
   CK(cudaMemcpyAsync(&h, &st->hdr[q % st->n_slots], sizeof(h), cudaMemcpyDeviceToHost, b->result_stream));
@@ -1526,7 +1578,8 @@ static int stream_wait_released(cpbus_stream* st, unsigned long long q, size_t n
 static int stream_enter(cpbus_stream* st, uint64_t now_ns) {
   cpbus* b = st->bus;
   int rc = dev_guard(b); if (rc) return rc;
-  if (*(volatile unsigned int*)b->h_err) return CPBUS_ETIMEDOUT;
+  if ((rc = follow_resolve(b))) return rc;
+  if ((rc = stream_error(b))) return rc;
   if ((rc = flush_staged(b, b->now))) return rc;
   if (now_ns < b->now) return CPBUS_EORDER;
   if (now_ns - b->last_watermark > max_window(b)) return CPBUS_EORDER;
@@ -1615,6 +1668,77 @@ int cpbus_stream_fanout(cpbus_stream_t* st, size_t n, uint64_t now_ns) try {
   return stream_fanout_prefix(st, n, now_ns, n - st->get_off);
 } CPBUS_CATCH
 
+// Outstanding follower launches: one wait on the last of them, then their records in launch order.  A launch that delivered
+// moves the stream, the clock and the publish ordinals exactly as cpbus_stream_fanout with the header's shape does; an
+// aborted one (and every follower behind it, each a no-op) changes nothing but the sticky error word.
+static int follow_resolve(cpbus* b) {
+  std::lock_guard<std::recursive_mutex> g(b->follow_mu);
+  if (b->follow_q.empty()) return CPBUS_OK;
+  int rc = dev_guard(b); if (rc) return rc;
+  CK(cudaEventRecord(b->follow_done, b->stream));
+  CK(cudaEventSynchronize(b->follow_done));
+  std::vector<cpbus::FollowPending> q;
+  q.swap(b->follow_q);
+  bool missing = false;
+  for (const cpbus::FollowPending& f : q) {
+    const volatile FollowRec* r = &b->h_follow[f.rec];
+    f.st->follow_out--;
+    if (r->status == kFollowPending) missing = true;
+    if (r->status != kFollowDelivered) continue;
+    const uint32_t n = r->n;
+    const uint64_t w = r->watermark;
+    f.st->get_seq++;
+    b->st.publishes += n; b->seq += n;
+    b->now = w; b->last_watermark = w;
+    if (n) dbg_mark_device_batch(b, f.launch_seq);
+  }
+  if (missing) { snprintf(g_cuda_err, sizeof(g_cuda_err), "a follower launch completed without its record"); return CPBUS_ECUDA; }
+  return CPBUS_OK;
+}
+
+// Every rank that does not know the batches' shapes: enqueue the fan-out of the stream's next not yet enqueued batch and
+// return.  The lead CTA takes n and the watermark from the slot header; the host learns them when it next resolves.
+int cpbus_stream_fanout_next(cpbus_stream_t* st) try {
+  if (!st) return CPBUS_EINVAL;
+  cpbus* b = st->bus;
+  if (b->lossless) return CPBUS_EINVAL;   // lossless followers agree on every round, which syncs anyway
+  std::lock_guard<std::recursive_mutex> g(b->follow_mu);
+  int rc = dev_guard(b); if (rc) return rc;
+  if (b->follow_q.size() >= (size_t)cpbus::kFollowMax && (rc = follow_resolve(b))) return rc;
+  if ((rc = stream_error(b))) return rc;
+  if (!b->h_follow) {
+    FollowRec *h = nullptr, *d = nullptr;
+    CK(cudaHostAlloc((void**)&h, sizeof(FollowRec) * cpbus::kFollowMax, cudaHostAllocMapped));
+    if (cudaHostGetDevicePointer((void**)&d, h, 0) != cudaSuccess) { cudaFreeHost(h); CK(cudaGetLastError()); return CPBUS_ECUDA; }
+    b->h_follow = h; b->d_follow = d;
+  }
+  if (!b->d_follow_clock) {
+    CK(cudaMalloc((void**)&b->d_follow_clock, 4 * sizeof(unsigned long long)));
+    CK(cudaMemsetAsync(b->d_follow_clock, 0, 4 * sizeof(unsigned long long), b->stream));
+  }
+  if (!b->follow_done) CK(cudaEventCreateWithFlags(&b->follow_done, cudaEventDisableTiming));
+  // The first follower after the host has resolved starts from the host clock (this bus's own staged events go out first,
+  // as in cpbus_stream_fanout); the ones queued behind it read their predecessor's watermark on the device.
+  const bool from_host = b->follow_q.empty();
+  if (from_host && (rc = flush_staged(b, b->now))) return rc;
+  const unsigned long long q = st->get_seq + 1 + st->follow_out;
+  const uint32_t slot = (uint32_t)(q % st->n_slots), slot2 = (uint32_t)((q + 2) % st->n_slots);
+  const int ri = b->follow_next;
+  b->h_follow[ri].status = kFollowPending;
+  StreamArgs sa;
+  sa.hdr = &st->hdr[slot]; sa.ack = &st->ack[4 * st->consumer]; sa.seq = q; sa.off = 0; sa.final = true;
+  sa.next_hdr = &st->hdr[slot2];
+  sa.follow_rec = b->d_follow + ri; sa.follow_from_host = from_host;
+  rc = launch_fanout(b, st->payload + (size_t)slot * st->B, b->B, b->now, /*staged=*/2,
+                     st->payload + (size_t)slot2 * st->B, b->d_pf_buf + (size_t)((q + 2) % kStreamPrefetch) * b->B, 0,
+                     /*batch_dep=*/false, /*account=*/true, &sa);
+  if (rc) return rc;
+  b->follow_next = (ri + 1) % cpbus::kFollowMax;
+  b->follow_q.push_back(cpbus::FollowPending{st, b->launch_seq, ri});
+  st->follow_out++;
+  return CPBUS_OK;
+} CPBUS_CATCH
+
 // Lossless stream across processes, step 1 of the exchange: post this shard's admitted prefix for the current round.
 // One-thread kernel on the bus stream (behind the admission pass when it ran); no host sync.
 int cpbus_stream_offer(cpbus_stream_t* st, size_t prefix, int stalled) try {
@@ -1624,7 +1748,7 @@ int cpbus_stream_offer(cpbus_stream_t* st, size_t prefix, int stalled) try {
   const size_t n = st->admit_q == st->get_seq + 1 ? st->admit_n : st->B;   // the batch's shape when this shard admitted it
   if (prefix > n - st->get_off || (stalled && prefix)) return CPBUS_EINVAL;
   int rc = dev_guard(b); if (rc) return rc;
-  if (*(volatile unsigned int*)b->h_err) return CPBUS_ETIMEDOUT;
+  if ((rc = stream_error(b))) return rc;
   const unsigned long long r = st->agree_round + 1;
   stream_offer_kernel<<<1, 1, 0, b->stream>>>(st->ack + stream_offer_word_index(st->consumer, r),
                                               stream_offer_word(r, stalled ? 1u : 0u, (uint32_t)prefix));
@@ -1642,7 +1766,7 @@ int cpbus_stream_agree(cpbus_stream_t* st, size_t* m) try {
   cpbus* b = st->bus;
   if (!b->lossless || !st->offered) return CPBUS_EINVAL;
   int rc = dev_guard(b); if (rc) return rc;
-  if (*(volatile unsigned int*)b->h_err) return CPBUS_ETIMEDOUT;
+  if ((rc = stream_error(b))) return rc;
   if (!st->h_agree) {
     StreamAgreeResult *h = nullptr, *d = nullptr;
     CK(cudaHostAlloc((void**)&h, sizeof(StreamAgreeResult), cudaHostAllocMapped));
@@ -1691,6 +1815,7 @@ int cpbus_drain(cpbus_t* b, uint32_t sub_id, cpbus_event* out, size_t cap, size_
   if (sub_id < b->cfg.sub_id_base || l >= b->n_next) return CPBUS_ENOENT;
   std::lock_guard<std::mutex> g(b->mu);
   int rc = dev_guard(b); if (rc) return rc;
+  if ((rc = follow_resolve(b))) return rc;
   uint64_t tail = 0, head = 0;
   uint64_t gone = 0;
   if ((rc = read_cursors(b, l, &tail, &head, &gone))) return rc;
@@ -1713,6 +1838,7 @@ int cpbus_drain_many(cpbus_t* b, uint32_t first_sub, uint32_t n, cpbus_event* ou
   if (first_sub < b->cfg.sub_id_base || (uint64_t)l + n > b->n_next) return CPBUS_ENOENT;
   std::lock_guard<std::mutex> g(b->mu);
   int rc = dev_guard(b); if (rc) return rc;
+  if ((rc = follow_resolve(b))) return rc;
   if (b->drain_cap < cap || b->drain_idx_cap < n) {   // device staging grows on demand and is kept
     if (b->drain_cap < cap) { cudaFree(b->d_drain); b->d_drain = nullptr; CK(cudaMalloc((void**)&b->d_drain, cap * sizeof(cpbus_event))); b->drain_cap = cap; }
     if (b->drain_idx_cap < n) { cudaFree(b->d_drain_idx); b->d_drain_idx = nullptr; CK(cudaMalloc((void**)&b->d_drain_idx, (size_t)n * sizeof(uint2) + 16)); b->drain_idx_cap = n; }
@@ -1750,6 +1876,7 @@ int cpbus_drain_ready(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start
   if (first_sub < b->cfg.sub_id_base || (uint64_t)l + n > b->n_next) return CPBUS_ENOENT;
   std::lock_guard<std::mutex> g(b->mu);
   int rc = dev_guard(b); if (rc) return rc;
+  if ((rc = follow_resolve(b))) return rc;
   const size_t rcap = std::min<size_t>(ready_cap, n);   // never more entries than mailboxes
   const uint32_t tiles = (n + kReadyTile - 1) / kReadyTile;
   // device staging grows on demand and is kept (the records share cpbus_drain_many's buffer)
@@ -1803,6 +1930,7 @@ int cpbus_consume_all(cpbus_t* b) try {
   if (!b) return CPBUS_EINVAL;
   std::lock_guard<std::mutex> g(b->mu);
   int rc = dev_guard(b); if (rc) return rc;
+  if ((rc = follow_resolve(b))) return rc;
   if (b->n_next) {
     const uint32_t threads = 256, grid = std::min<uint32_t>((b->n_next + threads - 1) / threads, (uint32_t)b->sm_count * 8);
     consume_all_kernel<<<grid, threads, 0, b->stream>>>(b->d_ctl, b->n_next);
@@ -1819,6 +1947,7 @@ int cpbus_peek_window(cpbus_t* b, uint32_t sub_id, cpbus_event* out, size_t cap,
   if (sub_id < b->cfg.sub_id_base || l >= b->n_next) return CPBUS_ENOENT;
   std::lock_guard<std::mutex> g(b->mu);
   int rc = dev_guard(b); if (rc) return rc;
+  if ((rc = follow_resolve(b))) return rc;
   uint64_t tail = 0, head = 0;
   if ((rc = read_cursors(b, l, &tail, &head))) return rc;
   const size_t take = (size_t)std::min<uint64_t>(std::min<uint64_t>(tail, b->R), cap);
@@ -1833,6 +1962,7 @@ int cpbus_digest(cpbus_t* b, uint32_t first_sub, uint32_t n, cpbus_digest_t* out
   if (first_sub < b->cfg.sub_id_base || (uint64_t)l + n > b->n_next) return CPBUS_ENOENT;
   std::lock_guard<std::mutex> g(b->mu);
   int rc = dev_guard(b); if (rc) return rc;
+  if ((rc = follow_resolve(b))) return rc;
   std::vector<SubCtl> c(n);
   CK(cudaMemcpyAsync(c.data(), b->d_ctl + l, (size_t)n * sizeof(SubCtl), cudaMemcpyDeviceToHost, b->stream));
   CK(cudaStreamSynchronize(b->stream));
@@ -1869,7 +1999,9 @@ int cpbus_digest_fold_end(cpbus_t* b, uint32_t ticket, uint64_t out[4]) try {
 
 int cpbus_digest_fold(cpbus_t* b, uint32_t first_sub, uint32_t n, uint64_t out[4]) try {
   uint32_t ticket = 0;
-  int rc = cpbus_digest_fold_begin(b, first_sub, n, &ticket);
+  int rc = b ? follow_resolve(b) : CPBUS_OK;
+  if (rc) return rc;
+  rc = cpbus_digest_fold_begin(b, first_sub, n, &ticket);
   return rc ? rc : cpbus_digest_fold_end(b, ticket, out);
 } CPBUS_CATCH
 
@@ -1927,6 +2059,7 @@ static int dbg_resolve(cpbus* b) {
 
 int cpbus_debug_events(cpbus_t* b, cpbus_event* out, size_t cap, size_t* n) try {
   if (!b || !n || (!out && cap)) return CPBUS_EINVAL;
+  { const int rc = follow_resolve(b); if (rc) return rc; }
   { const int rc = dbg_resolve(b); if (rc) return rc; }
   size_t k = 0;
   for (;;) {
@@ -1946,6 +2079,7 @@ int cpbus_stats(cpbus_t* b, cpbus_stats_t* out) try {
   if (!b || !out) return CPBUS_EINVAL;
   std::lock_guard<std::mutex> g(b->mu);
   int rc = dev_guard(b); if (rc) return rc;
+  if ((rc = follow_resolve(b))) return rc;
   CK(cudaMemsetAsync(&b->d_stats->overwritten, 0, sizeof(unsigned long long), b->stream));
   if (!b->lossless && b->n_next) {
     const uint32_t threads = 256, grid = std::min<uint32_t>((b->n_next + threads - 1) / threads, (uint32_t)b->sm_count * 4);
@@ -1973,6 +2107,7 @@ int cpbus_publish_counts(cpbus_t* b, cpbus_pair_count* out, size_t cap, size_t* 
   if (!b || !n || (!out && cap)) return CPBUS_EINVAL;
   std::lock_guard<std::mutex> g(b->mu);
   int rc = dev_guard(b); if (rc) return rc;
+  if ((rc = follow_resolve(b))) return rc;
   std::unordered_map<uint64_t, uint64_t> merged;
   for (size_t i = 0; i < b->pub_pairs.keys.size(); i++) if (b->pub_pairs.keys[i]) merged[b->pub_pairs.keys[i] - 1] += b->pub_pairs.cnts[i];
   if (b->launch_seq) {

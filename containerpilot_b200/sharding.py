@@ -185,6 +185,15 @@ class ShardedBus(_ShardOps):
             nat.check(rc, "cpbus_stream_fanout_prefix")
         return rc
 
+    def follow(self, k: int = 1):
+        """Enqueue fan-outs of the stream's next `k` batches on this rank without knowing their shapes: each launch takes
+        n and the watermark from the slot header (`cpbus_stream_fanout_next`), so a rank that holds only subscriber shards
+        never sees the events and never syncs per batch.  Throughput mode only."""
+        if self.lossless:
+            raise RuntimeError("a lossless ShardedBus agrees on every batch's admitted prefix (fanout), which needs its shape")
+        for _ in range(k):
+            nat.check(self.bus.stream_fanout_next(self._st), "cpbus_stream_fanout_next")
+
     def publish(self, events: np.ndarray, now_ns: int) -> int:
         """put + fanout for callers that do not pipeline.  Lossless mode: one round, no retry (EAGAIN: drain, then
         `fanout` again)."""
@@ -383,6 +392,11 @@ class LocalShardedBus:
                 nat.check(r, "cpbus_stream_fanout_prefix")
             rc = r
         return rc
+
+    def follow(self, g: int, k: int = 1):
+        """Enqueue fan-outs of the stream's next `k` batches on shard `g` without their shapes (`cpbus_stream_fanout_next`)."""
+        for _ in range(k):
+            nat.check(self.shards[g][2].stream_fanout_next(self._st[g]), "cpbus_stream_fanout_next")
 
     def drain(self, sub_id: int, cap: int | None = None) -> np.ndarray:
         """Consumer side: up to `cap` records of global subscriber `sub_id`, from the shard that owns it."""

@@ -249,6 +249,8 @@ int cpbus_publish_device_staged(cpbus_t* bus, const void* d_events, size_t n, ui
  *   other ranks    : cpbus_stream_open(bus, handle, consumer_index (1..n_consumers-1), &st)
  *   every step     : [publisher] cpbus_stream_put(st, events, n, now_ns, flags)   (may run ahead by < n_slots batches)
  *                    [all ranks] cpbus_stream_fanout(st, n, now_ns)
+ *   followers      : [ranks that are never told n, now_ns] cpbus_stream_fanout_next(st) — the kernel reads them from the slot
+ *                    header; may be called ahead of the publisher (throughput mode only)
  * Lossless mode (CPBUS_CFG_LOSSLESS): a stalled publish must stop at the same event on every shard — the shortest of the
  * prefixes the shards can take — so the fan-out is split in two and the driver takes the minimum in between:
  *   every step     : [publisher] cpbus_stream_put(st, events, n, now_ns, flags)
@@ -270,10 +272,11 @@ int cpbus_publish_device_staged(cpbus_t* bus, const void* d_events, size_t n, ui
  * While the mailboxes provably have room, admission costs no kernel and no host sync (as for cpbus_flush).  A batch's slot
  * is acknowledged only when its last record has been fanned out, so the publisher cannot run more than n_slots batches
  * ahead of the slowest shard.  Plain cpbus_stream_fanout returns CPBUS_EINVAL on a lossless bus.
- * The consumers must be told n and now_ns of every batch by the caller: SPMD drivers know them; others ask cpbus_stream_poll,
- * which reads them from the slot header (the kernel cross-checks n either way).  CPBUS_EAGAIN from _put: the slot's previous batch is still not acknowledged by every
+ * cpbus_stream_fanout must be told n and now_ns of every batch by the caller: SPMD drivers know them; others follow with
+ * cpbus_stream_fanout_next, or ask cpbus_stream_poll, which reads them from the slot header (the kernel cross-checks n).  CPBUS_EAGAIN from _put: the slot's previous batch is still not acknowledged by every
  * consumer after the stream timeout (or at once with CPBUS_PUT_NOWAIT) — call again after the consumers have advanced.  CPBUS_ETIMEDOUT from _fanout/_status: an earlier stream
- * launch gave up waiting for its batch (bounded in-kernel wait, cpbus_stream_set_timeout) and delivered nothing. */
+ * launch gave up waiting for its batch (bounded in-kernel wait, cpbus_stream_set_timeout) and delivered nothing; CPBUS_EORDER
+ * from every stream call: a follower's batch was behind the clock or beyond the timer window (see _fanout_next). */
 typedef struct cpbus_stream cpbus_stream_t;
 #define CPBUS_PUT_STAMP 0x0u /* records are stamped like cpbus_publish: seq = running publish ordinal, ts = now_ns,
                                 target = ALL, flags = 0; only code/source_id are read from the caller's records */
@@ -318,6 +321,22 @@ int cpbus_stream_agree(cpbus_stream_t* st, size_t* m);                   /* wait
 /* For a consumer whose driver does not know the batches' shapes: *ready = 1 and {n, now_ns} of the NEXT batch if the publisher
  * has released it, *ready = 0 otherwise (one 32-byte read of the slot header, synchronous).  Then cpbus_stream_fanout(st, n, now_ns). */
 int cpbus_stream_poll(cpbus_stream_t* st, int* ready, size_t* n, uint64_t* now_ns);
+/* Stream followers: a consumer that never learns the batches' shapes (a rank that holds only subscriber shards).
+ * _fanout_next enqueues the fan-out of the stream's next batch on the bus stream and returns at once: the kernel's lead CTA
+ * takes n and the watermark from the slot header it acquires anyway.  Call it several times in a row to run ahead of the
+ * publisher; each launch waits in the kernel for its batch, bounded by the stream timeout.  The result equals
+ * cpbus_stream_fanout(st, n, now_ns) with the header's n and watermark: mailboxes, digests, ticks, step result, the slot's
+ * acknowledgement, published_by_code, cpbus_publish_counts and cpbus_debug_events.
+ * The host learns what the launches took lazily: every call that reads or changes the bus's host state (publish, send,
+ * advance, flush, sync, membership, timers, stats, drains, digests, debug events, publish counts, the other stream calls but
+ * _put) first waits for the last outstanding follower and folds in their records; the asynchronous tickets
+ * (cpbus_step_result_*, cpbus_digest_fold_begin/_end) do not.  At most 8 followers are outstanding; the 9th resolves first.
+ * A followed batch whose watermark lies behind this bus's clock, or steps further than 32/timers_per_sub periods of the
+ * fastest periodic timer, delivers nothing, fires no timer and is not acknowledged; every follower queued behind it does
+ * nothing, and cpbus_stream_status and every later stream call on this bus return CPBUS_EORDER (sticky, as
+ * CPBUS_ETIMEDOUT is for a batch that never arrives).  CPBUS_EINVAL: NULL, or a lossless bus (lossless consumers poll and
+ * run the admit / offer / agree round, which syncs once per round anyway). */
+int cpbus_stream_fanout_next(cpbus_stream_t* st);
 int cpbus_stream_status(cpbus_stream_t* st);                       /* CPBUS_OK or the sticky error */
 int cpbus_stream_set_timeout(cpbus_stream_t* st, uint32_t microseconds);   /* in-kernel wait bound; default 2 s */
 int cpbus_stream_close(cpbus_stream_t* st);                        /* importers close before the owner */
