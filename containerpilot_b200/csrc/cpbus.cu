@@ -131,10 +131,7 @@ struct cpbus {
   unsigned long long* d_ready_hdr = nullptr;   // device alias of h_ready_hdr
   uint32_t subs_per_warp = 0;             // 0 = auto
   uint32_t order_block = 0;               // mask order is built per block of this many consecutive subscribers (0 = one global order)
-  bool order_heavy_first = true;          // within a block: masks with more codes first (CPBUS_ORDER_HEAVY=0: plain mask order)
   bool pdl = true;                        // programmatic dependent launch of consecutive fan-outs
-  int h2d_spin_us = 30;                   // how long cpbus_flush waits on the host for the batch's H2D before inserting a stream wait
-  bool zero_copy = false;                 // fan-out pulls host-staged batches straight from pinned memory (experiment: CPBUS_ZERO_COPY=1)
   cudaEvent_t launched = nullptr;         // recorded after the latest fan-out (step results are read on the copy stream)
   int hints = -1;                         // -1 auto; bit0: control blocks / timer slots evict_last in L2
   static constexpr int kFoldSlots = 8;
@@ -142,15 +139,12 @@ struct cpbus {
   cudaEvent_t fold_done[kFoldSlots] = {};
   uint32_t fold_next = 0;
   static constexpr int kStage = 8;         // staging ring: the host may run several flushes ahead of the GPU
-  static constexpr int kEpoch = 4;         // a `consumed` event is recorded only after every kEpoch-th buffer, so that most
-                                           // consecutive fan-outs are adjacent in the stream (programmatic dependent launch)
   static constexpr int kDevSlots = 64, kDevEpoch = 16;
   cpbus_event* d_stage = nullptr;          // kDevSlots x batch_cap records: device side of the staging ring
   cudaEvent_t epoch_done[kDevSlots / kDevEpoch] = {};   // on the bus stream, after the last fan-out of each epoch of slots
   uint32_t dev_slot = 0;
   cpbus_event* h_batch[kStage] = {};       // pinned staging
   cudaEvent_t h2d_done[kStage] = {};       // on copy_stream: batch c has reached HBM
-  cudaEvent_t consumed[kStage] = {};       // on the bus stream: the fan-out that read d_batch[c] has finished
   cudaStream_t copy_stream = nullptr;      // H2D of batch i+1 overlaps the fan-out of batch i
   cudaStream_t result_stream = nullptr;    // D2H of step results: must not queue in front of the next batch's H2D
   // per-launch results written by the fan-out kernel itself (no extra kernel to read a step's result)
@@ -172,7 +166,6 @@ struct cpbus {
   uint32_t* d_order = nullptr;            // active subscribers sorted by code mask (ORDERED fan-out)
   uint32_t n_order = 0, n_filtered = 0;   // n_filtered: active subscribers whose mask is not CPBUS_MASK_ALL
   bool order_dirty = true;
-  int use_order = 1;                      // CPBUS_ORDER: 0 never, 1 when some subscriber is filtered (default), 2 also for all-ones masks (experiment)
   std::vector<size_t> oneshot_idx;        // armed one-shot timers (index into h_timers)
   std::vector<HostTimer> h_timers;        // N*K, allocated on first timer
   uint32_t n_next = 0, n_active = 0, n_timers = 0;
@@ -293,7 +286,7 @@ static void mask_order(const uint32_t* masks, const uint8_t* active, uint32_t n,
 int rebuild_order(cpbus* b) {
   std::vector<uint32_t> order;
   static_assert(sizeof(b->h_active[0]) == 1, "h_active is a byte vector");
-  mask_order(b->h_mask.data(), reinterpret_cast<const uint8_t*>(b->h_active.data()), b->n_next, b->R, b->order_block, b->order_heavy_first, order);
+  mask_order(b->h_mask.data(), reinterpret_cast<const uint8_t*>(b->h_active.data()), b->n_next, b->R, b->order_block, /*heavy_first=*/true, order);
   b->n_order = (uint32_t)order.size();
   if (b->n_order) {
     CK(cudaMemcpyAsync(b->d_order, order.data(), (size_t)b->n_order * 4, cudaMemcpyHostToDevice, b->stream));
@@ -381,7 +374,7 @@ int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, in
   const bool pairs_on = b->n_paired > 0 && b->d_pairs;
   p.pairs = pairs_on ? b->d_pairs : nullptr;
   size_t smem = fanout_smem_bytes(p.smem_cap) + (pairs_on ? kPairFilterBytes : 0);   // + the batch's {code, source} presence filter
-  if (!pairs_on && !p.timers_on && (b->use_order == 2 || (b->use_order == 1 && b->n_filtered > 0))) {
+  if (!pairs_on && !p.timers_on && b->n_filtered > 0) {
     if (b->order_dirty) { const int rc_order = rebuild_order(b); if (rc_order) return rc_order; }
     if (b->n_order) {
       const uint32_t scale = std::max(1u, (p.n_ev + 128u) / 256u);
@@ -414,12 +407,12 @@ int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, in
     grid = std::max(1u, (need + spw - 1) / spw);
     // The range's control blocks (and timer slots) are staged in shared memory stage_subs at a time, in what the batch
     // leaves of the shared memory at the residency that the batch plus the smallest round (one subscriber per warp)
-    // allows, at most CPBUS_CTAS_PER_SM CTAs per SM.  Staging can therefore cost a resident CTA only where the batch
+    // allows, at most kCtasPerSm CTAs per SM.  Staging can therefore cost a resident CTA only where the batch
     // leaves less than that smallest round.
     const size_t off = fanout_stage_off(p.smem_cap);
     const size_t per_sub = sizeof(SubCtl) + (p.timers_on ? (size_t)b->K * sizeof(DevTimer) : 0);
     const size_t min_round = (size_t)kWarpsPerCta * per_sub;
-    const size_t ctas = std::max<size_t>(1, std::min<size_t>(CPBUS_CTAS_PER_SM, b->smem_per_sm / (off + min_round + b->smem_reserved)));
+    const size_t ctas = std::max<size_t>(1, std::min<size_t>(kCtasPerSm, b->smem_per_sm / (off + min_round + b->smem_reserved)));
     const size_t room = std::min<size_t>(kFanoutMaxSmem, b->smem_per_sm / ctas - b->smem_reserved) - off;   // >= min_round
     p.stage_subs = std::max<uint32_t>(kWarpsPerCta, (uint32_t)std::min<size_t>((size_t)kWarpsPerCta * spw, room / per_sub) & ~7u);
     smem = off + p.stage_subs * per_sub;
@@ -511,17 +504,6 @@ int flush_staged(cpbus* b, uint64_t w) {
   if (n == 0 && w == b->last_watermark) return CPBUS_OK;
   const int c = b->cur;
   int rc;
-  if (b->zero_copy && !b->lossless) {
-    // Zero-copy ingest: the pinned staging buffer is mapped into the device address space; CTA 0 of the fan-out pulls the
-    // batch over PCIe in its prologue (the staged path) — no H2D op, no stream waits, consecutive fan-outs stay adjacent.
-    rc = launch_fanout(b, b->h_batch[c], n, w, /*staged=*/1);
-    if (rc) return rc;
-    if ((c & (cpbus::kEpoch - 1)) == cpbus::kEpoch - 1) CK(cudaEventRecord(b->consumed[c], b->stream));
-    b->n_staged = 0;
-    b->cur = (b->cur + 1) % cpbus::kStage;
-    CK(cudaEventSynchronize(b->consumed[b->cur | (cpbus::kEpoch - 1)]));   // the launch that read the buffer we are about to overwrite has finished
-    return CPBUS_OK;
-  }
   // Device staging is a long ring (kDevSlots batches): a slot is reused only kDevSlots flushes later, far beyond how far the
   // host can run ahead, so the H2D never has to wait for an old fan-out and lands within microseconds.  Reuse safety is a
   // host-side check once per epoch of kDevEpoch slots (almost always already satisfied).
@@ -531,7 +513,7 @@ int flush_staged(cpbus* b, uint64_t w) {
   if (n) {
     CK(cudaMemcpyAsync(d_dst, b->h_batch[c], (size_t)n * sizeof(cpbus_event), cudaMemcpyHostToDevice, b->copy_stream));
     CK(cudaEventRecord(b->h2d_done[c], b->copy_stream));
-    // Give the 8-16 KiB copy a few microseconds to land.  If it has, the bus stream needs no wait node, consecutive fan-outs
+    // Give the 8-16 KiB copy up to 30 us to land.  If it has, the bus stream needs no wait node, consecutive fan-outs
     // stay adjacent in the stream and the next launch's prologue overlaps this one's tail (programmatic dependent launch).
     bool landed = false;
     const auto t_spin = std::chrono::steady_clock::now();
@@ -539,7 +521,7 @@ int flush_staged(cpbus* b, uint64_t w) {
       const cudaError_t q = cudaEventQuery(b->h2d_done[c]);
       if (q == cudaSuccess) { landed = true; break; }
       if (q != cudaErrorNotReady) { CK(q); }
-    } while (std::chrono::steady_clock::now() - t_spin < std::chrono::microseconds(b->h2d_spin_us));
+    } while (std::chrono::steady_clock::now() - t_spin < std::chrono::microseconds(30));
     if (!landed) CK(cudaStreamWaitEvent(b->stream, b->h2d_done[c], 0));
   }
   bool ok = true;
@@ -688,14 +670,10 @@ int cpbus_create(const cpbus_config* cfg, cpbus_t** out) try {
   b->lossless = cfg->flags & CPBUS_CFG_LOSSLESS; b->use_digest = cfg->flags & CPBUS_CFG_DIGEST;
   b->room_lb = R;
   b->store = cfg->store_path == CPBUS_STORE_AUTO ? CPBUS_STORE_V8 : (int)cfg->store_path;
-  if (const char* e = getenv("CPBUS_H2D_SPIN_US")) b->h2d_spin_us = atoi(e);
-  if (const char* e = getenv("CPBUS_ORDER")) b->use_order = atoi(e);
   if (const char* e = getenv("CPBUS_PDL")) b->pdl = atoi(e) != 0;
-  if (const char* e = getenv("CPBUS_ZERO_COPY")) b->zero_copy = atoi(e) != 0;
   if (const char* e = getenv("CPBUS_HINTS")) b->hints = atoi(e);
   if (const char* e = getenv("CPBUS_SUBS_PER_WARP")) b->subs_per_warp = (uint32_t)atoi(e);   // tuning knob for experiments
   if (const char* e = getenv("CPBUS_ORDER_BLOCK")) b->order_block = (uint32_t)atoll(e);
-  if (const char* e = getenv("CPBUS_ORDER_HEAVY")) b->order_heavy_first = atoi(e) != 0;
   int rc = CPBUS_OK;
   auto fail = [&](int code) { cpbus_destroy(b); return code; };
   if (cfg->device >= 0) b->device = cfg->device;
@@ -733,7 +711,6 @@ int cpbus_create(const cpbus_config* cfg, cpbus_t** out) try {
   for (int i = 0; i < cpbus::kStage; i++) {
     if (cudaMallocHost((void**)&b->h_batch[i], (size_t)B * sizeof(cpbus_event)) != cudaSuccess) return fail(CPBUS_ENOMEM);
     if (cudaEventCreateWithFlags(&b->h2d_done[i], cudaEventDisableTiming) != cudaSuccess) return fail(CPBUS_ECUDA);
-    if (cudaEventCreateWithFlags(&b->consumed[i], cudaEventDisableTiming) != cudaSuccess) return fail(CPBUS_ECUDA);
   }
   ALLOC(b->d_batch_local, (size_t)B * sizeof(cpbus_event));
   if (b->lossless) ALLOC(b->d_admit_batch, (size_t)B * sizeof(cpbus_event));
@@ -793,7 +770,6 @@ int cpbus_destroy(cpbus_t* b) try {
   for (int i = 0; i < cpbus::kStage; i++) {
     if (b->h_batch[i]) cudaFreeHost(b->h_batch[i]);
     if (b->h2d_done[i]) cudaEventDestroy(b->h2d_done[i]);
-    if (b->consumed[i]) cudaEventDestroy(b->consumed[i]);
   }
   cudaFree(b->d_stage);
   for (int i = 0; i < cpbus::kDevSlots / cpbus::kDevEpoch; i++) if (b->epoch_done[i]) cudaEventDestroy(b->epoch_done[i]);

@@ -56,8 +56,6 @@
 
   const bool keep = p.hints & 1u;
   // (the evict_last policy is materialised at each use — one instruction — rather than held in two registers)
-  if (CPBUS_ORD_PF && ORDERED && pos + lane < min(pos + p.spw, p.n_order))   // mask order scatters the ids: lane l prefetches ITS mailbox's control block
-    asm volatile("prefetch.global.L2 [%0];" ::"l"(p.ctl + my_ids));
 
   // ---- per-batch descriptor: computed ONCE per launch by CTA 0, copied by everyone else ----
   // descriptor = [rhash | meta | Q | summary {present, has_unicast, hist[32]}]: 24*cap + 16 + 160 bytes, the same layout in
@@ -279,9 +277,9 @@
   // (2-way conflict on every record read); at a 16-byte stride they touch all
   // eight.  All 2n chunks are read into registers (n <= 1024: at most 8 per thread), barrier, then written to their
   // plane: two barriers and 8 shared-memory instructions per thread per CTA, against ~2000 record reads per thread.
-  // Not in the ORDERED build: its gathered reads do no better on planes than with the lane-swapped halves, and not with
-  // the bulk store path, which copies whole records out of shared memory.
-  constexpr bool PLANAR = CPBUS_PLANAR && STORE != CPBUS_STORE_BULK && !ORDERED;
+  // Not in the ORDERED build: its gathered reads do no better on planes, and not with the bulk store path, which copies
+  // whole records out of shared memory.
+  constexpr bool PLANAR = STORE != CPBUS_STORE_BULK && !ORDERED;
   const uint32_t hi_off = cap;                                         // in 16-byte units
   if (PLANAR && n) {
     uint4* sq = reinterpret_cast<uint4*>(s_batch);
@@ -327,106 +325,6 @@
     bulk_g2s_hint(const_cast<uint4*>(s_ctl4), p.ctl + first, rn * (uint32_t)sizeof(SubCtl), &s_sum->mbar_state, keep);
     if (tim_bytes) bulk_g2s_hint(const_cast<uint4*>(s_tim4), p.timers + (size_t)first * K, tim_bytes, &s_sum->mbar_state, keep);
   };
-  // ================= ORDERED build, no unicast in the batch: whole RUNS of equal masks at a time =================
-  // The warp's block is <= 32 consecutive positions of the mask order; lane l owns position pos + l for the whole block
-  // (its id is in my_ids, its control block in registers: ONE load instruction brings the block's control blocks in).
-  // A run of L mailboxes with the same mask word shares the filter pass AND the record reads: each gathered record is
-  // stored to all L rings back to back, so the index-list -> gather -> select chain is paid once per run, not per mailbox
-  bool runs_done = false;
-  if constexpr (ORDERED && !TIMERS && !PAIRS && CPBUS_ORD_RUNS) {
-    if (!s_dsum[1]) {   // CTA-uniform: no unicast record in this batch
-      runs_done = true;
-      const uint32_t present_r = s_dsum[0];
-      const uint32_t Rm_r = p.ring_cap - 1;
-      const uint4* s4r = reinterpret_cast<const uint4*>(s_batch);
-      const uint32_t swr = ((uint32_t)lane >> 2) & 1u;
-      uint16_t* my_idx = reinterpret_cast<uint16_t*>(s_tick + warp * max(32u, cap / 2u));
-      const uint32_t nb = pos < pos_end ? pos_end - pos : 0u;
-      const bool mine = (uint32_t)lane < nb;
-      uint4 ma = make_uint4(0, 0, 0, 0), mb = ma;
-      if (mine) ld_sector(p.ctl + my_ids, ma, mb, keep);
-      const uint32_t my_m = mine ? mb.z : 0u;
-      const uint64_t p32 = s_pow[32];
-      uint32_t j = 0;
-      while (j < nb) {
-        const uint32_t m = __shfl_sync(0xffffffffu, my_m, j);
-        if (!(m & kActiveBit)) { j++; continue; }
-        const uint32_t eq = __ballot_sync(0xffffffffu, mine && my_m == m) >> j;          // bit 0 = lane j itself
-        const uint32_t L = (eq == 0xffffffffu) ? 32u : (uint32_t)__ffs(~eq) - 1u;          // consecutive mailboxes with this mask word
-        const bool dense = (m & present_r) == present_r;
-        uint32_t k = n;
-        if (!dense) {   // pass 1: ballot 32 events at a time; matching lanes append their event index to the warp's scratch list
-          uint32_t base = 0;
-          const uint32_t nchunks = (n + 31) >> 5;
-          for (uint32_t c0 = 0; c0 < nchunks; c0 += 4) {
-            uint32_t cbit[4];
-#pragma unroll
-            for (uint32_t u = 0; u < 4; u++) {
-              const uint32_t i = (c0 + u) * 32 + lane;
-              cbit[u] = i < n ? s_meta[i].x : 0u;
-            }
-#pragma unroll
-            for (uint32_t u = 0; u < 4; u++) {
-              const bool match = (m & cbit[u]) != 0;
-              const uint32_t w = __ballot_sync(0xffffffffu, match);
-              if (match) my_idx[base + __popc(w & ((1u << lane) - 1u))] = (uint16_t)((c0 + u) * 32 + lane);
-              base += __popc(w);
-            }
-          }
-          k = base;
-          __syncwarp();
-        }
-        // pass 2: lane -> output slot; every record read once, stored to the L rings of the run
-        uint64_t acc = 0;
-        for (uint32_t o0 = 0; o0 < k; o0 += 64) {   // warp-uniform trip count (the shuffles below need every lane)
-          const uint32_t o = o0 + lane;
-          const bool v0 = o < k, v1 = o + 32 < k;
-          uint32_t i0 = o, i1 = o + 32;
-          if (!dense) { i0 = v0 ? my_idx[o] : 0u; i1 = v1 ? my_idx[o + 32] : 0u; }
-          uint4 a0, b0, a1, b1;
-          if (v0) lds_record<true, PLANAR>(s4r, i0, swr, a0, b0, hi_off);
-          if (v1) lds_record<true, PLANAR>(s4r, i1, swr, a1, b1, hi_off);
-          if (DIGEST && !dense) {
-            if (v0) acc = acc * p32 + s_rhash[i0];
-            if (v1) acc = acc * p32 + s_rhash[i1];
-          }
-#pragma unroll 2
-          for (uint32_t t = j; t < j + L; t++) {
-            const uint32_t tl = __shfl_sync(0xffffffffu, ma.x, t);                        // low word of the tail: all the ring index needs
-            const uint32_t id = __shfl_sync(0xffffffffu, my_ids, t);
-            cpbus_event* ring = p.ring + (size_t)id * p.ring_cap;
-            if (v0) st_v8(ring + ((tl + o) & Rm_r), a0, b0);
-            if (v1) st_v8(ring + ((tl + o + 32) & Rm_r), a1, b1);
-          }
-        }
-        uint64_t dsum = 0;
-        if (DIGEST && k) {
-          if (dense) dsum = s_q[n];
-          else {   // per-lane Horner in P^32, then one power per lane: lane l wrote outputs l, l+32, ...; its last one is o_last
-            const uint32_t cnt = k > (uint32_t)lane ? (k - lane + 31u) / 32u : 0u;
-            dsum = cnt ? acc * s_pow[k - 1 - (lane + 32u * (cnt - 1u))] : 0ull;
-            dsum = warp_sum64(dsum);
-          }
-        }
-        if (k && (uint32_t)lane >= j && (uint32_t)lane < j + L) {   // each lane of the run writes ITS mailbox's control block back
-          const uint64_t tail = ((uint64_t)ma.y << 32) | ma.x, dig = ((uint64_t)mb.y << 32) | mb.x;
-          const uint64_t nt = tail + k;
-          const uint64_t nd = DIGEST ? dig * s_pow[k] + dsum : dig;
-          st_sector(p.ctl + my_ids, make_uint4((uint32_t)nt, (uint32_t)(nt >> 32), ma.z, ma.w),
-                    make_uint4((uint32_t)nd, (uint32_t)(nd >> 32), mb.z, 0u), keep);
-          atomicAdd(&s_sum->acc_deliv, k);
-          if (DIGEST) {
-            const uint32_t f = (uint32_t)nd ^ (uint32_t)(nd >> 32);
-            atomicAdd(&s_sum->acc_dig_lo, f & 0xFFFFu);
-            atomicAdd(&s_sum->acc_dig_hi, f >> 16);
-          }
-        }
-        __syncwarp();   // my_idx is rewritten by the next run's pass 1
-        j += L;
-      }
-    }
-  }
-  if (runs_done) pos = pos_end;   // nothing left for the per-mailbox loop below
   uint4 ca = make_uint4(0, 0, 0, 0), cb = ca, ta = ca;
   if (ORDERED && pos < pos_end) ld_sector(p.ctl + s, ca, cb, keep);   // software pipeline, stage 0: first control block
   const uint32_t present = s_dsum[0];
@@ -612,7 +510,7 @@
       if (DIGEST) dsum = s_q[n];
     } else if (dense) {
       // ================= dense run with interleaved ticks: O(#ticks) bookkeeping =================
-      constexpr bool cold_early = CPBUS_COLD_EARLY && !STAGED;
+      constexpr bool cold_early = !STAGED;
       if (cold_early && TIMERS && tk_slot < nslots) {   // cold half of the timer slot {source_id, fired}: needed only for the tick records
         const uint4 cold = tim_half(1);                 // after the copy loop, but loaded HERE so that its DRAM round trip hides under the copy
         tk_src = cold.x; tk_fired = cold.y;
@@ -623,7 +521,6 @@
       // event i lands at i + #{ticks with pos <= i}.  Lane r keeps the r-th smallest tick position in a register, so per
       // 32-event chunk the count is two ballots and a bit mask — no shared-memory round trip in the copy loop (the my_tick[]
       // loads feeding these compares would otherwise stall it).
-#if CPBUS_TICKS_REG
       const uint32_t T = (uint32_t)lane < n_ticks ? my_tick[lane] : 0xFFFFFFFFu;
       // destination of event i = c0 + lane of the chunk starting at c0
       auto slot_of = [&](uint32_t c0) -> uint32_t {
@@ -641,31 +538,17 @@
         return out;
       };
       uint32_t c0 = 0;
-#if CPBUS_UNROLL2
 #pragma unroll 1
       for (; c0 + 64 <= n; c0 += 64) {   // two chunks per iteration: both records' shared-memory loads are in flight before the selects
         const uint32_t o0 = slot_of(c0), o1 = slot_of(c0 + 32);
         copy_record_pairs<PLANAR>(s4, hi_off, ring, (uint32_t)tail, Rm, c0 + lane, o0, true);
         copy_record_pairs<PLANAR>(s4, hi_off, ring, (uint32_t)tail, Rm, c0 + 32 + lane, o1, true);
       }
-#endif
 #pragma unroll 1
       for (; c0 < n; c0 += 32) {
         const uint32_t out = slot_of(c0);
         copy_record_pairs<PLANAR>(s4, hi_off, ring, (uint32_t)tail, Rm, c0 + lane, out, c0 + lane < n);
       }
-#else
-      // Tick positions are sorted, so the count is warp-uniform for a whole 32-event chunk unless a tick falls strictly inside it
-      uint32_t t_idx = 0;
-#pragma unroll 1
-      for (uint32_t c0 = 0; c0 < n; c0 += 32) {
-        while (t_idx < n_ticks && my_tick[t_idx] <= c0) t_idx++;
-        const uint32_t i = c0 + lane;
-        uint32_t out = i + t_idx;
-        for (uint32_t t = t_idx; t < n_ticks && my_tick[t] < c0 + 32; t++) out += (my_tick[t] <= i) ? 1u : 0u;
-        copy_record_pairs<PLANAR>(s4, hi_off, ring, (uint32_t)tail, Rm, i, out, i < n);
-      }
-#endif
       if (!cold_early && TIMERS && tk_slot < nslots) {
         const uint4 cold = tim_half(1);
         tk_src = cold.x; tk_fired = cold.y;

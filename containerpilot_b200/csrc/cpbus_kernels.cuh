@@ -24,39 +24,8 @@ constexpr int kWarpsPerCta = 8;
 constexpr int kThreads = kWarpsPerCta * 32;
 // Every variant of the fan-out kernel is held to 64 registers => 4 CTAs (32 warps) per SM.  ptxas (CUDA 12.9, sm_90a) spills
 // nothing in the plain (dense and timers, with or without digest) and ORDERED variants, and 40-76 bytes in the PAIRS
-// variants.  Occupancy is the biggest single lever (DESIGN.md §4.1); the macro exists for A/B builds.
-#ifndef CPBUS_CTAS_PER_SM
-#define CPBUS_CTAS_PER_SM 4
-#endif
-// A/B build switches (build variants with -D...=0/1 and time them on one GPU; the defaults are the chosen variants)
-#ifndef CPBUS_SWIZZLE
-#define CPBUS_SWIZZLE 2      // shared-memory record reads with lanes 4-7 of each quarter warp fetching their halves in swapped order:
-                             // 0 = never, 1 = every path, 2 = only gathered reads.  Only lds_record uses it, i.e. the per-lane
-                             // reads of the CPBUS_ORD_RUNS variant; every other path copies records with copy_record_pairs.
-                             // The swizzle removes the bank conflicts everywhere, but on the dense paths the two extra live
-                             // registers per record cost more than the conflicts do.
-#endif
-#ifndef CPBUS_TICKS_REG
-#define CPBUS_TICKS_REG 1    // dense+ticks copy loop: tick positions in registers (ballots) instead of shared-memory loads
-#endif
-#ifndef CPBUS_COLD_EARLY
-#define CPBUS_COLD_EARLY 1   // PAIRS build: cold half of the timer slot loaded before the copy loop instead of after it (the plain
-#endif                       // build reads it from its shared-memory staging)
-#ifndef CPBUS_UNROLL2
-#define CPBUS_UNROLL2 1      // dense+ticks loop: two 32-event chunks per iteration
-#endif
-#ifndef CPBUS_ORD_PF
-#define CPBUS_ORD_PF 0       // ORDERED build: prefetch.L2 of the whole block's control blocks once the ids are known
-#endif
-#ifndef CPBUS_PLANAR
-#define CPBUS_PLANAR 1       // the staged batch is re-laid in shared memory as two 16-byte planes (lo[i] = bytes 0-15 of record i, hi[i] =
-#endif                       // bytes 16-31) before the copy loops: a lane's two LDS.128 are then conflict-free on the dense paths with no
-                             // select and no extra register (the lane-swapped reads of CPBUS_SWIZZLE cost registers)
-#ifndef CPBUS_ORD_RUNS
-#define CPBUS_ORD_RUNS 0     // ORDERED build: process runs of equal masks as a unit (records read once, stored to every ring of the run).
-                             // Bit-exact, but off by default: the rings then receive 1-2 KiB per visit instead of one contiguous
-                             // multi-KiB append, which can cost more than the saved gathers.
-#endif
+// variants.  Occupancy is the biggest single lever (DESIGN.md §4.1).
+constexpr int kCtasPerSm = 4;
 constexpr uint32_t kActiveBit = 0x80000000u;   // mask word: subscriber is subscribed
 constexpr int kTimerHintShift = 24;            // mask word bits 24..27: #timer slots to look at
 constexpr uint32_t kPairBit = 0x10000000u;     // mask word bit 28: subscriber has a {code, source} pair table
@@ -312,21 +281,6 @@ __device__ __forceinline__ void st_half(void* dst, const uint4& a, bool hinted) 
     asm volatile("st.global.L2::cache_hint.v4.b32 [%0], {%1,%2,%3,%4}, %5;" ::"l"(dst), "r"(a.x), "r"(a.y), "r"(a.z), "r"(a.w), "l"(pol) : "memory");
   else st_v4(dst, a);
 }
-// One lane reads one staged 32-byte record as two 16-byte shared-memory loads.  At a 32-byte lane stride the eight lanes
-// of a quarter warp (one LDS.128 wavefront) touch only four distinct 16-byte bank groups: a 2-way conflict on every read.
-// Lanes 4-7 of each quarter therefore fetch their two halves in the opposite order: each wavefront then covers all 32
-// banks, and two selects per register put the halves back in place.  No re-layout of the TMA-staged batch is needed.
-template <bool GATHER = false, bool PL = false>
-__device__ __forceinline__ void lds_record(const uint4* s4, uint32_t i, uint32_t sw, uint4& a, uint4& b, uint32_t hi = 0) {
-  if (PL) { a = s4[i]; b = s4[hi + i]; return; }   // planar staging: plane lo at s4, plane hi at s4 + hi
-  if (CPBUS_SWIZZLE == 0 || (CPBUS_SWIZZLE == 2 && !GATHER)) {
-    a = s4[2 * i]; b = s4[2 * i + 1];
-    return;
-  }
-  const uint4 x = s4[2 * i + sw], y = s4[2 * i + (sw ^ 1u)];
-  a.x = sw ? y.x : x.x; a.y = sw ? y.y : x.y; a.z = sw ? y.z : x.z; a.w = sw ? y.w : x.w;
-  b.x = sw ? x.x : y.x; b.y = sw ? x.y : y.y; b.z = sw ? x.z : y.z; b.w = sw ? x.w : y.w;
-}
 // TMA 1-D bulk copies (SASS: UBLKCP)
 __device__ __forceinline__ void bulk_g2s(void* sdst, const void* gsrc, uint32_t bytes, uint64_t* mbar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
@@ -413,13 +367,13 @@ __host__ __device__ inline size_t fanout_stage_off(uint32_t cap) { return (fanou
 // The body is included twice, so that the existing kernels are compiled from exactly the code they always were (an
 // inlined device function in their place changes how ptxas allocates the PAIRS variants) and FOLLOW costs them nothing.
 template <int STORE, bool TIMERS, bool DIGEST, bool ORDERED, bool PAIRS = false>
-__global__ void __launch_bounds__(kThreads, CPBUS_CTAS_PER_SM) fanout_kernel(const FanoutParams p) {
+__global__ void __launch_bounds__(kThreads, kCtasPerSm) fanout_kernel(const FanoutParams p) {
   constexpr bool FOLLOW = false;
 #include "cpbus_fanout_body.cuh"
 }
 // Stream follower (cpbus_stream_fanout_next): the same fan-out, shape and watermark taken from the slot header
 template <int STORE, bool TIMERS, bool DIGEST, bool ORDERED, bool PAIRS = false>
-__global__ void __launch_bounds__(kThreads, CPBUS_CTAS_PER_SM) fanout_follow_kernel(const FanoutParams p) {
+__global__ void __launch_bounds__(kThreads, kCtasPerSm) fanout_follow_kernel(const FanoutParams p) {
   constexpr bool FOLLOW = true;
 #include "cpbus_fanout_body.cuh"
 }
