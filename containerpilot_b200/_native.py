@@ -94,6 +94,8 @@ SYMBOLS = {
     "cpbus_stream_agree": (C.c_int, [C.c_void_p, _P(C.c_size_t)]),
     "cpbus_stream_poll": (C.c_int, [C.c_void_p, _P(C.c_int), _P(C.c_size_t), _P(C.c_uint64)]),
     "cpbus_stream_fanout_next": (C.c_int, [C.c_void_p]),
+    "cpbus_stream_round_next": (C.c_int, [C.c_void_p]),
+    "cpbus_stream_progress": (C.c_int, [C.c_void_p, _P(C.c_uint64), _P(C.c_size_t), _P(C.c_uint64)]),
     "cpbus_stream_status": (C.c_int, [C.c_void_p]),
     "cpbus_stream_set_timeout": (C.c_int, [C.c_void_p, C.c_uint32]),
     "cpbus_stream_close": (C.c_int, [C.c_void_p]),

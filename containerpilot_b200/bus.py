@@ -222,6 +222,20 @@ class Bus:
         that reads or changes this bus's host state."""
         return self._lib.cpbus_stream_fanout_next(st)
 
+    def stream_round_next(self, st) -> int:
+        """lossless follower: enqueue one admission round (admit, offer, agree, fan out the agreed prefix) on the device for
+        this shard's current batch; returns at once.  Every shard must enqueue the same sequence of rounds."""
+        return self._lib.cpbus_stream_round_next(st)
+
+    def stream_progress(self, st) -> tuple[int, int, int, int]:
+        """resolve outstanding followers and rounds: (status, batches completely fanned out, records of the next batch
+        already delivered, rounds that moved nothing).  status is the sticky stream error (OK when none)."""
+        b, off, stalled = C.c_uint64(), C.c_size_t(), C.c_uint64()
+        rc = self._lib.cpbus_stream_progress(st, C.byref(b), C.byref(off), C.byref(stalled))
+        if rc not in (nat.OK, nat.EORDER, nat.ETIMEDOUT):
+            nat.check(rc, "cpbus_stream_progress")
+        return rc, b.value, off.value, stalled.value
+
     def stream_status(self, st) -> int:
         return self._lib.cpbus_stream_status(st)
 

@@ -109,8 +109,14 @@ struct cpbus {
   uint32_t stream_spin_us = 0;                // bound of the in-kernel wait for a stream batch (0 = 2 s)
   // follower launches (cpbus_stream_fanout_next): enqueued without the batch's shape, resolved lazily (follow_resolve)
   static constexpr int kFollowMax = 8;        // outstanding at most; the next one resolves first
-  struct FollowPending { cpbus_stream* st; unsigned long long launch_seq; int rec; };
+  // kind: a follower, a lossless round (cpbus_stream_round_next: rec indexes h_round) or a cpbus_consume_all issued
+  // behind outstanding rounds (no record: it resets the room bound in order)
+  enum FollowKind { kFollower, kRound, kConsumeAll };
+  struct FollowPending { cpbus_stream* st; unsigned long long launch_seq; int rec; FollowKind kind; };
   std::vector<FollowPending> follow_q;        // outstanding, in launch order
+  RoundRec* h_round = nullptr;                // pinned + mapped: kFollowMax records written by the round agree kernels
+  RoundRec* d_round_rec = nullptr;            // device alias of h_round
+  RoundDev* d_round = nullptr;                // lossless rounds: the device copy of the room bound and clock, round scratch
   FollowRec* h_follow = nullptr;              // pinned + mapped: kFollowMax records written by the lead CTAs
   FollowRec* d_follow = nullptr;              // device alias of h_follow
   unsigned long long* d_follow_clock = nullptr;   // 4 words: {watermark, launch ordinal} by launch parity
@@ -298,28 +304,67 @@ int rebuild_order(cpbus* b) {
 
 constexpr int kFanoutMaxSmem = 200 * 1024;
 
+enum { kLaunchPlain = 0, kLaunchFollow = 1, kLaunchRound = 2 };
+
 template <int STORE, bool TIMERS, bool DIGEST, bool ORDERED, bool PAIRS = false>
-int launch_fanout_t(cpbus* b, const FanoutParams& p, uint32_t grid, size_t smem, bool follow) {
-  static bool attr_done[2][64] = {};   // per instantiation AND per device: function attributes are per-device state
-  void (*kernel)(FanoutParams) = follow ? fanout_follow_kernel<STORE, TIMERS, DIGEST, ORDERED, PAIRS>
-                                        : fanout_kernel<STORE, TIMERS, DIGEST, ORDERED, PAIRS>;
+int launch_fanout_t(cpbus* b, const FanoutParams& p, uint32_t grid, size_t smem, int kind) {
+  static bool attr_done[3][64] = {};   // per instantiation AND per device: function attributes are per-device state
+  void (*kernel)(FanoutParams) = kind == kLaunchRound  ? fanout_round_kernel<STORE, TIMERS, DIGEST, ORDERED, PAIRS>
+                               : kind == kLaunchFollow ? fanout_follow_kernel<STORE, TIMERS, DIGEST, ORDERED, PAIRS>
+                                                       : fanout_kernel<STORE, TIMERS, DIGEST, ORDERED, PAIRS>;
   const int dev = b->device & 63;
-  if (!attr_done[follow][dev]) {
+  if (!attr_done[kind][dev]) {
     CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kFanoutMaxSmem));
-    attr_done[follow][dev] = true;
+    attr_done[kind][dev] = true;
   }
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = smem; cfg.stream = b->stream;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;   // PDL: the next fan-out's prologue overlaps this one's tail
   attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = b->pdl ? 1 : 0;
+  // (a round's fan-out reads what the agree kernel in front of it wrote: launched without PDL, see fanout_round_kernel)
+  cfg.attrs = attr; cfg.numAttrs = b->pdl && kind != kLaunchRound ? 1 : 0;
   CK(cudaLaunchKernelEx(&cfg, kernel, p));
   CK(cudaGetLastError());
   return CPBUS_OK;
 }
 
 uint64_t max_window(const cpbus* b);
+
+// Lossless rounds wait in the kernel: for the publisher's header (decide) and for the other shards' offers (agree).  With
+// CUDA's lazy module loading, the first launch of a kernel loads it, and a load may wait for the kernels already running on
+// the device — such as a round waiting for a batch that this very thread has yet to put, or for an offer that another shard
+// of this thread has yet to queue.  So every kernel a lossless bus may launch while its rounds wait is loaded up front, once
+// per device, when the bus is created.
+template <int ST>
+int preload_round_fanouts() {
+  void (*ks[])(FanoutParams) = {
+      fanout_round_kernel<ST, false, false, false>, fanout_round_kernel<ST, false, true, false>,
+      fanout_round_kernel<ST, true, false, false>, fanout_round_kernel<ST, true, true, false>,
+      fanout_round_kernel<ST, false, false, true>, fanout_round_kernel<ST, false, true, true>,
+      fanout_round_kernel<ST, true, false, false, true>, fanout_round_kernel<ST, true, true, false, true>};
+  for (auto k : ks) CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, kFanoutMaxSmem));
+  return CPBUS_OK;
+}
+
+int preload_round_kernels(cpbus* b) {
+  static bool done[64] = {};
+  static std::mutex mu;
+  std::lock_guard<std::mutex> g(mu);
+  if (done[b->device & 63]) return CPBUS_OK;
+  int rc;
+  if ((rc = preload_round_fanouts<CPBUS_STORE_V4>()) || (rc = preload_round_fanouts<CPBUS_STORE_V8>()) ||
+      (rc = preload_round_fanouts<CPBUS_STORE_BULK>()))
+    return rc;
+  cudaFuncAttributes a;
+  CK(cudaFuncGetAttributes(&a, stream_round_decide_kernel));
+  CK(cudaFuncGetAttributes(&a, stream_round_admit_kernel));
+  CK(cudaFuncGetAttributes(&a, stream_round_agree_kernel));
+  CK(cudaFuncGetAttributes(&a, consume_all_kernel));     // cpbus_consume_all queues behind waiting rounds
+  CK(cudaFuncGetAttributes(&a, digest_fold_kernel));     // as does cpbus_digest_fold_begin
+  done[b->device & 63] = true;
+  return CPBUS_OK;
+}
 
 // fan out `n` records at d_src with watermark w (all checks done by the caller)
 struct StreamArgs {   // stream mode (cpbus_stream_fanout_prefix): where this batch's header / ack words live
@@ -328,6 +373,7 @@ struct StreamArgs {   // stream mode (cpbus_stream_fanout_prefix): where this ba
   uint32_t off = 0; bool final = true;   // records delivered before this launch; whether it completes the batch
   FollowRec* follow_rec = nullptr;       // follower launch (cpbus_stream_fanout_next): n and the watermark come from the header
   bool follow_from_host = false;         // ... and the previous watermark is the host clock rather than the clock words
+  const RoundDev* round = nullptr;       // lossless round (cpbus_stream_round_next): m, the watermark and the source from the agree kernel
 };
 
 int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, int staged = 0,
@@ -348,7 +394,9 @@ int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, in
     p.stream_hdr = sa->hdr; p.stream_ack = sa->ack; p.stream_seq = sa->seq; p.stream_next_hdr = sa->next_hdr;
     p.stream_off = sa->off; p.stream_final = sa->final ? 1u : 0u;
   }
-  const bool follow = sa && sa->follow_rec;
+  const bool follow = sa && sa->follow_rec, round = sa && sa->round;
+  const int kind = round ? kLaunchRound : follow ? kLaunchFollow : kLaunchPlain;
+  p.round = round ? sa->round : nullptr;
   if (follow) {   // n = batch_cap sizes the launch; the kernel takes the batch's own n and watermark from the header
     p.follow_clock = b->d_follow_clock; p.follow_rec = sa->follow_rec; p.follow_window = max_window(b);
     p.follow_from_host = sa->follow_from_host ? 1u : 0u;
@@ -420,14 +468,14 @@ int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, in
   const int variant = pairs_on ? (p.use_digest ? 7 : 6) : (p.timers_on ? 2 : 0) | (p.use_digest ? 1 : 0) | (p.order ? 4 : 0);
 #define CPBUS_DISPATCH(ST)                                                                \
   switch (variant) {                                                                     \
-    case 0: rc = launch_fanout_t<ST, false, false, false>(b, p, grid, smem, follow); break;      \
-    case 1: rc = launch_fanout_t<ST, false, true, false>(b, p, grid, smem, follow); break;       \
-    case 2: rc = launch_fanout_t<ST, true, false, false>(b, p, grid, smem, follow); break;       \
-    case 3: rc = launch_fanout_t<ST, true, true, false>(b, p, grid, smem, follow); break;        \
-    case 4: rc = launch_fanout_t<ST, false, false, true>(b, p, grid, smem, follow); break;       \
-    case 5: rc = launch_fanout_t<ST, false, true, true>(b, p, grid, smem, follow); break;        \
-    case 6: rc = launch_fanout_t<ST, true, false, false, true>(b, p, grid, smem, follow); break; \
-    default: rc = launch_fanout_t<ST, true, true, false, true>(b, p, grid, smem, follow); break; \
+    case 0: rc = launch_fanout_t<ST, false, false, false>(b, p, grid, smem, kind); break;      \
+    case 1: rc = launch_fanout_t<ST, false, true, false>(b, p, grid, smem, kind); break;       \
+    case 2: rc = launch_fanout_t<ST, true, false, false>(b, p, grid, smem, kind); break;       \
+    case 3: rc = launch_fanout_t<ST, true, true, false>(b, p, grid, smem, kind); break;        \
+    case 4: rc = launch_fanout_t<ST, false, false, true>(b, p, grid, smem, kind); break;       \
+    case 5: rc = launch_fanout_t<ST, false, true, true>(b, p, grid, smem, kind); break;        \
+    case 6: rc = launch_fanout_t<ST, true, false, false, true>(b, p, grid, smem, kind); break; \
+    default: rc = launch_fanout_t<ST, true, true, false, true>(b, p, grid, smem, kind); break; \
   }
   switch (b->store) {
     case CPBUS_STORE_V4: CPBUS_DISPATCH(CPBUS_STORE_V4); break;
@@ -436,7 +484,9 @@ int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, in
   }
 #undef CPBUS_DISPATCH
   if (rc) return rc;
-  b->st.batches++; b->st.kernel_launches++;
+  b->st.kernel_launches++;
+  if (round) return CPBUS_OK;    // batches, clock and debug-ring marker: when the round is resolved, if it delivered
+  b->st.batches++;
   if (follow) return CPBUS_OK;   // clock and debug-ring marker: when the launch is resolved (follow_resolve)
   b->last_watermark = w;
   if (account && n) dbg_mark_device_batch(b, p.launch_seq);
@@ -447,12 +497,7 @@ int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, in
 // Fast path: true when n records with watermark w provably fit (or nothing has to be admitted) — no kernel, no sync.
 bool admit_fits(cpbus* b, uint32_t n, uint64_t w) {
   if (!b->lossless || b->n_next == 0) return true;
-  // the most this launch can append to ONE mailbox: every event of the batch + every firing of its timer slots in the window
-  uint64_t need = n;
-  if (b->n_timers && b->K) {
-    const uint64_t per_slot = (b->min_period != UINT64_MAX && w > b->last_watermark) ? (w - b->last_watermark) / b->min_period + 2 : 2;
-    need += (uint64_t)b->K * per_slot;
-  }
+  const uint64_t need = admit_need(n, w, b->last_watermark, b->min_period, b->K, b->n_timers && b->K);
   if (b->room_lb >= need) { b->room_lb -= need; b->st.admit_skipped++; return true; }
   return false;
 }
@@ -570,6 +615,13 @@ int stage_one(cpbus* b, uint32_t code, uint32_t source_id, uint32_t target, uint
 bool is_pow2(uint32_t x) { return x && !(x & (x - 1)); }
 
 }  // namespace
+
+// outstanding followers and rounds that hold one of the kFollowMax records
+static int follow_records(const cpbus* b) {
+  int n = 0;
+  for (const cpbus::FollowPending& f : b->follow_q) n += f.kind != cpbus::kConsumeAll ? 1 : 0;
+  return n;
+}
 
 extern "C" {
 static int follow_resolve(cpbus* b);
@@ -713,7 +765,18 @@ int cpbus_create(const cpbus_config* cfg, cpbus_t** out) try {
     if (cudaEventCreateWithFlags(&b->h2d_done[i], cudaEventDisableTiming) != cudaSuccess) return fail(CPBUS_ECUDA);
   }
   ALLOC(b->d_batch_local, (size_t)B * sizeof(cpbus_event));
-  if (b->lossless) ALLOC(b->d_admit_batch, (size_t)B * sizeof(cpbus_event));
+  if (b->lossless) {
+    ALLOC(b->d_admit_batch, (size_t)B * sizeof(cpbus_event));
+    // lossless rounds (cpbus_stream_round_next): device state and the host records, allocated here rather than by the
+    // first round, while no round of any shard can be waiting on the device
+    ALLOC(b->d_round, sizeof(RoundDev));
+    RoundDev init{};
+    init.room_full = R;
+    if (cudaMemcpyAsync(b->d_round, &init, sizeof(init), cudaMemcpyHostToDevice, b->stream) != cudaSuccess) return fail(CPBUS_ECUDA);
+    if (cudaHostAlloc((void**)&b->h_round, sizeof(RoundRec) * cpbus::kFollowMax, cudaHostAllocMapped) != cudaSuccess) return fail(CPBUS_ENOMEM);
+    if (cudaHostGetDevicePointer((void**)&b->d_round_rec, b->h_round, 0) != cudaSuccess) return fail(CPBUS_ECUDA);
+    if ((rc = preload_round_kernels(b))) return fail(rc);
+  }
   ALLOC(b->d_pf_buf, (size_t)kStreamPrefetch * B * sizeof(cpbus_event)); ALLOC(b->d_pf_state, 64);
   ALLOC(b->d_acct, sizeof(DevPubAcct));
   if (cudaMemsetAsync(b->d_pf_state, 0, 64, b->stream) != cudaSuccess ||
@@ -762,6 +825,8 @@ int cpbus_destroy(cpbus_t* b) try {
   while (!b->streams.empty()) cpbus_stream_close(b->streams.back());
   if (b->h_follow) cudaFreeHost(b->h_follow);
   cudaFree(b->d_follow_clock);
+  if (b->h_round) cudaFreeHost(b->h_round);
+  cudaFree(b->d_round);
   if (b->follow_done) cudaEventDestroy(b->follow_done);
   cudaFree(b->d_ring); cudaFree(b->d_ctl); cudaFree(b->d_order); cudaFree(b->d_pairs);
   cudaFree(b->d_timers); cudaFree(b->d_stats); cudaFree(b->d_fold); cudaFree(b->d_pow); cudaFree(b->d_desc); cudaFree(b->d_desc_ready);
@@ -1325,6 +1390,8 @@ struct cpbus_stream {
   uint32_t get_off = 0;                      // lossless mode: records of batch get_seq + 1 already delivered
   uint32_t follow_out = 0;                   // follower launches of batches get_seq + 1 .. not yet resolved
   unsigned long long seen_seq = 0;           // highest batch whose release this consumer has seen from the host
+  RoundCursor* d_cursor = nullptr;           // lossless rounds (cpbus_stream_round_next): {batch, offset} on the device
+  unsigned long long stalled_rounds = 0;     // ... rounds resolved so far that moved nothing
   unsigned long long pub_seq = 0;            // publisher: publish ordinal stamped into the next record (CPBUS_PUT_STAMP)
   unsigned long long min_ack = 0;            // publisher: cached min over the consumers' acks
   // publisher staging: pinned payload + header buffers, copies on their own stream
@@ -1348,6 +1415,10 @@ static int stream_bind(cpbus_stream* st) {
   st->hdr = reinterpret_cast<StreamHdr*>(st->base + stream_hdr_off());
   st->ack = reinterpret_cast<unsigned long long*>(st->base + stream_ack_off(st->n_slots));
   st->payload = reinterpret_cast<cpbus_event*>(st->base + stream_payload_off(st->n_slots));
+  if (st->bus->lossless && cudaMalloc((void**)&st->d_cursor, sizeof(RoundCursor)) != cudaSuccess) {   // rounds' cursor
+    snprintf(g_cuda_err, sizeof(g_cuda_err), "cudaMalloc(%zu) failed", sizeof(RoundCursor));
+    return CPBUS_ENOMEM;
+  }
   return CPBUS_OK;
 }
 
@@ -1369,7 +1440,7 @@ int cpbus_stream_create(cpbus_t* b, uint32_t n_slots, uint32_t n_consumers, cpbu
   cudaIpcMemHandle_t h;
   if (cudaIpcGetMemHandle(&h, st->base) != cudaSuccess) { snprintf(g_cuda_err, sizeof(g_cuda_err), "cudaIpcGetMemHandle failed"); return fail(CPBUS_ECUDA); }
   memcpy(handle, &h, 64);
-  stream_bind(st);
+  if ((rc = stream_bind(st))) return fail(rc);
   if (cudaStreamCreateWithFlags(&st->put_stream, cudaStreamNonBlocking) != cudaSuccess) return fail(CPBUS_ECUDA);
   for (int i = 0; i < cpbus_stream::kStage; i++) {
     if (cudaMallocHost((void**)&st->h_stage[i], (size_t)b->B * sizeof(cpbus_event)) != cudaSuccess) return fail(CPBUS_ENOMEM);
@@ -1400,7 +1471,7 @@ int cpbus_stream_open(cpbus_t* b, const unsigned char handle[64], uint32_t consu
     return e != cudaSuccess ? CPBUS_ECUDA : CPBUS_EINVAL;
   }
   st->n_slots = meta.n_slots; st->n_consumers = meta.n_consumers; st->B = meta.batch_cap;
-  stream_bind(st);
+  if ((rc = stream_bind(st))) { cudaIpcCloseMemHandle(st->base); delete st; return rc; }
   b->streams.push_back(st);
   *out = st;
   return CPBUS_OK;
@@ -1425,7 +1496,7 @@ int cpbus_stream_attach(cpbus_t* b, cpbus_stream_t* owner, uint32_t consumer_ind
   if (!st) return CPBUS_ENOMEM;
   st->bus = b; st->attached = true; st->consumer = consumer_index;
   st->n_slots = owner->n_slots; st->n_consumers = owner->n_consumers; st->B = owner->B; st->base = owner->base;
-  stream_bind(st);
+  if ((rc = stream_bind(st))) { delete st; return rc; }
   b->streams.push_back(st);
   *out = st;
   return CPBUS_OK;
@@ -1446,6 +1517,7 @@ int cpbus_stream_close(cpbus_stream_t* st) try {
   if (st->h_ack) cudaFreeHost(st->h_ack);
   if (st->h_agree) cudaFreeHost(st->h_agree);
   if (st->agree_done) cudaEventDestroy(st->agree_done);
+  cudaFree(st->d_cursor);
   if (st->base) { if (st->owner) cudaFree(st->base); else if (!st->attached) cudaIpcCloseMemHandle(st->base); }
   b->streams.erase(std::remove(b->streams.begin(), b->streams.end(), st), b->streams.end());
   delete st;
@@ -1644,9 +1716,30 @@ int cpbus_stream_fanout(cpbus_stream_t* st, size_t n, uint64_t now_ns) try {
   return stream_fanout_prefix(st, n, now_ns, n - st->get_off);
 } CPBUS_CATCH
 
-// Outstanding follower launches: one wait on the last of them, then their records in launch order.  A launch that delivered
-// moves the stream, the clock and the publish ordinals exactly as cpbus_stream_fanout with the header's shape does; an
-// aborted one (and every follower behind it, each a no-op) changes nothing but the sticky error word.
+// Outstanding follower launches and lossless rounds: one wait on the last of them, then their records in launch order.  A
+// launch that delivered moves the stream, the clock and the publish ordinals exactly as cpbus_stream_fanout with the
+// header's shape does; an aborted one (and every follower behind it, each a no-op) changes nothing but the sticky error
+// word.  A round moves the host state as the host-driven round with the same outcome (cpbus_stream_admit, _offer, _agree,
+// then _fanout_prefix of the agreed prefix) would have moved it.
+static void round_fold(cpbus* b, const cpbus::FollowPending& f) {
+  const volatile RoundRec* r = &b->h_round[f.rec];
+  cpbus_stream* st = f.st;
+  const uint32_t status = r->status;
+  if (status == kFollowAborted || status == kFollowSkipped) return;
+  if (r->admit == kRoundAdmitPass) b->st.admit_passes++;
+  else if (r->admit == kRoundAdmitSkipped) b->st.admit_skipped++;
+  b->room_lb = r->room;
+  if (status == kRoundStalled) { st->stalled_rounds++; return; }
+  const uint32_t m = r->m;
+  const uint64_t w = r->watermark;
+  b->st.batches++;
+  b->st.publishes += m; b->seq += m;
+  b->now = w; b->last_watermark = w;
+  if (m) dbg_mark_device_batch(b, f.launch_seq);
+  if (status == kFollowDelivered) { st->get_seq++; st->get_off = 0; }
+  else { st->get_off += m; b->st.admit_partial++; }
+}
+
 static int follow_resolve(cpbus* b) {
   std::lock_guard<std::recursive_mutex> g(b->follow_mu);
   if (b->follow_q.empty()) return CPBUS_OK;
@@ -1657,8 +1750,14 @@ static int follow_resolve(cpbus* b) {
   q.swap(b->follow_q);
   bool missing = false;
   for (const cpbus::FollowPending& f : q) {
-    const volatile FollowRec* r = &b->h_follow[f.rec];
+    if (f.kind == cpbus::kConsumeAll) { b->room_lb = b->R; continue; }
     f.st->follow_out--;
+    if (f.kind == cpbus::kRound) {
+      if (b->h_round[f.rec].status == kFollowPending) missing = true;
+      else round_fold(b, f);
+      continue;
+    }
+    const volatile FollowRec* r = &b->h_follow[f.rec];
     if (r->status == kFollowPending) missing = true;
     if (r->status != kFollowDelivered) continue;
     const uint32_t n = r->n;
@@ -1668,7 +1767,7 @@ static int follow_resolve(cpbus* b) {
     b->now = w; b->last_watermark = w;
     if (n) dbg_mark_device_batch(b, f.launch_seq);
   }
-  if (missing) { snprintf(g_cuda_err, sizeof(g_cuda_err), "a follower launch completed without its record"); return CPBUS_ECUDA; }
+  if (missing) { snprintf(g_cuda_err, sizeof(g_cuda_err), "a follower launch or round completed without its record"); return CPBUS_ECUDA; }
   return CPBUS_OK;
 }
 
@@ -1680,7 +1779,7 @@ int cpbus_stream_fanout_next(cpbus_stream_t* st) try {
   if (b->lossless) return CPBUS_EINVAL;   // lossless followers agree on every round, which syncs anyway
   std::lock_guard<std::recursive_mutex> g(b->follow_mu);
   int rc = dev_guard(b); if (rc) return rc;
-  if (b->follow_q.size() >= (size_t)cpbus::kFollowMax && (rc = follow_resolve(b))) return rc;
+  if (follow_records(b) >= cpbus::kFollowMax && (rc = follow_resolve(b))) return rc;
   if ((rc = stream_error(b))) return rc;
   if (!b->h_follow) {
     FollowRec *h = nullptr, *d = nullptr;
@@ -1710,9 +1809,71 @@ int cpbus_stream_fanout_next(cpbus_stream_t* st) try {
                      /*batch_dep=*/false, /*account=*/true, &sa);
   if (rc) return rc;
   b->follow_next = (ri + 1) % cpbus::kFollowMax;
-  b->follow_q.push_back(cpbus::FollowPending{st, b->launch_seq, ri});
+  b->follow_q.push_back(cpbus::FollowPending{st, b->launch_seq, ri, cpbus::kFollower});
   st->follow_out++;
   return CPBUS_OK;
+} CPBUS_CATCH
+
+// Lossless stream, one admission round enqueued on the device: decide (one CTA), the exact admission pass (grid; every
+// CTA returns at once on the fast path), offer + agree (one CTA), the fan-out of the agreed prefix.  The host learns the
+// outcome when it next resolves (follow_resolve), like a follower's.
+int cpbus_stream_round_next(cpbus_stream_t* st) try {
+  if (!st) return CPBUS_EINVAL;
+  cpbus* b = st->bus;
+  if (!b->lossless || st->offered) return CPBUS_EINVAL;   // throughput mode needs no agreement; not inside an explicit round
+  std::lock_guard<std::recursive_mutex> g(b->follow_mu);
+  int rc = dev_guard(b); if (rc) return rc;
+  if (follow_records(b) >= cpbus::kFollowMax && (rc = follow_resolve(b))) return rc;
+  if ((rc = stream_error(b))) return rc;
+  if (!b->follow_done) CK(cudaEventCreateWithFlags(&b->follow_done, cudaEventDisableTiming));
+  // The first round after the host has resolved takes the bus state from the host (this bus's own staged events go out
+  // first, as in cpbus_stream_admit); the ones queued behind it use the device copy.  Likewise the stream's cursor.
+  const bool seed_bus = b->follow_q.empty(), seed_cur = st->follow_out == 0;
+  if (seed_bus && (rc = flush_staged(b, b->now))) return rc;
+  const int ri = b->follow_next;
+  b->h_round[ri].status = kFollowPending;
+  RoundParams P{};
+  P.dev = b->d_round; P.cur = st->d_cursor; P.rec = b->d_round_rec + ri;
+  P.hdr = st->hdr; P.payload = st->payload; P.ack = st->ack;
+  P.n_slots = st->n_slots; P.B = st->B; P.consumer = st->consumer; P.n_consumers = st->n_consumers;
+  P.round = st->agree_round + 1;
+  P.spin_us = b->stream_spin_us; P.err_word = b->d_err;
+  P.admit_batch = b->d_admit_batch; P.ctl = b->d_ctl; P.timers = b->d_timers; P.stats = b->d_stats;
+  P.pairs = b->n_paired > 0 ? b->d_pairs : nullptr;
+  P.n_subs = b->n_next; P.ring_cap = b->R; P.K = b->K; P.sub_base = b->cfg.sub_id_base;
+  P.timers_armed = b->n_timers > 0 && b->K > 0;
+  P.min_period = b->min_period; P.window = max_window(b);
+  P.seed_bus = seed_bus; P.seed_room = b->room_lb; P.seed_now = b->now; P.seed_wm = b->last_watermark;
+  P.seed_cur = seed_cur; P.seed_batch = st->get_seq + 1; P.seed_off = st->get_off;
+  stream_round_decide_kernel<<<1, kThreads, 0, b->stream>>>(P);
+  CK(cudaGetLastError());
+  b->st.kernel_launches++;
+  if (b->n_next) {
+    stream_round_admit_kernel<<<(b->n_next + 255) / 256, 256, 0, b->stream>>>(P);
+    CK(cudaGetLastError());
+    b->st.kernel_launches++;
+  }
+  stream_round_agree_kernel<<<1, kStreamMaxConsumers, 0, b->stream>>>(P);
+  CK(cudaGetLastError());
+  b->st.kernel_launches++;
+  st->agree_round = P.round;
+  StreamArgs sa;
+  sa.ack = &st->ack[4 * st->consumer]; sa.round = b->d_round;
+  rc = launch_fanout(b, st->payload, b->B, b->now, /*staged=*/2, nullptr, nullptr, 0, /*batch_dep=*/false, /*account=*/true, &sa);
+  // (a failed launch leaves the round's record pending: the next resolution reports it)
+  b->follow_next = (ri + 1) % cpbus::kFollowMax;
+  b->follow_q.push_back(cpbus::FollowPending{st, b->launch_seq, ri, cpbus::kRound});
+  st->follow_out++;
+  return rc;
+} CPBUS_CATCH
+
+int cpbus_stream_progress(cpbus_stream_t* st, uint64_t* batches, size_t* offset, uint64_t* stalled_rounds) try {
+  if (!st || !batches || !offset || !stalled_rounds) return CPBUS_EINVAL;
+  cpbus* b = st->bus;
+  int rc = dev_guard(b); if (rc) return rc;
+  if ((rc = follow_resolve(b))) return rc;
+  *batches = st->get_seq; *offset = st->get_off; *stalled_rounds = st->stalled_rounds;
+  return stream_error(b);
 } CPBUS_CATCH
 
 // Lossless stream across processes, step 1 of the exchange: post this shard's admitted prefix for the current round.
@@ -1906,12 +2067,20 @@ int cpbus_consume_all(cpbus_t* b) try {
   if (!b) return CPBUS_EINVAL;
   std::lock_guard<std::mutex> g(b->mu);
   int rc = dev_guard(b); if (rc) return rc;
-  if ((rc = follow_resolve(b))) return rc;
+  std::lock_guard<std::recursive_mutex> gf(b->follow_mu);
+  // Behind outstanding lossless rounds (the only thing a lossless bus queues) it does not wait: it is ordered behind them
+  // on the bus stream, resets the device room bound there, and joins the queue so that resolution resets the host's in order.
+  const bool behind_rounds = b->lossless && !b->follow_q.empty();
+  if (!behind_rounds && (rc = follow_resolve(b))) return rc;
   if (b->n_next) {
     const uint32_t threads = 256, grid = std::min<uint32_t>((b->n_next + threads - 1) / threads, (uint32_t)b->sm_count * 8);
     consume_all_kernel<<<grid, threads, 0, b->stream>>>(b->d_ctl, b->n_next);
     CK(cudaGetLastError());
     b->st.kernel_launches++;
+  }
+  if (behind_rounds) {
+    CK(cudaMemcpyAsync(&b->d_round->room, &b->d_round->room_full, sizeof(unsigned long long), cudaMemcpyDeviceToDevice, b->stream));
+    b->follow_q.push_back(cpbus::FollowPending{nullptr, 0ull, -1, cpbus::kConsumeAll});
   }
   b->room_lb = b->R;   // stream-ordered behind every earlier fan-out: from here on every mailbox is empty
   return CPBUS_OK;

@@ -1,5 +1,5 @@
-// Body of fanout_kernel and fanout_follow_kernel (cpbus_kernels.cuh includes it inside both, with FOLLOW = false / true).
-// Not a standalone header.
+// Body of fanout_kernel, fanout_follow_kernel and fanout_round_kernel (cpbus_kernels.cuh includes it inside each, with
+// FOLLOW / ROUND = false / false, true / false and true / true).  Not a standalone header.
   constexpr bool STAGED = !ORDERED && !PAIRS;
   extern __shared__ __align__(128) unsigned char smem[];
   const uint32_t cap = p.smem_cap;
@@ -18,6 +18,7 @@
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   uint32_t n = FOLLOW ? 0u : p.n_ev;   // FOLLOW: set from the descriptor summary (word kFollowN) once it is in
   uint64_t w_follow = 0;               // FOLLOW: the batch's watermark, in place of p.w_now
+  unsigned long long round_ack = 0;    // ROUND, lead thread 0: the batch this launch completes (0: partial, no acknowledgement)
 
   // ---- stage the batch: one elected thread drives the TMA engine ----
   // Programmatic dependent launch: this kernel may begin while the previous fan-out is still draining its last wave.
@@ -104,7 +105,20 @@
   if (own_desc) {
     if (lead && tid < kResultSub * 4) reinterpret_cast<unsigned long long*>(p.result_next)[tid] = 0ull;   // next launch's result slot
     if (tid < 40) s_dsum[tid] = 0;
-    if constexpr (FOLLOW) {
+    if constexpr (ROUND) {
+      __syncthreads();   // thread 0 writes the shape into the summary below
+      // The shape the shards agreed on, written by this shard's agree kernel (complete before this launch started: no PDL)
+      if (tid == 0) {
+        const volatile RoundDev* rd = p.round;
+        if (!rd->go) s_sum->abort_launch = 1u;
+        else {
+          const unsigned long long w = rd->w;
+          s_dsum[kFollowN] = rd->m; s_dsum[kFollowWLo] = (uint32_t)w; s_dsum[kFollowWHi] = (uint32_t)(w >> 32);
+          s_dsum[kRoundSrc] = rd->src;
+          if (lead && rd->final) round_ack = rd->q;
+        }
+      }
+    } else if constexpr (FOLLOW) {
       __syncthreads();   // thread 0 writes the shape into the summary below
       // The clock: the host's, or the watermark the previous follower launch wrote (its lead did so before that launch let
       // this one start: acquired with its launch ordinal, bounded like the header).  Then the slot header, as below.
@@ -192,7 +206,7 @@
       w_follow = ((uint64_t)s_dsum[kFollowWHi] << 32) | s_dsum[kFollowWLo];
     }
     if (staged && n && !ab) {   // peer pull: plain 16-byte loads on the NVLink-mapped pointer, into shared memory and the local copy
-      const uint4* src = reinterpret_cast<const uint4*>(FOLLOW ? batch_src : p.batch);
+      const uint4* src = reinterpret_cast<const uint4*>(ROUND ? p.batch + s_dsum[kRoundSrc] : FOLLOW ? batch_src : p.batch);
       uint4* loc = reinterpret_cast<uint4*>(p.batch_local);
       uint4* dst = reinterpret_cast<uint4*>(s_batch);
       for (uint32_t i = tid; i < 2 * n; i += kThreads) {
@@ -204,8 +218,8 @@
     }
     mbar_wait(&s_sum->mbar, 0);
     __syncthreads();
-    if (lead && stream && tid == 0 && !ab && p.stream_final)   // the batch is out of the shared ring: the publisher may reuse the slot
-      asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(p.stream_ack), "l"(p.stream_seq) : "memory");
+    if (lead && stream && tid == 0 && !ab && (ROUND ? round_ack != 0 : p.stream_final))   // the batch is out of the shared ring: the publisher may reuse the slot
+      asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(p.stream_ack), "l"(ROUND ? round_ack : p.stream_seq) : "memory");
     const uint32_t nd = ab ? 0u : n;
     {
       uint32_t present = 0, uni = 0;

@@ -140,6 +140,59 @@ __host__ __device__ inline unsigned long long stream_offer_word(unsigned long lo
 // agree kernel -> host (pinned, mapped): the agreed prefix, the OR of the stall bits, 0 / kErrStreamTimeout
 struct __align__(16) StreamAgreeResult { uint32_t m, stalled, status, pad; };
 
+// Lossless admission fast path (host cpbus_stream_admit / cpbus_flush and the device round alike): the most one launch of
+// n records with watermark w can append to ONE mailbox — every record, plus every firing of its K timer slots in the window.
+__host__ __device__ inline uint64_t admit_need(uint64_t n, uint64_t w, uint64_t last_wm, uint64_t min_period, uint32_t K,
+                                              bool timers_armed) {
+  if (!timers_armed) return n;
+  const uint64_t per_slot = (min_period != ~0ull && w > last_wm) ? (w - last_wm) / min_period + 2 : 2;
+  return n + (uint64_t)K * per_slot;
+}
+
+// Lossless stream rounds on the device (cpbus_stream_round_next): decide (one CTA) -> exact admission pass (grid, exits at
+// once on the fast path) -> offer + agree (one CTA) -> fan-out of the agreed prefix (fanout_round_kernel).  Each kernel
+// hands the next one its result in RoundDev, on the bus stream; none of them is launched with programmatic dependent
+// launch, so each starts after its predecessor has completed and its writes are visible.
+// RoundDev: the device copy of the bus state the rounds move (authoritative while rounds are outstanding) and this round's
+// scratch.  RoundCursor: a stream's position, {batch, records of it already delivered}.
+struct __align__(16) RoundCursor { unsigned long long batch; uint32_t off, pad; };
+enum : uint32_t { kRoundOk = 0u, kRoundSkip = 1u, kRoundAbort = 2u };                 // RoundDev::status (decide)
+enum : uint32_t { kRoundAdmitNone = 0u, kRoundAdmitSkipped = 1u, kRoundAdmitPass = 2u };   // how the prefix was admitted
+struct __align__(32) RoundDev {
+  unsigned long long room;       // lower bound of the free slots of the fullest mailbox (cpbus::room_lb)
+  unsigned long long now, last_wm;   // the bus clock and the last launched watermark
+  unsigned long long poison;     // an earlier round aborted: every round queued behind it is a no-op
+  unsigned long long room_full;  // ring_cap: what cpbus_consume_all copies into `room`, ordered on the stream
+  // decide -> exact pass -> agree
+  unsigned long long q, hw;      // this round's batch ordinal and its header's watermark
+  uint32_t off, rem, status, admit;
+  // agree -> fan-out: deliver m records from payload index src with watermark w; final: acknowledge batch q
+  unsigned long long w;
+  uint32_t go, m, src, final;
+};
+// per-round record for the host (pinned, mapped), written by the agree kernel.  status: kFollowDelivered (the batch is
+// complete), kRoundPartial, kRoundStalled (nothing moved: some shard stalled, or the agreed prefix is 0), kFollowAborted,
+// kFollowSkipped (queued behind an aborted round)
+enum : uint32_t { kRoundPartial = 3u, kRoundStalled = 4u };
+struct __align__(32) RoundRec { uint32_t m, status; unsigned long long watermark, room; uint32_t admit, pad; };
+struct RoundParams {
+  RoundDev* dev; RoundCursor* cur; RoundRec* rec;
+  const StreamHdr* hdr; const cpbus_event* payload; unsigned long long* ack;   // the stream (peer pointers off the publisher)
+  uint32_t n_slots, B, consumer, n_consumers;
+  unsigned long long round;
+  uint32_t spin_us; unsigned int* err_word;
+  // admission
+  cpbus_event* admit_batch; const SubCtl* ctl; const DevTimer* timers; DevStats* stats; const uint2* pairs;
+  uint32_t n_subs, ring_cap, K, sub_base, timers_armed;
+  uint64_t min_period, window;
+  // the first round after the host resolved: the bus state and / or the cursor come from the host
+  uint32_t seed_bus, seed_cur;
+  unsigned long long seed_room, seed_now, seed_wm, seed_batch;
+  uint32_t seed_off;
+};
+// where the round fan-out's source index travels to the other CTAs: a spare word of the descriptor summary
+constexpr uint32_t kRoundSrc = 37;
+
 struct FanoutParams {
   const cpbus_event* batch;   // n_ev records, sorted by ts (HBM)
   cpbus_event* ring;          // [n_subs][R]
@@ -187,6 +240,8 @@ struct FanoutParams {
   FollowRec* follow_rec;             // host-mapped: what this launch took (written by the lead CTA)
   uint64_t follow_window;            // widest watermark step of one launch (UINT64_MAX: no periodic timer armed)
   uint32_t follow_from_host;         // 1: the previous watermark is w_now (the host clock), not the clock words
+  // ---- lossless round (fanout_round_kernel only): n, the watermark and the source come from the agree kernel ----
+  const RoundDev* round;
 };
 
 // ---------------------------------------------------------------- helpers ---
@@ -364,26 +419,38 @@ __host__ __device__ inline size_t fanout_stage_off(uint32_t cap) { return (fanou
 // FOLLOW (fanout_follow_kernel, stream mode only): the host does not know the batch's shape.  The lead CTA reads n and the
 // watermark from the slot header it acquires anyway, checks the watermark against the device clock (the previous follower's
 // watermark) and publishes both with the descriptor; the batch always travels through the lead's local copy.
-// The body is included twice, so that the existing kernels are compiled from exactly the code they always were (an
-// inlined device function in their place changes how ptxas allocates the PAIRS variants) and FOLLOW costs them nothing.
+// ROUND (fanout_round_kernel, lossless stream rounds only; FOLLOW is set too): the shape is what this shard's round agreed
+// on.  The lead CTA reads {m, watermark, source index, final} from RoundDev, which the agree kernel wrote earlier on the
+// same stream; the kernel is launched without programmatic dependent launch, so that read needs no griddepcontrol.wait.
+// A round that delivers nothing (a stall, a prefix of 0, an error) runs as an aborted launch: no record, no tick, no ack.
+// The body is included once per kernel, so that the existing kernels are compiled from exactly the code they always were
+// (an inlined device function in their place changes how ptxas allocates the PAIRS variants) and FOLLOW and ROUND cost
+// them nothing.
 template <int STORE, bool TIMERS, bool DIGEST, bool ORDERED, bool PAIRS = false>
 __global__ void __launch_bounds__(kThreads, kCtasPerSm) fanout_kernel(const FanoutParams p) {
-  constexpr bool FOLLOW = false;
+  constexpr bool FOLLOW = false, ROUND = false;
 #include "cpbus_fanout_body.cuh"
 }
 // Stream follower (cpbus_stream_fanout_next): the same fan-out, shape and watermark taken from the slot header
 template <int STORE, bool TIMERS, bool DIGEST, bool ORDERED, bool PAIRS = false>
 __global__ void __launch_bounds__(kThreads, kCtasPerSm) fanout_follow_kernel(const FanoutParams p) {
-  constexpr bool FOLLOW = true;
+  constexpr bool FOLLOW = true, ROUND = false;
+#include "cpbus_fanout_body.cuh"
+}
+// Lossless stream round (cpbus_stream_round_next): the same fan-out of the prefix the shards agreed on
+template <int STORE, bool TIMERS, bool DIGEST, bool ORDERED, bool PAIRS = false>
+__global__ void __launch_bounds__(kThreads, kCtasPerSm) fanout_round_kernel(const FanoutParams p) {
+  constexpr bool FOLLOW = true, ROUND = true;
 #include "cpbus_fanout_body.cuh"
 }
 
 // Lossless mode (reference semantics, events/subscriber.go:30-32: a full channel
 // blocks the sender): before a batch is fanned out, count for every mailbox what
-// the batch would append and flag any that lacks the room.  Thread per subscriber.
-__global__ void admit_kernel(const cpbus_event* batch, uint32_t n_ev, uint64_t w_now, const SubCtl* ctl,
-                             const DevTimer* timers, uint32_t n_subs, uint32_t ring_cap, uint32_t K, uint32_t sub_base,
-                             uint32_t timers_on, DevStats* stats, const uint2* pairs) {
+// the batch would append and flag any that lacks the room.  Thread per subscriber.  (admit_kernel, and the exact pass
+// of a lossless stream round, stream_round_admit_kernel)
+__device__ __forceinline__ void admit_body(const cpbus_event* batch, uint32_t n_ev, uint64_t w_now, const SubCtl* ctl,
+                                           const DevTimer* timers, uint32_t n_subs, uint32_t ring_cap, uint32_t K,
+                                           uint32_t sub_base, uint32_t timers_on, DevStats* stats, const uint2* pairs) {
   __shared__ uint32_t hist[32];
   __shared__ uint32_t s_uni;
   __shared__ unsigned long long s_max;
@@ -467,6 +534,11 @@ __global__ void admit_kernel(const cpbus_event* batch, uint32_t n_ev, uint64_t w
   // following batches while they provably fit
   __syncthreads();
   if (threadIdx.x == 0 && s_max) atomicMax(&stats->admit_max_used, s_max);
+}
+__global__ void admit_kernel(const cpbus_event* batch, uint32_t n_ev, uint64_t w_now, const SubCtl* ctl,
+                             const DevTimer* timers, uint32_t n_subs, uint32_t ring_cap, uint32_t K, uint32_t sub_base,
+                             uint32_t timers_on, DevStats* stats, const uint2* pairs) {
+  admit_body(batch, n_ev, w_now, ctl, timers, n_subs, ring_cap, K, sub_base, timers_on, stats, pairs);
 }
 
 // Device-side consumer: every mailbox is read to the end and its records are discarded (head = tail).  Stands in for
@@ -691,13 +763,14 @@ __global__ void stream_offer_kernel(unsigned long long* word, unsigned long long
 
 // One CTA of kStreamMaxConsumers threads, lane c = consumer c: acquire every shard's offer of round `round` (bounded by the
 // stream timeout), then the minimum prefix and the OR of the stall bits.  A missing offer sets the sticky error word.
-__global__ void __launch_bounds__(kStreamMaxConsumers) stream_agree_kernel(const unsigned long long* ack, uint32_t n_consumers,
-                                                                          unsigned long long round, uint32_t spin_us,
-                                                                          StreamAgreeResult* out, unsigned int* err_word) {
+// (stream_agree_kernel and stream_round_agree_kernel: every thread of the CTA calls it, thread 0 gets the result; flags:
+// bit 0 some shard stalled, bit 1 some offer missing)
+__device__ __forceinline__ void agree_offers(const unsigned long long* ack, uint32_t n_consumers, unsigned long long round,
+                                             uint32_t spin_us, uint32_t& prefix, uint32_t& flags) {
   __shared__ uint32_t s_min[kStreamMaxConsumers / 32], s_flags[kStreamMaxConsumers / 32];
   const uint32_t c = threadIdx.x, lane = c & 31u, w = c >> 5;
   const unsigned long long tag = round & kOfferRoundMask;
-  uint32_t prefix = 0xFFFFFFFFu, flags = 0;   // flags: bit 0 stalled, bit 1 missing
+  prefix = 0xFFFFFFFFu; flags = 0;
   if (c < n_consumers) {
     const unsigned long long* word = ack + stream_offer_word_index(c, round);
     const unsigned long long budget = (spin_us ? (unsigned long long)spin_us : 2000000ull) * 1000ull;
@@ -717,14 +790,153 @@ __global__ void __launch_bounds__(kStreamMaxConsumers) stream_agree_kernel(const
   flags = __reduce_or_sync(0xFFFFFFFFu, flags);
   if (lane == 0) { s_min[w] = prefix; s_flags[w] = flags; }
   __syncthreads();
-  if (c == 0) {
+  if (c == 0)
     for (uint32_t i = 1; i < blockDim.x / 32; i++) { prefix = min(prefix, s_min[i]); flags |= s_flags[i]; }
+}
+__global__ void __launch_bounds__(kStreamMaxConsumers) stream_agree_kernel(const unsigned long long* ack, uint32_t n_consumers,
+                                                                          unsigned long long round, uint32_t spin_us,
+                                                                          StreamAgreeResult* out, unsigned int* err_word) {
+  uint32_t prefix, flags;
+  agree_offers(ack, n_consumers, round, spin_us, prefix, flags);
+  if (threadIdx.x == 0) {
     const uint32_t status = (flags & 2u) ? kErrStreamTimeout : 0u;
     if (status) asm volatile("st.relaxed.sys.global.u32 [%0], %1;" ::"l"(err_word), "r"(status) : "memory");   // host-mapped, sticky
     out->m = flags ? 0u : prefix;
     out->stalled = flags & 1u;
     out->status = status;
   }
+}
+
+// ---- lossless stream rounds on the device (cpbus_stream_round_next) -----------------------------------------------------
+// Step 1, one CTA: the cursor's batch header (acquired across the link, bounded by the stream timeout), the clock checks
+// cpbus_stream_admit makes on the host, and the fast path against the device room bound.  When the bound cannot prove the
+// fit, the CTA copies the remainder of the batch into local memory for the exact pass.  A batch that never arrives, that
+// does not match the cursor, or that lies behind the clock or beyond the timer window poisons the bus's rounds and sets the
+// sticky error word.
+__global__ void __launch_bounds__(kThreads) stream_round_decide_kernel(const RoundParams P) {
+  __shared__ uint32_t s_rem, s_src, s_pass;
+  RoundDev* d = P.dev;
+  if (threadIdx.x == 0) {
+    if (P.seed_bus) { d->room = P.seed_room; d->now = P.seed_now; d->last_wm = P.seed_wm; d->poison = 0; }
+    if (P.seed_cur) { P.cur->batch = P.seed_batch; P.cur->off = P.seed_off; }
+    const unsigned long long q = P.cur->batch;
+    const uint32_t off = P.cur->off;
+    uint32_t status = kRoundOk, admit = kRoundAdmitNone, rem = 0;
+    unsigned long long hw = 0;
+    if (d->poison) status = kRoundSkip;
+    else {
+      const StreamHdr* h = P.hdr + q % P.n_slots;
+      const unsigned long long budget = (P.spin_us ? (unsigned long long)P.spin_us : 2000000ull) * 1000ull;
+      unsigned long long seen, t0, t1;
+      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
+      for (;;) {
+        asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(seen) : "l"(&h->seq) : "memory");
+        if (seen >= q) break;
+        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1));
+        if (t1 - t0 > budget) break;
+        __nanosleep(64);
+      }
+      unsigned int err = 0;
+      if (seen != q) err = kErrStreamTimeout;
+      else {
+        uint32_t hn;
+        asm volatile("ld.relaxed.sys.global.u32 %0, [%1];" : "=r"(hn) : "l"(&h->n) : "memory");
+        asm volatile("ld.relaxed.sys.global.u64 %0, [%1];" : "=l"(hw) : "l"(&h->watermark) : "memory");
+        if (hn > P.B || hn < off) err = kErrStreamShape;
+        else if (hw < d->now || hw - d->last_wm > P.window) err = kErrFollowOrder;
+        else rem = hn - off;
+      }
+      if (err) {
+        asm volatile("st.relaxed.sys.global.u32 [%0], %1;" ::"l"(P.err_word), "r"(err) : "memory");   // host-mapped, sticky
+        d->poison = 1;
+        status = kRoundAbort;
+      } else if (P.n_subs) {
+        const uint64_t need = admit_need(rem, hw, d->last_wm, P.min_period, P.K, P.timers_armed != 0);
+        if (d->room >= need) { d->room -= need; admit = kRoundAdmitSkipped; }
+        else {
+          admit = kRoundAdmitPass;
+          P.stats->admit_overflow = 0; P.stats->overwritten = 0; P.stats->admit_max_used = 0; P.stats->admit_deficit = 0;
+        }
+      }
+    }
+    d->q = q; d->off = off; d->rem = rem; d->hw = hw; d->status = status; d->admit = admit;
+    s_rem = rem; s_src = (uint32_t)(q % P.n_slots) * P.B + off; s_pass = admit == kRoundAdmitPass ? 1u : 0u;
+  }
+  __syncthreads();
+  if (!s_pass) return;
+  const uint4* src = reinterpret_cast<const uint4*>(P.payload + s_src);
+  uint4* dst = reinterpret_cast<uint4*>(P.admit_batch);
+  for (uint32_t i = threadIdx.x; i < 2u * s_rem; i += blockDim.x) {
+    uint4 v;
+    asm volatile("ld.global.relaxed.sys.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(src + i) : "memory");
+    dst[i] = v;
+  }
+}
+
+// Step 2, the grid: the exact admission pass over the local copy, when step 1 could not prove the fit.  On the fast path
+// every CTA returns at once.
+__global__ void stream_round_admit_kernel(const RoundParams P) {
+  if (P.dev->admit != kRoundAdmitPass) return;   // CTA-uniform
+  admit_body(P.admit_batch, P.dev->rem, P.dev->hw, P.ctl, P.timers, P.n_subs, P.ring_cap, P.K, P.sub_base, P.timers_armed,
+             P.stats, P.pairs);
+}
+
+// Step 3, one CTA of kStreamMaxConsumers threads: this shard's admissible prefix (cpbus_stream_admit's rules), its offer
+// word, the wait for every shard's offer of the round, and the round's outcome: the fan-out's shape in RoundDev, the
+// cursor and the clock moved, the host's record.  A missing offer sets the sticky error word and poisons the bus's rounds.
+__global__ void __launch_bounds__(kStreamMaxConsumers) stream_round_agree_kernel(const RoundParams P) {
+  __shared__ uint32_t s_go;
+  RoundDev* d = P.dev;
+  if (threadIdx.x == 0) {
+    s_go = d->status == kRoundOk ? 1u : 0u;
+    if (s_go) {
+      const uint32_t rem = d->rem;
+      uint32_t p = rem, stalled = 0;
+      if (d->admit == kRoundAdmitPass) {
+        const bool ok = P.stats->admit_overflow == 0;
+        if (!ok) p = rem - (uint32_t)min((unsigned long long)rem, P.stats->admit_deficit);
+        const unsigned long long used = P.stats->admit_max_used;
+        d->room = used >= P.ring_cap ? 0ull : P.ring_cap - used;
+        // every record fits, but not the ticks due after the last of them: hold the last record back, or stall
+        if (!ok && p == rem) { if (rem == 0) stalled = 1; else p = rem - 1; }
+      }
+      asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(P.ack + stream_offer_word_index(P.consumer, P.round)),
+                   "l"(stream_offer_word(P.round, stalled, stalled ? 0u : p)) : "memory");
+    }
+  }
+  __syncthreads();
+  uint32_t m = 0, flags = 0;
+  if (s_go) agree_offers(P.ack, P.n_consumers, P.round, P.spin_us, m, flags);   // (s_go is CTA-uniform)
+  if (threadIdx.x != 0) return;
+  uint32_t rs;
+  unsigned long long w = 0;
+  d->go = 0;
+  if (!s_go) rs = d->status == kRoundSkip ? kFollowSkipped : kFollowAborted;
+  else if (flags & 2u) {
+    asm volatile("st.relaxed.sys.global.u32 [%0], %1;" ::"l"(P.err_word), "r"(kErrStreamTimeout) : "memory");   // host-mapped, sticky
+    d->poison = 1;
+    rs = kFollowAborted;
+  } else if ((flags & 1u) || (m == 0 && d->rem != 0)) rs = kRoundStalled;
+  else {
+    const bool final = m == d->rem;
+    const uint32_t src = (uint32_t)(d->q % P.n_slots) * P.B + d->off;
+    w = d->hw;
+    if (final) { P.cur->batch = d->q + 1; P.cur->off = 0; }
+    else {
+      // like a partial cpbus_stream_fanout_prefix: the watermark is the last delivered record's timestamp
+      unsigned long long ts;
+      asm volatile("ld.relaxed.sys.global.u64 %0, [%1];" : "=l"(ts) : "l"(&P.payload[src + m - 1].ts_ns) : "memory");
+      w = min(d->hw, max(ts, d->last_wm));
+      d->room = 0;
+      P.cur->off = d->off + m;
+    }
+    d->now = w; d->last_wm = w;
+    d->go = 1; d->m = m; d->src = src; d->final = final ? 1u : 0u; d->w = w;
+    rs = final ? kFollowDelivered : kRoundPartial;
+  }
+  volatile RoundRec* r = P.rec;
+  r->m = d->go ? m : 0u; r->watermark = w; r->room = d->room; r->admit = d->admit;
+  r->status = rs;
 }
 #endif  // __CUDACC__
 

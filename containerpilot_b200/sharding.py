@@ -75,6 +75,30 @@ def _agree(bus, st) -> int | None:
         return None
 
 
+def drive_rounds(queue_round, progress, T: int, pump=None, depth: int = 4) -> int:
+    """Lossless followers told only the number of batches T: queue admission rounds until batch T is complete.
+
+    `queue_round()` enqueues ONE round on every shard the caller drives (cpbus_stream_round_next); `progress()` resolves and
+    returns (batches complete, offset, stalled rounds) (cpbus_stream_progress); `pump()` lets the consumers run.  At most
+    min(depth, T - batches) rounds are queued between resolutions — one round completes at most one batch, so none reaches
+    past batch T — and the pump runs between rounds and after each resolution.  Every rank that runs this with the same T
+    sees the same outcomes, so every rank queues the same rounds and all stop together.  Returns the rounds queued."""
+    if not 1 <= depth <= 8:
+        raise ValueError("depth must be 1..8 (outstanding rounds per bus)")
+    queued = 0
+    done = progress()[0]
+    while done < T:
+        for i in range(min(depth, T - done)):
+            if i and pump is not None:
+                pump()
+            queue_round()
+            queued += 1
+        done = progress()[0]
+        if done < T and pump is not None:
+            pump()
+    return queued
+
+
 class _ShardOps:
     """What both drivers share: a shard is a `Bus` plus its end of the publisher's stream."""
 
@@ -193,6 +217,25 @@ class ShardedBus(_ShardOps):
             raise RuntimeError("a lossless ShardedBus agrees on every batch's admitted prefix (fanout), which needs its shape")
         for _ in range(k):
             nat.check(self.bus.stream_fanout_next(self._st), "cpbus_stream_fanout_next")
+
+    def follow_rounds(self, k: int = 1):
+        """Lossless mode: enqueue `k` admission rounds on this rank without knowing the batches' shapes
+        (`cpbus_stream_round_next`): admit, offer, agree and the fan-out of the agreed prefix all run on the device, and the
+        host never waits for them.  Every rank must queue the same rounds."""
+        if not self.lossless:
+            raise RuntimeError("rounds agree on an admitted prefix: a throughput-mode ShardedBus follows with follow()")
+        for _ in range(k):
+            nat.check(self.bus.stream_round_next(self._st), "cpbus_stream_round_next")
+
+    def progress(self) -> tuple[int, int, int]:
+        """Resolve outstanding followers / rounds: (batches complete, records of the next one delivered, stalled rounds)."""
+        rc, done, off, stalled = self.bus.stream_progress(self._st)
+        nat.check(rc, "cpbus_stream_progress")
+        return done, off, stalled
+
+    def run_rounds(self, T: int, pump=None, depth: int = 4) -> int:
+        """Lossless followers: queue rounds until this rank has completely fanned out T batches (`drive_rounds`)."""
+        return drive_rounds(lambda: self.follow_rounds(1), self.progress, T, pump, depth)
 
     def publish(self, events: np.ndarray, now_ns: int) -> int:
         """put + fanout for callers that do not pipeline.  Lossless mode: one round, no retry (EAGAIN: drain, then
@@ -397,6 +440,33 @@ class LocalShardedBus:
         """Enqueue fan-outs of the stream's next `k` batches on shard `g` without their shapes (`cpbus_stream_fanout_next`)."""
         for _ in range(k):
             nat.check(self.shards[g][2].stream_fanout_next(self._st[g]), "cpbus_stream_fanout_next")
+
+    def follow_rounds(self, g: int, k: int = 1):
+        """Lossless mode: enqueue `k` admission rounds on shard `g` (`cpbus_stream_round_next`).  A round waits on the
+        device for every shard's offer, so queue each round on every shard before the host resolves any of them
+        (`run_rounds` does)."""
+        if not self.lossless:
+            raise RuntimeError("rounds agree on an admitted prefix: a throughput-mode bus follows with follow()")
+        for _ in range(k):
+            nat.check(self.shards[g][2].stream_round_next(self._st[g]), "cpbus_stream_round_next")
+
+    def progress(self) -> tuple[int, int, int]:
+        """Resolve every shard: (batches complete, records of the next one delivered, stalled rounds), equal on every shard."""
+        got = []
+        for g, (_, _, bus) in enumerate(self.shards):
+            rc, done, off, stalled = bus.stream_progress(self._st[g])
+            nat.check(rc, "cpbus_stream_progress")
+            got.append((done, off, stalled))
+        if len(set(got)) != 1:
+            raise RuntimeError(f"shards resolved to different positions: {got}")
+        return got[0]
+
+    def run_rounds(self, T: int, pump=None, depth: int = 4) -> int:
+        """Lossless followers on every shard: queue rounds (each on every shard in turn) until T batches are complete."""
+        def one():
+            for g in range(self.world):
+                self.follow_rounds(g, 1)
+        return drive_rounds(one, self.progress, T, pump, depth)
 
     def drain(self, sub_id: int, cap: int | None = None) -> np.ndarray:
         """Consumer side: up to `cap` records of global subscriber `sub_id`, from the shard that owns it."""

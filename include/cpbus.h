@@ -250,7 +250,7 @@ int cpbus_publish_device_staged(cpbus_t* bus, const void* d_events, size_t n, ui
  *   every step     : [publisher] cpbus_stream_put(st, events, n, now_ns, flags)   (may run ahead by < n_slots batches)
  *                    [all ranks] cpbus_stream_fanout(st, n, now_ns)
  *   followers      : [ranks that are never told n, now_ns] cpbus_stream_fanout_next(st) — the kernel reads them from the slot
- *                    header; may be called ahead of the publisher (throughput mode only)
+ *                    header; may be called ahead of the publisher (throughput mode; lossless: cpbus_stream_round_next)
  * Lossless mode (CPBUS_CFG_LOSSLESS): a stalled publish must stop at the same event on every shard — the shortest of the
  * prefixes the shards can take — so the fan-out is split in two and the driver takes the minimum in between:
  *   every step     : [publisher] cpbus_stream_put(st, events, n, now_ns, flags)
@@ -334,9 +334,37 @@ int cpbus_stream_poll(cpbus_stream_t* st, int* ready, size_t* n, uint64_t* now_n
  * A followed batch whose watermark lies behind this bus's clock, or steps further than 32/timers_per_sub periods of the
  * fastest periodic timer, delivers nothing, fires no timer and is not acknowledged; every follower queued behind it does
  * nothing, and cpbus_stream_status and every later stream call on this bus return CPBUS_EORDER (sticky, as
- * CPBUS_ETIMEDOUT is for a batch that never arrives).  CPBUS_EINVAL: NULL, or a lossless bus (lossless consumers poll and
- * run the admit / offer / agree round, which syncs once per round anyway). */
+ * CPBUS_ETIMEDOUT is for a batch that never arrives).  CPBUS_EINVAL: NULL, or a lossless bus (lossless followers queue
+ * rounds with cpbus_stream_round_next). */
 int cpbus_stream_fanout_next(cpbus_stream_t* st);
+/* Lossless followers: one admission round enqueued on the bus stream, never waited for on the host.  The round takes this
+ * shard's current batch — the first one it has not completely delivered when the round runs, which the host may not know
+ * yet — and does on the device what one host-driven round does with the header's n and watermark: it acquires the slot
+ * header (bounded wait), computes this shard's admissible prefix of the undelivered remainder by cpbus_stream_admit's rules,
+ * posts the offer word, waits for every shard's offer of the same round (bounded by the stream timeout) and fans out the
+ * agreed m records.  A partial round's watermark is its last record's; the batch's slot is acknowledged, and the device
+ * cursor moves to the next batch, when the round completes it.  If any shard stalls, the round delivers nothing and fires
+ * no timer.  Every shard must enqueue the same sequence of rounds (as with _offer / _agree; round numbers continue the
+ * count of _agree, one per call); one round completes at most one batch.
+ *   [all shards, per round]  cpbus_stream_round_next(st)        (queue several; one thread driving several shards queues
+ *                                                                the same round on every shard before the next one)
+ *   [now and then]           cpbus_stream_progress(st, &T_done, &offset, &stalled)   resolve; let the consumers drain
+ * The host learns the outcomes lazily, through the followers' queue (at most 8 outstanding; the 9th call resolves first)
+ * and the same per-launch records: every call that reads or changes host state resolves first, and then the bus state
+ * (stream position, clock, publish counts and ordinals, room bound, admit_passes / _skipped / _partial, debug-ring
+ * entries) is what the host-driven rounds with the same outcomes leave.  After resolution a driver may switch freely
+ * between rounds and explicit admit / offer / agree / fanout_prefix.  While rounds are outstanding the device copy of the
+ * room bound is authoritative; cpbus_consume_all does not wait for them: it is ordered behind them on the bus stream and
+ * resets that copy there.  A round whose batch lies behind this bus's clock or beyond its timer window posts no offer and
+ * sets the sticky CPBUS_EORDER; the rounds queued behind it do nothing, and the other shards' rounds give up waiting for
+ * its offer (sticky CPBUS_ETIMEDOUT).  CPBUS_EINVAL: NULL, a throughput-mode bus, or an explicit offer pending. */
+int cpbus_stream_round_next(cpbus_stream_t* st);
+/* Resolves outstanding followers and rounds, then: *batches = batches this consumer has completely fanned out, *offset =
+ * records of the next one already delivered (0 for throughput followers), *stalled_rounds = rounds so far that moved
+ * nothing (some shard stalled, or the agreed prefix was 0).  A driver told only the number of batches T queues at most
+ * T - *batches rounds at a time: never past the last batch, and every rank decides alike.  Returns the sticky stream error
+ * (the outputs are set either way). */
+int cpbus_stream_progress(cpbus_stream_t* st, uint64_t* batches, size_t* offset, uint64_t* stalled_rounds);
 int cpbus_stream_status(cpbus_stream_t* st);                       /* CPBUS_OK or the sticky error */
 int cpbus_stream_set_timeout(cpbus_stream_t* st, uint32_t microseconds);   /* in-kernel wait bound; default 2 s */
 int cpbus_stream_close(cpbus_stream_t* st);                        /* importers close before the owner */
