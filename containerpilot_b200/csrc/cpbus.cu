@@ -214,6 +214,22 @@ int dev_guard(cpbus* b) {
   return CPBUS_OK;
 }
 
+// Pinned host memory that the device writes through a mapping: *h and its device alias *d, set only on success.
+template <class T>
+cudaError_t mapped_alloc(size_t bytes, T** h, T** d) {
+  void *ph = nullptr, *pd = nullptr;
+  cudaError_t e = cudaHostAlloc(&ph, bytes, cudaHostAllocMapped);
+  if (e != cudaSuccess) return e;
+  if ((e = cudaHostGetDevicePointer(&pd, ph, 0)) != cudaSuccess) { cudaFreeHost(ph); return e; }
+  *h = static_cast<T*>(ph); *d = static_cast<T*>(pd);
+  return cudaSuccess;
+}
+
+// How long the host waits for a stream's consumers or publisher (cpbus_stream_set_timeout; 0 = 2 s).
+std::chrono::microseconds stream_budget(const cpbus* b) {
+  return std::chrono::microseconds(b->stream_spin_us ? b->stream_spin_us : 2000000u);
+}
+
 // The sticky stream error of this bus: a followed batch out of order (CPBUS_EORDER), otherwise a batch that never arrived or
 // did not match its header (CPBUS_ETIMEDOUT).
 int stream_error(const cpbus* b) {
@@ -376,9 +392,18 @@ struct StreamArgs {   // stream mode (cpbus_stream_fanout_prefix): where this ba
   const RoundDev* round = nullptr;       // lossless round (cpbus_stream_round_next): m, the watermark and the source from the agree kernel
 };
 
-int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, int staged = 0,
-                  const cpbus_event* prefetch_src = nullptr, cpbus_event* prefetch_dst = nullptr, uint32_t prefetch_n = 0,
-                  bool batch_dep = false, bool account = false, const StreamArgs* sa = nullptr) {
+struct LaunchOpts {
+  int staged = 0;                          // 1: the batch may live in a peer GPU's HBM; 2: a stream batch (`stream`)
+  const cpbus_event* pf_src = nullptr;     // a later batch of pf_n records that this launch pulls into pf_dst
+  cpbus_event* pf_dst = nullptr;
+  uint32_t pf_n = 0;
+  bool batch_dep = false;                  // the batch was written by the immediately preceding launch
+  bool account = false;                    // the lead CTA accounts the batch (it did not pass through cpbus_publish)
+  const StreamArgs* stream = nullptr;
+};
+
+int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, const LaunchOpts& o = {}) {
+  const StreamArgs* sa = o.stream;
   if (b->n_next == 0 && !sa) return CPBUS_OK;
   if (n == 0 && b->n_timers == 0 && !sa) return CPBUS_OK;   // (a stream batch is always consumed: its slot must be acknowledged)
   FanoutParams p{};
@@ -387,8 +412,8 @@ int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, in
   p.desc_ready = b->d_desc_ready + (p.launch_seq & 1) * 16; p.w_now = w;
   p.result = b->d_result + (size_t)(p.launch_seq % kResultRing) * kResultSub;
   p.result_next = b->d_result + (size_t)((p.launch_seq + 1) % kResultRing) * kResultSub;
-  p.batch_local = b->d_batch_local; p.staged = (uint32_t)staged;
-  p.err_word = b->d_err; p.acct = account ? b->d_acct : nullptr;
+  p.batch_local = b->d_batch_local; p.staged = (uint32_t)o.staged;
+  p.err_word = b->d_err; p.acct = o.account ? b->d_acct : nullptr;
   p.pf_state = b->d_pf_state; p.pf_buf = b->d_pf_buf; p.pf_stride = b->B; p.spin_us = b->stream_spin_us;
   if (sa) {
     p.stream_hdr = sa->hdr; p.stream_ack = sa->ack; p.stream_seq = sa->seq; p.stream_next_hdr = sa->next_hdr;
@@ -401,8 +426,8 @@ int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, in
     p.follow_clock = b->d_follow_clock; p.follow_rec = sa->follow_rec; p.follow_window = max_window(b);
     p.follow_from_host = sa->follow_from_host ? 1u : 0u;
   }
-  p.prefetch_src = prefetch_src; p.prefetch_dst = prefetch_dst; p.prefetch_n = prefetch_n;
-  p.batch_dep = batch_dep ? 1u : 0u; p.n_ev = n;
+  p.prefetch_src = o.pf_src; p.prefetch_dst = o.pf_dst; p.prefetch_n = o.pf_n;
+  p.batch_dep = o.batch_dep ? 1u : 0u; p.n_ev = n;
   p.n_subs = b->n_next; p.ring_cap = b->R; p.K = b->K; p.sub_base = b->cfg.sub_id_base;
   p.use_digest = b->use_digest; p.lossless = b->lossless; p.timers_on = b->n_timers > 0 && b->K > 0;
   p.smem_cap = (n + 31u) & ~31u;
@@ -485,11 +510,10 @@ int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, in
 #undef CPBUS_DISPATCH
   if (rc) return rc;
   b->st.kernel_launches++;
-  if (round) return CPBUS_OK;    // batches, clock and debug-ring marker: when the round is resolved, if it delivered
-  b->st.batches++;
-  if (follow) return CPBUS_OK;   // clock and debug-ring marker: when the launch is resolved (follow_resolve)
+  if (!round) b->st.batches++;   // (a round's batch counts when it is resolved, if it delivered)
+  if (sa) return CPBUS_OK;       // (the caller folds a stream launch in once its outcome is known: stream_delivered)
   b->last_watermark = w;
-  if (account && n) dbg_mark_device_batch(b, p.launch_seq);
+  if (o.account && n) dbg_mark_device_batch(b, p.launch_seq);
   return CPBUS_OK;
 }
 
@@ -625,6 +649,12 @@ static int follow_records(const cpbus* b) {
 
 extern "C" {
 static int follow_resolve(cpbus* b);
+// The opening of the entry points that read or change host-side bus state: this bus's device, then the outstanding
+// followers and rounds folded in (DESIGN.md §8, lazy resolution).
+static int enter(cpbus* b) {
+  const int rc = dev_guard(b);
+  return rc ? rc : follow_resolve(b);
+}
 // Nothing may unwind through the C boundary (cgo, ctypes): every status-returning entry point is a function-try-block.
 #define CPBUS_CATCH                                                                                   \
   catch (const std::bad_alloc&) { return CPBUS_ENOMEM; }                                              \
@@ -773,17 +803,20 @@ int cpbus_create(const cpbus_config* cfg, cpbus_t** out) try {
     RoundDev init{};
     init.room_full = R;
     if (cudaMemcpyAsync(b->d_round, &init, sizeof(init), cudaMemcpyHostToDevice, b->stream) != cudaSuccess) return fail(CPBUS_ECUDA);
-    if (cudaHostAlloc((void**)&b->h_round, sizeof(RoundRec) * cpbus::kFollowMax, cudaHostAllocMapped) != cudaSuccess) return fail(CPBUS_ENOMEM);
-    if (cudaHostGetDevicePointer((void**)&b->d_round_rec, b->h_round, 0) != cudaSuccess) return fail(CPBUS_ECUDA);
+    if (mapped_alloc(sizeof(RoundRec) * cpbus::kFollowMax, &b->h_round, &b->d_round_rec) != cudaSuccess) return fail(CPBUS_ENOMEM);
     if ((rc = preload_round_kernels(b))) return fail(rc);
+  } else {   // followers (cpbus_stream_fanout_next): their records and the clock words, zeroed
+    if (mapped_alloc(sizeof(FollowRec) * cpbus::kFollowMax, &b->h_follow, &b->d_follow) != cudaSuccess) return fail(CPBUS_ENOMEM);
+    ALLOC(b->d_follow_clock, 4 * sizeof(unsigned long long));
+    if (cudaMemsetAsync(b->d_follow_clock, 0, 4 * sizeof(unsigned long long), b->stream) != cudaSuccess) return fail(CPBUS_ECUDA);
   }
+  if (cudaEventCreateWithFlags(&b->follow_done, cudaEventDisableTiming) != cudaSuccess) return fail(CPBUS_ECUDA);
   ALLOC(b->d_pf_buf, (size_t)kStreamPrefetch * B * sizeof(cpbus_event)); ALLOC(b->d_pf_state, 64);
   ALLOC(b->d_acct, sizeof(DevPubAcct));
   if (cudaMemsetAsync(b->d_pf_state, 0, 64, b->stream) != cudaSuccess ||
       cudaMemsetAsync(b->d_acct, 0, sizeof(DevPubAcct), b->stream) != cudaSuccess) return fail(CPBUS_ECUDA);
-  if (cudaHostAlloc((void**)&b->h_err, 64, cudaHostAllocMapped) != cudaSuccess) return fail(CPBUS_ENOMEM);
+  if (mapped_alloc(64, &b->h_err, &b->d_err) != cudaSuccess) return fail(CPBUS_ENOMEM);
   memset(b->h_err, 0, 64);
-  if (cudaHostGetDevicePointer((void**)&b->d_err, b->h_err, 0) != cudaSuccess) return fail(CPBUS_ECUDA);
   if (cudaMallocHost((void**)&b->h_acct, offsetof(DevPubAcct, pair_key)) != cudaSuccess) return fail(CPBUS_ENOMEM);
   for (int i = 0; i < cpbus::kPrefetch; i++) ALLOC(b->d_prefetch[i], (size_t)B * sizeof(cpbus_event));
   ALLOC(b->d_result, sizeof(DevResultSlot) * kResultRing * kResultSub);
@@ -918,8 +951,7 @@ int cpbus_source(cpbus_t* b, uint32_t id, char* out, size_t cap, size_t* len) tr
 int cpbus_subscribe_many(cpbus_t* b, const uint32_t* masks, uint32_t n, uint32_t* first_sub_id) try {
   if (!b || !n) return CPBUS_EINVAL;
   if ((uint64_t)b->n_next + n > b->N) return CPBUS_ENOSPC;
-  int rc = dev_guard(b); if (rc) return rc;
-  if ((rc = follow_resolve(b))) return rc;
+  int rc = enter(b); if (rc) return rc;
   if ((rc = flush_staged(b, b->now))) return rc;   // ordered with publishes (events/bus.go:105-107 takes the same lock)
   const uint32_t first = b->n_next;
   std::vector<SubCtl> blocks(n);
@@ -950,8 +982,7 @@ int cpbus_subscribe_pairs(cpbus_t* b, uint32_t mask, const cpbus_pair* pairs, ui
   for (uint32_t j = 0; j < n_pairs; j++)
     if (!((mask >> pairs[j].code) & 1u)) row[used++] = make_uint2(pairs[j].code, pairs[j].source_id);
   if (used == 0) return cpbus_subscribe_many(b, &mask, 1, sub_id);
-  int rc = dev_guard(b); if (rc) return rc;
-  if ((rc = follow_resolve(b))) return rc;
+  int rc = enter(b); if (rc) return rc;
   if (!b->d_pairs) {
     if (cudaMalloc((void**)&b->d_pairs, (size_t)b->N * CPBUS_MAX_PAIRS * sizeof(uint2)) != cudaSuccess) {
       snprintf(g_cuda_err, sizeof(g_cuda_err), "cudaMalloc(pair tables) failed");
@@ -980,8 +1011,7 @@ int cpbus_subscribe_pairs_many(cpbus_t* b, const uint32_t* masks, const cpbus_pa
     for (uint32_t j = 0; j < n_pairs[i]; j++) if (pairs[(size_t)i * CPBUS_MAX_PAIRS + j].code >= CPBUS_N_CODES) return CPBUS_EINVAL;
   }
   if ((uint64_t)b->n_next + n > b->N) return CPBUS_ENOSPC;
-  int rc = dev_guard(b); if (rc) return rc;
-  if ((rc = follow_resolve(b))) return rc;
+  int rc = enter(b); if (rc) return rc;
   if (!b->d_pairs) {
     if (cudaMalloc((void**)&b->d_pairs, (size_t)b->N * CPBUS_MAX_PAIRS * sizeof(uint2)) != cudaSuccess) {
       snprintf(g_cuda_err, sizeof(g_cuda_err), "cudaMalloc(pair tables) failed");
@@ -1017,8 +1047,7 @@ int cpbus_unsubscribe(cpbus_t* b, uint32_t sub_id) try {
   if (!b) return CPBUS_EINVAL;
   const uint32_t l = sub_id - b->cfg.sub_id_base;
   if (sub_id < b->cfg.sub_id_base || l >= b->n_next) return CPBUS_ENOENT;
-  int rc = dev_guard(b); if (rc) return rc;
-  if ((rc = follow_resolve(b))) return rc;
+  int rc = enter(b); if (rc) return rc;
   if ((rc = flush_staged(b, b->now))) return rc;
   // second Unsubscribe drives the WaitGroup negative in Go (events/bus.go:121) => panic
   if (!b->h_active[l]) return CPBUS_ECLOSED;
@@ -1048,8 +1077,7 @@ int cpbus_set_mask(cpbus_t* b, uint32_t sub_id, uint32_t mask) try {
   const uint32_t l = sub_id - b->cfg.sub_id_base;
   if (sub_id < b->cfg.sub_id_base || l >= b->n_next) return CPBUS_ENOENT;
   if (!b->h_active[l]) return CPBUS_ECLOSED;
-  int rc = dev_guard(b); if (rc) return rc;
-  if ((rc = follow_resolve(b))) return rc;
+  int rc = enter(b); if (rc) return rc;
   if ((rc = flush_staged(b, b->now))) return rc;
   mask &= CPBUS_MASK_ALL;
   if (b->h_mask[l] != CPBUS_MASK_ALL) b->n_filtered--;
@@ -1071,8 +1099,7 @@ int cpbus_timer_add(cpbus_t* b, uint32_t sub_id, uint64_t period_ns, uint32_t so
   if (!b->K) return CPBUS_ENOSPC;
   const uint32_t l = sub_id - b->cfg.sub_id_base;
   if (sub_id < b->cfg.sub_id_base || l >= b->n_next) return CPBUS_ENOENT;
-  int rc = dev_guard(b); if (rc) return rc;
-  if ((rc = follow_resolve(b))) return rc;
+  int rc = enter(b); if (rc) return rc;
   if ((rc = flush_staged(b, b->now))) return rc;
   if (b->h_timers.empty()) b->h_timers.resize((size_t)b->N * b->K);
   retire_oneshots(b, b->last_watermark);
@@ -1100,8 +1127,7 @@ int cpbus_timer_add_many(cpbus_t* b, uint32_t first_sub, uint32_t n, uint64_t pe
   if (!b->K) return CPBUS_ENOSPC;
   const uint32_t l0 = first_sub - b->cfg.sub_id_base;
   if (first_sub < b->cfg.sub_id_base || (uint64_t)l0 + n > b->n_next) return CPBUS_ENOENT;
-  int rc = dev_guard(b); if (rc) return rc;
-  if ((rc = follow_resolve(b))) return rc;
+  int rc = enter(b); if (rc) return rc;
   if ((rc = flush_staged(b, b->now))) return rc;
   if (b->h_timers.empty()) b->h_timers.resize((size_t)b->N * b->K);
   // bulk arm: uses slot 0 of each subscriber (must be free)
@@ -1135,8 +1161,7 @@ int cpbus_timer_cancel(cpbus_t* b, uint32_t timer_id) try {
   const uint32_t slot_index = timer_id & kTimerSlotMask, gen = timer_id >> kTimerSlotBits;
   const uint32_t l = slot_index / b->K, k = slot_index % b->K;
   if (l >= b->n_next) return CPBUS_ENOENT;
-  int rc = dev_guard(b); if (rc) return rc;
-  if ((rc = follow_resolve(b))) return rc;
+  int rc = enter(b); if (rc) return rc;
   if ((rc = flush_staged(b, b->now))) return rc;   // firings due before the cancel still happen
   retire_oneshots(b, b->last_watermark);
   HostTimer& t = b->h_timers[(size_t)l * b->K + k];
@@ -1150,8 +1175,7 @@ int cpbus_timer_cancel(cpbus_t* b, uint32_t timer_id) try {
 
 int cpbus_publish(cpbus_t* b, const cpbus_event* ev, size_t n) try {
   if (!b || (!ev && n)) return CPBUS_EINVAL;
-  int rc = dev_guard(b); if (rc) return rc;
-  if ((rc = follow_resolve(b))) return rc;
+  int rc = enter(b); if (rc) return rc;
   for (size_t i = 0; i < n; i++) {   // counter slots of the whole burst: requested up front, touched in the loop below
     if (ev[i].code < CPBUS_N_CODES && ev[i].code != CPBUS_METRIC) b->pub_pairs.prefetch(((uint64_t)ev[i].code << 32) | ev[i].source_id);
   }
@@ -1183,8 +1207,7 @@ int cpbus_send(cpbus_t* b, uint32_t sub_id, const cpbus_event* ev) try {
   const uint32_t l = sub_id - b->cfg.sub_id_base;
   if (sub_id < b->cfg.sub_id_base || l >= b->n_next) return CPBUS_ENOENT;
   if (!b->h_active[l]) return CPBUS_ECLOSED;   // the mailbox is gone (Go: send on a closed channel panics)
-  int rc = dev_guard(b); if (rc) return rc;
-  if ((rc = follow_resolve(b))) return rc;
+  int rc = enter(b); if (rc) return rc;
   if ((rc = stage_one(b, ev->code, ev->source_id, sub_id, CPBUS_F_UNICAST))) return rc;
   b->st.publishes++;
   return CPBUS_OK;
@@ -1209,15 +1232,13 @@ int cpbus_advance(cpbus_t* b, uint64_t now_ns) try {
 
 int cpbus_flush(cpbus_t* b) try {
   if (!b) return CPBUS_EINVAL;
-  int rc = dev_guard(b); if (rc) return rc;
-  if ((rc = follow_resolve(b))) return rc;
+  int rc = enter(b); if (rc) return rc;
   return flush_staged(b, b->now);
 } CPBUS_CATCH
 
 int cpbus_sync(cpbus_t* b) try {
   if (!b) return CPBUS_EINVAL;
-  int rc = dev_guard(b); if (rc) return rc;
-  if ((rc = follow_resolve(b))) return rc;
+  int rc = enter(b); if (rc) return rc;
   CK(cudaStreamSynchronize(b->stream));
   return CPBUS_OK;
 } CPBUS_CATCH
@@ -1280,8 +1301,7 @@ static int publish_device_split(cpbus_t* b, const cpbus_event* d_events, size_t 
 static int publish_device_impl(cpbus_t* b, const void* d_events, size_t n, uint64_t watermark_ns, bool staged,
                                const void* d_next, size_t n_next) {
   if (!b || (!d_events && n) || ((uintptr_t)d_events & 31u) || n_next > b->B || ((uintptr_t)d_next & 31u)) return CPBUS_EINVAL;
-  int rc = dev_guard(b); if (rc) return rc;
-  if ((rc = follow_resolve(b))) return rc;
+  int rc = enter(b); if (rc) return rc;
   if ((rc = flush_staged(b, b->now))) return rc;
   if (watermark_ns < b->now) return CPBUS_EORDER;
   if (staged && b->lossless) return CPBUS_EINVAL;   // admission would have to read the peer batch: not supported
@@ -1311,15 +1331,16 @@ static int publish_device_impl(cpbus_t* b, const void* d_events, size_t n, uint6
       for (int i = 0; i < cpbus::kPrefetch; i++) if (b->pf_ptr[i] == d_events) b->pf_ptr[i] = nullptr;   // consumed (and any older copy dropped)
     }
   }
-  const cpbus_event* pf_src = nullptr; cpbus_event* pf_dst = nullptr;
+  LaunchOpts o;
+  o.staged = staged ? 1 : 0; o.pf_n = (uint32_t)n_next; o.batch_dep = dep; o.account = true;
   int slot = -1;
   if (d_next && n_next) {
     slot = b->pf_next;
     if (b->d_prefetch[slot] == src) slot = (slot + 1) % cpbus::kPrefetch;   // never overwrite the buffer this launch reads
-    pf_src = (const cpbus_event*)d_next; pf_dst = b->d_prefetch[slot];
+    o.pf_src = (const cpbus_event*)d_next; o.pf_dst = b->d_prefetch[slot];
     for (int i = 0; i < cpbus::kPrefetch; i++) if (b->pf_ptr[i] == d_next) b->pf_ptr[i] = nullptr;   // superseded
   }
-  if ((rc = launch_fanout(b, src, (uint32_t)n, watermark_ns, staged ? 1 : 0, pf_src, pf_dst, (uint32_t)n_next, dep, /*account=*/true))) return rc;
+  if ((rc = launch_fanout(b, src, (uint32_t)n, watermark_ns, o))) return rc;
   if (slot >= 0) { b->pf_ptr[slot] = d_next; b->pf_n[slot] = n_next; b->pf_seq[slot] = b->launch_seq; b->pf_next = (slot + 1) % cpbus::kPrefetch; }
   b->st.publishes += n; b->seq += n;
   return CPBUS_OK;
@@ -1547,7 +1568,6 @@ int cpbus_stream_put(cpbus_stream_t* st, const cpbus_event* ev, size_t n, uint64
     // consumers' kernels; refresh the cached minimum, and — unless the caller asked not to wait — give consumers that
     // are merely behind (their launches are queued, the GPUs are busy) up to the stream timeout to get there.
     const auto t0 = std::chrono::steady_clock::now();
-    const auto budget = std::chrono::microseconds(b->stream_spin_us ? b->stream_spin_us : 2000000u);
     for (;;) {
       CK(cudaMemcpyAsync(st->h_ack, st->ack, (size_t)st->n_consumers * 32, cudaMemcpyDeviceToHost, st->put_stream));
       CK(cudaStreamSynchronize(st->put_stream));
@@ -1555,7 +1575,7 @@ int cpbus_stream_put(cpbus_stream_t* st, const cpbus_event* ev, size_t n, uint64
       for (uint32_t c = 0; c < st->n_consumers; c++) m = std::min(m, st->h_ack[4 * c]);
       st->min_ack = m;
       if (st->min_ack + st->n_slots >= q) break;
-      if ((flags & CPBUS_PUT_NOWAIT) || std::chrono::steady_clock::now() - t0 > budget || *(volatile unsigned int*)b->h_err) return CPBUS_EAGAIN;
+      if ((flags & CPBUS_PUT_NOWAIT) || std::chrono::steady_clock::now() - t0 > stream_budget(b) || *(volatile unsigned int*)b->h_err) return CPBUS_EAGAIN;
       std::this_thread::sleep_for(std::chrono::microseconds(20));
     }
   }
@@ -1588,8 +1608,7 @@ int cpbus_stream_put(cpbus_stream_t* st, const cpbus_event* ev, size_t n, uint64
 int cpbus_stream_poll(cpbus_stream_t* st, int* ready, size_t* n, uint64_t* now_ns) try {
   if (!st || !ready) return CPBUS_EINVAL;
   cpbus* b = st->bus;
-  int rc = dev_guard(b); if (rc) return rc;
-  if ((rc = follow_resolve(b))) return rc;
+  int rc = enter(b); if (rc) return rc;
   if ((rc = stream_error(b))) return rc;
   const unsigned long long q = st->get_seq + 1;
   StreamHdr h{};
@@ -1607,7 +1626,6 @@ static int stream_wait_released(cpbus_stream* st, unsigned long long q, size_t n
   if (st->seen_seq >= q) return CPBUS_OK;
   cpbus* b = st->bus;
   const auto t0 = std::chrono::steady_clock::now();
-  const auto budget = std::chrono::microseconds(b->stream_spin_us ? b->stream_spin_us : 2000000u);
   for (;;) {
     StreamHdr h{};
     CK(cudaMemcpyAsync(&h, &st->hdr[q % st->n_slots], sizeof(h), cudaMemcpyDeviceToHost, b->result_stream));
@@ -1617,7 +1635,7 @@ static int stream_wait_released(cpbus_stream* st, unsigned long long q, size_t n
       st->seen_seq = q;
       return CPBUS_OK;
     }
-    if (std::chrono::steady_clock::now() - t0 > budget) return CPBUS_ETIMEDOUT;
+    if (std::chrono::steady_clock::now() - t0 > stream_budget(b)) return CPBUS_ETIMEDOUT;
     std::this_thread::sleep_for(std::chrono::microseconds(20));
   }
 }
@@ -1625,8 +1643,7 @@ static int stream_wait_released(cpbus_stream* st, unsigned long long q, size_t n
 // The checks every stream call makes before it admits or launches anything (clock, window, this bus's own staged events).
 static int stream_enter(cpbus_stream* st, uint64_t now_ns) {
   cpbus* b = st->bus;
-  int rc = dev_guard(b); if (rc) return rc;
-  if ((rc = follow_resolve(b))) return rc;
+  int rc = enter(b); if (rc) return rc;
   if ((rc = stream_error(b))) return rc;
   if ((rc = flush_staged(b, b->now))) return rc;
   if (now_ns < b->now) return CPBUS_EORDER;
@@ -1662,6 +1679,35 @@ int cpbus_stream_admit(cpbus_stream_t* st, size_t n, uint64_t now_ns, size_t* pr
   return CPBUS_OK;
 } CPBUS_CATCH
 
+// Consumer st's launch of batch q from record `off` of its slot: the header and this consumer's ack word and, without
+// lossless mode, the batch after next for the kernel to prefetch (a lossless batch may take several launches, each reading
+// its part of the slot, so lossless launches neither request nor take the prefetch).  Returns where the records start.
+static const cpbus_event* stream_launch(const cpbus_stream* st, unsigned long long q, uint32_t off, bool final, StreamArgs& sa,
+                                        LaunchOpts& o) {
+  const cpbus* b = st->bus;
+  const uint32_t slot = (uint32_t)(q % st->n_slots), slot2 = (uint32_t)((q + 2) % st->n_slots);
+  sa.hdr = &st->hdr[slot]; sa.ack = &st->ack[4 * st->consumer]; sa.seq = q; sa.off = off; sa.final = final;
+  o.staged = 2; o.account = true; o.stream = &sa;
+  if (!b->lossless) {
+    sa.next_hdr = &st->hdr[slot2];
+    o.pf_src = st->payload + (size_t)slot2 * st->B; o.pf_dst = b->d_pf_buf + (size_t)((q + 2) % kStreamPrefetch) * b->B;
+  }
+  return st->payload + (size_t)slot * st->B + off;
+}
+
+// A stream launch that delivered m records with watermark w, folded into the host state; `final`: it completed its batch.
+// The host-driven launch, a resolved follower and a resolved round all fold here, so each moves the host state exactly as
+// the others with the same outcome do.
+static void stream_delivered(cpbus* b, cpbus_stream* st, uint32_t m, uint64_t w, bool final, unsigned long long launch_seq) {
+  b->st.publishes += m; b->seq += m;
+  b->now = w; b->last_watermark = w;
+  if (m) dbg_mark_device_batch(b, launch_seq);
+  if (final) { st->get_seq++; st->get_off = 0; return; }
+  st->get_off += m;
+  b->room_lb = 0;
+  b->st.admit_partial++;
+}
+
 // Fan out the next m undelivered records of the current batch (throughput mode: m = the whole batch, in one launch).
 static int stream_fanout_prefix(cpbus_stream* st, size_t n, uint64_t now_ns, size_t m) {
   cpbus* b = st->bus;
@@ -1670,9 +1716,8 @@ static int stream_fanout_prefix(cpbus_stream* st, size_t n, uint64_t now_ns, siz
   if (m == 0 && !final) return CPBUS_EAGAIN;
   const unsigned long long q = st->get_seq + 1;
   StreamArgs sa;
-  const uint32_t slot = (uint32_t)(q % st->n_slots), slot2 = (uint32_t)((q + 2) % st->n_slots);
-  sa.hdr = &st->hdr[slot]; sa.ack = &st->ack[4 * st->consumer]; sa.seq = q; sa.off = st->get_off; sa.final = final;
-  const cpbus_event* src = st->payload + (size_t)slot * st->B + st->get_off;
+  LaunchOpts o;
+  const cpbus_event* src = stream_launch(st, q, st->get_off, final, sa, o);
   uint64_t w = now_ns;
   if (!final) {
     // Like a partial cpbus_flush: the watermark is the last delivered record's timestamp, so the ticks due after it go with
@@ -1687,21 +1732,9 @@ static int stream_fanout_prefix(cpbus_stream* st, size_t n, uint64_t now_ns, siz
   // this bus's own staged events would fire the ticks due by now_ns on their own, in front of the undelivered records and
   // without their admission.
   b->now = w;
-  if (b->lossless) {   // no device-managed prefetch: a batch may take several launches, each reads its part of the slot
-    rc = launch_fanout(b, src, (uint32_t)m, w, /*staged=*/2, nullptr, nullptr, 0, /*batch_dep=*/false, /*account=*/true, &sa);
-  } else {
-    sa.next_hdr = &st->hdr[slot2];
-    rc = launch_fanout(b, src, (uint32_t)m, w, /*staged=*/2,
-                       st->payload + (size_t)slot2 * st->B, b->d_pf_buf + (size_t)((q + 2) % kStreamPrefetch) * b->B, 0,
-                       /*batch_dep=*/false, /*account=*/true, &sa);
-  }
-  if (rc) return rc;
-  b->st.publishes += m; b->seq += m;
-  if (final) { st->get_seq = q; st->get_off = 0; return CPBUS_OK; }
-  st->get_off += (uint32_t)m;
-  b->room_lb = 0;
-  b->st.admit_partial++;
-  return CPBUS_EAGAIN;
+  if ((rc = launch_fanout(b, src, (uint32_t)m, w, o))) return rc;
+  stream_delivered(b, st, (uint32_t)m, w, final, b->launch_seq);
+  return final ? CPBUS_OK : CPBUS_EAGAIN;
 }
 
 int cpbus_stream_fanout_prefix(cpbus_stream_t* st, size_t n, uint64_t now_ns, size_t m) try {
@@ -1730,14 +1763,8 @@ static void round_fold(cpbus* b, const cpbus::FollowPending& f) {
   else if (r->admit == kRoundAdmitSkipped) b->st.admit_skipped++;
   b->room_lb = r->room;
   if (status == kRoundStalled) { st->stalled_rounds++; return; }
-  const uint32_t m = r->m;
-  const uint64_t w = r->watermark;
   b->st.batches++;
-  b->st.publishes += m; b->seq += m;
-  b->now = w; b->last_watermark = w;
-  if (m) dbg_mark_device_batch(b, f.launch_seq);
-  if (status == kFollowDelivered) { st->get_seq++; st->get_off = 0; }
-  else { st->get_off += m; b->st.admit_partial++; }
+  stream_delivered(b, st, r->m, r->watermark, status == kFollowDelivered, f.launch_seq);
 }
 
 static int follow_resolve(cpbus* b) {
@@ -1759,16 +1786,34 @@ static int follow_resolve(cpbus* b) {
     }
     const volatile FollowRec* r = &b->h_follow[f.rec];
     if (r->status == kFollowPending) missing = true;
-    if (r->status != kFollowDelivered) continue;
-    const uint32_t n = r->n;
-    const uint64_t w = r->watermark;
-    f.st->get_seq++;
-    b->st.publishes += n; b->seq += n;
-    b->now = w; b->last_watermark = w;
-    if (n) dbg_mark_device_batch(b, f.launch_seq);
+    if (r->status == kFollowDelivered) stream_delivered(b, f.st, r->n, r->watermark, /*final=*/true, f.launch_seq);
   }
   if (missing) { snprintf(g_cuda_err, sizeof(g_cuda_err), "a follower launch or round completed without its record"); return CPBUS_ECUDA; }
   return CPBUS_OK;
+}
+
+// The opening of an enqueue (cpbus_stream_fanout_next, _round_next), under follow_mu: a free record (with kFollowMax
+// outstanding, the queue is resolved first), record *ri marked pending.  The first launch after the host has resolved
+// (*seed) starts from the host's state, this bus's own staged events flushed first as in the host-driven calls; the ones
+// queued behind it take their predecessor's state on the device.
+static int follow_begin(cpbus* b, cpbus::FollowKind kind, int* ri, bool* seed) {
+  int rc = dev_guard(b); if (rc) return rc;
+  if (follow_records(b) >= cpbus::kFollowMax && (rc = follow_resolve(b))) return rc;
+  if ((rc = stream_error(b))) return rc;
+  *seed = b->follow_q.empty();
+  if (*seed && (rc = flush_staged(b, b->now))) return rc;
+  *ri = b->follow_next;
+  if (kind == cpbus::kRound) b->h_round[*ri].status = kFollowPending;
+  else b->h_follow[*ri].status = kFollowPending;
+  return CPBUS_OK;
+}
+
+// ... and its close: record ri joins the queue, behind the launch that writes it.
+static void follow_end(cpbus_stream* st, cpbus::FollowKind kind, int ri) {
+  cpbus* b = st->bus;
+  b->follow_next = (ri + 1) % cpbus::kFollowMax;
+  b->follow_q.push_back(cpbus::FollowPending{st, b->launch_seq, ri, kind});
+  st->follow_out++;
 }
 
 // Every rank that does not know the batches' shapes: enqueue the fan-out of the stream's next not yet enqueued batch and
@@ -1778,39 +1823,14 @@ int cpbus_stream_fanout_next(cpbus_stream_t* st) try {
   cpbus* b = st->bus;
   if (b->lossless) return CPBUS_EINVAL;   // lossless followers agree on every round, which syncs anyway
   std::lock_guard<std::recursive_mutex> g(b->follow_mu);
-  int rc = dev_guard(b); if (rc) return rc;
-  if (follow_records(b) >= cpbus::kFollowMax && (rc = follow_resolve(b))) return rc;
-  if ((rc = stream_error(b))) return rc;
-  if (!b->h_follow) {
-    FollowRec *h = nullptr, *d = nullptr;
-    CK(cudaHostAlloc((void**)&h, sizeof(FollowRec) * cpbus::kFollowMax, cudaHostAllocMapped));
-    if (cudaHostGetDevicePointer((void**)&d, h, 0) != cudaSuccess) { cudaFreeHost(h); CK(cudaGetLastError()); return CPBUS_ECUDA; }
-    b->h_follow = h; b->d_follow = d;
-  }
-  if (!b->d_follow_clock) {
-    CK(cudaMalloc((void**)&b->d_follow_clock, 4 * sizeof(unsigned long long)));
-    CK(cudaMemsetAsync(b->d_follow_clock, 0, 4 * sizeof(unsigned long long), b->stream));
-  }
-  if (!b->follow_done) CK(cudaEventCreateWithFlags(&b->follow_done, cudaEventDisableTiming));
-  // The first follower after the host has resolved starts from the host clock (this bus's own staged events go out first,
-  // as in cpbus_stream_fanout); the ones queued behind it read their predecessor's watermark on the device.
-  const bool from_host = b->follow_q.empty();
-  if (from_host && (rc = flush_staged(b, b->now))) return rc;
-  const unsigned long long q = st->get_seq + 1 + st->follow_out;
-  const uint32_t slot = (uint32_t)(q % st->n_slots), slot2 = (uint32_t)((q + 2) % st->n_slots);
-  const int ri = b->follow_next;
-  b->h_follow[ri].status = kFollowPending;
+  int ri = 0; bool from_host = false;
+  int rc = follow_begin(b, cpbus::kFollower, &ri, &from_host); if (rc) return rc;
   StreamArgs sa;
-  sa.hdr = &st->hdr[slot]; sa.ack = &st->ack[4 * st->consumer]; sa.seq = q; sa.off = 0; sa.final = true;
-  sa.next_hdr = &st->hdr[slot2];
+  LaunchOpts o;
+  const cpbus_event* src = stream_launch(st, st->get_seq + 1 + st->follow_out, 0, /*final=*/true, sa, o);
   sa.follow_rec = b->d_follow + ri; sa.follow_from_host = from_host;
-  rc = launch_fanout(b, st->payload + (size_t)slot * st->B, b->B, b->now, /*staged=*/2,
-                     st->payload + (size_t)slot2 * st->B, b->d_pf_buf + (size_t)((q + 2) % kStreamPrefetch) * b->B, 0,
-                     /*batch_dep=*/false, /*account=*/true, &sa);
-  if (rc) return rc;
-  b->follow_next = (ri + 1) % cpbus::kFollowMax;
-  b->follow_q.push_back(cpbus::FollowPending{st, b->launch_seq, ri, cpbus::kFollower});
-  st->follow_out++;
+  if ((rc = launch_fanout(b, src, b->B, b->now, o))) return rc;
+  follow_end(st, cpbus::kFollower, ri);
   return CPBUS_OK;
 } CPBUS_CATCH
 
@@ -1822,16 +1842,9 @@ int cpbus_stream_round_next(cpbus_stream_t* st) try {
   cpbus* b = st->bus;
   if (!b->lossless || st->offered) return CPBUS_EINVAL;   // throughput mode needs no agreement; not inside an explicit round
   std::lock_guard<std::recursive_mutex> g(b->follow_mu);
-  int rc = dev_guard(b); if (rc) return rc;
-  if (follow_records(b) >= cpbus::kFollowMax && (rc = follow_resolve(b))) return rc;
-  if ((rc = stream_error(b))) return rc;
-  if (!b->follow_done) CK(cudaEventCreateWithFlags(&b->follow_done, cudaEventDisableTiming));
-  // The first round after the host has resolved takes the bus state from the host (this bus's own staged events go out
-  // first, as in cpbus_stream_admit); the ones queued behind it use the device copy.  Likewise the stream's cursor.
-  const bool seed_bus = b->follow_q.empty(), seed_cur = st->follow_out == 0;
-  if (seed_bus && (rc = flush_staged(b, b->now))) return rc;
-  const int ri = b->follow_next;
-  b->h_round[ri].status = kFollowPending;
+  int ri = 0; bool seed_bus = false;
+  int rc = follow_begin(b, cpbus::kRound, &ri, &seed_bus); if (rc) return rc;
+  const bool seed_cur = st->follow_out == 0;   // likewise the stream's cursor, while none of this stream's rounds is queued
   RoundParams P{};
   P.dev = b->d_round; P.cur = st->d_cursor; P.rec = b->d_round_rec + ri;
   P.hdr = st->hdr; P.payload = st->payload; P.ack = st->ack;
@@ -1859,19 +1872,17 @@ int cpbus_stream_round_next(cpbus_stream_t* st) try {
   st->agree_round = P.round;
   StreamArgs sa;
   sa.ack = &st->ack[4 * st->consumer]; sa.round = b->d_round;
-  rc = launch_fanout(b, st->payload, b->B, b->now, /*staged=*/2, nullptr, nullptr, 0, /*batch_dep=*/false, /*account=*/true, &sa);
-  // (a failed launch leaves the round's record pending: the next resolution reports it)
-  b->follow_next = (ri + 1) % cpbus::kFollowMax;
-  b->follow_q.push_back(cpbus::FollowPending{st, b->launch_seq, ri, cpbus::kRound});
-  st->follow_out++;
+  LaunchOpts o;
+  o.staged = 2; o.account = true; o.stream = &sa;
+  rc = launch_fanout(b, st->payload, b->B, b->now, o);
+  follow_end(st, cpbus::kRound, ri);   // (a failed launch leaves the round's record pending: the next resolution reports it)
   return rc;
 } CPBUS_CATCH
 
 int cpbus_stream_progress(cpbus_stream_t* st, uint64_t* batches, size_t* offset, uint64_t* stalled_rounds) try {
   if (!st || !batches || !offset || !stalled_rounds) return CPBUS_EINVAL;
   cpbus* b = st->bus;
-  int rc = dev_guard(b); if (rc) return rc;
-  if ((rc = follow_resolve(b))) return rc;
+  int rc = enter(b); if (rc) return rc;
   *batches = st->get_seq; *offset = st->get_off; *stalled_rounds = st->stalled_rounds;
   return stream_error(b);
 } CPBUS_CATCH
@@ -1904,12 +1915,7 @@ int cpbus_stream_agree(cpbus_stream_t* st, size_t* m) try {
   if (!b->lossless || !st->offered) return CPBUS_EINVAL;
   int rc = dev_guard(b); if (rc) return rc;
   if ((rc = stream_error(b))) return rc;
-  if (!st->h_agree) {
-    StreamAgreeResult *h = nullptr, *d = nullptr;
-    CK(cudaHostAlloc((void**)&h, sizeof(StreamAgreeResult), cudaHostAllocMapped));
-    if (cudaHostGetDevicePointer((void**)&d, h, 0) != cudaSuccess) { cudaFreeHost(h); CK(cudaGetLastError()); return CPBUS_ECUDA; }
-    st->h_agree = h; st->d_agree = d;
-  }
+  if (!st->h_agree) CK(mapped_alloc(sizeof(StreamAgreeResult), &st->h_agree, &st->d_agree));
   if (!st->agree_done) CK(cudaEventCreateWithFlags(&st->agree_done, cudaEventDisableTiming));
   const unsigned long long r = st->agree_round + 1;
   stream_agree_kernel<<<1, kStreamMaxConsumers, 0, b->stream>>>(st->ack, st->n_consumers, r, b->stream_spin_us, st->d_agree, b->d_err);
@@ -1951,8 +1957,7 @@ int cpbus_drain(cpbus_t* b, uint32_t sub_id, cpbus_event* out, size_t cap, size_
   const uint32_t l = sub_id - b->cfg.sub_id_base;
   if (sub_id < b->cfg.sub_id_base || l >= b->n_next) return CPBUS_ENOENT;
   std::lock_guard<std::mutex> g(b->mu);
-  int rc = dev_guard(b); if (rc) return rc;
-  if ((rc = follow_resolve(b))) return rc;
+  int rc = enter(b); if (rc) return rc;
   uint64_t tail = 0, head = 0;
   uint64_t gone = 0;
   if ((rc = read_cursors(b, l, &tail, &head, &gone))) return rc;
@@ -1974,8 +1979,7 @@ int cpbus_drain_many(cpbus_t* b, uint32_t first_sub, uint32_t n, cpbus_event* ou
   const uint32_t l = first_sub - b->cfg.sub_id_base;
   if (first_sub < b->cfg.sub_id_base || (uint64_t)l + n > b->n_next) return CPBUS_ENOENT;
   std::lock_guard<std::mutex> g(b->mu);
-  int rc = dev_guard(b); if (rc) return rc;
-  if ((rc = follow_resolve(b))) return rc;
+  int rc = enter(b); if (rc) return rc;
   if (b->drain_cap < cap || b->drain_idx_cap < n) {   // device staging grows on demand and is kept
     if (b->drain_cap < cap) { cudaFree(b->d_drain); b->d_drain = nullptr; CK(cudaMalloc((void**)&b->d_drain, cap * sizeof(cpbus_event))); b->drain_cap = cap; }
     if (b->drain_idx_cap < n) { cudaFree(b->d_drain_idx); b->d_drain_idx = nullptr; CK(cudaMalloc((void**)&b->d_drain_idx, (size_t)n * sizeof(uint2) + 16)); b->drain_idx_cap = n; }
@@ -2012,8 +2016,7 @@ int cpbus_drain_ready(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start
   const uint32_t l = first_sub - b->cfg.sub_id_base;
   if (first_sub < b->cfg.sub_id_base || (uint64_t)l + n > b->n_next) return CPBUS_ENOENT;
   std::lock_guard<std::mutex> g(b->mu);
-  int rc = dev_guard(b); if (rc) return rc;
-  if ((rc = follow_resolve(b))) return rc;
+  int rc = enter(b); if (rc) return rc;
   const size_t rcap = std::min<size_t>(ready_cap, n);   // never more entries than mailboxes
   const uint32_t tiles = (n + kReadyTile - 1) / kReadyTile;
   // device staging grows on demand and is kept (the records share cpbus_drain_many's buffer)
@@ -2032,12 +2035,7 @@ int cpbus_drain_ready(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start
     CK(cudaMalloc((void**)&b->d_ready_lb, (kReadyLbOffset + (size_t)tiles) * sizeof(unsigned long long)));
     b->ready_lb_tiles = tiles;
   }
-  if (!b->h_ready_hdr) {
-    unsigned long long *h = nullptr, *d = nullptr;
-    CK(cudaHostAlloc((void**)&h, 64, cudaHostAllocMapped));
-    if (cudaHostGetDevicePointer((void**)&d, h, 0) != cudaSuccess) { cudaFreeHost(h); CK(cudaGetLastError()); return CPBUS_ECUDA; }
-    b->h_ready_hdr = h; b->d_ready_hdr = d;
-  }
+  if (!b->h_ready_hdr) CK(mapped_alloc(64, &b->h_ready_hdr, &b->d_ready_hdr));
   CK(cudaMemsetAsync(b->d_ready_lb + kReadyHdrWords, 0, (kReadyLbOffset - kReadyHdrWords + (size_t)tiles) * sizeof(unsigned long long),
                      b->stream));
   const uint32_t rot = start_sub - first_sub;
@@ -2091,8 +2089,7 @@ int cpbus_peek_window(cpbus_t* b, uint32_t sub_id, cpbus_event* out, size_t cap,
   const uint32_t l = sub_id - b->cfg.sub_id_base;
   if (sub_id < b->cfg.sub_id_base || l >= b->n_next) return CPBUS_ENOENT;
   std::lock_guard<std::mutex> g(b->mu);
-  int rc = dev_guard(b); if (rc) return rc;
-  if ((rc = follow_resolve(b))) return rc;
+  int rc = enter(b); if (rc) return rc;
   uint64_t tail = 0, head = 0;
   if ((rc = read_cursors(b, l, &tail, &head))) return rc;
   const size_t take = (size_t)std::min<uint64_t>(std::min<uint64_t>(tail, b->R), cap);
@@ -2106,8 +2103,7 @@ int cpbus_digest(cpbus_t* b, uint32_t first_sub, uint32_t n, cpbus_digest_t* out
   const uint32_t l = first_sub - b->cfg.sub_id_base;
   if (first_sub < b->cfg.sub_id_base || (uint64_t)l + n > b->n_next) return CPBUS_ENOENT;
   std::lock_guard<std::mutex> g(b->mu);
-  int rc = dev_guard(b); if (rc) return rc;
-  if ((rc = follow_resolve(b))) return rc;
+  int rc = enter(b); if (rc) return rc;
   std::vector<SubCtl> c(n);
   CK(cudaMemcpyAsync(c.data(), b->d_ctl + l, (size_t)n * sizeof(SubCtl), cudaMemcpyDeviceToHost, b->stream));
   CK(cudaStreamSynchronize(b->stream));
@@ -2223,8 +2219,7 @@ int cpbus_debug_events(cpbus_t* b, cpbus_event* out, size_t cap, size_t* n) try 
 int cpbus_stats(cpbus_t* b, cpbus_stats_t* out) try {
   if (!b || !out) return CPBUS_EINVAL;
   std::lock_guard<std::mutex> g(b->mu);
-  int rc = dev_guard(b); if (rc) return rc;
-  if ((rc = follow_resolve(b))) return rc;
+  int rc = enter(b); if (rc) return rc;
   CK(cudaMemsetAsync(&b->d_stats->overwritten, 0, sizeof(unsigned long long), b->stream));
   if (!b->lossless && b->n_next) {
     const uint32_t threads = 256, grid = std::min<uint32_t>((b->n_next + threads - 1) / threads, (uint32_t)b->sm_count * 4);
@@ -2251,8 +2246,7 @@ int cpbus_stats(cpbus_t* b, cpbus_stats_t* out) try {
 int cpbus_publish_counts(cpbus_t* b, cpbus_pair_count* out, size_t cap, size_t* n) try {
   if (!b || !n || (!out && cap)) return CPBUS_EINVAL;
   std::lock_guard<std::mutex> g(b->mu);
-  int rc = dev_guard(b); if (rc) return rc;
-  if ((rc = follow_resolve(b))) return rc;
+  int rc = enter(b); if (rc) return rc;
   std::unordered_map<uint64_t, uint64_t> merged;
   for (size_t i = 0; i < b->pub_pairs.keys.size(); i++) if (b->pub_pairs.keys[i]) merged[b->pub_pairs.keys[i] - 1] += b->pub_pairs.cnts[i];
   if (b->launch_seq) {

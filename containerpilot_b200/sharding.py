@@ -75,6 +75,14 @@ def _agree(bus, st) -> int | None:
         return None
 
 
+def _fanout_prefix(bus, st, n: int, now_ns: int, m: int) -> int:
+    """cpbus_stream_fanout_prefix of the agreed prefix m: nat.OK (batch complete) or nat.EAGAIN (records remain)"""
+    rc = bus.stream_fanout_prefix(st, n, now_ns, m)
+    if rc not in (nat.OK, nat.EAGAIN):
+        nat.check(rc, "cpbus_stream_fanout_prefix")
+    return rc
+
+
 def drive_rounds(queue_round, progress, T: int, pump=None, depth: int = 4) -> int:
     """Lossless followers told only the number of batches T: queue admission rounds until batch T is complete.
 
@@ -204,10 +212,7 @@ class ShardedBus(_ShardOps):
         m = _agree(self.bus, self._st)
         if m is None:
             return nat.EAGAIN                       # some rank stalled: nothing goes out anywhere
-        rc = self.bus.stream_fanout_prefix(self._st, n, now_ns, m)
-        if rc not in (nat.OK, nat.EAGAIN):
-            nat.check(rc, "cpbus_stream_fanout_prefix")
-        return rc
+        return _fanout_prefix(self.bus, self._st, n, now_ns, m)
 
     def follow(self, k: int = 1):
         """Enqueue fan-outs of the stream's next `k` batches on this rank without knowing their shapes: each launch takes
@@ -394,28 +399,29 @@ class LocalShardedBus:
             for g, (_, _, bus) in enumerate(self.shards):
                 nat.check(bus.stream_fanout(self._st[g], n, now_ns), "cpbus_stream_fanout")
             return nat.OK
-        if self.agree == "device":
-            return self._fanout_device_agree(n, now_ns)
-        m = None
-        for g, (_, _, bus) in enumerate(self.shards):
-            try:
-                p = bus.stream_admit(self._st[g], n, now_ns)
-            except nat.CpbusError as ex:
-                if ex.status != nat.EAGAIN:
-                    raise
-                return nat.EAGAIN                   # nothing can go out on this shard, so nothing goes out anywhere
-            m = p if m is None else min(m, p)
+        m = self._agree_device(n, now_ns) if self.agree == "device" else self._agree_host(n, now_ns)
+        if m is None:
+            return nat.EAGAIN                       # some shard stalled: nothing goes out anywhere
         rc = nat.OK
         for g, (_, _, bus) in enumerate(self.shards):
-            r = bus.stream_fanout_prefix(self._st[g], n, now_ns, m)
-            if r not in (nat.OK, nat.EAGAIN):
-                nat.check(r, "cpbus_stream_fanout_prefix")
-            rc = r
+            rc = _fanout_prefix(bus, self._st[g], n, now_ns, m)
         return rc
 
-    def _fanout_device_agree(self, n: int, now_ns: int) -> int:
+    def _agree_host(self, n: int, now_ns: int) -> int | None:
+        """The shortest prefix any shard admits, or None at the first shard that stalls (the later ones are not admitted:
+        their room bounds and admission counters stay as they are)."""
+        m = None
+        for g, (_, _, bus) in enumerate(self.shards):
+            p, stalled = _admit_or_stall(bus, self._st[g], n, now_ns)
+            if stalled:
+                return None
+            m = p if m is None else min(m, p)
+        return m
+
+    def _agree_device(self, n: int, now_ns: int) -> int | None:
         """One admission round through the publisher's memory (what `ShardedBus(lossless=True)` does on each rank): every
-        shard offers before any shard waits, and every shard agrees, so the round advances in lockstep."""
+        shard offers before any shard waits, and every shard agrees, so the round advances in lockstep.  The agreed prefix,
+        or None when some shard stalled."""
         offers = []
         for g, (_, _, bus) in enumerate(self.shards):
             offers.append(_admit_or_stall(bus, self._st[g], n, now_ns))
@@ -426,15 +432,7 @@ class LocalShardedBus:
         self.last_round = (offers, agreed)
         if len(set(agreed)) != 1:                   # every agree kernel read the same words
             raise RuntimeError(f"shards agreed on different prefixes: {agreed}")
-        if agreed[0] is None:
-            return nat.EAGAIN
-        rc = nat.OK
-        for g, (_, _, bus) in enumerate(self.shards):
-            r = bus.stream_fanout_prefix(self._st[g], n, now_ns, agreed[g])
-            if r not in (nat.OK, nat.EAGAIN):
-                nat.check(r, "cpbus_stream_fanout_prefix")
-            rc = r
-        return rc
+        return agreed[0]
 
     def follow(self, g: int, k: int = 1):
         """Enqueue fan-outs of the stream's next `k` batches on shard `g` without their shapes (`cpbus_stream_fanout_next`)."""
