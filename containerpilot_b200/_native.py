@@ -128,6 +128,14 @@ SYMBOLS = {
     "cpbus_record_hash": (C.c_uint64, [_P(Event)]),
     "cpbus_digest_multiplier": (C.c_uint64, []),
 }
+# the group (one handle over several shards): cpbus_group_<name> takes the arguments of cpbus_<name>
+GROUP_CALLS = ("intern", "intern_ephemeral", "source", "subscribe", "subscribe_many", "subscribe_pairs", "subscribe_pairs_many",
+               "unsubscribe", "set_mask", "timer_add", "timer_add_many", "timer_cancel", "publish", "send", "advance", "flush",
+               "sync", "drain", "drain_ready", "consume_all", "peek_window", "digest", "digest_fold", "debug_events", "stats",
+               "publish_counts")
+SYMBOLS["cpbus_group_create"] = (C.c_int, [_P(Config), C.c_void_p, C.c_uint32, _P(C.c_void_p)])
+SYMBOLS["cpbus_group_destroy"] = (C.c_int, [C.c_void_p])
+SYMBOLS.update({f"cpbus_group_{name}": SYMBOLS[f"cpbus_{name}"] for name in GROUP_CALLS})
 
 _lib = None
 

@@ -730,9 +730,8 @@ uint64_t cpbus_record_hash(const cpbus_event* e) {
 }
 uint64_t cpbus_digest_multiplier(void) { return kDigestP; }
 
-int cpbus_create(const cpbus_config* cfg, cpbus_t** out) try {
-  if (!cfg || !out) return CPBUS_EINVAL;
-  *out = nullptr;
+// The checks cpbus_create makes of a config (cpbus_group_create makes them of the total); R and B get the defaults applied.
+static int config_check(const cpbus_config* cfg, uint32_t* R_out, uint32_t* B_out) {
   const uint32_t R = cfg->ring_cap ? cfg->ring_cap : 1024;
   const uint32_t B = cfg->batch_cap ? cfg->batch_cap : std::min(256u, R / 2);
   const uint32_t K = cfg->timers_per_sub;
@@ -740,6 +739,16 @@ int cpbus_create(const cpbus_config* cfg, cpbus_t** out) try {
   if (!(K == 0 || K == 1 || K == 2 || K == 4 || K == 8)) return CPBUS_EINVAL;
   if ((uint64_t)cfg->n_max_subs * std::max(K, 1u) > kTimerSlotMask) return CPBUS_EINVAL;   // timer ids keep 6 generation bits
   if (cfg->store_path > CPBUS_STORE_BULK) return CPBUS_EINVAL;
+  *R_out = R; *B_out = B;
+  return CPBUS_OK;
+}
+
+int cpbus_create(const cpbus_config* cfg, cpbus_t** out) try {
+  if (!cfg || !out) return CPBUS_EINVAL;
+  *out = nullptr;
+  uint32_t R = 0, B = 0;
+  if (config_check(cfg, &R, &B)) return CPBUS_EINVAL;
+  const uint32_t K = cfg->timers_per_sub;
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
     snprintf(g_cuda_err, sizeof(g_cuda_err), "no CUDA device visible");
@@ -2008,10 +2017,23 @@ int cpbus_drain_many(cpbus_t* b, uint32_t first_sub, uint32_t n, cpbus_event* ou
 // Sparse drain: only the mailboxes that hold records.  The scan kernel reads each control block of the range once and
 // writes the ready list of the taken prefix; the gather kernel copies their runs and hands the 3-word header to the host
 // through mapped pinned memory.  One sync reads the header; a second one follows the two copies sized by it.
+// The body of cpbus_drain_ready, without its cap >= ring_cap check: a group hands each shard the cap its earlier shards
+// left, which can be smaller.  *all_taken: every ready mailbox of the range was taken (then *next_sub = start_sub).
+static int drain_ready_impl(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start_sub, cpbus_event* out, size_t cap,
+                            cpbus_ready* ready, size_t ready_cap, size_t* n_ready, size_t* total, uint32_t* next_sub,
+                            bool* all_taken);
+
 int cpbus_drain_ready(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start_sub, cpbus_event* out, size_t cap,
                       cpbus_ready* ready, size_t ready_cap, size_t* n_ready, size_t* total, uint32_t* next_sub) try {
   if (!b || !out || !ready || !n_ready || !total || !next_sub || !n || !ready_cap) return CPBUS_EINVAL;
   if (cap < b->R || cap > 0xFFFFFFFFull) return CPBUS_EINVAL;   // cap >= ring_cap: a ready mailbox always fits an empty call
+  bool all_taken = false;
+  return drain_ready_impl(b, first_sub, n, start_sub, out, cap, ready, ready_cap, n_ready, total, next_sub, &all_taken);
+} CPBUS_CATCH
+
+static int drain_ready_impl(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start_sub, cpbus_event* out, size_t cap,
+                            cpbus_ready* ready, size_t ready_cap, size_t* n_ready, size_t* total, uint32_t* next_sub,
+                            bool* all_taken) {
   if (start_sub < first_sub || start_sub - first_sub >= n) return CPBUS_EINVAL;
   const uint32_t l = first_sub - b->cfg.sub_id_base;
   if (first_sub < b->cfg.sub_id_base || (uint64_t)l + n > b->n_next) return CPBUS_ENOENT;
@@ -2056,9 +2078,10 @@ int cpbus_drain_ready(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start
     CK(cudaStreamSynchronize(b->stream));
   }
   *n_ready = nr; *total = tot;
+  *all_taken = cut >= n;
   *next_sub = cut >= n ? start_sub : first_sub + (uint32_t)((rot + cut) % n);
   return CPBUS_OK;
-} CPBUS_CATCH
+}
 
 // Device-side consumer: every mailbox of this shard is read to the end and its records are discarded.
 int cpbus_consume_all(cpbus_t* b) try {
@@ -2267,6 +2290,558 @@ int cpbus_device_ptrs(cpbus_t* b, void** ring, void** ctl) try {
   if (!b) return CPBUS_EINVAL;
   if (ring) *ring = b->d_ring;
   if (ctl) *ctl = b->d_ctl;
+  return CPBUS_OK;
+} CPBUS_CATCH
+
+// ---- the group: one bus handle over the GPUs of a box (include/cpbus.h: cpbus_group_*) ----------------------------------
+// The group keeps the host state a single bus keeps for the whole id space — staged records, seq, clock, last launched
+// watermark, the timer table that sets the clock window, debug ring and publish counts — and makes the flushes the single
+// bus makes (flush_staged, stage_one, cpbus_advance).  A flush becomes one RAW stream batch that every shard fans out in
+// full: in lossless mode the group first runs the single bus's admission (admit) on every shard and puts only the prefix
+// every shard can take, with the single bus's partial watermark.  (cpbus_stream_admit would hold a batch back until the
+// ticks due by its watermark fit too, where a partial cpbus_flush delivers the records and stalls on the ticks alone.)
+// Shard clocks: a shard's clock is its last launched watermark; a shard without timers is moved to the group clock with
+// cpbus_advance right before a timer is armed on it (no launch: it has no timer window), so every shard's `now + period`
+// is the single bus's.  A shard with timers already has the group clock there (the group has just flushed at `now`).
+struct cpbus_group {
+  std::vector<cpbus*> shards;
+  std::vector<cpbus_stream*> streams;   // streams[0] owns the ring (shard 0), the others are attached
+  std::vector<uint32_t> first;          // global index (sub_id_base not applied) of each shard's subscriber 0; + a sentinel
+  uint32_t base = 0, N = 0, B = 0, K = 0;
+  bool lossless = false;
+  uint32_t n_next = 0, n_active = 0;
+  std::vector<cpbus_event> staged;      // B records
+  size_t n_staged = 0;
+  uint64_t now = 0, last_watermark = 0, seq = 0;
+  // the single bus's timer bookkeeping over global slots (subscriber * K + k): what sets the clock window and when an empty
+  // flush launches
+  struct Slot { bool active = false, oneshot = false; uint64_t next_due = 0; };
+  std::vector<Slot> timers;             // N * K, allocated on first use (as the single bus's h_timers)
+  std::vector<size_t> oneshot_idx;
+  uint32_t n_timers = 0;
+  uint64_t min_period = UINT64_MAX;
+  int dbg_head = -1, dbg_tail = 0;
+  cpbus_event dbg[10]{};
+  PairCounter pub_pairs;
+  uint64_t publishes = 0, by_code[CPBUS_N_CODES] = {};
+};
+
+static uint32_t group_shard_of(const cpbus_group* g, uint32_t index) {   // index < N
+  return (uint32_t)(std::upper_bound(g->first.begin(), g->first.end(), index) - g->first.begin()) - 1;
+}
+
+static uint64_t group_window(const cpbus_group* g) {   // max_window of the single bus
+  if (!g->K || g->n_timers == 0 || g->min_period == UINT64_MAX) return UINT64_MAX;
+  const uint64_t J = 32u / g->K;
+  return g->min_period > UINT64_MAX / J ? UINT64_MAX : g->min_period * J;
+}
+
+// retire_oneshots of the single bus, for the group's table and, at the same moment, every shard's own: a shard's timer
+// count (and so its window) then never lags the group's
+static void group_retire(cpbus_group* g) {
+  size_t keep = 0;
+  for (size_t i = 0; i < g->oneshot_idx.size(); i++) {
+    cpbus_group::Slot& t = g->timers[g->oneshot_idx[i]];
+    if (t.active && t.oneshot && t.next_due <= g->last_watermark) { t.active = false; g->n_timers--; continue; }
+    if (t.active && t.oneshot) g->oneshot_idx[keep++] = g->oneshot_idx[i];
+  }
+  g->oneshot_idx.resize(keep);
+  if (g->n_timers == 0) g->min_period = UINT64_MAX;
+  for (cpbus* s : g->shards) if (!s->h_timers.empty()) retire_oneshots(s, s->last_watermark);
+}
+
+// One launch of the single bus: the same early returns as launch_fanout, otherwise one stream batch on every shard.
+static int group_launch(cpbus_group* g, const cpbus_event* ev, uint32_t n, uint64_t w) {
+  if (g->n_next == 0) return CPBUS_OK;
+  if (n == 0 && g->n_timers == 0) return CPBUS_OK;
+  int rc = cpbus_stream_put(g->streams[0], ev, n, w, CPBUS_PUT_RAW);
+  if (rc) return rc;
+  for (cpbus_stream* st : g->streams)   // the whole batch: already admitted on every shard, so it completes in one launch
+    if ((rc = cpbus_stream_fanout_prefix(st, n, w, n))) return rc;
+  g->last_watermark = w;
+  return CPBUS_OK;
+}
+
+// Lossless admission of the staged records on every shard (admit), the single bus's verdict being the conjunction and its
+// prefix the minimum.  The records reach a shard's device only when its room bound cannot prove the fit.
+static int group_admit(cpbus_group* g, uint32_t n, uint64_t w, bool* ok, uint32_t* m) {
+  *ok = true; *m = n;
+  for (cpbus* s : g->shards) {
+    if (admit_fits(s, n, w)) continue;
+    int rc = dev_guard(s); if (rc) return rc;
+    if (n) CK(cudaMemcpyAsync(s->d_admit_batch, g->staged.data(), (size_t)n * sizeof(cpbus_event), cudaMemcpyHostToDevice, s->stream));
+    bool ok_s = true;
+    uint32_t m_s = n;
+    if ((rc = admit_pass(s, s->d_admit_batch, n, w, &ok_s, &m_s))) return rc;
+    if (!ok_s) { *ok = false; *m = std::min(*m, m_s); }
+  }
+  return CPBUS_OK;
+}
+
+// flush_staged of the single bus
+static int group_flush(cpbus_group* g, uint64_t w) {
+  const uint32_t n = (uint32_t)g->n_staged;
+  if (n == 0 && g->n_timers == 0) { g->last_watermark = std::max(g->last_watermark, w); return CPBUS_OK; }
+  if (n == 0 && w == g->last_watermark) return CPBUS_OK;
+  bool ok = true;
+  uint32_t m = n;
+  int rc;
+  if (g->lossless && (rc = group_admit(g, n, w, &ok, &m))) return rc;
+  if (!ok) {
+    if (m == 0) return CPBUS_EAGAIN;
+    if ((rc = group_launch(g, g->staged.data(), m, g->staged[m - 1].ts_ns))) return rc;
+    std::copy(g->staged.begin() + m, g->staged.begin() + n, g->staged.begin());
+    g->n_staged = n - m;
+    for (cpbus* s : g->shards) { s->room_lb = 0; s->st.admit_partial++; }
+    return CPBUS_EAGAIN;
+  }
+  if ((rc = group_launch(g, g->staged.data(), n, w))) return rc;
+  g->n_staged = 0;
+  return CPBUS_OK;
+}
+
+// stage_one of the single bus: seq is one ordinal over publishes and sends
+static int group_stage(cpbus_group* g, uint32_t code, uint32_t source_id, uint32_t target, uint32_t flags) {
+  if (g->n_staged == g->B) { const int rc = group_flush(g, g->now); if (rc) return rc; }
+  cpbus_event& e = g->staged[g->n_staged++];
+  e.seq = g->seq++; e.ts_ns = g->now; e.code = code; e.source_id = source_id; e.target = target; e.flags = flags;
+  return CPBUS_OK;
+}
+
+// the owning shard of global id `sub_id` and its local index; false: not a subscribed-so-far id
+static bool group_locate(const cpbus_group* g, uint32_t sub_id, cpbus** s, uint32_t* l) {
+  const uint32_t i = sub_id - g->base;
+  if (sub_id < g->base || i >= g->n_next) return false;
+  const uint32_t k = group_shard_of(g, i);
+  *s = g->shards[k]; *l = i - g->first[k];
+  return true;
+}
+
+// Arm timers on shard s: a shard without timers takes the group clock first (cpbus_advance launches nothing there).
+static int group_shard_clock(cpbus_group* g, cpbus* s) {
+  if (s->now == g->now) return CPBUS_OK;
+  if (s->n_timers) return CPBUS_ECUDA;   // cannot happen: the group has just flushed at now, which moved this shard there
+  return cpbus_advance(s, g->now);
+}
+
+int cpbus_group_destroy(cpbus_group_t* g) try {
+  if (!g) return CPBUS_EINVAL;
+  for (size_t i = g->streams.size(); i-- > 0;) if (g->streams[i]) cpbus_stream_close(g->streams[i]);   // importers first
+  for (cpbus* s : g->shards) if (s) cpbus_destroy(s);
+  delete g;
+  return CPBUS_OK;
+} CPBUS_CATCH
+
+int cpbus_group_create(const cpbus_config* cfg, const int32_t* devices, uint32_t n_devices, cpbus_group_t** out) try {
+  if (!cfg || !devices || !n_devices || !out || cfg->stream || n_devices > kStreamMaxConsumers) return CPBUS_EINVAL;
+  *out = nullptr;
+  uint32_t R = 0, B = 0;
+  if (config_check(cfg, &R, &B) || cfg->n_max_subs < n_devices) return CPBUS_EINVAL;
+  cpbus_group* g = new (std::nothrow) cpbus_group();
+  if (!g) return CPBUS_ENOMEM;
+  g->base = cfg->sub_id_base; g->N = cfg->n_max_subs; g->B = B; g->K = cfg->timers_per_sub;
+  g->lossless = cfg->flags & CPBUS_CFG_LOSSLESS;
+  g->staged.resize(B);
+  auto fail = [&](int code) { cpbus_group_destroy(g); return code; };
+  const uint32_t each = g->N / n_devices, extra = g->N % n_devices;   // sharding.shard_range
+  for (uint32_t k = 0; k < n_devices; k++) {
+    const uint32_t first = k * each + std::min(k, extra), count = each + (k < extra ? 1u : 0u);
+    cpbus_config c = *cfg;
+    c.n_max_subs = count; c.device = devices[k]; c.sub_id_base = g->base + first;
+    cpbus* s = nullptr;
+    const int rc = cpbus_create(&c, &s);
+    if (rc) return fail(rc);
+    g->shards.push_back(s); g->first.push_back(first);
+  }
+  g->first.push_back(g->N);
+  unsigned char handle[64];
+  cpbus_stream* st0 = nullptr;
+  int rc = cpbus_stream_create(g->shards[0], 8, n_devices, &st0, handle);
+  if (rc) return fail(rc);
+  g->streams.push_back(st0);
+  for (uint32_t k = 1; k < n_devices; k++) {
+    cpbus_stream* st = nullptr;
+    if ((rc = cpbus_stream_attach(g->shards[k], st0, k, &st))) return fail(rc);
+    g->streams.push_back(st);
+  }
+  *out = g;
+  return CPBUS_OK;
+} CPBUS_CATCH
+
+int cpbus_group_intern(cpbus_group_t* g, const char* s, size_t len, uint32_t* source_id) try {
+  return g ? cpbus_intern(g->shards[0], s, len, source_id) : CPBUS_EINVAL;
+} CPBUS_CATCH
+int cpbus_group_intern_ephemeral(cpbus_group_t* g, const char* s, size_t len, uint32_t* source_id) try {
+  return g ? cpbus_intern_ephemeral(g->shards[0], s, len, source_id) : CPBUS_EINVAL;
+} CPBUS_CATCH
+int cpbus_group_source(cpbus_group_t* g, uint32_t source_id, char* out, size_t cap, size_t* len) try {
+  return g ? cpbus_source(g->shards[0], source_id, out, cap, len) : CPBUS_EINVAL;
+} CPBUS_CATCH
+
+// Subscribers [n_next, n_next + n) across the shards that own them; fn(shard, offset into the caller's arrays, count).
+extern "C++" {
+template <class Fn>
+static int group_each_range(cpbus_group* g, uint32_t first_index, uint32_t n, Fn&& fn) {
+  for (uint32_t done = 0; done < n;) {
+    const uint32_t i = first_index + done, k = group_shard_of(g, i);
+    const uint32_t cnt = std::min(n - done, g->first[k + 1] - i);
+    const int rc = fn(g->shards[k], i - g->first[k], done, cnt);
+    if (rc) return rc;
+    done += cnt;
+  }
+  return CPBUS_OK;
+}
+}
+
+int cpbus_group_subscribe_many(cpbus_group_t* g, const uint32_t* masks, uint32_t n, uint32_t* first_sub_id) try {
+  if (!g || !n) return CPBUS_EINVAL;
+  if ((uint64_t)g->n_next + n > g->N) return CPBUS_ENOSPC;
+  int rc = group_flush(g, g->now); if (rc) return rc;
+  const uint32_t first = g->n_next;
+  rc = group_each_range(g, first, n, [&](cpbus* s, uint32_t, uint32_t off, uint32_t cnt) -> int {
+    uint32_t id = 0;
+    return cpbus_subscribe_many(s, masks ? masks + off : nullptr, cnt, &id);
+  });
+  if (rc) return rc;
+  g->n_next += n; g->n_active += n;
+  if (first_sub_id) *first_sub_id = g->base + first;
+  return CPBUS_OK;
+} CPBUS_CATCH
+
+int cpbus_group_subscribe(cpbus_group_t* g, uint32_t mask, uint32_t* sub_id) { return cpbus_group_subscribe_many(g, &mask, 1, sub_id); }
+
+int cpbus_group_subscribe_pairs(cpbus_group_t* g, uint32_t mask, const cpbus_pair* pairs, uint32_t n_pairs, uint32_t* sub_id) try {
+  if (!g || n_pairs > CPBUS_MAX_PAIRS || (n_pairs && !pairs)) return CPBUS_EINVAL;
+  for (uint32_t j = 0; j < n_pairs; j++) if (pairs[j].code >= CPBUS_N_CODES) return CPBUS_EINVAL;
+  if (g->n_next >= g->N) return CPBUS_ENOSPC;
+  int rc = group_flush(g, g->now); if (rc) return rc;
+  const uint32_t k = group_shard_of(g, g->n_next);
+  uint32_t id = 0;
+  if ((rc = cpbus_subscribe_pairs(g->shards[k], mask, pairs, n_pairs, &id))) return rc;
+  g->n_next++; g->n_active++;
+  if (sub_id) *sub_id = id;
+  return CPBUS_OK;
+} CPBUS_CATCH
+
+int cpbus_group_subscribe_pairs_many(cpbus_group_t* g, const uint32_t* masks, const cpbus_pair* pairs, const uint32_t* n_pairs,
+                                     uint32_t n, uint32_t* first_sub_id) try {
+  if (!g || !n || !masks || !pairs || !n_pairs) return CPBUS_EINVAL;
+  for (uint32_t i = 0; i < n; i++) {
+    if (n_pairs[i] > CPBUS_MAX_PAIRS) return CPBUS_EINVAL;
+    for (uint32_t j = 0; j < n_pairs[i]; j++) if (pairs[(size_t)i * CPBUS_MAX_PAIRS + j].code >= CPBUS_N_CODES) return CPBUS_EINVAL;
+  }
+  if ((uint64_t)g->n_next + n > g->N) return CPBUS_ENOSPC;
+  int rc = group_flush(g, g->now); if (rc) return rc;
+  const uint32_t first = g->n_next;
+  rc = group_each_range(g, first, n, [&](cpbus* s, uint32_t, uint32_t off, uint32_t cnt) -> int {
+    uint32_t id = 0;
+    return cpbus_subscribe_pairs_many(s, masks + off, pairs + (size_t)off * CPBUS_MAX_PAIRS, n_pairs + off, cnt, &id);
+  });
+  if (rc) return rc;
+  g->n_next += n; g->n_active += n;
+  if (first_sub_id) *first_sub_id = g->base + first;
+  return CPBUS_OK;
+} CPBUS_CATCH
+
+int cpbus_group_unsubscribe(cpbus_group_t* g, uint32_t sub_id) try {
+  if (!g) return CPBUS_EINVAL;
+  cpbus* s = nullptr; uint32_t l = 0;
+  if (!group_locate(g, sub_id, &s, &l)) return CPBUS_ENOENT;
+  int rc = group_flush(g, g->now); if (rc) return rc;
+  if ((rc = cpbus_unsubscribe(s, sub_id))) return rc;
+  if (g->K && !g->timers.empty())
+    for (uint32_t k = 0; k < g->K; k++) {
+      cpbus_group::Slot& t = g->timers[(size_t)(sub_id - g->base) * g->K + k];
+      if (t.active) { t.active = false; g->n_timers--; }
+    }
+  g->n_active--;
+  return CPBUS_OK;
+} CPBUS_CATCH
+
+int cpbus_group_set_mask(cpbus_group_t* g, uint32_t sub_id, uint32_t mask) try {
+  if (!g) return CPBUS_EINVAL;
+  cpbus* s = nullptr; uint32_t l = 0;
+  if (!group_locate(g, sub_id, &s, &l)) return CPBUS_ENOENT;
+  if (!s->h_active[l]) return CPBUS_ECLOSED;
+  const int rc = group_flush(g, g->now); if (rc) return rc;
+  return cpbus_set_mask(s, sub_id, mask);
+} CPBUS_CATCH
+
+int cpbus_group_timer_add(cpbus_group_t* g, uint32_t sub_id, uint64_t period_ns, uint32_t source_id, int oneshot, uint32_t* timer_id) try {
+  if (!g || !period_ns) return CPBUS_EINVAL;
+  if (!g->K) return CPBUS_ENOSPC;
+  cpbus* s = nullptr; uint32_t l = 0;
+  if (!group_locate(g, sub_id, &s, &l)) return CPBUS_ENOENT;
+  int rc = group_flush(g, g->now); if (rc) return rc;
+  if (g->timers.empty()) g->timers.resize((size_t)g->N * g->K);
+  group_retire(g);
+  if (!s->h_active[l]) return CPBUS_ECLOSED;
+  if ((rc = group_shard_clock(g, s))) return rc;
+  uint32_t id = 0;
+  if ((rc = cpbus_timer_add(s, sub_id, period_ns, source_id, oneshot, &id))) return rc;
+  const uint32_t shard_base_slot = (sub_id - l - g->base) * g->K;   // global slot of the shard's slot 0
+  const size_t slot = (size_t)(id & kTimerSlotMask) + shard_base_slot;
+  cpbus_group::Slot& t = g->timers[slot];
+  t.active = true; t.oneshot = oneshot != 0; t.next_due = g->now + period_ns;
+  g->n_timers++;
+  if (!oneshot) g->min_period = std::min(g->min_period, period_ns);
+  else g->oneshot_idx.push_back(slot);
+  if (timer_id) *timer_id = (uint32_t)slot | (id & ~kTimerSlotMask);
+  return CPBUS_OK;
+} CPBUS_CATCH
+
+int cpbus_group_timer_add_many(cpbus_group_t* g, uint32_t first_sub, uint32_t n, uint64_t period_ns, const uint32_t* source_ids,
+                               uint32_t source_id0, int oneshot) try {
+  if (!g || !period_ns || !n) return CPBUS_EINVAL;
+  if (!g->K) return CPBUS_ENOSPC;
+  const uint32_t i0 = first_sub - g->base;
+  if (first_sub < g->base || (uint64_t)i0 + n > g->n_next) return CPBUS_ENOENT;
+  int rc = group_flush(g, g->now); if (rc) return rc;
+  if (g->timers.empty()) g->timers.resize((size_t)g->N * g->K);
+  group_retire(g);
+  // the single bus checks every subscriber before it arms any
+  for (uint32_t i = 0; i < n; i++) {
+    cpbus* s = nullptr; uint32_t l = 0;
+    group_locate(g, first_sub + i, &s, &l);
+    if (!s->h_active[l]) return CPBUS_ECLOSED;
+    if (g->timers[(size_t)(i0 + i) * g->K].active) return CPBUS_ENOSPC;
+  }
+  rc = group_each_range(g, i0, n, [&](cpbus* s, uint32_t l, uint32_t off, uint32_t cnt) -> int {
+    const int rc_clock = group_shard_clock(g, s);
+    if (rc_clock) return rc_clock;
+    return cpbus_timer_add_many(s, s->cfg.sub_id_base + l, cnt, period_ns, source_ids ? source_ids + off : nullptr,
+                                source_id0 + off, oneshot);
+  });
+  if (rc) return rc;
+  for (uint32_t i = 0; i < n; i++) {
+    const size_t slot = (size_t)(i0 + i) * g->K;
+    cpbus_group::Slot& t = g->timers[slot];
+    t.active = true; t.oneshot = oneshot != 0; t.next_due = g->now + period_ns;
+    if (oneshot) g->oneshot_idx.push_back(slot);
+  }
+  g->n_timers += n;
+  if (!oneshot) g->min_period = std::min(g->min_period, period_ns);
+  return CPBUS_OK;
+} CPBUS_CATCH
+
+int cpbus_group_timer_cancel(cpbus_group_t* g, uint32_t timer_id) try {
+  if (!g) return CPBUS_EINVAL;
+  if (!g->K || g->timers.empty()) return CPBUS_ENOENT;
+  const uint32_t slot = timer_id & kTimerSlotMask, i = slot / g->K;
+  if (i >= g->n_next) return CPBUS_ENOENT;
+  int rc = group_flush(g, g->now); if (rc) return rc;
+  group_retire(g);
+  const uint32_t k = group_shard_of(g, i);
+  const uint32_t local = (slot - g->first[k] * g->K) | (timer_id & ~kTimerSlotMask);
+  if ((rc = cpbus_timer_cancel(g->shards[k], local))) return rc;
+  g->timers[slot].active = false; g->n_timers--;
+  if (g->n_timers == 0) g->min_period = UINT64_MAX;
+  return CPBUS_OK;
+} CPBUS_CATCH
+
+static void group_dbg_put(cpbus_group* g, const cpbus_event& e) {   // dbg_ring_put
+  g->dbg[(g->dbg_head + 1) % 10] = e;
+  const int old = g->dbg_head;
+  g->dbg_head = (g->dbg_head + 1) % 10;
+  if (old != -1 && g->dbg_head == g->dbg_tail) g->dbg_tail = (g->dbg_tail + 1) % 10;
+}
+
+int cpbus_group_publish(cpbus_group_t* g, const cpbus_event* ev, size_t n) try {
+  if (!g || (!ev && n)) return CPBUS_EINVAL;
+  auto dbg_tail = [&](size_t published) {   // as cpbus_publish: the last 10 of the burst
+    for (size_t j = published > 10 ? published - 10 : 0; j < published; j++) {
+      cpbus_event e{};
+      e.seq = g->seq - (published - j); e.ts_ns = g->now; e.code = ev[j].code; e.source_id = ev[j].source_id; e.target = CPBUS_TARGET_ALL;
+      group_dbg_put(g, e);
+    }
+  };
+  for (size_t i = 0; i < n; i++) if (ev[i].code >= CPBUS_N_CODES) return CPBUS_EINVAL;
+  for (size_t i = 0; i < n; i++) {
+    const uint32_t code = ev[i].code;
+    const int rc = group_stage(g, code, ev[i].source_id, CPBUS_TARGET_ALL, 0);
+    if (rc) { dbg_tail(i); return rc; }
+    if (code != CPBUS_METRIC) { g->by_code[code]++; g->pub_pairs.add(((uint64_t)code << 32) | ev[i].source_id, 1); }
+    g->publishes++;
+  }
+  dbg_tail(n);
+  return CPBUS_OK;
+} CPBUS_CATCH
+
+int cpbus_group_send(cpbus_group_t* g, uint32_t sub_id, const cpbus_event* ev) try {
+  if (!g || !ev || ev->code >= CPBUS_N_CODES) return CPBUS_EINVAL;
+  cpbus* s = nullptr; uint32_t l = 0;
+  if (!group_locate(g, sub_id, &s, &l)) return CPBUS_ENOENT;
+  if (!s->h_active[l]) return CPBUS_ECLOSED;
+  const int rc = group_stage(g, ev->code, ev->source_id, sub_id, CPBUS_F_UNICAST);
+  if (rc) return rc;
+  g->publishes++;
+  return CPBUS_OK;
+} CPBUS_CATCH
+
+int cpbus_group_advance(cpbus_group_t* g, uint64_t now_ns) try {
+  if (!g) return CPBUS_EINVAL;
+  if (now_ns < g->now) return CPBUS_EORDER;
+  if (now_ns == g->now) return CPBUS_OK;
+  const uint64_t win = group_window(g);   // the single bus's grid: a stream batch never steps past a shard's window
+  while (win != UINT64_MAX && now_ns - g->last_watermark > win) {
+    g->now = g->last_watermark + win;
+    const int rc = group_flush(g, g->now); if (rc) return rc;
+  }
+  g->now = now_ns;
+  return CPBUS_OK;
+} CPBUS_CATCH
+
+int cpbus_group_flush(cpbus_group_t* g) try {
+  return g ? group_flush(g, g->now) : CPBUS_EINVAL;
+} CPBUS_CATCH
+
+int cpbus_group_sync(cpbus_group_t* g) try {
+  if (!g) return CPBUS_EINVAL;
+  for (cpbus* s : g->shards) { const int rc = cpbus_sync(s); if (rc) return rc; }
+  return CPBUS_OK;
+} CPBUS_CATCH
+
+int cpbus_group_drain(cpbus_group_t* g, uint32_t sub_id, cpbus_event* out, size_t cap, size_t* n, uint64_t* lost) try {
+  if (!g || !n || (!out && cap)) return CPBUS_EINVAL;
+  cpbus* s = nullptr; uint32_t l = 0;
+  if (!group_locate(g, sub_id, &s, &l)) return CPBUS_ENOENT;
+  return cpbus_drain(s, sub_id, out, cap, n, lost);
+} CPBUS_CATCH
+
+// The first ready mailbox of [a, a + cnt) on shard s (cnt when none): where a walk with no room left stops.
+static int group_first_ready(cpbus* s, uint32_t l, uint32_t cnt, uint32_t* at) {
+  std::vector<SubCtl> c(cnt);
+  int rc = dev_guard(s); if (rc) return rc;
+  CK(cudaMemcpyAsync(c.data(), s->d_ctl + l, (size_t)cnt * sizeof(SubCtl), cudaMemcpyDeviceToHost, s->stream));
+  CK(cudaStreamSynchronize(s->stream));
+  *at = cnt;
+  for (uint32_t i = 0; i < cnt; i++) if (c[i].tail > c[i].head) { *at = i; break; }
+  return CPBUS_OK;
+}
+
+// The cyclic walk of cpbus_drain_ready over the shards: each piece of the walk that lies on one shard is drained there with
+// the cap and ready entries still left, and the walk stops at the first mailbox that does not fit, as the single call does.
+int cpbus_group_drain_ready(cpbus_group_t* g, uint32_t first_sub, uint32_t n, uint32_t start_sub, cpbus_event* out, size_t cap,
+                            cpbus_ready* ready, size_t ready_cap, size_t* n_ready, size_t* total, uint32_t* next_sub) try {
+  if (!g || !out || !ready || !n_ready || !total || !next_sub || !n || !ready_cap) return CPBUS_EINVAL;
+  if (cap < g->shards[0]->R || cap > 0xFFFFFFFFull) return CPBUS_EINVAL;
+  if (start_sub < first_sub || start_sub - first_sub >= n) return CPBUS_EINVAL;
+  const uint32_t i0 = first_sub - g->base;
+  if (first_sub < g->base || (uint64_t)i0 + n > g->n_next) return CPBUS_ENOENT;
+  size_t nr = 0, tot = 0, ready_left = std::min<size_t>(ready_cap, n);
+  const uint32_t rot = start_sub - first_sub;
+  *next_sub = start_sub;
+  for (uint32_t done = 0; done < n;) {
+    const uint32_t i = i0 + (rot + done) % n;                       // global index of the walk's next mailbox
+    const uint32_t k = group_shard_of(g, i);
+    const uint32_t wrap = i0 + n - i;                               // the walk wraps to first_sub after this many
+    const uint32_t cnt = std::min({n - done, g->first[k + 1] - i, wrap});
+    cpbus* s = g->shards[k];
+    const uint32_t l = i - g->first[k], a = g->base + i;
+    if (ready_left == 0 || tot == cap) {                           // no room: the next ready mailbox ends the walk
+      uint32_t at = cnt;
+      const int rc = group_first_ready(s, l, cnt, &at); if (rc) return rc;
+      if (at < cnt) { *next_sub = a + at; break; }
+      done += cnt;
+      continue;
+    }
+    size_t nr_s = 0, tot_s = 0;
+    uint32_t next_s = a;
+    bool all = false;
+    const int rc = drain_ready_impl(s, a, cnt, a, out + tot, cap - tot, ready + nr, ready_left, &nr_s, &tot_s, &next_s, &all);
+    if (rc) return rc;
+    for (size_t j = 0; j < nr_s; j++) ready[nr + j].offset += (uint32_t)tot;
+    nr += nr_s; tot += tot_s; ready_left -= nr_s;
+    if (!all) { *next_sub = next_s; break; }
+    done += cnt;
+  }
+  *n_ready = nr; *total = tot;
+  return CPBUS_OK;
+} CPBUS_CATCH
+
+int cpbus_group_consume_all(cpbus_group_t* g) try {
+  if (!g) return CPBUS_EINVAL;
+  for (cpbus* s : g->shards) { const int rc = cpbus_consume_all(s); if (rc) return rc; }
+  return CPBUS_OK;
+} CPBUS_CATCH
+
+int cpbus_group_peek_window(cpbus_group_t* g, uint32_t sub_id, cpbus_event* out, size_t cap, size_t* n) try {
+  if (!g || !n || (!out && cap)) return CPBUS_EINVAL;
+  cpbus* s = nullptr; uint32_t l = 0;
+  if (!group_locate(g, sub_id, &s, &l)) return CPBUS_ENOENT;
+  return cpbus_peek_window(s, sub_id, out, cap, n);
+} CPBUS_CATCH
+
+int cpbus_group_digest(cpbus_group_t* g, uint32_t first_sub, uint32_t n, cpbus_digest_t* out) try {
+  if (!g || !out || !n) return CPBUS_EINVAL;
+  const uint32_t i0 = first_sub - g->base;
+  if (first_sub < g->base || (uint64_t)i0 + n > g->n_next) return CPBUS_ENOENT;
+  return group_each_range(g, i0, n, [&](cpbus* s, uint32_t l, uint32_t off, uint32_t cnt) -> int {
+    return cpbus_digest(s, s->cfg.sub_id_base + l, cnt, out + off);
+  });
+} CPBUS_CATCH
+
+int cpbus_group_digest_fold(cpbus_group_t* g, uint32_t first_sub, uint32_t n, uint64_t out[4]) try {
+  if (!g || !out || !n) return CPBUS_EINVAL;
+  const uint32_t i0 = first_sub - g->base;
+  if (first_sub < g->base || (uint64_t)i0 + n > g->n_next) return CPBUS_ENOENT;
+  uint64_t acc[4] = {0, 0, 0, 0};
+  const int rc = group_each_range(g, i0, n, [&](cpbus* s, uint32_t l, uint32_t, uint32_t cnt) -> int {
+    uint64_t part[4];
+    const int rc_s = cpbus_digest_fold(s, s->cfg.sub_id_base + l, cnt, part);
+    if (rc_s) return rc_s;
+    acc[0] += part[0]; acc[1] += part[1]; acc[2] ^= part[2]; acc[3] += part[3];   // sums add, the hash term XORs
+    return CPBUS_OK;
+  });
+  if (rc) return rc;
+  for (int j = 0; j < 4; j++) out[j] = acc[j];
+  return CPBUS_OK;
+} CPBUS_CATCH
+
+int cpbus_group_debug_events(cpbus_group_t* g, cpbus_event* out, size_t cap, size_t* n) try {   // cpbus_debug_events
+  if (!g || !n || (!out && cap)) return CPBUS_EINVAL;
+  size_t k = 0;
+  for (;;) {
+    if (g->dbg_head == -1) break;
+    const cpbus_event e = g->dbg[g->dbg_tail % 10];
+    if (g->dbg_tail == g->dbg_head) { g->dbg_head = -1; g->dbg_tail = 0; }
+    else g->dbg_tail = (g->dbg_tail + 1) % 10;
+    if (e.code == CPBUS_NONE && e.source_id == 0) break;
+    if (k < cap) out[k] = e;
+    k++;
+  }
+  *n = k;
+  return CPBUS_OK;
+} CPBUS_CATCH
+
+int cpbus_group_stats(cpbus_group_t* g, cpbus_stats_t* out) try {
+  if (!g || !out) return CPBUS_EINVAL;
+  cpbus_stats_t sum{}, s0{};
+  for (cpbus* s : g->shards) {
+    cpbus_stats_t x{};
+    const int rc = cpbus_stats(s, &x); if (rc) return rc;
+    if (s == g->shards[0]) s0 = x;   // the intern table's figures
+    sum.deliveries += x.deliveries; sum.ticks += x.ticks; sum.overwritten += x.overwritten;
+    sum.batches += x.batches; sum.kernel_launches += x.kernel_launches; sum.device_splits += x.device_splits;
+    sum.admit_passes += x.admit_passes; sum.admit_skipped += x.admit_skipped; sum.admit_partial += x.admit_partial;
+  }
+  group_retire(g);
+  sum.publishes = g->publishes;
+  for (int c = 0; c < CPBUS_N_CODES; c++) sum.published_by_code[c] = g->by_code[c];
+  sum.n_subs = g->n_active; sum.n_timers = g->n_timers; sum.now_ns = g->now;
+  sum.intern_entries = s0.intern_entries; sum.intern_bytes = s0.intern_bytes;
+  sum.ephemeral_live = s0.ephemeral_live; sum.ephemeral_recycled = s0.ephemeral_recycled;
+  *out = sum;
+  return CPBUS_OK;
+} CPBUS_CATCH
+
+int cpbus_group_publish_counts(cpbus_group_t* g, cpbus_pair_count* out, size_t cap, size_t* n) try {
+  if (!g || !n || (!out && cap)) return CPBUS_EINVAL;
+  std::vector<std::pair<uint64_t, uint64_t>> v;
+  for (size_t i = 0; i < g->pub_pairs.keys.size(); i++) if (g->pub_pairs.keys[i]) v.emplace_back(g->pub_pairs.keys[i] - 1, g->pub_pairs.cnts[i]);
+  std::sort(v.begin(), v.end());
+  for (size_t i = 0; i < v.size() && i < cap; i++) out[i] = cpbus_pair_count{(uint32_t)(v[i].first >> 32), (uint32_t)v[i].first, v[i].second};
+  *n = v.size();
   return CPBUS_OK;
 } CPBUS_CATCH
 

@@ -179,6 +179,22 @@ class Context {
 };
 
 namespace detail {
+// The bus behind an EventBus: one cpbus_t, or a group of shards over several GPUs (cpbus_group_t), which answers every
+// call the mirror makes exactly as one bus would.
+struct Handle { cpbus_t* one = nullptr; cpbus_group_t* group = nullptr; };
+}  // namespace detail
+#define EVENTS_CPBUS_CALL(name)                                                                          \
+  template <class... A>                                                                                \
+  inline int cpbus_##name(const detail::Handle& h, A... a) {                                           \
+    return h.group ? ::cpbus_group_##name(h.group, a...) : ::cpbus_##name(h.one, a...);                \
+  }
+EVENTS_CPBUS_CALL(subscribe) EVENTS_CPBUS_CALL(subscribe_pairs) EVENTS_CPBUS_CALL(unsubscribe) EVENTS_CPBUS_CALL(set_mask)
+EVENTS_CPBUS_CALL(publish) EVENTS_CPBUS_CALL(send) EVENTS_CPBUS_CALL(advance) EVENTS_CPBUS_CALL(flush)
+EVENTS_CPBUS_CALL(timer_add) EVENTS_CPBUS_CALL(timer_cancel) EVENTS_CPBUS_CALL(drain) EVENTS_CPBUS_CALL(drain_ready)
+EVENTS_CPBUS_CALL(debug_events) EVENTS_CPBUS_CALL(intern) EVENTS_CPBUS_CALL(intern_ephemeral) EVENTS_CPBUS_CALL(source)
+#undef EVENTS_CPBUS_CALL
+
+namespace detail {
 // which Subscriber (of which bus) owns a channel: kept by Subscribe / Unsubscribe, looked up by the timer functions
 // (Go needs no such table because the timer goroutine writes the channel itself)
 struct RxOwner { EventBus* bus; Subscriber* sub; };
@@ -190,14 +206,20 @@ class EventBus {   // events/bus.go:12-22
   enum class Clock { Virtual, Monotonic };
   // NewEventBus() — events/bus.go:72-88.  Clock::Virtual: time moves only through Advance() (tests);
   // Clock::Monotonic: a pump thread feeds std::chrono::steady_clock every millisecond.
-  explicit EventBus(Clock clock = Clock::Monotonic, uint32_t n_max_subs = 256, uint32_t mailbox_cap = 1024) : clock_(clock) {
+  explicit EventBus(Clock clock = Clock::Monotonic, uint32_t n_max_subs = 256, uint32_t mailbox_cap = 1024)
+      : EventBus(std::vector<int32_t>{}, clock, n_max_subs, mailbox_cap) {}
+  // The same bus on a group of shards, shard g on devices[g] (cpbus_group_create; devices may repeat).  Empty: one bus on
+  // the current device.
+  EventBus(const std::vector<int32_t>& devices, Clock clock, uint32_t n_max_subs = 256, uint32_t mailbox_cap = 1024) : clock_(clock) {
     cpbus_config cfg{};
     cfg.n_max_subs = n_max_subs; cfg.ring_cap = mailbox_cap; cfg.batch_cap = mailbox_cap >= 512 ? 256 : mailbox_cap / 2;
     cfg.timers_per_sub = 4; cfg.flags = CPBUS_CFG_LOSSLESS | CPBUS_CFG_DIGEST; cfg.device = -1;
     batch_cap_ = cfg.batch_cap;
     drain_cap_ = std::max<size_t>(kDrainCap, mailbox_cap);
-    int rc = cpbus_create(&cfg, &h_);
-    if (rc) throw std::runtime_error(std::string("cpbus_create: ") + cpbus_strerror(rc) + " " + cpbus_last_cuda_error());
+    const int rc = devices.empty() ? ::cpbus_create(&cfg, &h_.one)
+                                   : ::cpbus_group_create(&cfg, devices.data(), (uint32_t)devices.size(), &h_.group);
+    if (rc) throw std::runtime_error(std::string(devices.empty() ? "cpbus_create: " : "cpbus_group_create: ") + cpbus_strerror(rc) +
+                                     " " + cpbus_last_cuda_error());
     start_ = std::chrono::steady_clock::now();
     life_->h = h_;
     { std::lock_guard<std::mutex> g(CurrentMutex()); CurrentSlot() = this; }
@@ -212,7 +234,8 @@ class EventBus {   // events/bus.go:12-22
       life_->alive = false;                       // ctx.OnDone hooks that fire later find a dead bus and do nothing
       for (auto& kv : registry_) detail::RxRegistry().erase(kv.first->Rx.get());
     }
-    cpbus_destroy(h_);
+    if (h_.group) cpbus_group_destroy(h_.group);
+    else cpbus_destroy(h_.one);
   }
   // The bus a bus-less call refers to (NewEventTimer on a channel nobody subscribed): the most recently created live one.
   // ContainerPilot has exactly one per App run (core/app.go:142).
@@ -338,7 +361,7 @@ class EventBus {   // events/bus.go:12-22
     auto it = counter_.find({code, source});
     return it == counter_.end() ? 0 : it->second;
   }
-  cpbus_t* handle() { return h_; }
+  cpbus_t* handle() { return h_.one; }   // (nullptr on a group)
 
  private:
   friend class Subscriber;
@@ -353,7 +376,7 @@ class EventBus {   // events/bus.go:12-22
   };
 
   // state a ctx.OnDone hook may still hold after the bus is gone
-  struct Life { std::recursive_mutex m; bool alive = true; cpbus_t* h = nullptr; };
+  struct Life { std::recursive_mutex m; bool alive = true; detail::Handle h; };
   static std::mutex& CurrentMutex() { static std::mutex m; return m; }
   static EventBus*& CurrentSlot() { static EventBus* b = nullptr; return b; }
 
@@ -493,7 +516,7 @@ class EventBus {   // events/bus.go:12-22
   size_t drain_cap_ = kDrainCap;               // records per cpbus_drain_ready call (at least one mailbox's capacity)
   std::vector<cpbus_event> drain_buf_;
   std::vector<cpbus_ready> drain_ready_;
-  cpbus_t* h_ = nullptr;
+  detail::Handle h_;
   std::shared_ptr<Life> life_ = std::make_shared<Life>();
   std::recursive_mutex& lock_ = life_->m;   // bus.lock (bus.go:14): serialises publishers and membership changes
   std::map<Chan*, std::unique_ptr<Subscriber>> implicit_;   // timer-only channels

@@ -34,6 +34,7 @@ import numpy as np
 
 from . import _native as nat
 from .bus import Bus, EVENT_DTYPE
+from .group import GroupBus
 
 # EventCode enum — events/events.go:21-39
 (None_, ExitSuccess, ExitFailed, Stopping, Stopped, StatusHealthy, StatusUnhealthy, StatusChanged, TimerExpired,
@@ -118,9 +119,14 @@ class EventBus:
     """EventBus — events/bus.go:12-22.  NewEventBus() == EventBus()."""
 
     def __init__(self, n_max_subs: int = 64, ring_cap: int = 1024, batch_cap: int = 256, timers_per_sub: int = 4,
-                 lossless: bool = True, **kw):
-        self._bus = Bus(n_max_subs, ring_cap=ring_cap, batch_cap=batch_cap, timers_per_sub=timers_per_sub,
-                        lossless=lossless, digest=True, **kw)
+                 lossless: bool = True, devices=None, **kw):
+        """`devices`: run on a group of shards, shard g on devices[g] (GroupBus); the answers are the single bus's"""
+        if devices is not None:
+            self._bus = GroupBus(n_max_subs, devices, ring_cap=ring_cap, batch_cap=batch_cap, timers_per_sub=timers_per_sub,
+                                 lossless=lossless, digest=True, **kw)
+        else:
+            self._bus = Bus(n_max_subs, ring_cap=ring_cap, batch_cap=batch_cap, timers_per_sub=timers_per_sub,
+                            lossless=lossless, digest=True, **kw)
         self.reload = False
         self._done = 0              # sync.WaitGroup counter (bus.go:16)
         self._subs = {}             # Subscriber -> sub_id  (registry, bus.go:13)

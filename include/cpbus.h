@@ -450,6 +450,60 @@ int cpbus_publish_counts(cpbus_t* bus, cpbus_pair_count* out, size_t cap, size_t
  * (bit 31 = subscribed, bits 24..27 = timer slots in use); u32 pad}. */
 int cpbus_device_ptrs(cpbus_t* bus, void** ring, void** ctl);
 
+/* ---- one bus handle over the GPUs of a box: the group ------------------------------------------------------------
+ * A group is G ordinary buses (shards) behind one handle, driven by one host thread (the single ContainerPilot process).
+ * Shard g lives on devices[g] (devices may repeat: several shards on one GPU) and owns a contiguous slice of the global
+ * subscriber ids, split as evenly as possible (the first n_max_subs % G shards take one more).  Shard 0 creates a stream
+ * (cpbus_stream_create) and the others attach to it; every flush of the group is one RAW stream batch that every shard
+ * fans out, so unicast sends travel in publish order and are delivered by the owning shard's kernel only.
+ * cfg is interpreted exactly as by cpbus_create, with n_max_subs = the total over the shards; cfg->stream must be NULL
+ * (each shard runs on its own library-owned stream) and n_max_subs >= n_devices.
+ *
+ * The contract: the cpbus_group_* twin of an entry point takes the same arguments and returns the same status codes as
+ * the single-bus call.  Any sequence of these calls, run on a group of G shards and on one bus created with the same
+ * cpbus_config, gives the same return codes, the same subscriber and timer ids, byte-identical drain, drain_ready (records,
+ * ready list and next_sub), peek_window, digest, digest_fold, debug_events and publish_counts outputs, and the same
+ * cpbus_stats except the launch-shaped counters (batches, kernel_launches, admit_passes, admit_skipped, admit_partial,
+ * device_splits).  This holds in throughput mode and in lossless mode (CPBUS_CFG_LOSSLESS), including where CPBUS_EAGAIN
+ * is returned and how many events cpbus_stats.publishes says a stalled publish took: the group stages, flushes, splits
+ * clock steps and cuts lossless prefixes where the single bus does, and admits each flush on every shard before it puts
+ * the part every shard can take into the stream.
+ * The intern table is shard 0's; the other shards only ever see source ids.  debug_events, publish_counts and
+ * published_by_code are the group's own host records; deliveries, ticks and overwritten are sums over the shards. */
+typedef struct cpbus_group cpbus_group_t;
+int cpbus_group_create(const cpbus_config* cfg, const int32_t* devices, uint32_t n_devices, cpbus_group_t** out);
+int cpbus_group_destroy(cpbus_group_t* g);
+int cpbus_group_intern(cpbus_group_t* g, const char* s, size_t len, uint32_t* source_id);
+int cpbus_group_intern_ephemeral(cpbus_group_t* g, const char* s, size_t len, uint32_t* source_id);
+int cpbus_group_source(cpbus_group_t* g, uint32_t source_id, char* out, size_t cap, size_t* len);
+int cpbus_group_subscribe(cpbus_group_t* g, uint32_t code_mask, uint32_t* sub_id);
+int cpbus_group_subscribe_many(cpbus_group_t* g, const uint32_t* code_masks, uint32_t n, uint32_t* first_sub_id);
+int cpbus_group_subscribe_pairs(cpbus_group_t* g, uint32_t code_mask, const cpbus_pair* pairs, uint32_t n_pairs, uint32_t* sub_id);
+int cpbus_group_subscribe_pairs_many(cpbus_group_t* g, const uint32_t* code_masks, const cpbus_pair* pairs,
+                                     const uint32_t* n_pairs, uint32_t n, uint32_t* first_sub_id);
+int cpbus_group_unsubscribe(cpbus_group_t* g, uint32_t sub_id);
+int cpbus_group_set_mask(cpbus_group_t* g, uint32_t sub_id, uint32_t code_mask);
+int cpbus_group_timer_add(cpbus_group_t* g, uint32_t sub_id, uint64_t period_ns, uint32_t source_id, int oneshot, uint32_t* timer_id);
+int cpbus_group_timer_add_many(cpbus_group_t* g, uint32_t first_sub, uint32_t n, uint64_t period_ns, const uint32_t* source_ids,
+                               uint32_t source_id0, int oneshot);
+int cpbus_group_timer_cancel(cpbus_group_t* g, uint32_t timer_id);
+int cpbus_group_publish(cpbus_group_t* g, const cpbus_event* ev, size_t n);
+int cpbus_group_send(cpbus_group_t* g, uint32_t sub_id, const cpbus_event* ev);
+int cpbus_group_advance(cpbus_group_t* g, uint64_t now_ns);
+int cpbus_group_flush(cpbus_group_t* g);
+int cpbus_group_sync(cpbus_group_t* g);
+int cpbus_group_drain(cpbus_group_t* g, uint32_t sub_id, cpbus_event* out, size_t cap, size_t* n, uint64_t* lost);
+int cpbus_group_drain_ready(cpbus_group_t* g, uint32_t first_sub, uint32_t n, uint32_t start_sub,
+                            cpbus_event* out, size_t cap, cpbus_ready* ready, size_t ready_cap,
+                            size_t* n_ready, size_t* total, uint32_t* next_sub);
+int cpbus_group_consume_all(cpbus_group_t* g);
+int cpbus_group_peek_window(cpbus_group_t* g, uint32_t sub_id, cpbus_event* out, size_t cap, size_t* n);
+int cpbus_group_digest(cpbus_group_t* g, uint32_t first_sub, uint32_t n, cpbus_digest_t* out);
+int cpbus_group_digest_fold(cpbus_group_t* g, uint32_t first_sub, uint32_t n, uint64_t out[4]);
+int cpbus_group_debug_events(cpbus_group_t* g, cpbus_event* out, size_t cap, size_t* n);
+int cpbus_group_stats(cpbus_group_t* g, cpbus_stats_t* out);
+int cpbus_group_publish_counts(cpbus_group_t* g, cpbus_pair_count* out, size_t cap, size_t* n);
+
 /* ---- names: EventCode.String (events/eventcode_string.go:9-15), FromString (events/events.go:52-86) ---- */
 const char* cpbus_code_name(int code);               /* NULL if out of range      */
 int cpbus_code_from_string(const char* name);        /* code, or -1 if not valid  */
