@@ -66,6 +66,11 @@ struct PairCounter {
 };
 
 struct HostTimer { bool active = false, oneshot = false; uint8_t gen = 0; uint64_t period = 0, next_due = 0; uint32_t source_id = 0; };
+// Due times saturate: one that would pass UINT64_MAX - 1 is kTimerIdle, "never".  The slot stays armed (it counts in
+// n_timers and can be cancelled); the kernel never fires a tick due at kTimerIdle.
+inline uint64_t due_after(uint64_t t, uint64_t period) { return period >= kTimerIdle - t ? kTimerIdle : t + period; }
+// a one-shot due by watermark w has fired on the device and disarmed itself
+inline bool oneshot_fired(uint64_t next_due, uint64_t w) { return next_due <= w && next_due != kTimerIdle; }
 // timer id = slot index (subscriber * K + k) | generation << 26: a late cancel from an old context cannot disarm a re-armed slot
 constexpr uint32_t kTimerSlotBits = 26, kTimerSlotMask = (1u << kTimerSlotBits) - 1u;
 
@@ -560,7 +565,7 @@ void retire_oneshots(cpbus* b, uint64_t w) {
   size_t keep = 0;
   for (size_t i = 0; i < b->oneshot_idx.size(); i++) {
     HostTimer& t = b->h_timers[b->oneshot_idx[i]];
-    if (t.active && t.oneshot && t.next_due <= w) { t.active = false; b->n_timers--; continue; }
+    if (t.active && t.oneshot && oneshot_fired(t.next_due, w)) { t.active = false; b->n_timers--; continue; }
     if (t.active && t.oneshot) b->oneshot_idx[keep++] = b->oneshot_idx[i];
   }
   b->oneshot_idx.resize(keep);
@@ -739,6 +744,7 @@ static int config_check(const cpbus_config* cfg, uint32_t* R_out, uint32_t* B_ou
   if (!(K == 0 || K == 1 || K == 2 || K == 4 || K == 8)) return CPBUS_EINVAL;
   if ((uint64_t)cfg->n_max_subs * std::max(K, 1u) > kTimerSlotMask) return CPBUS_EINVAL;   // timer ids keep 6 generation bits
   if (cfg->store_path > CPBUS_STORE_BULK) return CPBUS_EINVAL;
+  if ((uint64_t)cfg->sub_id_base + cfg->n_max_subs > CPBUS_TARGET_ALL) return CPBUS_EINVAL;   // every gid stays below CPBUS_TARGET_ALL
   *R_out = R; *B_out = B;
   return CPBUS_OK;
 }
@@ -1116,7 +1122,7 @@ int cpbus_timer_add(cpbus_t* b, uint32_t sub_id, uint64_t period_ns, uint32_t so
   for (uint32_t k = 0; k < b->K; k++) {
     HostTimer& t = b->h_timers[(size_t)l * b->K + k];
     if (t.active) continue;
-    t.active = true; t.oneshot = oneshot != 0; t.period = period_ns; t.next_due = b->now + period_ns; t.source_id = source_id;
+    t.active = true; t.oneshot = oneshot != 0; t.period = period_ns; t.next_due = due_after(b->now, period_ns); t.source_id = source_id;
     DevTimer d{}; d.next_due = t.next_due; d.period = oneshot ? 0 : period_ns; d.source_id = source_id; d.fired = 0;
     CK(cudaMemcpyAsync(b->d_timers + (size_t)l * b->K + k, &d, sizeof(d), cudaMemcpyHostToDevice, b->stream));
     CK(cudaStreamSynchronize(b->stream));
@@ -1151,7 +1157,7 @@ int cpbus_timer_add_many(cpbus_t* b, uint32_t first_sub, uint32_t n, uint64_t pe
   CK(cudaStreamSynchronize(b->stream));
   for (uint32_t i = 0; i < n; i++) {
     HostTimer& t = b->h_timers[(size_t)(l0 + i) * b->K];
-    t.active = true; t.oneshot = oneshot != 0; t.period = period_ns; t.next_due = b->now + period_ns;
+    t.active = true; t.oneshot = oneshot != 0; t.period = period_ns; t.next_due = due_after(b->now, period_ns);
     t.source_id = source_ids ? source_ids[i] : source_id0 + i;
     DevTimer& d = dev[(size_t)i * b->K];
     d.next_due = t.next_due; d.period = oneshot ? 0 : period_ns; d.source_id = t.source_id; d.fired = 0; d.pad[0] = d.pad[1] = 0;
@@ -1349,8 +1355,10 @@ static int publish_device_impl(cpbus_t* b, const void* d_events, size_t n, uint6
     o.pf_src = (const cpbus_event*)d_next; o.pf_dst = b->d_prefetch[slot];
     for (int i = 0; i < cpbus::kPrefetch; i++) if (b->pf_ptr[i] == d_next) b->pf_ptr[i] = nullptr;   // superseded
   }
+  const unsigned long long seq0 = b->launch_seq;
   if ((rc = launch_fanout(b, src, (uint32_t)n, watermark_ns, o))) return rc;
-  if (slot >= 0) { b->pf_ptr[slot] = d_next; b->pf_n[slot] = n_next; b->pf_seq[slot] = b->launch_seq; b->pf_next = (slot + 1) % cpbus::kPrefetch; }
+  // an empty batch with no timer armed launches nothing, so nothing pulled d_next: the cache must not claim it
+  if (slot >= 0 && b->launch_seq != seq0) { b->pf_ptr[slot] = d_next; b->pf_n[slot] = n_next; b->pf_seq[slot] = b->launch_seq; b->pf_next = (slot + 1) % cpbus::kPrefetch; }
   b->st.publishes += n; b->seq += n;
   return CPBUS_OK;
 }
@@ -2342,7 +2350,7 @@ static void group_retire(cpbus_group* g) {
   size_t keep = 0;
   for (size_t i = 0; i < g->oneshot_idx.size(); i++) {
     cpbus_group::Slot& t = g->timers[g->oneshot_idx[i]];
-    if (t.active && t.oneshot && t.next_due <= g->last_watermark) { t.active = false; g->n_timers--; continue; }
+    if (t.active && t.oneshot && oneshot_fired(t.next_due, g->last_watermark)) { t.active = false; g->n_timers--; continue; }
     if (t.active && t.oneshot) g->oneshot_idx[keep++] = g->oneshot_idx[i];
   }
   g->oneshot_idx.resize(keep);
@@ -2582,7 +2590,7 @@ int cpbus_group_timer_add(cpbus_group_t* g, uint32_t sub_id, uint64_t period_ns,
   const uint32_t shard_base_slot = (sub_id - l - g->base) * g->K;   // global slot of the shard's slot 0
   const size_t slot = (size_t)(id & kTimerSlotMask) + shard_base_slot;
   cpbus_group::Slot& t = g->timers[slot];
-  t.active = true; t.oneshot = oneshot != 0; t.next_due = g->now + period_ns;
+  t.active = true; t.oneshot = oneshot != 0; t.next_due = due_after(g->now, period_ns);
   g->n_timers++;
   if (!oneshot) g->min_period = std::min(g->min_period, period_ns);
   else g->oneshot_idx.push_back(slot);
@@ -2616,7 +2624,7 @@ int cpbus_group_timer_add_many(cpbus_group_t* g, uint32_t first_sub, uint32_t n,
   for (uint32_t i = 0; i < n; i++) {
     const size_t slot = (size_t)(i0 + i) * g->K;
     cpbus_group::Slot& t = g->timers[slot];
-    t.active = true; t.oneshot = oneshot != 0; t.next_due = g->now + period_ns;
+    t.active = true; t.oneshot = oneshot != 0; t.next_due = due_after(g->now, period_ns);
     if (oneshot) g->oneshot_idx.push_back(slot);
   }
   g->n_timers += n;

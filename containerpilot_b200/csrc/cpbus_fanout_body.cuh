@@ -229,7 +229,10 @@
         const uint32_t code = (uint32_t)w.z, target = (uint32_t)w.w;
         uint32_t codebit = 0;
         if (target == CPBUS_TARGET_ALL) {
-          if (code < 32) { codebit = 1u << code; atomicAdd(&s_dsum[2 + code], 1u); }
+          // a code outside the enum (only a complete record can carry one) takes bit / bucket kCodeOutOfRange, which no
+          // control word carries: no mailbox selects it, dense runs are off for the batch and its publish is not counted
+          const uint32_t c = min(code, kCodeOutOfRange);
+          codebit = 1u << c; atomicAdd(&s_dsum[2 + c], 1u);
           present |= codebit;
         } else uni = 1;
         s_meta[i] = make_uint2(codebit, target);
@@ -453,8 +456,11 @@
         const uint4 hot = tim_half(0);
         tk_due0 = ((uint64_t)hot.y << 32) | hot.x; tk_period = ((uint64_t)hot.w << 32) | hot.z;
       }
-      tk_due = tk_due0 + (uint64_t)tk_j * tk_period;
-      tk_valid = tk_due0 != kTimerIdle && tk_due <= (FOLLOW ? w_follow : p.w_now) && (tk_j == 0 || tk_period != 0);
+      // due times saturate: a candidate whose sum passes UINT64_MAX - 1 never comes
+      const uint64_t step = (uint64_t)tk_j * tk_period;
+      tk_due = tk_due0 + step;
+      const bool wraps = __umul64hi(tk_j, tk_period) != 0 || tk_due < step || tk_due == kTimerIdle;
+      tk_valid = tk_due0 != kTimerIdle && !wraps && tk_due <= (FOLLOW ? w_follow : p.w_now) && (tk_j == 0 || tk_period != 0);
       tk_mask = __ballot_sync(0xffffffffu, tk_valid);
       n_ticks = __popc(tk_mask);
       if (n_ticks) {
@@ -754,8 +760,10 @@
       const uint32_t fired_here = __popc(tk_mask & slotmask);
       if (TIMERS && tk_j == 0 && tk_slot < nslots && fired_here) {
         unsigned char* t = reinterpret_cast<unsigned char*>(&p.timers[(size_t)s * K + tk_slot]);
-        // this lane has tk_j == 0, so tk_due is the slot's next_due as loaded
-        const uint64_t nd = tk_period ? tk_due + (uint64_t)fired_here * tk_period : kTimerIdle;   // one-shot disarms itself
+        // this lane has tk_j == 0, so tk_due is the slot's next_due as loaded.  A one-shot disarms itself; a periodic re-arm
+        // past UINT64_MAX - 1 saturates to kTimerIdle (never fires again; the host still counts the slot as armed)
+        const uint64_t step = (uint64_t)fired_here * tk_period;
+        const uint64_t nd = (tk_period && __umul64hi(fired_here, tk_period) == 0 && step < kTimerIdle - tk_due) ? tk_due + step : kTimerIdle;
         st_half(t, make_uint4((uint32_t)nd, (uint32_t)(nd >> 32), (uint32_t)tk_period, (uint32_t)(tk_period >> 32)), keep);
         st_half(t + 16, make_uint4(tk_src, tk_fired + fired_here, 0u, 0u), keep);
       }
@@ -799,12 +807,12 @@
   if (blockIdx.x == 0 && p.acct && !aborted) {
     // device-published batch: publish accounting (events/bus.go:128-139), done here — after the lead CTA's own mailboxes —
     // so that it never delays the fan-out (the staged batch and its descriptor are still intact in shared memory)
-    if (tid < 32 && tid != CPBUS_METRIC && s_dsum[2 + tid]) atomicAdd(&p.acct->by_code[tid], (unsigned long long)s_dsum[2 + tid]);
+    if (tid < CPBUS_N_CODES && tid != CPBUS_METRIC && s_dsum[2 + tid]) atomicAdd(&p.acct->by_code[tid], (unsigned long long)s_dsum[2 + tid]);
     for (uint32_t i = tid; i < n; i += kThreads) {
       if (s_meta[i].y != CPBUS_TARGET_ALL) continue;
       const uint2 cs = ev_code_src(i);
       const uint32_t code = cs.x;
-      if (code == CPBUS_METRIC || code >= 32u) continue;
+      if (code == CPBUS_METRIC || code >= CPBUS_N_CODES) continue;
       const unsigned long long key = (((unsigned long long)code << 32) | cs.y) + 1ull;
       uint32_t slot = pair_key_hash(code, cs.y) & (kAcctPairSlots - 1u);
       bool placed = false;
@@ -818,7 +826,7 @@
       DevDbgTail* t = &p.acct->tail[p.launch_seq % kAcctDbgRing];
       uint32_t* idx = s_tick;                                      // every warp of this CTA is past its main loop (barrier above)
       uint32_t kept = 0, nb = 0;
-      for (uint32_t c = 0; c < 32; c++) nb += s_dsum[2 + c];
+      for (uint32_t c = 0; c <= kCodeOutOfRange; c++) nb += s_dsum[2 + c];
       for (uint32_t i = n; i > 0 && kept < (uint32_t)kAcctDbgKeep; i--)
         if (s_meta[i - 1].y == CPBUS_TARGET_ALL) idx[kept++] = i - 1;
       for (uint32_t j = 0; j < kept; j++) {

@@ -30,6 +30,10 @@ constexpr uint32_t kActiveBit = 0x80000000u;   // mask word: subscriber is subsc
 constexpr int kTimerHintShift = 24;            // mask word bits 24..27: #timer slots to look at
 constexpr uint32_t kPairBit = 0x10000000u;     // mask word bit 28: subscriber has a {code, source} pair table
 constexpr uint32_t kPairNone = 0xFFFFFFFFu;    // code of an unused pair slot
+// Fan-out staging: the `present` bit and histogram bucket of every broadcast code >= CPBUS_N_CODES.  The mask word never
+// carries bit 17 (code mask in bits 0..16, bookkeeping from bit 24 up), so no mailbox selects such a record.
+constexpr uint32_t kCodeOutOfRange = CPBUS_N_CODES;
+static_assert(kCodeOutOfRange < (uint32_t)kTimerHintShift,"the out-of-range bit must lie between the code mask and the mask word's bookkeeping bits");
 // PAIRS build: per-CTA presence filter over the batch's broadcast {code, source} keys (2 probes into 32,768 bits:
 // ~0.1 % false positives at 512 events, never a false negative).  A pair-filtered mailbox whose cases are all absent
 // from the batch is finished after 16 lanes x 2 shared-memory probes instead of a 512-event x 16-pair scan.
@@ -488,10 +492,12 @@ __device__ __forceinline__ void admit_body(const cpbus_event* batch, uint32_t n_
       for (uint32_t i = 0; i < n_ev; i++) if (batch[i].target == gid) k++;
     }
     const uint32_t nslots = timers_on ? min((m >> kTimerHintShift) & 0xFu, K) : 0u;
+    // due times saturate at kTimerIdle - 1 (the fan-out kernel never fires a tick due at kTimerIdle): count up to there
+    const uint64_t w_due = min(w_now, kTimerIdle - 1);
     for (uint32_t t = 0; t < nslots; t++) {
       const DevTimer tm = timers[(size_t)s * K + t];
-      if (tm.next_due != kTimerIdle && tm.next_due <= w_now)
-        k += tm.period ? (w_now - tm.next_due) / tm.period + 1u : 1u;
+      if (tm.next_due != kTimerIdle && tm.next_due <= w_due)
+        k += tm.period ? (w_due - tm.next_due) / tm.period + 1u : 1u;
     }
     const unsigned long long used = c.tail - c.head + k;
     if (used > ring_cap) {
@@ -508,7 +514,8 @@ __device__ __forceinline__ void admit_body(const cpbus_event* batch, uint32_t n_
         unsigned long long tks = 0;
         for (uint32_t t = 0; t < nslots; t++) {
           const DevTimer tm = timers[(size_t)s * K + t];
-          if (tm.next_due != kTimerIdle && tm.next_due <= e.ts_ns) tks += tm.period ? (e.ts_ns - tm.next_due) / tm.period + 1u : 1u;
+          const uint64_t ts = min(e.ts_ns, kTimerIdle - 1);
+          if (tm.next_due != kTimerIdle && tm.next_due <= ts) tks += tm.period ? (ts - tm.next_due) / tm.period + 1u : 1u;
         }
         bool want;
         if (e.target == CPBUS_TARGET_ALL) {

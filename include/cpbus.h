@@ -103,7 +103,9 @@ typedef struct cpbus_config {
   uint32_t flags;          /* CPBUS_CFG_*                                         */
   int32_t  device;         /* CUDA device ordinal; -1 = current device            */
   uint32_t sub_id_base;    /* global id of this shard's subscriber 0 (multi-GPU:
-                              contiguous shards, SURVEY.md §8e)                   */
+                              contiguous shards, SURVEY.md §8e); sub_id_base +
+                              n_max_subs <= 0xFFFFFFFF (CPBUS_EINVAL otherwise), so
+                              no gid equals CPBUS_TARGET_ALL                      */
   uint32_t store_path;     /* CPBUS_STORE_*                                       */
   void*    stream;         /* cudaStream_t to run on; NULL = library-owned stream */
   uint32_t grid_ctas;      /* 0 = auto (multiple of the SM count)                 */
@@ -183,7 +185,9 @@ int cpbus_set_mask(cpbus_t* bus, uint32_t sub_id, uint32_t code_mask);
 /* ---- timers: NewEventTimer / NewEventTimeout (events/timer.go:40-71 / 12-37).
  *      The first firing is due at now + period_ns; a periodic timer then fires
  *      every period_ns, a one-shot exactly once.  cancel = ctx.Done().  A timer id carries a generation: cancelling an
- *      id whose slot has fired (one-shot) or been re-armed since returns CPBUS_ENOENT and touches nothing. ---- */
+ *      id whose slot has fired (one-shot) or been re-armed since returns CPBUS_ENOENT and touches nothing.
+ *      Due times saturate: a first or re-armed due time past UINT64_MAX - 1 means "never" (the timer stays armed, counts
+ *      in n_timers and can be cancelled, but does not fire). ---- */
 int cpbus_timer_add(cpbus_t* bus, uint32_t sub_id, uint64_t period_ns, uint32_t source_id, int oneshot, uint32_t* timer_id);
 /* one periodic timer per subscriber [first_sub, first_sub+n); source_ids[i] (or source_id0+i if NULL) */
 int cpbus_timer_add_many(cpbus_t* bus, uint32_t first_sub, uint32_t n, uint64_t period_ns, const uint32_t* source_ids, uint32_t source_id0, int oneshot);
@@ -218,7 +222,9 @@ int cpbus_sync(cpbus_t* bus);
  * records and a watermark step of up to 32/timers_per_sub periods of the fastest armed
  * timer; a batch beyond either is cut into several launches (the cut reads the records'
  * timestamps back, 8 bytes each: a slow path, counted in cpbus_stats.device_splits).
- * Lossless mode keeps the strict form: CPBUS_EINVAL / CPBUS_EORDER for such a batch. */
+ * Lossless mode keeps the strict form: CPBUS_EINVAL / CPBUS_EORDER for such a batch.
+ * A broadcast record whose code is >= CPBUS_N_CODES reaches no mailbox (no mask bit or pair selects it); it counts in
+ * stats.publishes and the debug ring but not in published_by_code or cpbus_publish_counts.  The bus's seq advances by n. */
 int cpbus_publish_device(cpbus_t* bus, const void* d_events, size_t n, uint64_t watermark_ns);
 /* (Batches published this way are accounted for by the kernel itself: cpbus_stats.published_by_code,
  * cpbus_publish_counts and cpbus_debug_events see their broadcast events exactly as if they had gone through cpbus_publish.) */

@@ -185,8 +185,9 @@ int orc_subscribe_pairs(orc_bus* b, uint32_t mask, const uint32_t* codes, const 
   return ORC_OK;
 }
 
+/* A broadcast code >= ORC_N_CODES (possible only in complete records) is matched by no mask bit and no pair. */
 static int wants(const orc_sub* s, uint32_t code, uint32_t source_id) {
-  if (code < 32 && ((s->mask >> code) & 1u)) return 1;
+  if (code < ORC_N_CODES && ((s->mask >> code) & 1u)) return 1;
   for (uint32_t j = 0; j < s->n_pairs; j++)
     if (s->pair_code[j] == code && s->pair_src[j] == source_id) return 1;
   return 0;
@@ -242,6 +243,12 @@ int orc_receive(orc_bus* b, uint32_t gid, uint32_t code, uint32_t source_id) {
   return ORC_OK;
 }
 
+/* Due times saturate: a sum past UINT64_MAX - 1 is ORC_NEVER, a due time that never comes (the timer stays armed). */
+#define ORC_NEVER UINT64_MAX
+static uint64_t due_after(uint64_t t, uint64_t period) {
+  return period >= ORC_NEVER - t ? ORC_NEVER : t + period;
+}
+
 /* NewEventTimer (events/timer.go:40-71) / NewEventTimeout (timer.go:12-37):
  * first firing one period after creation; periodic repeats every period. */
 int orc_timer_add(orc_bus* b, uint32_t gid, uint64_t period_ns, uint32_t source_id, int oneshot, uint32_t* timer_id) {
@@ -253,7 +260,7 @@ int orc_timer_add(orc_bus* b, uint32_t gid, uint64_t period_ns, uint32_t source_
     if (s->timers[k].active) continue;
     orc_timer* t = &s->timers[k];
     t->active = 1; t->oneshot = oneshot; t->period = period_ns;
-    t->next_due = b->now + period_ns; t->source_id = source_id; t->fired = 0;
+    t->next_due = due_after(b->now, period_ns); t->source_id = source_id; t->fired = 0;
     s->n_active_timers++; b->n_timers++;
     if (t->next_due < b->min_due) b->min_due = t->next_due;
     if (timer_id) *timer_id = (gid - b->base) * b->K + k;
@@ -287,7 +294,7 @@ int orc_advance(orc_bus* b, uint64_t now_ns) {
         int best = -1;
         for (uint32_t k = 0; k < b->K; k++) {
           orc_timer* t = &s->timers[k];
-          if (!t->active || t->next_due > now_ns) continue;
+          if (!t->active || t->next_due > now_ns || t->next_due == ORC_NEVER) continue;
           if (best < 0 || t->next_due < s->timers[best].next_due) best = (int)k;
         }
         if (best < 0) break;
@@ -298,7 +305,7 @@ int orc_advance(orc_bus* b, uint64_t now_ns) {
         b->ticks++;
         t->fired++;
         if (t->oneshot) { t->active = 0; s->n_active_timers--; b->n_timers--; }
-        else t->next_due += t->period;
+        else t->next_due = due_after(t->next_due, t->period);
       }
       for (uint32_t k = 0; k < b->K; k++)
         if (s->timers[k].active && s->timers[k].next_due < new_min) new_min = s->timers[k].next_due;
@@ -322,7 +329,8 @@ int orc_publish_many(orc_bus* b, const uint32_t* codes, const uint32_t* sources,
  * streams): the clock first reaches each record's ts (timers due by then fire before it, timer.go:59-67); a broadcast
  * record is then delivered exactly like Publish (bus.go:125-140) and a unicast one like Receive (subscriber.go:30-32),
  * but with the record's OWN seq/ts.  A unicast target outside this shard is some other shard's business.  Finally the
- * clock reaches `watermark`. */
+ * clock reaches `watermark`.  The bus's own publish ordinal advances by one per record: the next host publish after n
+ * records carries the previous ordinal + n, whatever seqs the records carried. */
 int orc_publish_records(orc_bus* b, const orc_event* recs, size_t n, uint64_t watermark_ns) {
   for (size_t r = 0; r < n; r++) {
     const orc_event* e = &recs[r];
@@ -338,7 +346,7 @@ int orc_publish_records(orc_bus* b, const orc_event* recs, size_t n, uint64_t wa
       orc_sub* s = sub_at(b, e->target);
       if (s && s->active) receive(b, s, e);
     }
-    b->seq = e->seq + 1;
+    b->seq++;   /* every record takes one publish ordinal, whatever seq it carries */
   }
   if (watermark_ns > b->now) return orc_advance(b, watermark_ns);
   return ORC_OK;

@@ -107,18 +107,19 @@ def test_create_rejects_bad_configs_before_touching_the_device():
 C_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "c")
 
 
-def build_c_smoke():
-    """tests/c/abi_smoke.c: the C-ABI called from plain C99 (what cgo-generated code does), -Wall -Wextra -Werror -pedantic"""
+def build_c_smoke(out_dir):
+    """tests/c/abi_smoke.c: the C-ABI called from plain C99 (what cgo-generated code does), -Wall -Wextra -Werror -pedantic.
+    The program is written to out_dir: the source tree may be read-only to the user running the tests."""
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    exe = os.path.join(C_DIR, "abi_smoke")
+    exe = os.path.join(str(out_dir), "abi_smoke")
     subprocess.check_call(["gcc", "-std=c99", "-Wall", "-Wextra", "-Werror", "-pedantic", "-I", os.path.join(root, "include"),
                            os.path.join(C_DIR, "abi_smoke.c"), "-L", os.path.join(root, "containerpilot_b200"), "-lcpbus",
                            "-Wl,-rpath," + os.path.join(root, "containerpilot_b200"), "-o", exe])
     return exe
 
 
-def test_header_is_plain_c99_and_a_c_caller_links():
-    exe = build_c_smoke()
+def test_header_is_plain_c99_and_a_c_caller_links(tmp_path):
+    exe = build_c_smoke(tmp_path)
     assert os.path.exists(exe)
     import torch
     if not torch.cuda.is_available():            # without a device the program must stop at cpbus_create with ENODEV, loudly

@@ -345,10 +345,10 @@ def test_masks_derived_from_the_switches_run_on_the_cuda_bus():
     bus.close()
 
 
-def test_plain_c_caller_of_the_c_abi():
+def test_plain_c_caller_of_the_c_abi(tmp_path):
     """tests/c/abi_smoke.c — include/cpbus.h from C99, the way cgo-generated code calls it: the jobs_test.go:15-48 sequence, a
     periodic timer, a code mask, DebugEvents, the {code, source} counts; every check is inside the program."""
     import subprocess
     from test_abi import build_c_smoke
-    r = subprocess.run([build_c_smoke()], capture_output=True, text=True, timeout=120)
+    r = subprocess.run([build_c_smoke(tmp_path)], capture_output=True, text=True, timeout=120)
     assert r.returncode == 0 and r.stdout.strip().endswith("PASS"), r.stdout + r.stderr
