@@ -9,6 +9,8 @@ from __future__ import annotations
 import ctypes as C
 import os
 
+import numpy as np
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("CPBUS_LIB") or os.path.join(HERE, "libcpbus.so")   # CPBUS_LIB: A/B builds of the same library
 
@@ -57,7 +59,16 @@ class PairCount(C.Structure):
     _fields_ = [("code", C.c_uint32), ("source_id", C.c_uint32), ("count", C.c_uint64)]
 
 
+class LagSummary(C.Structure):
+    """cpbus_lag_summary: cpbus_lagging's figures over the whole range"""
+    _fields_ = [("active", C.c_uint64), ("lagging", C.c_uint64), ("backlog_total", C.c_uint64),
+                ("backlog_max", C.c_uint64), ("lost_total", C.c_uint64), ("hist", C.c_uint64 * 33)]
+
+
 assert C.sizeof(Event) == 32
+# cpbus_lag: one entry of cpbus_lagging's list
+LAG_DTYPE = np.dtype([("sub_id", "<u4"), ("backlog", "<u4"), ("lost", "<u8")])
+assert LAG_DTYPE.itemsize == 16
 
 # every symbol include/cpbus.h declares: (restype, argtypes)
 _P = C.POINTER
@@ -106,6 +117,9 @@ SYMBOLS = {
     "cpbus_drain_many": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, _P(C.c_size_t)]),
     "cpbus_drain_ready": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p,
                                     C.c_size_t, _P(C.c_size_t), _P(C.c_size_t), _P(C.c_uint32)]),
+    "cpbus_lagging": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t,
+                                _P(C.c_size_t), _P(C.c_uint32), _P(LagSummary)]),
+    "cpbus_blockers": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, _P(C.c_size_t)]),
     "cpbus_consume_all": (C.c_int, [C.c_void_p]),
     "cpbus_peek_window": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t, _P(C.c_size_t)]),
     "cpbus_digest": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]),
@@ -131,8 +145,8 @@ SYMBOLS = {
 # the group (one handle over several shards): cpbus_group_<name> takes the arguments of cpbus_<name>
 GROUP_CALLS = ("intern", "intern_ephemeral", "source", "subscribe", "subscribe_many", "subscribe_pairs", "subscribe_pairs_many",
                "unsubscribe", "set_mask", "timer_add", "timer_add_many", "timer_cancel", "publish", "send", "advance", "flush",
-               "sync", "drain", "drain_ready", "consume_all", "peek_window", "digest", "digest_fold", "debug_events", "stats",
-               "publish_counts")
+               "sync", "drain", "drain_ready", "lagging", "blockers", "consume_all", "peek_window", "digest", "digest_fold",
+               "debug_events", "stats", "publish_counts")
 SYMBOLS["cpbus_group_create"] = (C.c_int, [_P(Config), C.c_void_p, C.c_uint32, _P(C.c_void_p)])
 SYMBOLS["cpbus_group_destroy"] = (C.c_int, [C.c_void_p])
 SYMBOLS.update({f"cpbus_group_{name}": SYMBOLS[f"cpbus_{name}"] for name in GROUP_CALLS})

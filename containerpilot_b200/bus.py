@@ -298,6 +298,33 @@ class Bus:
                   "cpbus_drain_ready")
         return out[: total.value], ready[: n_ready.value], next_sub.value
 
+    def lagging(self, first_sub: int, n: int, start_sub: int | None = None, min_backlog: int = 1, cap: int | None = None):
+        """Read-only consumer backlog of mailboxes [first_sub, first_sub+n) in cyclic order from start_sub (default
+        first_sub): returns (entries, next_sub, summary).  entries is a LAG_DTYPE array of the first `cap` (default n)
+        subscribed mailboxes with backlog >= min_backlog; next_sub continues the walk; summary is a dict over the whole
+        range (active, lagging, backlog_total, backlog_max, lost_total, hist)."""
+        start_sub = first_sub if start_sub is None else start_sub
+        cap = n if cap is None else cap
+        out = np.zeros(max(1, min(cap, n)), dtype=nat.LAG_DTYPE)
+        n_out, next_sub, s = C.c_size_t(), C.c_uint32(), nat.LagSummary()
+        nat.check(self._lib.cpbus_lagging(self._h, first_sub, n, start_sub, min_backlog, out.ctypes.data if cap else None, cap,
+                                          C.byref(n_out), C.byref(next_sub), C.byref(s)), "cpbus_lagging")
+        summary = {k: getattr(s, k) for k, _ in nat.LagSummary._fields_ if k != "hist"}
+        summary["hist"] = list(s.hist)
+        return out[: n_out.value], next_sub.value, summary
+
+    def blockers(self, cap: int | None = None) -> np.ndarray:
+        """Lossless mode: the global ids of the mailboxes the next flush cannot get past, ascending (the first `cap`;
+        default all of them).  Empty in throughput mode."""
+        n = C.c_size_t()
+        want = 1024 if cap is None else cap
+        while True:
+            out = np.zeros(max(1, want), dtype=np.uint32)
+            nat.check(self._lib.cpbus_blockers(self._h, out.ctypes.data if want else None, want, C.byref(n)), "cpbus_blockers")
+            if cap is not None or n.value <= want:   # (the query changes no state: asking again gives the same list)
+                return out[: min(want, n.value)]
+            want = n.value
+
     def peek_window(self, sub_id: int, cap: int | None = None) -> np.ndarray:
         cap = cap or self.ring_cap
         out = np.zeros(cap, dtype=EVENT_DTYPE)

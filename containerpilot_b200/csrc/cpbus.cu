@@ -140,6 +140,12 @@ struct cpbus {
   cpbus_ready* d_ready = nullptr; uint32_t* d_ready_slot = nullptr; size_t ready_stage_cap = 0;
   unsigned long long* h_ready_hdr = nullptr;   // pinned + mapped: the header the gather kernel hands to the host
   unsigned long long* d_ready_hdr = nullptr;   // device alias of h_ready_hdr
+  // cpbus_lagging / cpbus_blockers: look-back and summary words sized for every subscriber, the header the scans hand to the
+  // host, the blocker ids (lossless buses) and the lagging entries (grown on demand); all but d_lag_lb pinned + mapped
+  unsigned long long* d_lag_lb = nullptr;
+  unsigned long long* h_lag_hdr = nullptr; unsigned long long* d_lag_hdr = nullptr;
+  uint32_t* h_block = nullptr; uint32_t* d_block = nullptr;
+  cpbus_lag* h_lag = nullptr; cpbus_lag* d_lag = nullptr; size_t lag_cap = 0;
   uint32_t subs_per_warp = 0;             // 0 = auto
   uint32_t order_block = 0;               // mask order is built per block of this many consecutive subscribers (0 = one global order)
   bool pdl = true;                        // programmatic dependent launch of consecutive fan-outs
@@ -383,6 +389,8 @@ int preload_round_kernels(cpbus* b) {
   CK(cudaFuncGetAttributes(&a, stream_round_agree_kernel));
   CK(cudaFuncGetAttributes(&a, consume_all_kernel));     // cpbus_consume_all queues behind waiting rounds
   CK(cudaFuncGetAttributes(&a, digest_fold_kernel));     // as does cpbus_digest_fold_begin
+  CK(cudaFuncGetAttributes(&a, blockers_scan_kernel));   // a stalled publisher's query on another shard of this thread
+  CK(cudaFuncGetAttributes(&a, lagging_scan_kernel));    // ... and the pump's
   done[b->device & 63] = true;
   return CPBUS_OK;
 }
@@ -832,6 +840,10 @@ int cpbus_create(const cpbus_config* cfg, cpbus_t** out) try {
       cudaMemsetAsync(b->d_acct, 0, sizeof(DevPubAcct), b->stream) != cudaSuccess) return fail(CPBUS_ECUDA);
   if (mapped_alloc(64, &b->h_err, &b->d_err) != cudaSuccess) return fail(CPBUS_ENOMEM);
   memset(b->h_err, 0, 64);
+  // cpbus_lagging / cpbus_blockers: allocated here, so that neither query allocates (or frees) while a round may wait
+  ALLOC(b->d_lag_lb, (kLagLbOffset + (N + kReadyTile - 1) / kReadyTile) * sizeof(unsigned long long));
+  if (mapped_alloc(kLagHdrWords * sizeof(unsigned long long), &b->h_lag_hdr, &b->d_lag_hdr) != cudaSuccess) return fail(CPBUS_ENOMEM);
+  if (b->lossless && mapped_alloc(N * sizeof(uint32_t), &b->h_block, &b->d_block) != cudaSuccess) return fail(CPBUS_ENOMEM);
   if (cudaMallocHost((void**)&b->h_acct, offsetof(DevPubAcct, pair_key)) != cudaSuccess) return fail(CPBUS_ENOMEM);
   for (int i = 0; i < cpbus::kPrefetch; i++) ALLOC(b->d_prefetch[i], (size_t)B * sizeof(cpbus_event));
   ALLOC(b->d_result, sizeof(DevResultSlot) * kResultRing * kResultSub);
@@ -891,6 +903,10 @@ int cpbus_destroy(cpbus_t* b) try {
   cudaFree(b->d_drain); cudaFree(b->d_drain_idx);
   cudaFree(b->d_ready_lb); cudaFree(b->d_ready); cudaFree(b->d_ready_slot);
   if (b->h_ready_hdr) cudaFreeHost(b->h_ready_hdr);
+  cudaFree(b->d_lag_lb);
+  if (b->h_lag_hdr) cudaFreeHost(b->h_lag_hdr);
+  if (b->h_block) cudaFreeHost(b->h_block);
+  if (b->h_lag) cudaFreeHost(b->h_lag);
   cudaFree(b->d_result); cudaFree(b->d_batch_local); cudaFree(b->d_admit_batch); cudaFree(b->d_pf_buf); cudaFree(b->d_pf_state); cudaFree(b->d_acct);
   if (b->h_err) cudaFreeHost(b->h_err);
   if (b->h_acct) cudaFreeHost(b->h_acct);
@@ -2091,6 +2107,90 @@ static int drain_ready_impl(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t
   return CPBUS_OK;
 }
 
+// Consumer backlog: one read-only scan of the range's control blocks; the entries and the header {selected, cut position,
+// summary} arrive in mapped pinned memory, so one sync is the only wait.  *all_returned: every lagging mailbox was returned.
+static int lagging_impl(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start_sub, uint32_t min_backlog, cpbus_lag* out,
+                        size_t cap, size_t* n_out, uint32_t* next_sub, cpbus_lag_summary* sum, bool* all_returned) {
+  static_assert(sizeof(cpbus_lag) == 16 && sizeof(cpbus_lag_summary) == kLagSumWords * sizeof(unsigned long long), "C-ABI layout");
+  if (start_sub < first_sub || start_sub - first_sub >= n) return CPBUS_EINVAL;
+  const uint32_t l = first_sub - b->cfg.sub_id_base;
+  if (first_sub < b->cfg.sub_id_base || (uint64_t)l + n > b->n_next) return CPBUS_ENOENT;
+  std::lock_guard<std::mutex> g(b->mu);
+  int rc = enter(b); if (rc) return rc;
+  const size_t ecap = std::min<size_t>(cap, n);   // never more entries than mailboxes
+  if (b->lag_cap < ecap) {
+    if (b->h_lag) cudaFreeHost(b->h_lag);
+    b->h_lag = nullptr; b->d_lag = nullptr; b->lag_cap = 0;
+    CK(mapped_alloc(ecap * sizeof(cpbus_lag), &b->h_lag, &b->d_lag));
+    b->lag_cap = ecap;
+  }
+  const uint32_t tiles = (n + kReadyTile - 1) / kReadyTile;
+  CK(cudaMemsetAsync(b->d_lag_lb, 0, (kLagLbOffset + (size_t)tiles) * sizeof(unsigned long long), b->stream));
+  const uint32_t rot = start_sub - first_sub;
+  lagging_scan_kernel<<<tiles, kThreads, 0, b->stream>>>(b->d_ctl, l, n, rot, b->R, b->lossless ? 1u : 0u, b->cfg.sub_id_base,
+                                                          min_backlog, ecap, b->d_lag_lb, b->d_lag, b->d_lag_hdr);
+  CK(cudaGetLastError());
+  b->st.kernel_launches++;
+  CK(cudaStreamSynchronize(b->stream));
+  const volatile unsigned long long* hdr = b->h_lag_hdr;
+  const uint64_t total = hdr[0], cut = hdr[1];
+  const size_t got = (size_t)std::min<uint64_t>(total, ecap);
+  if (got) memcpy(out, b->h_lag, got * sizeof(cpbus_lag));
+  if (sum) {
+    uint64_t w[kLagSumWords];
+    for (uint32_t i = 0; i < kLagSumWords; i++) w[i] = hdr[2 + i];
+    memcpy(sum, w, sizeof(w));
+  }
+  *n_out = got;
+  *all_returned = total <= ecap;
+  *next_sub = *all_returned ? start_sub : first_sub + (uint32_t)((rot + cut) % n);
+  return CPBUS_OK;
+}
+
+int cpbus_lagging(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start_sub, uint32_t min_backlog, cpbus_lag* out,
+                  size_t cap, size_t* n_out, uint32_t* next_sub, cpbus_lag_summary* sum) try {
+  if (!b || !n_out || !next_sub || !n || (!out && cap)) return CPBUS_EINVAL;
+  bool all = false;
+  return lagging_impl(b, first_sub, n, start_sub, min_backlog, out, cap, n_out, next_sub, sum, &all);
+} CPBUS_CATCH
+
+// The subscribed mailboxes of this shard that refuse the next unit U of a lossless flush: the record `rec` (NULL: ticks
+// only) with the ticks due by t.  The caller holds b->mu and has resolved.  No kernel when the room bound proves that U fits
+// (admit_fits without taking anything from the bound).
+static int blockers_impl(cpbus* b, const cpbus_event* rec, uint64_t t, uint32_t* out, size_t cap, size_t* n) {
+  *n = 0;
+  const bool timers_on = b->n_timers > 0 && b->K > 0;
+  if (b->n_next == 0 || b->room_lb >= admit_need(rec ? 1 : 0, t, b->last_watermark, b->min_period, b->K, timers_on)) return CPBUS_OK;
+  const uint32_t tiles = (b->n_next + kReadyTile - 1) / kReadyTile;
+  CK(cudaMemsetAsync(b->d_lag_lb, 0, (kLagLbOffset + (size_t)tiles) * sizeof(unsigned long long), b->stream));
+  const size_t ecap = std::min<size_t>(cap, b->n_next);
+  blockers_scan_kernel<<<tiles, kThreads, 0, b->stream>>>(b->d_ctl, b->d_timers, b->n_paired > 0 ? b->d_pairs : nullptr, b->n_next,
+                                                           b->R, b->K, b->cfg.sub_id_base, timers_on ? 1u : 0u, rec ? 1u : 0u,
+                                                           rec ? *rec : cpbus_event{}, t, ecap, b->d_lag_lb, b->d_block,
+                                                           b->d_lag_hdr);
+  CK(cudaGetLastError());
+  b->st.kernel_launches++;
+  CK(cudaStreamSynchronize(b->stream));
+  const size_t total = (size_t)*(const volatile unsigned long long*)b->h_lag_hdr;
+  if (total && ecap) memcpy(out, b->h_block, std::min(total, ecap) * sizeof(uint32_t));
+  *n = total;
+  return CPBUS_OK;
+}
+
+int cpbus_blockers(cpbus_t* b, uint32_t* out, size_t cap, size_t* n) try {
+  if (!b || !n || (!out && cap)) return CPBUS_EINVAL;
+  std::lock_guard<std::mutex> g(b->mu);
+  int rc = enter(b); if (rc) return rc;
+  *n = 0;
+  if (!b->lossless) return CPBUS_OK;
+  if (b->n_staged) {   // U = the first staged record with the ticks due by its ts_ns
+    const cpbus_event e = b->h_batch[b->cur][0];
+    return blockers_impl(b, &e, e.ts_ns, out, cap, n);
+  }
+  if (b->n_timers == 0 || b->now == b->last_watermark) return CPBUS_OK;   // the next flush launches nothing (flush_staged)
+  return blockers_impl(b, nullptr, b->now, out, cap, n);
+} CPBUS_CATCH
+
 // Device-side consumer: every mailbox of this shard is read to the end and its records are discarded.
 int cpbus_consume_all(cpbus_t* b) try {
   if (!b) return CPBUS_EINVAL;
@@ -2764,6 +2864,64 @@ int cpbus_group_drain_ready(cpbus_group_t* g, uint32_t first_sub, uint32_t n, ui
     done += cnt;
   }
   *n_ready = nr; *total = tot;
+  return CPBUS_OK;
+} CPBUS_CATCH
+
+// The cyclic walk of cpbus_lagging over the shards: each piece on one shard is scanned with the cap still left; the first
+// piece that could not return all of its lagging mailboxes sets next_sub, and every piece adds to the summary.
+int cpbus_group_lagging(cpbus_group_t* g, uint32_t first_sub, uint32_t n, uint32_t start_sub, uint32_t min_backlog, cpbus_lag* out,
+                        size_t cap, size_t* n_out, uint32_t* next_sub, cpbus_lag_summary* sum) try {
+  if (!g || !n_out || !next_sub || !n || (!out && cap)) return CPBUS_EINVAL;
+  if (start_sub < first_sub || start_sub - first_sub >= n) return CPBUS_EINVAL;
+  const uint32_t i0 = first_sub - g->base;
+  if (first_sub < g->base || (uint64_t)i0 + n > g->n_next) return CPBUS_ENOENT;
+  const uint32_t rot = start_sub - first_sub;
+  cpbus_lag_summary acc{};
+  size_t got = 0;
+  bool cut = false;
+  *next_sub = start_sub;
+  for (uint32_t done = 0; done < n;) {
+    const uint32_t i = i0 + (rot + done) % n;                       // global index of the walk's next mailbox
+    const uint32_t k = group_shard_of(g, i);
+    const uint32_t cnt = std::min({n - done, g->first[k + 1] - i, i0 + n - i});
+    const uint32_t a = g->base + i;
+    cpbus_lag_summary part{};
+    size_t n_s = 0;
+    uint32_t next_s = a;
+    bool all = false;
+    const int rc = lagging_impl(g->shards[k], a, cnt, a, min_backlog, out ? out + got : nullptr, cap - got, &n_s, &next_s, &part, &all);
+    if (rc) return rc;
+    got += n_s;
+    if (!all && !cut) { *next_sub = next_s; cut = true; }
+    acc.active += part.active; acc.lagging += part.lagging; acc.backlog_total += part.backlog_total;
+    acc.backlog_max = std::max(acc.backlog_max, part.backlog_max); acc.lost_total += part.lost_total;
+    for (int h = 0; h < 33; h++) acc.hist[h] += part.hist[h];
+    done += cnt;
+  }
+  *n_out = got;
+  if (sum) *sum = acc;
+  return CPBUS_OK;
+} CPBUS_CATCH
+
+// The group's next unit (its staged remainder and clock, as cpbus_blockers reads the single bus's) on every shard; the
+// shards own ascending id ranges, so their lists concatenate in ascending order.
+int cpbus_group_blockers(cpbus_group_t* g, uint32_t* out, size_t cap, size_t* n) try {
+  if (!g || !n || (!out && cap)) return CPBUS_EINVAL;
+  *n = 0;
+  if (!g->lossless) return CPBUS_OK;
+  const cpbus_event* rec = g->n_staged ? &g->staged[0] : nullptr;
+  if (!rec && (g->n_timers == 0 || g->now == g->last_watermark)) return CPBUS_OK;   // the next flush launches nothing
+  const uint64_t t = rec ? rec->ts_ns : g->now;
+  size_t tot = 0;
+  for (cpbus* s : g->shards) {
+    std::lock_guard<std::mutex> lk(s->mu);
+    int rc = enter(s); if (rc) return rc;
+    const size_t used = std::min(tot, cap);
+    size_t n_s = 0;
+    if ((rc = blockers_impl(s, rec, t, out ? out + used : nullptr, cap - used, &n_s))) return rc;
+    tot += n_s;
+  }
+  *n = tot;
   return CPBUS_OK;
 } CPBUS_CATCH
 

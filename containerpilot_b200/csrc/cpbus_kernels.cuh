@@ -743,6 +743,215 @@ __global__ void __launch_bounds__(kThreads) drain_ready_gather_kernel(const cpbu
   }
 }
 
+// ---- consumer backlog (cpbus_lagging) and the mailboxes a lossless flush waits on (cpbus_blockers) ----------------------
+// Read-only scans over the control blocks.  Each numbers the mailboxes it selects in position order with the single-pass
+// decoupled look-back of drain_ready_scan_kernel, reduced to one count per tile: flag (bits 62-63, kLbAgg / kLbIncl) |
+// selected mailboxes (bits 0-61).  Work buffer `lb`: [0] tile counter, [1] CTAs done, [2] selected mailboxes, [3] position
+// of the first selected mailbox not returned, [kLagSumOffset ..) summary (cpbus_lag_summary), [kLagLbOffset ..) tile status.
+constexpr uint32_t kLagHist = 33;
+constexpr uint32_t kLagSumWords = 5 + kLagHist;   // active, lagging, backlog_total, backlog_max, lost_total, hist[33]
+constexpr uint32_t kLagSumOffset = 8, kLagLbOffset = 48;
+constexpr uint32_t kLagHdrWords = 2 + kLagSumWords;   // handed to the host: {selected, cut position, summary}
+static_assert(kLagSumOffset + kLagSumWords <= kLagLbOffset, "summary words overlap the tile status");
+constexpr unsigned long long kLbCountMask = (1ull << 62) - 1;
+
+// Position order index of every selected item of this thread's kReadyItems items (item k = position
+// tile * kReadyTile + k * kThreads + threadIdx.x).  The last tile writes the total to *total.
+__device__ __forceinline__ void select_compact(const bool (&sel)[kReadyItems], unsigned long long (&idx)[kReadyItems],
+                                               uint32_t tile, unsigned long long* lb, unsigned long long* total) {
+  __shared__ uint32_t s_cnt[32];             // per (item, warp) chunk: selected mailboxes, then their exclusive prefix
+  __shared__ unsigned long long s_base;
+  unsigned long long* status = lb + kLagLbOffset;
+  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  uint32_t before[kReadyItems];
+#pragma unroll
+  for (uint32_t k = 0; k < kReadyItems; k++) {
+    const uint32_t bal = __ballot_sync(0xffffffffu, sel[k]);
+    before[k] = __popc(bal & ((1u << lane) - 1u));
+    if (lane == 0) s_cnt[k * kWarpsPerCta + warp] = __popc(bal);
+  }
+  __syncthreads();
+  if (warp == 0) {
+    const uint32_t c0 = s_cnt[lane];
+    uint32_t c = c0;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const uint32_t co = __shfl_up_sync(0xffffffffu, c, o);
+      if ((int)lane >= o) c += co;
+    }
+    s_cnt[lane] = c - c0;
+    const unsigned long long agg = __shfl_sync(0xffffffffu, c, 31);
+    unsigned long long ex = 0;
+    if (tile == 0) {
+      if (lane == 0) *reinterpret_cast<volatile unsigned long long*>(status) = kLbIncl | agg;
+    } else {
+      if (lane == 0) *reinterpret_cast<volatile unsigned long long*>(status + tile) = kLbAgg | agg;
+      for (int pred = (int)tile - 1;; pred -= 32) {
+        const int j = pred - (int)lane;
+        unsigned long long v = kLbIncl;   // before tile 0: an empty inclusive prefix (never summed, tile 0 stops the walk)
+        do {
+          if (j >= 0) v = *reinterpret_cast<volatile unsigned long long*>(status + j);
+        } while (__any_sync(0xffffffffu, (v >> 62) == 0));
+        const uint32_t incl = __ballot_sync(0xffffffffu, (v >> 62) == 2);
+        const uint32_t stop = incl ? (uint32_t)(__ffs(incl) - 1) : 31u;
+        ex += warp_sum64(lane <= stop ? v & kLbCountMask : 0ull);
+        if (incl) break;
+      }
+      if (lane == 0) *reinterpret_cast<volatile unsigned long long*>(status + tile) = kLbIncl | (ex + agg);
+    }
+    if (lane == 0) {
+      s_base = ex;
+      if (tile == gridDim.x - 1) *total = ex + agg;
+    }
+  }
+  __syncthreads();
+#pragma unroll
+  for (uint32_t k = 0; k < kReadyItems; k++) idx[k] = s_base + s_cnt[k * kWarpsPerCta + warp] + before[k];
+}
+
+// Mailboxes [first, first + n) in cyclic position order from rot (as drain_ready_scan_kernel).  A subscribed mailbox holds
+// backlog = tail - cursor records (cursor = head, or in throughput mode max(head, tail - ring_cap)) and has lost cursor -
+// head; it is listed when backlog >= min_backlog.  Entries [0, cap) go straight to the host's mapped buffer `out`; the
+// summary is gathered per CTA in shared memory, added into lb with one atomic per field, and the last CTA to finish hands
+// {selected, cut position, summary} to the host through mapped memory (h_hdr).  Nothing is written to the control blocks.
+__global__ void __launch_bounds__(kThreads) lagging_scan_kernel(const SubCtl* __restrict__ ctl, uint32_t first, uint32_t n,
+                                                                uint32_t rot, uint32_t ring_cap, uint32_t lossless,
+                                                                uint32_t sub_base, uint32_t min_backlog, unsigned long long cap,
+                                                                unsigned long long* lb, cpbus_lag* __restrict__ out,
+                                                                unsigned long long* h_hdr) {
+  __shared__ uint32_t s_tile, s_last;
+  __shared__ uint32_t s_hist[kLagHist];
+  __shared__ unsigned long long s_sum[5];
+  const uint32_t lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) s_tile = atomicAdd(reinterpret_cast<unsigned int*>(lb), 1u);
+  if (threadIdx.x < kLagHist) s_hist[threadIdx.x] = 0;
+  if (threadIdx.x < 5) s_sum[threadIdx.x] = 0;
+  __syncthreads();
+  const uint32_t tile = s_tile;
+  bool sel[kReadyItems];
+  uint32_t loc[kReadyItems], bl[kReadyItems];
+  unsigned long long lost[kReadyItems], idx[kReadyItems];
+  unsigned long long act = 0, lag = 0, btot = 0, bmax = 0, ltot = 0;
+#pragma unroll
+  for (uint32_t k = 0; k < kReadyItems; k++) {   // item k of the tile = positions k*kThreads .. +kThreads: coalesced loads
+    const uint32_t p = tile * kReadyTile + k * kThreads + threadIdx.x;
+    sel[k] = false; loc[k] = 0; bl[k] = 0; lost[k] = 0;
+    if (p < n) {
+      unsigned long long q = (unsigned long long)rot + p;
+      if (q >= n) q -= n;
+      const uint32_t l = first + (uint32_t)q;
+      const ulonglong2 th = *reinterpret_cast<const ulonglong2*>(ctl + l);   // {tail, head}
+      const uint32_t m = ctl[l].mask;
+      if (m & kActiveBit) {
+        unsigned long long c = th.y;
+        if (!lossless && th.x > ring_cap && th.x - ring_cap > c) c = th.x - ring_cap;   // overwritten before being taken
+        const uint32_t b = (uint32_t)(th.x - c);
+        loc[k] = l; bl[k] = b; lost[k] = c - th.y;
+        sel[k] = b >= min_backlog;
+        act++; lag += sel[k] ? 1u : 0u; btot += b; ltot += c - th.y; bmax = b > bmax ? b : bmax;
+        atomicAdd(&s_hist[b ? 32 - __clz(b) : 0], 1u);   // [0] = 0, [k] = [2^(k-1), 2^k)
+      }
+    }
+  }
+  act = warp_sum64(act); lag = warp_sum64(lag); btot = warp_sum64(btot); ltot = warp_sum64(ltot);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) { const unsigned long long x = shfl64(bmax, (int)(lane ^ o)); bmax = x > bmax ? x : bmax; }
+  if (lane == 0) {
+    atomicAdd(&s_sum[0], act); atomicAdd(&s_sum[1], lag); atomicAdd(&s_sum[2], btot); atomicMax(&s_sum[3], bmax);
+    atomicAdd(&s_sum[4], ltot);
+  }
+  select_compact(sel, idx, tile, lb, lb + 2);   // (its __syncthreads also orders the shared summary)
+#pragma unroll
+  for (uint32_t k = 0; k < kReadyItems; k++) {
+    if (!sel[k]) continue;
+    if (idx[k] < cap) out[idx[k]] = cpbus_lag{sub_base + loc[k], bl[k], lost[k]};
+    else if (idx[k] == cap) lb[3] = tile * kReadyTile + k * kThreads + threadIdx.x;   // the first one not returned
+  }
+  if (tile == gridDim.x - 1 && threadIdx.x == 0 && lb[2] <= cap) lb[3] = n;   // every selected mailbox was returned
+  unsigned long long* sum = lb + kLagSumOffset;
+  if (threadIdx.x < 5) {
+    const unsigned long long v = s_sum[threadIdx.x];
+    if (v) { if (threadIdx.x == 3) atomicMax(&sum[3], v); else atomicAdd(&sum[threadIdx.x], v); }
+  } else if (threadIdx.x < 5 + kLagHist) {
+    const uint32_t v = s_hist[threadIdx.x - 5];
+    if (v) atomicAdd(&sum[threadIdx.x], (unsigned long long)v);
+  }
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) s_last = atomicAdd(reinterpret_cast<unsigned int*>(lb + 1), 1u) == gridDim.x - 1;
+  __syncthreads();
+  if (s_last && threadIdx.x < kLagHdrWords) {   // every CTA's atomics and header words are in: hand them over
+    __threadfence();
+    h_hdr[threadIdx.x] = reinterpret_cast<volatile unsigned long long*>(lb)[threadIdx.x < 2 ? 2 + threadIdx.x
+                                                                                            : kLagSumOffset + threadIdx.x - 2];
+  }
+}
+
+// The share of mailbox s in the next unit U of a lossless flush: the ticks of its armed slots due by t, counted and
+// saturated as admit_body counts them, plus one if it takes U's record (has_rec).  Only the hot half {next_due, period} of
+// a timer slot is read, and only for the slots the mask word's hint names; the pair row only for a broadcast record whose
+// code is not in the mask.  (cpbus_blockers only: admit_body keeps its own loop.)
+__device__ __forceinline__ unsigned long long unit_share(uint32_t s, uint32_t m, const DevTimer* __restrict__ timers, uint32_t K,
+                                                         uint32_t timers_on, const uint2* __restrict__ pairs, uint32_t has_rec,
+                                                         const cpbus_event& rec, uint64_t t, uint32_t gid) {
+  unsigned long long k = 0;
+  const uint32_t nslots = timers_on ? min((m >> kTimerHintShift) & 0xFu, K) : 0u;
+  const uint64_t w_due = min(t, kTimerIdle - 1);
+  for (uint32_t j = 0; j < nslots; j++) {
+    const ulonglong2 hot = *reinterpret_cast<const ulonglong2*>(timers + (size_t)s * K + j);   // {next_due, period}
+    if (hot.x != kTimerIdle && hot.x <= w_due) k += hot.y ? (w_due - hot.x) / hot.y + 1u : 1u;
+  }
+  if (has_rec) {
+    bool want;
+    if (rec.target == CPBUS_TARGET_ALL) {
+      want = rec.code < CPBUS_N_CODES && ((m >> rec.code) & 1u);
+      if (!want && rec.code < CPBUS_N_CODES && pairs && (m & kPairBit)) {
+        const uint2* my = pairs + (size_t)s * CPBUS_MAX_PAIRS;
+        for (uint32_t j = 0; j < CPBUS_MAX_PAIRS && !want; j++) {
+          const uint2 pr = my[j];
+          if (pr.x == kPairNone) break;
+          want = pr.x == rec.code && pr.y == rec.source_id;
+        }
+      }
+    } else want = rec.target == gid;
+    k += want ? 1u : 0u;
+  }
+  return k;
+}
+
+// cpbus_blockers: the subscribed mailboxes whose share of U exceeds their room ring_cap - (tail - head), ascending.  Ids
+// [0, cap) go straight to the host's mapped buffer `out`; the last tile writes how many there are to h_total.
+__global__ void __launch_bounds__(kThreads) blockers_scan_kernel(const SubCtl* __restrict__ ctl, const DevTimer* __restrict__ timers,
+                                                                 const uint2* __restrict__ pairs, uint32_t n, uint32_t ring_cap,
+                                                                 uint32_t K, uint32_t sub_base, uint32_t timers_on,
+                                                                 uint32_t has_rec, const cpbus_event rec, uint64_t t,
+                                                                 unsigned long long cap, unsigned long long* lb,
+                                                                 uint32_t* __restrict__ out, unsigned long long* h_total) {
+  __shared__ uint32_t s_tile;
+  if (threadIdx.x == 0) s_tile = atomicAdd(reinterpret_cast<unsigned int*>(lb), 1u);
+  __syncthreads();
+  const uint32_t tile = s_tile;
+  bool sel[kReadyItems];
+  unsigned long long idx[kReadyItems];
+#pragma unroll
+  for (uint32_t k = 0; k < kReadyItems; k++) {
+    const uint32_t s = tile * kReadyTile + k * kThreads + threadIdx.x;
+    sel[k] = false;
+    if (s < n) {
+      const ulonglong2 th = *reinterpret_cast<const ulonglong2*>(ctl + s);   // {tail, head}
+      const uint32_t m = ctl[s].mask;
+      if (m & kActiveBit) {
+        const unsigned long long room = ring_cap - min((unsigned long long)ring_cap, th.x - th.y);
+        sel[k] = unit_share(s, m, timers, K, timers_on, pairs, has_rec, rec, t, sub_base + s) > room;
+      }
+    }
+  }
+  select_compact(sel, idx, tile, lb, h_total);
+#pragma unroll
+  for (uint32_t k = 0; k < kReadyItems; k++)
+    if (sel[k] && idx[k] < cap) out[idx[k]] = sub_base + tile * kReadyTile + k * kThreads + threadIdx.x;
+}
+
 // (count, digest) folds over a range of mailboxes: one 32-byte result instead of 16 B per subscriber
 __global__ void digest_fold_kernel(const SubCtl* ctl, uint32_t first, uint32_t n, uint32_t sub_base,
                                    unsigned long long* out4) {

@@ -192,6 +192,7 @@ EVENTS_CPBUS_CALL(subscribe) EVENTS_CPBUS_CALL(subscribe_pairs) EVENTS_CPBUS_CAL
 EVENTS_CPBUS_CALL(publish) EVENTS_CPBUS_CALL(send) EVENTS_CPBUS_CALL(advance) EVENTS_CPBUS_CALL(flush)
 EVENTS_CPBUS_CALL(timer_add) EVENTS_CPBUS_CALL(timer_cancel) EVENTS_CPBUS_CALL(drain) EVENTS_CPBUS_CALL(drain_ready)
 EVENTS_CPBUS_CALL(debug_events) EVENTS_CPBUS_CALL(intern) EVENTS_CPBUS_CALL(intern_ephemeral) EVENTS_CPBUS_CALL(source)
+EVENTS_CPBUS_CALL(lagging) EVENTS_CPBUS_CALL(blockers)
 #undef EVENTS_CPBUS_CALL
 
 namespace detail {
@@ -362,6 +363,45 @@ class EventBus {   // events/bus.go:12-22
     return it == counter_.end() ? 0 : it->second;
   }
   cpbus_t* handle() { return h_.one; }   // (nullptr on a group)
+
+  // ---- extensions, NOT in the reference API ----
+  // The subscribers whose full mailboxes the next flush cannot get past (cpbus_blockers: what a goroutine dump of the Go bus
+  // shows as the channel the publisher sits on), timer-only channels' implicit subscribers included, in id order.  Reads
+  // state only: nothing is flushed or pumped.
+  std::vector<Subscriber*> Blocking() {
+    std::lock_guard<std::recursive_mutex> l(lock_);
+    std::vector<uint32_t> ids(64);
+    size_t n = 0;
+    for (;;) {
+      Check(cpbus_blockers(h_, ids.data(), ids.size(), &n), "cpbus_blockers");
+      if (n <= ids.size()) break;
+      ids.resize(n);
+    }
+    std::vector<Subscriber*> out;
+    for (size_t i = 0; i < n; i++) {
+      auto it = by_id_.find(ids[i]);
+      if (it != by_id_.end()) out.push_back(it->second);
+    }
+    return out;
+  }
+  // Every subscribed mailbox holding at least `min_backlog` undrained records (cpbus_lagging), in id order.
+  struct Lag { Subscriber* sub; uint32_t backlog; uint64_t lost; };
+  std::vector<Lag> Lagging(uint32_t min_backlog = 1) {
+    std::lock_guard<std::recursive_mutex> l(lock_);
+    std::vector<Lag> out;
+    if (by_id_.empty()) return out;
+    const uint32_t lo = by_id_.begin()->first, n = by_id_.rbegin()->first - lo + 1;
+    std::vector<cpbus_lag> ent(n);
+    size_t got = 0;
+    uint32_t next = lo;
+    Check(cpbus_lagging(h_, lo, n, lo, min_backlog, ent.data(), ent.size(), &got, &next, (cpbus_lag_summary*)nullptr),
+          "cpbus_lagging");
+    for (size_t i = 0; i < got; i++) {
+      auto it = by_id_.find(ent[i].sub_id);
+      if (it != by_id_.end()) out.push_back(Lag{it->second, ent[i].backlog, ent[i].lost});
+    }
+    return out;
+  }
 
  private:
   friend class Subscriber;

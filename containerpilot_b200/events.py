@@ -10,6 +10,8 @@ Same names, argument meaning and error behaviour as the Go API
     Publisher / Subscriber (+ Rx)                      events/publisher.go, subscriber.go
     NewEventTimer / NewEventTimeout                    events/timer.go
 
+Extensions that the reference does not have are marked as such: `EventBus.Blocking()` and `EventBus.Lagging()`.
+
 `NewEventTimer` / `NewEventTimeout` take any `Chan`, exactly as the Go functions take any `chan Event`
 (events/timer.go:12-16,40-45): when the channel is not the Rx of a subscribed Subscriber (a Watch's private channel,
 watches/watches.go:37,71) the bus gives it a mailbox of its own — an implicit subscriber with an empty code mask that
@@ -226,6 +228,30 @@ class EventBus:
         if rc == nat.EAGAIN:
             raise BlockingIOError("flush would block: a subscriber mailbox is full")
         nat.check(rc, "cpbus_flush")
+
+    # ---- extensions, NOT in the reference API: who holds the publisher up, who falls behind ----
+    def _by_id(self):
+        """mailbox id -> Subscriber, the implicit timer-only ones included"""
+        out = {sid: s for s, sid in self._subs.items()}
+        out.update({s._id: s for s in self._implicit.values() if s._id is not None})
+        return out
+
+    def Blocking(self):
+        """The Subscribers whose full mailboxes the next flush cannot get past (what a goroutine dump of the Go bus shows
+        as the channel the publisher sits on), implicit timer-only ones included, in id order.  Empty in throughput mode
+        and while nothing is blocked.  Reads state only: nothing is flushed or drained."""
+        by_id = self._by_id()
+        return [by_id[int(i)] for i in self._bus.blockers() if int(i) in by_id]
+
+    def Lagging(self, min_backlog: int = 1):
+        """[(Subscriber, backlog, lost)] for every subscribed mailbox holding at least `min_backlog` undrained records, in
+        id order; `lost` counts records overwritten before they were drained (throughput mode only)."""
+        by_id = self._by_id()
+        if not by_id:
+            return []
+        n = max(by_id) + 1 - self._bus.sub_id_base
+        ent, _, _ = self._bus.lagging(self._bus.sub_id_base, n, min_backlog=min_backlog)
+        return [(by_id[int(e["sub_id"])], int(e["backlog"]), int(e["lost"])) for e in ent if int(e["sub_id"]) in by_id]
 
     # ---- used by Chan / Subscriber ----
     def _send(self, sub, event: Event):

@@ -415,6 +415,41 @@ typedef struct cpbus_ready {
 int cpbus_drain_ready(cpbus_t* bus, uint32_t first_sub, uint32_t n, uint32_t start_sub,
                       cpbus_event* out, size_t cap, cpbus_ready* ready, size_t ready_cap,
                       size_t* n_ready, size_t* total, uint32_t* next_sub);
+/* Consumer backlog, read-only: which subscribed mailboxes fall behind and by how much, without consuming anything (head never
+ * moves; a drain after this call returns exactly what it would have returned without it).  Mailboxes [first_sub,
+ * first_sub+n) are visited in cyclic id order from start_sub, as by cpbus_drain_ready; only subscribed ones count (the implicit
+ * mask-0 timer mailboxes included).  out[0 .. *n_out) = the first `cap` mailboxes with backlog >= min_backlog, in that
+ * order (min_backlog == 0: every subscribed mailbox).  *next_sub = the first such mailbox not returned, or start_sub when all
+ * were: passing it back visits every lagging mailbox exactly once.  *sum (may be NULL) covers the whole range whatever cap
+ * is.  Runs on the bus stream behind every earlier fan-out; does not flush staged events; the same state and arguments give
+ * byte-identical outputs.  Cost: one read of the range's control blocks on the device; host traffic is 16 * n_out bytes
+ * plus the summary and a constant; one stream synchronisation.
+ * CPBUS_EINVAL: n == 0, start_sub outside the range, a NULL n_out / next_sub, or out == NULL with cap > 0.
+ * CPBUS_ENOENT: the range is not within this shard's subscribers. */
+typedef struct cpbus_lag {
+  uint32_t sub_id;   /* global id (sub_id_base applied)                                                          */
+  uint32_t backlog;  /* undrained records: tail - cursor, cursor = head (lossless) or max(head, tail - ring_cap)    */
+  uint64_t lost;     /* throughput mode: cursor - head, exactly cpbus_ready.lost; 0 in lossless mode               */
+} cpbus_lag;         /* sizeof == 16 */
+typedef struct cpbus_lag_summary {
+  uint64_t active;          /* subscribed mailboxes in the range                                                  */
+  uint64_t lagging;         /* ... with backlog >= min_backlog                                                    */
+  uint64_t backlog_total, backlog_max, lost_total;   /* over the subscribed mailboxes of the range                */
+  uint64_t hist[33];        /* subscribed mailboxes by backlog: [0] = 0, [k] = [2^(k-1), 2^k)                     */
+} cpbus_lag_summary;
+int cpbus_lagging(cpbus_t* bus, uint32_t first_sub, uint32_t n, uint32_t start_sub, uint32_t min_backlog,
+                  cpbus_lag* out, size_t cap, size_t* n_out, uint32_t* next_sub, cpbus_lag_summary* sum);
+/* Lossless mode: the mailboxes the next flush cannot get past (what a Go goroutine dump shows as the channel the publisher
+ * sits on).  The next unit U is the first staged record together with every tick due at or before its ts_ns; with nothing
+ * staged, the ticks due by the bus clock that the next flush would fire.  A subscribed mailbox blocks when its share of U —
+ * the ticks of its armed slots due by then, plus one if it takes the record (code mask, {code, source} case, or unicast
+ * target) — exceeds its room ring_cap - (tail - head): its admissible prefix of the staged remainder is 0.
+ * out[0 .. min(cap, *n)) = the smallest blocking global ids, ascending; *n = how many there are.  After CPBUS_EAGAIN from
+ * cpbus_flush, cpbus_publish, cpbus_send, cpbus_advance or a membership / timer call, *n >= 1, and draining exactly these
+ * mailboxes lets the next flush deliver at least U (U takes at most 32/timers_per_sub + 1 ticks per slot plus one record,
+ * below ring_cap).  Changes no state and flushes nothing; no kernel when the room bound proves that U fits, and none in
+ * throughput mode (*n = 0).  CPBUS_EINVAL: NULL bus or n, or out == NULL with cap > 0. */
+int cpbus_blockers(cpbus_t* bus, uint32_t* out, size_t cap, size_t* n);
 /* Device-side consumer: every mailbox is read to the end and its records are discarded (head = tail), ordered behind
  * every earlier fan-out on the bus stream.  For subscribers nobody reads, and for measuring the lossless mode with
  * consumers that keep up. */
@@ -502,6 +537,11 @@ int cpbus_group_drain(cpbus_group_t* g, uint32_t sub_id, cpbus_event* out, size_
 int cpbus_group_drain_ready(cpbus_group_t* g, uint32_t first_sub, uint32_t n, uint32_t start_sub,
                             cpbus_event* out, size_t cap, cpbus_ready* ready, size_t ready_cap,
                             size_t* n_ready, size_t* total, uint32_t* next_sub);
+/* _lagging walks the shards in the single call's cyclic order with the cap that is left (as _drain_ready) and sums the
+ * summaries (backlog_max: the maximum); _blockers evaluates the group's staged remainder and clock on every shard. */
+int cpbus_group_lagging(cpbus_group_t* g, uint32_t first_sub, uint32_t n, uint32_t start_sub, uint32_t min_backlog,
+                        cpbus_lag* out, size_t cap, size_t* n_out, uint32_t* next_sub, cpbus_lag_summary* sum);
+int cpbus_group_blockers(cpbus_group_t* g, uint32_t* out, size_t cap, size_t* n);
 int cpbus_group_consume_all(cpbus_group_t* g);
 int cpbus_group_peek_window(cpbus_group_t* g, uint32_t sub_id, cpbus_event* out, size_t cap, size_t* n);
 int cpbus_group_digest(cpbus_group_t* g, uint32_t first_sub, uint32_t n, cpbus_digest_t* out);
