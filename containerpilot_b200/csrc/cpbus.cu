@@ -74,17 +74,37 @@ inline bool oneshot_fired(uint64_t next_due, uint64_t w) { return next_due <= w 
 // timer id = slot index (subscriber * K + k) | generation << 26: a late cancel from an old context cannot disarm a re-armed slot
 constexpr uint32_t kTimerSlotBits = 26, kTimerSlotMask = (1u << kTimerSlotBits) - 1u;
 
+// The host front end: what the single bus (cpbus) and the group (cpbus_group) keep over their whole id space, and what the
+// rules below share — the clock window (max_window), timer arming and retirement, staging (stage_one), the publish loop
+// (publish_burst), the clock's advance (advance_clock), the debug ring and the publish counts.
+struct HostFront {
+  uint32_t B = 0, K = 0;                  // batch_cap, timers per subscriber
+  // clock and ordinals
+  uint64_t now = 0, last_watermark = 0, seq = 0;
+  size_t n_staged = 0;
+  std::vector<HostTimer> h_timers;        // N*K, allocated on first timer
+  std::vector<size_t> oneshot_idx;        // armed one-shot timers (index into h_timers)
+  uint32_t n_timers = 0;
+  uint64_t min_period = UINT64_MAX;       // conservative lower bound over armed periodic timers
+  // DebugEvents ring (events/bus.go:18-21, 24-54)
+  int dbg_head = -1, dbg_tail = 0;
+  cpbus_event dbg[10]{};
+  std::deque<DbgItem> dbg_pending;        // debug-ring entries not yet enqueued (events, or markers of device batches)
+  PairCounter pub_pairs;                  // host publishes by (code << 32 | source_id), Metric excluded (bus.go:130-132)
+  uint64_t publishes = 0, published_by_code[CPBUS_N_CODES] = {};   // host publishes and sends; by code (Metric excluded)
+};
+
 }  // namespace
 
 struct cpbus_stream;
 
-struct cpbus {
+struct cpbus : HostFront {
   cpbus_config cfg{};
   int device = 0, sm_count = 132;
   size_t smem_per_sm = 228 * 1024, smem_reserved = 1024;   // shared memory per SM, and what the system keeps per CTA
   cudaStream_t stream = nullptr;
   bool own_stream = false;
-  uint32_t N = 0, R = 0, B = 0, K = 0;
+  uint32_t N = 0, R = 0;
   int store = CPBUS_STORE_V8;
   bool lossless = false, use_digest = false;
 
@@ -131,8 +151,6 @@ struct cpbus {
   // accounting of device-published batches (cpbus_publish_device*, cpbus_stream_fanout): done by the kernel's lead CTA
   DevPubAcct* d_acct = nullptr;
   DevPubAcct* h_acct = nullptr;               // pinned staging for cpbus_stats / cpbus_debug_events / cpbus_publish_counts
-  std::deque<DbgItem> dbg_pending;            // debug-ring entries not yet enqueued (events, or markers of device batches)
-  PairCounter pub_pairs;                              // host publishes by (code << 32 | source_id), Metric excluded (bus.go:130-132)
   cpbus_event* d_drain = nullptr; size_t drain_cap = 0;        // cpbus_drain_many staging
   uint2* d_drain_idx = nullptr; size_t drain_idx_cap = 0;
   // cpbus_drain_ready staging (records go to d_drain): header + tile counter + tile status, ready list, ring slot of each run
@@ -172,7 +190,6 @@ struct cpbus {
   DevStats* h_stats = nullptr;            // pinned
   unsigned long long* h_fold = nullptr;   // pinned
   int cur = 0;
-  size_t n_staged = 0;
 
   // registry mirror (events/bus.go:13 `registry map[*Subscriber]bool`)
   std::vector<uint32_t> h_mask;
@@ -183,21 +200,12 @@ struct cpbus {
   uint32_t* d_order = nullptr;            // active subscribers sorted by code mask (ORDERED fan-out)
   uint32_t n_order = 0, n_filtered = 0;   // n_filtered: active subscribers whose mask is not CPBUS_MASK_ALL
   bool order_dirty = true;
-  std::vector<size_t> oneshot_idx;        // armed one-shot timers (index into h_timers)
-  std::vector<HostTimer> h_timers;        // N*K, allocated on first timer
-  uint32_t n_next = 0, n_active = 0, n_timers = 0;
-  uint64_t min_period = UINT64_MAX;       // conservative lower bound over armed periodic timers
+  uint32_t n_next = 0, n_active = 0;
 
-  // clock and ordinals
-  uint64_t now = 0, last_watermark = 0, seq = 0;
   // lossless mode: a lower bound of the free slots of the FULLEST mailbox.  While a batch provably fits (bound >= what it
   // can append to one mailbox) the admission pass and its host sync are skipped; the bound is refreshed exactly whenever
   // the admission kernel does run, and reset by cpbus_consume_all.
   uint64_t room_lb = 0;
-
-  // DebugEvents ring (events/bus.go:18-21, 24-54)
-  int dbg_head = -1, dbg_tail = 0;
-  cpbus_event dbg[10]{};
 
   // intern table (Event.Source string <-> u32)
   std::unordered_map<std::string, uint32_t> intern;
@@ -213,6 +221,26 @@ struct cpbus {
 
   cpbus_stats_t st{};
   std::mutex mu;   // drain/stats from a second thread
+};
+
+// The group: one bus handle over the GPUs of a box (include/cpbus.h: cpbus_group_*).  Its host front end is the single
+// bus's, over the whole id space, and so are the rules that run on it (stage_one, publish_burst, advance_clock, the timer
+// table that sets the clock window, the debug ring and publish counts); only its flush differs (flush_staged of a group).
+// A flush becomes one RAW stream batch that every shard fans out in full: in lossless mode the group first runs the single
+// bus's admission (admit) on every shard and puts only the prefix every shard can take, with the single bus's partial
+// watermark.  (cpbus_stream_admit would hold a batch back until the ticks due by its watermark fit too, where a partial
+// cpbus_flush delivers the records and stalls on the ticks alone.)
+// Shard clocks: a shard's clock is its last launched watermark; a shard without timers is moved to the group clock with
+// cpbus_advance right before a timer is armed on it (no launch: it has no timer window), so every shard's `now + period`
+// is the single bus's.  A shard with timers already has the group clock there (the group has just flushed at `now`).
+struct cpbus_group : HostFront {
+  std::vector<cpbus*> shards;
+  std::vector<cpbus_stream*> streams;   // streams[0] owns the ring (shard 0), the others are attached
+  std::vector<uint32_t> first;          // global index (sub_id_base not applied) of each shard's subscriber 0; + a sentinel
+  uint32_t base = 0, N = 0;
+  bool lossless = false;
+  uint32_t n_next = 0, n_active = 0;
+  std::vector<cpbus_event> staged;      // B records
 };
 
 namespace {
@@ -258,19 +286,36 @@ uint32_t mask_word(const cpbus* b, uint32_t local) {
   return (b->h_mask[local] & CPBUS_MASK_ALL) | (hint << kTimerHintShift) | pair_bit | kActiveBit;
 }
 
-void dbg_ring_put(cpbus* b, const cpbus_event& e) {   // events/bus.go:24-31
-  b->dbg[(b->dbg_head + 1) % 10] = e;
-  int old = b->dbg_head;
-  b->dbg_head = (b->dbg_head + 1) % 10;
-  if (old != -1 && b->dbg_head == b->dbg_tail) b->dbg_tail = (b->dbg_tail + 1) % 10;
+void dbg_ring_put(HostFront* f, const cpbus_event& e) {   // events/bus.go:24-31
+  f->dbg[(f->dbg_head + 1) % 10] = e;
+  int old = f->dbg_head;
+  f->dbg_head = (f->dbg_head + 1) % 10;
+  if (old != -1 && f->dbg_head == f->dbg_tail) f->dbg_tail = (f->dbg_tail + 1) % 10;
 }
 
 // While the broadcast events of a device-published batch are still unknown to the host (a marker is pending), later
-// enqueues queue up behind it so that the ring keeps the global publish order; cpbus_debug_events resolves them.
-void dbg_enqueue(cpbus* b, const cpbus_event& e) {
-  if (b->dbg_pending.empty()) { dbg_ring_put(b, e); return; }
-  b->dbg_pending.push_back(DbgItem{false, 0ull, e});
-  if (b->dbg_pending.size() > (size_t)kAcctDbgRing) b->dbg_pending.pop_front();
+// enqueues queue up behind it so that the ring keeps the global publish order; cpbus_debug_events resolves them.  (A group
+// queues no markers: for it this is a put.)
+void dbg_enqueue(HostFront* f, const cpbus_event& e) {
+  if (f->dbg_pending.empty()) { dbg_ring_put(f, e); return; }
+  f->dbg_pending.push_back(DbgItem{false, 0ull, e});
+  if (f->dbg_pending.size() > (size_t)kAcctDbgRing) f->dbg_pending.pop_front();
+}
+
+// DebugEvents (events/bus.go:34-54): empties the ring oldest first, up to a NonEvent; returns how many it read (the first
+// cap of them go to out)
+size_t dbg_read(HostFront* f, cpbus_event* out, size_t cap) {
+  size_t k = 0;
+  for (;;) {
+    if (f->dbg_head == -1) break;
+    const cpbus_event e = f->dbg[f->dbg_tail % 10];
+    if (f->dbg_tail == f->dbg_head) { f->dbg_head = -1; f->dbg_tail = 0; }
+    else f->dbg_tail = (f->dbg_tail + 1) % 10;
+    if (e.code == CPBUS_NONE && e.source_id == 0) break;   // == NonEvent
+    if (k < cap) out[k] = e;
+    k++;
+  }
+  return k;
 }
 
 void dbg_mark_device_batch(cpbus* b, unsigned long long launch) {
@@ -356,7 +401,7 @@ int launch_fanout_t(cpbus* b, const FanoutParams& p, uint32_t grid, size_t smem,
   return CPBUS_OK;
 }
 
-uint64_t max_window(const cpbus* b);
+uint64_t max_window(const HostFront* f);
 
 // Lossless rounds wait in the kernel: for the publisher's header (decide) and for the other shards' offers (agree).  With
 // CUDA's lazy module loading, the first launch of a kernel loads it, and a load may wait for the kernels already running on
@@ -569,21 +614,47 @@ int admit(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, bool* ok, 
 
 // host mirror of one-shot timers that have fired on the device (events/timer.go:19-33):
 // a one-shot whose due time is <= the last launched watermark has disarmed itself.
-void retire_oneshots(cpbus* b, uint64_t w) {
+void retire_oneshots(HostFront* f, uint64_t w) {
   size_t keep = 0;
-  for (size_t i = 0; i < b->oneshot_idx.size(); i++) {
-    HostTimer& t = b->h_timers[b->oneshot_idx[i]];
-    if (t.active && t.oneshot && oneshot_fired(t.next_due, w)) { t.active = false; b->n_timers--; continue; }
-    if (t.active && t.oneshot) b->oneshot_idx[keep++] = b->oneshot_idx[i];
+  for (size_t i = 0; i < f->oneshot_idx.size(); i++) {
+    HostTimer& t = f->h_timers[f->oneshot_idx[i]];
+    if (t.active && t.oneshot && oneshot_fired(t.next_due, w)) { t.active = false; f->n_timers--; continue; }
+    if (t.active && t.oneshot) f->oneshot_idx[keep++] = f->oneshot_idx[i];
   }
-  b->oneshot_idx.resize(keep);
-  if (b->n_timers == 0) b->min_period = UINT64_MAX;
+  f->oneshot_idx.resize(keep);
+  if (f->n_timers == 0) f->min_period = UINT64_MAX;
+}
+
+// Arm table slot `slot` (subscriber * K + k) at the clock: periodic timers bound the clock window, one-shots wait for
+// retirement.
+HostTimer& timer_arm(HostFront* f, size_t slot, uint64_t period, uint32_t source_id, bool oneshot) {
+  HostTimer& t = f->h_timers[slot];
+  t.active = true; t.oneshot = oneshot; t.period = period; t.next_due = due_after(f->now, period); t.source_id = source_id;
+  f->n_timers++;
+  if (!oneshot) f->min_period = std::min(f->min_period, period);
+  else f->oneshot_idx.push_back(slot);
+  return t;
+}
+
+// Disarm table slot `slot` if it is armed.  A cancel (reset_bound) lets the window's bound go with the last timer; an
+// unsubscribe keeps the stale bound, which narrows the window (and so the launch grid) until a cancel or a retirement.
+void timer_disarm(HostFront* f, size_t slot, bool reset_bound) {
+  HostTimer& t = f->h_timers[slot];
+  if (t.active) { t.active = false; f->n_timers--; }
+  if (reset_bound && f->n_timers == 0) f->min_period = UINT64_MAX;
+}
+
+// True when a flush to watermark w launches nothing: no record is staged, and no timer is armed (the watermark then
+// follows the clock) or the clock has not moved since the last launch.
+bool flush_idle(HostFront* f, uint64_t w) {
+  if (f->n_staged) return false;
+  if (f->n_timers == 0) { f->last_watermark = std::max(f->last_watermark, w); return true; }
+  return w == f->last_watermark;
 }
 
 int flush_staged(cpbus* b, uint64_t w) {
+  if (flush_idle(b, w)) return CPBUS_OK;
   const uint32_t n = (uint32_t)b->n_staged;
-  if (n == 0 && b->n_timers == 0) { b->last_watermark = std::max(b->last_watermark, w); return CPBUS_OK; }   // nothing armed: the watermark follows the clock
-  if (n == 0 && w == b->last_watermark) return CPBUS_OK;
   const int c = b->cur;
   int rc;
   // Device staging is a long ring (kDevSlots batches): a slot is reused only kDevSlots flushes later, far beyond how far the
@@ -636,17 +707,138 @@ int flush_staged(cpbus* b, uint64_t w) {
   return CPBUS_OK;
 }
 
-uint64_t max_window(const cpbus* b) {
-  if (!b->K || b->n_timers == 0 || b->min_period == UINT64_MAX) return UINT64_MAX;
-  const uint64_t J = 32u / b->K;
-  return b->min_period > UINT64_MAX / J ? UINT64_MAX : b->min_period * J;
+// One launch of the single bus: the same early returns as launch_fanout, otherwise one stream batch on every shard.
+int group_launch(cpbus_group* g, const cpbus_event* ev, uint32_t n, uint64_t w) {
+  if (g->n_next == 0) return CPBUS_OK;
+  if (n == 0 && g->n_timers == 0) return CPBUS_OK;
+  int rc = cpbus_stream_put(g->streams[0], ev, n, w, CPBUS_PUT_RAW);
+  if (rc) return rc;
+  for (cpbus_stream* st : g->streams)   // the whole batch: already admitted on every shard, so it completes in one launch
+    if ((rc = cpbus_stream_fanout_prefix(st, n, w, n))) return rc;
+  g->last_watermark = w;
+  return CPBUS_OK;
 }
 
-int stage_one(cpbus* b, uint32_t code, uint32_t source_id, uint32_t target, uint32_t flags) {
-  if (b->n_staged == b->B) { int rc = flush_staged(b, b->now); if (rc) return rc; }
-  cpbus_event& e = b->h_batch[b->cur][b->n_staged++];
-  e.seq = b->seq++; e.ts_ns = b->now; e.code = code; e.source_id = source_id; e.target = target; e.flags = flags;
+// Lossless admission of the staged records on every shard (admit), the single bus's verdict being the conjunction and its
+// prefix the minimum.  The records reach a shard's device only when its room bound cannot prove the fit.
+int group_admit(cpbus_group* g, uint32_t n, uint64_t w, bool* ok, uint32_t* m) {
+  *ok = true; *m = n;
+  for (cpbus* s : g->shards) {
+    if (admit_fits(s, n, w)) continue;
+    int rc = dev_guard(s); if (rc) return rc;
+    if (n) CK(cudaMemcpyAsync(s->d_admit_batch, g->staged.data(), (size_t)n * sizeof(cpbus_event), cudaMemcpyHostToDevice, s->stream));
+    bool ok_s = true;
+    uint32_t m_s = n;
+    if ((rc = admit_pass(s, s->d_admit_batch, n, w, &ok_s, &m_s))) return rc;
+    if (!ok_s) { *ok = false; *m = std::min(*m, m_s); }
+  }
   return CPBUS_OK;
+}
+
+// The group's flush: the single bus's outcome (the whole staged batch, or in lossless mode the prefix every shard can take
+// with the partial watermark), as one stream batch
+int flush_staged(cpbus_group* g, uint64_t w) {
+  if (flush_idle(g, w)) return CPBUS_OK;
+  const uint32_t n = (uint32_t)g->n_staged;
+  bool ok = true;
+  uint32_t m = n;
+  int rc;
+  if (g->lossless && (rc = group_admit(g, n, w, &ok, &m))) return rc;
+  if (!ok) {
+    if (m == 0) return CPBUS_EAGAIN;
+    if ((rc = group_launch(g, g->staged.data(), m, g->staged[m - 1].ts_ns))) return rc;
+    std::copy(g->staged.begin() + m, g->staged.begin() + n, g->staged.begin());
+    g->n_staged = n - m;
+    for (cpbus* s : g->shards) { s->room_lb = 0; s->st.admit_partial++; }
+    return CPBUS_EAGAIN;
+  }
+  if ((rc = group_launch(g, g->staged.data(), n, w))) return rc;
+  g->n_staged = 0;
+  return CPBUS_OK;
+}
+
+// where the next staged record goes
+cpbus_event* staging(cpbus* b) { return b->h_batch[b->cur]; }
+cpbus_event* staging(cpbus_group* g) { return g->staged.data(); }
+
+uint64_t max_window(const HostFront* f) {
+  if (!f->K || f->n_timers == 0 || f->min_period == UINT64_MAX) return UINT64_MAX;
+  const uint64_t J = 32u / f->K;
+  return f->min_period > UINT64_MAX / J ? UINT64_MAX : f->min_period * J;
+}
+
+// stage_one, publish_burst and advance_clock run on the single bus and on the group alike (Owner = cpbus or cpbus_group):
+// one body each, with the owner's own flush.
+template <class Owner>
+int stage_one(Owner* o, uint32_t code, uint32_t source_id, uint32_t target, uint32_t flags) {
+  if (o->n_staged == o->B) { int rc = flush_staged(o, o->now); if (rc) return rc; }
+  cpbus_event& e = staging(o)[o->n_staged++];
+  e.seq = o->seq++; e.ts_ns = o->now; e.code = code; e.source_id = source_id; e.target = target; e.flags = flags;
+  return CPBUS_OK;
+}
+
+// Publish a burst (events/bus.go:126-139): nothing of a burst with an invalid code is published.
+template <class Owner>
+int publish_burst(Owner* o, const cpbus_event* ev, size_t n) {
+  for (size_t i = 0; i < n; i++) {   // counter slots of the whole burst: requested up front, touched in the loop below
+    if (ev[i].code < CPBUS_N_CODES && ev[i].code != CPBUS_METRIC) o->pub_pairs.prefetch(((uint64_t)ev[i].code << 32) | ev[i].source_id);
+  }
+  // The debug ring holds 10 entries (events/bus.go:24-31): of a burst only the last 10 published can ever be seen, so only
+  // those are enqueued — including when the call stops early (CPBUS_EAGAIN from an automatic flush in lossless mode).
+  auto dbg_tail = [&](size_t published) {
+    for (size_t j = published > 10 ? published - 10 : 0; j < published; j++) {
+      cpbus_event e{};
+      e.seq = o->seq - (published - j); e.ts_ns = o->now; e.code = ev[j].code; e.source_id = ev[j].source_id; e.target = CPBUS_TARGET_ALL;
+      dbg_enqueue(o, e);
+    }
+  };
+  for (size_t i = 0; i < n; i++) if (ev[i].code >= CPBUS_N_CODES) return CPBUS_EINVAL;
+  for (size_t i = 0; i < n; i++) {
+    const uint32_t code = ev[i].code;
+    const int rc = stage_one(o, code, ev[i].source_id, CPBUS_TARGET_ALL, 0);
+    if (rc) { dbg_tail(i); return rc; }
+    if (code != CPBUS_METRIC) {                                  // events/bus.go:130-132
+      o->published_by_code[code]++;
+      o->pub_pairs.add(((uint64_t)code << 32) | ev[i].source_id, 1);
+    }
+    o->publishes++;
+  }
+  dbg_tail(n);                                                   // events/bus.go:139
+  return CPBUS_OK;
+}
+
+// Move the clock to now_ns.  The kernel looks at <= 32/K candidate firings per timer slot per launch: every flush window is
+// kept within that many periods of the fastest periodic timer (for a group, a stream batch never steps past a shard's window).
+template <class Owner>
+int advance_clock(Owner* o, uint64_t now_ns) {
+  if (now_ns < o->now) return CPBUS_EORDER;
+  if (now_ns == o->now) return CPBUS_OK;
+  const uint64_t win = max_window(o);
+  while (win != UINT64_MAX && now_ns - o->last_watermark > win) {
+    o->now = o->last_watermark + win;
+    const int rc = flush_staged(o, o->now); if (rc) return rc;
+  }
+  o->now = now_ns;
+  return CPBUS_OK;
+}
+
+// Whether ids [first, first + n) lie in [base, base + n_next), the ids subscribed so far; *index = first - base.
+bool id_range(uint32_t base, uint32_t n_next, uint32_t first, uint64_t n, uint32_t* index) {
+  *index = first - base;
+  return first >= base && (uint64_t)*index + n <= n_next;
+}
+
+// cpbus_publish_counts: the host publish counts of f and n_dev device-counted pairs (key + 1 per slot, 0 = empty), merged by
+// {code, source} and sorted; *n = how many pairs there are, the first cap of them go to out.
+void pair_counts(const HostFront* f, const unsigned long long* dev_keys, const unsigned long long* dev_cnts, size_t n_dev,
+                 cpbus_pair_count* out, size_t cap, size_t* n) {
+  std::unordered_map<uint64_t, uint64_t> merged;
+  for (size_t i = 0; i < f->pub_pairs.keys.size(); i++) if (f->pub_pairs.keys[i]) merged[f->pub_pairs.keys[i] - 1] += f->pub_pairs.cnts[i];
+  for (size_t i = 0; i < n_dev; i++) if (dev_keys[i]) merged[dev_keys[i] - 1] += dev_cnts[i];
+  std::vector<std::pair<uint64_t, uint64_t>> v(merged.begin(), merged.end());
+  std::sort(v.begin(), v.end());
+  for (size_t i = 0; i < v.size() && i < cap; i++) out[i] = cpbus_pair_count{(uint32_t)(v[i].first >> 32), (uint32_t)v[i].first, v[i].second};
+  *n = v.size();
 }
 
 bool is_pow2(uint32_t x) { return x && !(x & (x - 1)); }
@@ -1076,8 +1268,8 @@ int cpbus_subscribe_pairs_many(cpbus_t* b, const uint32_t* masks, const cpbus_pa
 
 int cpbus_unsubscribe(cpbus_t* b, uint32_t sub_id) try {
   if (!b) return CPBUS_EINVAL;
-  const uint32_t l = sub_id - b->cfg.sub_id_base;
-  if (sub_id < b->cfg.sub_id_base || l >= b->n_next) return CPBUS_ENOENT;
+  uint32_t l = 0;
+  if (!id_range(b->cfg.sub_id_base, b->n_next, sub_id, 1, &l)) return CPBUS_ENOENT;
   int rc = enter(b); if (rc) return rc;
   if ((rc = flush_staged(b, b->now))) return rc;
   // second Unsubscribe drives the WaitGroup negative in Go (events/bus.go:121) => panic
@@ -1089,10 +1281,7 @@ int cpbus_unsubscribe(cpbus_t* b, uint32_t sub_id) try {
   const uint32_t word = 0;
   CK(cudaMemcpyAsync(&b->d_ctl[l].mask, &word, 4, cudaMemcpyHostToDevice, b->stream));
   if (b->K && !b->h_timers.empty()) {
-    for (uint32_t k = 0; k < b->K; k++) {
-      HostTimer& t = b->h_timers[(size_t)l * b->K + k];
-      if (t.active) { t.active = false; b->n_timers--; }
-    }
+    for (uint32_t k = 0; k < b->K; k++) timer_disarm(b, (size_t)l * b->K + k, /*reset_bound=*/false);
     CK(cudaMemsetAsync(b->d_timers + (size_t)l * b->K, 0xFF, b->K * sizeof(DevTimer), b->stream));
   }
   CK(cudaStreamSynchronize(b->stream));
@@ -1105,8 +1294,8 @@ int cpbus_unsubscribe(cpbus_t* b, uint32_t sub_id) try {
 // NewEventTimer on a channel that was not subscribed, watches/watches.go:37,71) is subscribed to the bus after all.
 int cpbus_set_mask(cpbus_t* b, uint32_t sub_id, uint32_t mask) try {
   if (!b) return CPBUS_EINVAL;
-  const uint32_t l = sub_id - b->cfg.sub_id_base;
-  if (sub_id < b->cfg.sub_id_base || l >= b->n_next) return CPBUS_ENOENT;
+  uint32_t l = 0;
+  if (!id_range(b->cfg.sub_id_base, b->n_next, sub_id, 1, &l)) return CPBUS_ENOENT;
   if (!b->h_active[l]) return CPBUS_ECLOSED;
   int rc = enter(b); if (rc) return rc;
   if ((rc = flush_staged(b, b->now))) return rc;
@@ -1128,23 +1317,19 @@ static int push_mask_words(cpbus* b, uint32_t first, uint32_t n) {
 int cpbus_timer_add(cpbus_t* b, uint32_t sub_id, uint64_t period_ns, uint32_t source_id, int oneshot, uint32_t* timer_id) try {
   if (!b || !period_ns) return CPBUS_EINVAL;
   if (!b->K) return CPBUS_ENOSPC;
-  const uint32_t l = sub_id - b->cfg.sub_id_base;
-  if (sub_id < b->cfg.sub_id_base || l >= b->n_next) return CPBUS_ENOENT;
+  uint32_t l = 0;
+  if (!id_range(b->cfg.sub_id_base, b->n_next, sub_id, 1, &l)) return CPBUS_ENOENT;
   int rc = enter(b); if (rc) return rc;
   if ((rc = flush_staged(b, b->now))) return rc;
   if (b->h_timers.empty()) b->h_timers.resize((size_t)b->N * b->K);
   retire_oneshots(b, b->last_watermark);
   if (!b->h_active[l]) return CPBUS_ECLOSED;
   for (uint32_t k = 0; k < b->K; k++) {
-    HostTimer& t = b->h_timers[(size_t)l * b->K + k];
-    if (t.active) continue;
-    t.active = true; t.oneshot = oneshot != 0; t.period = period_ns; t.next_due = due_after(b->now, period_ns); t.source_id = source_id;
+    if (b->h_timers[(size_t)l * b->K + k].active) continue;
+    HostTimer& t = timer_arm(b, (size_t)l * b->K + k, period_ns, source_id, oneshot != 0);
     DevTimer d{}; d.next_due = t.next_due; d.period = oneshot ? 0 : period_ns; d.source_id = source_id; d.fired = 0;
     CK(cudaMemcpyAsync(b->d_timers + (size_t)l * b->K + k, &d, sizeof(d), cudaMemcpyHostToDevice, b->stream));
     CK(cudaStreamSynchronize(b->stream));
-    b->n_timers++;
-    if (!oneshot) b->min_period = std::min(b->min_period, period_ns);
-    else b->oneshot_idx.push_back((size_t)l * b->K + k);
     t.gen = (uint8_t)((t.gen + 1) & 0x3F);
     if (timer_id) *timer_id = (l * b->K + k) | ((uint32_t)t.gen << kTimerSlotBits);
     return push_mask_words(b, l, 1);
@@ -1156,8 +1341,8 @@ int cpbus_timer_add_many(cpbus_t* b, uint32_t first_sub, uint32_t n, uint64_t pe
                          uint32_t source_id0, int oneshot) try {
   if (!b || !period_ns || !n) return CPBUS_EINVAL;
   if (!b->K) return CPBUS_ENOSPC;
-  const uint32_t l0 = first_sub - b->cfg.sub_id_base;
-  if (first_sub < b->cfg.sub_id_base || (uint64_t)l0 + n > b->n_next) return CPBUS_ENOENT;
+  uint32_t l0 = 0;
+  if (!id_range(b->cfg.sub_id_base, b->n_next, first_sub, n, &l0)) return CPBUS_ENOENT;
   int rc = enter(b); if (rc) return rc;
   if ((rc = flush_staged(b, b->now))) return rc;
   if (b->h_timers.empty()) b->h_timers.resize((size_t)b->N * b->K);
@@ -1172,17 +1357,12 @@ int cpbus_timer_add_many(cpbus_t* b, uint32_t first_sub, uint32_t n, uint64_t pe
   CK(cudaMemcpyAsync(dev.data(), b->d_timers + (size_t)l0 * b->K, dev.size() * sizeof(DevTimer), cudaMemcpyDeviceToHost, b->stream));
   CK(cudaStreamSynchronize(b->stream));
   for (uint32_t i = 0; i < n; i++) {
-    HostTimer& t = b->h_timers[(size_t)(l0 + i) * b->K];
-    t.active = true; t.oneshot = oneshot != 0; t.period = period_ns; t.next_due = due_after(b->now, period_ns);
-    t.source_id = source_ids ? source_ids[i] : source_id0 + i;
+    const HostTimer& t = timer_arm(b, (size_t)(l0 + i) * b->K, period_ns, source_ids ? source_ids[i] : source_id0 + i, oneshot != 0);
     DevTimer& d = dev[(size_t)i * b->K];
     d.next_due = t.next_due; d.period = oneshot ? 0 : period_ns; d.source_id = t.source_id; d.fired = 0; d.pad[0] = d.pad[1] = 0;
-    if (oneshot) b->oneshot_idx.push_back((size_t)(l0 + i) * b->K);
   }
   CK(cudaMemcpyAsync(b->d_timers + (size_t)l0 * b->K, dev.data(), dev.size() * sizeof(DevTimer), cudaMemcpyHostToDevice, b->stream));
   CK(cudaStreamSynchronize(b->stream));
-  b->n_timers += n;
-  if (!oneshot) b->min_period = std::min(b->min_period, period_ns);
   return push_mask_words(b, l0, n);
 } CPBUS_CATCH
 
@@ -1195,70 +1375,36 @@ int cpbus_timer_cancel(cpbus_t* b, uint32_t timer_id) try {
   int rc = enter(b); if (rc) return rc;
   if ((rc = flush_staged(b, b->now))) return rc;   // firings due before the cancel still happen
   retire_oneshots(b, b->last_watermark);
-  HostTimer& t = b->h_timers[(size_t)l * b->K + k];
+  const HostTimer& t = b->h_timers[(size_t)l * b->K + k];
   if (!t.active || t.gen != gen) return CPBUS_ENOENT;   // already fired / cancelled, or the slot has been re-armed since
-  t.active = false; b->n_timers--;
+  timer_disarm(b, (size_t)l * b->K + k, /*reset_bound=*/true);
   CK(cudaMemsetAsync(b->d_timers + (size_t)l * b->K + k, 0xFF, sizeof(DevTimer), b->stream));
   CK(cudaStreamSynchronize(b->stream));
-  if (b->n_timers == 0) b->min_period = UINT64_MAX;
   return push_mask_words(b, l, 1);
 } CPBUS_CATCH
 
 int cpbus_publish(cpbus_t* b, const cpbus_event* ev, size_t n) try {
   if (!b || (!ev && n)) return CPBUS_EINVAL;
   int rc = enter(b); if (rc) return rc;
-  for (size_t i = 0; i < n; i++) {   // counter slots of the whole burst: requested up front, touched in the loop below
-    if (ev[i].code < CPBUS_N_CODES && ev[i].code != CPBUS_METRIC) b->pub_pairs.prefetch(((uint64_t)ev[i].code << 32) | ev[i].source_id);
-  }
-  // The debug ring holds 10 entries (events/bus.go:24-31): of a burst only the last 10 published can ever be seen, so only
-  // those are enqueued — including when the call stops early (CPBUS_EAGAIN from an automatic flush in lossless mode).
-  auto dbg_tail = [&](size_t published) {
-    for (size_t j = published > 10 ? published - 10 : 0; j < published; j++) {
-      cpbus_event e{};
-      e.seq = b->seq - (published - j); e.ts_ns = b->now; e.code = ev[j].code; e.source_id = ev[j].source_id; e.target = CPBUS_TARGET_ALL;
-      dbg_enqueue(b, e);
-    }
-  };
-  for (size_t i = 0; i < n; i++) if (ev[i].code >= CPBUS_N_CODES) return CPBUS_EINVAL;   // nothing of an invalid burst is published
-  for (size_t i = 0; i < n; i++) {
-    const uint32_t code = ev[i].code;
-    if ((rc = stage_one(b, code, ev[i].source_id, CPBUS_TARGET_ALL, 0))) { dbg_tail(i); return rc; }
-    if (code != CPBUS_METRIC) {                                  // events/bus.go:130-132
-      b->st.published_by_code[code]++;
-      b->pub_pairs.add(((uint64_t)code << 32) | ev[i].source_id, 1);
-    }
-    b->st.publishes++;
-  }
-  dbg_tail(n);                                                   // events/bus.go:139
-  return CPBUS_OK;
+  return publish_burst(b, ev, n);
 } CPBUS_CATCH
 
 int cpbus_send(cpbus_t* b, uint32_t sub_id, const cpbus_event* ev) try {
   if (!b || !ev || ev->code >= CPBUS_N_CODES) return CPBUS_EINVAL;
-  const uint32_t l = sub_id - b->cfg.sub_id_base;
-  if (sub_id < b->cfg.sub_id_base || l >= b->n_next) return CPBUS_ENOENT;
+  uint32_t l = 0;
+  if (!id_range(b->cfg.sub_id_base, b->n_next, sub_id, 1, &l)) return CPBUS_ENOENT;
   if (!b->h_active[l]) return CPBUS_ECLOSED;   // the mailbox is gone (Go: send on a closed channel panics)
   int rc = enter(b); if (rc) return rc;
   if ((rc = stage_one(b, ev->code, ev->source_id, sub_id, CPBUS_F_UNICAST))) return rc;
-  b->st.publishes++;
+  b->publishes++;
   return CPBUS_OK;
 } CPBUS_CATCH
 
 int cpbus_advance(cpbus_t* b, uint64_t now_ns) try {
   if (!b) return CPBUS_EINVAL;
   int rc = follow_resolve(b); if (rc) return rc;   // the clock moves with the batches that followers fanned out
-  if (now_ns < b->now) return CPBUS_EORDER;
-  if (now_ns == b->now) return CPBUS_OK;
-  if ((rc = dev_guard(b))) return rc;
-  // the kernel looks at <= 32/K candidate firings per timer slot per launch: keep every
-  // flush window within that many periods of the fastest periodic timer
-  const uint64_t win = max_window(b);
-  while (win != UINT64_MAX && now_ns - b->last_watermark > win) {
-    b->now = b->last_watermark + win;
-    if ((rc = flush_staged(b, b->now))) return rc;
-  }
-  b->now = now_ns;
-  return CPBUS_OK;
+  if (now_ns > b->now && (rc = dev_guard(b))) return rc;
+  return advance_clock(b, now_ns);
 } CPBUS_CATCH
 
 int cpbus_flush(cpbus_t* b) try {
@@ -1375,7 +1521,7 @@ static int publish_device_impl(cpbus_t* b, const void* d_events, size_t n, uint6
   if ((rc = launch_fanout(b, src, (uint32_t)n, watermark_ns, o))) return rc;
   // an empty batch with no timer armed launches nothing, so nothing pulled d_next: the cache must not claim it
   if (slot >= 0 && b->launch_seq != seq0) { b->pf_ptr[slot] = d_next; b->pf_n[slot] = n_next; b->pf_seq[slot] = b->launch_seq; b->pf_next = (slot + 1) % cpbus::kPrefetch; }
-  b->st.publishes += n; b->seq += n;
+  b->publishes += n; b->seq += n;
   return CPBUS_OK;
 }
 
@@ -1732,7 +1878,7 @@ static const cpbus_event* stream_launch(const cpbus_stream* st, unsigned long lo
 // The host-driven launch, a resolved follower and a resolved round all fold here, so each moves the host state exactly as
 // the others with the same outcome do.
 static void stream_delivered(cpbus* b, cpbus_stream* st, uint32_t m, uint64_t w, bool final, unsigned long long launch_seq) {
-  b->st.publishes += m; b->seq += m;
+  b->publishes += m; b->seq += m;
   b->now = w; b->last_watermark = w;
   if (m) dbg_mark_device_batch(b, launch_seq);
   if (final) { st->get_seq++; st->get_off = 0; return; }
@@ -1987,8 +2133,8 @@ static int copy_slots(cpbus* b, uint32_t l, uint64_t from, size_t n, cpbus_event
 
 int cpbus_drain(cpbus_t* b, uint32_t sub_id, cpbus_event* out, size_t cap, size_t* n, uint64_t* lost) try {
   if (!b || !n || (!out && cap)) return CPBUS_EINVAL;
-  const uint32_t l = sub_id - b->cfg.sub_id_base;
-  if (sub_id < b->cfg.sub_id_base || l >= b->n_next) return CPBUS_ENOENT;
+  uint32_t l = 0;
+  if (!id_range(b->cfg.sub_id_base, b->n_next, sub_id, 1, &l)) return CPBUS_ENOENT;
   std::lock_guard<std::mutex> g(b->mu);
   int rc = enter(b); if (rc) return rc;
   uint64_t tail = 0, head = 0;
@@ -2009,8 +2155,8 @@ int cpbus_drain(cpbus_t* b, uint32_t sub_id, cpbus_event* out, size_t cap, size_
 int cpbus_drain_many(cpbus_t* b, uint32_t first_sub, uint32_t n, cpbus_event* out, size_t cap, uint32_t* offsets,
                      uint32_t* counts, size_t* total) try {
   if (!b || !n || !out || !cap || !offsets || !counts || !total || cap > 0xFFFFFFFFull) return CPBUS_EINVAL;
-  const uint32_t l = first_sub - b->cfg.sub_id_base;
-  if (first_sub < b->cfg.sub_id_base || (uint64_t)l + n > b->n_next) return CPBUS_ENOENT;
+  uint32_t l = 0;
+  if (!id_range(b->cfg.sub_id_base, b->n_next, first_sub, n, &l)) return CPBUS_ENOENT;
   std::lock_guard<std::mutex> g(b->mu);
   int rc = enter(b); if (rc) return rc;
   if (b->drain_cap < cap || b->drain_idx_cap < n) {   // device staging grows on demand and is kept
@@ -2059,8 +2205,8 @@ static int drain_ready_impl(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t
                             cpbus_ready* ready, size_t ready_cap, size_t* n_ready, size_t* total, uint32_t* next_sub,
                             bool* all_taken) {
   if (start_sub < first_sub || start_sub - first_sub >= n) return CPBUS_EINVAL;
-  const uint32_t l = first_sub - b->cfg.sub_id_base;
-  if (first_sub < b->cfg.sub_id_base || (uint64_t)l + n > b->n_next) return CPBUS_ENOENT;
+  uint32_t l = 0;
+  if (!id_range(b->cfg.sub_id_base, b->n_next, first_sub, n, &l)) return CPBUS_ENOENT;
   std::lock_guard<std::mutex> g(b->mu);
   int rc = enter(b); if (rc) return rc;
   const size_t rcap = std::min<size_t>(ready_cap, n);   // never more entries than mailboxes
@@ -2113,8 +2259,8 @@ static int lagging_impl(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t sta
                         size_t cap, size_t* n_out, uint32_t* next_sub, cpbus_lag_summary* sum, bool* all_returned) {
   static_assert(sizeof(cpbus_lag) == 16 && sizeof(cpbus_lag_summary) == kLagSumWords * sizeof(unsigned long long), "C-ABI layout");
   if (start_sub < first_sub || start_sub - first_sub >= n) return CPBUS_EINVAL;
-  const uint32_t l = first_sub - b->cfg.sub_id_base;
-  if (first_sub < b->cfg.sub_id_base || (uint64_t)l + n > b->n_next) return CPBUS_ENOENT;
+  uint32_t l = 0;
+  if (!id_range(b->cfg.sub_id_base, b->n_next, first_sub, n, &l)) return CPBUS_ENOENT;
   std::lock_guard<std::mutex> g(b->mu);
   int rc = enter(b); if (rc) return rc;
   const size_t ecap = std::min<size_t>(cap, n);   // never more entries than mailboxes
@@ -2217,8 +2363,8 @@ int cpbus_consume_all(cpbus_t* b) try {
 
 int cpbus_peek_window(cpbus_t* b, uint32_t sub_id, cpbus_event* out, size_t cap, size_t* n) try {
   if (!b || !n || (!out && cap)) return CPBUS_EINVAL;
-  const uint32_t l = sub_id - b->cfg.sub_id_base;
-  if (sub_id < b->cfg.sub_id_base || l >= b->n_next) return CPBUS_ENOENT;
+  uint32_t l = 0;
+  if (!id_range(b->cfg.sub_id_base, b->n_next, sub_id, 1, &l)) return CPBUS_ENOENT;
   std::lock_guard<std::mutex> g(b->mu);
   int rc = enter(b); if (rc) return rc;
   uint64_t tail = 0, head = 0;
@@ -2231,8 +2377,8 @@ int cpbus_peek_window(cpbus_t* b, uint32_t sub_id, cpbus_event* out, size_t cap,
 
 int cpbus_digest(cpbus_t* b, uint32_t first_sub, uint32_t n, cpbus_digest_t* out) try {
   if (!b || !out || !n) return CPBUS_EINVAL;
-  const uint32_t l = first_sub - b->cfg.sub_id_base;
-  if (first_sub < b->cfg.sub_id_base || (uint64_t)l + n > b->n_next) return CPBUS_ENOENT;
+  uint32_t l = 0;
+  if (!id_range(b->cfg.sub_id_base, b->n_next, first_sub, n, &l)) return CPBUS_ENOENT;
   std::lock_guard<std::mutex> g(b->mu);
   int rc = enter(b); if (rc) return rc;
   std::vector<SubCtl> c(n);
@@ -2244,8 +2390,8 @@ int cpbus_digest(cpbus_t* b, uint32_t first_sub, uint32_t n, cpbus_digest_t* out
 
 int cpbus_digest_fold_begin(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t* ticket) try {
   if (!b || !ticket || !n) return CPBUS_EINVAL;
-  const uint32_t l = first_sub - b->cfg.sub_id_base;
-  if (first_sub < b->cfg.sub_id_base || (uint64_t)l + n > b->n_next) return CPBUS_ENOENT;
+  uint32_t l = 0;
+  if (!id_range(b->cfg.sub_id_base, b->n_next, first_sub, n, &l)) return CPBUS_ENOENT;
   std::lock_guard<std::mutex> g(b->mu);
   int rc = dev_guard(b); if (rc) return rc;
   const uint32_t slot = b->fold_next++ % cpbus::kFoldSlots;
@@ -2333,17 +2479,7 @@ int cpbus_debug_events(cpbus_t* b, cpbus_event* out, size_t cap, size_t* n) try 
   if (!b || !n || (!out && cap)) return CPBUS_EINVAL;
   { const int rc = follow_resolve(b); if (rc) return rc; }
   { const int rc = dbg_resolve(b); if (rc) return rc; }
-  size_t k = 0;
-  for (;;) {
-    if (b->dbg_head == -1) break;
-    const cpbus_event e = b->dbg[b->dbg_tail % 10];
-    if (b->dbg_tail == b->dbg_head) { b->dbg_head = -1; b->dbg_tail = 0; }
-    else b->dbg_tail = (b->dbg_tail + 1) % 10;
-    if (e.code == CPBUS_NONE && e.source_id == 0) break;   // == NonEvent
-    if (k < cap) out[k] = e;
-    k++;
-  }
-  *n = k;
+  *n = dbg_read(b, out, cap);
   return CPBUS_OK;
 } CPBUS_CATCH
 
@@ -2368,7 +2504,9 @@ int cpbus_stats(cpbus_t* b, cpbus_stats_t* out) try {
   b->st.intern_entries = b->sources.size(); b->st.intern_bytes = b->intern_bytes;
   b->st.ephemeral_live = b->eph_live; b->st.ephemeral_recycled = b->eph_recycled;
   *out = b->st;
-  for (int c = 0; c < CPBUS_N_CODES; c++) out->published_by_code[c] += b->h_acct->by_code[c];   // device-published batches (kernel-counted)
+  out->publishes = b->publishes;
+  for (int c = 0; c < CPBUS_N_CODES; c++)   // + device-published batches (kernel-counted)
+    out->published_by_code[c] = b->published_by_code[c] + b->h_acct->by_code[c];
   return CPBUS_OK;
 } CPBUS_CATCH
 
@@ -2378,19 +2516,14 @@ int cpbus_publish_counts(cpbus_t* b, cpbus_pair_count* out, size_t cap, size_t* 
   if (!b || !n || (!out && cap)) return CPBUS_EINVAL;
   std::lock_guard<std::mutex> g(b->mu);
   int rc = enter(b); if (rc) return rc;
-  std::unordered_map<uint64_t, uint64_t> merged;
-  for (size_t i = 0; i < b->pub_pairs.keys.size(); i++) if (b->pub_pairs.keys[i]) merged[b->pub_pairs.keys[i] - 1] += b->pub_pairs.cnts[i];
+  std::vector<unsigned long long> keys, cnts;
   if (b->launch_seq) {
-    std::vector<unsigned long long> keys(kAcctPairSlots), cnts(kAcctPairSlots);
+    keys.resize(kAcctPairSlots); cnts.resize(kAcctPairSlots);
     CK(cudaMemcpyAsync(keys.data(), b->d_acct->pair_key, sizeof(unsigned long long) * kAcctPairSlots, cudaMemcpyDeviceToHost, b->stream));
     CK(cudaMemcpyAsync(cnts.data(), b->d_acct->pair_cnt, sizeof(unsigned long long) * kAcctPairSlots, cudaMemcpyDeviceToHost, b->stream));
     CK(cudaStreamSynchronize(b->stream));
-    for (uint32_t i = 0; i < kAcctPairSlots; i++) if (keys[i]) merged[keys[i] - 1] += cnts[i];
   }
-  std::vector<std::pair<uint64_t, uint64_t>> v(merged.begin(), merged.end());
-  std::sort(v.begin(), v.end());
-  for (size_t i = 0; i < v.size() && i < cap; i++) out[i] = cpbus_pair_count{(uint32_t)(v[i].first >> 32), (uint32_t)v[i].first, v[i].second};
-  *n = v.size();
+  pair_counts(b, keys.data(), cnts.data(), keys.size(), out, cap, n);
   return CPBUS_OK;
 } CPBUS_CATCH
 
@@ -2401,125 +2534,22 @@ int cpbus_device_ptrs(cpbus_t* b, void** ring, void** ctl) try {
   return CPBUS_OK;
 } CPBUS_CATCH
 
-// ---- the group: one bus handle over the GPUs of a box (include/cpbus.h: cpbus_group_*) ----------------------------------
-// The group keeps the host state a single bus keeps for the whole id space — staged records, seq, clock, last launched
-// watermark, the timer table that sets the clock window, debug ring and publish counts — and makes the flushes the single
-// bus makes (flush_staged, stage_one, cpbus_advance).  A flush becomes one RAW stream batch that every shard fans out in
-// full: in lossless mode the group first runs the single bus's admission (admit) on every shard and puts only the prefix
-// every shard can take, with the single bus's partial watermark.  (cpbus_stream_admit would hold a batch back until the
-// ticks due by its watermark fit too, where a partial cpbus_flush delivers the records and stalls on the ticks alone.)
-// Shard clocks: a shard's clock is its last launched watermark; a shard without timers is moved to the group clock with
-// cpbus_advance right before a timer is armed on it (no launch: it has no timer window), so every shard's `now + period`
-// is the single bus's.  A shard with timers already has the group clock there (the group has just flushed at `now`).
-struct cpbus_group {
-  std::vector<cpbus*> shards;
-  std::vector<cpbus_stream*> streams;   // streams[0] owns the ring (shard 0), the others are attached
-  std::vector<uint32_t> first;          // global index (sub_id_base not applied) of each shard's subscriber 0; + a sentinel
-  uint32_t base = 0, N = 0, B = 0, K = 0;
-  bool lossless = false;
-  uint32_t n_next = 0, n_active = 0;
-  std::vector<cpbus_event> staged;      // B records
-  size_t n_staged = 0;
-  uint64_t now = 0, last_watermark = 0, seq = 0;
-  // the single bus's timer bookkeeping over global slots (subscriber * K + k): what sets the clock window and when an empty
-  // flush launches
-  struct Slot { bool active = false, oneshot = false; uint64_t next_due = 0; };
-  std::vector<Slot> timers;             // N * K, allocated on first use (as the single bus's h_timers)
-  std::vector<size_t> oneshot_idx;
-  uint32_t n_timers = 0;
-  uint64_t min_period = UINT64_MAX;
-  int dbg_head = -1, dbg_tail = 0;
-  cpbus_event dbg[10]{};
-  PairCounter pub_pairs;
-  uint64_t publishes = 0, by_code[CPBUS_N_CODES] = {};
-};
-
+// ---- the group: one bus handle over the GPUs of a box (include/cpbus.h: cpbus_group_*; struct cpbus_group) ---------------
 static uint32_t group_shard_of(const cpbus_group* g, uint32_t index) {   // index < N
   return (uint32_t)(std::upper_bound(g->first.begin(), g->first.end(), index) - g->first.begin()) - 1;
 }
 
-static uint64_t group_window(const cpbus_group* g) {   // max_window of the single bus
-  if (!g->K || g->n_timers == 0 || g->min_period == UINT64_MAX) return UINT64_MAX;
-  const uint64_t J = 32u / g->K;
-  return g->min_period > UINT64_MAX / J ? UINT64_MAX : g->min_period * J;
-}
-
-// retire_oneshots of the single bus, for the group's table and, at the same moment, every shard's own: a shard's timer
-// count (and so its window) then never lags the group's
+// retire_oneshots for the group's table and, at the same moment, every shard's own: a shard's timer count (and so its
+// window) then never lags the group's
 static void group_retire(cpbus_group* g) {
-  size_t keep = 0;
-  for (size_t i = 0; i < g->oneshot_idx.size(); i++) {
-    cpbus_group::Slot& t = g->timers[g->oneshot_idx[i]];
-    if (t.active && t.oneshot && oneshot_fired(t.next_due, g->last_watermark)) { t.active = false; g->n_timers--; continue; }
-    if (t.active && t.oneshot) g->oneshot_idx[keep++] = g->oneshot_idx[i];
-  }
-  g->oneshot_idx.resize(keep);
-  if (g->n_timers == 0) g->min_period = UINT64_MAX;
+  retire_oneshots(g, g->last_watermark);
   for (cpbus* s : g->shards) if (!s->h_timers.empty()) retire_oneshots(s, s->last_watermark);
-}
-
-// One launch of the single bus: the same early returns as launch_fanout, otherwise one stream batch on every shard.
-static int group_launch(cpbus_group* g, const cpbus_event* ev, uint32_t n, uint64_t w) {
-  if (g->n_next == 0) return CPBUS_OK;
-  if (n == 0 && g->n_timers == 0) return CPBUS_OK;
-  int rc = cpbus_stream_put(g->streams[0], ev, n, w, CPBUS_PUT_RAW);
-  if (rc) return rc;
-  for (cpbus_stream* st : g->streams)   // the whole batch: already admitted on every shard, so it completes in one launch
-    if ((rc = cpbus_stream_fanout_prefix(st, n, w, n))) return rc;
-  g->last_watermark = w;
-  return CPBUS_OK;
-}
-
-// Lossless admission of the staged records on every shard (admit), the single bus's verdict being the conjunction and its
-// prefix the minimum.  The records reach a shard's device only when its room bound cannot prove the fit.
-static int group_admit(cpbus_group* g, uint32_t n, uint64_t w, bool* ok, uint32_t* m) {
-  *ok = true; *m = n;
-  for (cpbus* s : g->shards) {
-    if (admit_fits(s, n, w)) continue;
-    int rc = dev_guard(s); if (rc) return rc;
-    if (n) CK(cudaMemcpyAsync(s->d_admit_batch, g->staged.data(), (size_t)n * sizeof(cpbus_event), cudaMemcpyHostToDevice, s->stream));
-    bool ok_s = true;
-    uint32_t m_s = n;
-    if ((rc = admit_pass(s, s->d_admit_batch, n, w, &ok_s, &m_s))) return rc;
-    if (!ok_s) { *ok = false; *m = std::min(*m, m_s); }
-  }
-  return CPBUS_OK;
-}
-
-// flush_staged of the single bus
-static int group_flush(cpbus_group* g, uint64_t w) {
-  const uint32_t n = (uint32_t)g->n_staged;
-  if (n == 0 && g->n_timers == 0) { g->last_watermark = std::max(g->last_watermark, w); return CPBUS_OK; }
-  if (n == 0 && w == g->last_watermark) return CPBUS_OK;
-  bool ok = true;
-  uint32_t m = n;
-  int rc;
-  if (g->lossless && (rc = group_admit(g, n, w, &ok, &m))) return rc;
-  if (!ok) {
-    if (m == 0) return CPBUS_EAGAIN;
-    if ((rc = group_launch(g, g->staged.data(), m, g->staged[m - 1].ts_ns))) return rc;
-    std::copy(g->staged.begin() + m, g->staged.begin() + n, g->staged.begin());
-    g->n_staged = n - m;
-    for (cpbus* s : g->shards) { s->room_lb = 0; s->st.admit_partial++; }
-    return CPBUS_EAGAIN;
-  }
-  if ((rc = group_launch(g, g->staged.data(), n, w))) return rc;
-  g->n_staged = 0;
-  return CPBUS_OK;
-}
-
-// stage_one of the single bus: seq is one ordinal over publishes and sends
-static int group_stage(cpbus_group* g, uint32_t code, uint32_t source_id, uint32_t target, uint32_t flags) {
-  if (g->n_staged == g->B) { const int rc = group_flush(g, g->now); if (rc) return rc; }
-  cpbus_event& e = g->staged[g->n_staged++];
-  e.seq = g->seq++; e.ts_ns = g->now; e.code = code; e.source_id = source_id; e.target = target; e.flags = flags;
-  return CPBUS_OK;
 }
 
 // the owning shard of global id `sub_id` and its local index; false: not a subscribed-so-far id
 static bool group_locate(const cpbus_group* g, uint32_t sub_id, cpbus** s, uint32_t* l) {
-  const uint32_t i = sub_id - g->base;
-  if (sub_id < g->base || i >= g->n_next) return false;
+  uint32_t i = 0;
+  if (!id_range(g->base, g->n_next, sub_id, 1, &i)) return false;
   const uint32_t k = group_shard_of(g, i);
   *s = g->shards[k]; *l = i - g->first[k];
   return true;
@@ -2599,12 +2629,35 @@ static int group_each_range(cpbus_group* g, uint32_t first_index, uint32_t n, Fn
   }
   return CPBUS_OK;
 }
+
+// The cyclic walk of a paged query (cpbus_drain_ready, cpbus_lagging) over ids [first_sub, first_sub + n) from start_sub, in
+// pieces that each lie on one shard: fn(shard, local index, id, count) returns CPBUS_OK to go on, kWalkEnd to end the walk,
+// or an error.  The checks are the single call's; *next_sub is set to start_sub (the walk found no cut) before the first piece.
+constexpr int kWalkEnd = 1;
+template <class Fn>
+static int group_walk(cpbus_group* g, uint32_t first_sub, uint32_t n, uint32_t start_sub, uint32_t* next_sub, Fn&& fn) {
+  if (start_sub < first_sub || start_sub - first_sub >= n) return CPBUS_EINVAL;
+  uint32_t i0 = 0;
+  if (!id_range(g->base, g->n_next, first_sub, n, &i0)) return CPBUS_ENOENT;
+  const uint32_t rot = start_sub - first_sub;
+  *next_sub = start_sub;
+  for (uint32_t done = 0; done < n;) {
+    const uint32_t i = i0 + (rot + done) % n;                       // global index of the walk's next mailbox
+    const uint32_t k = group_shard_of(g, i);
+    const uint32_t wrap = i0 + n - i;                               // the walk wraps to first_sub after this many
+    const uint32_t cnt = std::min({n - done, g->first[k + 1] - i, wrap});
+    const int rc = fn(g->shards[k], i - g->first[k], g->base + i, cnt);
+    if (rc) return rc == kWalkEnd ? CPBUS_OK : rc;
+    done += cnt;
+  }
+  return CPBUS_OK;
+}
 }
 
 int cpbus_group_subscribe_many(cpbus_group_t* g, const uint32_t* masks, uint32_t n, uint32_t* first_sub_id) try {
   if (!g || !n) return CPBUS_EINVAL;
   if ((uint64_t)g->n_next + n > g->N) return CPBUS_ENOSPC;
-  int rc = group_flush(g, g->now); if (rc) return rc;
+  int rc = flush_staged(g, g->now); if (rc) return rc;
   const uint32_t first = g->n_next;
   rc = group_each_range(g, first, n, [&](cpbus* s, uint32_t, uint32_t off, uint32_t cnt) -> int {
     uint32_t id = 0;
@@ -2622,7 +2675,7 @@ int cpbus_group_subscribe_pairs(cpbus_group_t* g, uint32_t mask, const cpbus_pai
   if (!g || n_pairs > CPBUS_MAX_PAIRS || (n_pairs && !pairs)) return CPBUS_EINVAL;
   for (uint32_t j = 0; j < n_pairs; j++) if (pairs[j].code >= CPBUS_N_CODES) return CPBUS_EINVAL;
   if (g->n_next >= g->N) return CPBUS_ENOSPC;
-  int rc = group_flush(g, g->now); if (rc) return rc;
+  int rc = flush_staged(g, g->now); if (rc) return rc;
   const uint32_t k = group_shard_of(g, g->n_next);
   uint32_t id = 0;
   if ((rc = cpbus_subscribe_pairs(g->shards[k], mask, pairs, n_pairs, &id))) return rc;
@@ -2639,7 +2692,7 @@ int cpbus_group_subscribe_pairs_many(cpbus_group_t* g, const uint32_t* masks, co
     for (uint32_t j = 0; j < n_pairs[i]; j++) if (pairs[(size_t)i * CPBUS_MAX_PAIRS + j].code >= CPBUS_N_CODES) return CPBUS_EINVAL;
   }
   if ((uint64_t)g->n_next + n > g->N) return CPBUS_ENOSPC;
-  int rc = group_flush(g, g->now); if (rc) return rc;
+  int rc = flush_staged(g, g->now); if (rc) return rc;
   const uint32_t first = g->n_next;
   rc = group_each_range(g, first, n, [&](cpbus* s, uint32_t, uint32_t off, uint32_t cnt) -> int {
     uint32_t id = 0;
@@ -2655,13 +2708,10 @@ int cpbus_group_unsubscribe(cpbus_group_t* g, uint32_t sub_id) try {
   if (!g) return CPBUS_EINVAL;
   cpbus* s = nullptr; uint32_t l = 0;
   if (!group_locate(g, sub_id, &s, &l)) return CPBUS_ENOENT;
-  int rc = group_flush(g, g->now); if (rc) return rc;
+  int rc = flush_staged(g, g->now); if (rc) return rc;
   if ((rc = cpbus_unsubscribe(s, sub_id))) return rc;
-  if (g->K && !g->timers.empty())
-    for (uint32_t k = 0; k < g->K; k++) {
-      cpbus_group::Slot& t = g->timers[(size_t)(sub_id - g->base) * g->K + k];
-      if (t.active) { t.active = false; g->n_timers--; }
-    }
+  if (g->K && !g->h_timers.empty())
+    for (uint32_t k = 0; k < g->K; k++) timer_disarm(g, (size_t)(sub_id - g->base) * g->K + k, /*reset_bound=*/false);
   g->n_active--;
   return CPBUS_OK;
 } CPBUS_CATCH
@@ -2671,7 +2721,7 @@ int cpbus_group_set_mask(cpbus_group_t* g, uint32_t sub_id, uint32_t mask) try {
   cpbus* s = nullptr; uint32_t l = 0;
   if (!group_locate(g, sub_id, &s, &l)) return CPBUS_ENOENT;
   if (!s->h_active[l]) return CPBUS_ECLOSED;
-  const int rc = group_flush(g, g->now); if (rc) return rc;
+  const int rc = flush_staged(g, g->now); if (rc) return rc;
   return cpbus_set_mask(s, sub_id, mask);
 } CPBUS_CATCH
 
@@ -2680,8 +2730,8 @@ int cpbus_group_timer_add(cpbus_group_t* g, uint32_t sub_id, uint64_t period_ns,
   if (!g->K) return CPBUS_ENOSPC;
   cpbus* s = nullptr; uint32_t l = 0;
   if (!group_locate(g, sub_id, &s, &l)) return CPBUS_ENOENT;
-  int rc = group_flush(g, g->now); if (rc) return rc;
-  if (g->timers.empty()) g->timers.resize((size_t)g->N * g->K);
+  int rc = flush_staged(g, g->now); if (rc) return rc;
+  if (g->h_timers.empty()) g->h_timers.resize((size_t)g->N * g->K);
   group_retire(g);
   if (!s->h_active[l]) return CPBUS_ECLOSED;
   if ((rc = group_shard_clock(g, s))) return rc;
@@ -2689,11 +2739,7 @@ int cpbus_group_timer_add(cpbus_group_t* g, uint32_t sub_id, uint64_t period_ns,
   if ((rc = cpbus_timer_add(s, sub_id, period_ns, source_id, oneshot, &id))) return rc;
   const uint32_t shard_base_slot = (sub_id - l - g->base) * g->K;   // global slot of the shard's slot 0
   const size_t slot = (size_t)(id & kTimerSlotMask) + shard_base_slot;
-  cpbus_group::Slot& t = g->timers[slot];
-  t.active = true; t.oneshot = oneshot != 0; t.next_due = due_after(g->now, period_ns);
-  g->n_timers++;
-  if (!oneshot) g->min_period = std::min(g->min_period, period_ns);
-  else g->oneshot_idx.push_back(slot);
+  timer_arm(g, slot, period_ns, source_id, oneshot != 0);
   if (timer_id) *timer_id = (uint32_t)slot | (id & ~kTimerSlotMask);
   return CPBUS_OK;
 } CPBUS_CATCH
@@ -2702,17 +2748,17 @@ int cpbus_group_timer_add_many(cpbus_group_t* g, uint32_t first_sub, uint32_t n,
                                uint32_t source_id0, int oneshot) try {
   if (!g || !period_ns || !n) return CPBUS_EINVAL;
   if (!g->K) return CPBUS_ENOSPC;
-  const uint32_t i0 = first_sub - g->base;
-  if (first_sub < g->base || (uint64_t)i0 + n > g->n_next) return CPBUS_ENOENT;
-  int rc = group_flush(g, g->now); if (rc) return rc;
-  if (g->timers.empty()) g->timers.resize((size_t)g->N * g->K);
+  uint32_t i0 = 0;
+  if (!id_range(g->base, g->n_next, first_sub, n, &i0)) return CPBUS_ENOENT;
+  int rc = flush_staged(g, g->now); if (rc) return rc;
+  if (g->h_timers.empty()) g->h_timers.resize((size_t)g->N * g->K);
   group_retire(g);
   // the single bus checks every subscriber before it arms any
   for (uint32_t i = 0; i < n; i++) {
     cpbus* s = nullptr; uint32_t l = 0;
     group_locate(g, first_sub + i, &s, &l);
     if (!s->h_active[l]) return CPBUS_ECLOSED;
-    if (g->timers[(size_t)(i0 + i) * g->K].active) return CPBUS_ENOSPC;
+    if (g->h_timers[(size_t)(i0 + i) * g->K].active) return CPBUS_ENOSPC;
   }
   rc = group_each_range(g, i0, n, [&](cpbus* s, uint32_t l, uint32_t off, uint32_t cnt) -> int {
     const int rc_clock = group_shard_clock(g, s);
@@ -2721,58 +2767,28 @@ int cpbus_group_timer_add_many(cpbus_group_t* g, uint32_t first_sub, uint32_t n,
                                 source_id0 + off, oneshot);
   });
   if (rc) return rc;
-  for (uint32_t i = 0; i < n; i++) {
-    const size_t slot = (size_t)(i0 + i) * g->K;
-    cpbus_group::Slot& t = g->timers[slot];
-    t.active = true; t.oneshot = oneshot != 0; t.next_due = due_after(g->now, period_ns);
-    if (oneshot) g->oneshot_idx.push_back(slot);
-  }
-  g->n_timers += n;
-  if (!oneshot) g->min_period = std::min(g->min_period, period_ns);
+  for (uint32_t i = 0; i < n; i++)
+    timer_arm(g, (size_t)(i0 + i) * g->K, period_ns, source_ids ? source_ids[i] : source_id0 + i, oneshot != 0);
   return CPBUS_OK;
 } CPBUS_CATCH
 
 int cpbus_group_timer_cancel(cpbus_group_t* g, uint32_t timer_id) try {
   if (!g) return CPBUS_EINVAL;
-  if (!g->K || g->timers.empty()) return CPBUS_ENOENT;
+  if (!g->K || g->h_timers.empty()) return CPBUS_ENOENT;
   const uint32_t slot = timer_id & kTimerSlotMask, i = slot / g->K;
   if (i >= g->n_next) return CPBUS_ENOENT;
-  int rc = group_flush(g, g->now); if (rc) return rc;
+  int rc = flush_staged(g, g->now); if (rc) return rc;
   group_retire(g);
   const uint32_t k = group_shard_of(g, i);
   const uint32_t local = (slot - g->first[k] * g->K) | (timer_id & ~kTimerSlotMask);
   if ((rc = cpbus_timer_cancel(g->shards[k], local))) return rc;
-  g->timers[slot].active = false; g->n_timers--;
-  if (g->n_timers == 0) g->min_period = UINT64_MAX;
+  timer_disarm(g, slot, /*reset_bound=*/true);
   return CPBUS_OK;
 } CPBUS_CATCH
 
-static void group_dbg_put(cpbus_group* g, const cpbus_event& e) {   // dbg_ring_put
-  g->dbg[(g->dbg_head + 1) % 10] = e;
-  const int old = g->dbg_head;
-  g->dbg_head = (g->dbg_head + 1) % 10;
-  if (old != -1 && g->dbg_head == g->dbg_tail) g->dbg_tail = (g->dbg_tail + 1) % 10;
-}
-
 int cpbus_group_publish(cpbus_group_t* g, const cpbus_event* ev, size_t n) try {
   if (!g || (!ev && n)) return CPBUS_EINVAL;
-  auto dbg_tail = [&](size_t published) {   // as cpbus_publish: the last 10 of the burst
-    for (size_t j = published > 10 ? published - 10 : 0; j < published; j++) {
-      cpbus_event e{};
-      e.seq = g->seq - (published - j); e.ts_ns = g->now; e.code = ev[j].code; e.source_id = ev[j].source_id; e.target = CPBUS_TARGET_ALL;
-      group_dbg_put(g, e);
-    }
-  };
-  for (size_t i = 0; i < n; i++) if (ev[i].code >= CPBUS_N_CODES) return CPBUS_EINVAL;
-  for (size_t i = 0; i < n; i++) {
-    const uint32_t code = ev[i].code;
-    const int rc = group_stage(g, code, ev[i].source_id, CPBUS_TARGET_ALL, 0);
-    if (rc) { dbg_tail(i); return rc; }
-    if (code != CPBUS_METRIC) { g->by_code[code]++; g->pub_pairs.add(((uint64_t)code << 32) | ev[i].source_id, 1); }
-    g->publishes++;
-  }
-  dbg_tail(n);
-  return CPBUS_OK;
+  return publish_burst(g, ev, n);
 } CPBUS_CATCH
 
 int cpbus_group_send(cpbus_group_t* g, uint32_t sub_id, const cpbus_event* ev) try {
@@ -2780,27 +2796,18 @@ int cpbus_group_send(cpbus_group_t* g, uint32_t sub_id, const cpbus_event* ev) t
   cpbus* s = nullptr; uint32_t l = 0;
   if (!group_locate(g, sub_id, &s, &l)) return CPBUS_ENOENT;
   if (!s->h_active[l]) return CPBUS_ECLOSED;
-  const int rc = group_stage(g, ev->code, ev->source_id, sub_id, CPBUS_F_UNICAST);
+  const int rc = stage_one(g, ev->code, ev->source_id, sub_id, CPBUS_F_UNICAST);
   if (rc) return rc;
   g->publishes++;
   return CPBUS_OK;
 } CPBUS_CATCH
 
 int cpbus_group_advance(cpbus_group_t* g, uint64_t now_ns) try {
-  if (!g) return CPBUS_EINVAL;
-  if (now_ns < g->now) return CPBUS_EORDER;
-  if (now_ns == g->now) return CPBUS_OK;
-  const uint64_t win = group_window(g);   // the single bus's grid: a stream batch never steps past a shard's window
-  while (win != UINT64_MAX && now_ns - g->last_watermark > win) {
-    g->now = g->last_watermark + win;
-    const int rc = group_flush(g, g->now); if (rc) return rc;
-  }
-  g->now = now_ns;
-  return CPBUS_OK;
+  return g ? advance_clock(g, now_ns) : CPBUS_EINVAL;
 } CPBUS_CATCH
 
 int cpbus_group_flush(cpbus_group_t* g) try {
-  return g ? group_flush(g, g->now) : CPBUS_EINVAL;
+  return g ? flush_staged(g, g->now) : CPBUS_EINVAL;
 } CPBUS_CATCH
 
 int cpbus_group_sync(cpbus_group_t* g) try {
@@ -2833,36 +2840,27 @@ int cpbus_group_drain_ready(cpbus_group_t* g, uint32_t first_sub, uint32_t n, ui
                             cpbus_ready* ready, size_t ready_cap, size_t* n_ready, size_t* total, uint32_t* next_sub) try {
   if (!g || !out || !ready || !n_ready || !total || !next_sub || !n || !ready_cap) return CPBUS_EINVAL;
   if (cap < g->shards[0]->R || cap > 0xFFFFFFFFull) return CPBUS_EINVAL;
-  if (start_sub < first_sub || start_sub - first_sub >= n) return CPBUS_EINVAL;
-  const uint32_t i0 = first_sub - g->base;
-  if (first_sub < g->base || (uint64_t)i0 + n > g->n_next) return CPBUS_ENOENT;
   size_t nr = 0, tot = 0, ready_left = std::min<size_t>(ready_cap, n);
-  const uint32_t rot = start_sub - first_sub;
-  *next_sub = start_sub;
-  for (uint32_t done = 0; done < n;) {
-    const uint32_t i = i0 + (rot + done) % n;                       // global index of the walk's next mailbox
-    const uint32_t k = group_shard_of(g, i);
-    const uint32_t wrap = i0 + n - i;                               // the walk wraps to first_sub after this many
-    const uint32_t cnt = std::min({n - done, g->first[k + 1] - i, wrap});
-    cpbus* s = g->shards[k];
-    const uint32_t l = i - g->first[k], a = g->base + i;
+  const int rc = group_walk(g, first_sub, n, start_sub, next_sub, [&](cpbus* s, uint32_t l, uint32_t a, uint32_t cnt) -> int {
     if (ready_left == 0 || tot == cap) {                           // no room: the next ready mailbox ends the walk
       uint32_t at = cnt;
-      const int rc = group_first_ready(s, l, cnt, &at); if (rc) return rc;
-      if (at < cnt) { *next_sub = a + at; break; }
-      done += cnt;
-      continue;
+      const int rc_s = group_first_ready(s, l, cnt, &at); if (rc_s) return rc_s;
+      if (at == cnt) return CPBUS_OK;
+      *next_sub = a + at;
+      return kWalkEnd;
     }
     size_t nr_s = 0, tot_s = 0;
     uint32_t next_s = a;
     bool all = false;
-    const int rc = drain_ready_impl(s, a, cnt, a, out + tot, cap - tot, ready + nr, ready_left, &nr_s, &tot_s, &next_s, &all);
-    if (rc) return rc;
+    const int rc_s = drain_ready_impl(s, a, cnt, a, out + tot, cap - tot, ready + nr, ready_left, &nr_s, &tot_s, &next_s, &all);
+    if (rc_s) return rc_s;
     for (size_t j = 0; j < nr_s; j++) ready[nr + j].offset += (uint32_t)tot;
     nr += nr_s; tot += tot_s; ready_left -= nr_s;
-    if (!all) { *next_sub = next_s; break; }
-    done += cnt;
-  }
+    if (all) return CPBUS_OK;
+    *next_sub = next_s;
+    return kWalkEnd;
+  });
+  if (rc) return rc;
   *n_ready = nr; *total = tot;
   return CPBUS_OK;
 } CPBUS_CATCH
@@ -2872,32 +2870,24 @@ int cpbus_group_drain_ready(cpbus_group_t* g, uint32_t first_sub, uint32_t n, ui
 int cpbus_group_lagging(cpbus_group_t* g, uint32_t first_sub, uint32_t n, uint32_t start_sub, uint32_t min_backlog, cpbus_lag* out,
                         size_t cap, size_t* n_out, uint32_t* next_sub, cpbus_lag_summary* sum) try {
   if (!g || !n_out || !next_sub || !n || (!out && cap)) return CPBUS_EINVAL;
-  if (start_sub < first_sub || start_sub - first_sub >= n) return CPBUS_EINVAL;
-  const uint32_t i0 = first_sub - g->base;
-  if (first_sub < g->base || (uint64_t)i0 + n > g->n_next) return CPBUS_ENOENT;
-  const uint32_t rot = start_sub - first_sub;
   cpbus_lag_summary acc{};
   size_t got = 0;
   bool cut = false;
-  *next_sub = start_sub;
-  for (uint32_t done = 0; done < n;) {
-    const uint32_t i = i0 + (rot + done) % n;                       // global index of the walk's next mailbox
-    const uint32_t k = group_shard_of(g, i);
-    const uint32_t cnt = std::min({n - done, g->first[k + 1] - i, i0 + n - i});
-    const uint32_t a = g->base + i;
+  const int rc = group_walk(g, first_sub, n, start_sub, next_sub, [&](cpbus* s, uint32_t, uint32_t a, uint32_t cnt) -> int {
     cpbus_lag_summary part{};
     size_t n_s = 0;
     uint32_t next_s = a;
     bool all = false;
-    const int rc = lagging_impl(g->shards[k], a, cnt, a, min_backlog, out ? out + got : nullptr, cap - got, &n_s, &next_s, &part, &all);
-    if (rc) return rc;
+    const int rc_s = lagging_impl(s, a, cnt, a, min_backlog, out ? out + got : nullptr, cap - got, &n_s, &next_s, &part, &all);
+    if (rc_s) return rc_s;
     got += n_s;
     if (!all && !cut) { *next_sub = next_s; cut = true; }
     acc.active += part.active; acc.lagging += part.lagging; acc.backlog_total += part.backlog_total;
     acc.backlog_max = std::max(acc.backlog_max, part.backlog_max); acc.lost_total += part.lost_total;
     for (int h = 0; h < 33; h++) acc.hist[h] += part.hist[h];
-    done += cnt;
-  }
+    return CPBUS_OK;
+  });
+  if (rc) return rc;
   *n_out = got;
   if (sum) *sum = acc;
   return CPBUS_OK;
@@ -2940,8 +2930,8 @@ int cpbus_group_peek_window(cpbus_group_t* g, uint32_t sub_id, cpbus_event* out,
 
 int cpbus_group_digest(cpbus_group_t* g, uint32_t first_sub, uint32_t n, cpbus_digest_t* out) try {
   if (!g || !out || !n) return CPBUS_EINVAL;
-  const uint32_t i0 = first_sub - g->base;
-  if (first_sub < g->base || (uint64_t)i0 + n > g->n_next) return CPBUS_ENOENT;
+  uint32_t i0 = 0;
+  if (!id_range(g->base, g->n_next, first_sub, n, &i0)) return CPBUS_ENOENT;
   return group_each_range(g, i0, n, [&](cpbus* s, uint32_t l, uint32_t off, uint32_t cnt) -> int {
     return cpbus_digest(s, s->cfg.sub_id_base + l, cnt, out + off);
   });
@@ -2949,8 +2939,8 @@ int cpbus_group_digest(cpbus_group_t* g, uint32_t first_sub, uint32_t n, cpbus_d
 
 int cpbus_group_digest_fold(cpbus_group_t* g, uint32_t first_sub, uint32_t n, uint64_t out[4]) try {
   if (!g || !out || !n) return CPBUS_EINVAL;
-  const uint32_t i0 = first_sub - g->base;
-  if (first_sub < g->base || (uint64_t)i0 + n > g->n_next) return CPBUS_ENOENT;
+  uint32_t i0 = 0;
+  if (!id_range(g->base, g->n_next, first_sub, n, &i0)) return CPBUS_ENOENT;
   uint64_t acc[4] = {0, 0, 0, 0};
   const int rc = group_each_range(g, i0, n, [&](cpbus* s, uint32_t l, uint32_t, uint32_t cnt) -> int {
     uint64_t part[4];
@@ -2966,17 +2956,7 @@ int cpbus_group_digest_fold(cpbus_group_t* g, uint32_t first_sub, uint32_t n, ui
 
 int cpbus_group_debug_events(cpbus_group_t* g, cpbus_event* out, size_t cap, size_t* n) try {   // cpbus_debug_events
   if (!g || !n || (!out && cap)) return CPBUS_EINVAL;
-  size_t k = 0;
-  for (;;) {
-    if (g->dbg_head == -1) break;
-    const cpbus_event e = g->dbg[g->dbg_tail % 10];
-    if (g->dbg_tail == g->dbg_head) { g->dbg_head = -1; g->dbg_tail = 0; }
-    else g->dbg_tail = (g->dbg_tail + 1) % 10;
-    if (e.code == CPBUS_NONE && e.source_id == 0) break;
-    if (k < cap) out[k] = e;
-    k++;
-  }
-  *n = k;
+  *n = dbg_read(g, out, cap);
   return CPBUS_OK;
 } CPBUS_CATCH
 
@@ -2993,7 +2973,7 @@ int cpbus_group_stats(cpbus_group_t* g, cpbus_stats_t* out) try {
   }
   group_retire(g);
   sum.publishes = g->publishes;
-  for (int c = 0; c < CPBUS_N_CODES; c++) sum.published_by_code[c] = g->by_code[c];
+  for (int c = 0; c < CPBUS_N_CODES; c++) sum.published_by_code[c] = g->published_by_code[c];
   sum.n_subs = g->n_active; sum.n_timers = g->n_timers; sum.now_ns = g->now;
   sum.intern_entries = s0.intern_entries; sum.intern_bytes = s0.intern_bytes;
   sum.ephemeral_live = s0.ephemeral_live; sum.ephemeral_recycled = s0.ephemeral_recycled;
@@ -3003,11 +2983,7 @@ int cpbus_group_stats(cpbus_group_t* g, cpbus_stats_t* out) try {
 
 int cpbus_group_publish_counts(cpbus_group_t* g, cpbus_pair_count* out, size_t cap, size_t* n) try {
   if (!g || !n || (!out && cap)) return CPBUS_EINVAL;
-  std::vector<std::pair<uint64_t, uint64_t>> v;
-  for (size_t i = 0; i < g->pub_pairs.keys.size(); i++) if (g->pub_pairs.keys[i]) v.emplace_back(g->pub_pairs.keys[i] - 1, g->pub_pairs.cnts[i]);
-  std::sort(v.begin(), v.end());
-  for (size_t i = 0; i < v.size() && i < cap; i++) out[i] = cpbus_pair_count{(uint32_t)(v[i].first >> 32), (uint32_t)v[i].first, v[i].second};
-  *n = v.size();
+  pair_counts(g, nullptr, nullptr, 0, out, cap, n);
   return CPBUS_OK;
 } CPBUS_CATCH
 
