@@ -18,12 +18,13 @@ N_CODES = 17
 MASK_ALL = 0x0001FFFF
 TARGET_ALL = 0xFFFFFFFF
 F_TICK, F_UNICAST = 0x1, 0x2
-CFG_LOSSLESS, CFG_DIGEST = 0x1, 0x2
+CFG_LOSSLESS, CFG_DIGEST, CFG_SPARSE_TICKS = 0x1, 0x2, 0x4
 STORE_AUTO, STORE_V4, STORE_V8, STORE_BULK = 0, 1, 2, 3
 
 OK, EINVAL, ENOMEM, ECUDA, EAGAIN, ENOSPC, ENOENT, ECLOSED, ENODEV, EORDER, ETIMEDOUT = 0, -1, -2, -3, -4, -5, -6, -7, -8, -9, -10
 PUT_STAMP, PUT_RAW, PUT_NOWAIT = 0, 1, 2
 EPHEMERAL_BIT, EPHEMERAL_SLOTS = 0x80000000, 65536
+DUE_CLOCK, DUE_ARM, DUE_ONESHOT, DUE_DISARM, DUE_UNSUB, DUE_LAUNCH = 0, 1, 2, 3, 4, 5
 
 
 class Event(C.Structure):
@@ -69,6 +70,10 @@ assert C.sizeof(Event) == 32
 # cpbus_lag: one entry of cpbus_lagging's list
 LAG_DTYPE = np.dtype([("sub_id", "<u4"), ("backlog", "<u4"), ("lost", "<u8")])
 assert LAG_DTYPE.itemsize == 16
+# cpbus_due_op / cpbus_due_fire: cpbus_due_trace's ops and what its launches fire
+DUE_OP_DTYPE = np.dtype([("kind", "<u4"), ("slot", "<u4"), ("value", "<u8")])
+DUE_FIRE_DTYPE = np.dtype([("launch", "<u8"), ("slot", "<u4"), ("pad", "<u4"), ("ticks", "<u8"), ("next_due", "<u8")])
+assert DUE_OP_DTYPE.itemsize == 16 and DUE_FIRE_DTYPE.itemsize == 32
 
 # every symbol include/cpbus.h declares: (restype, argtypes)
 _P = C.POINTER
@@ -139,6 +144,7 @@ SYMBOLS = {
     "cpbus_abi_version": (C.c_uint32, []),
     "cpbus_split_plan": (C.c_int, [C.c_void_p, C.c_size_t, C.c_uint32, C.c_uint64, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p, C.c_size_t, _P(C.c_size_t)]),
     "cpbus_mask_order": (C.c_size_t, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int, C.c_void_p]),
+    "cpbus_due_trace": (C.c_int, [C.c_void_p, C.c_size_t, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t, _P(C.c_size_t)]),
     "cpbus_record_hash": (C.c_uint64, [_P(Event)]),
     "cpbus_digest_multiplier": (C.c_uint64, []),
 }

@@ -13,6 +13,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <deque>
+#include <map>
 #include <mutex>
 #include <new>
 #include <string>
@@ -73,6 +74,103 @@ inline uint64_t due_after(uint64_t t, uint64_t period) { return period >= kTimer
 inline bool oneshot_fired(uint64_t next_due, uint64_t w) { return next_due <= w && next_due != kTimerIdle; }
 // timer id = slot index (subscriber * K + k) | generation << 26: a late cancel from an old context cannot disarm a re-armed slot
 constexpr uint32_t kTimerSlotBits = 26, kTimerSlotMask = (1u << kTimerSlotBits) - 1u;
+
+// The due index of a CPBUS_CFG_SPARSE_TICKS bus: every armed slot whose next due time is not kTimerIdle, as {due, slot}
+// entries in buckets of 2^kDueShift ns of due time (a calendar queue: a std::map from bucket to an unsorted vector of
+// entries, with a lower bound of the bucket's due times).  Arming appends to one bucket, O(1) after the bucket's lookup;
+// a launch to w takes the buckets wholly at or before w and scans the one that w falls in.  Nothing is removed from the
+// middle of a bucket: a cancel, an unsubscribe or a re-arm bumps the slot's version, and an entry whose version is not the
+// slot's any more is stale and skipped (32-bit versions, so a stale entry never passes for a live one the way a 6-bit
+// timer-id generation could).  The whole index is rebuilt when stale entries outnumber the live ones.  A live slot's due
+// time is also its HostTimer::next_due.  (A binary heap was measured first: at 10^6 slots each pop costs ~20 cache misses,
+// ~2 us per due slot on the host; DESIGN.md §4.6.)
+struct DueIndex {
+  static constexpr int kDueShift = 20;   // ~1 ms of due time per bucket: the pump's step
+  struct Entry { uint64_t due; uint32_t slot, ver; };
+  struct Bucket { uint64_t lo = kTimerIdle; std::vector<Entry> e; };   // lo <= every live due in e
+  std::map<uint64_t, Bucket> buckets;
+  std::vector<uint32_t> ver;      // per slot
+  std::vector<uint8_t> live;      // per slot: its current entry is in a bucket
+  size_t n_live = 0, n_entries = 0;
+  bool stale(const Entry& e) const { return ver[e.slot] != e.ver; }
+  void init(size_t n_slots) { buckets.clear(); hot = nullptr; ver.assign(n_slots, 0); live.assign(n_slots, 0); n_live = n_entries = 0; }
+  void drop(uint32_t slot) {
+    ver[slot]++;
+    if (live[slot]) { live[slot] = 0; n_live--; }
+  }
+  Bucket* hot = nullptr;          // the bucket the last insert went to (re-arms of one launch mostly share one)
+  uint64_t hot_key = 0;
+  void insert(const Entry& e) {
+    const uint64_t k = e.due >> kDueShift;
+    if (!hot || hot_key != k) { hot = &buckets[k]; hot_key = k; }
+    hot->e.push_back(e); hot->lo = std::min(hot->lo, e.due);
+    n_entries++;
+  }
+  void put(uint32_t slot, uint64_t due) {
+    drop(slot);
+    if (due == kTimerIdle) return;   // "never": not indexed, though the slot stays armed
+    live[slot] = 1; n_live++;
+    insert(Entry{due, slot, ver[slot]});
+    if (n_entries > 2 * n_live + 64) compact();
+  }
+  void compact() {
+    std::map<uint64_t, Bucket> old;
+    old.swap(buckets);
+    hot = nullptr; n_entries = 0;
+    for (auto& kv : old) for (const Entry& e : kv.second.e) if (!stale(e)) insert(e);
+  }
+  // a lower bound of the earliest due time (kTimerIdle: nothing indexed); exact unless the first bucket holds stale entries
+  uint64_t min_due() const { return buckets.empty() ? kTimerIdle : buckets.begin()->second.lo; }
+  // The live slots due at or before w, appended to *out in no particular order, when there are at most cap of them (true);
+  // false as soon as there are more.  Reads only the buckets that begin at or before w.
+  bool collect(uint64_t w, size_t cap, std::vector<uint32_t>* out) const {
+    size_t found = 0;
+    for (auto it = buckets.begin(); it != buckets.end() && it->first <= (w >> kDueShift); ++it)
+      for (const Entry& e : it->second.e)
+        if (e.due <= w && !stale(e)) {
+          if (++found > cap) return false;
+          out->push_back(e.slot);
+        }
+    return true;
+  }
+};
+
+// Firings of a periodic slot due at `due` <= w in one launch to w, as the kernel counts them: the candidates due + j *
+// period <= w that do not reach kTimerIdle.  And the due time after k firings, saturating like the kernel's re-arm.
+inline uint64_t due_ticks(uint64_t due, uint64_t period, uint64_t w) { return (std::min(w, kTimerIdle - 1) - due) / period + 1; }
+inline uint64_t due_rearm(uint64_t due, uint64_t period, uint64_t k) {
+  uint64_t step = 0;
+  return (__builtin_mul_overflow(k, period, &step) || step >= kTimerIdle - due) ? kTimerIdle : due + step;
+}
+
+// After a launch to watermark w (any kernel that fires timers): every live slot due at or before w has fired on the device.
+// A one-shot is done and leaves the index (retire_oneshots retires it in the host table as before); a periodic slot moves on
+// by k = (w - due) / period + 1 periods into a later bucket.  on_fire(slot, ticks, next due) is told about each.  Each bucket
+// that begins at or before w is taken out whole and its entries are fired, dropped as stale, or (only in the bucket w falls
+// in) put back: O(due slots + that bucket), at most one pass over the table when every slot is due.
+template <class F>
+void due_fire(DueIndex& x, std::vector<HostTimer>& tm, uint64_t w, F&& on_fire) {
+  const uint64_t last = w >> DueIndex::kDueShift;
+  for (auto it = x.buckets.begin(); it != x.buckets.end() && it->first <= last;) {
+    std::vector<DueIndex::Entry> v;
+    v.swap(it->second.e);
+    it = x.buckets.erase(it);   // (re-arms land after w, so in this bucket at the earliest: never in front of `it`)
+    x.hot = nullptr;
+    x.n_entries -= v.size();
+    for (const DueIndex::Entry& e : v) {
+      if (x.stale(e)) continue;
+      if (e.due > w) { x.insert(e); continue; }
+      HostTimer& t = tm[e.slot];
+      if (t.oneshot) { x.drop(e.slot); on_fire(e.slot, (uint64_t)1, kTimerIdle); continue; }
+      const uint64_t k = due_ticks(t.next_due, t.period, w);
+      t.next_due = due_rearm(t.next_due, t.period, k);
+      on_fire(e.slot, k, t.next_due);
+      if (t.next_due == kTimerIdle) { x.drop(e.slot); continue; }
+      x.ver[e.slot]++;   // a new entry for the slot, still live
+      x.insert(DueIndex::Entry{t.next_due, e.slot, x.ver[e.slot]});
+    }
+  }
+}
 
 // The host front end: what the single bus (cpbus) and the group (cpbus_group) keep over their whole id space, and what the
 // rules below share — the clock window (max_window), timer arming and retirement, staging (stage_one), the publish loop
@@ -206,6 +304,15 @@ struct cpbus : HostFront {
   // can append to one mailbox) the admission pass and its host sync are skipped; the bound is refreshed exactly whenever
   // the admission kernel does run, and reset by cpbus_consume_all.
   uint64_t room_lb = 0;
+
+  // CPBUS_CFG_SPARSE_TICKS: the armed slots by due time, and the tick kernel's list of due mailboxes ({local index, due-slot
+  // bits}), staged in pinned memory and copied on the copy stream into a device buffer that grows on demand
+  bool sparse = false;
+  DueIndex due;
+  std::vector<uint32_t> due_slots;
+  uint2* h_tick_list = nullptr; uint2* d_tick_list = nullptr; size_t tick_list_cap = 0;
+  cudaEvent_t tick_list_done = nullptr;   // on copy_stream: the list has reached HBM (and left the pinned buffer)
+  cudaEvent_t tick_done = nullptr;        // on the bus stream: the tick kernel is done with the list
 
   // intern table (Event.Source string <-> u32)
   std::unordered_map<std::string, uint32_t> intern;
@@ -571,8 +678,97 @@ int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, co
   if (!round) b->st.batches++;   // (a round's batch counts when it is resolved, if it delivered)
   if (sa) return CPBUS_OK;       // (the caller folds a stream launch in once its outcome is known: stream_delivered)
   b->last_watermark = w;
+  if (b->sparse) due_fire(b->due, b->h_timers, w, [](uint32_t, uint64_t, uint64_t) {});
   if (o.account && n) dbg_mark_device_batch(b, p.launch_seq);
   return CPBUS_OK;
+}
+
+// CPBUS_CFG_SPARSE_TICKS: the tick kernel over the due mailboxes in h_tick_list[0, n), to watermark w.  The list goes up on
+// the copy stream once the previous tick kernel is done with the device buffer; the kernel runs on the bus stream behind
+// every earlier launch (no programmatic dependent launch: it neither waits for nor releases a fan-out's prologue).
+int launch_ticks(cpbus* b, size_t n, uint64_t w) {
+  CK(cudaStreamWaitEvent(b->copy_stream, b->tick_done, 0));
+  CK(cudaMemcpyAsync(b->d_tick_list, b->h_tick_list, n * sizeof(uint2), cudaMemcpyHostToDevice, b->copy_stream));
+  CK(cudaEventRecord(b->tick_list_done, b->copy_stream));
+  CK(cudaStreamWaitEvent(b->stream, b->tick_list_done, 0));
+  TickScatterParams p{};
+  p.list = b->d_tick_list; p.n_list = (uint32_t)n;
+  p.ring = b->d_ring; p.ctl = b->d_ctl; p.timers = b->d_timers; p.stats = b->d_stats; p.pow_table = b->d_pow;
+  p.launch_seq = ++b->launch_seq;
+  p.result = b->d_result + (size_t)(p.launch_seq % kResultRing) * kResultSub;
+  p.result_next = b->d_result + (size_t)((p.launch_seq + 1) % kResultRing) * kResultSub;
+  p.w_now = w; p.ring_cap = b->R; p.K = b->K; p.sub_base = b->cfg.sub_id_base; p.use_digest = b->use_digest ? 1u : 0u;
+  tick_scatter_kernel<<<(uint32_t)((n + kWarpsPerCta - 1) / kWarpsPerCta), kThreads, 0, b->stream>>>(p);
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(b->tick_done, b->stream));
+  b->st.kernel_launches++;
+  b->last_watermark = w;
+  due_fire(b->due, b->h_timers, w, [](uint32_t, uint64_t, uint64_t) {});
+  return CPBUS_OK;
+}
+
+// The pinned list buffer is free for n entries: the previous list has left it, or both buffers are regrown (behind every
+// kernel that may still read the old device buffer).
+int tick_list_room(cpbus* b, size_t n) {
+  if (n <= b->tick_list_cap) { CK(cudaEventSynchronize(b->tick_list_done)); return CPBUS_OK; }
+  CK(cudaStreamSynchronize(b->stream)); CK(cudaStreamSynchronize(b->copy_stream));
+  cudaFree(b->d_tick_list); cudaFreeHost(b->h_tick_list);
+  b->d_tick_list = nullptr; b->h_tick_list = nullptr; b->tick_list_cap = 0;
+  const size_t cap = std::max<size_t>(n, 1024);
+  CK(cudaMalloc((void**)&b->d_tick_list, cap * sizeof(uint2)));
+  CK(cudaMallocHost((void**)&b->h_tick_list, cap * sizeof(uint2)));
+  b->tick_list_cap = cap;
+  return CPBUS_OK;
+}
+
+// The host timer table, allocated by the first timer, and with it the due index.
+void timer_table(cpbus* b) {
+  b->h_timers.resize((size_t)b->N * b->K);
+  if (b->sparse) b->due.init(b->h_timers.size());
+}
+
+// Due slots beyond which a flush with no record takes the full fan-out instead of the tick kernel.  Measured on an H100
+// (DESIGN.md §4.6): at 1,048,576 subscribers the tick path wins at N/1,024 due slots and loses at N/128.
+size_t sparse_max(const cpbus* b) { return std::max<size_t>(32, b->n_next / 1024); }
+
+// CPBUS_CFG_SPARSE_TICKS, nothing staged: true when the flush is done without the full fan-out (*rc = its status): no tick
+// due in (last watermark, w] launches nothing; up to sparse_max due slots launch the tick kernel.  False: the full fan-out
+// follows — more due slots than that, or (lossless) a room bound that cannot prove the largest share of one mailbox fits.
+bool sparse_flush(cpbus* b, uint64_t w, int* rc) {
+  *rc = CPBUS_OK;
+  if (b->due.min_due() > w) { b->last_watermark = w; return true; }
+  std::vector<uint32_t>& due = b->due_slots;
+  due.clear();
+  if (!b->due.collect(w, sparse_max(b), &due)) return false;
+  if (due.empty()) {   // only stale entries in front (min_due is a lower bound): nothing to launch, drop them
+    b->last_watermark = w;
+    due_fire(b->due, b->h_timers, w, [](uint32_t, uint64_t, uint64_t) {});
+    return true;
+  }
+  std::sort(due.begin(), due.end());
+  uint64_t most = 0;   // the most ticks one mailbox takes
+  std::vector<uint2> list;
+  for (size_t i = 0; i < due.size();) {
+    const uint32_t l = due[i] / b->K;
+    uint32_t bits = 0;
+    uint64_t ticks = 0;
+    for (; i < due.size() && due[i] / b->K == l; i++) {
+      const HostTimer& t = b->h_timers[due[i]];
+      bits |= 1u << (due[i] % b->K);
+      ticks += t.oneshot ? 1 : due_ticks(t.next_due, t.period, w);
+    }
+    list.push_back(make_uint2(l, bits));
+    most = std::max(most, ticks);
+  }
+  const size_t n = list.size();
+  if (b->lossless) {
+    if (b->room_lb < most) return false;
+    b->room_lb -= most; b->st.admit_skipped++;
+  }
+  if ((*rc = tick_list_room(b, n))) return true;
+  std::copy(list.begin(), list.end(), b->h_tick_list);
+  *rc = launch_ticks(b, n, w);
+  return true;
 }
 
 // lossless admission (reference: the sender blocks on a full channel, events/subscriber.go:30-32)
@@ -654,9 +850,10 @@ bool flush_idle(HostFront* f, uint64_t w) {
 
 int flush_staged(cpbus* b, uint64_t w) {
   if (flush_idle(b, w)) return CPBUS_OK;
+  int rc;
+  if (b->sparse && !b->n_staged && sparse_flush(b, w, &rc)) return rc;
   const uint32_t n = (uint32_t)b->n_staged;
   const int c = b->cur;
-  int rc;
   // Device staging is a long ring (kDevSlots batches): a slot is reused only kDevSlots flushes later, far beyond how far the
   // host can run ahead, so the H2D never has to wait for an old fan-out and lands within microseconds.  Reuse safety is a
   // host-side check once per epoch of kDevEpoch slots (almost always already satisfied).
@@ -887,6 +1084,54 @@ size_t cpbus_mask_order(const uint32_t* masks, const uint8_t* active, uint32_t n
     return order.size();
   } catch (const std::bad_alloc&) { return 0; }
 }
+// The due index of a sparse-ticks bus over a table of n_slots slots, driven by ops instead of the bus's entry points (arms
+// start at the clock as timer_arm does; a launch fires what due_fire fires after a launch of the bus).
+int cpbus_due_trace(const cpbus_due_op* ops, size_t n_ops, uint32_t n_slots, uint32_t K, cpbus_due_fire* out, size_t cap,
+                    size_t* n_out) try {
+  if ((!ops && n_ops) || !n_out || (cap && !out) || !(K == 1 || K == 2 || K == 4 || K == 8)) return CPBUS_EINVAL;
+  std::vector<HostTimer> tm(n_slots);
+  DueIndex x;
+  x.init(n_slots);
+  uint64_t clock = 0, last = 0, launches = 0;
+  size_t n = 0;
+  std::vector<cpbus_due_fire> fired;
+  for (size_t i = 0; i < n_ops; i++) {
+    const cpbus_due_op& op = ops[i];
+    switch (op.kind) {
+      case CPBUS_DUE_CLOCK: clock = op.value; break;
+      case CPBUS_DUE_ARM:
+      case CPBUS_DUE_ONESHOT: {
+        if (op.slot >= n_slots || !op.value) return CPBUS_EINVAL;
+        HostTimer& t = tm[op.slot];
+        t.active = true; t.oneshot = op.kind == CPBUS_DUE_ONESHOT; t.period = op.value; t.next_due = due_after(clock, op.value);
+        x.put(op.slot, t.next_due);
+        break;
+      }
+      case CPBUS_DUE_DISARM:
+        if (op.slot >= n_slots) return CPBUS_EINVAL;
+        tm[op.slot].active = false; x.drop(op.slot);
+        break;
+      case CPBUS_DUE_UNSUB:
+        if ((uint64_t)op.slot * K + K > n_slots) return CPBUS_EINVAL;
+        for (uint32_t k = 0; k < K; k++) { tm[op.slot * K + k].active = false; x.drop(op.slot * K + k); }
+        break;
+      case CPBUS_DUE_LAUNCH:
+        if (op.value < last) return CPBUS_EINVAL;
+        last = op.value;
+        fired.clear();
+        due_fire(x, tm, op.value, [&](uint32_t s, uint64_t ticks, uint64_t nd) {
+          fired.push_back(cpbus_due_fire{launches, s, 0u, ticks, nd});
+        });
+        std::sort(fired.begin(), fired.end(), [](const cpbus_due_fire& a, const cpbus_due_fire& b) { return a.slot < b.slot; });
+        for (const cpbus_due_fire& f : fired) { if (n < cap) out[n] = f; n++; }
+        launches++;
+        break;
+      default: return CPBUS_EINVAL;
+    }
+  }
+  *n_out = n;
+  return CPBUS_OK;
+} CPBUS_CATCH
 
 const char* cpbus_last_cuda_error(void) { return g_cuda_err; }
 
@@ -965,6 +1210,7 @@ int cpbus_create(const cpbus_config* cfg, cpbus_t** out) try {
   b->cfg = *cfg; b->cfg.ring_cap = R; b->cfg.batch_cap = B;
   b->N = cfg->n_max_subs; b->R = R; b->B = B; b->K = K;
   b->lossless = cfg->flags & CPBUS_CFG_LOSSLESS; b->use_digest = cfg->flags & CPBUS_CFG_DIGEST;
+  b->sparse = cfg->flags & CPBUS_CFG_SPARSE_TICKS;
   b->room_lb = R;
   b->store = cfg->store_path == CPBUS_STORE_AUTO ? CPBUS_STORE_V8 : (int)cfg->store_path;
   if (const char* e = getenv("CPBUS_PDL")) b->pdl = atoi(e) != 0;
@@ -1002,6 +1248,9 @@ int cpbus_create(const cpbus_config* cfg, cpbus_t** out) try {
   if (cudaStreamCreateWithFlags(&b->copy_stream, cudaStreamNonBlocking) != cudaSuccess) return fail(CPBUS_ECUDA);
   if (cudaStreamCreateWithFlags(&b->result_stream, cudaStreamNonBlocking) != cudaSuccess) return fail(CPBUS_ECUDA);
   if (cudaEventCreateWithFlags(&b->launched, cudaEventDisableTiming) != cudaSuccess) return fail(CPBUS_ECUDA);
+  if (b->sparse && (cudaEventCreateWithFlags(&b->tick_list_done, cudaEventDisableTiming) != cudaSuccess ||
+                    cudaEventCreateWithFlags(&b->tick_done, cudaEventDisableTiming) != cudaSuccess))
+    return fail(CPBUS_ECUDA);
   ALLOC(b->d_stage, (size_t)cpbus::kDevSlots * B * sizeof(cpbus_event));
   for (int i = 0; i < cpbus::kDevSlots / cpbus::kDevEpoch; i++)
     if (cudaEventCreateWithFlags(&b->epoch_done[i], cudaEventDisableTiming) != cudaSuccess) return fail(CPBUS_ECUDA);
@@ -1092,7 +1341,11 @@ int cpbus_destroy(cpbus_t* b) try {
   for (int i = 0; i < cpbus::kDevSlots / cpbus::kDevEpoch; i++) if (b->epoch_done[i]) cudaEventDestroy(b->epoch_done[i]);
   if (b->copy_stream) cudaStreamDestroy(b->copy_stream);
   if (b->launched) cudaEventDestroy(b->launched);
-  cudaFree(b->d_drain); cudaFree(b->d_drain_idx);
+  if (b->tick_list_done) cudaEventDestroy(b->tick_list_done);
+  if (b->tick_done) cudaEventDestroy(b->tick_done);
+  cudaFree(b->d_tick_list);
+  if (b->h_tick_list) cudaFreeHost(b->h_tick_list);
+  cudaFree(b->d_drain);cudaFree(b->d_drain_idx);
   cudaFree(b->d_ready_lb); cudaFree(b->d_ready); cudaFree(b->d_ready_slot);
   if (b->h_ready_hdr) cudaFreeHost(b->h_ready_hdr);
   cudaFree(b->d_lag_lb);
@@ -1281,7 +1534,10 @@ int cpbus_unsubscribe(cpbus_t* b, uint32_t sub_id) try {
   const uint32_t word = 0;
   CK(cudaMemcpyAsync(&b->d_ctl[l].mask, &word, 4, cudaMemcpyHostToDevice, b->stream));
   if (b->K && !b->h_timers.empty()) {
-    for (uint32_t k = 0; k < b->K; k++) timer_disarm(b, (size_t)l * b->K + k, /*reset_bound=*/false);
+    for (uint32_t k = 0; k < b->K; k++) {
+      timer_disarm(b, (size_t)l * b->K + k, /*reset_bound=*/false);
+      if (b->sparse) b->due.drop(l * b->K + k);
+    }
     CK(cudaMemsetAsync(b->d_timers + (size_t)l * b->K, 0xFF, b->K * sizeof(DevTimer), b->stream));
   }
   CK(cudaStreamSynchronize(b->stream));
@@ -1321,12 +1577,13 @@ int cpbus_timer_add(cpbus_t* b, uint32_t sub_id, uint64_t period_ns, uint32_t so
   if (!id_range(b->cfg.sub_id_base, b->n_next, sub_id, 1, &l)) return CPBUS_ENOENT;
   int rc = enter(b); if (rc) return rc;
   if ((rc = flush_staged(b, b->now))) return rc;
-  if (b->h_timers.empty()) b->h_timers.resize((size_t)b->N * b->K);
+  if (b->h_timers.empty()) timer_table(b);
   retire_oneshots(b, b->last_watermark);
   if (!b->h_active[l]) return CPBUS_ECLOSED;
   for (uint32_t k = 0; k < b->K; k++) {
     if (b->h_timers[(size_t)l * b->K + k].active) continue;
     HostTimer& t = timer_arm(b, (size_t)l * b->K + k, period_ns, source_id, oneshot != 0);
+    if (b->sparse) b->due.put(l * b->K + k, t.next_due);
     DevTimer d{}; d.next_due = t.next_due; d.period = oneshot ? 0 : period_ns; d.source_id = source_id; d.fired = 0;
     CK(cudaMemcpyAsync(b->d_timers + (size_t)l * b->K + k, &d, sizeof(d), cudaMemcpyHostToDevice, b->stream));
     CK(cudaStreamSynchronize(b->stream));
@@ -1345,7 +1602,7 @@ int cpbus_timer_add_many(cpbus_t* b, uint32_t first_sub, uint32_t n, uint64_t pe
   if (!id_range(b->cfg.sub_id_base, b->n_next, first_sub, n, &l0)) return CPBUS_ENOENT;
   int rc = enter(b); if (rc) return rc;
   if ((rc = flush_staged(b, b->now))) return rc;
-  if (b->h_timers.empty()) b->h_timers.resize((size_t)b->N * b->K);
+  if (b->h_timers.empty()) timer_table(b);
   // bulk arm: uses slot 0 of each subscriber (must be free)
   retire_oneshots(b, b->last_watermark);
   for (uint32_t i = 0; i < n; i++) {
@@ -1358,6 +1615,7 @@ int cpbus_timer_add_many(cpbus_t* b, uint32_t first_sub, uint32_t n, uint64_t pe
   CK(cudaStreamSynchronize(b->stream));
   for (uint32_t i = 0; i < n; i++) {
     const HostTimer& t = timer_arm(b, (size_t)(l0 + i) * b->K, period_ns, source_ids ? source_ids[i] : source_id0 + i, oneshot != 0);
+    if (b->sparse) b->due.put((l0 + i) * b->K, t.next_due);
     DevTimer& d = dev[(size_t)i * b->K];
     d.next_due = t.next_due; d.period = oneshot ? 0 : period_ns; d.source_id = t.source_id; d.fired = 0; d.pad[0] = d.pad[1] = 0;
   }
@@ -1378,6 +1636,7 @@ int cpbus_timer_cancel(cpbus_t* b, uint32_t timer_id) try {
   const HostTimer& t = b->h_timers[(size_t)l * b->K + k];
   if (!t.active || t.gen != gen) return CPBUS_ENOENT;   // already fired / cancelled, or the slot has been re-armed since
   timer_disarm(b, (size_t)l * b->K + k, /*reset_bound=*/true);
+  if (b->sparse) b->due.drop(l * b->K + k);
   CK(cudaMemsetAsync(b->d_timers + (size_t)l * b->K + k, 0xFF, sizeof(DevTimer), b->stream));
   CK(cudaStreamSynchronize(b->stream));
   return push_mask_words(b, l, 1);
@@ -1625,6 +1884,7 @@ static int stream_bind(cpbus_stream* st) {
 int cpbus_stream_create(cpbus_t* b, uint32_t n_slots, uint32_t n_consumers, cpbus_stream_t** out, unsigned char handle[64]) try {
   if (!b || !out || !handle || n_slots < 4 || n_consumers == 0 || n_consumers > kStreamMaxConsumers) return CPBUS_EINVAL;
   *out = nullptr;
+  if (b->sparse) return CPBUS_EINVAL;   // stream launches move the clock on the device, past the host's due index
   int rc = dev_guard(b); if (rc) return rc;
   cpbus_stream* st = new (std::nothrow) cpbus_stream();
   if (!st) return CPBUS_ENOMEM;
@@ -1655,6 +1915,7 @@ int cpbus_stream_create(cpbus_t* b, uint32_t n_slots, uint32_t n_consumers, cpbu
 int cpbus_stream_open(cpbus_t* b, const unsigned char handle[64], uint32_t consumer_index, cpbus_stream_t** out) try {
   if (!b || !out || !handle || consumer_index == 0 || consumer_index >= kStreamMaxConsumers) return CPBUS_EINVAL;
   *out = nullptr;
+  if (b->sparse) return CPBUS_EINVAL;
   int rc = dev_guard(b); if (rc) return rc;      // the IMPORTING device must be current: the mapping is made for it
   cpbus_stream* st = new (std::nothrow) cpbus_stream();
   if (!st) return CPBUS_ENOMEM;
@@ -1681,7 +1942,7 @@ int cpbus_stream_open(cpbus_t* b, const unsigned char handle[64], uint32_t consu
 // pointer is used directly, with peer access enabled when the consumer's bus lives on another GPU.
 int cpbus_stream_attach(cpbus_t* b, cpbus_stream_t* owner, uint32_t consumer_index, cpbus_stream_t** out) try {
   if (!b || !owner || !owner->owner || !out || consumer_index == 0 || consumer_index >= owner->n_consumers) return CPBUS_EINVAL;
-  if (b->B != owner->B) return CPBUS_EINVAL;
+  if (b->B != owner->B || b->sparse) return CPBUS_EINVAL;
   *out = nullptr;
   int rc = dev_guard(b); if (rc) return rc;
   if (b->device != owner->bus->device) {
@@ -2573,6 +2834,7 @@ int cpbus_group_destroy(cpbus_group_t* g) try {
 int cpbus_group_create(const cpbus_config* cfg, const int32_t* devices, uint32_t n_devices, cpbus_group_t** out) try {
   if (!cfg || !devices || !n_devices || !out || cfg->stream || n_devices > kStreamMaxConsumers) return CPBUS_EINVAL;
   *out = nullptr;
+  if (cfg->flags & CPBUS_CFG_SPARSE_TICKS) return CPBUS_EINVAL;   // the group's flush is a stream batch (see cpbus_stream_create)
   uint32_t R = 0, B = 0;
   if (config_check(cfg, &R, &B) || cfg->n_max_subs < n_devices) return CPBUS_EINVAL;
   cpbus_group* g = new (std::nothrow) cpbus_group();

@@ -215,6 +215,7 @@ class EventBus {   // events/bus.go:12-22
     cpbus_config cfg{};
     cfg.n_max_subs = n_max_subs; cfg.ring_cap = mailbox_cap; cfg.batch_cap = mailbox_cap >= 512 ? 256 : mailbox_cap / 2;
     cfg.timers_per_sub = 4; cfg.flags = CPBUS_CFG_LOSSLESS | CPBUS_CFG_DIGEST; cfg.device = -1;
+    if (devices.empty()) cfg.flags |= CPBUS_CFG_SPARSE_TICKS;   // the 1 ms pump launches only for due ticks (a group has no such mode)
     batch_cap_ = cfg.batch_cap;
     drain_cap_ = std::max<size_t>(kDrainCap, mailbox_cap);
     const int rc = devices.empty() ? ::cpbus_create(&cfg, &h_.one)

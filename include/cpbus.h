@@ -86,6 +86,18 @@ enum {
                                    throughput mode (no consumer needed).          */
 #define CPBUS_CFG_DIGEST   0x2u /* maintain the per-subscriber order-sensitive
                                    64-bit digest in-kernel                       */
+#define CPBUS_CFG_SPARSE_TICKS 0x4u /* a flush with no staged record costs what is due: the
+                                   host keeps an index of the armed timer slots by due
+                                   time; a flush with no tick due launches nothing, and
+                                   one with a few due ticks launches one small kernel over
+                                   the mailboxes that own them (the full fan-out past
+                                   max(32, subscribers/1024) due slots, and in lossless mode when the
+                                   room bound cannot prove that the ticks fit).  Results
+                                   are those of a bus without the flag making the same
+                                   calls, except cpbus_stats.batches, kernel_launches,
+                                   admit_passes and admit_skipped.  Not supported on a
+                                   group (cpbus_group_create) or with streams
+                                   (cpbus_stream_create/_open/_attach): CPBUS_EINVAL. */
 
 /* cpbus_config.store_path: how records reach the rings (all are bit-identical) */
 enum {
@@ -469,7 +481,9 @@ int cpbus_digest_fold_end(cpbus_t* bus, uint32_t ticket, uint64_t out[4]);
 /* Result of the LAST fan-out launch, written by the kernel itself: out = {records delivered by that launch,
  * ticks among them, sum over every mailbox it appended to of fold32(new digest) with
  * fold32(x) = low32(x ^ (x >> 32)), launch ordinal}.
- * _begin enqueues a 256-byte D2H on the bus stream (up to 8 outstanding tickets), _end waits for it. */
+ * _begin enqueues a 256-byte D2H on the bus stream (up to 8 outstanding tickets), _end waits for it.
+ * On a CPBUS_CFG_SPARSE_TICKS bus the tick kernel of a flush with no staged record is such a launch too, and a flush that
+ * launched nothing leaves the result as it was. */
 int cpbus_step_result_begin(cpbus_t* bus, uint32_t* ticket);
 int cpbus_step_result_end(cpbus_t* bus, uint32_t ticket, uint64_t out[4]);
 
@@ -575,6 +589,22 @@ int cpbus_split_plan(const uint64_t* ts, size_t n, uint32_t batch_cap, uint64_t 
  * results never depend on this order. */
 size_t cpbus_mask_order(const uint32_t* masks, const uint8_t* active, uint32_t n, uint32_t ring_cap, uint32_t block,
                         int heavy_first, uint32_t* out);
+/* The due index of a CPBUS_CFG_SPARSE_TICKS bus, as a pure host function (no device needed): ops[0..n_ops) run in order
+ * over a table of n_slots timer slots (slot = subscriber * K + k).  Each op is {kind, slot, value}:
+ *   CPBUS_DUE_CLOCK     the clock becomes value (arming is relative to it)
+ *   CPBUS_DUE_ARM       arm `slot` periodic with period value (> 0): first due = clock + value, saturating at "never"
+ *   CPBUS_DUE_ONESHOT   arm `slot` as a one-shot due at clock + value
+ *   CPBUS_DUE_DISARM    cancel `slot`
+ *   CPBUS_DUE_UNSUB     disarm the K slots of subscriber `slot`
+ *   CPBUS_DUE_LAUNCH    a launch to watermark value: every armed slot due at or before it fires
+ * Each LAUNCH appends, for every slot that fires, in ascending slot order, {launch ordinal (0-based), slot, ticks, next due
+ * (UINT64_MAX: never, or a one-shot that is done)} to out; *n_out = how many entries there are (the first cap are written).
+ * CPBUS_EINVAL: a slot out of range, a period of 0, K not in {1, 2, 4, 8}, or a launch behind the previous launch. */
+enum { CPBUS_DUE_CLOCK = 0, CPBUS_DUE_ARM = 1, CPBUS_DUE_ONESHOT = 2, CPBUS_DUE_DISARM = 3, CPBUS_DUE_UNSUB = 4, CPBUS_DUE_LAUNCH = 5 };
+typedef struct cpbus_due_op { uint32_t kind, slot; uint64_t value; } cpbus_due_op;                       /* sizeof == 16 */
+typedef struct cpbus_due_fire { uint64_t launch; uint32_t slot, pad; uint64_t ticks, next_due; } cpbus_due_fire; /* sizeof == 32 */
+int cpbus_due_trace(const cpbus_due_op* ops, size_t n_ops, uint32_t n_slots, uint32_t K, cpbus_due_fire* out, size_t cap,
+                    size_t* n_out);
 
 #ifdef __cplusplus
 }
