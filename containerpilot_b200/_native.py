@@ -125,6 +125,7 @@ SYMBOLS = {
     "cpbus_lagging": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t,
                                 _P(C.c_size_t), _P(C.c_uint32), _P(LagSummary)]),
     "cpbus_blockers": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, _P(C.c_size_t)]),
+    "cpbus_stream_blockers": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, _P(C.c_size_t)]),
     "cpbus_consume_all": (C.c_int, [C.c_void_p]),
     "cpbus_peek_window": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t, _P(C.c_size_t)]),
     "cpbus_digest": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]),

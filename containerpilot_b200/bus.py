@@ -327,6 +327,20 @@ class Bus:
                 return out[: min(want, n.value)]
             want = n.value
 
+    def stream_blockers(self, st, cap: int | None = None) -> np.ndarray:
+        """Lossless stream shard: the global ids of the mailboxes that give this shard an admissible prefix of 0 for its
+        current batch, ascending (the first `cap`; default all of them).  Empty in throughput mode and while the publisher
+        has not released the batch."""
+        n = C.c_size_t()
+        want = 1024 if cap is None else cap
+        while True:
+            out = np.zeros(max(1, want), dtype=np.uint32)
+            nat.check(self._lib.cpbus_stream_blockers(st, out.ctypes.data if want else None, want, C.byref(n)),
+                      "cpbus_stream_blockers")
+            if cap is not None or n.value <= want:   # (the query changes no state: asking again gives the same list)
+                return out[: min(want, n.value)]
+            want = n.value
+
     def peek_window(self, sub_id: int, cap: int | None = None) -> np.ndarray:
         cap = cap or self.ring_cap
         out = np.zeros(cap, dtype=EVENT_DTYPE)

@@ -2598,6 +2598,36 @@ int cpbus_blockers(cpbus_t* b, uint32_t* out, size_t cap, size_t* n) try {
   return blockers_impl(b, nullptr, b->now, out, cap, n);
 } CPBUS_CATCH
 
+// The next unit of a lossless stream shard, by cpbus_stream_admit's rules: the undelivered remainder of its current batch
+// (after resolution, the batch and offset the device cursor holds) with the watermark from the slot header.  r >= 2
+// records: the first with the ticks due by its ts_ns; r = 1: that record with the ticks due by the watermark (admit holds
+// a last record back when those do not fit); r = 0: the ticks due by the watermark.  The record is one 32-byte copy from
+// the slot, local or peer-mapped, as cpbus_stream_admit copies the remainder.
+int cpbus_stream_blockers(cpbus_stream_t* st, uint32_t* out, size_t cap, size_t* n) try {
+  if (!st || !n || (!out && cap)) return CPBUS_EINVAL;
+  *n = 0;
+  cpbus* b = st->bus;
+  std::lock_guard<std::mutex> g(b->mu);
+  int rc = enter(b); if (rc) return rc;
+  if ((rc = stream_error(b))) return rc;
+  if (!b->lossless) return CPBUS_OK;
+  const unsigned long long q = st->get_seq + 1;
+  StreamHdr h{};
+  CK(cudaMemcpyAsync(&h, &st->hdr[q % st->n_slots], sizeof(h), cudaMemcpyDeviceToHost, b->result_stream));
+  CK(cudaStreamSynchronize(b->result_stream));
+  if (h.seq != q) return CPBUS_OK;   // not released yet: the shard waits for the publisher, not for a consumer
+  if (h.n > st->B || h.n < st->get_off) return CPBUS_EINVAL;
+  // A watermark behind the clock or beyond the timer window makes admission fail with CPBUS_EORDER, not stall.
+  if (h.watermark < b->now || h.watermark - b->last_watermark > max_window(b)) return CPBUS_OK;
+  const uint32_t rem = h.n - st->get_off;
+  if (rem == 0) return blockers_impl(b, nullptr, h.watermark, out, cap, n);
+  cpbus_event e{};
+  CK(cudaMemcpyAsync(&e, st->payload + (size_t)(q % st->n_slots) * st->B + st->get_off, sizeof(e), cudaMemcpyDefault,
+                     b->result_stream));
+  CK(cudaStreamSynchronize(b->result_stream));
+  return blockers_impl(b, &e, rem == 1 ? h.watermark : e.ts_ns, out, cap, n);
+} CPBUS_CATCH
+
 // Device-side consumer: every mailbox of this shard is read to the end and its records are discarded.
 int cpbus_consume_all(cpbus_t* b) try {
   if (!b) return CPBUS_EINVAL;

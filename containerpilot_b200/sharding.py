@@ -107,6 +107,46 @@ def drive_rounds(queue_round, progress, T: int, pump=None, depth: int = 4) -> in
     return queued
 
 
+def _walk(ranges, first_sub: int, n: int, start_sub: int) -> list[tuple[int, int, int]]:
+    """cpbus_group_lagging's walk over shards that own the contiguous id ranges `ranges` [(first, count)]: mailboxes
+    [first_sub, first_sub + n) in cyclic order from start_sub, as pieces (shard, first id, count) in visiting order."""
+    if n <= 0 or not first_sub <= start_sub < first_sub + n:
+        raise nat.CpbusError(nat.EINVAL, "lagging")
+    out, done = [], 0
+    while done < n:
+        i = first_sub + (start_sub - first_sub + done) % n
+        k = next((k for k, (f, c) in enumerate(ranges) if f <= i < f + c), None)
+        if k is None:
+            raise nat.CpbusError(nat.ENOENT, "lagging")
+        f, c = ranges[k]
+        cnt = min(n - done, f + c - i, first_sub + n - i)
+        out.append((k, i, cnt))
+        done += cnt
+    return out
+
+
+_SUMMARY_WORDS = ("active", "lagging", "backlog_total", "backlog_max", "lost_total")
+
+
+def _merge_lagging(pieces, cap: int, start_sub: int):
+    """pieces in visiting order, each (entries, next_sub, summary) of one shard's part scanned with at least the cap left
+    at that point: (entries, next_sub, summary) of the whole walk.  Entries are taken with the cap that is left; the first
+    piece that cannot return all of its lagging mailboxes sets next_sub; summaries add, backlog_max is the maximum."""
+    ents, got, nxt, cut = [], 0, start_sub, False
+    acc = {"active": 0, "lagging": 0, "backlog_total": 0, "backlog_max": 0, "lost_total": 0, "hist": [0] * 33}
+    for e, nx, s in pieces:
+        left = cap - got
+        ents.append(e[:left])
+        got += len(ents[-1])
+        if not cut and s["lagging"] > len(ents[-1]):
+            nxt, cut = (int(e["sub_id"][left]) if left < len(e) else nx), True
+        for k in ("active", "lagging", "backlog_total", "lost_total"):
+            acc[k] += s[k]
+        acc["backlog_max"] = max(acc["backlog_max"], s["backlog_max"])
+        acc["hist"] = [a + b for a, b in zip(acc["hist"], s["hist"])]
+    return (np.concatenate(ents) if ents else np.zeros(0, dtype=nat.LAG_DTYPE)), nxt, acc
+
+
 class _ShardOps:
     """What both drivers share: a shard is a `Bus` plus its end of the publisher's stream."""
 
@@ -148,9 +188,10 @@ class ShardedBus(_ShardOps):
         self.dist, self.rank, self.world = dist, rank, world
         self.lossless = lossless
         if subs_per_rank is not None:               # weak scaling: fixed shard size
-            self.first, self.count = rank * subs_per_rank, subs_per_rank
+            self._ranges = [(r * subs_per_rank, subs_per_rank) for r in range(world)]
         else:
-            self.first, self.count = shard_range(n_subs_total, world, rank)
+            self._ranges = [shard_range(n_subs_total, world, r) for r in range(world)]
+        self.first, self.count = self._ranges[rank]
         self.bus = bus_factory(max(self.count, 1), ring_cap=ring_cap, batch_cap=batch_cap, timers_per_sub=timers_per_sub, digest=digest,
                        device=device, sub_id_base=self.first, store_path=store_path, stream=stream, grid_ctas=grid_ctas,
                        lossless=lossless)
@@ -307,6 +348,59 @@ class ShardedBus(_ShardOps):
     def barrier(self):
         if self.world > 1:
             self.dist.barrier()
+
+    # -- consumer backlog over every shard (collective: every rank calls, every rank gets the same answer) --
+    def _all_gather_words(self, words: np.ndarray) -> list[np.ndarray]:
+        """every rank's uint64 vector: one all_gather of the lengths, one of the padded vectors"""
+        if self.world == 1:
+            return [words]
+        import torch
+        dev = "cuda" if self.dist.get_backend() == "nccl" else "cpu"
+        n = torch.tensor([words.size], dtype=torch.int64, device=dev)
+        ns = [torch.zeros_like(n) for _ in range(self.world)]
+        self.dist.all_gather(ns, n)
+        ns = [int(x) for x in ns]
+        buf = torch.zeros(max(1, max(ns)), dtype=torch.int64, device=dev)
+        buf[:words.size] = torch.from_numpy(np.ascontiguousarray(words, dtype=np.uint64).view(np.int64)).to(dev)
+        got = [torch.zeros_like(buf) for _ in range(self.world)]
+        self.dist.all_gather(got, buf)
+        return [g[:k].cpu().numpy().view(np.uint64) for g, k in zip(got, ns)]
+
+    def blockers(self, cap: int | None = None) -> np.ndarray:
+        """Lossless mode: the global ids of the mailboxes the stream's current round waits on, over every rank, ascending
+        (the first `cap`; default all).  Each rank asks its own shard (cpbus_stream_blockers); one exchange merges them.
+        Resolves this rank's outstanding rounds: call it between run_rounds / follow_rounds calls, on every rank."""
+        mine = self.bus.stream_blockers(self._st, cap).astype(np.uint64)
+        ids = np.sort(np.concatenate(self._all_gather_words(mine))).astype(np.uint32)
+        return ids if cap is None else ids[:cap]
+
+    def lagging(self, first_sub: int, n: int, start_sub: int | None = None, min_backlog: int = 1, cap: int | None = None):
+        """`Bus.lagging` over mailboxes [first_sub, first_sub+n) of every rank: the walk of cpbus_group_lagging over the
+        ranks' shards (entries in cyclic order from start_sub, the first `cap`; next_sub; summaries added, backlog_max the
+        maximum).  Each rank scans its own pieces; one exchange merges them.  Collective, like `blockers`."""
+        start_sub = first_sub if start_sub is None else start_sub
+        cap = n if cap is None else cap
+        walk = _walk(self._ranges, first_sub, n, start_sub)
+        words = []                                  # per own piece: j, entries, next_sub, summary, entries' words
+        for j, (k, a, cnt) in enumerate(walk):
+            if k != self.rank:
+                continue
+            e, nx, s = self.bus.lagging(a, cnt, start_sub=a, min_backlog=min_backlog, cap=cap)
+            words += [j, len(e), nx] + [s[f] for f in _SUMMARY_WORDS] + list(s["hist"])
+            words += [int(x) for r in e for x in (r["sub_id"], r["backlog"], r["lost"])]
+        pieces = {}
+        for w in self._all_gather_words(np.array(words, dtype=np.uint64)):
+            at = 0
+            while at < len(w):
+                j, m, nx = (int(x) for x in w[at:at + 3])
+                s = dict(zip(_SUMMARY_WORDS, (int(x) for x in w[at + 3:at + 8])))
+                s["hist"] = [int(x) for x in w[at + 8:at + 41]]
+                e = np.zeros(m, dtype=nat.LAG_DTYPE)
+                rows = w[at + 41:at + 41 + 3 * m].reshape(m, 3)
+                e["sub_id"], e["backlog"], e["lost"] = rows[:, 0], rows[:, 1], rows[:, 2]
+                pieces[j] = (e, nx, s)
+                at += 41 + 3 * m
+        return _merge_lagging([pieces[j] for j in range(len(walk))], cap, start_sub)
 
     # -- reductions (verification, statistics) -----------------------------
     def digest_fold_all(self):
@@ -474,6 +568,24 @@ class LocalShardedBus:
         """Device-side consumer on every shard: every mailbox read to the end, records discarded."""
         for _, _, bus in self.shards:
             bus.consume_all()
+
+    def blockers(self, cap: int | None = None) -> np.ndarray:
+        """Lossless mode: the global ids of the mailboxes the stream's current round waits on, over every shard, ascending
+        (the first `cap`; default all): each shard's cpbus_stream_blockers.  Resolves outstanding rounds: call it between
+        run_rounds / follow_rounds calls."""
+        ids = np.sort(np.concatenate([bus.stream_blockers(self._st[g], cap) for g, (_, _, bus) in enumerate(self.shards)]))
+        return ids if cap is None else ids[:cap]
+
+    def lagging(self, first_sub: int, n: int, start_sub: int | None = None, min_backlog: int = 1, cap: int | None = None):
+        """`Bus.lagging` over mailboxes [first_sub, first_sub+n) of every shard, as one bus with the same mailboxes answers
+        it: the walk of cpbus_group_lagging, each shard's piece scanned with the cap still left."""
+        start_sub = first_sub if start_sub is None else start_sub
+        cap = n if cap is None else cap
+        pieces, got = [], 0
+        for k, a, cnt in _walk([(f, c) for f, c, _ in self.shards], first_sub, n, start_sub):
+            pieces.append(self.shards[k][2].lagging(a, cnt, start_sub=a, min_backlog=min_backlog, cap=cap - got))
+            got += len(pieces[-1][0])
+        return _merge_lagging(pieces, cap, start_sub)
 
     def sync(self):
         for _, _, bus in self.shards:

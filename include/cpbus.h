@@ -462,6 +462,22 @@ int cpbus_lagging(cpbus_t* bus, uint32_t first_sub, uint32_t n, uint32_t start_s
  * below ring_cap).  Changes no state and flushes nothing; no kernel when the room bound proves that U fits, and none in
  * throughput mode (*n = 0).  CPBUS_EINVAL: NULL bus or n, or out == NULL with cap > 0. */
 int cpbus_blockers(cpbus_t* bus, uint32_t* out, size_t cap, size_t* n);
+/* Lossless stream shard: the subscribed mailboxes of this shard that give it an admissible prefix of 0 for its current
+ * batch, the one after the last it completed, at its stored offset.  (cpbus_blockers on a stream shard looks at the bus's
+ * own staged records and clock, not at the stream.)  The next unit U is the undelivered remainder's, by cpbus_stream_admit's
+ * rules with the batch's n and watermark from the slot header: with r >= 2 records left, the first of them with the ticks
+ * due by its ts_ns; with r = 1, that record with the ticks due by the watermark (admit holds a last record back when those
+ * ticks do not fit); with r = 0, the ticks due by the watermark.  A mailbox blocks when its share of U exceeds its room, as
+ * for cpbus_blockers.  out[0 .. min(cap, *n)) = the smallest blocking global ids, ascending; *n = how many there are.
+ * *n >= 1 exactly when cpbus_stream_admit(st, n_batch, watermark, &p) on this shard would return CPBUS_EAGAIN, or p = 0
+ * with records left (with nothing staged on the bus itself), and draining exactly these mailboxes makes that admit return p >= 1, or complete
+ * an empty remainder.  Outstanding followers and rounds are resolved first: after a stalled device round the answer is for
+ * the batch and offset the device cursor holds.  A batch the publisher has not released yet, or whose watermark admission
+ * refuses with CPBUS_EORDER, gives *n = 0.  Changes no state: no flush, admission, offer or room-bound change; reads the
+ * slot header (and U's record, 32 bytes) across the link; no kernel when the room bound proves that U fits, and none in
+ * throughput mode (*n = 0).  Returns the sticky stream error as cpbus_stream_status does.  CPBUS_EINVAL: NULL st or n, or
+ * out == NULL with cap > 0. */
+int cpbus_stream_blockers(cpbus_stream_t* st, uint32_t* out, size_t cap, size_t* n);
 /* Device-side consumer: every mailbox is read to the end and its records are discarded (head = tail), ordered behind
  * every earlier fan-out on the bus stream.  For subscribers nobody reads, and for measuring the lossless mode with
  * consumers that keep up. */
