@@ -18,7 +18,7 @@ N_CODES = 17
 MASK_ALL = 0x0001FFFF
 TARGET_ALL = 0xFFFFFFFF
 F_TICK, F_UNICAST = 0x1, 0x2
-CFG_LOSSLESS, CFG_DIGEST, CFG_SPARSE_TICKS = 0x1, 0x2, 0x4
+CFG_LOSSLESS, CFG_DIGEST, CFG_SPARSE_TICKS, CFG_SPARSE_RECORDS = 0x1, 0x2, 0x4, 0x8
 STORE_AUTO, STORE_V4, STORE_V8, STORE_BULK = 0, 1, 2, 3
 
 OK, EINVAL, ENOMEM, ECUDA, EAGAIN, ENOSPC, ENOENT, ECLOSED, ENODEV, EORDER, ETIMEDOUT = 0, -1, -2, -3, -4, -5, -6, -7, -8, -9, -10
@@ -74,6 +74,9 @@ assert LAG_DTYPE.itemsize == 16
 DUE_OP_DTYPE = np.dtype([("kind", "<u4"), ("slot", "<u4"), ("value", "<u8")])
 DUE_FIRE_DTYPE = np.dtype([("launch", "<u8"), ("slot", "<u4"), ("pad", "<u4"), ("ticks", "<u8"), ("next_due", "<u8")])
 assert DUE_OP_DTYPE.itemsize == 16 and DUE_FIRE_DTYPE.itemsize == 32
+# cpbus_plan_entry: one mailbox of cpbus_sparse_plan's plan
+PLAN_ENTRY_DTYPE = np.dtype([("local", "<u4"), ("due_bits", "<u4"), ("first", "<u4"), ("count", "<u4")])
+assert PLAN_ENTRY_DTYPE.itemsize == 16
 
 # every symbol include/cpbus.h declares: (restype, argtypes)
 _P = C.POINTER
@@ -146,6 +149,9 @@ SYMBOLS = {
     "cpbus_split_plan": (C.c_int, [C.c_void_p, C.c_size_t, C.c_uint32, C.c_uint64, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p, C.c_size_t, _P(C.c_size_t)]),
     "cpbus_mask_order": (C.c_size_t, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int, C.c_void_p]),
     "cpbus_due_trace": (C.c_int, [C.c_void_p, C.c_size_t, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t, _P(C.c_size_t)]),
+    "cpbus_sparse_plan": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p,
+                                    C.c_size_t, C.c_void_p, C.c_size_t, C.c_uint32, C.c_size_t, C.c_size_t, C.c_void_p,
+                                    C.c_size_t, C.c_void_p, C.c_size_t, _P(C.c_size_t), _P(C.c_size_t)]),
     "cpbus_record_hash": (C.c_uint64, [_P(Event)]),
     "cpbus_digest_multiplier": (C.c_uint64, []),
 }

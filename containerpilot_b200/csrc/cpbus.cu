@@ -172,6 +172,178 @@ void due_fire(DueIndex& x, std::vector<HostTimer>& tm, uint64_t w, F&& on_fire) 
   }
 }
 
+// The subscription index of a CPBUS_CFG_SPARSE_RECORDS bus: who takes a broadcast record, by code and by exact case.
+//  * Per code: the count of subscribed mailboxes whose mask has the code's bit, and their list while the count is at most
+//    `keep`.  A code past `keep` drops its list and keeps only the count: planning ends at once on such a code (it reaches
+//    more mailboxes than the plan may), so an all-ones fleet holds 17 counts, not 17 N entries.  The list comes back by a scan
+//    of the table when the plan next meets the code with few enough subscribers.  Entries are removed lazily: an entry is
+//    live while its subscriber is subscribed and has the bit; `listed` (one word per subscriber) says which lists hold an
+//    entry for it, so a bit that comes back revives the old entry instead of adding a second one, and a list is compacted
+//    when its stale entries outnumber the live ones by 64.  Bound per code: 2 * min(count, keep) + 64 entries.
+//  * Per exact case {code, source}: the subscribers with that case.  Cases are set at subscription and never change, so an
+//    entry is live while its subscriber is subscribed; every subscriber's cases are kept (8 bytes each, the device table
+//    keeps 8 too) so that an unsubscribe can find its lists, and a list is compacted when half of it is stale (+ 64).
+//    Bound: 8 bytes per case ever subscribed and 2 * live + 64 entries per case.
+// Maintenance is O(mask bits + cases) per subscriber and call, amortized.  `slot` (one word per subscriber, all UINT32_MAX
+// between plans) maps a mailbox to its plan entry while a plan is built.
+struct SubIndex {
+  size_t keep = 0;
+  uint32_t cnt[CPBUS_N_CODES] = {}, stale[CPBUS_N_CODES] = {};
+  bool ok[CPBUS_N_CODES] = {};                       // list[c] is kept
+  std::vector<uint32_t> list[CPBUS_N_CODES];
+  std::vector<uint32_t> listed;                      // per subscriber: bit c <=> list[c] holds an entry for it
+  struct Case { std::vector<uint32_t> subs; size_t stale = 0; };
+  std::unordered_map<uint64_t, Case> cases;          // (code << 32 | source) -> subscribers
+  std::vector<uint64_t> case_keys;                   // every subscriber's cases, in subscription order
+  std::vector<uint32_t> case_first;                  // per subscriber (allocated with the first case): its cases in case_keys
+  std::vector<uint8_t> case_n;
+  std::vector<uint32_t> slot;                        // per subscriber: its entry in the plan being built (UINT32_MAX: none)
+
+  static bool takes(const uint32_t* mask, const uint8_t* active, uint32_t l, uint32_t c) {
+    return active[l] && ((mask[l] >> c) & 1u);
+  }
+  void init(size_t n, size_t keep_n) {
+    keep = keep_n;
+    listed.assign(n, 0); slot.assign(n, UINT32_MAX);
+    for (uint32_t c = 0; c < CPBUS_N_CODES; c++) { cnt[c] = stale[c] = 0; ok[c] = true; list[c].clear(); }
+    cases.clear(); case_keys.clear(); case_first.clear(); case_n.clear();
+  }
+  void drop(uint32_t c) {
+    for (uint32_t l : list[c]) listed[l] &= ~(1u << c);
+    std::vector<uint32_t>().swap(list[c]);
+    ok[c] = false; stale[c] = 0;
+  }
+  void compact(uint32_t c, const uint32_t* mask, const uint8_t* active) {
+    size_t o = 0;
+    for (uint32_t l : list[c]) {
+      if (takes(mask, active, l, c)) list[c][o++] = l;
+      else listed[l] &= ~(1u << c);
+    }
+    list[c].resize(o); stale[c] = 0;
+  }
+  void rebuild(uint32_t c, const uint32_t* mask, const uint8_t* active, uint32_t n) {
+    list[c].clear();
+    for (uint32_t l = 0; l < n; l++)
+      if (takes(mask, active, l, c)) { list[c].push_back(l); listed[l] |= 1u << c; }
+    ok[c] = true; stale[c] = 0;
+  }
+  // subscriber l has gained the codes in `bits` (it is subscribed and its mask has them)
+  void add_codes(uint32_t l, uint32_t bits) {
+    for (uint32_t c = 0; c < CPBUS_N_CODES; c++) {
+      if (!((bits >> c) & 1u)) continue;
+      cnt[c]++;
+      if (!ok[c]) continue;
+      if (cnt[c] > keep) { drop(c); continue; }
+      if ((listed[l] >> c) & 1u) stale[c]--;   // its old entry is live again
+      else { list[c].push_back(l); listed[l] |= 1u << c; }
+    }
+  }
+  // subscriber l has lost the codes in `bits` (mask / active already say so)
+  void remove_codes(uint32_t l, uint32_t bits, const uint32_t* mask, const uint8_t* active) {
+    for (uint32_t c = 0; c < CPBUS_N_CODES; c++) {
+      if (!((bits >> c) & 1u)) continue;
+      cnt[c]--;
+      if (!ok[c] || !((listed[l] >> c) & 1u)) continue;
+      if (++stale[c] > cnt[c] + 64) compact(c, mask, active);
+    }
+  }
+  // subscriber l (just subscribed) has the exact cases keys[0..n)
+  void add_cases(uint32_t l, const uint64_t* keys, uint32_t n) {
+    if (!n) return;
+    if (case_first.empty()) { case_first.assign(listed.size(), 0); case_n.assign(listed.size(), 0); }
+    case_first[l] = (uint32_t)case_keys.size(); case_n[l] = (uint8_t)n;
+    for (uint32_t j = 0; j < n; j++) {
+      case_keys.push_back(keys[j]);
+      Case& k = cases[keys[j]];
+      if (k.subs.empty() || k.subs.back() != l) k.subs.push_back(l);   // (a case listed twice: one entry)
+    }
+  }
+  // subscriber l has been unsubscribed
+  void remove_cases(uint32_t l, const uint8_t* active) {
+    if (case_n.empty() || !case_n[l]) return;
+    const uint64_t* keys = case_keys.data() + case_first[l];
+    for (uint32_t j = 0; j < case_n[l]; j++) {
+      if (std::find(keys, keys + j, keys[j]) != keys + j) continue;
+      auto it = cases.find(keys[j]);
+      Case& k = it->second;
+      if (++k.stale * 2 <= k.subs.size() + 64) continue;
+      size_t o = 0;
+      for (uint32_t s : k.subs) if (active[s]) k.subs[o++] = s;
+      k.subs.resize(o); k.stale = 0;
+      if (!o) cases.erase(it);
+    }
+    case_n[l] = 0;
+  }
+};
+
+// The plan of a sparse record flush (cpbus_sparse_plan is this function over an index built from its arguments).  For each
+// record: a unicast record goes to its target if subscribed; a broadcast record to the live entries of its code's list and to
+// the subscribers with its exact case whose mask lacks the code (the fan-out's rule: mask bit or case).  A code with more
+// than max_m subscribers ends the planning at once, so a dense fleet costs O(records).  Each mailbox gets a plan entry the
+// first time it turns up (x.slot maps it there), so the planning also ends as soon as a (max_m + 1)-th one does; the
+// {mailbox, record} pairs are appended in record order.  The entries (at most max_m) are then sorted and the record indices
+// scattered to them in that order: O(records planned + max_m log max_m), each entry's indices ascending.  False: the flush
+// takes the full fan-out (more than max_m due slots or candidates, or more than max_d records planned).
+bool sparse_plan(SubIndex& x, const uint32_t* mask, const uint8_t* active, uint32_t n_subs, uint32_t base,
+                 const cpbus_event* rec, size_t n, const std::vector<uint32_t>& due, uint32_t K, size_t max_m, size_t max_d,
+                 std::vector<uint64_t>& pairs, std::vector<cpbus_plan_entry>& out, std::vector<uint32_t>& idx) {
+  out.clear(); idx.clear(); pairs.clear();
+  struct Reset {   // x.slot goes back to all UINT32_MAX whichever way the planning ends
+    SubIndex& x; std::vector<cpbus_plan_entry>& out;
+    ~Reset() { for (const cpbus_plan_entry& e : out) x.slot[e.local] = UINT32_MAX; }
+  } reset{x, out};
+  auto entry = [&](uint32_t l) -> cpbus_plan_entry* {   // nullptr: one mailbox too many
+    uint32_t& s = x.slot[l];
+    if (s == UINT32_MAX) {
+      if (out.size() == max_m) return nullptr;
+      s = (uint32_t)out.size();
+      out.push_back(cpbus_plan_entry{l, 0u, 0u, 0u});
+    }
+    return &out[s];
+  };
+  if (due.size() > max_m) return false;
+  for (uint32_t d : due) entry(d / K)->due_bits |= 1u << (d % K);
+  auto take = [&](uint32_t l, size_t i) -> bool {
+    cpbus_plan_entry* e = entry(l);
+    if (!e) return false;
+    e->count++;
+    pairs.push_back((uint64_t)l << 32 | i);
+    return true;
+  };
+  for (size_t i = 0; i < n; i++) {
+    const cpbus_event& r = rec[i];
+    if (r.target != CPBUS_TARGET_ALL) {
+      const uint32_t l = r.target - base;
+      if (r.target >= base && l < n_subs && active[l] && !take(l, i)) return false;
+    } else if (r.code < CPBUS_N_CODES) {
+      const uint32_t c = r.code;
+      if (x.cnt[c] > max_m) return false;
+      if (!x.ok[c]) x.rebuild(c, mask, active, n_subs);
+      for (uint32_t l : x.list[c])
+        if (SubIndex::takes(mask, active, l, c) && !take(l, i)) return false;
+      if (!x.cases.empty()) {
+        auto it = x.cases.find((uint64_t)c << 32 | r.source_id);
+        if (it != x.cases.end())
+          for (uint32_t l : it->second.subs)
+            if (active[l] && !((mask[l] >> c) & 1u) && !take(l, i)) return false;
+      }
+    }
+    if (pairs.size() > max_d) return false;
+  }
+  std::sort(out.begin(), out.end(), [](const cpbus_plan_entry& a, const cpbus_plan_entry& b) { return a.local < b.local; });
+  uint32_t first = 0;
+  for (uint32_t s = 0; s < out.size(); s++) {
+    x.slot[out[s].local] = s;
+    out[s].first = first; first += out[s].count; out[s].count = 0;
+  }
+  idx.resize(pairs.size());
+  for (uint64_t p : pairs) {
+    cpbus_plan_entry& e = out[x.slot[(uint32_t)(p >> 32)]];
+    idx[e.first + e.count++] = (uint32_t)p;
+  }
+  return true;
+}
+
 // The host front end: what the single bus (cpbus) and the group (cpbus_group) keep over their whole id space, and what the
 // rules below share — the clock window (max_window), timer arming and retirement, staging (stage_one), the publish loop
 // (publish_burst), the clock's advance (advance_clock), the debug ring and the publish counts.
@@ -313,6 +485,18 @@ struct cpbus : HostFront {
   uint2* h_tick_list = nullptr; uint2* d_tick_list = nullptr; size_t tick_list_cap = 0;
   cudaEvent_t tick_list_done = nullptr;   // on copy_stream: the list has reached HBM (and left the pinned buffer)
   cudaEvent_t tick_done = nullptr;        // on the bus stream: the tick kernel is done with the list
+
+  // CPBUS_CFG_SPARSE_RECORDS: the subscription index, the plan of the flush (entries, record indices, and the {mailbox,
+  // record} pairs it is sorted from), staged in pinned memory as [entries | indices] and copied on the copy stream into a
+  // device buffer that grows on demand
+  bool sparse_records = false;
+  SubIndex rec_index;
+  std::vector<cpbus_plan_entry> plan;
+  std::vector<uint32_t> plan_idx;
+  std::vector<uint64_t> plan_pairs;
+  unsigned char* h_plan = nullptr; unsigned char* d_plan = nullptr; size_t plan_bytes_cap = 0;
+  cudaEvent_t plan_done = nullptr;        // on copy_stream: the plan (and the batch in front of it) has reached HBM
+  cudaEvent_t records_done = nullptr;     // on the bus stream: the record kernel is done with the plan
 
   // intern table (Event.Source string <-> u32)
   std::unordered_map<std::string, uint32_t> intern;
@@ -771,6 +955,111 @@ bool sparse_flush(cpbus* b, uint64_t w, int* rc) {
   return true;
 }
 
+// CPBUS_CFG_SPARSE_RECORDS: candidate mailboxes (the tick path's threshold) and planned record deliveries beyond which a flush
+// with staged records takes the full fan-out.  Measured on an H100 (DESIGN.md §4.7).
+size_t records_max_mailboxes(const cpbus* b) { return sparse_max(b); }
+size_t records_max_deliveries(const cpbus* b) { return std::max<size_t>(1024, b->n_next / 256); }
+
+// The pinned plan buffer is free for `bytes`: the previous plan has left it, or both buffers are regrown (behind every
+// kernel that may still read the old device buffer).
+int plan_room(cpbus* b, size_t bytes) {
+  if (bytes <= b->plan_bytes_cap) { CK(cudaEventSynchronize(b->plan_done)); return CPBUS_OK; }
+  CK(cudaStreamSynchronize(b->stream)); CK(cudaStreamSynchronize(b->copy_stream));
+  cudaFree(b->d_plan); cudaFreeHost(b->h_plan);
+  b->d_plan = nullptr; b->h_plan = nullptr; b->plan_bytes_cap = 0;
+  const size_t cap = std::max<size_t>(bytes, 64 << 10);
+  CK(cudaMalloc((void**)&b->d_plan, cap));
+  CK(cudaMallocHost((void**)&b->h_plan, cap));
+  b->plan_bytes_cap = cap;
+  return CPBUS_OK;
+}
+
+// The record kernel over b->plan, to watermark w, for the staged batch.  The batch takes the next device staging slot as
+// in flush_staged (epoch events, 30 us landing spin); the plan follows it on the copy stream once the previous record kernel
+// is done with the device buffer.  The kernel runs on the bus stream behind every earlier launch, without programmatic
+// dependent launch.  A plan without a mailbox launches nothing and copies nothing.  Then the staging buffer moves on and
+// the clock and the due index follow the launch, as after a fan-out.
+int launch_records(cpbus* b, uint64_t w) {
+  const size_t n_list = b->plan.size(), n_idx = b->plan_idx.size();
+  const uint32_t n = (uint32_t)b->n_staged;
+  const int c = b->cur;
+  if (n_list) {
+    const size_t list_bytes = n_list * sizeof(cpbus_plan_entry), bytes = list_bytes + n_idx * sizeof(uint32_t);
+    int rc = plan_room(b, bytes); if (rc) return rc;
+    memcpy(b->h_plan, b->plan.data(), list_bytes);
+    memcpy(b->h_plan + list_bytes, b->plan_idx.data(), n_idx * sizeof(uint32_t));
+    const uint32_t slot = b->dev_slot;
+    cpbus_event* d_dst = b->d_stage + (size_t)slot * b->B;
+    if (slot % cpbus::kDevEpoch == 0) CK(cudaEventSynchronize(b->epoch_done[slot / cpbus::kDevEpoch]));
+    CK(cudaMemcpyAsync(d_dst, b->h_batch[c], (size_t)n * sizeof(cpbus_event), cudaMemcpyHostToDevice, b->copy_stream));
+    CK(cudaEventRecord(b->h2d_done[c], b->copy_stream));
+    CK(cudaStreamWaitEvent(b->copy_stream, b->records_done, 0));
+    CK(cudaMemcpyAsync(b->d_plan, b->h_plan, bytes, cudaMemcpyHostToDevice, b->copy_stream));
+    CK(cudaEventRecord(b->plan_done, b->copy_stream));
+    bool landed = false;
+    const auto t_spin = std::chrono::steady_clock::now();
+    do {
+      const cudaError_t q = cudaEventQuery(b->plan_done);
+      if (q == cudaSuccess) { landed = true; break; }
+      if (q != cudaErrorNotReady) { CK(q); }
+    } while (std::chrono::steady_clock::now() - t_spin < std::chrono::microseconds(30));
+    if (!landed) CK(cudaStreamWaitEvent(b->stream, b->plan_done, 0));
+    RecordScatterParams p{};
+    p.list = reinterpret_cast<const uint4*>(b->d_plan); p.n_list = (uint32_t)n_list;
+    p.idx = reinterpret_cast<const uint32_t*>(b->d_plan + list_bytes); p.batch = d_dst;
+    p.ring = b->d_ring; p.ctl = b->d_ctl; p.timers = b->d_timers; p.stats = b->d_stats; p.pow_table = b->d_pow;
+    p.launch_seq = ++b->launch_seq;
+    p.result = b->d_result + (size_t)(p.launch_seq % kResultRing) * kResultSub;
+    p.result_next = b->d_result + (size_t)((p.launch_seq + 1) % kResultRing) * kResultSub;
+    p.w_now = w; p.ring_cap = b->R; p.K = b->K; p.sub_base = b->cfg.sub_id_base; p.use_digest = b->use_digest ? 1u : 0u;
+    record_scatter_kernel<<<(uint32_t)((n_list + kWarpsPerCta - 1) / kWarpsPerCta), kThreads, 0, b->stream>>>(p);
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(b->records_done, b->stream));
+    b->st.kernel_launches++;
+    if (slot % cpbus::kDevEpoch == cpbus::kDevEpoch - 1) CK(cudaEventRecord(b->epoch_done[slot / cpbus::kDevEpoch], b->stream));
+    b->dev_slot = (slot + 1) % cpbus::kDevSlots;
+    b->cur = (b->cur + 1) % cpbus::kStage;
+  }
+  b->n_staged = 0;
+  if (b->n_next) {   // (the fan-out of a bus without subscribers launches nothing and leaves the watermark where it was)
+    b->last_watermark = w;
+    due_fire(b->due, b->h_timers, w, [](uint32_t, uint64_t, uint64_t) {});
+  }
+  if (n_list) CK(cudaEventSynchronize(b->h2d_done[b->cur]));   // the pinned buffer we are about to overwrite has left the host
+  return CPBUS_OK;
+}
+
+// CPBUS_CFG_SPARSE_RECORDS, records staged: true when the flush is done without the full fan-out (*rc = its status): the
+// staged records and the ticks due by w reach at most records_max_mailboxes mailboxes with at most records_max_deliveries
+// records, and (lossless) the room bound covers the most that one of them takes, records and ticks.  False: the full
+// fan-out follows, with admission and the partial prefix as before.
+bool record_flush(cpbus* b, uint64_t w, int* rc) {
+  *rc = CPBUS_OK;
+  const size_t max_m = records_max_mailboxes(b);
+  std::vector<uint32_t>& due = b->due_slots;
+  due.clear();
+  if (b->due.min_due() <= w && !b->due.collect(w, max_m, &due)) return false;
+  if (!sparse_plan(b->rec_index, b->h_mask.data(), b->h_active.data(), b->n_next, b->cfg.sub_id_base, b->h_batch[b->cur],
+                   b->n_staged, due, b->K, max_m, records_max_deliveries(b), b->plan_pairs, b->plan, b->plan_idx))
+    return false;
+  if (b->lossless) {
+    uint64_t most = 0;   // the most one mailbox takes
+    for (const cpbus_plan_entry& e : b->plan) {
+      uint64_t take = e.count;
+      for (uint32_t k = 0; k < b->K; k++) {
+        if (!((e.due_bits >> k) & 1u)) continue;
+        const HostTimer& t = b->h_timers[(size_t)e.local * b->K + k];
+        take += t.oneshot ? 1 : due_ticks(t.next_due, t.period, w);
+      }
+      most = std::max(most, take);
+    }
+    if (b->room_lb < most) return false;
+    b->room_lb -= most; b->st.admit_skipped++;
+  }
+  *rc = launch_records(b, w);
+  return true;
+}
+
 // lossless admission (reference: the sender blocks on a full channel, events/subscriber.go:30-32)
 // Fast path: true when n records with watermark w provably fit (or nothing has to be admitted) — no kernel, no sync.
 bool admit_fits(cpbus* b, uint32_t n, uint64_t w) {
@@ -852,6 +1141,7 @@ int flush_staged(cpbus* b, uint64_t w) {
   if (flush_idle(b, w)) return CPBUS_OK;
   int rc;
   if (b->sparse && !b->n_staged && sparse_flush(b, w, &rc)) return rc;
+  if (b->sparse_records && b->n_staged && record_flush(b, w, &rc)) return rc;
   const uint32_t n = (uint32_t)b->n_staged;
   const int c = b->cur;
   // Device staging is a long ring (kDevSlots batches): a slot is reused only kDevSlots flushes later, far beyond how far the
@@ -1132,6 +1422,47 @@ int cpbus_due_trace(const cpbus_due_op* ops, size_t n_ops, uint32_t n_slots, uin
   *n_out = n;
   return CPBUS_OK;
 } CPBUS_CATCH
+// The plan of a sparse-records flush over an index built from the arguments, with the bus's own planning code (keep =
+// max_mailboxes: a code with more subscribers keeps only its count, as on a bus).
+int cpbus_sparse_plan(const uint32_t* masks, const uint8_t* active, uint32_t n_subs, const cpbus_pair* pairs,
+                      const uint32_t* n_pairs, uint32_t sub_id_base, const cpbus_event* records, size_t n_records,
+                      const uint32_t* due_slots, size_t n_due, uint32_t K, size_t max_mailboxes, size_t max_deliveries,
+                      cpbus_plan_entry* out, size_t cap, uint32_t* rec_idx, size_t idx_cap, size_t* n_out, size_t* n_idx) try {
+  if ((!masks && n_subs) || (!records && n_records) || (!due_slots && n_due) || (pairs && !n_pairs) || !n_out || !n_idx ||
+      (cap && !out) || (idx_cap && !rec_idx) || !(K == 0 || K == 1 || K == 2 || K == 4 || K == 8) || (!K && n_due))
+    return CPBUS_EINVAL;
+  for (size_t d = 0; d < n_due; d++) if (due_slots[d] / K >= n_subs) return CPBUS_EINVAL;
+  if (pairs) for (uint32_t l = 0; l < n_subs; l++) if (n_pairs[l] > CPBUS_MAX_PAIRS) return CPBUS_EINVAL;
+  std::vector<uint32_t> mask(n_subs);
+  std::vector<uint8_t> act(n_subs, 1);
+  for (uint32_t l = 0; l < n_subs; l++) { mask[l] = masks[l] & CPBUS_MASK_ALL; if (active) act[l] = active[l] ? 1 : 0; }
+  SubIndex x;
+  x.init(n_subs, max_mailboxes);
+  for (uint32_t l = 0; l < n_subs; l++) {
+    if (!act[l]) continue;
+    x.add_codes(l, mask[l]);
+    if (!pairs) continue;
+    uint64_t keys[CPBUS_MAX_PAIRS];
+    for (uint32_t j = 0; j < n_pairs[l]; j++) {
+      const cpbus_pair& pr = pairs[(size_t)l * CPBUS_MAX_PAIRS + j];
+      keys[j] = (uint64_t)pr.code << 32 | pr.source_id;
+    }
+    x.add_cases(l, keys, n_pairs[l]);
+  }
+  std::vector<uint32_t> due(due_slots, due_slots + n_due);
+  std::sort(due.begin(), due.end());
+  due.erase(std::unique(due.begin(), due.end()), due.end());
+  std::vector<uint64_t> scratch;
+  std::vector<cpbus_plan_entry> plan;
+  std::vector<uint32_t> idx;
+  if (!sparse_plan(x, mask.data(), act.data(), n_subs, sub_id_base, records, n_records, due, K, max_mailboxes, max_deliveries,
+                   scratch, plan, idx))
+    return CPBUS_ENOSPC;
+  std::copy(plan.begin(), plan.begin() + std::min(cap, plan.size()), out);
+  std::copy(idx.begin(), idx.begin() + std::min(idx_cap, idx.size()), rec_idx);
+  *n_out = plan.size(); *n_idx = idx.size();
+  return CPBUS_OK;
+} CPBUS_CATCH
 
 const char* cpbus_last_cuda_error(void) { return g_cuda_err; }
 
@@ -1199,6 +1530,7 @@ int cpbus_create(const cpbus_config* cfg, cpbus_t** out) try {
   *out = nullptr;
   uint32_t R = 0, B = 0;
   if (config_check(cfg, &R, &B)) return CPBUS_EINVAL;
+  if ((cfg->flags & CPBUS_CFG_SPARSE_RECORDS) && !(cfg->flags & CPBUS_CFG_SPARSE_TICKS)) return CPBUS_EINVAL;   // the due index finds the ticks
   const uint32_t K = cfg->timers_per_sub;
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
@@ -1211,6 +1543,7 @@ int cpbus_create(const cpbus_config* cfg, cpbus_t** out) try {
   b->N = cfg->n_max_subs; b->R = R; b->B = B; b->K = K;
   b->lossless = cfg->flags & CPBUS_CFG_LOSSLESS; b->use_digest = cfg->flags & CPBUS_CFG_DIGEST;
   b->sparse = cfg->flags & CPBUS_CFG_SPARSE_TICKS;
+  b->sparse_records = cfg->flags & CPBUS_CFG_SPARSE_RECORDS;
   b->room_lb = R;
   b->store = cfg->store_path == CPBUS_STORE_AUTO ? CPBUS_STORE_V8 : (int)cfg->store_path;
   if (const char* e = getenv("CPBUS_PDL")) b->pdl = atoi(e) != 0;
@@ -1250,6 +1583,9 @@ int cpbus_create(const cpbus_config* cfg, cpbus_t** out) try {
   if (cudaEventCreateWithFlags(&b->launched, cudaEventDisableTiming) != cudaSuccess) return fail(CPBUS_ECUDA);
   if (b->sparse && (cudaEventCreateWithFlags(&b->tick_list_done, cudaEventDisableTiming) != cudaSuccess ||
                     cudaEventCreateWithFlags(&b->tick_done, cudaEventDisableTiming) != cudaSuccess))
+    return fail(CPBUS_ECUDA);
+  if (b->sparse_records && (cudaEventCreateWithFlags(&b->plan_done, cudaEventDisableTiming) != cudaSuccess ||
+                            cudaEventCreateWithFlags(&b->records_done, cudaEventDisableTiming) != cudaSuccess))
     return fail(CPBUS_ECUDA);
   ALLOC(b->d_stage, (size_t)cpbus::kDevSlots * B * sizeof(cpbus_event));
   for (int i = 0; i < cpbus::kDevSlots / cpbus::kDevEpoch; i++)
@@ -1312,6 +1648,7 @@ int cpbus_create(const cpbus_config* cfg, cpbus_t** out) try {
   }
   b->h_mask.assign(N, 0);
   b->h_active.assign(N, 0);
+  if (b->sparse_records) b->rec_index.init(N, 2 * std::max<size_t>(32, N / 1024));   // lists of up to twice the largest cap
   b->intern.emplace(std::string(), 0u);   // "" -> 0 so that NonEvent == {None, 0} (events/events.go:45)
   b->sources.emplace_back();
   *out = b;
@@ -1345,6 +1682,10 @@ int cpbus_destroy(cpbus_t* b) try {
   if (b->tick_done) cudaEventDestroy(b->tick_done);
   cudaFree(b->d_tick_list);
   if (b->h_tick_list) cudaFreeHost(b->h_tick_list);
+  if (b->plan_done) cudaEventDestroy(b->plan_done);
+  if (b->records_done) cudaEventDestroy(b->records_done);
+  cudaFree(b->d_plan);
+  if (b->h_plan) cudaFreeHost(b->h_plan);
   cudaFree(b->d_drain);cudaFree(b->d_drain_idx);
   cudaFree(b->d_ready_lb); cudaFree(b->d_ready); cudaFree(b->d_ready_slot);
   if (b->h_ready_hdr) cudaFreeHost(b->h_ready_hdr);
@@ -1437,6 +1778,7 @@ int cpbus_subscribe_many(cpbus_t* b, const uint32_t* masks, uint32_t n, uint32_t
     blocks[i].mask = b->h_mask[first + i] | kActiveBit;
     b->h_active[first + i] = 1;
     if (b->h_mask[first + i] != CPBUS_MASK_ALL) b->n_filtered++;
+    if (b->sparse_records) b->rec_index.add_codes(first + i, b->h_mask[first + i]);
   }
   CK(cudaMemcpyAsync(b->d_ctl + first, blocks.data(), (size_t)n * sizeof(SubCtl), cudaMemcpyHostToDevice, b->stream));
   CK(cudaStreamSynchronize(b->stream));
@@ -1474,6 +1816,11 @@ int cpbus_subscribe_pairs(cpbus_t* b, uint32_t mask, const cpbus_pair* pairs, ui
   CK(cudaMemcpyAsync(b->d_pairs + (size_t)l * CPBUS_MAX_PAIRS, row, sizeof(row), cudaMemcpyHostToDevice, b->stream));
   CK(cudaStreamSynchronize(b->stream));   // `row` is on the stack
   b->h_npairs[l] = (uint8_t)used; b->n_paired++;
+  if (b->sparse_records) {
+    uint64_t keys[CPBUS_MAX_PAIRS];
+    for (uint32_t j = 0; j < used; j++) keys[j] = (uint64_t)row[j].x << 32 | row[j].y;
+    b->rec_index.add_cases(l, keys, used);
+  }
   if ((rc = push_mask_words(b, l, 1))) return rc;
   if (sub_id) *sub_id = id;
   return CPBUS_OK;
@@ -1510,6 +1857,14 @@ int cpbus_subscribe_pairs_many(cpbus_t* b, const uint32_t* masks, const cpbus_pa
     }
     b->h_npairs[l0 + i] = (uint8_t)used;
     if (used) paired++;
+    if (b->sparse_records && used) {
+      uint64_t keys[CPBUS_MAX_PAIRS];
+      for (uint32_t j = 0; j < used; j++) {
+        const uint2 r = rows[(size_t)i * CPBUS_MAX_PAIRS + j];
+        keys[j] = (uint64_t)r.x << 32 | r.y;
+      }
+      b->rec_index.add_cases(l0 + i, keys, used);
+    }
   }
   CK(cudaMemcpyAsync(b->d_pairs + (size_t)l0 * CPBUS_MAX_PAIRS, rows.data(), rows.size() * sizeof(uint2), cudaMemcpyHostToDevice, b->stream));
   CK(cudaStreamSynchronize(b->stream));
@@ -1530,6 +1885,10 @@ int cpbus_unsubscribe(cpbus_t* b, uint32_t sub_id) try {
   b->h_active[l] = 0;
   if (b->h_mask[l] != CPBUS_MASK_ALL) b->n_filtered--;
   if (!b->h_npairs.empty() && b->h_npairs[l]) { b->h_npairs[l] = 0; b->n_paired--; }
+  if (b->sparse_records) {
+    b->rec_index.remove_codes(l, b->h_mask[l], b->h_mask.data(), b->h_active.data());
+    b->rec_index.remove_cases(l, b->h_active.data());
+  }
   b->order_dirty = true;
   const uint32_t word = 0;
   CK(cudaMemcpyAsync(&b->d_ctl[l].mask, &word, 4, cudaMemcpyHostToDevice, b->stream));
@@ -1558,7 +1917,12 @@ int cpbus_set_mask(cpbus_t* b, uint32_t sub_id, uint32_t mask) try {
   mask &= CPBUS_MASK_ALL;
   if (b->h_mask[l] != CPBUS_MASK_ALL) b->n_filtered--;
   if (mask != CPBUS_MASK_ALL) b->n_filtered++;
+  const uint32_t old = b->h_mask[l];
   b->h_mask[l] = mask; b->order_dirty = true;
+  if (b->sparse_records) {
+    b->rec_index.add_codes(l, mask & ~old);
+    b->rec_index.remove_codes(l, old & ~mask, b->h_mask.data(), b->h_active.data());
+  }
   return push_mask_words(b, l, 1);
 } CPBUS_CATCH
 
@@ -2865,6 +3229,7 @@ int cpbus_group_create(const cpbus_config* cfg, const int32_t* devices, uint32_t
   if (!cfg || !devices || !n_devices || !out || cfg->stream || n_devices > kStreamMaxConsumers) return CPBUS_EINVAL;
   *out = nullptr;
   if (cfg->flags & CPBUS_CFG_SPARSE_TICKS) return CPBUS_EINVAL;   // the group's flush is a stream batch (see cpbus_stream_create)
+  if (cfg->flags & CPBUS_CFG_SPARSE_RECORDS) return CPBUS_EINVAL;
   uint32_t R = 0, B = 0;
   if (config_check(cfg, &R, &B) || cfg->n_max_subs < n_devices) return CPBUS_EINVAL;
   cpbus_group* g = new (std::nothrow) cpbus_group();

@@ -98,6 +98,23 @@ enum {
                                    admit_passes and admit_skipped.  Not supported on a
                                    group (cpbus_group_create) or with streams
                                    (cpbus_stream_create/_open/_attach): CPBUS_EINVAL. */
+#define CPBUS_CFG_SPARSE_RECORDS 0x8u /* a flush with staged records that reach few
+                                   mailboxes costs what it delivers: the host keeps an index
+                                   of the subscribers by code (a count per code, and the list
+                                   while it is short) and by exact {code, source} case, and
+                                   such a flush launches one small kernel over exactly the
+                                   mailboxes that take a record or own a due tick (the full
+                                   fan-out past max(32, subscribers/1024) such mailboxes or
+                                   past max(1024, subscribers/256) records planned, and in
+                                   lossless mode when the room bound cannot prove that one
+                                   mailbox's records and ticks fit).  Requires
+                                   CPBUS_CFG_SPARSE_TICKS (CPBUS_EINVAL otherwise).  Results
+                                   are those of a bus without the flag making the same calls,
+                                   except cpbus_stats.batches, kernel_launches, admit_passes
+                                   and admit_skipped; a flush that launched nothing (no
+                                   mailbox takes anything) leaves the step result as it was.
+                                   Device batches (cpbus_publish_device*) always take the
+                                   full fan-out.  Not supported on a group: CPBUS_EINVAL. */
 
 /* cpbus_config.store_path: how records reach the rings (all are bit-identical) */
 enum {
@@ -499,7 +516,7 @@ int cpbus_digest_fold_end(cpbus_t* bus, uint32_t ticket, uint64_t out[4]);
  * fold32(x) = low32(x ^ (x >> 32)), launch ordinal}.
  * _begin enqueues a 256-byte D2H on the bus stream (up to 8 outstanding tickets), _end waits for it.
  * On a CPBUS_CFG_SPARSE_TICKS bus the tick kernel of a flush with no staged record is such a launch too, and a flush that
- * launched nothing leaves the result as it was. */
+ * launched nothing leaves the result as it was.  So is the record kernel of a CPBUS_CFG_SPARSE_RECORDS flush. */
 int cpbus_step_result_begin(cpbus_t* bus, uint32_t* ticket);
 int cpbus_step_result_end(cpbus_t* bus, uint32_t ticket, uint64_t out[4]);
 
@@ -621,6 +638,25 @@ typedef struct cpbus_due_op { uint32_t kind, slot; uint64_t value; } cpbus_due_o
 typedef struct cpbus_due_fire { uint64_t launch; uint32_t slot, pad; uint64_t ticks, next_due; } cpbus_due_fire; /* sizeof == 32 */
 int cpbus_due_trace(const cpbus_due_op* ops, size_t n_ops, uint32_t n_slots, uint32_t K, cpbus_due_fire* out, size_t cap,
                     size_t* n_out);
+/* The plan of a CPBUS_CFG_SPARSE_RECORDS flush, as a pure host function (no device needed; the bus runs the same code over
+ * its own index).  Subscriber l < n_subs is subscribed when active[l] != 0 (active == NULL: all), with code mask masks[l]
+ * and, when pairs != NULL, the exact cases pairs[l * CPBUS_MAX_PAIRS + j] for j < n_pairs[l] (taken as stored: a case
+ * matches whatever the mask holds).  It takes record i of records[0..n_records) when the record is broadcast (target ==
+ * CPBUS_TARGET_ALL) and its code's bit is in the mask or {code, source_id} is one of its cases, or when the record is
+ * unicast to its id sub_id_base + l.  due_slots[0..n_due) are timer slots (subscriber * K + k, K in {0, 1, 2, 4, 8}) due
+ * in this flush.  The candidates are the subscribed mailboxes that take a record and the mailboxes of the due slots.
+ * Each candidate, in ascending order, gets one entry {local index, bitmask of its due slots (bit k), first, count}: its
+ * records are rec_idx[first .. first + count), ascending (batch order).  *n_out = candidates, *n_idx = records planned;
+ * the first cap entries and the first idx_cap indices are written.
+ * CPBUS_ENOSPC when the flush takes the full fan-out instead: more than max_mailboxes due slots or candidates (a broadcast
+ * code with more than max_mailboxes subscribers ends the planning at once), or more than max_deliveries planned records.
+ * CPBUS_EINVAL: a NULL array with a non-zero count, a due slot of a subscriber >= n_subs, n_pairs[l] > CPBUS_MAX_PAIRS,
+ * or K not in {0, 1, 2, 4, 8}. */
+typedef struct cpbus_plan_entry { uint32_t local, due_bits, first, count; } cpbus_plan_entry;   /* sizeof == 16 */
+int cpbus_sparse_plan(const uint32_t* masks, const uint8_t* active, uint32_t n_subs, const cpbus_pair* pairs,
+                      const uint32_t* n_pairs, uint32_t sub_id_base, const cpbus_event* records, size_t n_records,
+                      const uint32_t* due_slots, size_t n_due, uint32_t K, size_t max_mailboxes, size_t max_deliveries,
+                      cpbus_plan_entry* out, size_t cap, uint32_t* rec_idx, size_t idx_cap, size_t* n_out, size_t* n_idx);
 
 #ifdef __cplusplus
 }
