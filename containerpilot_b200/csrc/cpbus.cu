@@ -185,7 +185,8 @@ void due_fire(DueIndex& x, std::vector<HostTimer>& tm, uint64_t w, F&& on_fire) 
 //    keeps 8 too) so that an unsubscribe can find its lists, and a list is compacted when half of it is stale (+ 64).
 //    Bound: 8 bytes per case ever subscribed and 2 * live + 64 entries per case.
 // Maintenance is O(mask bits + cases) per subscriber and call, amortized.  `slot` (one word per subscriber, all UINT32_MAX
-// between plans) maps a mailbox to its plan entry while a plan is built.
+// between plans) maps a mailbox to its plan entry while a plan is built.  A CPBUS_CFG_SPARSE_TICKS bus without the records
+// flag plans due ticks alone: it sizes `slot` and nothing else.
 struct SubIndex {
   size_t keep = 0;
   uint32_t cnt[CPBUS_N_CODES] = {}, stale[CPBUS_N_CODES] = {};
@@ -477,19 +478,13 @@ struct cpbus : HostFront {
   // the admission kernel does run, and reset by cpbus_consume_all.
   uint64_t room_lb = 0;
 
-  // CPBUS_CFG_SPARSE_TICKS: the armed slots by due time, and the tick kernel's list of due mailboxes ({local index, due-slot
-  // bits}), staged in pinned memory and copied on the copy stream into a device buffer that grows on demand
-  bool sparse = false;
+  // CPBUS_CFG_SPARSE_TICKS: the armed slots by due time, and the plan of a sparse flush (entries, record indices, and the
+  // {mailbox, record} pairs it is sorted from), staged in pinned memory as [entries | indices] and copied on the copy stream
+  // into a device buffer that grows on demand.  CPBUS_CFG_SPARSE_RECORDS: records are planned too, from the subscription
+  // index.
+  bool sparse = false, sparse_records = false;
   DueIndex due;
   std::vector<uint32_t> due_slots;
-  uint2* h_tick_list = nullptr; uint2* d_tick_list = nullptr; size_t tick_list_cap = 0;
-  cudaEvent_t tick_list_done = nullptr;   // on copy_stream: the list has reached HBM (and left the pinned buffer)
-  cudaEvent_t tick_done = nullptr;        // on the bus stream: the tick kernel is done with the list
-
-  // CPBUS_CFG_SPARSE_RECORDS: the subscription index, the plan of the flush (entries, record indices, and the {mailbox,
-  // record} pairs it is sorted from), staged in pinned memory as [entries | indices] and copied on the copy stream into a
-  // device buffer that grows on demand
-  bool sparse_records = false;
   SubIndex rec_index;
   std::vector<cpbus_plan_entry> plan;
   std::vector<uint32_t> plan_idx;
@@ -751,6 +746,17 @@ struct LaunchOpts {
   const StreamArgs* stream = nullptr;
 };
 
+// The step-result sub-slots of launch ordinal `seq`: a launch adds into its own and zeroes its successor's.
+DevResultSlot* result_slot(const cpbus* b, unsigned long long seq) {
+  return b->d_result + (size_t)(seq % kResultRing) * kResultSub;
+}
+
+// A launch (or a flush with nothing to launch) has reached watermark w: the clock, and the due index, follow it.
+void launched_to(cpbus* b, uint64_t w) {
+  b->last_watermark = w;
+  if (b->sparse) due_fire(b->due, b->h_timers, w, [](uint32_t, uint64_t, uint64_t) {});
+}
+
 int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, const LaunchOpts& o = {}) {
   const StreamArgs* sa = o.stream;
   if (b->n_next == 0 && !sa) return CPBUS_OK;
@@ -759,8 +765,7 @@ int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, co
   p.batch = d_src; p.ring = b->d_ring; p.ctl = b->d_ctl; p.timers = b->d_timers; p.stats = b->d_stats; p.pow_table = b->d_pow; p.launch_seq = ++b->launch_seq;
   p.desc = b->d_desc + (p.launch_seq & 1) * ((fanout_desc_bytes(2048) + 255) & ~(size_t)255);   // two descriptor buffers: launch i+1 may write while launch i reads
   p.desc_ready = b->d_desc_ready + (p.launch_seq & 1) * 16; p.w_now = w;
-  p.result = b->d_result + (size_t)(p.launch_seq % kResultRing) * kResultSub;
-  p.result_next = b->d_result + (size_t)((p.launch_seq + 1) % kResultRing) * kResultSub;
+  p.result = result_slot(b, p.launch_seq); p.result_next = result_slot(b, p.launch_seq + 1);
   p.batch_local = b->d_batch_local; p.staged = (uint32_t)o.staged;
   p.err_word = b->d_err; p.acct = o.account ? b->d_acct : nullptr;
   p.pf_state = b->d_pf_state; p.pf_buf = b->d_pf_buf; p.pf_stride = b->B; p.spin_us = b->stream_spin_us;
@@ -861,47 +866,8 @@ int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, co
   b->st.kernel_launches++;
   if (!round) b->st.batches++;   // (a round's batch counts when it is resolved, if it delivered)
   if (sa) return CPBUS_OK;       // (the caller folds a stream launch in once its outcome is known: stream_delivered)
-  b->last_watermark = w;
-  if (b->sparse) due_fire(b->due, b->h_timers, w, [](uint32_t, uint64_t, uint64_t) {});
+  launched_to(b, w);
   if (o.account && n) dbg_mark_device_batch(b, p.launch_seq);
-  return CPBUS_OK;
-}
-
-// CPBUS_CFG_SPARSE_TICKS: the tick kernel over the due mailboxes in h_tick_list[0, n), to watermark w.  The list goes up on
-// the copy stream once the previous tick kernel is done with the device buffer; the kernel runs on the bus stream behind
-// every earlier launch (no programmatic dependent launch: it neither waits for nor releases a fan-out's prologue).
-int launch_ticks(cpbus* b, size_t n, uint64_t w) {
-  CK(cudaStreamWaitEvent(b->copy_stream, b->tick_done, 0));
-  CK(cudaMemcpyAsync(b->d_tick_list, b->h_tick_list, n * sizeof(uint2), cudaMemcpyHostToDevice, b->copy_stream));
-  CK(cudaEventRecord(b->tick_list_done, b->copy_stream));
-  CK(cudaStreamWaitEvent(b->stream, b->tick_list_done, 0));
-  TickScatterParams p{};
-  p.list = b->d_tick_list; p.n_list = (uint32_t)n;
-  p.ring = b->d_ring; p.ctl = b->d_ctl; p.timers = b->d_timers; p.stats = b->d_stats; p.pow_table = b->d_pow;
-  p.launch_seq = ++b->launch_seq;
-  p.result = b->d_result + (size_t)(p.launch_seq % kResultRing) * kResultSub;
-  p.result_next = b->d_result + (size_t)((p.launch_seq + 1) % kResultRing) * kResultSub;
-  p.w_now = w; p.ring_cap = b->R; p.K = b->K; p.sub_base = b->cfg.sub_id_base; p.use_digest = b->use_digest ? 1u : 0u;
-  tick_scatter_kernel<<<(uint32_t)((n + kWarpsPerCta - 1) / kWarpsPerCta), kThreads, 0, b->stream>>>(p);
-  CK(cudaGetLastError());
-  CK(cudaEventRecord(b->tick_done, b->stream));
-  b->st.kernel_launches++;
-  b->last_watermark = w;
-  due_fire(b->due, b->h_timers, w, [](uint32_t, uint64_t, uint64_t) {});
-  return CPBUS_OK;
-}
-
-// The pinned list buffer is free for n entries: the previous list has left it, or both buffers are regrown (behind every
-// kernel that may still read the old device buffer).
-int tick_list_room(cpbus* b, size_t n) {
-  if (n <= b->tick_list_cap) { CK(cudaEventSynchronize(b->tick_list_done)); return CPBUS_OK; }
-  CK(cudaStreamSynchronize(b->stream)); CK(cudaStreamSynchronize(b->copy_stream));
-  cudaFree(b->d_tick_list); cudaFreeHost(b->h_tick_list);
-  b->d_tick_list = nullptr; b->h_tick_list = nullptr; b->tick_list_cap = 0;
-  const size_t cap = std::max<size_t>(n, 1024);
-  CK(cudaMalloc((void**)&b->d_tick_list, cap * sizeof(uint2)));
-  CK(cudaMallocHost((void**)&b->h_tick_list, cap * sizeof(uint2)));
-  b->tick_list_cap = cap;
   return CPBUS_OK;
 }
 
@@ -911,54 +877,55 @@ void timer_table(cpbus* b) {
   if (b->sparse) b->due.init(b->h_timers.size());
 }
 
-// Due slots beyond which a flush with no record takes the full fan-out instead of the tick kernel.  Measured on an H100
-// (DESIGN.md §4.6): at 1,048,576 subscribers the tick path wins at N/1,024 due slots and loses at N/128.
-size_t sparse_max(const cpbus* b) { return std::max<size_t>(32, b->n_next / 1024); }
-
-// CPBUS_CFG_SPARSE_TICKS, nothing staged: true when the flush is done without the full fan-out (*rc = its status): no tick
-// due in (last watermark, w] launches nothing; up to sparse_max due slots launch the tick kernel.  False: the full fan-out
-// follows — more due slots than that, or (lossless) a room bound that cannot prove the largest share of one mailbox fits.
-bool sparse_flush(cpbus* b, uint64_t w, int* rc) {
-  *rc = CPBUS_OK;
-  if (b->due.min_due() > w) { b->last_watermark = w; return true; }
-  std::vector<uint32_t>& due = b->due_slots;
-  due.clear();
-  if (!b->due.collect(w, sparse_max(b), &due)) return false;
-  if (due.empty()) {   // only stale entries in front (min_due is a lower bound): nothing to launch, drop them
-    b->last_watermark = w;
-    due_fire(b->due, b->h_timers, w, [](uint32_t, uint64_t, uint64_t) {});
-    return true;
+// Device staging is a long ring (kDevSlots batches): a slot is reused only kDevSlots flushes later, far beyond how far the
+// host can run ahead, so the H2D never has to wait for an old fan-out and lands within microseconds.  Reuse safety is a
+// host-side check once per epoch of kDevEpoch slots (almost always already satisfied).  stage_batch takes the next slot
+// (*d_dst) and puts the n records of the current pinned buffer on their way into it; retire_slot follows the launch that
+// reads the slot.
+int stage_batch(cpbus* b, uint32_t n, cpbus_event** d_dst) {
+  const uint32_t slot = b->dev_slot;
+  *d_dst = b->d_stage + (size_t)slot * b->B;
+  if (slot % cpbus::kDevEpoch == 0) CK(cudaEventSynchronize(b->epoch_done[slot / cpbus::kDevEpoch]));   // last round's users of this epoch are done
+  if (n) {
+    CK(cudaMemcpyAsync(*d_dst, b->h_batch[b->cur], (size_t)n * sizeof(cpbus_event), cudaMemcpyHostToDevice, b->copy_stream));
+    CK(cudaEventRecord(b->h2d_done[b->cur], b->copy_stream));
   }
-  std::sort(due.begin(), due.end());
-  uint64_t most = 0;   // the most ticks one mailbox takes
-  std::vector<uint2> list;
-  for (size_t i = 0; i < due.size();) {
-    const uint32_t l = due[i] / b->K;
-    uint32_t bits = 0;
-    uint64_t ticks = 0;
-    for (; i < due.size() && due[i] / b->K == l; i++) {
-      const HostTimer& t = b->h_timers[due[i]];
-      bits |= 1u << (due[i] % b->K);
-      ticks += t.oneshot ? 1 : due_ticks(t.next_due, t.period, w);
-    }
-    list.push_back(make_uint2(l, bits));
-    most = std::max(most, ticks);
-  }
-  const size_t n = list.size();
-  if (b->lossless) {
-    if (b->room_lb < most) return false;
-    b->room_lb -= most; b->st.admit_skipped++;
-  }
-  if ((*rc = tick_list_room(b, n))) return true;
-  std::copy(list.begin(), list.end(), b->h_tick_list);
-  *rc = launch_ticks(b, n, w);
-  return true;
+  return CPBUS_OK;
 }
 
-// CPBUS_CFG_SPARSE_RECORDS: candidate mailboxes (the tick path's threshold) and planned record deliveries beyond which a flush
-// with staged records takes the full fan-out.  Measured on an H100 (DESIGN.md §4.7).
-size_t records_max_mailboxes(const cpbus* b) { return sparse_max(b); }
-size_t records_max_deliveries(const cpbus* b) { return std::max<size_t>(1024, b->n_next / 256); }
+int retire_slot(cpbus* b) {
+  const uint32_t slot = b->dev_slot;
+  if (slot % cpbus::kDevEpoch == cpbus::kDevEpoch - 1) CK(cudaEventRecord(b->epoch_done[slot / cpbus::kDevEpoch], b->stream));
+  b->dev_slot = (slot + 1) % cpbus::kDevSlots;
+  return CPBUS_OK;
+}
+
+// Give the 8-16 KiB copy that `copied` marks up to 30 us to land.  If it has, the bus stream needs no wait node, consecutive
+// fan-outs stay adjacent in the stream and the next launch's prologue overlaps this one's tail (programmatic dependent launch).
+int await_copy(cpbus* b, cudaEvent_t copied) {
+  const auto t_spin = std::chrono::steady_clock::now();
+  do {
+    const cudaError_t q = cudaEventQuery(copied);
+    if (q == cudaSuccess) return CPBUS_OK;
+    if (q != cudaErrorNotReady) { CK(q); }
+  } while (std::chrono::steady_clock::now() - t_spin < std::chrono::microseconds(30));
+  CK(cudaStreamWaitEvent(b->stream, copied, 0));
+  return CPBUS_OK;
+}
+
+// The staged batch has been launched whole: staging moves on to the next pinned buffer.
+int next_buffer(cpbus* b) {
+  b->cur = (b->cur + 1) % cpbus::kStage;
+  CK(cudaEventSynchronize(b->h2d_done[b->cur]));   // the pinned buffer we are about to overwrite has left the host
+  return CPBUS_OK;
+}
+
+// CPBUS_CFG_SPARSE_TICKS: mailboxes (due slots, or candidates of a plan) and planned record deliveries beyond which a flush
+// takes the full fan-out.  Measured on an H100 (DESIGN.md §4.6, §4.7): at 1,048,576 subscribers a dedicated tick kernel won
+// at N/1,024 due slots and lost at N/128; the record kernel on timer-only plans costs the same as that kernel at N/1,024
+// (the rows re-measured in §4.6), so the cap stays.
+size_t sparse_max(const cpbus* b) { return std::max<size_t>(32, b->n_next / 1024); }
+size_t sparse_max_deliveries(const cpbus* b) { return std::max<size_t>(1024, b->n_next / 256); }
 
 // The pinned plan buffer is free for `bytes`: the previous plan has left it, or both buffers are regrown (behind every
 // kernel that may still read the old device buffer).
@@ -974,73 +941,63 @@ int plan_room(cpbus* b, size_t bytes) {
   return CPBUS_OK;
 }
 
-// The record kernel over b->plan, to watermark w, for the staged batch.  The batch takes the next device staging slot as
-// in flush_staged (epoch events, 30 us landing spin); the plan follows it on the copy stream once the previous record kernel
-// is done with the device buffer.  The kernel runs on the bus stream behind every earlier launch, without programmatic
-// dependent launch.  A plan without a mailbox launches nothing and copies nothing.  Then the staging buffer moves on and
-// the clock and the due index follow the launch, as after a fan-out.
-int launch_records(cpbus* b, uint64_t w) {
+// The record kernel over b->plan, to watermark w.  The plan goes up on the copy stream once the previous record kernel is
+// done with the device buffer, and the kernel runs on the bus stream behind every earlier launch, without programmatic
+// dependent launch.  With records staged, the batch takes the next device staging slot in front of the plan, the landing
+// spin waits for both, and the staging buffer moves on.  A flush of due ticks alone has no batch: the bus stream waits for
+// the plan.  A plan without a mailbox launches nothing and copies nothing.  The clock and the due index follow, as after a
+// fan-out.
+int launch_sparse(cpbus* b, uint64_t w) {
   const size_t n_list = b->plan.size(), n_idx = b->plan_idx.size();
   const uint32_t n = (uint32_t)b->n_staged;
-  const int c = b->cur;
   if (n_list) {
     const size_t list_bytes = n_list * sizeof(cpbus_plan_entry), bytes = list_bytes + n_idx * sizeof(uint32_t);
     int rc = plan_room(b, bytes); if (rc) return rc;
     memcpy(b->h_plan, b->plan.data(), list_bytes);
     memcpy(b->h_plan + list_bytes, b->plan_idx.data(), n_idx * sizeof(uint32_t));
-    const uint32_t slot = b->dev_slot;
-    cpbus_event* d_dst = b->d_stage + (size_t)slot * b->B;
-    if (slot % cpbus::kDevEpoch == 0) CK(cudaEventSynchronize(b->epoch_done[slot / cpbus::kDevEpoch]));
-    CK(cudaMemcpyAsync(d_dst, b->h_batch[c], (size_t)n * sizeof(cpbus_event), cudaMemcpyHostToDevice, b->copy_stream));
-    CK(cudaEventRecord(b->h2d_done[c], b->copy_stream));
+    cpbus_event* d_dst = nullptr;
+    if (n && (rc = stage_batch(b, n, &d_dst))) return rc;
     CK(cudaStreamWaitEvent(b->copy_stream, b->records_done, 0));
     CK(cudaMemcpyAsync(b->d_plan, b->h_plan, bytes, cudaMemcpyHostToDevice, b->copy_stream));
     CK(cudaEventRecord(b->plan_done, b->copy_stream));
-    bool landed = false;
-    const auto t_spin = std::chrono::steady_clock::now();
-    do {
-      const cudaError_t q = cudaEventQuery(b->plan_done);
-      if (q == cudaSuccess) { landed = true; break; }
-      if (q != cudaErrorNotReady) { CK(q); }
-    } while (std::chrono::steady_clock::now() - t_spin < std::chrono::microseconds(30));
-    if (!landed) CK(cudaStreamWaitEvent(b->stream, b->plan_done, 0));
+    if (n) { if ((rc = await_copy(b, b->plan_done))) return rc; }
+    else CK(cudaStreamWaitEvent(b->stream, b->plan_done, 0));
     RecordScatterParams p{};
     p.list = reinterpret_cast<const uint4*>(b->d_plan); p.n_list = (uint32_t)n_list;
     p.idx = reinterpret_cast<const uint32_t*>(b->d_plan + list_bytes); p.batch = d_dst;
     p.ring = b->d_ring; p.ctl = b->d_ctl; p.timers = b->d_timers; p.stats = b->d_stats; p.pow_table = b->d_pow;
     p.launch_seq = ++b->launch_seq;
-    p.result = b->d_result + (size_t)(p.launch_seq % kResultRing) * kResultSub;
-    p.result_next = b->d_result + (size_t)((p.launch_seq + 1) % kResultRing) * kResultSub;
+    p.result = result_slot(b, p.launch_seq); p.result_next = result_slot(b, p.launch_seq + 1);
     p.w_now = w; p.ring_cap = b->R; p.K = b->K; p.sub_base = b->cfg.sub_id_base; p.use_digest = b->use_digest ? 1u : 0u;
     record_scatter_kernel<<<(uint32_t)((n_list + kWarpsPerCta - 1) / kWarpsPerCta), kThreads, 0, b->stream>>>(p);
     CK(cudaGetLastError());
     CK(cudaEventRecord(b->records_done, b->stream));
     b->st.kernel_launches++;
-    if (slot % cpbus::kDevEpoch == cpbus::kDevEpoch - 1) CK(cudaEventRecord(b->epoch_done[slot / cpbus::kDevEpoch], b->stream));
-    b->dev_slot = (slot + 1) % cpbus::kDevSlots;
-    b->cur = (b->cur + 1) % cpbus::kStage;
+    if (n && (rc = retire_slot(b))) return rc;
   }
   b->n_staged = 0;
-  if (b->n_next) {   // (the fan-out of a bus without subscribers launches nothing and leaves the watermark where it was)
-    b->last_watermark = w;
-    due_fire(b->due, b->h_timers, w, [](uint32_t, uint64_t, uint64_t) {});
-  }
-  if (n_list) CK(cudaEventSynchronize(b->h2d_done[b->cur]));   // the pinned buffer we are about to overwrite has left the host
-  return CPBUS_OK;
+  // (n_next == 0: records staged on a bus without subscribers, which has no timer either; like the fan-out, the flush
+  // launches nothing and leaves the watermark where it was.  A flush of due ticks alone always has subscribers.)
+  if (b->n_next) launched_to(b, w);
+  return n_list && n ? next_buffer(b) : CPBUS_OK;
 }
 
-// CPBUS_CFG_SPARSE_RECORDS, records staged: true when the flush is done without the full fan-out (*rc = its status): the
-// staged records and the ticks due by w reach at most records_max_mailboxes mailboxes with at most records_max_deliveries
-// records, and (lossless) the room bound covers the most that one of them takes, records and ticks.  False: the full
-// fan-out follows, with admission and the partial prefix as before.
-bool record_flush(cpbus* b, uint64_t w, int* rc) {
+// CPBUS_CFG_SPARSE_TICKS, with nothing staged or with CPBUS_CFG_SPARSE_RECORDS: true when the flush is done without the full
+// fan-out (*rc = its status).  No record staged and no tick due in (last watermark, w]: no launch.  Otherwise the ticks due
+// by w and the staged records are planned, and a plan within the caps launches the record kernel over its mailboxes (none:
+// no launch).  False: the full fan-out follows, with admission and the partial prefix as before — past a cap, or (lossless)
+// when the room bound cannot prove that the most one mailbox takes, records and ticks, fits.
+bool sparse_flush(cpbus* b, uint64_t w, int* rc) {
   *rc = CPBUS_OK;
-  const size_t max_m = records_max_mailboxes(b);
+  const bool ticks = b->due.min_due() <= w;
+  if (!ticks && !b->n_staged) { b->last_watermark = w; return true; }
+  const size_t max_m = sparse_max(b);
   std::vector<uint32_t>& due = b->due_slots;
   due.clear();
-  if (b->due.min_due() <= w && !b->due.collect(w, max_m, &due)) return false;
+  if (ticks && !b->due.collect(w, max_m, &due)) return false;
+  if (due.empty() && !b->n_staged) { launched_to(b, w); return true; }   // only stale entries in front (min_due is a lower bound): drop them
   if (!sparse_plan(b->rec_index, b->h_mask.data(), b->h_active.data(), b->n_next, b->cfg.sub_id_base, b->h_batch[b->cur],
-                   b->n_staged, due, b->K, max_m, records_max_deliveries(b), b->plan_pairs, b->plan, b->plan_idx))
+                   b->n_staged, due, b->K, max_m, sparse_max_deliveries(b), b->plan_pairs, b->plan, b->plan_idx))
     return false;
   if (b->lossless) {
     uint64_t most = 0;   // the most one mailbox takes
@@ -1056,7 +1013,7 @@ bool record_flush(cpbus* b, uint64_t w, int* rc) {
     if (b->room_lb < most) return false;
     b->room_lb -= most; b->st.admit_skipped++;
   }
-  *rc = launch_records(b, w);
+  *rc = launch_sparse(b, w);
   return true;
 }
 
@@ -1140,30 +1097,11 @@ bool flush_idle(HostFront* f, uint64_t w) {
 int flush_staged(cpbus* b, uint64_t w) {
   if (flush_idle(b, w)) return CPBUS_OK;
   int rc;
-  if (b->sparse && !b->n_staged && sparse_flush(b, w, &rc)) return rc;
-  if (b->sparse_records && b->n_staged && record_flush(b, w, &rc)) return rc;
+  if (b->sparse && (!b->n_staged || b->sparse_records) && sparse_flush(b, w, &rc)) return rc;
   const uint32_t n = (uint32_t)b->n_staged;
   const int c = b->cur;
-  // Device staging is a long ring (kDevSlots batches): a slot is reused only kDevSlots flushes later, far beyond how far the
-  // host can run ahead, so the H2D never has to wait for an old fan-out and lands within microseconds.  Reuse safety is a
-  // host-side check once per epoch of kDevEpoch slots (almost always already satisfied).
-  const uint32_t slot = b->dev_slot;
-  cpbus_event* d_dst = b->d_stage + (size_t)slot * b->B;
-  if (slot % cpbus::kDevEpoch == 0) CK(cudaEventSynchronize(b->epoch_done[slot / cpbus::kDevEpoch]));   // last round's users of this epoch are done
-  if (n) {
-    CK(cudaMemcpyAsync(d_dst, b->h_batch[c], (size_t)n * sizeof(cpbus_event), cudaMemcpyHostToDevice, b->copy_stream));
-    CK(cudaEventRecord(b->h2d_done[c], b->copy_stream));
-    // Give the 8-16 KiB copy up to 30 us to land.  If it has, the bus stream needs no wait node, consecutive fan-outs
-    // stay adjacent in the stream and the next launch's prologue overlaps this one's tail (programmatic dependent launch).
-    bool landed = false;
-    const auto t_spin = std::chrono::steady_clock::now();
-    do {
-      const cudaError_t q = cudaEventQuery(b->h2d_done[c]);
-      if (q == cudaSuccess) { landed = true; break; }
-      if (q != cudaErrorNotReady) { CK(q); }
-    } while (std::chrono::steady_clock::now() - t_spin < std::chrono::microseconds(30));
-    if (!landed) CK(cudaStreamWaitEvent(b->stream, b->h2d_done[c], 0));
-  }
+  cpbus_event* d_dst;
+  if ((rc = stage_batch(b, n, &d_dst)) || (n && (rc = await_copy(b, b->h2d_done[c])))) return rc;
   bool ok = true;
   uint32_t m = n;
   rc = admit(b, d_dst, n, w, &ok, &m);
@@ -1174,24 +1112,16 @@ int flush_staged(cpbus* b, uint64_t w) {
     // event — keep the rest staged and report the stall; the caller lets the consumers run and flushes again.
     if (m == 0) return CPBUS_EAGAIN;
     const uint64_t w_part = b->h_batch[c][m - 1].ts_ns;
-    rc = launch_fanout(b, d_dst, m, w_part);
-    if (rc) return rc;
-    if (slot % cpbus::kDevEpoch == cpbus::kDevEpoch - 1) CK(cudaEventRecord(b->epoch_done[slot / cpbus::kDevEpoch], b->stream));
-    b->dev_slot = (slot + 1) % cpbus::kDevSlots;
+    if ((rc = launch_fanout(b, d_dst, m, w_part)) || (rc = retire_slot(b))) return rc;
     memmove(b->h_batch[c], b->h_batch[c] + m, (size_t)(n - m) * sizeof(cpbus_event));   // (the H2D of this buffer completed before the admission pass)
     b->n_staged = n - m;
     b->room_lb = 0;
     b->st.admit_partial++;
     return CPBUS_EAGAIN;
   }
-  rc = launch_fanout(b, d_dst, n, w);
-  if (rc) return rc;
-  if (slot % cpbus::kDevEpoch == cpbus::kDevEpoch - 1) CK(cudaEventRecord(b->epoch_done[slot / cpbus::kDevEpoch], b->stream));
-  b->dev_slot = (slot + 1) % cpbus::kDevSlots;
+  if ((rc = launch_fanout(b, d_dst, n, w)) || (rc = retire_slot(b))) return rc;
   b->n_staged = 0;
-  b->cur = (b->cur + 1) % cpbus::kStage;
-  CK(cudaEventSynchronize(b->h2d_done[b->cur]));   // the pinned buffer we are about to overwrite has left the host
-  return CPBUS_OK;
+  return next_buffer(b);
 }
 
 // One launch of the single bus: the same early returns as launch_fanout, otherwise one stream batch on every shard.
@@ -1581,11 +1511,8 @@ int cpbus_create(const cpbus_config* cfg, cpbus_t** out) try {
   if (cudaStreamCreateWithFlags(&b->copy_stream, cudaStreamNonBlocking) != cudaSuccess) return fail(CPBUS_ECUDA);
   if (cudaStreamCreateWithFlags(&b->result_stream, cudaStreamNonBlocking) != cudaSuccess) return fail(CPBUS_ECUDA);
   if (cudaEventCreateWithFlags(&b->launched, cudaEventDisableTiming) != cudaSuccess) return fail(CPBUS_ECUDA);
-  if (b->sparse && (cudaEventCreateWithFlags(&b->tick_list_done, cudaEventDisableTiming) != cudaSuccess ||
-                    cudaEventCreateWithFlags(&b->tick_done, cudaEventDisableTiming) != cudaSuccess))
-    return fail(CPBUS_ECUDA);
-  if (b->sparse_records && (cudaEventCreateWithFlags(&b->plan_done, cudaEventDisableTiming) != cudaSuccess ||
-                            cudaEventCreateWithFlags(&b->records_done, cudaEventDisableTiming) != cudaSuccess))
+  if (b->sparse && (cudaEventCreateWithFlags(&b->plan_done, cudaEventDisableTiming) != cudaSuccess ||
+                    cudaEventCreateWithFlags(&b->records_done, cudaEventDisableTiming) != cudaSuccess))
     return fail(CPBUS_ECUDA);
   ALLOC(b->d_stage, (size_t)cpbus::kDevSlots * B * sizeof(cpbus_event));
   for (int i = 0; i < cpbus::kDevSlots / cpbus::kDevEpoch; i++)
@@ -1649,6 +1576,7 @@ int cpbus_create(const cpbus_config* cfg, cpbus_t** out) try {
   b->h_mask.assign(N, 0);
   b->h_active.assign(N, 0);
   if (b->sparse_records) b->rec_index.init(N, 2 * std::max<size_t>(32, N / 1024));   // lists of up to twice the largest cap
+  else if (b->sparse) b->rec_index.slot.assign(N, UINT32_MAX);
   b->intern.emplace(std::string(), 0u);   // "" -> 0 so that NonEvent == {None, 0} (events/events.go:45)
   b->sources.emplace_back();
   *out = b;
@@ -1678,10 +1606,6 @@ int cpbus_destroy(cpbus_t* b) try {
   for (int i = 0; i < cpbus::kDevSlots / cpbus::kDevEpoch; i++) if (b->epoch_done[i]) cudaEventDestroy(b->epoch_done[i]);
   if (b->copy_stream) cudaStreamDestroy(b->copy_stream);
   if (b->launched) cudaEventDestroy(b->launched);
-  if (b->tick_list_done) cudaEventDestroy(b->tick_list_done);
-  if (b->tick_done) cudaEventDestroy(b->tick_done);
-  cudaFree(b->d_tick_list);
-  if (b->h_tick_list) cudaFreeHost(b->h_tick_list);
   if (b->plan_done) cudaEventDestroy(b->plan_done);
   if (b->records_done) cudaEventDestroy(b->records_done);
   cudaFree(b->d_plan);
@@ -3085,7 +3009,7 @@ int cpbus_step_result_begin(cpbus_t* b, uint32_t* ticket) try {
   std::lock_guard<std::mutex> g(b->mu);
   int rc = dev_guard(b); if (rc) return rc;
   const uint32_t t = b->result_next++ % 8;
-  const DevResultSlot* src = b->d_result + (size_t)(b->launch_seq % kResultRing) * kResultSub;
+  const DevResultSlot* src = result_slot(b, b->launch_seq);
   // read it on a side stream, behind an event recorded after the launch: neither the next fan-out nor the next batch's
   // H2D queues behind this D2H
   CK(cudaEventRecord(b->launched, b->stream));

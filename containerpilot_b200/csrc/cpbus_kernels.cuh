@@ -971,130 +971,22 @@ __global__ void digest_fold_kernel(const SubCtl* ctl, uint32_t first, uint32_t n
   if (blockIdx.x == 0 && threadIdx.x == 0) out4[3] = n;
 }
 
-// Sparse timer delivery (CPBUS_CFG_SPARSE_TICKS): a flush with no staged record and few due ticks.  The host's due index
-// lists the mailboxes that own due slots, ascending, each with the bitmask of its due slots.  One warp per mailbox does what
-// the fan-out kernel does for a mailbox that takes ticks and no record: lane (slot = lane / J, j = lane % J) is candidate
-// firing j of a slot, overflowing candidates are rejected, the firings <= w are ranked by (due, slot) and appended at
-// tail + rank, the digest is extended, each slot that fired is re-armed (saturating) and the control block is written back
-// as one sector.  Rings, control blocks and timer slots end up bit-identical to what the fan-out kernel leaves.  The tick
-// arithmetic is restated here, not shared with the fan-out body, so that no existing kernel changes.
-struct TickScatterParams {
-  const uint2* list;                 // n_list x {local subscriber index, bitmask of its due slots}, ascending
-  uint32_t n_list;
-  cpbus_event* ring; SubCtl* ctl; DevTimer* timers; DevStats* stats;
-  const uint64_t* pow_table;
-  DevResultSlot* result;             // this launch's sub-slots (zeroed by the previous launch) ...
-  DevResultSlot* result_next;        // ... and the next launch's, zeroed here
-  unsigned long long launch_seq;
-  uint64_t w_now;
-  uint32_t ring_cap, K, sub_base, use_digest;
-};
-
-__global__ void __launch_bounds__(kThreads) tick_scatter_kernel(const TickScatterParams p) {
-  __shared__ uint32_t s_ticks, s_dig_lo, s_dig_hi;
-  const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
-  if (tid == 0) { s_ticks = 0; s_dig_lo = 0; s_dig_hi = 0; }
-  if (blockIdx.x == 0 && tid < kResultSub * 4) reinterpret_cast<unsigned long long*>(p.result_next)[tid] = 0ull;
-  __syncthreads();
-  const uint32_t K = p.K, J = 32u / K;
-  const uint32_t slot = lane / J, j = lane % J;
-  const uint32_t i = blockIdx.x * kWarpsPerCta + warp;
-  if (i < p.n_list) {   // warp-uniform
-    const uint2 e = p.list[i];
-    const uint32_t s = e.x;
-    uint4 c0, c1;
-    ld_sector(p.ctl + s, c0, c1, false);
-    const uint32_t m = c1.z;
-    const uint32_t nslots = (m & kActiveBit) ? min((m >> kTimerHintShift) & 0xFu, K) : 0u;
-    DevTimer* tp = p.timers + (size_t)s * K + slot;
-    uint64_t due0 = kTimerIdle, period = 0;
-    if (slot < nslots && ((e.y >> slot) & 1u)) {
-      const uint4 hot = *reinterpret_cast<const uint4*>(tp);
-      due0 = ((uint64_t)hot.y << 32) | hot.x; period = ((uint64_t)hot.w << 32) | hot.z;
-    }
-    const uint64_t step = (uint64_t)j * period, due = due0 + step;
-    const bool wraps = __umul64hi(j, period) != 0 || due < step || due == kTimerIdle;
-    const bool valid = due0 != kTimerIdle && !wraps && due <= p.w_now && (j == 0 || period != 0);
-    const uint32_t fired_mask = __ballot_sync(0xffffffffu, valid);
-    const uint32_t k = __popc(fired_mask);
-    if (k) {   // warp-uniform
-      uint32_t rank = 0;
-#pragma unroll 1
-      for (uint32_t t = 0; t < 32; t++) {
-        if (!((fired_mask >> t) & 1u)) continue;   // warp-uniform
-        const uint64_t od = shfl64(due, t);
-        const uint32_t os = __shfl_sync(0xffffffffu, slot, t);
-        rank += (od < due || (od == due && os < slot)) ? 1u : 0u;
-      }
-      uint32_t src = 0, fired = 0;
-      if (valid) {   // cold half {source_id, fired}: only slots that fire
-        const uint4 cold = *reinterpret_cast<const uint4*>(reinterpret_cast<const unsigned char*>(tp) + 16);
-        src = cold.x; fired = cold.y;
-      }
-      const uint64_t tail = ((uint64_t)c0.y << 32) | c0.x;
-      uint64_t dsum = 0;
-      if (valid) {   // the tick record {seq = firing ordinal, ts = due, TimerExpired, source, target = gid, F_TICK}
-        const uint64_t w0 = (uint64_t)fired + j, w1 = due;
-        const uint64_t w2 = (uint64_t)CPBUS_TIMER_EXPIRED | ((uint64_t)src << 32);
-        const uint64_t w3 = (uint64_t)(p.sub_base + s) | ((uint64_t)CPBUS_F_TICK << 32);
-        cpbus_event* ring = p.ring + (size_t)s * p.ring_cap;
-        st_v8(ring + (((uint32_t)tail + rank) & (p.ring_cap - 1u)),
-              make_uint4((uint32_t)w0, (uint32_t)(w0 >> 32), (uint32_t)w1, (uint32_t)(w1 >> 32)),
-              make_uint4((uint32_t)w2, (uint32_t)(w2 >> 32), (uint32_t)w3, (uint32_t)(w3 >> 32)));
-        if (p.use_digest) dsum = record_hash_words(w0, w1, w2, w3) * p.pow_table[k - 1 - rank];
-      }
-      if (p.use_digest) dsum = warp_sum64(dsum);
-      // re-arm: the lane of candidate 0 of each slot that fired (a one-shot disarms itself; past UINT64_MAX - 1: never)
-      const uint32_t slotmask = (J == 32 ? 0xffffffffu : ((1u << J) - 1u)) << (slot * J);
-      const uint32_t fired_here = __popc(fired_mask & slotmask);
-      if (j == 0 && fired_here) {
-        const uint64_t st = (uint64_t)fired_here * period;
-        const uint64_t nd = (period && __umul64hi(fired_here, period) == 0 && st < kTimerIdle - due) ? due + st : kTimerIdle;
-        unsigned char* t = reinterpret_cast<unsigned char*>(tp);
-        st_v4(t, make_uint4((uint32_t)nd, (uint32_t)(nd >> 32), (uint32_t)period, (uint32_t)(period >> 32)));
-        st_v4(t + 16, make_uint4(src, fired + fired_here, 0u, 0u));
-      }
-      if (lane == 0) {
-        const uint64_t dig = ((uint64_t)c1.y << 32) | c1.x;
-        const uint64_t nt = tail + k, nd = p.use_digest ? dig * p.pow_table[k] + dsum : dig;
-        st_v8(p.ctl + s, make_uint4((uint32_t)nt, (uint32_t)(nt >> 32), c0.z, c0.w),   // head: consumer-owned, passed through
-              make_uint4((uint32_t)nd, (uint32_t)(nd >> 32), m, 0u));
-        atomicAdd(&s_ticks, k);
-        if (p.use_digest) {
-          const uint32_t f = (uint32_t)nd ^ (uint32_t)(nd >> 32);
-          atomicAdd(&s_dig_lo, f & 0xFFFFu);
-          atomicAdd(&s_dig_hi, f >> 16);
-        }
-      }
-    }
-  }
-  __syncthreads();
-  if (tid == 0) {   // the fan-out kernel's accounting: every record here is a tick
-    DevStatSlot* st = &p.stats->slot[blockIdx.x % kStatSlots];
-    DevResultSlot* rs = &p.result[blockIdx.x % kResultSub];
-    if (s_ticks) {
-      atomicAdd(&st->deliveries, (unsigned long long)s_ticks); atomicAdd(&st->ticks, (unsigned long long)s_ticks);
-      atomicAdd(&rs->deliveries, (unsigned long long)s_ticks); atomicAdd(&rs->ticks, (unsigned long long)s_ticks);
-    }
-    if (s_dig_lo | s_dig_hi) atomicAdd(&rs->digest_sum, (unsigned long long)s_dig_lo + ((unsigned long long)s_dig_hi << 16));
-    if (blockIdx.x == 0) atomicAdd(&rs->launch_seq, p.launch_seq);
-  }
-}
-
-// Sparse record delivery (CPBUS_CFG_SPARSE_RECORDS): a flush whose staged records reach few mailboxes.  The host's plan
-// lists every mailbox that takes a record or owns a due tick, ascending, as {local index, bitmask of its due slots, first,
-// count}: its records are batch[idx[first .. first + count)] in batch order.  One warp per mailbox does what the fan-out
-// kernel does for it: the firings <= w are found and ranked by (due, slot) as in tick_scatter_kernel, a tick due at d is
-// placed in front of every record with ts >= d (record q lands at q + #{ticks whose lower bound among the records' ts is <=
-// q}), the records are copied by lane pairs (each store instruction fills 16 whole 32-byte sectors), the digest is
-// extended over the merged sequence, fired slots are re-armed (saturating) and the control block is written back as one
-// sector.  Rings, control blocks and timer slots end up bit-identical to what the fan-out kernel leaves.  The tick
-// arithmetic is restated here, not shared with the fan-out body or the tick kernel, so that no existing kernel changes.
+// Sparse delivery (CPBUS_CFG_SPARSE_TICKS, CPBUS_CFG_SPARSE_RECORDS): a flush whose due ticks and staged records reach few
+// mailboxes.  The host's plan lists every mailbox that takes a record or owns a due tick, ascending, as {local index, bitmask
+// of its due slots, first, count}: its records are batch[idx[first .. first + count)] in batch order (a flush of due ticks
+// alone: count 0 everywhere, and neither idx nor batch is read).  One warp per mailbox does what the fan-out kernel does for
+// it: lane (slot = lane / J, j = lane % J) is candidate firing j of a slot, overflowing candidates are rejected, the firings
+// <= w are ranked by (due, slot), a tick due at d is placed in front of every record with ts >= d (record q lands at q +
+// #{ticks whose lower bound among the records' ts is <= q}), the records are copied by lane pairs (each store instruction
+// fills 16 whole 32-byte sectors), the digest is extended over the merged sequence, fired slots are re-armed (saturating) and
+// the control block is written back as one sector.  Rings, control blocks and timer slots end up bit-identical to what the
+// fan-out kernel leaves.  The tick arithmetic is restated here, not shared with the fan-out body, so that the fan-out kernel
+// stays as it is.
 struct RecordScatterParams {
   const uint4* list;                 // n_list x {local subscriber index, due-slot bits, first, count}, ascending
   uint32_t n_list;
   const uint32_t* idx;               // record indices of every entry, each entry's ascending
-  const cpbus_event* batch;          // the flush's records (the device staging slot), sorted by ts
+  const cpbus_event* batch;          // the flush's records (the device staging slot), sorted by ts; nullptr: none
   cpbus_event* ring; SubCtl* ctl; DevTimer* timers; DevStats* stats;
   const uint64_t* pow_table;
   DevResultSlot* result;             // this launch's sub-slots (zeroed by the previous launch) ...

@@ -515,8 +515,8 @@ int cpbus_digest_fold_end(cpbus_t* bus, uint32_t ticket, uint64_t out[4]);
  * ticks among them, sum over every mailbox it appended to of fold32(new digest) with
  * fold32(x) = low32(x ^ (x >> 32)), launch ordinal}.
  * _begin enqueues a 256-byte D2H on the bus stream (up to 8 outstanding tickets), _end waits for it.
- * On a CPBUS_CFG_SPARSE_TICKS bus the tick kernel of a flush with no staged record is such a launch too, and a flush that
- * launched nothing leaves the result as it was.  So is the record kernel of a CPBUS_CFG_SPARSE_RECORDS flush. */
+ * On a CPBUS_CFG_SPARSE_TICKS bus the sparse kernel of a flush (due ticks alone, or with CPBUS_CFG_SPARSE_RECORDS also
+ * records) is such a launch too, and a flush that launched nothing leaves the result as it was. */
 int cpbus_step_result_begin(cpbus_t* bus, uint32_t* ticket);
 int cpbus_step_result_end(cpbus_t* bus, uint32_t ticket, uint64_t out[4]);
 

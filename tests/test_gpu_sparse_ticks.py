@@ -145,10 +145,10 @@ def test_launch_counts_by_path(lossless):
         b0, b1, _ = step(500)                  # nothing due
         assert b1 == b0
         r0 = sparse.step_result_end(sparse.step_result_begin())
-        b0, b1, (rp, rs) = step(1000)          # 20 due slots: one tick kernel, not a fan-out batch
+        b0, b1, (rp, rs) = step(1000)          # 20 due slots: one sparse kernel, not a fan-out batch
         assert b1 == (b0[0] + 1, b0[1])
         assert rs[:3] == rp[:3] and rs[0] == rs[1] == 20 and rs[3] != r0[3]
-        b0, b1, _ = step(1500)                 # idle again: the step result stays that of the tick kernel
+        b0, b1, _ = step(1500)                 # idle again: the step result stays that of the sparse kernel
         assert b1 == b0 and sparse.step_result_end(sparse.step_result_begin()) == rs
         b0, b1, (rp, rs) = step(7000)          # 20 + 1,000 due: the full fan-out
         assert b1[1] == b0[1] + 1 and rs[:3] == rp[:3] and rs[1] == 20 * 6 + 1000

@@ -1,7 +1,7 @@
 """Sparse record delivery (CPBUS_CFG_SPARSE_RECORDS) without a GPU: the flag and the plan export, a plain-C99 caller,
 cpbus_create's and the group's refusal of the flag, and the plan (cpbus_sparse_plan, the bus's own planning code) against
 a model built on tests/py_model.py's delivery rule on seeded fleets: code masks, exact cases, unsubscribed and mask-0
-mailboxes, unicast records and due timer slots.  It gives up exactly at the caps.
+mailboxes, unicast records and due timer slots, and flushes of due ticks alone.  It gives up exactly at the caps.
 The bus itself needs a GPU: tests/test_gpu_sparse_records.py."""
 import ctypes as C
 import os
@@ -113,9 +113,10 @@ def model(masks, active, pairs, base, rec, due, K):
     return [(l, bits.get(l, 0), took.get(l, [])) for l in sorted(set(took) | set(bits))]
 
 
-def fleet(rng, n, n_rec, K):
+def fleet(rng, n, n_rec, K, max_due=11):
     """a seeded fleet: all-ones, sparse and mask-0 subscribers, some with exact cases, a share unsubscribed; a batch of
-    broadcast records (a few out-of-range codes) and unicast sends (some to unsubscribed or foreign ids); due slots"""
+    broadcast records (a few out-of-range codes) and unicast sends (some to unsubscribed or foreign ids); up to max_due
+    due slots"""
     kind = rng.random(n)
     masks = np.where(kind < 0.1, nat.MASK_ALL, np.where(kind < 0.3, 0, 1 << rng.integers(0, 17, n))).astype(np.uint32)
     masks |= np.where(rng.random(n) < 0.3, 1 << rng.integers(0, 17, n), 0).astype(np.uint32)
@@ -132,23 +133,33 @@ def fleet(rng, n, n_rec, K):
     uni = rng.random(n_rec) < 0.2
     rec["target"] = np.where(uni, base + rng.integers(0, n + 3, n_rec), nat.TARGET_ALL)
     rec["flags"] = np.where(uni, nat.F_UNICAST, 0)
-    due = rng.choice(n * K, size=min(n * K, int(rng.integers(0, 12))), replace=False).tolist() if K else []
+    due = rng.choice(n * K, size=min(n * K, int(rng.integers(0, max_due + 1))), replace=False).tolist() if K else []
     return masks, active, pairs, base, rec, due
 
 
-@pytest.mark.parametrize("seed", range(300))
+@pytest.mark.parametrize("seed", range(400))
 def test_plan_against_the_delivery_rule(seed):
     rng = np.random.default_rng(seed)
     K = [0, 1, 2, 4, 8][seed % 5]
     n = int(rng.integers(1, 90))
-    masks, active, pairs, base, rec, due = fleet(rng, n, int(rng.integers(0, 64)), K)
+    if seed % 4 == 3:   # a flush of due ticks alone, up to every slot of the fleet
+        masks, active, pairs, base, rec, due = fleet(rng, n, 0, K, max_due=n * K)
+    else:
+        masks, active, pairs, base, rec, due = fleet(rng, n, int(rng.integers(0, 64)), K)
     want = model(masks, active, pairs, base, rec, due, K)
     n_cand, n_deliv = len(want), sum(len(r) for _, _, r in want)
     max_m = max(n_cand, len(due), 1)
     rc, got = plan(masks, active, pairs, base, rec, due, K, max_m, n_deliv)
     assert rc == nat.OK and got == want
+    if not len(rec):                      # one entry per due mailbox, ascending, with its due-slot bits and no record
+        bits = {}
+        for slot in due:
+            bits[slot // K] = bits.get(slot // K, 0) | 1 << (slot % K)
+        assert got == [(l, bits[l], []) for l in sorted(bits)]
     assert plan(masks, active, pairs, base, rec, due, K, max_m + 1 + seed % 7, n_deliv + seed % 3) == (nat.OK, want)
-    if n_cand > 1 or len(due) > 1:        # one mailbox fewer than needed: the full fan-out
+    # one mailbox fewer than needed: the full fan-out.  The cap counts due slots as well as mailboxes, so without records
+    # (max_m = len(due) >= n_cand) this pins the due-slot cap, the one the bus's due index applies before it plans
+    if n_cand > 1 or len(due) > 1:
         assert plan(masks, active, pairs, base, rec, due, K, max_m - 1, n_deliv)[0] == nat.ENOSPC
     if n_deliv:                           # one record fewer than needed
         assert plan(masks, active, pairs, base, rec, due, K, max_m, n_deliv - 1)[0] == nat.ENOSPC
