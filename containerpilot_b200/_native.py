@@ -19,12 +19,14 @@ MASK_ALL = 0x0001FFFF
 TARGET_ALL = 0xFFFFFFFF
 F_TICK, F_UNICAST = 0x1, 0x2
 CFG_LOSSLESS, CFG_DIGEST, CFG_SPARSE_TICKS, CFG_SPARSE_RECORDS = 0x1, 0x2, 0x4, 0x8
+CFG_DROP_MISSED_TICKS = 0x10
 STORE_AUTO, STORE_V4, STORE_V8, STORE_BULK = 0, 1, 2, 3
 
 OK, EINVAL, ENOMEM, ECUDA, EAGAIN, ENOSPC, ENOENT, ECLOSED, ENODEV, EORDER, ETIMEDOUT = 0, -1, -2, -3, -4, -5, -6, -7, -8, -9, -10
 PUT_STAMP, PUT_RAW, PUT_NOWAIT = 0, 1, 2
 EPHEMERAL_BIT, EPHEMERAL_SLOTS = 0x80000000, 65536
 DUE_CLOCK, DUE_ARM, DUE_ONESHOT, DUE_DISARM, DUE_UNSUB, DUE_LAUNCH = 0, 1, 2, 3, 4, 5
+DUE_CATCHUP = 6
 
 
 class Event(C.Structure):

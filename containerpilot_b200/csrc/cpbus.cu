@@ -172,6 +172,26 @@ void due_fire(DueIndex& x, std::vector<HostTimer>& tm, uint64_t w, F&& on_fire) 
   }
 }
 
+// CPBUS_CFG_DROP_MISSED_TICKS: the catch-up of a clock step to `now` in the due index, as timer_catchup_kernel does it on the
+// device.  Every live periodic slot due at d <= now whose next firing is also <= now moves to d + k * period, k = (now - d) /
+// period (below kTimerIdle: the kernel's candidates stop there too), under a new version; the slots that move are appended
+// to *moved.  Reads the buckets that begin at or before now: O(entries due by now).
+inline void due_catchup(DueIndex& x, std::vector<HostTimer>& tm, uint64_t now, std::vector<uint32_t>* moved) {
+  const uint64_t w = std::min(now, kTimerIdle - 1);
+  const size_t first = moved->size();
+  for (auto it = x.buckets.begin(); it != x.buckets.end() && it->first <= (w >> DueIndex::kDueShift); ++it)
+    for (const DueIndex::Entry& e : it->second.e) {
+      if (x.stale(e) || e.due > w) continue;
+      const HostTimer& t = tm[e.slot];
+      if (!t.oneshot && w - e.due >= t.period) moved->push_back(e.slot);
+    }
+  for (size_t i = first; i < moved->size(); i++) {   // (put may rebuild the buckets: not while they are walked)
+    HostTimer& t = tm[(*moved)[i]];
+    t.next_due += (w - t.next_due) / t.period * t.period;
+    x.put((*moved)[i], t.next_due);
+  }
+}
+
 // The subscription index of a CPBUS_CFG_SPARSE_RECORDS bus: who takes a broadcast record, by code and by exact case.
 //  * Per code: the count of subscribed mailboxes whose mask has the code's bit, and their list while the count is at most
 //    `keep`.  A code past `keep` drops its list and keeps only the count: planning ends at once on such a code (it reaches
@@ -357,6 +377,7 @@ struct HostFront {
   std::vector<size_t> oneshot_idx;        // armed one-shot timers (index into h_timers)
   uint32_t n_timers = 0;
   uint64_t min_period = UINT64_MAX;       // conservative lower bound over armed periodic timers
+  bool drop_missed = false;               // CPBUS_CFG_DROP_MISSED_TICKS: a long clock step drops missed periodic ticks
   // DebugEvents ring (events/bus.go:18-21, 24-54)
   int dbg_head = -1, dbg_tail = 0;
   cpbus_event dbg[10]{};
@@ -492,6 +513,9 @@ struct cpbus : HostFront {
   unsigned char* h_plan = nullptr; unsigned char* d_plan = nullptr; size_t plan_bytes_cap = 0;
   cudaEvent_t plan_done = nullptr;        // on copy_stream: the plan (and the batch in front of it) has reached HBM
   cudaEvent_t records_done = nullptr;     // on the bus stream: the record kernel is done with the plan
+  // CPBUS_CFG_DROP_MISSED_TICKS on a sparse bus: the slots a catch-up moves (host index), and their device copy
+  std::vector<uint32_t> catchup_slots;
+  uint32_t* d_catchup = nullptr; size_t catchup_cap = 0;
 
   // intern table (Event.Source string <-> u32)
   std::unordered_map<std::string, uint32_t> intern;
@@ -1224,12 +1248,60 @@ int publish_burst(Owner* o, const cpbus_event* ev, size_t n) {
   return CPBUS_OK;
 }
 
+// CPBUS_CFG_DROP_MISSED_TICKS: the catch-up of a clock step to `now`, after a flush to the old clock.  timer_catchup_kernel
+// runs on the bus stream behind every earlier launch: over the whole slot table of a dense bus, and over exactly the slots
+// that the due index moved (due_catchup) on a sparse one, where no slot moving means no launch.
+int catch_up(cpbus* b, uint64_t now) {
+  if (!b->K || b->n_timers == 0 || b->h_timers.empty() || b->n_next == 0) return CPBUS_OK;
+  const uint32_t* list = nullptr;
+  size_t n = (size_t)b->n_next * b->K;
+  if (b->sparse) {
+    b->catchup_slots.clear();
+    due_catchup(b->due, b->h_timers, now, &b->catchup_slots);
+    n = b->catchup_slots.size();
+    if (!n) return CPBUS_OK;
+    if (n > b->catchup_cap) {   // (behind every kernel that may still read the old list)
+      CK(cudaStreamSynchronize(b->stream));
+      cudaFree(b->d_catchup);
+      b->d_catchup = nullptr; b->catchup_cap = 0;
+      const size_t cap = std::max<size_t>(n, 1024);
+      CK(cudaMalloc((void**)&b->d_catchup, cap * sizeof(uint32_t)));
+      b->catchup_cap = cap;
+    }
+    // (pageable source: the call returns once the list has been taken, and the copy runs in stream order)
+    CK(cudaMemcpyAsync(b->d_catchup, b->catchup_slots.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice, b->stream));
+    list = b->d_catchup;
+  }
+  timer_catchup_kernel<<<(uint32_t)((n + kThreads - 1) / kThreads), kThreads, 0, b->stream>>>(b->d_timers, list, (uint32_t)n, now);
+  CK(cudaGetLastError());
+  b->st.kernel_launches++;
+  return CPBUS_OK;
+}
+
+// The group: the same catch-up on every shard that has timers (its shards are dense buses).
+int catch_up(cpbus_group* g, uint64_t now) {
+  for (cpbus* s : g->shards) {
+    if (!s->K || s->n_timers == 0) continue;
+    int rc = dev_guard(s);
+    if (rc || (rc = catch_up(s, now))) return rc;
+  }
+  return CPBUS_OK;
+}
+
 // Move the clock to now_ns.  The kernel looks at <= 32/K candidate firings per timer slot per launch: every flush window is
 // kept within that many periods of the fastest periodic timer (for a group, a stream batch never steps past a shard's window).
+// CPBUS_CFG_DROP_MISSED_TICKS: only a step longer than the shortest period can hold two firings of one timer.  On such a
+// step, what is due by the old clock is delivered on its own first (the previous step's window split keeps that flush within
+// the window; CPBUS_EAGAIN leaves the clock where it was), then every periodic timer with missed firings moves to its last
+// one, so the window split below launches at most one firing per slot.
 template <class Owner>
 int advance_clock(Owner* o, uint64_t now_ns) {
   if (now_ns < o->now) return CPBUS_EORDER;
   if (now_ns == o->now) return CPBUS_OK;
+  if (o->drop_missed && o->n_timers && o->min_period != UINT64_MAX && now_ns - o->now > o->min_period) {
+    int rc = flush_staged(o, o->now);
+    if (rc || (rc = catch_up(o, now_ns))) return rc;
+  }
   const uint64_t win = max_window(o);
   while (win != UINT64_MAX && now_ns - o->last_watermark > win) {
     o->now = o->last_watermark + win;
@@ -1335,6 +1407,13 @@ int cpbus_due_trace(const cpbus_due_op* ops, size_t n_ops, uint32_t n_slots, uin
         if ((uint64_t)op.slot * K + K > n_slots) return CPBUS_EINVAL;
         for (uint32_t k = 0; k < K; k++) { tm[op.slot * K + k].active = false; x.drop(op.slot * K + k); }
         break;
+      case CPBUS_DUE_CATCHUP: {
+        if (op.value < last) return CPBUS_EINVAL;
+        std::vector<uint32_t> moved;
+        due_catchup(x, tm, op.value, &moved);
+        clock = op.value;
+        break;
+      }
       case CPBUS_DUE_LAUNCH:
         if (op.value < last) return CPBUS_EINVAL;
         last = op.value;
@@ -1474,6 +1553,7 @@ int cpbus_create(const cpbus_config* cfg, cpbus_t** out) try {
   b->lossless = cfg->flags & CPBUS_CFG_LOSSLESS; b->use_digest = cfg->flags & CPBUS_CFG_DIGEST;
   b->sparse = cfg->flags & CPBUS_CFG_SPARSE_TICKS;
   b->sparse_records = cfg->flags & CPBUS_CFG_SPARSE_RECORDS;
+  b->drop_missed = cfg->flags & CPBUS_CFG_DROP_MISSED_TICKS;
   b->room_lb = R;
   b->store = cfg->store_path == CPBUS_STORE_AUTO ? CPBUS_STORE_V8 : (int)cfg->store_path;
   if (const char* e = getenv("CPBUS_PDL")) b->pdl = atoi(e) != 0;
@@ -1610,6 +1690,7 @@ int cpbus_destroy(cpbus_t* b) try {
   if (b->records_done) cudaEventDestroy(b->records_done);
   cudaFree(b->d_plan);
   if (b->h_plan) cudaFreeHost(b->h_plan);
+  cudaFree(b->d_catchup);
   cudaFree(b->d_drain);cudaFree(b->d_drain_idx);
   cudaFree(b->d_ready_lb); cudaFree(b->d_ready); cudaFree(b->d_ready_slot);
   if (b->h_ready_hdr) cudaFreeHost(b->h_ready_hdr);
@@ -2072,7 +2153,9 @@ static int publish_device_impl(cpbus_t* b, const void* d_events, size_t n, uint6
   return CPBUS_OK;
 }
 
+// (CPBUS_CFG_DROP_MISSED_TICKS: a device batch moves the clock by its watermark, which no cpbus_advance sees)
 int cpbus_publish_device(cpbus_t* b, const void* d_events, size_t n, uint64_t watermark_ns) try {
+  if (b && b->drop_missed) return CPBUS_EINVAL;
   return publish_device_impl(b, d_events, n, watermark_ns, false, nullptr, 0);
 } CPBUS_CATCH
 
@@ -2081,6 +2164,7 @@ int cpbus_publish_device(cpbus_t* b, const void* d_events, size_t n, uint64_t wa
 // HBM and publishes it with the batch descriptor; if the caller names the NEXT batch, that one is pulled by the
 // same launch while its stores are in flight, so the following call starts from local memory.  No collective.
 int cpbus_publish_device_staged(cpbus_t* b, const void* d_events, size_t n, uint64_t watermark_ns, const void* d_next, size_t n_next) try {
+  if (b && b->drop_missed) return CPBUS_EINVAL;
   return publish_device_impl(b, d_events, n, watermark_ns, true, d_next, n_next);
 } CPBUS_CATCH
 
@@ -2173,6 +2257,7 @@ int cpbus_stream_create(cpbus_t* b, uint32_t n_slots, uint32_t n_consumers, cpbu
   if (!b || !out || !handle || n_slots < 4 || n_consumers == 0 || n_consumers > kStreamMaxConsumers) return CPBUS_EINVAL;
   *out = nullptr;
   if (b->sparse) return CPBUS_EINVAL;   // stream launches move the clock on the device, past the host's due index
+  if (b->drop_missed) return CPBUS_EINVAL;   // ... and by watermarks that no cpbus_advance sees
   int rc = dev_guard(b); if (rc) return rc;
   cpbus_stream* st = new (std::nothrow) cpbus_stream();
   if (!st) return CPBUS_ENOMEM;
@@ -2203,7 +2288,7 @@ int cpbus_stream_create(cpbus_t* b, uint32_t n_slots, uint32_t n_consumers, cpbu
 int cpbus_stream_open(cpbus_t* b, const unsigned char handle[64], uint32_t consumer_index, cpbus_stream_t** out) try {
   if (!b || !out || !handle || consumer_index == 0 || consumer_index >= kStreamMaxConsumers) return CPBUS_EINVAL;
   *out = nullptr;
-  if (b->sparse) return CPBUS_EINVAL;
+  if (b->sparse || b->drop_missed) return CPBUS_EINVAL;
   int rc = dev_guard(b); if (rc) return rc;      // the IMPORTING device must be current: the mapping is made for it
   cpbus_stream* st = new (std::nothrow) cpbus_stream();
   if (!st) return CPBUS_ENOMEM;
@@ -2230,7 +2315,7 @@ int cpbus_stream_open(cpbus_t* b, const unsigned char handle[64], uint32_t consu
 // pointer is used directly, with peer access enabled when the consumer's bus lives on another GPU.
 int cpbus_stream_attach(cpbus_t* b, cpbus_stream_t* owner, uint32_t consumer_index, cpbus_stream_t** out) try {
   if (!b || !owner || !owner->owner || !out || consumer_index == 0 || consumer_index >= owner->n_consumers) return CPBUS_EINVAL;
-  if (b->B != owner->B || b->sparse) return CPBUS_EINVAL;
+  if (b->B != owner->B || b->sparse || b->drop_missed) return CPBUS_EINVAL;
   *out = nullptr;
   int rc = dev_guard(b); if (rc) return rc;
   if (b->device != owner->bus->device) {
@@ -3160,6 +3245,7 @@ int cpbus_group_create(const cpbus_config* cfg, const int32_t* devices, uint32_t
   if (!g) return CPBUS_ENOMEM;
   g->base = cfg->sub_id_base; g->N = cfg->n_max_subs; g->B = B; g->K = cfg->timers_per_sub;
   g->lossless = cfg->flags & CPBUS_CFG_LOSSLESS;
+  g->drop_missed = cfg->flags & CPBUS_CFG_DROP_MISSED_TICKS;   // the group catches its shards up itself (catch_up)
   g->staged.resize(B);
   auto fail = [&](int code) { cpbus_group_destroy(g); return code; };
   const uint32_t each = g->N / n_devices, extra = g->N % n_devices;   // sharding.shard_range
@@ -3167,6 +3253,7 @@ int cpbus_group_create(const cpbus_config* cfg, const int32_t* devices, uint32_t
     const uint32_t first = k * each + std::min(k, extra), count = each + (k < extra ? 1u : 0u);
     cpbus_config c = *cfg;
     c.n_max_subs = count; c.device = devices[k]; c.sub_id_base = g->base + first;
+    c.flags &= ~CPBUS_CFG_DROP_MISSED_TICKS;   // (a flagged shard would refuse the group's streams)
     cpbus* s = nullptr;
     const int rc = cpbus_create(&c, &s);
     if (rc) return fail(rc);

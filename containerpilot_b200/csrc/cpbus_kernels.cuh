@@ -1124,6 +1124,27 @@ __global__ void __launch_bounds__(kThreads) record_scatter_kernel(const RecordSc
   }
 }
 
+// CPBUS_CFG_DROP_MISSED_TICKS: the catch-up of a clock step to `now`, run after a flush to the old clock, so every firing due
+// at or before it has been delivered.  One thread per timer slot: slots[i] (a sparse bus's host index names the slots that
+// move) or slot i of the whole table (slots == nullptr).  A periodic slot due at d <= now whose next firing d + period is
+// also <= now moves k = (now - d) / period periods on, to the last firing of its grid <= now, and its ordinal `fired` counts
+// the k skipped firings (32-bit, wrapping like every tick's seq).  Due times stay below kTimerIdle, as the fan-out's
+// candidates do.  Any other slot (disarmed, one-shot, "never", not due, or one firing due) is read in its hot half only.
+__global__ void __launch_bounds__(kThreads) timer_catchup_kernel(DevTimer* __restrict__ timers, const uint32_t* __restrict__ slots,
+                                                                 uint32_t n, uint64_t now) {
+  const uint32_t i = blockIdx.x * kThreads + threadIdx.x;
+  if (i >= n) return;
+  DevTimer* tp = timers + (slots ? slots[i] : i);
+  const uint4 hot = *reinterpret_cast<const uint4*>(tp);
+  const uint64_t due = ((uint64_t)hot.y << 32) | hot.x, period = ((uint64_t)hot.w << 32) | hot.z;
+  const uint64_t w = min(now, kTimerIdle - 1);
+  if (period == 0 || due == kTimerIdle || due > w || w - due < period) return;
+  const uint64_t k = (w - due) / period;   // >= 1; due + k * period <= w < kTimerIdle
+  const uint64_t nd = due + k * period;
+  *reinterpret_cast<uint4*>(tp) = make_uint4((uint32_t)nd, (uint32_t)(nd >> 32), hot.z, hot.w);
+  tp->fired += (uint32_t)k;
+}
+
 // Lossless stream across processes: post this shard's offer word into the publisher's memory (peer mapping elsewhere).
 // Stream-ordered behind the admission pass; the release orders nothing else, it makes the word itself visible system-wide.
 __global__ void stream_offer_kernel(unsigned long long* word, unsigned long long value) {

@@ -208,18 +208,21 @@ class EventBus {   // events/bus.go:12-22
   // NewEventBus() — events/bus.go:72-88.  Clock::Virtual: time moves only through Advance() (tests);
   // Clock::Monotonic: a pump thread feeds std::chrono::steady_clock every millisecond.
   // sparse_records: CPBUS_CFG_SPARSE_RECORDS, a Publish whose events reach few mailboxes launches only over them (one bus only).
+  // drop_missed_ticks: CPBUS_CFG_DROP_MISSED_TICKS, a clock step across several periods of a timer delivers its last tick
+  // only, as Go's time.Ticker does.
   explicit EventBus(Clock clock = Clock::Monotonic, uint32_t n_max_subs = 256, uint32_t mailbox_cap = 1024,
-                    bool sparse_records = false)
-      : EventBus(std::vector<int32_t>{}, clock, n_max_subs, mailbox_cap, sparse_records) {}
+                    bool sparse_records = false, bool drop_missed_ticks = false)
+      : EventBus(std::vector<int32_t>{}, clock, n_max_subs, mailbox_cap, sparse_records, drop_missed_ticks) {}
   // The same bus on a group of shards, shard g on devices[g] (cpbus_group_create; devices may repeat).  Empty: one bus on
   // the current device.  A group refuses sparse_records (std::runtime_error).
   EventBus(const std::vector<int32_t>& devices, Clock clock, uint32_t n_max_subs = 256, uint32_t mailbox_cap = 1024,
-           bool sparse_records = false) : clock_(clock) {
+           bool sparse_records = false, bool drop_missed_ticks = false) : clock_(clock) {
     cpbus_config cfg{};
     cfg.n_max_subs = n_max_subs; cfg.ring_cap = mailbox_cap; cfg.batch_cap = mailbox_cap >= 512 ? 256 : mailbox_cap / 2;
     cfg.timers_per_sub = 4; cfg.flags = CPBUS_CFG_LOSSLESS | CPBUS_CFG_DIGEST; cfg.device = -1;
     if (devices.empty()) cfg.flags |= CPBUS_CFG_SPARSE_TICKS;   // the 1 ms pump launches only for due ticks (a group has no such mode)
     if (sparse_records) cfg.flags |= CPBUS_CFG_SPARSE_RECORDS;
+    if (drop_missed_ticks) cfg.flags |= CPBUS_CFG_DROP_MISSED_TICKS;
     batch_cap_ = cfg.batch_cap;
     drain_cap_ = std::max<size_t>(kDrainCap, mailbox_cap);
     const int rc = devices.empty() ? ::cpbus_create(&cfg, &h_.one)

@@ -121,20 +121,23 @@ class EventBus:
     """EventBus — events/bus.go:12-22.  NewEventBus() == EventBus()."""
 
     def __init__(self, n_max_subs: int = 64, ring_cap: int = 1024, batch_cap: int = 256, timers_per_sub: int = 4,
-                 lossless: bool = True, devices=None, sparse_records: bool = False, **kw):
+                 lossless: bool = True, devices=None, sparse_records: bool = False, drop_missed_ticks: bool = False, **kw):
         """`devices`: run on a group of shards, shard g on devices[g] (GroupBus); the answers are the single bus's.
         The single bus is created with sparse timer delivery (CPBUS_CFG_SPARSE_TICKS): a pump step with nothing due
         launches nothing.  A group does not take that flag.
         `sparse_records` (single bus only): CPBUS_CFG_SPARSE_RECORDS, a Publish whose events reach few mailboxes
-        launches only over them."""
+        launches only over them.
+        `drop_missed_ticks`: CPBUS_CFG_DROP_MISSED_TICKS, a clock step across several periods of a NewEventTimer delivers
+        one tick, not one per period, as the Go ticker does (timer.go; its channel holds one tick)."""
         if sparse_records and devices is not None:
             raise ValueError("sparse_records: a group of shards does not take CPBUS_CFG_SPARSE_RECORDS")
         if devices is not None:
             self._bus = GroupBus(n_max_subs, devices, ring_cap=ring_cap, batch_cap=batch_cap, timers_per_sub=timers_per_sub,
-                                 lossless=lossless, digest=True, **kw)
+                                 lossless=lossless, digest=True, drop_missed_ticks=drop_missed_ticks, **kw)
         else:
             self._bus = Bus(n_max_subs, ring_cap=ring_cap, batch_cap=batch_cap, timers_per_sub=timers_per_sub,
-                            lossless=lossless, digest=True, sparse_ticks=True, sparse_records=sparse_records, **kw)
+                            lossless=lossless, digest=True, sparse_ticks=True, sparse_records=sparse_records,
+                            drop_missed_ticks=drop_missed_ticks, **kw)
         self.reload = False
         self._done = 0              # sync.WaitGroup counter (bus.go:16)
         self._subs = {}             # Subscriber -> sub_id  (registry, bus.go:13)

@@ -29,13 +29,15 @@ class _GroupCalls:
 class GroupBus(Bus):
     def __init__(self, n_max_subs: int, devices, ring_cap: int = 1024, batch_cap: int = 256, timers_per_sub: int = 0,
                  lossless: bool = False, digest: bool = True, sub_id_base: int = 0, store_path: int = nat.STORE_AUTO,
-                 grid_ctas: int = 0):
+                 grid_ctas: int = 0, drop_missed_ticks: bool = False):
+        """`drop_missed_ticks`: CPBUS_CFG_DROP_MISSED_TICKS, as on `Bus`"""
         self._h = C.c_void_p()
         lib = nat.load()
         self._lib = _GroupCalls(lib)
         cfg = nat.Config()
         cfg.n_max_subs, cfg.ring_cap, cfg.batch_cap, cfg.timers_per_sub = n_max_subs, ring_cap, batch_cap, timers_per_sub
-        cfg.flags = (nat.CFG_LOSSLESS if lossless else 0) | (nat.CFG_DIGEST if digest else 0)
+        cfg.flags = ((nat.CFG_LOSSLESS if lossless else 0) | (nat.CFG_DIGEST if digest else 0)
+                     | (nat.CFG_DROP_MISSED_TICKS if drop_missed_ticks else 0))
         cfg.device, cfg.sub_id_base, cfg.store_path, cfg.grid_ctas = -1, sub_id_base, store_path, grid_ctas
         devs = np.ascontiguousarray(list(devices), dtype=np.int32)
         nat.check(lib.cpbus_group_create(C.byref(cfg), devs.ctypes.data, devs.size, C.byref(self._h)), "cpbus_group_create")

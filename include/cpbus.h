@@ -115,6 +115,38 @@ enum {
                                    mailbox takes anything) leaves the step result as it was.
                                    Device batches (cpbus_publish_device*) always take the
                                    full fan-out.  Not supported on a group: CPBUS_EINVAL. */
+#define CPBUS_CFG_DROP_MISSED_TICKS 0x10u /* periodic timers drop missed ticks like Go's time.Ticker
+                                   (NewEventTimer reads a ticker whose channel holds one tick,
+                                   so a late wake-up delivers one tick, not a burst).  When
+                                   cpbus_advance moves the clock from c to now, an armed periodic
+                                   timer with k >= 2 firings due in (c, now] delivers only the
+                                   last, due at d_last (the largest point of its grid <= now that
+                                   is below UINT64_MAX), and next fires at d_last + period: the
+                                   phase is kept.  The tick is the usual {seq, ts = d_last,
+                                   TimerExpired, source, owner, F_TICK}, and seq stays the
+                                   firing ordinal on the grid: the skipped firings are counted,
+                                   so a gap of g between consecutive seqs of one timer means g
+                                   ticks were dropped.  Firings due at or before c and one-shots
+                                   are unaffected.  The bus compares each step with the shortest
+                                   period armed since no timer was left armed (a lower bound: a
+                                   cancel or an unsubscribe does not raise it).  A step no longer
+                                   than that bound behaves exactly as without the flag.  A longer
+                                   step first flushes what is staged and due at c, then runs one
+                                   catch-up kernel; where it gives no timer two firings it
+                                   delivers the same records as an unflagged bus, but the flush
+                                   adds launches and, in lossless mode, may return CPBUS_EAGAIN
+                                   where an unflagged bus would not (with the clock unchanged).
+                                   The caller's step is the rule's resolution: a pump advancing
+                                   every 1 ms with periods of seconds changes nothing in steady
+                                   state.  The rule covers cpbus_advance, and cpbus_group_advance
+                                   on a group created with the flag (which gives the flagged
+                                   single bus's results).
+                                   Valid with every other flag; a flagged sparse bus gives the
+                                   results of a flagged dense twin.  Streams and device batches
+                                   move the clock by watermarks no cpbus_advance sees, so
+                                   cpbus_stream_create/_open/_attach and cpbus_publish_device
+                                   /_staged return CPBUS_EINVAL on a flagged bus (the group's own
+                                   internal streams excepted); lifting that is future work. */
 
 /* cpbus_config.store_path: how records reach the rings (all are bit-identical) */
 enum {
@@ -239,7 +271,9 @@ int cpbus_publish(cpbus_t* bus, const cpbus_event* ev, size_t n);
  * Subscriber.Receive, events/subscriber.go:30).  Ordered with publishes. */
 int cpbus_send(cpbus_t* bus, uint32_t sub_id, const cpbus_event* ev);
 /* Move the virtual clock; timers whose due time <= now_ns fire at the next flush,
- * ordered before any event published after this call. */
+ * ordered before any event published after this call.  On a CPBUS_CFG_DROP_MISSED_TICKS bus a step longer than the
+ * shortest period drops the missed ticks (see the flag); in lossless mode it may return CPBUS_EAGAIN from the flush it makes
+ * first, with the clock unchanged. */
 int cpbus_advance(cpbus_t* bus, uint64_t now_ns);
 /* Launch the fan-out for everything staged (async on the bus stream). */
 int cpbus_flush(cpbus_t* bus);
@@ -630,10 +664,14 @@ size_t cpbus_mask_order(const uint32_t* masks, const uint8_t* active, uint32_t n
  *   CPBUS_DUE_DISARM    cancel `slot`
  *   CPBUS_DUE_UNSUB     disarm the K slots of subscriber `slot`
  *   CPBUS_DUE_LAUNCH    a launch to watermark value: every armed slot due at or before it fires
+ *   CPBUS_DUE_CATCHUP   the clock becomes value, with the CPBUS_CFG_DROP_MISSED_TICKS catch-up and no firing: every
+ *                       periodic slot due at d <= value whose next firing d + period is also <= value moves to the last
+ *                       firing of its grid <= value (below UINT64_MAX); CPBUS_EINVAL when value is behind the last launch
  * Each LAUNCH appends, for every slot that fires, in ascending slot order, {launch ordinal (0-based), slot, ticks, next due
  * (UINT64_MAX: never, or a one-shot that is done)} to out; *n_out = how many entries there are (the first cap are written).
  * CPBUS_EINVAL: a slot out of range, a period of 0, K not in {1, 2, 4, 8}, or a launch behind the previous launch. */
-enum { CPBUS_DUE_CLOCK = 0, CPBUS_DUE_ARM = 1, CPBUS_DUE_ONESHOT = 2, CPBUS_DUE_DISARM = 3, CPBUS_DUE_UNSUB = 4, CPBUS_DUE_LAUNCH = 5 };
+enum { CPBUS_DUE_CLOCK = 0, CPBUS_DUE_ARM = 1, CPBUS_DUE_ONESHOT = 2, CPBUS_DUE_DISARM = 3, CPBUS_DUE_UNSUB = 4, CPBUS_DUE_LAUNCH = 5,
+       CPBUS_DUE_CATCHUP = 6 };
 typedef struct cpbus_due_op { uint32_t kind, slot; uint64_t value; } cpbus_due_op;                       /* sizeof == 16 */
 typedef struct cpbus_due_fire { uint64_t launch; uint32_t slot, pad; uint64_t ticks, next_due; } cpbus_due_fire; /* sizeof == 32 */
 int cpbus_due_trace(const cpbus_due_op* ops, size_t n_ops, uint32_t n_slots, uint32_t K, cpbus_due_fire* out, size_t cap,
