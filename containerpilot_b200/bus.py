@@ -124,6 +124,25 @@ class Bus:
     def unsubscribe(self, sub_id: int):
         nat.check(self._lib.cpbus_unsubscribe(self._h, sub_id), "cpbus_unsubscribe")
 
+    def _membership_many(self, name: str, arrays) -> np.ndarray:
+        n = arrays[0].size
+        status = np.zeros(n, dtype=np.int32)
+        nat.check(getattr(self._lib, name)(self._h, *[a.ctypes.data if n else None for a in arrays], n,
+                                           status.ctypes.data if n else None, None), name)
+        return status
+
+    def unsubscribe_many(self, sub_ids) -> np.ndarray:
+        """cpbus_unsubscribe for every id in order, in one call: the int32 status each single call would have returned
+        (OK, ENOENT or ECLOSED).  Raises on any other return, CPBUS_EAGAIN included (nothing was applied)."""
+        return self._membership_many("cpbus_unsubscribe_many", [np.ascontiguousarray(sub_ids, dtype=np.uint32)])
+
+    def set_mask_many(self, sub_ids, masks) -> np.ndarray:
+        """cpbus_set_mask(sub_ids[i], masks[i]) in order, in one call: the per-element statuses, as unsubscribe_many"""
+        ids, m = np.ascontiguousarray(sub_ids, dtype=np.uint32), np.ascontiguousarray(masks, dtype=np.uint32)
+        if ids.shape != m.shape:
+            raise ValueError("sub_ids and masks differ in length")
+        return self._membership_many("cpbus_set_mask_many", [ids, m])
+
     # -- timers ------------------------------------------------------------
     def timer_add(self, sub_id: int, period_ns: int, source_id: int, oneshot: bool = False) -> int:
         out = C.c_uint32()
@@ -139,6 +158,10 @@ class Bus:
 
     def timer_cancel(self, timer_id: int):
         nat.check(self._lib.cpbus_timer_cancel(self._h, timer_id), "cpbus_timer_cancel")
+
+    def timer_cancel_many(self, timer_ids) -> np.ndarray:
+        """cpbus_timer_cancel for every id in order, in one call: the per-element statuses (OK or ENOENT)"""
+        return self._membership_many("cpbus_timer_cancel_many", [np.ascontiguousarray(timer_ids, dtype=np.uint32)])
 
     # -- hot path ----------------------------------------------------------
     def publish(self, code: int, source_id: int = 0) -> int:

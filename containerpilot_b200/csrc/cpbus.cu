@@ -516,6 +516,8 @@ struct cpbus : HostFront {
   // CPBUS_CFG_DROP_MISSED_TICKS on a sparse bus: the slots a catch-up moves (host index), and their device copy
   std::vector<uint32_t> catchup_slots;
   uint32_t* d_catchup = nullptr; size_t catchup_cap = 0;
+  // the bulk membership calls (cpbus_unsubscribe_many, ...): device copy of the coalesced per-mailbox list, grown on demand
+  MemberOp* d_member = nullptr; size_t member_cap = 0;
 
   // intern table (Event.Source string <-> u32)
   std::unordered_map<std::string, uint32_t> intern;
@@ -1691,6 +1693,7 @@ int cpbus_destroy(cpbus_t* b) try {
   cudaFree(b->d_plan);
   if (b->h_plan) cudaFreeHost(b->h_plan);
   cudaFree(b->d_catchup);
+  cudaFree(b->d_member);
   cudaFree(b->d_drain);cudaFree(b->d_drain_idx);
   cudaFree(b->d_ready_lb); cudaFree(b->d_ready); cudaFree(b->d_ready_slot);
   if (b->h_ready_hdr) cudaFreeHost(b->h_ready_hdr);
@@ -1879,12 +1882,9 @@ int cpbus_subscribe_pairs_many(cpbus_t* b, const uint32_t* masks, const cpbus_pa
   return CPBUS_OK;
 } CPBUS_CATCH
 
-int cpbus_unsubscribe(cpbus_t* b, uint32_t sub_id) try {
-  if (!b) return CPBUS_EINVAL;
-  uint32_t l = 0;
-  if (!id_range(b->cfg.sub_id_base, b->n_next, sub_id, 1, &l)) return CPBUS_ENOENT;
-  int rc = enter(b); if (rc) return rc;
-  if ((rc = flush_staged(b, b->now))) return rc;
+// The host half of cpbus_unsubscribe, after its flush: CPBUS_ECLOSED, or the registry, the sparse indexes and the timer
+// table updated.  *clear = the timer slots whose device copies are to be disarmed: all K once the table exists.
+static int unsubscribe_host(cpbus* b, uint32_t l, uint32_t* clear) {
   // second Unsubscribe drives the WaitGroup negative in Go (events/bus.go:121) => panic
   if (!b->h_active[l]) return CPBUS_ECLOSED;
   b->h_active[l] = 0;
@@ -1895,19 +1895,44 @@ int cpbus_unsubscribe(cpbus_t* b, uint32_t sub_id) try {
     b->rec_index.remove_cases(l, b->h_active.data());
   }
   b->order_dirty = true;
-  const uint32_t word = 0;
-  CK(cudaMemcpyAsync(&b->d_ctl[l].mask, &word, 4, cudaMemcpyHostToDevice, b->stream));
+  *clear = 0;
   if (b->K && !b->h_timers.empty()) {
     for (uint32_t k = 0; k < b->K; k++) {
       timer_disarm(b, (size_t)l * b->K + k, /*reset_bound=*/false);
       if (b->sparse) b->due.drop(l * b->K + k);
     }
-    CK(cudaMemsetAsync(b->d_timers + (size_t)l * b->K, 0xFF, b->K * sizeof(DevTimer), b->stream));
+    *clear = (1u << b->K) - 1u;
   }
-  CK(cudaStreamSynchronize(b->stream));
   b->n_active--;
   return CPBUS_OK;
+}
+
+int cpbus_unsubscribe(cpbus_t* b, uint32_t sub_id) try {
+  if (!b) return CPBUS_EINVAL;
+  uint32_t l = 0, clear = 0;
+  if (!id_range(b->cfg.sub_id_base, b->n_next, sub_id, 1, &l)) return CPBUS_ENOENT;
+  int rc = enter(b); if (rc) return rc;
+  if ((rc = flush_staged(b, b->now))) return rc;
+  if ((rc = unsubscribe_host(b, l, &clear))) return rc;
+  const uint32_t word = 0;
+  CK(cudaMemcpyAsync(&b->d_ctl[l].mask, &word, 4, cudaMemcpyHostToDevice, b->stream));
+  if (clear) CK(cudaMemsetAsync(b->d_timers + (size_t)l * b->K, 0xFF, b->K * sizeof(DevTimer), b->stream));
+  CK(cudaStreamSynchronize(b->stream));
+  return CPBUS_OK;
 } CPBUS_CATCH
+
+// The host half of cpbus_set_mask, after its flush.
+static void set_mask_host(cpbus* b, uint32_t l, uint32_t mask) {
+  mask &= CPBUS_MASK_ALL;
+  if (b->h_mask[l] != CPBUS_MASK_ALL) b->n_filtered--;
+  if (mask != CPBUS_MASK_ALL) b->n_filtered++;
+  const uint32_t old = b->h_mask[l];
+  b->h_mask[l] = mask; b->order_dirty = true;
+  if (b->sparse_records) {
+    b->rec_index.add_codes(l, mask & ~old);
+    b->rec_index.remove_codes(l, old & ~mask, b->h_mask.data(), b->h_active.data());
+  }
+}
 
 // Change a subscriber's code mask in place (ordered with publishes like Subscribe): the subscriber keeps its mailbox,
 // its timers and its exact cases.  Used when a mailbox that so far only received timer ticks / direct sends (mask 0:
@@ -1919,15 +1944,7 @@ int cpbus_set_mask(cpbus_t* b, uint32_t sub_id, uint32_t mask) try {
   if (!b->h_active[l]) return CPBUS_ECLOSED;
   int rc = enter(b); if (rc) return rc;
   if ((rc = flush_staged(b, b->now))) return rc;
-  mask &= CPBUS_MASK_ALL;
-  if (b->h_mask[l] != CPBUS_MASK_ALL) b->n_filtered--;
-  if (mask != CPBUS_MASK_ALL) b->n_filtered++;
-  const uint32_t old = b->h_mask[l];
-  b->h_mask[l] = mask; b->order_dirty = true;
-  if (b->sparse_records) {
-    b->rec_index.add_codes(l, mask & ~old);
-    b->rec_index.remove_codes(l, old & ~mask, b->h_mask.data(), b->h_active.data());
-  }
+  set_mask_host(b, l, mask);
   return push_mask_words(b, l, 1);
 } CPBUS_CATCH
 
@@ -1993,22 +2010,125 @@ int cpbus_timer_add_many(cpbus_t* b, uint32_t first_sub, uint32_t n, uint64_t pe
   return push_mask_words(b, l0, n);
 } CPBUS_CATCH
 
-int cpbus_timer_cancel(cpbus_t* b, uint32_t timer_id) try {
-  if (!b) return CPBUS_EINVAL;
+// cpbus_timer_cancel's refusal before its flush (CPBUS_ENOENT: no such slot), or CPBUS_OK with the slot's mailbox and index
+static int timer_cancel_check(const cpbus* b, uint32_t timer_id, uint32_t* l, uint32_t* k) {
   if (!b->K || b->h_timers.empty()) return CPBUS_ENOENT;
-  const uint32_t slot_index = timer_id & kTimerSlotMask, gen = timer_id >> kTimerSlotBits;
-  const uint32_t l = slot_index / b->K, k = slot_index % b->K;
-  if (l >= b->n_next) return CPBUS_ENOENT;
-  int rc = enter(b); if (rc) return rc;
-  if ((rc = flush_staged(b, b->now))) return rc;   // firings due before the cancel still happen
-  retire_oneshots(b, b->last_watermark);
+  const uint32_t slot_index = timer_id & kTimerSlotMask;
+  *l = slot_index / b->K; *k = slot_index % b->K;
+  return *l < b->n_next ? CPBUS_OK : CPBUS_ENOENT;
+}
+
+// The host half of cpbus_timer_cancel, after its flush and the one-shots' retirement.
+static int timer_cancel_host(cpbus* b, uint32_t timer_id, uint32_t l, uint32_t k) {
   const HostTimer& t = b->h_timers[(size_t)l * b->K + k];
-  if (!t.active || t.gen != gen) return CPBUS_ENOENT;   // already fired / cancelled, or the slot has been re-armed since
+  if (!t.active || t.gen != timer_id >> kTimerSlotBits) return CPBUS_ENOENT;   // already fired / cancelled, or the slot has been re-armed since
   timer_disarm(b, (size_t)l * b->K + k, /*reset_bound=*/true);
   if (b->sparse) b->due.drop(l * b->K + k);
+  return CPBUS_OK;
+}
+
+int cpbus_timer_cancel(cpbus_t* b, uint32_t timer_id) try {
+  if (!b) return CPBUS_EINVAL;
+  uint32_t l = 0, k = 0;
+  int rc = timer_cancel_check(b, timer_id, &l, &k); if (rc) return rc;
+  if ((rc = enter(b))) return rc;
+  if ((rc = flush_staged(b, b->now))) return rc;   // firings due before the cancel still happen
+  retire_oneshots(b, b->last_watermark);
+  if ((rc = timer_cancel_host(b, timer_id, l, k))) return rc;
   CK(cudaMemsetAsync(b->d_timers + (size_t)l * b->K + k, 0xFF, sizeof(DevTimer), b->stream));
   CK(cudaStreamSynchronize(b->stream));
   return push_mask_words(b, l, 1);
+} CPBUS_CATCH
+
+// The bulk membership calls (cpbus_unsubscribe_many, cpbus_set_mask_many, cpbus_timer_cancel_many): each element as its
+// single call would apply it, in array order.  check(i) is element i's refusal before the single call's flush (CPBUS_OK:
+// none); the flush runs once, where the first element that passes its check would run it, then after_flush(), then
+// apply(i, &l, &clear) for each element that passed: CPBUS_OK with its mailbox l and the timer slots it disarms, or its
+// refusal.  The flush's CPBUS_EAGAIN (or an error) is returned with nothing applied and status / applied not written.
+// Every mailbox an applied element touched then gets one membership_kernel entry with its final mask word: one H2D copy,
+// one launch and one synchronisation, where the single calls take one synchronised round trip each.
+extern "C++" {
+template <class Check, class AfterFlush, class Apply>
+static int membership_many(cpbus* b, uint32_t n, int* status, uint32_t* applied, Check&& check, AfterFlush&& after_flush,
+                           Apply&& apply) {
+  std::vector<int> st(n);
+  bool any = false;
+  for (uint32_t i = 0; i < n; i++) any |= (st[i] = check(i)) == CPBUS_OK;
+  std::vector<uint64_t> touched;   // mailbox << 32 | timer slots disarmed, one per applied element
+  if (any) {
+    int rc = enter(b); if (rc) return rc;
+    if ((rc = flush_staged(b, b->now))) return rc;
+    after_flush();
+    for (uint32_t i = 0; i < n; i++) {
+      if (st[i] != CPBUS_OK) continue;
+      uint32_t l = 0, clear = 0;
+      if ((st[i] = apply(i, &l, &clear)) == CPBUS_OK) touched.push_back((uint64_t)l << 32 | clear);
+    }
+  }
+  if (!touched.empty()) {
+    std::sort(touched.begin(), touched.end());
+    std::vector<MemberOp> ops;
+    for (uint64_t t : touched) {
+      const uint32_t l = (uint32_t)(t >> 32);
+      if (ops.empty() || ops.back().local != l) ops.push_back(MemberOp{l, 0u, 0u, 0u});
+      ops.back().clear_slots |= (uint32_t)t;
+    }
+    for (MemberOp& op : ops) op.mask_word = mask_word(b, op.local);
+    if (ops.size() > b->member_cap) {   // (every bulk call ends in a synchronisation: no kernel reads the old list)
+      cudaFree(b->d_member);
+      b->d_member = nullptr; b->member_cap = 0;
+      const size_t cap = std::max<size_t>(ops.size(), 1024);
+      CK(cudaMalloc((void**)&b->d_member, cap * sizeof(MemberOp)));
+      b->member_cap = cap;
+    }
+    // (pageable source: the call returns once the list has been taken, and the copy runs in stream order)
+    CK(cudaMemcpyAsync(b->d_member, ops.data(), ops.size() * sizeof(MemberOp), cudaMemcpyHostToDevice, b->stream));
+    membership_kernel<<<(uint32_t)((ops.size() + kThreads - 1) / kThreads), kThreads, 0, b->stream>>>(
+        b->d_ctl, b->d_timers, b->d_member, (uint32_t)ops.size(), b->K);
+    CK(cudaGetLastError());
+    b->st.kernel_launches++;
+    CK(cudaStreamSynchronize(b->stream));
+  }
+  uint32_t ok = 0;
+  for (uint32_t i = 0; i < n; i++) ok += st[i] == CPBUS_OK ? 1u : 0u;
+  if (status && n) memcpy(status, st.data(), (size_t)n * sizeof(int));
+  if (applied) *applied = ok;
+  return CPBUS_OK;
+}
+}
+
+int cpbus_unsubscribe_many(cpbus_t* b, const uint32_t* sub_ids, uint32_t n, int* status, uint32_t* applied) try {
+  if (!b || (!sub_ids && n)) return CPBUS_EINVAL;
+  return membership_many(b, n, status, applied,
+      [&](uint32_t i) { uint32_t l; return id_range(b->cfg.sub_id_base, b->n_next, sub_ids[i], 1, &l) ? CPBUS_OK : CPBUS_ENOENT; },
+      [] {},
+      [&](uint32_t i, uint32_t* l, uint32_t* clear) { *l = sub_ids[i] - b->cfg.sub_id_base; return unsubscribe_host(b, *l, clear); });
+} CPBUS_CATCH
+
+int cpbus_set_mask_many(cpbus_t* b, const uint32_t* sub_ids, const uint32_t* code_masks, uint32_t n, int* status,
+                        uint32_t* applied) try {
+  if (!b || ((!sub_ids || !code_masks) && n)) return CPBUS_EINVAL;
+  return membership_many(b, n, status, applied,
+      [&](uint32_t i) {
+        uint32_t l = 0;
+        if (!id_range(b->cfg.sub_id_base, b->n_next, sub_ids[i], 1, &l)) return CPBUS_ENOENT;
+        return b->h_active[l] ? CPBUS_OK : CPBUS_ECLOSED;
+      },
+      [] {},
+      [&](uint32_t i, uint32_t* l, uint32_t*) { *l = sub_ids[i] - b->cfg.sub_id_base; set_mask_host(b, *l, code_masks[i]); return CPBUS_OK; });
+} CPBUS_CATCH
+
+int cpbus_timer_cancel_many(cpbus_t* b, const uint32_t* timer_ids, uint32_t n, int* status, uint32_t* applied) try {
+  if (!b || (!timer_ids && n)) return CPBUS_EINVAL;
+  return membership_many(b, n, status, applied,
+      [&](uint32_t i) { uint32_t l, k; return timer_cancel_check(b, timer_ids[i], &l, &k); },
+      [&] { retire_oneshots(b, b->last_watermark); },
+      [&](uint32_t i, uint32_t* l, uint32_t* clear) {
+        uint32_t k = 0;
+        timer_cancel_check(b, timer_ids[i], l, &k);
+        *clear = 1u << k;
+        return timer_cancel_host(b, timer_ids[i], *l, k);
+      });
 } CPBUS_CATCH
 
 int cpbus_publish(cpbus_t* b, const cpbus_event* ev, size_t n) try {
@@ -3452,6 +3572,112 @@ int cpbus_group_timer_cancel(cpbus_group_t* g, uint32_t timer_id) try {
   if ((rc = cpbus_timer_cancel(g->shards[k], local))) return rc;
   timer_disarm(g, slot, /*reset_bound=*/true);
   return CPBUS_OK;
+} CPBUS_CATCH
+
+// The group's bulk membership calls: the single group calls' loop.  check(i, &k) is element i's refusal before the group's
+// flush (CPBUS_OK: none, and k = its shard); the group flushes once, where the first element that passes would, then
+// after_flush(); then each shard with work takes its elements, in array order, in one call of the shard's bulk call:
+// run(k, elements, their statuses), which also keeps the group's own records of the elements the shard applied.  Shards
+// are independent, and the group's records of these calls (n_active, n_timers, min_period) end where the interleaved loop
+// leaves them.
+extern "C++" {
+template <class Check, class AfterFlush, class Run>
+static int group_membership_many(cpbus_group* g, uint32_t n, int* status, uint32_t* applied, Check&& check,
+                                 AfterFlush&& after_flush, Run&& run) {
+  std::vector<int> st(n);
+  std::vector<std::vector<uint32_t>> work(g->shards.size());
+  bool any = false;
+  for (uint32_t i = 0; i < n; i++) {
+    uint32_t k = 0;
+    if ((st[i] = check(i, &k)) == CPBUS_OK) { work[k].push_back(i); any = true; }
+  }
+  if (any) {
+    int rc = flush_staged(g, g->now); if (rc) return rc;
+    after_flush();
+    std::vector<int> st_k;
+    for (uint32_t k = 0; k < g->shards.size(); k++) {
+      if (work[k].empty()) continue;
+      st_k.assign(work[k].size(), CPBUS_OK);
+      if ((rc = run(k, work[k], st_k.data()))) return rc;
+      for (size_t j = 0; j < work[k].size(); j++) st[work[k][j]] = st_k[j];
+    }
+  }
+  uint32_t ok = 0;
+  for (uint32_t i = 0; i < n; i++) ok += st[i] == CPBUS_OK ? 1u : 0u;
+  if (status && n) memcpy(status, st.data(), (size_t)n * sizeof(int));
+  if (applied) *applied = ok;
+  return CPBUS_OK;
+}
+}
+
+int cpbus_group_unsubscribe_many(cpbus_group_t* g, const uint32_t* sub_ids, uint32_t n, int* status, uint32_t* applied) try {
+  if (!g || (!sub_ids && n)) return CPBUS_EINVAL;
+  std::vector<uint32_t> ids;
+  return group_membership_many(g, n, status, applied,
+      [&](uint32_t i, uint32_t* k) {
+        cpbus* s = nullptr; uint32_t l = 0;
+        if (!group_locate(g, sub_ids[i], &s, &l)) return CPBUS_ENOENT;
+        *k = group_shard_of(g, sub_ids[i] - g->base);
+        return CPBUS_OK;
+      },
+      [] {},
+      [&](uint32_t k, const std::vector<uint32_t>& el, int* st) -> int {
+        ids.resize(el.size());
+        for (size_t j = 0; j < el.size(); j++) ids[j] = sub_ids[el[j]];
+        const int rc = cpbus_unsubscribe_many(g->shards[k], ids.data(), (uint32_t)ids.size(), st, nullptr);
+        if (rc) return rc;
+        for (size_t j = 0; j < el.size(); j++) {
+          if (st[j] != CPBUS_OK) continue;
+          if (g->K && !g->h_timers.empty())
+            for (uint32_t t = 0; t < g->K; t++) timer_disarm(g, (size_t)(ids[j] - g->base) * g->K + t, /*reset_bound=*/false);
+          g->n_active--;
+        }
+        return CPBUS_OK;
+      });
+} CPBUS_CATCH
+
+int cpbus_group_set_mask_many(cpbus_group_t* g, const uint32_t* sub_ids, const uint32_t* code_masks, uint32_t n, int* status,
+                              uint32_t* applied) try {
+  if (!g || ((!sub_ids || !code_masks) && n)) return CPBUS_EINVAL;
+  std::vector<uint32_t> ids, masks;
+  return group_membership_many(g, n, status, applied,
+      [&](uint32_t i, uint32_t* k) {
+        cpbus* s = nullptr; uint32_t l = 0;
+        if (!group_locate(g, sub_ids[i], &s, &l)) return CPBUS_ENOENT;
+        if (!s->h_active[l]) return CPBUS_ECLOSED;
+        *k = group_shard_of(g, sub_ids[i] - g->base);
+        return CPBUS_OK;
+      },
+      [] {},
+      [&](uint32_t k, const std::vector<uint32_t>& el, int* st) -> int {
+        ids.resize(el.size()); masks.resize(el.size());
+        for (size_t j = 0; j < el.size(); j++) { ids[j] = sub_ids[el[j]]; masks[j] = code_masks[el[j]]; }
+        return cpbus_set_mask_many(g->shards[k], ids.data(), masks.data(), (uint32_t)ids.size(), st, nullptr);
+      });
+} CPBUS_CATCH
+
+int cpbus_group_timer_cancel_many(cpbus_group_t* g, const uint32_t* timer_ids, uint32_t n, int* status, uint32_t* applied) try {
+  if (!g || (!timer_ids && n)) return CPBUS_EINVAL;
+  std::vector<uint32_t> ids;
+  return group_membership_many(g, n, status, applied,
+      [&](uint32_t i, uint32_t* k) {
+        if (!g->K || g->h_timers.empty()) return CPBUS_ENOENT;
+        const uint32_t slot = timer_ids[i] & kTimerSlotMask;
+        if (slot / g->K >= g->n_next) return CPBUS_ENOENT;
+        *k = group_shard_of(g, slot / g->K);
+        return CPBUS_OK;
+      },
+      [&] { group_retire(g); },
+      [&](uint32_t k, const std::vector<uint32_t>& el, int* st) -> int {
+        ids.resize(el.size());   // the shard's own timer ids, as cpbus_group_timer_cancel maps them
+        for (size_t j = 0; j < el.size(); j++)
+          ids[j] = ((timer_ids[el[j]] & kTimerSlotMask) - g->first[k] * g->K) | (timer_ids[el[j]] & ~kTimerSlotMask);
+        const int rc = cpbus_timer_cancel_many(g->shards[k], ids.data(), (uint32_t)ids.size(), st, nullptr);
+        if (rc) return rc;
+        for (size_t j = 0; j < el.size(); j++)
+          if (st[j] == CPBUS_OK) timer_disarm(g, timer_ids[el[j]] & kTimerSlotMask, /*reset_bound=*/true);
+        return CPBUS_OK;
+      });
 } CPBUS_CATCH
 
 int cpbus_group_publish(cpbus_group_t* g, const cpbus_event* ev, size_t n) try {

@@ -1145,6 +1145,31 @@ __global__ void __launch_bounds__(kThreads) timer_catchup_kernel(DevTimer* __res
   tp->fired += (uint32_t)k;
 }
 
+// The bulk membership calls (cpbus_unsubscribe_many, cpbus_set_mask_many, cpbus_timer_cancel_many): one entry per mailbox,
+// its final state after the call.  The host coalesces every element that touches a mailbox into one entry, so no two threads
+// write one mailbox.
+struct __align__(16) MemberOp {
+  uint32_t local;        // mailbox (shard-local index)
+  uint32_t mask_word;    // its control block's mask word, as mask_word() leaves it
+  uint32_t clear_slots;  // bit k: timer slot k is disarmed (every byte 0xFF, as cpbus_create leaves an idle slot)
+  uint32_t pad;
+};
+
+// One thread per entry: the mask word, then the cleared timer slots.  The ring, tail, head and digest are not touched.
+__global__ void __launch_bounds__(kThreads) membership_kernel(SubCtl* __restrict__ ctl, DevTimer* __restrict__ timers,
+                                                              const MemberOp* __restrict__ ops, uint32_t n, uint32_t K) {
+  const uint32_t i = blockIdx.x * kThreads + threadIdx.x;
+  if (i >= n) return;
+  const MemberOp op = ops[i];
+  ctl[op.local].mask = op.mask_word;
+  const uint4 idle = make_uint4(~0u, ~0u, ~0u, ~0u);
+  for (uint32_t k = 0; k < K; k++)
+    if ((op.clear_slots >> k) & 1u) {
+      uint4* tp = reinterpret_cast<uint4*>(timers + (size_t)op.local * K + k);
+      tp[0] = idle; tp[1] = idle;
+    }
+}
+
 // Lossless stream across processes: post this shard's offer word into the publisher's memory (peer mapping elsewhere).
 // Stream-ordered behind the admission pass; the release orders nothing else, it makes the word itself visible system-wide.
 __global__ void stream_offer_kernel(unsigned long long* word, unsigned long long value) {

@@ -192,7 +192,7 @@ EVENTS_CPBUS_CALL(subscribe) EVENTS_CPBUS_CALL(subscribe_pairs) EVENTS_CPBUS_CAL
 EVENTS_CPBUS_CALL(publish) EVENTS_CPBUS_CALL(send) EVENTS_CPBUS_CALL(advance) EVENTS_CPBUS_CALL(flush)
 EVENTS_CPBUS_CALL(timer_add) EVENTS_CPBUS_CALL(timer_cancel) EVENTS_CPBUS_CALL(drain) EVENTS_CPBUS_CALL(drain_ready)
 EVENTS_CPBUS_CALL(debug_events) EVENTS_CPBUS_CALL(intern) EVENTS_CPBUS_CALL(intern_ephemeral) EVENTS_CPBUS_CALL(source)
-EVENTS_CPBUS_CALL(lagging) EVENTS_CPBUS_CALL(blockers)
+EVENTS_CPBUS_CALL(lagging) EVENTS_CPBUS_CALL(blockers) EVENTS_CPBUS_CALL(unsubscribe_many)
 #undef EVENTS_CPBUS_CALL
 
 namespace detail {
@@ -304,6 +304,42 @@ class EventBus {   // events/bus.go:12-22
       sub->id_ = UINT32_MAX;
     }
     done_.Done();   // negative counter => panic, as sync.WaitGroup does (bus.go:121)
+  }
+
+  // Unsubscribe for every subscriber in order, with one cpbus_unsubscribe_many for the whole list (tearing down a job group:
+  // one flush and one launch instead of a synchronised round trip per subscriber).  What was published before reaches
+  // each Rx, as with Unsubscribe.  The WaitGroup is counted down once per entry after the bus call, so a negative counter
+  // panics there, with every listed subscriber already unsubscribed.
+  void UnsubscribeMany(const std::vector<EventSubscriber*>& subscribers) {
+    std::lock_guard<std::recursive_mutex> l(lock_);
+    std::vector<Subscriber*> subs;
+    std::vector<uint32_t> ids;
+    for (EventSubscriber* s : subscribers) {
+      auto* sub = dynamic_cast<Subscriber*>(s);
+      if (!sub) throw Panic("interface conversion: EventSubscriber is not *Subscriber");
+      subs.push_back(sub);
+    }
+    FlushLocked();
+    for (Subscriber* sub : subs) {
+      auto it = registry_.find(sub);
+      if (it == registry_.end() || std::find(ids.begin(), ids.end(), it->second) != ids.end()) continue;
+      DrainOne(sub, /*blocking=*/false);
+      ids.push_back(it->second);
+    }
+    if (!ids.empty()) {
+      Retry([&] { return cpbus_unsubscribe_many(h_, ids.data(), (uint32_t)ids.size(), (int*)nullptr, (uint32_t*)nullptr); },
+            "cpbus_unsubscribe_many");
+      for (Subscriber* sub : subs) {
+        auto it = registry_.find(sub);
+        if (it == registry_.end()) continue;
+        by_id_.erase(it->second);
+        pending_subs_.erase(sub);
+        registry_.erase(it);
+        if (sub->Rx) detail::RxRegistry().erase(sub->Rx.get());
+        sub->id_ = UINT32_MAX;
+      }
+    }
+    for (size_t i = 0; i < subs.size(); i++) done_.Done();
   }
 
   void Publish(const Event& event) {   // bus.go:125-140

@@ -254,6 +254,26 @@ int cpbus_timer_add(cpbus_t* bus, uint32_t sub_id, uint64_t period_ns, uint32_t 
 int cpbus_timer_add_many(cpbus_t* bus, uint32_t first_sub, uint32_t n, uint64_t period_ns, const uint32_t* source_ids, uint32_t source_id0, int oneshot);
 int cpbus_timer_cancel(cpbus_t* bus, uint32_t timer_id);
 
+/* ---- bulk membership changes: cpbus_unsubscribe / cpbus_set_mask / cpbus_timer_cancel for many ids in one call.
+ * Each element is applied exactly as the single call would apply it, in array order, and the call goes on past an element
+ * the single call would refuse without touching anything (CPBUS_ENOENT, CPBUS_ECLOSED).  status[i] (status may be NULL) =
+ * what the single call would have returned for element i at its turn; *applied (may be NULL) = how many returned CPBUS_OK.
+ * Loop equivalence: a bus that calls cpbus_X_many(ids, n) and a twin that calls cpbus_X(ids[i]) for i = 0 .. n-1 give the
+ * same results afterwards (every later return code, drain, drain_ready, peek_window, digest, fold, lagging, blockers,
+ * debug event and publish count, and every cpbus_stats field but batches, kernel_launches, admit_* and device_splits).  So:
+ *  - an id listed twice acts twice: unsubscribe gives CPBUS_OK then CPBUS_ECLOSED; set_mask keeps the last mask; a timer
+ *    id is cancelled once, and its second entry gets CPBUS_ENOENT;
+ *  - ordered with publishes: one flush of the staged events runs first, where the first element that gets past its
+ *    single call's up-front checks would run it (none gets past them: no flush).  In lossless mode its CPBUS_EAGAIN is
+ *    returned with nothing applied, and status / applied are not written;
+ *  - CPBUS_EINVAL (checked first): bus NULL, or an array NULL with n > 0.  n == 0: CPBUS_OK, the bus is not read.
+ * The device work is one H2D copy of one entry per mailbox touched, one kernel launch and one stream synchronisation (none
+ * when nothing is applied), instead of a synchronised round trip per id.  code_masks[i] goes with sub_ids[i]. ---- */
+int cpbus_unsubscribe_many(cpbus_t* bus, const uint32_t* sub_ids, uint32_t n, int* status, uint32_t* applied);
+int cpbus_set_mask_many(cpbus_t* bus, const uint32_t* sub_ids, const uint32_t* code_masks, uint32_t n, int* status,
+                        uint32_t* applied);
+int cpbus_timer_cancel_many(cpbus_t* bus, const uint32_t* timer_ids, uint32_t n, int* status, uint32_t* applied);
+
 /* ---- the hot path: EventBus.Publish (events/bus.go:125-140) ---- */
 /* Stages n events; only code/source_id are read from ev (seq, ts, target, flags
  * are stamped by the bus).  Flushes automatically whenever batch_cap is reached.
@@ -609,6 +629,11 @@ int cpbus_group_timer_add(cpbus_group_t* g, uint32_t sub_id, uint64_t period_ns,
 int cpbus_group_timer_add_many(cpbus_group_t* g, uint32_t first_sub, uint32_t n, uint64_t period_ns, const uint32_t* source_ids,
                                uint32_t source_id0, int oneshot);
 int cpbus_group_timer_cancel(cpbus_group_t* g, uint32_t timer_id);
+/* the bulk membership calls: each shard with work takes its ids, in array order, in one call of the shard's bulk call */
+int cpbus_group_unsubscribe_many(cpbus_group_t* g, const uint32_t* sub_ids, uint32_t n, int* status, uint32_t* applied);
+int cpbus_group_set_mask_many(cpbus_group_t* g, const uint32_t* sub_ids, const uint32_t* code_masks, uint32_t n, int* status,
+                              uint32_t* applied);
+int cpbus_group_timer_cancel_many(cpbus_group_t* g, const uint32_t* timer_ids, uint32_t n, int* status, uint32_t* applied);
 int cpbus_group_publish(cpbus_group_t* g, const cpbus_event* ev, size_t n);
 int cpbus_group_send(cpbus_group_t* g, uint32_t sub_id, const cpbus_event* ev);
 int cpbus_group_advance(cpbus_group_t* g, uint64_t now_ns);
