@@ -79,6 +79,9 @@ assert DUE_OP_DTYPE.itemsize == 16 and DUE_FIRE_DTYPE.itemsize == 32
 # cpbus_plan_entry: one mailbox of cpbus_sparse_plan's plan
 PLAN_ENTRY_DTYPE = np.dtype([("local", "<u4"), ("due_bits", "<u4"), ("first", "<u4"), ("count", "<u4")])
 assert PLAN_ENTRY_DTYPE.itemsize == 16
+# cpbus_timer_spec: one timer of cpbus_timer_add_list's list
+TIMER_SPEC_DTYPE = np.dtype([("period_ns", "<u8"), ("sub_id", "<u4"), ("source_id", "<u4"), ("oneshot", "<u4"), ("pad", "<u4")])
+assert TIMER_SPEC_DTYPE.itemsize == 24
 
 # every symbol include/cpbus.h declares: (restype, argtypes)
 _P = C.POINTER
@@ -100,6 +103,7 @@ SYMBOLS = {
     "cpbus_unsubscribe_many": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, _P(C.c_uint32)]),
     "cpbus_set_mask_many": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, _P(C.c_uint32)]),
     "cpbus_timer_cancel_many": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, _P(C.c_uint32)]),
+    "cpbus_timer_add_list": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, _P(C.c_uint32)]),
     "cpbus_publish": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
     "cpbus_send": (C.c_int, [C.c_void_p, C.c_uint32, _P(Event)]),
     "cpbus_advance": (C.c_int, [C.c_void_p, C.c_uint64]),
@@ -163,7 +167,7 @@ SYMBOLS = {
 # the group (one handle over several shards): cpbus_group_<name> takes the arguments of cpbus_<name>
 GROUP_CALLS = ("intern", "intern_ephemeral", "source", "subscribe", "subscribe_many", "subscribe_pairs", "subscribe_pairs_many",
                "unsubscribe", "set_mask", "timer_add", "timer_add_many", "timer_cancel", "unsubscribe_many", "set_mask_many",
-               "timer_cancel_many", "publish", "send", "advance", "flush",
+               "timer_cancel_many", "timer_add_list", "publish", "send", "advance", "flush",
                "sync", "drain", "drain_ready", "lagging", "blockers", "consume_all", "peek_window", "digest", "digest_fold",
                "debug_events", "stats", "publish_counts")
 SYMBOLS["cpbus_group_create"] = (C.c_int, [_P(Config), C.c_void_p, C.c_uint32, _P(C.c_void_p)])

@@ -156,6 +156,23 @@ class Bus:
             ptr = arr.ctypes.data
         nat.check(self._lib.cpbus_timer_add_many(self._h, first_sub, n, period_ns, ptr, source_id0, int(oneshot)), "cpbus_timer_add_many")
 
+    def timer_add_list(self, sub_ids, periods_ns, source_ids, oneshot=False) -> tuple[np.ndarray, np.ndarray]:
+        """cpbus_timer_add(sub_ids[i], periods_ns[i], source_ids[i], oneshot[i]) in order, in one call: (timer_ids, status),
+        the uint32 id of each armed timer (0 where status[i] is not OK) and the int32 status each single call would have
+        returned.  `oneshot` is one flag for every timer or one per timer.  Raises on any other return, CPBUS_EAGAIN
+        included (nothing was applied)."""
+        ids = np.ascontiguousarray(sub_ids, dtype=np.uint32)
+        n = ids.size
+        specs = np.zeros(n, dtype=nat.TIMER_SPEC_DTYPE)
+        specs["sub_id"] = ids
+        specs["period_ns"] = np.asarray(periods_ns, dtype=np.uint64)
+        specs["source_id"] = np.asarray(source_ids, dtype=np.uint32)
+        specs["oneshot"] = np.asarray(oneshot, dtype=bool)
+        timer_ids, status = np.zeros(n, dtype=np.uint32), np.zeros(n, dtype=np.int32)
+        ptrs = [a.ctypes.data if n else None for a in (specs, timer_ids, status)]
+        nat.check(self._lib.cpbus_timer_add_list(self._h, ptrs[0], n, ptrs[1], ptrs[2], None), "cpbus_timer_add_list")
+        return timer_ids, status
+
     def timer_cancel(self, timer_id: int):
         nat.check(self._lib.cpbus_timer_cancel(self._h, timer_id), "cpbus_timer_cancel")
 

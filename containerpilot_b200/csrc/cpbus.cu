@@ -518,6 +518,8 @@ struct cpbus : HostFront {
   uint32_t* d_catchup = nullptr; size_t catchup_cap = 0;
   // the bulk membership calls (cpbus_unsubscribe_many, ...): device copy of the coalesced per-mailbox list, grown on demand
   MemberOp* d_member = nullptr; size_t member_cap = 0;
+  // cpbus_timer_add_list: device copy of the armed slots' list, grown on demand
+  TimerArmOp* d_arm = nullptr; size_t arm_cap = 0;
 
   // intern table (Event.Source string <-> u32)
   std::unordered_map<std::string, uint32_t> intern;
@@ -1694,6 +1696,7 @@ int cpbus_destroy(cpbus_t* b) try {
   if (b->h_plan) cudaFreeHost(b->h_plan);
   cudaFree(b->d_catchup);
   cudaFree(b->d_member);
+  cudaFree(b->d_arm);
   cudaFree(b->d_drain);cudaFree(b->d_drain_idx);
   cudaFree(b->d_ready_lb); cudaFree(b->d_ready); cudaFree(b->d_ready_slot);
   if (b->h_ready_hdr) cudaFreeHost(b->h_ready_hdr);
@@ -2129,6 +2132,75 @@ int cpbus_timer_cancel_many(cpbus_t* b, const uint32_t* timer_ids, uint32_t n, i
         *clear = 1u << k;
         return timer_cancel_host(b, timer_ids[i], *l, k);
       });
+} CPBUS_CATCH
+
+static_assert(sizeof(cpbus_timer_spec) == 24, "cpbus_timer_spec is part of the ABI");
+static_assert(sizeof(TimerArmOp) == 32, "timer_arm_kernel reads an entry as two 16-byte words");
+
+// cpbus_timer_add's refusals before its flush: CPBUS_EINVAL, CPBUS_ENOSPC (no timer slots at all), CPBUS_ENOENT
+static int timer_add_check(const cpbus* b, const cpbus_timer_spec& s) {
+  if (!s.period_ns) return CPBUS_EINVAL;
+  if (!b->K) return CPBUS_ENOSPC;
+  uint32_t l = 0;
+  return id_range(b->cfg.sub_id_base, b->n_next, s.sub_id, 1, &l) ? CPBUS_OK : CPBUS_ENOENT;
+}
+
+// cpbus_timer_add for each element in array order, with one flush and one timer_arm_kernel launch: each applied element
+// arms the host table (and the due index) as the single call does, and its slot gets one entry carrying its DevTimer image
+// and the mailbox's final mask word.
+int cpbus_timer_add_list(cpbus_t* b, const cpbus_timer_spec* specs, uint32_t n, uint32_t* timer_ids, int* status,
+                         uint32_t* applied) try {
+  if (!b || (!specs && n)) return CPBUS_EINVAL;
+  std::vector<int> st(n);
+  std::vector<uint32_t> ids(n);
+  bool any = false;
+  for (uint32_t i = 0; i < n; i++) any |= (st[i] = timer_add_check(b, specs[i])) == CPBUS_OK;
+  std::vector<TimerArmOp> ops;
+  if (any) {
+    int rc = enter(b); if (rc) return rc;
+    if ((rc = flush_staged(b, b->now))) return rc;
+    if (b->h_timers.empty()) timer_table(b);
+    // Once for the whole list, where the loop retires before every element: a one-shot armed here is due after the clock,
+    // which no launched watermark passes, so the loop would retire none of this call's own one-shots between elements.
+    retire_oneshots(b, b->last_watermark);
+    for (uint32_t i = 0; i < n; i++) {
+      if (st[i] != CPBUS_OK) continue;
+      const cpbus_timer_spec& s = specs[i];
+      const uint32_t l = s.sub_id - b->cfg.sub_id_base;
+      if (!b->h_active[l]) { st[i] = CPBUS_ECLOSED; continue; }
+      uint32_t k = 0;
+      while (k < b->K && b->h_timers[(size_t)l * b->K + k].active) k++;
+      if (k == b->K) { st[i] = CPBUS_ENOSPC; continue; }
+      const uint32_t slot = l * b->K + k;
+      HostTimer& t = timer_arm(b, slot, s.period_ns, s.source_id, s.oneshot != 0);
+      if (b->sparse) b->due.put(slot, t.next_due);
+      t.gen = (uint8_t)((t.gen + 1) & 0x3F);
+      ids[i] = slot | ((uint32_t)t.gen << kTimerSlotBits);
+      ops.push_back(TimerArmOp{t.next_due, s.oneshot ? 0 : s.period_ns, s.source_id, slot, l, 0u});
+    }
+  }
+  if (!ops.empty()) {
+    for (TimerArmOp& op : ops) op.mask_word = mask_word(b, op.local);
+    if (ops.size() > b->arm_cap) {   // (every list call ends in a synchronisation: no kernel reads the old list)
+      cudaFree(b->d_arm);
+      b->d_arm = nullptr; b->arm_cap = 0;
+      const size_t cap = std::max<size_t>(ops.size(), 1024);
+      CK(cudaMalloc((void**)&b->d_arm, cap * sizeof(TimerArmOp)));
+      b->arm_cap = cap;
+    }
+    // (pageable source: the call returns once the list has been taken, and the copy runs in stream order)
+    CK(cudaMemcpyAsync(b->d_arm, ops.data(), ops.size() * sizeof(TimerArmOp), cudaMemcpyHostToDevice, b->stream));
+    timer_arm_kernel<<<(uint32_t)((ops.size() + kThreads - 1) / kThreads), kThreads, 0, b->stream>>>(
+        b->d_ctl, b->d_timers, b->d_arm, (uint32_t)ops.size());
+    CK(cudaGetLastError());
+    b->st.kernel_launches++;
+    CK(cudaStreamSynchronize(b->stream));
+  }
+  if (timer_ids)
+    for (uint32_t i = 0; i < n; i++) if (st[i] == CPBUS_OK) timer_ids[i] = ids[i];
+  if (status && n) memcpy(status, st.data(), (size_t)n * sizeof(int));
+  if (applied) *applied = (uint32_t)ops.size();
+  return CPBUS_OK;
 } CPBUS_CATCH
 
 int cpbus_publish(cpbus_t* b, const cpbus_event* ev, size_t n) try {
@@ -3678,6 +3750,47 @@ int cpbus_group_timer_cancel_many(cpbus_group_t* g, const uint32_t* timer_ids, u
           if (st[j] == CPBUS_OK) timer_disarm(g, timer_ids[el[j]] & kTimerSlotMask, /*reset_bound=*/true);
         return CPBUS_OK;
       });
+} CPBUS_CATCH
+
+int cpbus_group_timer_add_list(cpbus_group_t* g, const cpbus_timer_spec* specs, uint32_t n, uint32_t* timer_ids, int* status,
+                               uint32_t* applied) try {
+  if (!g || (!specs && n)) return CPBUS_EINVAL;
+  std::vector<int> st(n);
+  std::vector<uint32_t> ids(n), shard_ids;
+  std::vector<cpbus_timer_spec> shard_specs;
+  const int rc = group_membership_many(g, n, st.data(), applied,
+      [&](uint32_t i, uint32_t* k) {
+        if (!specs[i].period_ns) return CPBUS_EINVAL;
+        if (!g->K) return CPBUS_ENOSPC;
+        cpbus* s = nullptr; uint32_t l = 0;
+        if (!group_locate(g, specs[i].sub_id, &s, &l)) return CPBUS_ENOENT;
+        *k = group_shard_of(g, specs[i].sub_id - g->base);
+        return CPBUS_OK;
+      },
+      [&] {
+        if (g->h_timers.empty()) g->h_timers.resize((size_t)g->N * g->K);
+        group_retire(g);
+      },
+      [&](uint32_t k, const std::vector<uint32_t>& el, int* st_k) -> int {
+        int rc_k = group_shard_clock(g, g->shards[k]); if (rc_k) return rc_k;
+        shard_specs.resize(el.size()); shard_ids.resize(el.size());
+        for (size_t j = 0; j < el.size(); j++) shard_specs[j] = specs[el[j]];
+        rc_k = cpbus_timer_add_list(g->shards[k], shard_specs.data(), (uint32_t)el.size(), shard_ids.data(), st_k, nullptr);
+        if (rc_k) return rc_k;
+        for (size_t j = 0; j < el.size(); j++) {   // the group's slot and id, as cpbus_group_timer_add maps them
+          if (st_k[j] != CPBUS_OK) continue;
+          const cpbus_timer_spec& s = shard_specs[j];
+          const size_t slot = (size_t)(shard_ids[j] & kTimerSlotMask) + (size_t)g->first[k] * g->K;
+          timer_arm(g, slot, s.period_ns, s.source_id, s.oneshot != 0);
+          ids[el[j]] = (uint32_t)slot | (shard_ids[j] & ~kTimerSlotMask);
+        }
+        return CPBUS_OK;
+      });
+  if (rc) return rc;
+  if (timer_ids)
+    for (uint32_t i = 0; i < n; i++) if (st[i] == CPBUS_OK) timer_ids[i] = ids[i];
+  if (status && n) memcpy(status, st.data(), (size_t)n * sizeof(int));
+  return CPBUS_OK;
 } CPBUS_CATCH
 
 int cpbus_group_publish(cpbus_group_t* g, const cpbus_event* ev, size_t n) try {

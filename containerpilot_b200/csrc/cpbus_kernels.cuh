@@ -1170,6 +1170,31 @@ __global__ void __launch_bounds__(kThreads) membership_kernel(SubCtl* __restrict
     }
 }
 
+// Bulk timer arming (cpbus_timer_add_list): one entry per armed slot.  A slot appears at most once per call (an arm list
+// holds no cancels, and nothing fires between its elements), and the entries of one mailbox carry the same final mask word.
+struct __align__(16) TimerArmOp {
+  uint64_t next_due;     // the slot's first due time, as timer_arm sets it
+  uint64_t period;       // 0 for a one-shot
+  uint32_t source_id;
+  uint32_t slot;         // shard-local timer slot (mailbox * K + k)
+  uint32_t local;        // its mailbox
+  uint32_t mask_word;    // the mailbox's control-block mask word after the whole call, as mask_word() leaves it
+};
+
+// One thread per entry: the slot's whole DevTimer image (what cpbus_timer_add copies: fired and pad 0) in two 16-byte
+// stores, then the mailbox's mask word.  The ring, tail, head and digest are not touched.
+__global__ void __launch_bounds__(kThreads) timer_arm_kernel(SubCtl* __restrict__ ctl, DevTimer* __restrict__ timers,
+                                                             const TimerArmOp* __restrict__ ops, uint32_t n) {
+  const uint32_t i = blockIdx.x * kThreads + threadIdx.x;
+  if (i >= n) return;
+  const uint4* op = reinterpret_cast<const uint4*>(ops + i);
+  const uint4 lo = op[0], hi = op[1];   // lo: next_due, period; hi: source_id, slot, local, mask_word
+  uint4* tp = reinterpret_cast<uint4*>(timers + hi.y);
+  tp[0] = lo;
+  tp[1] = make_uint4(hi.x, 0u, 0u, 0u);
+  ctl[hi.z].mask = hi.w;
+}
+
 // Lossless stream across processes: post this shard's offer word into the publisher's memory (peer mapping elsewhere).
 // Stream-ordered behind the admission pass; the release orders nothing else, it makes the word itself visible system-wide.
 __global__ void stream_offer_kernel(unsigned long long* word, unsigned long long value) {

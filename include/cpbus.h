@@ -250,7 +250,9 @@ int cpbus_set_mask(cpbus_t* bus, uint32_t sub_id, uint32_t code_mask);
  *      Due times saturate: a first or re-armed due time past UINT64_MAX - 1 means "never" (the timer stays armed, counts
  *      in n_timers and can be cancelled, but does not fire). ---- */
 int cpbus_timer_add(cpbus_t* bus, uint32_t sub_id, uint64_t period_ns, uint32_t source_id, int oneshot, uint32_t* timer_id);
-/* one periodic timer per subscriber [first_sub, first_sub+n); source_ids[i] (or source_id0+i if NULL) */
+/* one periodic timer per subscriber [first_sub, first_sub+n); source_ids[i] (or source_id0+i if NULL).  It arms slot 0 of
+ * each subscriber, returns no timer ids and does not advance the slots' generations; cpbus_timer_add_list arms timers with
+ * their own owners, periods and kinds and returns their ids. */
 int cpbus_timer_add_many(cpbus_t* bus, uint32_t first_sub, uint32_t n, uint64_t period_ns, const uint32_t* source_ids, uint32_t source_id0, int oneshot);
 int cpbus_timer_cancel(cpbus_t* bus, uint32_t timer_id);
 
@@ -273,6 +275,37 @@ int cpbus_unsubscribe_many(cpbus_t* bus, const uint32_t* sub_ids, uint32_t n, in
 int cpbus_set_mask_many(cpbus_t* bus, const uint32_t* sub_ids, const uint32_t* code_masks, uint32_t n, int* status,
                         uint32_t* applied);
 int cpbus_timer_cancel_many(cpbus_t* bus, const uint32_t* timer_ids, uint32_t n, int* status, uint32_t* applied);
+
+/* ---- bulk timer arming: cpbus_timer_add for many timers in one call, each with its own owner, period and kind.
+ * Loop equivalence, as for the bulk membership calls above: a bus that calls cpbus_timer_add_list(specs, n) and a twin that
+ * calls cpbus_timer_add(s.sub_id, s.period_ns, s.source_id, s.oneshot, &id) for each specs[i] in order give the same
+ * statuses and ids and the same results afterwards (every later return code, drain, drain_ready, peek_window, digest,
+ * fold, lagging, blockers, debug event and publish count, and every cpbus_stats field but batches, kernel_launches,
+ * admit_* and device_splits).  So:
+ *  - status[i] (status may be NULL) = what cpbus_timer_add would have returned for element i at its turn: CPBUS_EINVAL
+ *    (period 0), CPBUS_ENOSPC (timers_per_sub == 0, or no free slot left), CPBUS_ENOENT (an id never handed out),
+ *    CPBUS_ECLOSED (an unsubscribed owner) or CPBUS_OK.  The call goes on past refused elements; *applied (may be NULL)
+ *    = how many got CPBUS_OK;
+ *  - timer_ids[i] (timer_ids may be NULL) is written for each CPBUS_OK element and left as it was otherwise.  An element
+ *    takes its owner's lowest free slot after the slots taken by earlier elements, so elements for one owner take
+ *    successive slots until timers_per_sub runs out.  Each arming advances the slot's 6-bit generation, as cpbus_timer_add
+ *    does: an id handed out before the slot was re-armed is stale for cpbus_timer_cancel / _cancel_many;
+ *  - ordered with publishes: one flush of the staged events runs where the first element that gets past the up-front
+ *    checks (period, timers_per_sub, id range) would run it (none gets past them: no flush), and then one-shots that have
+ *    fired free their slots.  In lossless mode the flush's CPBUS_EAGAIN is returned with nothing applied, and status,
+ *    timer_ids and applied are not written;
+ *  - CPBUS_EINVAL (checked first): bus NULL, or specs NULL with n > 0.  n == 0: CPBUS_OK, the bus is not read.
+ * The device work is one H2D copy of one entry per armed slot, one kernel launch and one stream synchronisation (none when
+ * nothing is applied), instead of two synchronised copies per timer.  pad is ignored. ---- */
+typedef struct cpbus_timer_spec {
+  uint64_t period_ns;  /* > 0 */
+  uint32_t sub_id;     /* owner */
+  uint32_t source_id;  /* Event.Source of its ticks */
+  uint32_t oneshot;    /* 0: periodic (NewEventTimer); else one-shot (NewEventTimeout) */
+  uint32_t pad;
+} cpbus_timer_spec;    /* 24 bytes */
+int cpbus_timer_add_list(cpbus_t* bus, const cpbus_timer_spec* specs, uint32_t n, uint32_t* timer_ids, int* status,
+                         uint32_t* applied);
 
 /* ---- the hot path: EventBus.Publish (events/bus.go:125-140) ---- */
 /* Stages n events; only code/source_id are read from ev (seq, ts, target, flags
@@ -634,6 +667,10 @@ int cpbus_group_unsubscribe_many(cpbus_group_t* g, const uint32_t* sub_ids, uint
 int cpbus_group_set_mask_many(cpbus_group_t* g, const uint32_t* sub_ids, const uint32_t* code_masks, uint32_t n, int* status,
                               uint32_t* applied);
 int cpbus_group_timer_cancel_many(cpbus_group_t* g, const uint32_t* timer_ids, uint32_t n, int* status, uint32_t* applied);
+/* bulk timer arming: each shard with work takes its elements, in array order, in one cpbus_timer_add_list call; the ids
+ * are global slots with their generation, as cpbus_group_timer_add returns them */
+int cpbus_group_timer_add_list(cpbus_group_t* g, const cpbus_timer_spec* specs, uint32_t n, uint32_t* timer_ids, int* status,
+                               uint32_t* applied);
 int cpbus_group_publish(cpbus_group_t* g, const cpbus_event* ev, size_t n);
 int cpbus_group_send(cpbus_group_t* g, uint32_t sub_id, const cpbus_event* ev);
 int cpbus_group_advance(cpbus_group_t* g, uint64_t now_ns);
