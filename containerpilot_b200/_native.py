@@ -134,6 +134,9 @@ SYMBOLS = {
     "cpbus_drain_many": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, _P(C.c_size_t)]),
     "cpbus_drain_ready": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p,
                                     C.c_size_t, _P(C.c_size_t), _P(C.c_size_t), _P(C.c_uint32)]),
+    "cpbus_take_ready": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p,
+                                   C.c_size_t, _P(C.c_size_t), _P(C.c_size_t), _P(C.c_uint32)]),
+    "cpbus_ack_many": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, _P(C.c_uint32)]),
     "cpbus_lagging": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t,
                                 _P(C.c_size_t), _P(C.c_uint32), _P(LagSummary)]),
     "cpbus_blockers": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, _P(C.c_size_t)]),
@@ -168,7 +171,7 @@ SYMBOLS = {
 GROUP_CALLS = ("intern", "intern_ephemeral", "source", "subscribe", "subscribe_many", "subscribe_pairs", "subscribe_pairs_many",
                "unsubscribe", "set_mask", "timer_add", "timer_add_many", "timer_cancel", "unsubscribe_many", "set_mask_many",
                "timer_cancel_many", "timer_add_list", "publish", "send", "advance", "flush",
-               "sync", "drain", "drain_ready", "lagging", "blockers", "consume_all", "peek_window", "digest", "digest_fold",
+               "sync", "drain", "drain_ready", "take_ready", "ack_many", "lagging", "blockers", "consume_all", "peek_window", "digest", "digest_fold",
                "debug_events", "stats", "publish_counts")
 SYMBOLS["cpbus_group_create"] = (C.c_int, [_P(Config), C.c_void_p, C.c_uint32, _P(C.c_void_p)])
 SYMBOLS["cpbus_group_destroy"] = (C.c_int, [C.c_void_p])

@@ -336,16 +336,31 @@ class Bus:
         next_sub).  ready is a READY_DTYPE array with one entry per mailbox taken; entry i's FIFO run is
         records[ready[i].offset : ready[i].offset + ready[i].count].  Pass next_sub back as start_sub to continue.
         `out`: a preallocated EVENT_DTYPE array of at least `cap` records; records is a view of it."""
+        return self._ready_call("cpbus_drain_ready", first_sub, n, start_sub, cap, ready_cap, out)
+
+    def take_ready(self, first_sub: int, n: int, start_sub: int, cap: int, ready_cap: int, out=None):
+        """Lossless mode: drain_ready that keeps the records' room until ack_many releases it (the records stay held in
+        their mailboxes and count against them).  Same arguments and return shape as drain_ready."""
+        return self._ready_call("cpbus_take_ready", first_sub, n, start_sub, cap, ready_cap, out)
+
+    def _ready_call(self, name: str, first_sub: int, n: int, start_sub: int, cap: int, ready_cap: int, out):
         if out is None:
             out = np.zeros(cap, dtype=EVENT_DTYPE)
         if len(out) < cap:
             raise ValueError("out holds fewer than cap records")
         ready = np.zeros(min(ready_cap, n), dtype=READY_DTYPE)
         n_ready, total, next_sub = C.c_size_t(), C.c_size_t(), C.c_uint32()
-        nat.check(self._lib.cpbus_drain_ready(self._h, first_sub, n, start_sub, out.ctypes.data, cap, ready.ctypes.data,
-                                              ready_cap, C.byref(n_ready), C.byref(total), C.byref(next_sub)),
-                  "cpbus_drain_ready")
+        nat.check(getattr(self._lib, name)(self._h, first_sub, n, start_sub, out.ctypes.data, cap, ready.ctypes.data,
+                                           ready_cap, C.byref(n_ready), C.byref(total), C.byref(next_sub)), name)
         return out[: total.value], ready[: n_ready.value], next_sub.value
+
+    def ack_many(self, sub_ids, counts) -> np.ndarray:
+        """Lossless mode: release the oldest counts[i] held records of sub_ids[i], in order, in one call: the int32 status
+        of each element (OK, ENOENT for an unknown id, EINVAL for more than the mailbox holds at that element's turn)."""
+        ids, cnt = np.ascontiguousarray(sub_ids, dtype=np.uint32), np.ascontiguousarray(counts, dtype=np.uint32)
+        if ids.shape != cnt.shape:
+            raise ValueError("sub_ids and counts differ in length")
+        return self._membership_many("cpbus_ack_many", [ids, cnt])
 
     def lagging(self, first_sub: int, n: int, start_sub: int | None = None, min_backlog: int = 1, cap: int | None = None):
         """Read-only consumer backlog of mailboxes [first_sub, first_sub+n) in cyclic order from start_sub (default

@@ -520,6 +520,12 @@ struct cpbus : HostFront {
   MemberOp* d_member = nullptr; size_t member_cap = 0;
   // cpbus_timer_add_list: device copy of the armed slots' list, grown on demand
   TimerArmOp* d_arm = nullptr; size_t arm_cap = 0;
+  // acknowledged drains (cpbus_take_ready / cpbus_ack_many): the take cursor of every mailbox, allocated (zero) by the first
+  // take; the ack list ([entries | elements], pinned staging and its device copy, grown on demand) and the statuses in
+  // mapped pinned memory
+  unsigned long long* d_taken = nullptr;
+  unsigned char* h_ack = nullptr; unsigned char* d_ack = nullptr; size_t ack_bytes_cap = 0;
+  int* h_ack_status = nullptr; int* d_ack_status = nullptr; size_t ack_status_cap = 0;
 
   // intern table (Event.Source string <-> u32)
   std::unordered_map<std::string, uint32_t> intern;
@@ -1697,6 +1703,9 @@ int cpbus_destroy(cpbus_t* b) try {
   cudaFree(b->d_catchup);
   cudaFree(b->d_member);
   cudaFree(b->d_arm);
+  cudaFree(b->d_taken); cudaFree(b->d_ack);
+  if (b->h_ack) cudaFreeHost(b->h_ack);
+  if (b->h_ack_status) cudaFreeHost(b->h_ack_status);
   cudaFree(b->d_drain);cudaFree(b->d_drain_idx);
   cudaFree(b->d_ready_lb); cudaFree(b->d_ready); cudaFree(b->d_ready_slot);
   if (b->h_ready_hdr) cudaFreeHost(b->h_ready_hdr);
@@ -3015,9 +3024,10 @@ int cpbus_drain_many(cpbus_t* b, uint32_t first_sub, uint32_t n, cpbus_event* ou
 // through mapped pinned memory.  One sync reads the header; a second one follows the two copies sized by it.
 // The body of cpbus_drain_ready, without its cap >= ring_cap check: a group hands each shard the cap its earlier shards
 // left, which can be smaller.  *all_taken: every ready mailbox of the range was taken (then *next_sub = start_sub).
+// take: cpbus_take_ready's scan (the caller has checked that the bus is lossless).
 static int drain_ready_impl(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start_sub, cpbus_event* out, size_t cap,
                             cpbus_ready* ready, size_t ready_cap, size_t* n_ready, size_t* total, uint32_t* next_sub,
-                            bool* all_taken);
+                            bool* all_taken, bool take = false);
 
 int cpbus_drain_ready(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start_sub, cpbus_event* out, size_t cap,
                       cpbus_ready* ready, size_t ready_cap, size_t* n_ready, size_t* total, uint32_t* next_sub) try {
@@ -3027,9 +3037,17 @@ int cpbus_drain_ready(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start
   return drain_ready_impl(b, first_sub, n, start_sub, out, cap, ready, ready_cap, n_ready, total, next_sub, &all_taken);
 } CPBUS_CATCH
 
+int cpbus_take_ready(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start_sub, cpbus_event* out, size_t cap,
+                     cpbus_ready* ready, size_t ready_cap, size_t* n_ready, size_t* total, uint32_t* next_sub) try {
+  if (!b || !out || !ready || !n_ready || !total || !next_sub || !n || !ready_cap) return CPBUS_EINVAL;
+  if (cap < b->R || cap > 0xFFFFFFFFull || !b->lossless) return CPBUS_EINVAL;
+  bool all_taken = false;
+  return drain_ready_impl(b, first_sub, n, start_sub, out, cap, ready, ready_cap, n_ready, total, next_sub, &all_taken, true);
+} CPBUS_CATCH
+
 static int drain_ready_impl(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start_sub, cpbus_event* out, size_t cap,
                             cpbus_ready* ready, size_t ready_cap, size_t* n_ready, size_t* total, uint32_t* next_sub,
-                            bool* all_taken) {
+                            bool* all_taken, bool take) {
   if (start_sub < first_sub || start_sub - first_sub >= n) return CPBUS_EINVAL;
   uint32_t l = 0;
   if (!id_range(b->cfg.sub_id_base, b->n_next, first_sub, n, &l)) return CPBUS_ENOENT;
@@ -3057,8 +3075,17 @@ static int drain_ready_impl(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t
   CK(cudaMemsetAsync(b->d_ready_lb + kReadyHdrWords, 0, (kReadyLbOffset - kReadyHdrWords + (size_t)tiles) * sizeof(unsigned long long),
                      b->stream));
   const uint32_t rot = start_sub - first_sub;
-  drain_ready_scan_kernel<<<tiles, kThreads, 0, b->stream>>>(b->d_ctl, l, n, rot, b->R, b->lossless ? 1u : 0u, b->cfg.sub_id_base,
-                                                              cap, rcap, b->d_ready_lb, b->d_ready, b->d_ready_slot);
+  if (take) {
+    if (!b->d_taken) {   // every cursor 0: max(0, head) = head, so nothing is held
+      CK(cudaMalloc((void**)&b->d_taken, (size_t)b->N * sizeof(unsigned long long)));
+      CK(cudaMemsetAsync(b->d_taken, 0, (size_t)b->N * sizeof(unsigned long long), b->stream));
+    }
+    take_ready_scan_kernel<<<tiles, kThreads, 0, b->stream>>>(b->d_ctl, b->d_taken, l, n, rot, b->R, b->cfg.sub_id_base, cap,
+                                                               rcap, b->d_ready_lb, b->d_ready, b->d_ready_slot);
+  } else {
+    drain_ready_scan_kernel<<<tiles, kThreads, 0, b->stream>>>(b->d_ctl, l, n, rot, b->R, b->lossless ? 1u : 0u, b->cfg.sub_id_base,
+                                                                cap, rcap, b->d_ready_lb, b->d_ready, b->d_ready_slot);
+  }
   CK(cudaGetLastError());
   const uint32_t gather_grid = (uint32_t)std::min<size_t>((size_t)b->sm_count * 4, (rcap + kWarpsPerCta - 1) / kWarpsPerCta);
   drain_ready_gather_kernel<<<gather_grid, kThreads, 0, b->stream>>>(b->d_ring, b->R, b->cfg.sub_id_base, b->d_ready,
@@ -3078,6 +3105,81 @@ static int drain_ready_impl(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t
   *next_sub = cut >= n ? start_sub : first_sub + (uint32_t)((rot + cut) % n);
   return CPBUS_OK;
 }
+
+// cpbus_ack_many on one bus (the caller has checked the arguments and that the bus is lossless): st[i] for every element.
+// Unknown ids get CPBUS_ENOENT and count 0 gets CPBUS_OK on the host; the others go to ack_kernel, one entry per mailbox
+// with its elements in array order.  Before the first take nothing is held, so they are refused without a launch.
+static int ack_many_impl(cpbus* b, const uint32_t* sub_ids, const uint32_t* counts, uint32_t n, int* st) {
+  std::vector<uint64_t> el;   // mailbox << 32 | element index: sorted, each mailbox's elements stay in array order
+  for (uint32_t i = 0; i < n; i++) {
+    uint32_t l = 0;
+    if (!id_range(b->cfg.sub_id_base, b->n_next, sub_ids[i], 1, &l)) st[i] = CPBUS_ENOENT;
+    else if (counts[i] == 0) st[i] = CPBUS_OK;
+    else if (!b->d_taken) st[i] = CPBUS_EINVAL;
+    else el.push_back((uint64_t)l << 32 | i);
+  }
+  if (el.empty()) return CPBUS_OK;
+  std::sort(el.begin(), el.end());
+  std::vector<AckOp> ops;
+  std::vector<uint2> elems(el.size());
+  for (size_t j = 0; j < el.size(); j++) {
+    const uint32_t l = (uint32_t)(el[j] >> 32), i = (uint32_t)el[j];
+    if (ops.empty() || ops.back().local != l) ops.push_back(AckOp{l, (uint32_t)j, 0u, 0u});
+    ops.back().n++;
+    elems[j] = make_uint2(counts[i], i);
+  }
+  std::lock_guard<std::mutex> g(b->mu);
+  int rc = enter(b); if (rc) return rc;
+  const size_t op_bytes = ops.size() * sizeof(AckOp), bytes = op_bytes + elems.size() * sizeof(uint2);
+  if (b->ack_bytes_cap < bytes) {   // (every call ends in a synchronisation: no copy or kernel reads the old list)
+    cudaFree(b->d_ack); b->d_ack = nullptr;
+    if (b->h_ack) cudaFreeHost(b->h_ack);
+    b->h_ack = nullptr; b->ack_bytes_cap = 0;
+    const size_t c = std::max<size_t>(bytes, 16384);
+    CK(cudaMalloc((void**)&b->d_ack, c));
+    CK(cudaHostAlloc((void**)&b->h_ack, c, cudaHostAllocDefault));
+    b->ack_bytes_cap = c;
+  }
+  if (b->ack_status_cap < n) {
+    if (b->h_ack_status) cudaFreeHost(b->h_ack_status);
+    b->h_ack_status = nullptr; b->d_ack_status = nullptr; b->ack_status_cap = 0;
+    const size_t c = std::max<size_t>(n, 1024);
+    CK(mapped_alloc(c * sizeof(int), &b->h_ack_status, &b->d_ack_status));
+    b->ack_status_cap = c;
+  }
+  memcpy(b->h_ack, ops.data(), op_bytes);
+  memcpy(b->h_ack + op_bytes, elems.data(), bytes - op_bytes);
+  CK(cudaMemcpyAsync(b->d_ack, b->h_ack, bytes, cudaMemcpyHostToDevice, b->stream));
+  ack_kernel<<<(uint32_t)((ops.size() + kThreads - 1) / kThreads), kThreads, 0, b->stream>>>(
+      b->d_ctl, b->d_taken, reinterpret_cast<const AckOp*>(b->d_ack), (uint32_t)ops.size(),
+      reinterpret_cast<const uint2*>(b->d_ack + op_bytes), b->d_ack_status);
+  CK(cudaGetLastError());
+  b->st.kernel_launches++;
+  CK(cudaStreamSynchronize(b->stream));
+  const volatile int* hs = b->h_ack_status;
+  for (const uint2& e : elems) st[e.y] = hs[e.y];
+  return CPBUS_OK;
+}
+
+// status (may be NULL) = st, *applied (may be NULL) = how many are CPBUS_OK
+static void ack_statuses(const std::vector<int>& st, int* status, uint32_t* applied) {
+  if (status) memcpy(status, st.data(), st.size() * sizeof(int));
+  if (applied) *applied = (uint32_t)std::count(st.begin(), st.end(), CPBUS_OK);
+}
+
+int cpbus_ack_many(cpbus_t* b, const uint32_t* sub_ids, const uint32_t* counts, uint32_t n, int* status, uint32_t* applied) try {
+  if (!b || ((!sub_ids || !counts) && n)) return CPBUS_EINVAL;
+  if (n == 0) {
+    if (applied) *applied = 0;
+    return CPBUS_OK;
+  }
+  if (!b->lossless) return CPBUS_EINVAL;   // throughput mode: a held record could be overwritten before its ack
+  std::vector<int> st(n);
+  const int rc = ack_many_impl(b, sub_ids, counts, n, st.data());
+  if (rc) return rc;
+  ack_statuses(st, status, applied);
+  return CPBUS_OK;
+} CPBUS_CATCH
 
 // Consumer backlog: one read-only scan of the range's control blocks; the entries and the header {selected, cut position,
 // summary} arrive in mapped pinned memory, so one sync is the only wait.  *all_returned: every lagging mailbox was returned.
@@ -3831,27 +3933,30 @@ int cpbus_group_drain(cpbus_group_t* g, uint32_t sub_id, cpbus_event* out, size_
 } CPBUS_CATCH
 
 // The first ready mailbox of [a, a + cnt) on shard s (cnt when none): where a walk with no room left stops.
-static int group_first_ready(cpbus* s, uint32_t l, uint32_t cnt, uint32_t* at) {
+// take: ready as cpbus_take_ready sees it (records past the take cursor).
+static int group_first_ready(cpbus* s, uint32_t l, uint32_t cnt, uint32_t* at, bool take = false) {
   std::vector<SubCtl> c(cnt);
+  std::vector<unsigned long long> tk(cnt, 0ull);
   int rc = dev_guard(s); if (rc) return rc;
   CK(cudaMemcpyAsync(c.data(), s->d_ctl + l, (size_t)cnt * sizeof(SubCtl), cudaMemcpyDeviceToHost, s->stream));
+  if (take && s->d_taken)
+    CK(cudaMemcpyAsync(tk.data(), s->d_taken + l, (size_t)cnt * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s->stream));
   CK(cudaStreamSynchronize(s->stream));
   *at = cnt;
-  for (uint32_t i = 0; i < cnt; i++) if (c[i].tail > c[i].head) { *at = i; break; }
+  for (uint32_t i = 0; i < cnt; i++) if (c[i].tail > std::max<uint64_t>(c[i].head, tk[i])) { *at = i; break; }
   return CPBUS_OK;
 }
 
-// The cyclic walk of cpbus_drain_ready over the shards: each piece of the walk that lies on one shard is drained there with
-// the cap and ready entries still left, and the walk stops at the first mailbox that does not fit, as the single call does.
-int cpbus_group_drain_ready(cpbus_group_t* g, uint32_t first_sub, uint32_t n, uint32_t start_sub, cpbus_event* out, size_t cap,
-                            cpbus_ready* ready, size_t ready_cap, size_t* n_ready, size_t* total, uint32_t* next_sub) try {
-  if (!g || !out || !ready || !n_ready || !total || !next_sub || !n || !ready_cap) return CPBUS_EINVAL;
-  if (cap < g->shards[0]->R || cap > 0xFFFFFFFFull) return CPBUS_EINVAL;
+// The cyclic walk of cpbus_drain_ready (take: cpbus_take_ready) over the shards: each piece of the walk that lies on one
+// shard is drained there with the cap and ready entries still left, and the walk stops at the first mailbox that does not
+// fit, as the single call does.  The caller has checked the arguments.
+static int group_drain_ready(cpbus_group* g, uint32_t first_sub, uint32_t n, uint32_t start_sub, cpbus_event* out, size_t cap,
+                             cpbus_ready* ready, size_t ready_cap, size_t* n_ready, size_t* total, uint32_t* next_sub, bool take) {
   size_t nr = 0, tot = 0, ready_left = std::min<size_t>(ready_cap, n);
   const int rc = group_walk(g, first_sub, n, start_sub, next_sub, [&](cpbus* s, uint32_t l, uint32_t a, uint32_t cnt) -> int {
     if (ready_left == 0 || tot == cap) {                           // no room: the next ready mailbox ends the walk
       uint32_t at = cnt;
-      const int rc_s = group_first_ready(s, l, cnt, &at); if (rc_s) return rc_s;
+      const int rc_s = group_first_ready(s, l, cnt, &at, take); if (rc_s) return rc_s;
       if (at == cnt) return CPBUS_OK;
       *next_sub = a + at;
       return kWalkEnd;
@@ -3859,7 +3964,8 @@ int cpbus_group_drain_ready(cpbus_group_t* g, uint32_t first_sub, uint32_t n, ui
     size_t nr_s = 0, tot_s = 0;
     uint32_t next_s = a;
     bool all = false;
-    const int rc_s = drain_ready_impl(s, a, cnt, a, out + tot, cap - tot, ready + nr, ready_left, &nr_s, &tot_s, &next_s, &all);
+    const int rc_s = drain_ready_impl(s, a, cnt, a, out + tot, cap - tot, ready + nr, ready_left, &nr_s, &tot_s, &next_s, &all,
+                                      take);
     if (rc_s) return rc_s;
     for (size_t j = 0; j < nr_s; j++) ready[nr + j].offset += (uint32_t)tot;
     nr += nr_s; tot += tot_s; ready_left -= nr_s;
@@ -3869,6 +3975,51 @@ int cpbus_group_drain_ready(cpbus_group_t* g, uint32_t first_sub, uint32_t n, ui
   });
   if (rc) return rc;
   *n_ready = nr; *total = tot;
+  return CPBUS_OK;
+}
+
+int cpbus_group_drain_ready(cpbus_group_t* g, uint32_t first_sub, uint32_t n, uint32_t start_sub, cpbus_event* out, size_t cap,
+                            cpbus_ready* ready, size_t ready_cap, size_t* n_ready, size_t* total, uint32_t* next_sub) try {
+  if (!g || !out || !ready || !n_ready || !total || !next_sub || !n || !ready_cap) return CPBUS_EINVAL;
+  if (cap < g->shards[0]->R || cap > 0xFFFFFFFFull) return CPBUS_EINVAL;
+  return group_drain_ready(g, first_sub, n, start_sub, out, cap, ready, ready_cap, n_ready, total, next_sub, false);
+} CPBUS_CATCH
+
+int cpbus_group_take_ready(cpbus_group_t* g, uint32_t first_sub, uint32_t n, uint32_t start_sub, cpbus_event* out, size_t cap,
+                           cpbus_ready* ready, size_t ready_cap, size_t* n_ready, size_t* total, uint32_t* next_sub) try {
+  if (!g || !out || !ready || !n_ready || !total || !next_sub || !n || !ready_cap) return CPBUS_EINVAL;
+  if (cap < g->shards[0]->R || cap > 0xFFFFFFFFull || !g->lossless) return CPBUS_EINVAL;
+  return group_drain_ready(g, first_sub, n, start_sub, out, cap, ready, ready_cap, n_ready, total, next_sub, true);
+} CPBUS_CATCH
+
+// Each shard with work takes its elements, in array order, in one cpbus_ack_many call; shards hold disjoint mailboxes, so
+// the statuses are the single bus's.
+int cpbus_group_ack_many(cpbus_group_t* g, const uint32_t* sub_ids, const uint32_t* counts, uint32_t n, int* status,
+                         uint32_t* applied) try {
+  if (!g || ((!sub_ids || !counts) && n)) return CPBUS_EINVAL;
+  if (n == 0) {
+    if (applied) *applied = 0;
+    return CPBUS_OK;
+  }
+  if (!g->lossless) return CPBUS_EINVAL;
+  std::vector<int> st(n);
+  std::vector<std::vector<uint32_t>> work(g->shards.size());
+  for (uint32_t i = 0; i < n; i++) {
+    cpbus* s = nullptr; uint32_t l = 0;
+    if (!group_locate(g, sub_ids[i], &s, &l)) st[i] = CPBUS_ENOENT;
+    else work[group_shard_of(g, sub_ids[i] - g->base)].push_back(i);
+  }
+  std::vector<uint32_t> ids, cnts;
+  std::vector<int> st_k;
+  for (uint32_t k = 0; k < g->shards.size(); k++) {
+    if (work[k].empty()) continue;
+    ids.resize(work[k].size()); cnts.resize(work[k].size()); st_k.resize(work[k].size());
+    for (size_t j = 0; j < work[k].size(); j++) { ids[j] = sub_ids[work[k][j]]; cnts[j] = counts[work[k][j]]; }
+    const int rc = ack_many_impl(g->shards[k], ids.data(), cnts.data(), (uint32_t)ids.size(), st_k.data());
+    if (rc) return rc;
+    for (size_t j = 0; j < work[k].size(); j++) st[work[k][j]] = st_k[j];
+  }
+  ack_statuses(st, status, applied);
   return CPBUS_OK;
 } CPBUS_CATCH
 

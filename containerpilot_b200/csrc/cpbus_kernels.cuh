@@ -616,11 +616,13 @@ __device__ __forceinline__ unsigned long long lb_pack(unsigned long long flag, u
 
 // hdr[0..2] = {mailboxes taken, records taken, position of the first ready mailbox that did not fit (n: none)}; exactly one
 // thread writes it: the one holding that mailbox, or the last tile when everything fits.
-__global__ void __launch_bounds__(kThreads) drain_ready_scan_kernel(SubCtl* __restrict__ ctl, uint32_t first, uint32_t n,
-                                                                    uint32_t rot, uint32_t ring_cap, uint32_t lossless,
-                                                                    uint32_t sub_base, unsigned long long cap,
-                                                                    unsigned long long ready_cap, unsigned long long* lb,
-                                                                    cpbus_ready* __restrict__ ready, uint32_t* __restrict__ slot) {
+// kTake (cpbus_take_ready, lossless only): a mailbox's cursor is max(take cursor, head), and taking it moves the take
+// cursor to tail instead of head.
+template <bool kTake>
+__device__ __forceinline__ void ready_scan(SubCtl* __restrict__ ctl, unsigned long long* __restrict__ taken, uint32_t first,
+                                           uint32_t n, uint32_t rot, uint32_t ring_cap, uint32_t lossless, uint32_t sub_base,
+                                           unsigned long long cap, unsigned long long ready_cap, unsigned long long* lb,
+                                           cpbus_ready* __restrict__ ready, uint32_t* __restrict__ slot) {
   __shared__ uint32_t s_tile;
   __shared__ uint32_t s_wr[32];              // per (item, warp) chunk: ready mailboxes, then their exclusive prefix in the tile
   __shared__ unsigned long long s_wc[32];    // ... and records
@@ -645,7 +647,12 @@ __global__ void __launch_bounds__(kThreads) drain_ready_scan_kernel(SubCtl* __re
       l = first + (uint32_t)q;
       const ulonglong2 th = *reinterpret_cast<const ulonglong2*>(ctl + l);   // {tail, head}
       t = th.x; h = th.y; c = h;
-      if (!lossless && t > ring_cap && t - ring_cap > c) c = t - ring_cap;   // overwritten before being taken
+      if constexpr (kTake) {
+        const unsigned long long tk = taken[l];
+        if (tk > c) c = tk;
+      } else {
+        if (!lossless && t > ring_cap && t - ring_cap > c) c = t - ring_cap;   // overwritten before being taken
+      }
     }
     loc[k] = l; tl[k] = t; hd[k] = h; cur[k] = c;
     uint32_t r = t != c ? 1u : 0u;
@@ -709,13 +716,38 @@ __global__ void __launch_bounds__(kThreads) drain_ready_scan_kernel(SubCtl* __re
     const unsigned long long r = s_base_r + s_wr[chunk] + r_in[k] - 1;        // entry index among the ready mailboxes
     const unsigned long long o = s_base_c + s_wc[chunk] + c_in[k] - cnt;      // first record of the run in `out`
     if (r < ready_cap && o + cnt <= cap) {
-      ready[r] = cpbus_ready{sub_base + loc[k], (uint32_t)cnt, (uint32_t)o, 0u, cur[k] - hd[k]};
-      slot[r] = (uint32_t)(cur[k] & (ring_cap - 1));
-      ctl[loc[k]].head = tl[k];
+      if constexpr (kTake) {
+        ready[r] = cpbus_ready{sub_base + loc[k], (uint32_t)cnt, (uint32_t)o, 0u, 0ull};
+        slot[r] = (uint32_t)(cur[k] & (ring_cap - 1));
+        taken[loc[k]] = tl[k];
+      } else {
+        ready[r] = cpbus_ready{sub_base + loc[k], (uint32_t)cnt, (uint32_t)o, 0u, cur[k] - hd[k]};
+        slot[r] = (uint32_t)(cur[k] & (ring_cap - 1));
+        ctl[loc[k]].head = tl[k];
+      }
     } else if (r == 0 || (r - 1 < ready_cap && o <= cap)) {   // its predecessor was taken: this one ends the call
       hdr[0] = r; hdr[1] = o; hdr[2] = tile * kReadyTile + k * kThreads + threadIdx.x;
     }
   }
+}
+
+__global__ void __launch_bounds__(kThreads) drain_ready_scan_kernel(SubCtl* __restrict__ ctl, uint32_t first, uint32_t n,
+                                                                    uint32_t rot, uint32_t ring_cap, uint32_t lossless,
+                                                                    uint32_t sub_base, unsigned long long cap,
+                                                                    unsigned long long ready_cap, unsigned long long* lb,
+                                                                    cpbus_ready* __restrict__ ready, uint32_t* __restrict__ slot) {
+  ready_scan<false>(ctl, nullptr, first, n, rot, ring_cap, lossless, sub_base, cap, ready_cap, lb, ready, slot);
+}
+
+// cpbus_take_ready: the same scan over a lossless bus, reading and moving the take cursors `taken` (one per mailbox); head
+// is read, never written.  The taken runs are copied by drain_ready_gather_kernel.
+__global__ void __launch_bounds__(kThreads) take_ready_scan_kernel(SubCtl* __restrict__ ctl,
+                                                                   unsigned long long* __restrict__ taken, uint32_t first,
+                                                                   uint32_t n, uint32_t rot, uint32_t ring_cap,
+                                                                   uint32_t sub_base, unsigned long long cap,
+                                                                   unsigned long long ready_cap, unsigned long long* lb,
+                                                                   cpbus_ready* __restrict__ ready, uint32_t* __restrict__ slot) {
+  ready_scan<true>(ctl, taken, first, n, rot, ring_cap, 1u, sub_base, cap, ready_cap, lb, ready, slot);
 }
 
 // Copies the taken runs: one warp per ready entry, lane pairs per record (each pair writes one whole 32-byte sector), and
@@ -1193,6 +1225,36 @@ __global__ void __launch_bounds__(kThreads) timer_arm_kernel(SubCtl* __restrict_
   tp[0] = lo;
   tp[1] = make_uint4(hi.x, 0u, 0u, 0u);
   ctl[hi.z].mask = hi.w;
+}
+
+// Acknowledged drains (cpbus_ack_many): one entry per mailbox, holding the index range [first, first + n) of its elements
+// in `elems` (in the call's array order).  An element is {records to release, its index in the call}.  The host builds one
+// entry per mailbox, so no two threads touch one mailbox.
+struct __align__(16) AckOp {
+  uint32_t local;   // mailbox (shard-local index)
+  uint32_t first, n;
+  uint32_t pad;
+};
+
+// One thread per entry: held = max(take cursor, head) - head; each element in order releases its count of the oldest held
+// records if that many are held (CPBUS_OK) and is refused otherwise (CPBUS_EINVAL).  The statuses go to the host through
+// mapped memory; head is stored once.  The ring, tail, digest, mask and take cursor are not touched.
+__global__ void __launch_bounds__(kThreads) ack_kernel(SubCtl* __restrict__ ctl, const unsigned long long* __restrict__ taken,
+                                                       const AckOp* __restrict__ ops, uint32_t n_ops,
+                                                       const uint2* __restrict__ elems, int* __restrict__ status) {
+  const uint32_t i = blockIdx.x * kThreads + threadIdx.x;
+  if (i >= n_ops) return;
+  const AckOp op = ops[i];
+  unsigned long long head = ctl[op.local].head;
+  const unsigned long long tk = taken[op.local];
+  unsigned long long held = tk > head ? tk - head : 0ull;
+  for (uint32_t j = op.first; j < op.first + op.n; j++) {
+    const uint2 e = elems[j];   // {count, index in the call}
+    const bool ok = e.x <= held;
+    if (ok) { head += e.x; held -= e.x; }
+    status[e.y] = ok ? CPBUS_OK : CPBUS_EINVAL;
+  }
+  ctl[op.local].head = head;
 }
 
 // Lossless stream across processes: post this shard's offer word into the publisher's memory (peer mapping elsewhere).

@@ -18,6 +18,7 @@
 #include <chrono>
 #include <condition_variable>
 #include <deque>
+#include <exception>
 #include <functional>
 #include <map>
 #include <memory>
@@ -146,7 +147,7 @@ class Subscriber : public EventSubscriber {   // events/subscriber.go:13-37
   friend void NewEventTimer(class Context&, const ChanPtr&, std::chrono::nanoseconds, const std::string&);
   uint32_t id_ = UINT32_MAX;
   bool implicit_ = false;       // made by the bus for a timer-only channel: not in the WaitGroup, released when Rx is closed
-  std::deque<Event> pending_;   // drained from HBM but Rx was full
+  std::deque<Event> pending_;   // drained from HBM but Rx was full (AckOnDelivery: exactly the mailbox's held records)
 };
 
 class Publisher : public EventPublisher {   // events/publisher.go:13-36
@@ -193,6 +194,7 @@ EVENTS_CPBUS_CALL(publish) EVENTS_CPBUS_CALL(send) EVENTS_CPBUS_CALL(advance) EV
 EVENTS_CPBUS_CALL(timer_add) EVENTS_CPBUS_CALL(timer_cancel) EVENTS_CPBUS_CALL(drain) EVENTS_CPBUS_CALL(drain_ready)
 EVENTS_CPBUS_CALL(debug_events) EVENTS_CPBUS_CALL(intern) EVENTS_CPBUS_CALL(intern_ephemeral) EVENTS_CPBUS_CALL(source)
 EVENTS_CPBUS_CALL(lagging) EVENTS_CPBUS_CALL(blockers) EVENTS_CPBUS_CALL(unsubscribe_many)
+EVENTS_CPBUS_CALL(take_ready) EVENTS_CPBUS_CALL(ack_many)
 #undef EVENTS_CPBUS_CALL
 
 namespace detail {
@@ -407,6 +409,7 @@ class EventBus {   // events/bus.go:12-22
     return it == counter_.end() ? 0 : it->second;
   }
   cpbus_t* handle() { return h_.one; }   // (nullptr on a group)
+  cpbus_group_t* group_handle() { return h_.group; }   // (nullptr on one bus)
 
   // ---- extensions, NOT in the reference API ----
   // The subscribers whose full mailboxes the next flush cannot get past (cpbus_blockers: what a goroutine dump of the Go bus
@@ -427,6 +430,23 @@ class EventBus {   // events/bus.go:12-22
       if (it != by_id_.end()) out.push_back(it->second);
     }
     return out;
+  }
+  // Back-pressure through the pump (off by default).  Off, the pump moves every ready record off the GPU into the
+  // subscriber's host queue, so a consumer that stops reading never fills its mailbox: the publisher never blocks on it and
+  // the queue has no bound.  On, the pump takes records with cpbus_take_ready, keeps them in the host queue while they
+  // still count against the mailbox, and after each pass releases what each channel accepted with one cpbus_ack_many.  The
+  // host queue then never holds more than mailbox_cap records per subscriber, and once channel capacity + mailbox_cap
+  // records wait for a consumer its mailbox is full: Blocking() names it and the next Publish blocks, as a Go publisher
+  // blocks on `sub.Rx <- event`.  std::logic_error while the host queue holds records (switch before publishing).
+  void AckOnDelivery(bool on) {
+    std::lock_guard<std::recursive_mutex> l(lock_);
+    if (!pending_subs_.empty()) throw std::logic_error("AckOnDelivery: the pump holds undelivered records");
+    ack_ = on;
+  }
+  // Records the pump holds on the host for `sub` (taken or drained from its mailbox, not yet accepted by its channel).
+  size_t Buffered(const Subscriber* sub) {
+    std::lock_guard<std::recursive_mutex> l(lock_);
+    return sub->pending_.size();
   }
   // Every subscribed mailbox holding at least `min_backlog` undrained records (cpbus_lagging), in id order.
   struct Lag { Subscriber* sub; uint32_t backlog; uint64_t lost; };
@@ -530,10 +550,14 @@ class EventBus {   // events/bus.go:12-22
   void DrainOne(Subscriber* sub, bool blocking) {
     if (sub->id_ == UINT32_MAX) return;
     cpbus_event buf[256];
+    size_t held = ack_ ? sub->pending_.size() : 0;   // cpbus_drain reads from head: the held records come first
     for (;;) {
       size_t n = 0; uint64_t lost = 0;
       Check(cpbus_drain(h_, sub->id_, buf, 256, &n, &lost), "cpbus_drain");
-      for (size_t i = 0; i < n; i++) sub->pending_.push_back(Event{(EventCode)buf[i].code, Source(buf[i].source_id)});
+      for (size_t i = 0; i < n; i++) {
+        if (held) { held--; continue; }
+        sub->pending_.push_back(Event{(EventCode)buf[i].code, Source(buf[i].source_id)});
+      }
       if (n < 256) break;
     }
     while (!sub->pending_.empty() && sub->Rx) {
@@ -545,7 +569,8 @@ class EventBus {   // events/bus.go:12-22
     else pending_subs_.insert(sub);
   }
   // Only the mailboxes that hold records (cpbus_drain_ready), then only the subscribers with pending records: the pump's
-  // cost follows what was delivered, not how many subscribers there are.
+  // cost follows what was delivered, not how many subscribers there are.  AckOnDelivery: cpbus_take_ready, then one
+  // cpbus_ack_many for what the channels accepted.
   void DrainAll(bool blocking) {
     if (by_id_.empty()) return;
     const uint32_t lo = by_id_.begin()->first, n = by_id_.rbegin()->first - lo + 1;
@@ -554,8 +579,12 @@ class EventBus {   // events/bus.go:12-22
     for (uint32_t start = lo;;) {   // resume at the first mailbox that did not fit: every mailbox gets its turn
       size_t n_ready = 0, total = 0;
       uint32_t next = lo;
-      Check(cpbus_drain_ready(h_, lo, n, start, drain_buf_.data(), drain_cap_, drain_ready_.data(), kReadyCap, &n_ready, &total, &next),
-            "cpbus_drain_ready");
+      if (ack_)
+        Check(cpbus_take_ready(h_, lo, n, start, drain_buf_.data(), drain_cap_, drain_ready_.data(), kReadyCap, &n_ready, &total, &next),
+              "cpbus_take_ready");
+      else
+        Check(cpbus_drain_ready(h_, lo, n, start, drain_buf_.data(), drain_cap_, drain_ready_.data(), kReadyCap, &n_ready, &total, &next),
+              "cpbus_drain_ready");
       for (size_t i = 0; i < n_ready; i++) {
         const cpbus_ready& e = drain_ready_[i];
         auto it = by_id_.find(e.sub_id);
@@ -568,20 +597,30 @@ class EventBus {   // events/bus.go:12-22
       start = next;
     }
     std::vector<Subscriber*> dead;
+    std::vector<uint32_t> ack_ids, ack_counts;   // AckOnDelivery: what each channel accepted
+    std::exception_ptr panic;
     for (auto it = pending_subs_.begin(); it != pending_subs_.end();) {
       Subscriber* sub = *it;
+      uint32_t sent = 0;
       try {
         while (!sub->pending_.empty() && sub->Rx) {
           if (blocking) sub->Rx->Send(sub->pending_.front());
           else if (!sub->Rx->TrySend(sub->pending_.front())) break;
           sub->pending_.pop_front();
+          sent++;
         }
       } catch (const Panic&) {
-        if (!sub->implicit_) throw;          // bus.go:135-137: publishing into a closed subscriber channel is a panic
-        dead.push_back(sub);                 // timer.go:50-54: the timer goroutine recovers and exits
+        if (!sub->implicit_) panic = std::current_exception();   // bus.go:135-137: publishing into a closed subscriber channel is a panic
+        else dead.push_back(sub);            // timer.go:50-54: the timer goroutine recovers and exits
       }
+      if (ack_ && sent) { ack_ids.push_back(sub->id_); ack_counts.push_back(sent); }
+      if (panic) break;
       it = sub->pending_.empty() ? pending_subs_.erase(it) : std::next(it);
     }
+    if (!ack_ids.empty())   // (the records the channels took leave their mailboxes even when a channel panicked)
+      Check(cpbus_ack_many(h_, ack_ids.data(), ack_counts.data(), (uint32_t)ack_ids.size(), (int*)nullptr, (uint32_t*)nullptr),
+            "cpbus_ack_many");
+    if (panic) std::rethrow_exception(panic);
     for (Subscriber* sub : dead) ReleaseImplicit(sub);
   }
   void PumpLoop() {
@@ -598,6 +637,7 @@ class EventBus {   // events/bus.go:12-22
 
   static constexpr size_t kDrainCap = 1 << 16, kReadyCap = 4096;
   size_t drain_cap_ = kDrainCap;               // records per cpbus_drain_ready call (at least one mailbox's capacity)
+  bool ack_ = false;                           // AckOnDelivery
   std::vector<cpbus_event> drain_buf_;
   std::vector<cpbus_ready> drain_ready_;
   detail::Handle h_;

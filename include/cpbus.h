@@ -531,6 +531,37 @@ typedef struct cpbus_ready {
 int cpbus_drain_ready(cpbus_t* bus, uint32_t first_sub, uint32_t n, uint32_t start_sub,
                       cpbus_event* out, size_t cap, cpbus_ready* ready, size_t ready_cap,
                       size_t* n_ready, size_t* total, uint32_t* next_sub);
+
+/* ---- acknowledged drains (lossless mode): copy a mailbox's records out but keep their room until the consumer's channel
+ * has them.  cpbus_drain_ready frees a mailbox as it copies it, so a pump that buffers on the host for a stalled consumer
+ * never lets its mailbox fill, and the publisher never stalls on it.  Take and ack split that in two:
+ * Each mailbox has a take cursor T (0 at subscribe); its effective value is taken = max(T, head), and its taken - head
+ * HELD records are the ones copied out and not yet released.
+ *  - cpbus_take_ready has the arguments, checks, walk, cuts, output layout and *next_sub rule of cpbus_drain_ready, but a
+ *    mailbox is ready when tail > taken, its run is [taken, tail), and taking it sets T = tail and leaves head alone.
+ *    cpbus_ready.lost and .pad are 0.  Like cpbus_drain_ready it runs on the bus stream behind every earlier launch and
+ *    does not flush staged events.
+ *  - cpbus_ack_many releases, for each element in array order, the oldest counts[i] held records of sub_ids[i] (head +=
+ *    counts[i]).  status[i] (status may be NULL): CPBUS_ENOENT (an id this bus never handed out, or outside this shard),
+ *    CPBUS_EINVAL (counts[i] exceeds what the mailbox holds at this element's turn: an id listed twice is checked against
+ *    what its earlier elements left) or CPBUS_OK (counts[i] == 0 included).  The call goes on past refused elements;
+ *    *applied (may be NULL) = how many got CPBUS_OK.  Unsubscribed mailboxes can be acked.  It does not flush.
+ *    After ack(id, k) the bus is in the state a bus that never takes reaches with cpbus_drain(id, cap = k) at that point;
+ *    only the take cursors differ.  The device work is one H2D copy of one entry per mailbox, one kernel launch and one
+ *    stream synchronisation; none when no element with counts[i] > 0 names a mailbox of this bus, or before its first take.
+ * Taking is invisible to everything else: held records stay in the ring, so a bus that takes and one that never drains
+ * give the same return codes and CPBUS_EAGAIN points of every publish, flush, advance, send, membership and stream
+ * admission call, the same blockers, stream_blockers and lagging (held records are backlog), windows, digests, folds, debug
+ * events and every cpbus_stats field but kernel_launches.  cpbus_drain, _drain_many, _drain_ready and _consume_all read
+ * from head, held records included; afterwards head >= T, so nothing is held.
+ * A pump that takes, hands the records to its consumers' channels and acks what each channel accepted holds at most
+ * ring_cap records per consumer, and a consumer that stops reading fills its mailbox and stalls the publisher.
+ * CPBUS_EINVAL: as cpbus_drain_ready, or a throughput-mode bus (held records could be overwritten before their ack); for
+ * ack_many, checked first, a NULL bus or an array NULL with n > 0.  ack_many with n == 0: CPBUS_OK, the bus is not read. */
+int cpbus_take_ready(cpbus_t* bus, uint32_t first_sub, uint32_t n, uint32_t start_sub,
+                     cpbus_event* out, size_t cap, cpbus_ready* ready, size_t ready_cap,
+                     size_t* n_ready, size_t* total, uint32_t* next_sub);
+int cpbus_ack_many(cpbus_t* bus, const uint32_t* sub_ids, const uint32_t* counts, uint32_t n, int* status, uint32_t* applied);
 /* Consumer backlog, read-only: which subscribed mailboxes fall behind and by how much, without consuming anything (head never
  * moves; a drain after this call returns exactly what it would have returned without it).  Mailboxes [first_sub,
  * first_sub+n) are visited in cyclic id order from start_sub, as by cpbus_drain_ready; only subscribed ones count (the implicit
@@ -680,6 +711,13 @@ int cpbus_group_drain(cpbus_group_t* g, uint32_t sub_id, cpbus_event* out, size_
 int cpbus_group_drain_ready(cpbus_group_t* g, uint32_t first_sub, uint32_t n, uint32_t start_sub,
                             cpbus_event* out, size_t cap, cpbus_ready* ready, size_t ready_cap,
                             size_t* n_ready, size_t* total, uint32_t* next_sub);
+/* acknowledged drains: _take_ready walks the shards as _drain_ready does; _ack_many gives each shard its elements, in array
+ * order, in one cpbus_ack_many call */
+int cpbus_group_take_ready(cpbus_group_t* g, uint32_t first_sub, uint32_t n, uint32_t start_sub,
+                           cpbus_event* out, size_t cap, cpbus_ready* ready, size_t ready_cap,
+                           size_t* n_ready, size_t* total, uint32_t* next_sub);
+int cpbus_group_ack_many(cpbus_group_t* g, const uint32_t* sub_ids, const uint32_t* counts, uint32_t n, int* status,
+                         uint32_t* applied);
 /* _lagging walks the shards in the single call's cyclic order with the cap that is left (as _drain_ready) and sums the
  * summaries (backlog_max: the maximum); _blockers evaluates the group's staged remainder and clock on every shard. */
 int cpbus_group_lagging(cpbus_group_t* g, uint32_t first_sub, uint32_t n, uint32_t start_sub, uint32_t min_backlog,
