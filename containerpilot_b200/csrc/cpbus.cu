@@ -6,6 +6,7 @@
 // There is NO CPU data path: without a CUDA device cpbus_create fails with
 // CPBUS_ENODEV, and nothing here touches oracle/.
 #include "cpbus_kernels.cuh"
+#include "cuda_owned.hpp"
 
 #include <algorithm>
 #include <chrono>
@@ -22,6 +23,7 @@
 #include <vector>
 
 using namespace cpbus_dev;
+using namespace cuda_owned;
 
 namespace {
 
@@ -401,28 +403,27 @@ struct cpbus : HostFront {
   bool lossless = false, use_digest = false;
 
   // HBM-resident state (SoA, one entry per subscriber of this shard)
-  cpbus_event* d_ring = nullptr;          // N * R records: each mailbox is one contiguous 32*R-byte ring
-  SubCtl* d_ctl = nullptr;                // N control blocks: {tail, head, digest, mask}, one sector each
-  DevTimer* d_timers = nullptr;           // N * K
-  DevStats* d_stats = nullptr;
-  uint64_t* d_pow = nullptr;              // P^0..: digest multiplier powers, TMA-loaded by every CTA
-  unsigned char* d_desc = nullptr;        // per-launch batch descriptor (CTA 0 writes, the others read)
-  unsigned long long* d_desc_ready = nullptr;
+  DeviceBuf<cpbus_event> d_ring;          // N * R records: each mailbox is one contiguous 32*R-byte ring
+  DeviceBuf<SubCtl> d_ctl;                // N control blocks: {tail, head, digest, mask}, one sector each
+  DeviceBuf<DevTimer> d_timers;           // N * K
+  DeviceBuf<DevStats> d_stats;
+  DeviceBuf<uint64_t> d_pow;              // P^0..: digest multiplier powers, TMA-loaded by every CTA
+  DeviceBuf<unsigned char> d_desc;        // per-launch batch descriptor (CTA 0 writes, the others read)
+  DeviceBuf<unsigned long long> d_desc_ready;
   unsigned long long launch_seq = 0;
-  cpbus_event* d_batch_local = nullptr;    // staged ingest: CTA 0's local copy of a peer batch
-  cpbus_event* d_admit_batch = nullptr;    // lossless stream: local copy of a slot's undelivered records for the admission pass
+  DeviceBuf<cpbus_event> d_batch_local;    // staged ingest: CTA 0's local copy of a peer batch
+  DeviceBuf<cpbus_event> d_admit_batch;    // lossless stream: local copy of a slot's undelivered records for the admission pass
   static constexpr int kPrefetch = 3;      // fused ingest: later batches pulled over NVLink by earlier launches
-  cpbus_event* d_prefetch[kPrefetch] = {};
+  DeviceBuf<cpbus_event> d_prefetch[kPrefetch];
   const void* pf_ptr[kPrefetch] = {};      // which peer batch sits in d_prefetch[i] ...
   size_t pf_n[kPrefetch] = {};
   unsigned long long pf_seq[kPrefetch] = {};   // ... and which launch wrote it
   int pf_next = 0;
   std::vector<void*> shared_owned, shared_mapped;   // cpbus_shared_alloc / cpbus_shared_open
   // stream mode (cpbus_stream_*): device-managed prefetch of later stream batches + sticky error word
-  unsigned long long* d_pf_state = nullptr;   // [kStreamPrefetch]: which stream batch sits in d_prefetch[i]
-  cpbus_event* d_pf_buf = nullptr;            // kStreamPrefetch x batch_cap records (one allocation)
-  unsigned int* h_err = nullptr;              // pinned + mapped: kErr* bits written by the fan-out kernel
-  unsigned int* d_err = nullptr;              // device alias of h_err
+  DeviceBuf<unsigned long long> d_pf_state;   // [kStreamPrefetch]: which stream batch sits in d_prefetch[i]
+  DeviceBuf<cpbus_event> d_pf_buf;            // kStreamPrefetch x batch_cap records (one allocation)
+  MappedBuf<unsigned int> h_err;              // kErr* bits written by the fan-out kernel
   uint32_t stream_spin_us = 0;                // bound of the in-kernel wait for a stream batch (0 = 2 s)
   // follower launches (cpbus_stream_fanout_next): enqueued without the batch's shape, resolved lazily (follow_resolve)
   static constexpr int kFollowMax = 8;        // outstanding at most; the next one resolves first
@@ -431,65 +432,65 @@ struct cpbus : HostFront {
   enum FollowKind { kFollower, kRound, kConsumeAll };
   struct FollowPending { cpbus_stream* st; unsigned long long launch_seq; int rec; FollowKind kind; };
   std::vector<FollowPending> follow_q;        // outstanding, in launch order
-  RoundRec* h_round = nullptr;                // pinned + mapped: kFollowMax records written by the round agree kernels
-  RoundRec* d_round_rec = nullptr;            // device alias of h_round
-  RoundDev* d_round = nullptr;                // lossless rounds: the device copy of the room bound and clock, round scratch
-  FollowRec* h_follow = nullptr;              // pinned + mapped: kFollowMax records written by the lead CTAs
-  FollowRec* d_follow = nullptr;              // device alias of h_follow
-  unsigned long long* d_follow_clock = nullptr;   // 4 words: {watermark, launch ordinal} by launch parity
+  MappedBuf<RoundRec> h_round;                // kFollowMax records written by the round agree kernels
+  DeviceBuf<RoundDev> d_round;                // lossless rounds: the device copy of the room bound and clock, round scratch
+  MappedBuf<FollowRec> h_follow;              // kFollowMax records written by the lead CTAs
+  DeviceBuf<unsigned long long> d_follow_clock;   // 4 words: {watermark, launch ordinal} by launch parity
   int follow_next = 0;
-  cudaEvent_t follow_done = nullptr;
+  CudaEvent follow_done;
   std::recursive_mutex follow_mu;              // the queue, when stats or drains on another thread resolve it
   // accounting of device-published batches (cpbus_publish_device*, cpbus_stream_fanout): done by the kernel's lead CTA
-  DevPubAcct* d_acct = nullptr;
-  DevPubAcct* h_acct = nullptr;               // pinned staging for cpbus_stats / cpbus_debug_events / cpbus_publish_counts
-  cpbus_event* d_drain = nullptr; size_t drain_cap = 0;        // cpbus_drain_many staging
-  uint2* d_drain_idx = nullptr; size_t drain_idx_cap = 0;
-  // cpbus_drain_ready staging (records go to d_drain): header + tile counter + tile status, ready list, ring slot of each run
-  unsigned long long* d_ready_lb = nullptr; size_t ready_lb_tiles = 0;
-  cpbus_ready* d_ready = nullptr; uint32_t* d_ready_slot = nullptr; size_t ready_stage_cap = 0;
-  unsigned long long* h_ready_hdr = nullptr;   // pinned + mapped: the header the gather kernel hands to the host
-  unsigned long long* d_ready_hdr = nullptr;   // device alias of h_ready_hdr
+  DeviceBuf<DevPubAcct> d_acct;
+  // pinned staging for cpbus_stats / cpbus_debug_events / cpbus_publish_counts: the fields of a DevPubAcct before pair_key
+  PinnedBuf<unsigned char> h_acct;
+  DevPubAcct* host_acct() const { return reinterpret_cast<DevPubAcct*>(h_acct.get()); }
+  DeviceBuf<cpbus_event> d_drain;             // cpbus_drain_many staging (grown)
+  DeviceBuf<uint2> d_drain_idx;
+  // cpbus_drain_ready staging (records go to d_drain; grown): header + tile counter + tile status, ready list, ring
+  // slot of each run, and the header the gather kernel hands to the host
+  DeviceBuf<unsigned long long> d_ready_lb;
+  DeviceBuf<cpbus_ready> d_ready; DeviceBuf<uint32_t> d_ready_slot;
+  MappedBuf<unsigned long long> h_ready_hdr;
   // cpbus_lagging / cpbus_blockers: look-back and summary words sized for every subscriber, the header the scans hand to the
-  // host, the blocker ids (lossless buses) and the lagging entries (grown on demand); all but d_lag_lb pinned + mapped
-  unsigned long long* d_lag_lb = nullptr;
-  unsigned long long* h_lag_hdr = nullptr; unsigned long long* d_lag_hdr = nullptr;
-  uint32_t* h_block = nullptr; uint32_t* d_block = nullptr;
-  cpbus_lag* h_lag = nullptr; cpbus_lag* d_lag = nullptr; size_t lag_cap = 0;
+  // host, the blocker ids (lossless buses) and the lagging entries (grown)
+  DeviceBuf<unsigned long long> d_lag_lb;
+  MappedBuf<unsigned long long> h_lag_hdr;
+  MappedBuf<uint32_t> h_block;
+  MappedBuf<cpbus_lag> h_lag;
   uint32_t subs_per_warp = 0;             // 0 = auto
   uint32_t order_block = 0;               // mask order is built per block of this many consecutive subscribers (0 = one global order)
   bool pdl = true;                        // programmatic dependent launch of consecutive fan-outs
-  cudaEvent_t launched = nullptr;         // recorded after the latest fan-out (step results are read on the copy stream)
+  CudaEvent launched;                     // recorded after the latest fan-out (step results are read on the copy stream)
   int hints = -1;                         // -1 auto; bit0: control blocks / timer slots evict_last in L2
   static constexpr int kFoldSlots = 8;
-  unsigned long long* d_fold = nullptr;   // kFoldSlots x 4 words
-  cudaEvent_t fold_done[kFoldSlots] = {};
+  DeviceBuf<unsigned long long> d_fold;   // kFoldSlots x 4 words
+  CudaEvent fold_done[kFoldSlots];
   uint32_t fold_next = 0;
   static constexpr int kStage = 8;         // staging ring: the host may run several flushes ahead of the GPU
   static constexpr int kDevSlots = 64, kDevEpoch = 16;
-  cpbus_event* d_stage = nullptr;          // kDevSlots x batch_cap records: device side of the staging ring
-  cudaEvent_t epoch_done[kDevSlots / kDevEpoch] = {};   // on the bus stream, after the last fan-out of each epoch of slots
+  DeviceBuf<cpbus_event> d_stage;          // kDevSlots x batch_cap records: device side of the staging ring
+  CudaEvent epoch_done[kDevSlots / kDevEpoch];   // on the bus stream, after the last fan-out of each epoch of slots
   uint32_t dev_slot = 0;
-  cpbus_event* h_batch[kStage] = {};       // pinned staging
-  cudaEvent_t h2d_done[kStage] = {};       // on copy_stream: batch c has reached HBM
-  cudaStream_t copy_stream = nullptr;      // H2D of batch i+1 overlaps the fan-out of batch i
-  cudaStream_t result_stream = nullptr;    // D2H of step results: must not queue in front of the next batch's H2D
+  PinnedBuf<cpbus_event> h_batch[kStage];  // staging
+  CudaEvent h2d_done[kStage];              // on copy_stream: batch c has reached HBM
+  CudaStream copy_stream;                  // H2D of batch i+1 overlaps the fan-out of batch i
+  CudaStream result_stream;                // D2H of step results: must not queue in front of the next batch's H2D
   // per-launch results written by the fan-out kernel itself (no extra kernel to read a step's result)
-  DevResultSlot* d_result = nullptr;       // kResultRing x kResultSub slots
-  DevResultSlot* h_result = nullptr;       // pinned, kFoldSlots tickets x kResultSub
-  cudaEvent_t result_done[8] = {};
+  DeviceBuf<DevResultSlot> d_result;       // kResultRing x kResultSub slots
+  PinnedBuf<DevResultSlot> h_result;       // kFoldSlots tickets x kResultSub
+  CudaEvent result_done[8];
   uint32_t result_next = 0;
-  DevStats* h_stats = nullptr;            // pinned
-  unsigned long long* h_fold = nullptr;   // pinned
+  PinnedBuf<DevStats> h_stats;
+  PinnedBuf<unsigned long long> h_fold;
   int cur = 0;
 
   // registry mirror (events/bus.go:13 `registry map[*Subscriber]bool`)
   std::vector<uint32_t> h_mask;
   std::vector<uint8_t> h_active;
   std::vector<uint8_t> h_npairs;          // second-level filter: exact {code, source} cases per subscriber (empty until first use)
-  uint2* d_pairs = nullptr;               // N x CPBUS_MAX_PAIRS, allocated by the first cpbus_subscribe_pairs
+  DeviceBuf<uint2> d_pairs;               // N x CPBUS_MAX_PAIRS, allocated by the first cpbus_subscribe_pairs (pair_tables)
   uint32_t n_paired = 0;                  // active subscribers with a pair table
-  uint32_t* d_order = nullptr;            // active subscribers sorted by code mask (ORDERED fan-out)
+  DeviceBuf<uint32_t> d_order;            // active subscribers sorted by code mask (ORDERED fan-out)
   uint32_t n_order = 0, n_filtered = 0;   // n_filtered: active subscribers whose mask is not CPBUS_MASK_ALL
   bool order_dirty = true;
   uint32_t n_next = 0, n_active = 0;
@@ -501,7 +502,7 @@ struct cpbus : HostFront {
 
   // CPBUS_CFG_SPARSE_TICKS: the armed slots by due time, and the plan of a sparse flush (entries, record indices, and the
   // {mailbox, record} pairs it is sorted from), staged in pinned memory as [entries | indices] and copied on the copy stream
-  // into a device buffer that grows on demand.  CPBUS_CFG_SPARSE_RECORDS: records are planned too, from the subscription
+  // into a device buffer (both grown).  CPBUS_CFG_SPARSE_RECORDS: records are planned too, from the subscription
   // index.
   bool sparse = false, sparse_records = false;
   DueIndex due;
@@ -510,22 +511,21 @@ struct cpbus : HostFront {
   std::vector<cpbus_plan_entry> plan;
   std::vector<uint32_t> plan_idx;
   std::vector<uint64_t> plan_pairs;
-  unsigned char* h_plan = nullptr; unsigned char* d_plan = nullptr; size_t plan_bytes_cap = 0;
-  cudaEvent_t plan_done = nullptr;        // on copy_stream: the plan (and the batch in front of it) has reached HBM
-  cudaEvent_t records_done = nullptr;     // on the bus stream: the record kernel is done with the plan
-  // CPBUS_CFG_DROP_MISSED_TICKS on a sparse bus: the slots a catch-up moves (host index), and their device copy
+  PinnedBuf<unsigned char> h_plan; DeviceBuf<unsigned char> d_plan;
+  CudaEvent plan_done;                    // on copy_stream: the plan (and the batch in front of it) has reached HBM
+  CudaEvent records_done;                 // on the bus stream: the record kernel is done with the plan
+  // CPBUS_CFG_DROP_MISSED_TICKS on a sparse bus: the slots a catch-up moves (host index), and their device copy (grown)
   std::vector<uint32_t> catchup_slots;
-  uint32_t* d_catchup = nullptr; size_t catchup_cap = 0;
-  // the bulk membership calls (cpbus_unsubscribe_many, ...): device copy of the coalesced per-mailbox list, grown on demand
-  MemberOp* d_member = nullptr; size_t member_cap = 0;
-  // cpbus_timer_add_list: device copy of the armed slots' list, grown on demand
-  TimerArmOp* d_arm = nullptr; size_t arm_cap = 0;
+  DeviceBuf<uint32_t> d_catchup;
+  // the bulk membership calls (cpbus_unsubscribe_many, ...): device copy of the coalesced per-mailbox list (grown)
+  DeviceBuf<MemberOp> d_member;
+  // cpbus_timer_add_list: device copy of the armed slots' list (grown)
+  DeviceBuf<TimerArmOp> d_arm;
   // acknowledged drains (cpbus_take_ready / cpbus_ack_many): the take cursor of every mailbox, allocated (zero) by the first
-  // take; the ack list ([entries | elements], pinned staging and its device copy, grown on demand) and the statuses in
-  // mapped pinned memory
-  unsigned long long* d_taken = nullptr;
-  unsigned char* h_ack = nullptr; unsigned char* d_ack = nullptr; size_t ack_bytes_cap = 0;
-  int* h_ack_status = nullptr; int* d_ack_status = nullptr; size_t ack_status_cap = 0;
+  // take; the ack list ([entries | elements], pinned staging and its device copy, grown) and the statuses (grown)
+  DeviceBuf<unsigned long long> d_taken;
+  PinnedBuf<unsigned char> h_ack; DeviceBuf<unsigned char> d_ack;
+  MappedBuf<int> h_ack_status;
 
   // intern table (Event.Source string <-> u32)
   std::unordered_map<std::string, uint32_t> intern;
@@ -571,17 +571,6 @@ int rebuild_order(cpbus* b);
 int dev_guard(cpbus* b) {
   CK(cudaSetDevice(b->device));
   return CPBUS_OK;
-}
-
-// Pinned host memory that the device writes through a mapping: *h and its device alias *d, set only on success.
-template <class T>
-cudaError_t mapped_alloc(size_t bytes, T** h, T** d) {
-  void *ph = nullptr, *pd = nullptr;
-  cudaError_t e = cudaHostAlloc(&ph, bytes, cudaHostAllocMapped);
-  if (e != cudaSuccess) return e;
-  if ((e = cudaHostGetDevicePointer(&pd, ph, 0)) != cudaSuccess) { cudaFreeHost(ph); return e; }
-  *h = static_cast<T*>(ph); *d = static_cast<T*>(pd);
-  return cudaSuccess;
 }
 
 // How long the host waits for a stream's consumers or publisher (cpbus_stream_set_timeout; 0 = 2 s).
@@ -801,7 +790,7 @@ int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, co
   p.desc_ready = b->d_desc_ready + (p.launch_seq & 1) * 16; p.w_now = w;
   p.result = result_slot(b, p.launch_seq); p.result_next = result_slot(b, p.launch_seq + 1);
   p.batch_local = b->d_batch_local; p.staged = (uint32_t)o.staged;
-  p.err_word = b->d_err; p.acct = o.account ? b->d_acct : nullptr;
+  p.err_word = b->h_err.dev(); p.acct = o.account ? b->d_acct.get() : nullptr;
   p.pf_state = b->d_pf_state; p.pf_buf = b->d_pf_buf; p.pf_stride = b->B; p.spin_us = b->stream_spin_us;
   if (sa) {
     p.stream_hdr = sa->hdr; p.stream_ack = sa->ack; p.stream_seq = sa->seq; p.stream_next_hdr = sa->next_hdr;
@@ -833,7 +822,7 @@ int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, co
   // PAIRS build (some subscriber has exact {code, source} cases): the timers build with the second-level test in its
   // general path; subscribers without a pair table take the same paths as before
   const bool pairs_on = b->n_paired > 0 && b->d_pairs;
-  p.pairs = pairs_on ? b->d_pairs : nullptr;
+  p.pairs = pairs_on ? b->d_pairs.get() : nullptr;
   size_t smem = fanout_smem_bytes(p.smem_cap) + (pairs_on ? kPairFilterBytes : 0);   // + the batch's {code, source} presence filter
   if (!pairs_on && !p.timers_on && b->n_filtered > 0) {
     if (b->order_dirty) { const int rc_order = rebuild_order(b); if (rc_order) return rc_order; }
@@ -964,14 +953,10 @@ size_t sparse_max_deliveries(const cpbus* b) { return std::max<size_t>(1024, b->
 // The pinned plan buffer is free for `bytes`: the previous plan has left it, or both buffers are regrown (behind every
 // kernel that may still read the old device buffer).
 int plan_room(cpbus* b, size_t bytes) {
-  if (bytes <= b->plan_bytes_cap) { CK(cudaEventSynchronize(b->plan_done)); return CPBUS_OK; }
+  if (bytes <= b->d_plan.size() && bytes <= b->h_plan.size()) { CK(cudaEventSynchronize(b->plan_done)); return CPBUS_OK; }
   CK(cudaStreamSynchronize(b->stream)); CK(cudaStreamSynchronize(b->copy_stream));
-  cudaFree(b->d_plan); cudaFreeHost(b->h_plan);
-  b->d_plan = nullptr; b->h_plan = nullptr; b->plan_bytes_cap = 0;
-  const size_t cap = std::max<size_t>(bytes, 64 << 10);
-  CK(cudaMalloc((void**)&b->d_plan, cap));
-  CK(cudaMallocHost((void**)&b->h_plan, cap));
-  b->plan_bytes_cap = cap;
+  CK(b->d_plan.grow(bytes, 64 << 10));
+  CK(b->h_plan.grow(bytes, 64 << 10));
   return CPBUS_OK;
 }
 
@@ -997,7 +982,7 @@ int launch_sparse(cpbus* b, uint64_t w) {
     if (n) { if ((rc = await_copy(b, b->plan_done))) return rc; }
     else CK(cudaStreamWaitEvent(b->stream, b->plan_done, 0));
     RecordScatterParams p{};
-    p.list = reinterpret_cast<const uint4*>(b->d_plan); p.n_list = (uint32_t)n_list;
+    p.list = reinterpret_cast<const uint4*>(b->d_plan.get()); p.n_list = (uint32_t)n_list;
     p.idx = reinterpret_cast<const uint32_t*>(b->d_plan + list_bytes); p.batch = d_dst;
     p.ring = b->d_ring; p.ctl = b->d_ctl; p.timers = b->d_timers; p.stats = b->d_stats; p.pow_table = b->d_pow;
     p.launch_seq = ++b->launch_seq;
@@ -1066,7 +1051,7 @@ int admit_pass(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, bool*
   const uint32_t threads = 256, grid = (b->n_next + threads - 1) / threads;
   admit_kernel<<<grid, threads, 0, b->stream>>>(d_src, n, w, b->d_ctl, b->d_timers, b->n_next, b->R, b->K,
                                                 b->cfg.sub_id_base, b->n_timers > 0 && b->K > 0, b->d_stats,
-                                                b->n_paired > 0 ? b->d_pairs : nullptr);
+                                                b->n_paired > 0 ? b->d_pairs.get() : nullptr);
   CK(cudaGetLastError());
   b->st.kernel_launches++; b->st.admit_passes++;
   CK(cudaMemcpyAsync(&b->h_stats->admit_overflow, &b->d_stats->admit_overflow, 4 * sizeof(unsigned long long),
@@ -1270,13 +1255,9 @@ int catch_up(cpbus* b, uint64_t now) {
     due_catchup(b->due, b->h_timers, now, &b->catchup_slots);
     n = b->catchup_slots.size();
     if (!n) return CPBUS_OK;
-    if (n > b->catchup_cap) {   // (behind every kernel that may still read the old list)
+    if (n > b->d_catchup.size()) {   // (behind every kernel that may still read the old list)
       CK(cudaStreamSynchronize(b->stream));
-      cudaFree(b->d_catchup);
-      b->d_catchup = nullptr; b->catchup_cap = 0;
-      const size_t cap = std::max<size_t>(n, 1024);
-      CK(cudaMalloc((void**)&b->d_catchup, cap * sizeof(uint32_t)));
-      b->catchup_cap = cap;
+      CK(b->d_catchup.grow(n, 1024));
     }
     // (pageable source: the call returns once the list has been taken, and the copy runs in stream order)
     CK(cudaMemcpyAsync(b->d_catchup, b->catchup_slots.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice, b->stream));
@@ -1587,69 +1568,58 @@ int cpbus_create(const cpbus_config* cfg, cpbus_t** out) try {
     b->own_stream = true;
   }
   const size_t N = b->N;
-#define ALLOC(ptr, bytes)                                                                     \
-  if (cudaMalloc((void**)&(ptr), (bytes)) != cudaSuccess) {                                   \
-    snprintf(g_cuda_err, sizeof(g_cuda_err), "cudaMalloc(%zu) failed", (size_t)(bytes));     \
-    return fail(CPBUS_ENOMEM);                                                                \
-  }
-  ALLOC(b->d_ring, N * R * sizeof(cpbus_event));
-  ALLOC(b->d_ctl, N * sizeof(SubCtl)); ALLOC(b->d_order, N * 4);
-  if (K) ALLOC(b->d_timers, N * K * sizeof(DevTimer));
-  ALLOC(b->d_stats, sizeof(DevStats)); ALLOC(b->d_fold, 32 * cpbus::kFoldSlots); ALLOC(b->d_pow, kPowTableLen * 8);
-  ALLOC(b->d_desc, 2 * ((fanout_desc_bytes(2048) + 255) & ~(size_t)255)); ALLOC(b->d_desc_ready, 256);
+  // device memory: CPBUS_ENOMEM, with the size the runtime refused
+  auto alloc = [](auto& buf, size_t n) {
+    if (buf.alloc(n) == cudaSuccess) return true;
+    snprintf(g_cuda_err, sizeof(g_cuda_err), "cudaMalloc(%zu) failed", n * sizeof(*buf.get()));
+    return false;
+  };
+  if (!alloc(b->d_ring, N * R) || !alloc(b->d_ctl, N) || !alloc(b->d_order, N) || (K && !alloc(b->d_timers, N * K)) ||
+      !alloc(b->d_stats, 1) || !alloc(b->d_fold, 4 * cpbus::kFoldSlots) || !alloc(b->d_pow, kPowTableLen) ||
+      !alloc(b->d_desc, 2 * ((fanout_desc_bytes(2048) + 255) & ~(size_t)255)) || !alloc(b->d_desc_ready, 32))
+    return fail(CPBUS_ENOMEM);
   if (cudaMemsetAsync(b->d_desc_ready, 0, 256, b->stream) != cudaSuccess) return fail(CPBUS_ECUDA);
-  if (cudaStreamCreateWithFlags(&b->copy_stream, cudaStreamNonBlocking) != cudaSuccess) return fail(CPBUS_ECUDA);
-  if (cudaStreamCreateWithFlags(&b->result_stream, cudaStreamNonBlocking) != cudaSuccess) return fail(CPBUS_ECUDA);
-  if (cudaEventCreateWithFlags(&b->launched, cudaEventDisableTiming) != cudaSuccess) return fail(CPBUS_ECUDA);
-  if (b->sparse && (cudaEventCreateWithFlags(&b->plan_done, cudaEventDisableTiming) != cudaSuccess ||
-                    cudaEventCreateWithFlags(&b->records_done, cudaEventDisableTiming) != cudaSuccess))
+  if (b->copy_stream.create() != cudaSuccess || b->result_stream.create() != cudaSuccess || b->launched.create() != cudaSuccess)
     return fail(CPBUS_ECUDA);
-  ALLOC(b->d_stage, (size_t)cpbus::kDevSlots * B * sizeof(cpbus_event));
-  for (int i = 0; i < cpbus::kDevSlots / cpbus::kDevEpoch; i++)
-    if (cudaEventCreateWithFlags(&b->epoch_done[i], cudaEventDisableTiming) != cudaSuccess) return fail(CPBUS_ECUDA);
+  if (b->sparse && (b->plan_done.create() != cudaSuccess || b->records_done.create() != cudaSuccess)) return fail(CPBUS_ECUDA);
+  if (!alloc(b->d_stage, (size_t)cpbus::kDevSlots * B)) return fail(CPBUS_ENOMEM);
+  for (CudaEvent& e : b->epoch_done) if (e.create() != cudaSuccess) return fail(CPBUS_ECUDA);
   for (int i = 0; i < cpbus::kStage; i++) {
-    if (cudaMallocHost((void**)&b->h_batch[i], (size_t)B * sizeof(cpbus_event)) != cudaSuccess) return fail(CPBUS_ENOMEM);
-    if (cudaEventCreateWithFlags(&b->h2d_done[i], cudaEventDisableTiming) != cudaSuccess) return fail(CPBUS_ECUDA);
+    if (b->h_batch[i].alloc(B) != cudaSuccess) return fail(CPBUS_ENOMEM);
+    if (b->h2d_done[i].create() != cudaSuccess) return fail(CPBUS_ECUDA);
   }
-  ALLOC(b->d_batch_local, (size_t)B * sizeof(cpbus_event));
+  if (!alloc(b->d_batch_local, B)) return fail(CPBUS_ENOMEM);
   if (b->lossless) {
-    ALLOC(b->d_admit_batch, (size_t)B * sizeof(cpbus_event));
     // lossless rounds (cpbus_stream_round_next): device state and the host records, allocated here rather than by the
     // first round, while no round of any shard can be waiting on the device
-    ALLOC(b->d_round, sizeof(RoundDev));
+    if (!alloc(b->d_admit_batch, B) || !alloc(b->d_round, 1)) return fail(CPBUS_ENOMEM);
     RoundDev init{};
     init.room_full = R;
     if (cudaMemcpyAsync(b->d_round, &init, sizeof(init), cudaMemcpyHostToDevice, b->stream) != cudaSuccess) return fail(CPBUS_ECUDA);
-    if (mapped_alloc(sizeof(RoundRec) * cpbus::kFollowMax, &b->h_round, &b->d_round_rec) != cudaSuccess) return fail(CPBUS_ENOMEM);
+    if (b->h_round.alloc(cpbus::kFollowMax) != cudaSuccess) return fail(CPBUS_ENOMEM);
     if ((rc = preload_round_kernels(b))) return fail(rc);
   } else {   // followers (cpbus_stream_fanout_next): their records and the clock words, zeroed
-    if (mapped_alloc(sizeof(FollowRec) * cpbus::kFollowMax, &b->h_follow, &b->d_follow) != cudaSuccess) return fail(CPBUS_ENOMEM);
-    ALLOC(b->d_follow_clock, 4 * sizeof(unsigned long long));
+    if (b->h_follow.alloc(cpbus::kFollowMax) != cudaSuccess || !alloc(b->d_follow_clock, 4)) return fail(CPBUS_ENOMEM);
     if (cudaMemsetAsync(b->d_follow_clock, 0, 4 * sizeof(unsigned long long), b->stream) != cudaSuccess) return fail(CPBUS_ECUDA);
   }
-  if (cudaEventCreateWithFlags(&b->follow_done, cudaEventDisableTiming) != cudaSuccess) return fail(CPBUS_ECUDA);
-  ALLOC(b->d_pf_buf, (size_t)kStreamPrefetch * B * sizeof(cpbus_event)); ALLOC(b->d_pf_state, 64);
-  ALLOC(b->d_acct, sizeof(DevPubAcct));
+  if (b->follow_done.create() != cudaSuccess) return fail(CPBUS_ECUDA);
+  if (!alloc(b->d_pf_buf, (size_t)kStreamPrefetch * B) || !alloc(b->d_pf_state, 8) || !alloc(b->d_acct, 1))
+    return fail(CPBUS_ENOMEM);
   if (cudaMemsetAsync(b->d_pf_state, 0, 64, b->stream) != cudaSuccess ||
       cudaMemsetAsync(b->d_acct, 0, sizeof(DevPubAcct), b->stream) != cudaSuccess) return fail(CPBUS_ECUDA);
-  if (mapped_alloc(64, &b->h_err, &b->d_err) != cudaSuccess) return fail(CPBUS_ENOMEM);
+  if (b->h_err.alloc(16) != cudaSuccess) return fail(CPBUS_ENOMEM);
   memset(b->h_err, 0, 64);
   // cpbus_lagging / cpbus_blockers: allocated here, so that neither query allocates (or frees) while a round may wait
-  ALLOC(b->d_lag_lb, (kLagLbOffset + (N + kReadyTile - 1) / kReadyTile) * sizeof(unsigned long long));
-  if (mapped_alloc(kLagHdrWords * sizeof(unsigned long long), &b->h_lag_hdr, &b->d_lag_hdr) != cudaSuccess) return fail(CPBUS_ENOMEM);
-  if (b->lossless && mapped_alloc(N * sizeof(uint32_t), &b->h_block, &b->d_block) != cudaSuccess) return fail(CPBUS_ENOMEM);
-  if (cudaMallocHost((void**)&b->h_acct, offsetof(DevPubAcct, pair_key)) != cudaSuccess) return fail(CPBUS_ENOMEM);
-  for (int i = 0; i < cpbus::kPrefetch; i++) ALLOC(b->d_prefetch[i], (size_t)B * sizeof(cpbus_event));
-  ALLOC(b->d_result, sizeof(DevResultSlot) * kResultRing * kResultSub);
+  if (!alloc(b->d_lag_lb, kLagLbOffset + (N + kReadyTile - 1) / kReadyTile) || b->h_lag_hdr.alloc(kLagHdrWords) != cudaSuccess ||
+      (b->lossless && b->h_block.alloc(N) != cudaSuccess) || b->h_acct.alloc(offsetof(DevPubAcct, pair_key)) != cudaSuccess)
+    return fail(CPBUS_ENOMEM);
+  for (auto& d : b->d_prefetch) if (!alloc(d, B)) return fail(CPBUS_ENOMEM);
+  if (!alloc(b->d_result, (size_t)kResultRing * kResultSub)) return fail(CPBUS_ENOMEM);
   if (cudaMemsetAsync(b->d_result, 0, sizeof(DevResultSlot) * kResultRing * kResultSub, b->stream) != cudaSuccess) return fail(CPBUS_ECUDA);
-  if (cudaMallocHost((void**)&b->h_result, sizeof(DevResultSlot) * 8 * kResultSub) != cudaSuccess) return fail(CPBUS_ENOMEM);
-  for (int i = 0; i < 8; i++)
-    if (cudaEventCreateWithFlags(&b->result_done[i], cudaEventDisableTiming) != cudaSuccess) return fail(CPBUS_ECUDA);
-#undef ALLOC
-  if (cudaMallocHost((void**)&b->h_stats, sizeof(DevStats)) != cudaSuccess) return fail(CPBUS_ENOMEM);
-  if (cudaMallocHost((void**)&b->h_fold, 32 * cpbus::kFoldSlots) != cudaSuccess) return fail(CPBUS_ENOMEM);
-  for (int i = 0; i < cpbus::kFoldSlots; i++)
-    if (cudaEventCreateWithFlags(&b->fold_done[i], cudaEventDisableTiming) != cudaSuccess) return fail(CPBUS_ECUDA);
+  if (b->h_result.alloc((size_t)8 * kResultSub) != cudaSuccess) return fail(CPBUS_ENOMEM);
+  for (CudaEvent& e : b->result_done) if (e.create() != cudaSuccess) return fail(CPBUS_ECUDA);
+  if (b->h_stats.alloc(1) != cudaSuccess || b->h_fold.alloc(4 * cpbus::kFoldSlots) != cudaSuccess) return fail(CPBUS_ENOMEM);
+  for (CudaEvent& e : b->fold_done) if (e.create() != cudaSuccess) return fail(CPBUS_ECUDA);
   // rings are NOT cleared: a slot is only ever read after it has been written (head/tail bound every read)
   bool ok = cudaMemsetAsync(b->d_ctl, 0, N * sizeof(SubCtl), b->stream) == cudaSuccess &&
             cudaMemsetAsync(b->d_stats, 0, sizeof(DevStats), b->stream) == cudaSuccess &&
@@ -1678,54 +1648,13 @@ int cpbus_destroy(cpbus_t* b) try {
   follow_resolve(b);
   cudaSetDevice(b->device);
   if (b->stream) cudaStreamSynchronize(b->stream);
-  while (!b->streams.empty()) cpbus_stream_close(b->streams.back());
-  if (b->h_follow) cudaFreeHost(b->h_follow);
-  cudaFree(b->d_follow_clock);
-  if (b->h_round) cudaFreeHost(b->h_round);
-  cudaFree(b->d_round);
-  if (b->follow_done) cudaEventDestroy(b->follow_done);
-  cudaFree(b->d_ring); cudaFree(b->d_ctl); cudaFree(b->d_order); cudaFree(b->d_pairs);
-  cudaFree(b->d_timers); cudaFree(b->d_stats); cudaFree(b->d_fold); cudaFree(b->d_pow); cudaFree(b->d_desc); cudaFree(b->d_desc_ready);
   if (b->copy_stream) cudaStreamSynchronize(b->copy_stream);
-  if (b->result_stream) { cudaStreamSynchronize(b->result_stream); cudaStreamDestroy(b->result_stream); }
-  for (int i = 0; i < cpbus::kStage; i++) {
-    if (b->h_batch[i]) cudaFreeHost(b->h_batch[i]);
-    if (b->h2d_done[i]) cudaEventDestroy(b->h2d_done[i]);
-  }
-  cudaFree(b->d_stage);
-  for (int i = 0; i < cpbus::kDevSlots / cpbus::kDevEpoch; i++) if (b->epoch_done[i]) cudaEventDestroy(b->epoch_done[i]);
-  if (b->copy_stream) cudaStreamDestroy(b->copy_stream);
-  if (b->launched) cudaEventDestroy(b->launched);
-  if (b->plan_done) cudaEventDestroy(b->plan_done);
-  if (b->records_done) cudaEventDestroy(b->records_done);
-  cudaFree(b->d_plan);
-  if (b->h_plan) cudaFreeHost(b->h_plan);
-  cudaFree(b->d_catchup);
-  cudaFree(b->d_member);
-  cudaFree(b->d_arm);
-  cudaFree(b->d_taken); cudaFree(b->d_ack);
-  if (b->h_ack) cudaFreeHost(b->h_ack);
-  if (b->h_ack_status) cudaFreeHost(b->h_ack_status);
-  cudaFree(b->d_drain);cudaFree(b->d_drain_idx);
-  cudaFree(b->d_ready_lb); cudaFree(b->d_ready); cudaFree(b->d_ready_slot);
-  if (b->h_ready_hdr) cudaFreeHost(b->h_ready_hdr);
-  cudaFree(b->d_lag_lb);
-  if (b->h_lag_hdr) cudaFreeHost(b->h_lag_hdr);
-  if (b->h_block) cudaFreeHost(b->h_block);
-  if (b->h_lag) cudaFreeHost(b->h_lag);
-  cudaFree(b->d_result); cudaFree(b->d_batch_local); cudaFree(b->d_admit_batch); cudaFree(b->d_pf_buf); cudaFree(b->d_pf_state); cudaFree(b->d_acct);
-  if (b->h_err) cudaFreeHost(b->h_err);
-  if (b->h_acct) cudaFreeHost(b->h_acct);
-  for (int i = 0; i < cpbus::kPrefetch; i++) cudaFree(b->d_prefetch[i]);
+  if (b->result_stream) cudaStreamSynchronize(b->result_stream);
+  while (!b->streams.empty()) cpbus_stream_close(b->streams.back());
   for (void* p : b->shared_mapped) cudaIpcCloseMemHandle(p);
   for (void* p : b->shared_owned) cudaFree(p);
-  if (b->h_result) cudaFreeHost(b->h_result);
-  for (int i = 0; i < 8; i++) if (b->result_done[i]) cudaEventDestroy(b->result_done[i]);
-  if (b->h_stats) cudaFreeHost(b->h_stats);
-  if (b->h_fold) cudaFreeHost(b->h_fold);
-  for (int i = 0; i < cpbus::kFoldSlots; i++) if (b->fold_done[i]) cudaEventDestroy(b->fold_done[i]);
   if (b->own_stream && b->stream) cudaStreamDestroy(b->stream);
-  delete b;
+  delete b;   // the owners free the bus's own memory, events and streams
   return CPBUS_OK;
 } CPBUS_CATCH
 
@@ -1811,6 +1740,19 @@ int cpbus_subscribe(cpbus_t* b, uint32_t mask, uint32_t* sub_id) { return cpbus_
 
 static int push_mask_words(cpbus* b, uint32_t first, uint32_t n);
 
+// The pair tables of every subscriber, allocated by the first subscription with pairs.
+static int pair_tables(cpbus* b) {
+  if (b->d_pairs) return CPBUS_OK;
+  const size_t n = (size_t)b->N * CPBUS_MAX_PAIRS;
+  if (b->d_pairs.alloc(n) != cudaSuccess) {
+    snprintf(g_cuda_err, sizeof(g_cuda_err), "cudaMalloc(pair tables) failed");
+    return CPBUS_ENOMEM;
+  }
+  CK(cudaMemsetAsync(b->d_pairs, 0xFF, n * sizeof(uint2), b->stream));   // every slot unused
+  b->h_npairs.assign(b->N, 0);
+  return CPBUS_OK;
+}
+
 int cpbus_subscribe_pairs(cpbus_t* b, uint32_t mask, const cpbus_pair* pairs, uint32_t n_pairs, uint32_t* sub_id) try {
   if (!b || n_pairs > CPBUS_MAX_PAIRS || (n_pairs && !pairs)) return CPBUS_EINVAL;
   for (uint32_t j = 0; j < n_pairs; j++) if (pairs[j].code >= CPBUS_N_CODES) return CPBUS_EINVAL;
@@ -1821,14 +1763,7 @@ int cpbus_subscribe_pairs(cpbus_t* b, uint32_t mask, const cpbus_pair* pairs, ui
     if (!((mask >> pairs[j].code) & 1u)) row[used++] = make_uint2(pairs[j].code, pairs[j].source_id);
   if (used == 0) return cpbus_subscribe_many(b, &mask, 1, sub_id);
   int rc = enter(b); if (rc) return rc;
-  if (!b->d_pairs) {
-    if (cudaMalloc((void**)&b->d_pairs, (size_t)b->N * CPBUS_MAX_PAIRS * sizeof(uint2)) != cudaSuccess) {
-      snprintf(g_cuda_err, sizeof(g_cuda_err), "cudaMalloc(pair tables) failed");
-      return CPBUS_ENOMEM;
-    }
-    CK(cudaMemsetAsync(b->d_pairs, 0xFF, (size_t)b->N * CPBUS_MAX_PAIRS * sizeof(uint2), b->stream));   // every slot unused
-    b->h_npairs.assign(b->N, 0);
-  }
+  if ((rc = pair_tables(b))) return rc;
   uint32_t id = 0;
   if ((rc = cpbus_subscribe_many(b, &mask, 1, &id))) return rc;
   const uint32_t l = id - b->cfg.sub_id_base;
@@ -1855,14 +1790,7 @@ int cpbus_subscribe_pairs_many(cpbus_t* b, const uint32_t* masks, const cpbus_pa
   }
   if ((uint64_t)b->n_next + n > b->N) return CPBUS_ENOSPC;
   int rc = enter(b); if (rc) return rc;
-  if (!b->d_pairs) {
-    if (cudaMalloc((void**)&b->d_pairs, (size_t)b->N * CPBUS_MAX_PAIRS * sizeof(uint2)) != cudaSuccess) {
-      snprintf(g_cuda_err, sizeof(g_cuda_err), "cudaMalloc(pair tables) failed");
-      return CPBUS_ENOMEM;
-    }
-    CK(cudaMemsetAsync(b->d_pairs, 0xFF, (size_t)b->N * CPBUS_MAX_PAIRS * sizeof(uint2), b->stream));   // every slot unused
-    b->h_npairs.assign(b->N, 0);
-  }
+  if ((rc = pair_tables(b))) return rc;
   uint32_t first = 0;
   if ((rc = cpbus_subscribe_many(b, masks, n, &first))) return rc;
   const uint32_t l0 = first - b->cfg.sub_id_base;
@@ -2086,13 +2014,7 @@ static int membership_many(cpbus* b, uint32_t n, int* status, uint32_t* applied,
       ops.back().clear_slots |= (uint32_t)t;
     }
     for (MemberOp& op : ops) op.mask_word = mask_word(b, op.local);
-    if (ops.size() > b->member_cap) {   // (every bulk call ends in a synchronisation: no kernel reads the old list)
-      cudaFree(b->d_member);
-      b->d_member = nullptr; b->member_cap = 0;
-      const size_t cap = std::max<size_t>(ops.size(), 1024);
-      CK(cudaMalloc((void**)&b->d_member, cap * sizeof(MemberOp)));
-      b->member_cap = cap;
-    }
+    CK(b->d_member.grow(ops.size(), 1024));   // (every bulk call ends in a synchronisation: no kernel reads the old list)
     // (pageable source: the call returns once the list has been taken, and the copy runs in stream order)
     CK(cudaMemcpyAsync(b->d_member, ops.data(), ops.size() * sizeof(MemberOp), cudaMemcpyHostToDevice, b->stream));
     membership_kernel<<<(uint32_t)((ops.size() + kThreads - 1) / kThreads), kThreads, 0, b->stream>>>(
@@ -2190,13 +2112,7 @@ int cpbus_timer_add_list(cpbus_t* b, const cpbus_timer_spec* specs, uint32_t n, 
   }
   if (!ops.empty()) {
     for (TimerArmOp& op : ops) op.mask_word = mask_word(b, op.local);
-    if (ops.size() > b->arm_cap) {   // (every list call ends in a synchronisation: no kernel reads the old list)
-      cudaFree(b->d_arm);
-      b->d_arm = nullptr; b->arm_cap = 0;
-      const size_t cap = std::max<size_t>(ops.size(), 1024);
-      CK(cudaMalloc((void**)&b->d_arm, cap * sizeof(TimerArmOp)));
-      b->arm_cap = cap;
-    }
+    CK(b->d_arm.grow(ops.size(), 1024));   // (every list call ends in a synchronisation: no kernel reads the old list)
     // (pageable source: the call returns once the list has been taken, and the copy runs in stream order)
     CK(cudaMemcpyAsync(b->d_arm, ops.data(), ops.size() * sizeof(TimerArmOp), cudaMemcpyHostToDevice, b->stream));
     timer_arm_kernel<<<(uint32_t)((ops.size() + kThreads - 1) / kThreads), kThreads, 0, b->stream>>>(
@@ -2422,32 +2338,31 @@ struct cpbus_stream {
   uint32_t get_off = 0;                      // lossless mode: records of batch get_seq + 1 already delivered
   uint32_t follow_out = 0;                   // follower launches of batches get_seq + 1 .. not yet resolved
   unsigned long long seen_seq = 0;           // highest batch whose release this consumer has seen from the host
-  RoundCursor* d_cursor = nullptr;           // lossless rounds (cpbus_stream_round_next): {batch, offset} on the device
+  DeviceBuf<RoundCursor> d_cursor;           // lossless rounds (cpbus_stream_round_next): {batch, offset} on the device
   unsigned long long stalled_rounds = 0;     // ... rounds resolved so far that moved nothing
   unsigned long long pub_seq = 0;            // publisher: publish ordinal stamped into the next record (CPBUS_PUT_STAMP)
   unsigned long long min_ack = 0;            // publisher: cached min over the consumers' acks
   // publisher staging: pinned payload + header buffers, copies on their own stream
   static constexpr int kStage = 8;
-  cpbus_event* h_stage[kStage] = {};
-  StreamHdr* h_hdr = nullptr;                // kStage headers
-  unsigned long long* h_ack = nullptr;       // kStreamMaxConsumers x 4 words
-  cudaEvent_t staged_done[kStage] = {};
-  cudaStream_t put_stream = nullptr;
+  PinnedBuf<cpbus_event> h_stage[kStage];
+  PinnedBuf<StreamHdr> h_hdr;                // kStage headers
+  PinnedBuf<unsigned long long> h_ack;       // kStreamMaxConsumers x 4 words
+  CudaEvent staged_done[kStage];
+  CudaStream put_stream;
   // lossless across processes (cpbus_stream_offer / _agree): admission rounds agreed so far, and this round's state
   unsigned long long agree_round = 0;
   bool offered = false;
   unsigned long long admit_q = 0;            // batch ordinal and shape of the latest cpbus_stream_admit (bounds an offer)
   size_t admit_n = 0;
-  StreamAgreeResult* h_agree = nullptr;      // pinned + mapped: written by the agree kernel
-  StreamAgreeResult* d_agree = nullptr;      // device alias of h_agree
-  cudaEvent_t agree_done = nullptr;
+  MappedBuf<StreamAgreeResult> h_agree;      // written by the agree kernel
+  CudaEvent agree_done;
 };
 
 static int stream_bind(cpbus_stream* st) {
   st->hdr = reinterpret_cast<StreamHdr*>(st->base + stream_hdr_off());
   st->ack = reinterpret_cast<unsigned long long*>(st->base + stream_ack_off(st->n_slots));
   st->payload = reinterpret_cast<cpbus_event*>(st->base + stream_payload_off(st->n_slots));
-  if (st->bus->lossless && cudaMalloc((void**)&st->d_cursor, sizeof(RoundCursor)) != cudaSuccess) {   // rounds' cursor
+  if (st->bus->lossless && st->d_cursor.alloc(1) != cudaSuccess) {   // rounds' cursor
     snprintf(g_cuda_err, sizeof(g_cuda_err), "cudaMalloc(%zu) failed", sizeof(RoundCursor));
     return CPBUS_ENOMEM;
   }
@@ -2475,13 +2390,13 @@ int cpbus_stream_create(cpbus_t* b, uint32_t n_slots, uint32_t n_consumers, cpbu
   if (cudaIpcGetMemHandle(&h, st->base) != cudaSuccess) { snprintf(g_cuda_err, sizeof(g_cuda_err), "cudaIpcGetMemHandle failed"); return fail(CPBUS_ECUDA); }
   memcpy(handle, &h, 64);
   if ((rc = stream_bind(st))) return fail(rc);
-  if (cudaStreamCreateWithFlags(&st->put_stream, cudaStreamNonBlocking) != cudaSuccess) return fail(CPBUS_ECUDA);
+  if (st->put_stream.create() != cudaSuccess) return fail(CPBUS_ECUDA);
   for (int i = 0; i < cpbus_stream::kStage; i++) {
-    if (cudaMallocHost((void**)&st->h_stage[i], (size_t)b->B * sizeof(cpbus_event)) != cudaSuccess) return fail(CPBUS_ENOMEM);
-    if (cudaEventCreateWithFlags(&st->staged_done[i], cudaEventDisableTiming) != cudaSuccess) return fail(CPBUS_ECUDA);
+    if (st->h_stage[i].alloc(b->B) != cudaSuccess) return fail(CPBUS_ENOMEM);
+    if (st->staged_done[i].create() != cudaSuccess) return fail(CPBUS_ECUDA);
   }
-  if (cudaMallocHost((void**)&st->h_hdr, sizeof(StreamHdr) * cpbus_stream::kStage) != cudaSuccess) return fail(CPBUS_ENOMEM);
-  if (cudaMallocHost((void**)&st->h_ack, (size_t)kStreamMaxConsumers * 32) != cudaSuccess) return fail(CPBUS_ENOMEM);
+  if (st->h_hdr.alloc(cpbus_stream::kStage) != cudaSuccess || st->h_ack.alloc((size_t)kStreamMaxConsumers * 4) != cudaSuccess)
+    return fail(CPBUS_ENOMEM);
   *out = st;
   return CPBUS_OK;
 } CPBUS_CATCH
@@ -2543,16 +2458,7 @@ int cpbus_stream_close(cpbus_stream_t* st) try {
   follow_resolve(b);   // (teardown: the records of outstanding followers are folded in before the stream goes)
   cudaSetDevice(b->device);
   cudaStreamSynchronize(b->stream);
-  if (st->put_stream) { cudaStreamSynchronize(st->put_stream); cudaStreamDestroy(st->put_stream); }
-  for (int i = 0; i < cpbus_stream::kStage; i++) {
-    if (st->h_stage[i]) cudaFreeHost(st->h_stage[i]);
-    if (st->staged_done[i]) cudaEventDestroy(st->staged_done[i]);
-  }
-  if (st->h_hdr) cudaFreeHost(st->h_hdr);
-  if (st->h_ack) cudaFreeHost(st->h_ack);
-  if (st->h_agree) cudaFreeHost(st->h_agree);
-  if (st->agree_done) cudaEventDestroy(st->agree_done);
-  cudaFree(st->d_cursor);
+  if (st->put_stream) cudaStreamSynchronize(st->put_stream);
   if (st->base) { if (st->owner) cudaFree(st->base); else if (!st->attached) cudaIpcCloseMemHandle(st->base); }
   b->streams.erase(std::remove(b->streams.begin(), b->streams.end(), st), b->streams.end());
   delete st;
@@ -2842,7 +2748,7 @@ int cpbus_stream_fanout_next(cpbus_stream_t* st) try {
   StreamArgs sa;
   LaunchOpts o;
   const cpbus_event* src = stream_launch(st, st->get_seq + 1 + st->follow_out, 0, /*final=*/true, sa, o);
-  sa.follow_rec = b->d_follow + ri; sa.follow_from_host = from_host;
+  sa.follow_rec = b->h_follow.dev() + ri; sa.follow_from_host = from_host;
   if ((rc = launch_fanout(b, src, b->B, b->now, o))) return rc;
   follow_end(st, cpbus::kFollower, ri);
   return CPBUS_OK;
@@ -2860,13 +2766,13 @@ int cpbus_stream_round_next(cpbus_stream_t* st) try {
   int rc = follow_begin(b, cpbus::kRound, &ri, &seed_bus); if (rc) return rc;
   const bool seed_cur = st->follow_out == 0;   // likewise the stream's cursor, while none of this stream's rounds is queued
   RoundParams P{};
-  P.dev = b->d_round; P.cur = st->d_cursor; P.rec = b->d_round_rec + ri;
+  P.dev = b->d_round; P.cur = st->d_cursor; P.rec = b->h_round.dev() + ri;
   P.hdr = st->hdr; P.payload = st->payload; P.ack = st->ack;
   P.n_slots = st->n_slots; P.B = st->B; P.consumer = st->consumer; P.n_consumers = st->n_consumers;
   P.round = st->agree_round + 1;
-  P.spin_us = b->stream_spin_us; P.err_word = b->d_err;
+  P.spin_us = b->stream_spin_us; P.err_word = b->h_err.dev();
   P.admit_batch = b->d_admit_batch; P.ctl = b->d_ctl; P.timers = b->d_timers; P.stats = b->d_stats;
-  P.pairs = b->n_paired > 0 ? b->d_pairs : nullptr;
+  P.pairs = b->n_paired > 0 ? b->d_pairs.get() : nullptr;
   P.n_subs = b->n_next; P.ring_cap = b->R; P.K = b->K; P.sub_base = b->cfg.sub_id_base;
   P.timers_armed = b->n_timers > 0 && b->K > 0;
   P.min_period = b->min_period; P.window = max_window(b);
@@ -2929,10 +2835,11 @@ int cpbus_stream_agree(cpbus_stream_t* st, size_t* m) try {
   if (!b->lossless || !st->offered) return CPBUS_EINVAL;
   int rc = dev_guard(b); if (rc) return rc;
   if ((rc = stream_error(b))) return rc;
-  if (!st->h_agree) CK(mapped_alloc(sizeof(StreamAgreeResult), &st->h_agree, &st->d_agree));
-  if (!st->agree_done) CK(cudaEventCreateWithFlags(&st->agree_done, cudaEventDisableTiming));
+  if (!st->h_agree) CK(st->h_agree.alloc(1));
+  if (!st->agree_done) CK(st->agree_done.create());
   const unsigned long long r = st->agree_round + 1;
-  stream_agree_kernel<<<1, kStreamMaxConsumers, 0, b->stream>>>(st->ack, st->n_consumers, r, b->stream_spin_us, st->d_agree, b->d_err);
+  stream_agree_kernel<<<1, kStreamMaxConsumers, 0, b->stream>>>(st->ack, st->n_consumers, r, b->stream_spin_us, st->h_agree.dev(),
+                                                                b->h_err.dev());
   CK(cudaGetLastError());
   b->st.kernel_launches++;
   st->agree_round = r; st->offered = false;
@@ -2994,10 +2901,8 @@ int cpbus_drain_many(cpbus_t* b, uint32_t first_sub, uint32_t n, cpbus_event* ou
   if (!id_range(b->cfg.sub_id_base, b->n_next, first_sub, n, &l)) return CPBUS_ENOENT;
   std::lock_guard<std::mutex> g(b->mu);
   int rc = enter(b); if (rc) return rc;
-  if (b->drain_cap < cap || b->drain_idx_cap < n) {   // device staging grows on demand and is kept
-    if (b->drain_cap < cap) { cudaFree(b->d_drain); b->d_drain = nullptr; CK(cudaMalloc((void**)&b->d_drain, cap * sizeof(cpbus_event))); b->drain_cap = cap; }
-    if (b->drain_idx_cap < n) { cudaFree(b->d_drain_idx); b->d_drain_idx = nullptr; CK(cudaMalloc((void**)&b->d_drain_idx, (size_t)n * sizeof(uint2) + 16)); b->drain_idx_cap = n; }
-  }
+  CK(b->d_drain.grow(cap));
+  CK(b->d_drain_idx.grow((size_t)n + 2));   // n entries, then 16 bytes for the kernel's cursor
   unsigned int* cursor = reinterpret_cast<unsigned int*>(b->d_drain_idx + n);
   CK(cudaMemsetAsync(cursor, 0, sizeof(unsigned int), b->stream));
   const uint32_t threads = 256, grid = std::min<uint32_t>((n + 7) / 8, (uint32_t)b->sm_count * 8);
@@ -3055,29 +2960,18 @@ static int drain_ready_impl(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t
   int rc = enter(b); if (rc) return rc;
   const size_t rcap = std::min<size_t>(ready_cap, n);   // never more entries than mailboxes
   const uint32_t tiles = (n + kReadyTile - 1) / kReadyTile;
-  // device staging grows on demand and is kept (the records share cpbus_drain_many's buffer)
-  if (b->drain_cap < cap) {
-    cudaFree(b->d_drain); b->d_drain = nullptr; b->drain_cap = 0;
-    CK(cudaMalloc((void**)&b->d_drain, cap * sizeof(cpbus_event))); b->drain_cap = cap;
-  }
-  if (b->ready_stage_cap < rcap) {
-    cudaFree(b->d_ready); cudaFree(b->d_ready_slot); b->d_ready = nullptr; b->d_ready_slot = nullptr; b->ready_stage_cap = 0;
-    CK(cudaMalloc((void**)&b->d_ready, rcap * sizeof(cpbus_ready)));
-    CK(cudaMalloc((void**)&b->d_ready_slot, rcap * sizeof(uint32_t)));
-    b->ready_stage_cap = rcap;
-  }
-  if (b->ready_lb_tiles < tiles) {
-    cudaFree(b->d_ready_lb); b->d_ready_lb = nullptr; b->ready_lb_tiles = 0;
-    CK(cudaMalloc((void**)&b->d_ready_lb, (kReadyLbOffset + (size_t)tiles) * sizeof(unsigned long long)));
-    b->ready_lb_tiles = tiles;
-  }
-  if (!b->h_ready_hdr) CK(mapped_alloc(64, &b->h_ready_hdr, &b->d_ready_hdr));
+  // the records share cpbus_drain_many's buffer
+  CK(b->d_drain.grow(cap));
+  CK(b->d_ready.grow(rcap));
+  CK(b->d_ready_slot.grow(rcap));
+  CK(b->d_ready_lb.grow(kReadyLbOffset + (size_t)tiles));
+  CK(b->h_ready_hdr.grow(8));
   CK(cudaMemsetAsync(b->d_ready_lb + kReadyHdrWords, 0, (kReadyLbOffset - kReadyHdrWords + (size_t)tiles) * sizeof(unsigned long long),
                      b->stream));
   const uint32_t rot = start_sub - first_sub;
   if (take) {
     if (!b->d_taken) {   // every cursor 0: max(0, head) = head, so nothing is held
-      CK(cudaMalloc((void**)&b->d_taken, (size_t)b->N * sizeof(unsigned long long)));
+      CK(b->d_taken.alloc(b->N));
       CK(cudaMemsetAsync(b->d_taken, 0, (size_t)b->N * sizeof(unsigned long long), b->stream));
     }
     take_ready_scan_kernel<<<tiles, kThreads, 0, b->stream>>>(b->d_ctl, b->d_taken, l, n, rot, b->R, b->cfg.sub_id_base, cap,
@@ -3089,7 +2983,7 @@ static int drain_ready_impl(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t
   CK(cudaGetLastError());
   const uint32_t gather_grid = (uint32_t)std::min<size_t>((size_t)b->sm_count * 4, (rcap + kWarpsPerCta - 1) / kWarpsPerCta);
   drain_ready_gather_kernel<<<gather_grid, kThreads, 0, b->stream>>>(b->d_ring, b->R, b->cfg.sub_id_base, b->d_ready,
-                                                                      b->d_ready_slot, b->d_ready_lb, b->d_drain, b->d_ready_hdr);
+                                                                      b->d_ready_slot, b->d_ready_lb, b->d_drain, b->h_ready_hdr.dev());
   CK(cudaGetLastError());
   b->st.kernel_launches += 2;
   CK(cudaStreamSynchronize(b->stream));
@@ -3131,28 +3025,16 @@ static int ack_many_impl(cpbus* b, const uint32_t* sub_ids, const uint32_t* coun
   std::lock_guard<std::mutex> g(b->mu);
   int rc = enter(b); if (rc) return rc;
   const size_t op_bytes = ops.size() * sizeof(AckOp), bytes = op_bytes + elems.size() * sizeof(uint2);
-  if (b->ack_bytes_cap < bytes) {   // (every call ends in a synchronisation: no copy or kernel reads the old list)
-    cudaFree(b->d_ack); b->d_ack = nullptr;
-    if (b->h_ack) cudaFreeHost(b->h_ack);
-    b->h_ack = nullptr; b->ack_bytes_cap = 0;
-    const size_t c = std::max<size_t>(bytes, 16384);
-    CK(cudaMalloc((void**)&b->d_ack, c));
-    CK(cudaHostAlloc((void**)&b->h_ack, c, cudaHostAllocDefault));
-    b->ack_bytes_cap = c;
-  }
-  if (b->ack_status_cap < n) {
-    if (b->h_ack_status) cudaFreeHost(b->h_ack_status);
-    b->h_ack_status = nullptr; b->d_ack_status = nullptr; b->ack_status_cap = 0;
-    const size_t c = std::max<size_t>(n, 1024);
-    CK(mapped_alloc(c * sizeof(int), &b->h_ack_status, &b->d_ack_status));
-    b->ack_status_cap = c;
-  }
+  // (every call ends in a synchronisation: no copy or kernel reads the old list)
+  CK(b->d_ack.grow(bytes, 16384));
+  CK(b->h_ack.grow(bytes, 16384));
+  CK(b->h_ack_status.grow(n, 1024));
   memcpy(b->h_ack, ops.data(), op_bytes);
   memcpy(b->h_ack + op_bytes, elems.data(), bytes - op_bytes);
   CK(cudaMemcpyAsync(b->d_ack, b->h_ack, bytes, cudaMemcpyHostToDevice, b->stream));
   ack_kernel<<<(uint32_t)((ops.size() + kThreads - 1) / kThreads), kThreads, 0, b->stream>>>(
-      b->d_ctl, b->d_taken, reinterpret_cast<const AckOp*>(b->d_ack), (uint32_t)ops.size(),
-      reinterpret_cast<const uint2*>(b->d_ack + op_bytes), b->d_ack_status);
+      b->d_ctl, b->d_taken, reinterpret_cast<const AckOp*>(b->d_ack.get()), (uint32_t)ops.size(),
+      reinterpret_cast<const uint2*>(b->d_ack + op_bytes), b->h_ack_status.dev());
   CK(cudaGetLastError());
   b->st.kernel_launches++;
   CK(cudaStreamSynchronize(b->stream));
@@ -3192,17 +3074,12 @@ static int lagging_impl(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t sta
   std::lock_guard<std::mutex> g(b->mu);
   int rc = enter(b); if (rc) return rc;
   const size_t ecap = std::min<size_t>(cap, n);   // never more entries than mailboxes
-  if (b->lag_cap < ecap) {
-    if (b->h_lag) cudaFreeHost(b->h_lag);
-    b->h_lag = nullptr; b->d_lag = nullptr; b->lag_cap = 0;
-    CK(mapped_alloc(ecap * sizeof(cpbus_lag), &b->h_lag, &b->d_lag));
-    b->lag_cap = ecap;
-  }
+  CK(b->h_lag.grow(ecap));
   const uint32_t tiles = (n + kReadyTile - 1) / kReadyTile;
   CK(cudaMemsetAsync(b->d_lag_lb, 0, (kLagLbOffset + (size_t)tiles) * sizeof(unsigned long long), b->stream));
   const uint32_t rot = start_sub - first_sub;
   lagging_scan_kernel<<<tiles, kThreads, 0, b->stream>>>(b->d_ctl, l, n, rot, b->R, b->lossless ? 1u : 0u, b->cfg.sub_id_base,
-                                                          min_backlog, ecap, b->d_lag_lb, b->d_lag, b->d_lag_hdr);
+                                                          min_backlog, ecap, b->d_lag_lb, b->h_lag.dev(), b->h_lag_hdr.dev());
   CK(cudaGetLastError());
   b->st.kernel_launches++;
   CK(cudaStreamSynchronize(b->stream));
@@ -3238,10 +3115,10 @@ static int blockers_impl(cpbus* b, const cpbus_event* rec, uint64_t t, uint32_t*
   const uint32_t tiles = (b->n_next + kReadyTile - 1) / kReadyTile;
   CK(cudaMemsetAsync(b->d_lag_lb, 0, (kLagLbOffset + (size_t)tiles) * sizeof(unsigned long long), b->stream));
   const size_t ecap = std::min<size_t>(cap, b->n_next);
-  blockers_scan_kernel<<<tiles, kThreads, 0, b->stream>>>(b->d_ctl, b->d_timers, b->n_paired > 0 ? b->d_pairs : nullptr, b->n_next,
+  blockers_scan_kernel<<<tiles, kThreads, 0, b->stream>>>(b->d_ctl, b->d_timers, b->n_paired > 0 ? b->d_pairs.get() : nullptr, b->n_next,
                                                            b->R, b->K, b->cfg.sub_id_base, timers_on ? 1u : 0u, rec ? 1u : 0u,
-                                                           rec ? *rec : cpbus_event{}, t, ecap, b->d_lag_lb, b->d_block,
-                                                           b->d_lag_hdr);
+                                                           rec ? *rec : cpbus_event{}, t, ecap, b->d_lag_lb, b->h_block.dev(),
+                                                           b->h_lag_hdr.dev());
   CK(cudaGetLastError());
   b->st.kernel_launches++;
   CK(cudaStreamSynchronize(b->stream));
@@ -3420,12 +3297,12 @@ static int dbg_resolve(cpbus* b) {
   for (const DbgItem& it : b->dbg_pending) any_marker |= it.marker;
   if (any_marker) {
     int rc = dev_guard(b); if (rc) return rc;
-    CK(cudaMemcpyAsync(b->h_acct->tail, b->d_acct->tail, sizeof(b->h_acct->tail), cudaMemcpyDeviceToHost, b->stream));
+    CK(cudaMemcpyAsync(b->host_acct()->tail, b->d_acct->tail, sizeof(b->host_acct()->tail), cudaMemcpyDeviceToHost, b->stream));
     CK(cudaStreamSynchronize(b->stream));
   }
   for (const DbgItem& it : b->dbg_pending) {
     if (!it.marker) { dbg_ring_put(b, it.ev); continue; }
-    const DevDbgTail& t = b->h_acct->tail[it.launch % kAcctDbgRing];
+    const DevDbgTail& t = b->host_acct()->tail[it.launch % kAcctDbgRing];
     if (t.launch_seq != it.launch) continue;
     for (uint32_t j = 0; j < t.n_kept && j < (uint32_t)kAcctDbgKeep; j++) dbg_ring_put(b, t.ev[j]);
   }
@@ -3452,7 +3329,8 @@ int cpbus_stats(cpbus_t* b, cpbus_stats_t* out) try {
     CK(cudaGetLastError());
   }
   CK(cudaMemcpyAsync(b->h_stats, b->d_stats, sizeof(DevStats), cudaMemcpyDeviceToHost, b->stream));
-  CK(cudaMemcpyAsync(b->h_acct->by_code, b->d_acct->by_code, sizeof(b->h_acct->by_code), cudaMemcpyDeviceToHost, b->stream));
+  CK(cudaMemcpyAsync(b->host_acct()->by_code, b->d_acct->by_code, sizeof(b->host_acct()->by_code), cudaMemcpyDeviceToHost,
+                     b->stream));
   CK(cudaStreamSynchronize(b->stream));
   retire_oneshots(b, b->last_watermark);
   b->st.deliveries = b->st.ticks = 0;
@@ -3464,7 +3342,7 @@ int cpbus_stats(cpbus_t* b, cpbus_stats_t* out) try {
   *out = b->st;
   out->publishes = b->publishes;
   for (int c = 0; c < CPBUS_N_CODES; c++)   // + device-published batches (kernel-counted)
-    out->published_by_code[c] = b->published_by_code[c] + b->h_acct->by_code[c];
+    out->published_by_code[c] = b->published_by_code[c] + b->host_acct()->by_code[c];
   return CPBUS_OK;
 } CPBUS_CATCH
 
