@@ -104,6 +104,8 @@ SYMBOLS = {
     "cpbus_set_mask_many": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, _P(C.c_uint32)]),
     "cpbus_timer_cancel_many": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, _P(C.c_uint32)]),
     "cpbus_timer_add_list": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, _P(C.c_uint32)]),
+    "cpbus_release_many": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, _P(C.c_uint32)]),
+    "cpbus_subscribe_list": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]),
     "cpbus_publish": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
     "cpbus_send": (C.c_int, [C.c_void_p, C.c_uint32, _P(Event)]),
     "cpbus_advance": (C.c_int, [C.c_void_p, C.c_uint64]),
@@ -170,7 +172,7 @@ SYMBOLS = {
 # the group (one handle over several shards): cpbus_group_<name> takes the arguments of cpbus_<name>
 GROUP_CALLS = ("intern", "intern_ephemeral", "source", "subscribe", "subscribe_many", "subscribe_pairs", "subscribe_pairs_many",
                "unsubscribe", "set_mask", "timer_add", "timer_add_many", "timer_cancel", "unsubscribe_many", "set_mask_many",
-               "timer_cancel_many", "timer_add_list", "publish", "send", "advance", "flush",
+               "timer_cancel_many", "timer_add_list", "release_many", "subscribe_list", "publish", "send", "advance", "flush",
                "sync", "drain", "drain_ready", "take_ready", "ack_many", "lagging", "blockers", "consume_all", "peek_window", "digest", "digest_fold",
                "debug_events", "stats", "publish_counts")
 SYMBOLS["cpbus_group_create"] = (C.c_int, [_P(Config), C.c_void_p, C.c_uint32, _P(C.c_void_p)])

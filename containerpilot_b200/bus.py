@@ -143,6 +143,33 @@ class Bus:
             raise ValueError("sub_ids and masks differ in length")
         return self._membership_many("cpbus_set_mask_many", [ids, m])
 
+    def release_many(self, sub_ids) -> np.ndarray:
+        """cpbus_release_many: give unsubscribed ids back for subscribe_list to hand out again.  The int32 status of each
+        element: OK, ENOENT (never handed out, or already released) or EINVAL (still subscribed).  Raises on any other
+        return, CPBUS_EAGAIN included (nothing was released).  An id must not be used after it is released."""
+        return self._membership_many("cpbus_release_many", [np.ascontiguousarray(sub_ids, dtype=np.uint32)])
+
+    def subscribe_list(self, masks, pairs=None) -> np.ndarray:
+        """cpbus_subscribe_list: subscribe len(masks) subscribers on the lowest free ids (released ones first) and return
+        their uint32 ids.  `pairs` (optional) = one list of exact (code, source_id) cases per subscriber, at most 16 each."""
+        m = np.ascontiguousarray(masks, dtype=np.uint32)
+        n = m.size
+        rows = cnt = None
+        if pairs is not None:
+            rows = np.full((max(n, 1), 16, 2), 0xFFFFFFFF, dtype=np.uint32)
+            cnt = np.zeros(max(n, 1), dtype=np.uint32)
+            for i, pr in enumerate(pairs):
+                if len(pr) > 16:
+                    raise nat.CpbusError(nat.EINVAL, "cpbus_subscribe_list")
+                cnt[i] = len(pr)
+                if len(pr):
+                    rows[i, :len(pr)] = np.asarray(pr, dtype=np.uint32).reshape(-1, 2)
+        ids = np.zeros(max(n, 1), dtype=np.uint32)
+        nat.check(self._lib.cpbus_subscribe_list(self._h, m.ctypes.data if n else None, None if rows is None else rows.ctypes.data,
+                                                  None if cnt is None else cnt.ctypes.data, n, ids.ctypes.data),
+                  "cpbus_subscribe_list")
+        return ids[:n]
+
     # -- timers ------------------------------------------------------------
     def timer_add(self, sub_id: int, period_ns: int, source_id: int, oneshot: bool = False) -> int:
         out = C.c_uint32()

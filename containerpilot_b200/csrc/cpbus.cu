@@ -14,6 +14,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <deque>
+#include <functional>
 #include <map>
 #include <mutex>
 #include <new>
@@ -205,7 +206,9 @@ inline void due_catchup(DueIndex& x, std::vector<HostTimer>& tm, uint64_t now, s
 //  * Per exact case {code, source}: the subscribers with that case.  Cases are set at subscription and never change, so an
 //    entry is live while its subscriber is subscribed; every subscriber's cases are kept (8 bytes each, the device table
 //    keeps 8 too) so that an unsubscribe can find its lists, and a list is compacted when half of it is stale (+ 64).
-//    Bound: 8 bytes per case ever subscribed and 2 * live + 64 entries per case.
+//    A subscriber's cases sit in a segment of case_keys that a later occupant of its slot reuses when its cases fit, and
+//    otherwise replaces by a segment of CPBUS_MAX_PAIRS: with slot reuse, at most n + CPBUS_MAX_PAIRS keys per slot.
+//    Bound: 8 bytes per case subscribed so far, at most 8 * (n + CPBUS_MAX_PAIRS) per slot, and 2 * live + 64 entries per case.
 // Maintenance is O(mask bits + cases) per subscriber and call, amortized.  `slot` (one word per subscriber, all UINT32_MAX
 // between plans) maps a mailbox to its plan entry while a plan is built.  A CPBUS_CFG_SPARSE_TICKS bus without the records
 // flag plans due ticks alone: it sizes `slot` and nothing else.
@@ -219,7 +222,7 @@ struct SubIndex {
   std::unordered_map<uint64_t, Case> cases;          // (code << 32 | source) -> subscribers
   std::vector<uint64_t> case_keys;                   // every subscriber's cases, in subscription order
   std::vector<uint32_t> case_first;                  // per subscriber (allocated with the first case): its cases in case_keys
-  std::vector<uint8_t> case_n;
+  std::vector<uint8_t> case_n, case_cap;             // per subscriber: its cases, and the size of its segment
   std::vector<uint32_t> slot;                        // per subscriber: its entry in the plan being built (UINT32_MAX: none)
 
   static bool takes(const uint32_t* mask, const uint8_t* active, uint32_t l, uint32_t c) {
@@ -229,7 +232,7 @@ struct SubIndex {
     keep = keep_n;
     listed.assign(n, 0); slot.assign(n, UINT32_MAX);
     for (uint32_t c = 0; c < CPBUS_N_CODES; c++) { cnt[c] = stale[c] = 0; ok[c] = true; list[c].clear(); }
-    cases.clear(); case_keys.clear(); case_first.clear(); case_n.clear();
+    cases.clear(); case_keys.clear(); case_first.clear(); case_n.clear(); case_cap.clear();
   }
   void drop(uint32_t c) {
     for (uint32_t l : list[c]) listed[l] &= ~(1u << c);
@@ -273,15 +276,20 @@ struct SubIndex {
   // subscriber l (just subscribed) has the exact cases keys[0..n)
   void add_cases(uint32_t l, const uint64_t* keys, uint32_t n) {
     if (!n) return;
-    if (case_first.empty()) { case_first.assign(listed.size(), 0); case_n.assign(listed.size(), 0); }
-    case_first[l] = (uint32_t)case_keys.size(); case_n[l] = (uint8_t)n;
+    if (case_first.empty()) { case_first.assign(listed.size(), 0); case_n.assign(listed.size(), 0); case_cap.assign(listed.size(), 0); }
+    if (case_cap[l] < n) {   // a new segment: n keys for a slot's first subscriber with cases, the most a reused slot can need
+      const uint32_t cap = case_cap[l] ? (uint32_t)CPBUS_MAX_PAIRS : n;
+      case_first[l] = (uint32_t)case_keys.size(); case_cap[l] = (uint8_t)cap;
+      case_keys.resize(case_keys.size() + cap);
+    }
+    case_n[l] = (uint8_t)n;
     for (uint32_t j = 0; j < n; j++) {
-      case_keys.push_back(keys[j]);
+      case_keys[case_first[l] + j] = keys[j];
       Case& k = cases[keys[j]];
       if (k.subs.empty() || k.subs.back() != l) k.subs.push_back(l);   // (a case listed twice: one entry)
     }
   }
-  // subscriber l has been unsubscribed
+  // subscriber l has been unsubscribed (its cases stay recorded for release_cases)
   void remove_cases(uint32_t l, const uint8_t* active) {
     if (case_n.empty() || !case_n[l]) return;
     const uint64_t* keys = case_keys.data() + case_first[l];
@@ -295,7 +303,30 @@ struct SubIndex {
       k.subs.resize(o); k.stale = 0;
       if (!o) cases.erase(it);
     }
+  }
+  // subscriber l, unsubscribed, is being released (cpbus_release_many): its cases go to *touched, and purge_released then
+  // takes the released subscribers' stale entries out of those lists, so that a later occupant of l with one of the same
+  // cases is listed once
+  void release_cases(uint32_t l, std::vector<uint64_t>* touched) {
+    if (case_n.empty() || !case_n[l]) return;
+    touched->insert(touched->end(), case_keys.begin() + case_first[l], case_keys.begin() + case_first[l] + case_n[l]);
     case_n[l] = 0;
+  }
+  // once per call: each touched list is filtered once, O(the touched lists' lengths) whatever number of its subscribers
+  // the call released
+  void purge_released(std::vector<uint64_t>& touched, const uint8_t* released) {
+    std::sort(touched.begin(), touched.end());
+    touched.erase(std::unique(touched.begin(), touched.end()), touched.end());
+    for (uint64_t key : touched) {
+      auto it = cases.find(key);
+      if (it == cases.end()) continue;   // (compacted away)
+      Case& k = it->second;
+      size_t o = 0;
+      for (uint32_t s : k.subs) if (!released[s]) k.subs[o++] = s;
+      const size_t gone = k.subs.size() - o;   // stale entries: a released subscriber was unsubscribed
+      k.subs.resize(o); k.stale = k.stale > gone ? k.stale - gone : 0;
+      if (!o) cases.erase(it);
+    }
   }
 };
 
@@ -494,6 +525,11 @@ struct cpbus : HostFront {
   uint32_t n_order = 0, n_filtered = 0;   // n_filtered: active subscribers whose mask is not CPBUS_MASK_ALL
   bool order_dirty = true;
   uint32_t n_next = 0, n_active = 0;
+  // subscriber id reuse (cpbus_release_many / cpbus_subscribe_list): released mailboxes below n_next, and the same ids as
+  // a min-heap that cpbus_subscribe_list hands out lowest first; the device copy of the slot-reset list (grown)
+  std::vector<uint8_t> h_released;
+  std::vector<uint32_t> free_ids;
+  DeviceBuf<unsigned char> d_reset;
 
   // lossless mode: a lower bound of the free slots of the FULLEST mailbox.  While a batch provably fits (bound >= what it
   // can append to one mailbox) the admission pass and its host sync are skipped; the bound is refreshed exactly whenever
@@ -560,6 +596,7 @@ struct cpbus_group : HostFront {
   uint32_t base = 0, N = 0;
   bool lossless = false;
   uint32_t n_next = 0, n_active = 0;
+  std::vector<uint32_t> free_ids;       // released global indices, a min-heap (cpbus_group_subscribe_list)
   std::vector<cpbus_event> staged;      // B records
 };
 
@@ -1308,6 +1345,12 @@ bool id_range(uint32_t base, uint32_t n_next, uint32_t first, uint64_t n, uint32
   return first >= base && (uint64_t)*index + n <= n_next;
 }
 
+// Whether sub_id names a mailbox of this bus that was handed out and not released since; *l = its index.  A released id
+// is refused as one never handed out; range calls keep n_next as their bound and see a released mailbox as empty.
+bool sub_index(const cpbus* b, uint32_t sub_id, uint32_t* l) {
+  return id_range(b->cfg.sub_id_base, b->n_next, sub_id, 1, l) && !b->h_released[*l];
+}
+
 // cpbus_publish_counts: the host publish counts of f and n_dev device-counted pairs (key + 1 per slot, 0 = empty), merged by
 // {code, source} and sorted; *n = how many pairs there are, the first cap of them go to out.
 void pair_counts(const HostFront* f, const unsigned long long* dev_keys, const unsigned long long* dev_cnts, size_t n_dev,
@@ -1635,6 +1678,7 @@ int cpbus_create(const cpbus_config* cfg, cpbus_t** out) try {
   }
   b->h_mask.assign(N, 0);
   b->h_active.assign(N, 0);
+  b->h_released.assign(N, 0);
   if (b->sparse_records) b->rec_index.init(N, 2 * std::max<size_t>(32, N / 1024));   // lists of up to twice the largest cap
   else if (b->sparse) b->rec_index.slot.assign(N, UINT32_MAX);
   b->intern.emplace(std::string(), 0u);   // "" -> 0 so that NonEvent == {None, 0} (events/events.go:45)
@@ -1714,6 +1758,32 @@ int cpbus_source(cpbus_t* b, uint32_t id, char* out, size_t cap, size_t* len) tr
   return CPBUS_OK;
 } CPBUS_CATCH
 
+// The host half of a subscription into mailbox l, fresh or reused, after the call's flush: the registry and the sparse
+// record index.  The caller writes the control block.
+static void subscribe_host(cpbus* b, uint32_t l, uint32_t mask) {
+  b->h_mask[l] = mask & CPBUS_MASK_ALL;
+  b->h_active[l] = 1;
+  if (b->h_mask[l] != CPBUS_MASK_ALL) b->n_filtered++;
+  if (b->sparse_records) b->rec_index.add_codes(l, b->h_mask[l]);
+}
+
+// The host half of subscriber l's exact cases, after subscribe_host, once the pair tables exist: the first n_pairs of
+// `pairs` whose code is not in the mask go to row[0 ..) (the caller fills the rest with kPairNone), to the registry and to
+// the sparse record index.  Returns how many there are.
+static uint32_t pairs_host(cpbus* b, uint32_t l, const cpbus_pair* pairs, uint32_t n_pairs, uint2* row) {
+  uint32_t used = 0;
+  for (uint32_t j = 0; j < n_pairs; j++)
+    if (!((b->h_mask[l] >> pairs[j].code) & 1u)) row[used++] = make_uint2(pairs[j].code, pairs[j].source_id);
+  b->h_npairs[l] = (uint8_t)used;
+  if (used) b->n_paired++;
+  if (b->sparse_records && used) {
+    uint64_t keys[CPBUS_MAX_PAIRS];
+    for (uint32_t j = 0; j < used; j++) keys[j] = (uint64_t)row[j].x << 32 | row[j].y;
+    b->rec_index.add_cases(l, keys, used);
+  }
+  return used;
+}
+
 int cpbus_subscribe_many(cpbus_t* b, const uint32_t* masks, uint32_t n, uint32_t* first_sub_id) try {
   if (!b || !n) return CPBUS_EINVAL;
   if ((uint64_t)b->n_next + n > b->N) return CPBUS_ENOSPC;
@@ -1723,11 +1793,8 @@ int cpbus_subscribe_many(cpbus_t* b, const uint32_t* masks, uint32_t n, uint32_t
   std::vector<SubCtl> blocks(n);
   memset(blocks.data(), 0, (size_t)n * sizeof(SubCtl));
   for (uint32_t i = 0; i < n; i++) {
-    b->h_mask[first + i] = (masks ? masks[i] : CPBUS_MASK_ALL) & CPBUS_MASK_ALL;
+    subscribe_host(b, first + i, masks ? masks[i] : CPBUS_MASK_ALL);
     blocks[i].mask = b->h_mask[first + i] | kActiveBit;
-    b->h_active[first + i] = 1;
-    if (b->h_mask[first + i] != CPBUS_MASK_ALL) b->n_filtered++;
-    if (b->sparse_records) b->rec_index.add_codes(first + i, b->h_mask[first + i]);
   }
   CK(cudaMemcpyAsync(b->d_ctl + first, blocks.data(), (size_t)n * sizeof(SubCtl), cudaMemcpyHostToDevice, b->stream));
   CK(cudaStreamSynchronize(b->stream));
@@ -1796,27 +1863,10 @@ int cpbus_subscribe_pairs_many(cpbus_t* b, const uint32_t* masks, const cpbus_pa
   const uint32_t l0 = first - b->cfg.sub_id_base;
   std::vector<uint2> rows((size_t)n * CPBUS_MAX_PAIRS, make_uint2(kPairNone, kPairNone));
   uint32_t paired = 0;
-  for (uint32_t i = 0; i < n; i++) {
-    const uint32_t m = masks[i] & CPBUS_MASK_ALL;
-    uint32_t used = 0;
-    for (uint32_t j = 0; j < n_pairs[i]; j++) {
-      const cpbus_pair& pr = pairs[(size_t)i * CPBUS_MAX_PAIRS + j];
-      if (!((m >> pr.code) & 1u)) rows[(size_t)i * CPBUS_MAX_PAIRS + used++] = make_uint2(pr.code, pr.source_id);
-    }
-    b->h_npairs[l0 + i] = (uint8_t)used;
-    if (used) paired++;
-    if (b->sparse_records && used) {
-      uint64_t keys[CPBUS_MAX_PAIRS];
-      for (uint32_t j = 0; j < used; j++) {
-        const uint2 r = rows[(size_t)i * CPBUS_MAX_PAIRS + j];
-        keys[j] = (uint64_t)r.x << 32 | r.y;
-      }
-      b->rec_index.add_cases(l0 + i, keys, used);
-    }
-  }
+  for (uint32_t i = 0; i < n; i++)
+    if (pairs_host(b, l0 + i, pairs + (size_t)i * CPBUS_MAX_PAIRS, n_pairs[i], rows.data() + (size_t)i * CPBUS_MAX_PAIRS)) paired++;
   CK(cudaMemcpyAsync(b->d_pairs + (size_t)l0 * CPBUS_MAX_PAIRS, rows.data(), rows.size() * sizeof(uint2), cudaMemcpyHostToDevice, b->stream));
   CK(cudaStreamSynchronize(b->stream));
-  b->n_paired += paired;
   if (paired && (rc = push_mask_words(b, l0, n))) return rc;
   if (first_sub_id) *first_sub_id = first;
   return CPBUS_OK;
@@ -1850,7 +1900,7 @@ static int unsubscribe_host(cpbus* b, uint32_t l, uint32_t* clear) {
 int cpbus_unsubscribe(cpbus_t* b, uint32_t sub_id) try {
   if (!b) return CPBUS_EINVAL;
   uint32_t l = 0, clear = 0;
-  if (!id_range(b->cfg.sub_id_base, b->n_next, sub_id, 1, &l)) return CPBUS_ENOENT;
+  if (!sub_index(b, sub_id, &l)) return CPBUS_ENOENT;
   int rc = enter(b); if (rc) return rc;
   if ((rc = flush_staged(b, b->now))) return rc;
   if ((rc = unsubscribe_host(b, l, &clear))) return rc;
@@ -1880,7 +1930,7 @@ static void set_mask_host(cpbus* b, uint32_t l, uint32_t mask) {
 int cpbus_set_mask(cpbus_t* b, uint32_t sub_id, uint32_t mask) try {
   if (!b) return CPBUS_EINVAL;
   uint32_t l = 0;
-  if (!id_range(b->cfg.sub_id_base, b->n_next, sub_id, 1, &l)) return CPBUS_ENOENT;
+  if (!sub_index(b, sub_id, &l)) return CPBUS_ENOENT;
   if (!b->h_active[l]) return CPBUS_ECLOSED;
   int rc = enter(b); if (rc) return rc;
   if ((rc = flush_staged(b, b->now))) return rc;
@@ -1900,7 +1950,7 @@ int cpbus_timer_add(cpbus_t* b, uint32_t sub_id, uint64_t period_ns, uint32_t so
   if (!b || !period_ns) return CPBUS_EINVAL;
   if (!b->K) return CPBUS_ENOSPC;
   uint32_t l = 0;
-  if (!id_range(b->cfg.sub_id_base, b->n_next, sub_id, 1, &l)) return CPBUS_ENOENT;
+  if (!sub_index(b, sub_id, &l)) return CPBUS_ENOENT;
   int rc = enter(b); if (rc) return rc;
   if ((rc = flush_staged(b, b->now))) return rc;
   if (b->h_timers.empty()) timer_table(b);
@@ -1926,6 +1976,7 @@ int cpbus_timer_add_many(cpbus_t* b, uint32_t first_sub, uint32_t n, uint64_t pe
   if (!b->K) return CPBUS_ENOSPC;
   uint32_t l0 = 0;
   if (!id_range(b->cfg.sub_id_base, b->n_next, first_sub, n, &l0)) return CPBUS_ENOENT;
+  for (uint32_t i = 0; i < n; i++) if (b->h_released[l0 + i]) return CPBUS_ENOENT;   // as an id never handed out
   int rc = enter(b); if (rc) return rc;
   if ((rc = flush_staged(b, b->now))) return rc;
   if (b->h_timers.empty()) timer_table(b);
@@ -2034,7 +2085,7 @@ static int membership_many(cpbus* b, uint32_t n, int* status, uint32_t* applied,
 int cpbus_unsubscribe_many(cpbus_t* b, const uint32_t* sub_ids, uint32_t n, int* status, uint32_t* applied) try {
   if (!b || (!sub_ids && n)) return CPBUS_EINVAL;
   return membership_many(b, n, status, applied,
-      [&](uint32_t i) { uint32_t l; return id_range(b->cfg.sub_id_base, b->n_next, sub_ids[i], 1, &l) ? CPBUS_OK : CPBUS_ENOENT; },
+      [&](uint32_t i) { uint32_t l; return sub_index(b, sub_ids[i], &l) ? CPBUS_OK : CPBUS_ENOENT; },
       [] {},
       [&](uint32_t i, uint32_t* l, uint32_t* clear) { *l = sub_ids[i] - b->cfg.sub_id_base; return unsubscribe_host(b, *l, clear); });
 } CPBUS_CATCH
@@ -2045,7 +2096,7 @@ int cpbus_set_mask_many(cpbus_t* b, const uint32_t* sub_ids, const uint32_t* cod
   return membership_many(b, n, status, applied,
       [&](uint32_t i) {
         uint32_t l = 0;
-        if (!id_range(b->cfg.sub_id_base, b->n_next, sub_ids[i], 1, &l)) return CPBUS_ENOENT;
+        if (!sub_index(b, sub_ids[i], &l)) return CPBUS_ENOENT;
         return b->h_active[l] ? CPBUS_OK : CPBUS_ECLOSED;
       },
       [] {},
@@ -2073,7 +2124,7 @@ static int timer_add_check(const cpbus* b, const cpbus_timer_spec& s) {
   if (!s.period_ns) return CPBUS_EINVAL;
   if (!b->K) return CPBUS_ENOSPC;
   uint32_t l = 0;
-  return id_range(b->cfg.sub_id_base, b->n_next, s.sub_id, 1, &l) ? CPBUS_OK : CPBUS_ENOENT;
+  return sub_index(b, s.sub_id, &l) ? CPBUS_OK : CPBUS_ENOENT;
 }
 
 // cpbus_timer_add for each element in array order, with one flush and one timer_arm_kernel launch: each applied element
@@ -2128,6 +2179,135 @@ int cpbus_timer_add_list(cpbus_t* b, const cpbus_timer_spec* specs, uint32_t n, 
   return CPBUS_OK;
 } CPBUS_CATCH
 
+// Subscriber id reuse.  Every mailbox a call touches gets one slot_reset_kernel entry: the list is [entries | pair rows],
+// one H2D copy, one launch and one synchronisation (none when nothing is applied).  A reset mailbox has all ring_cap slots
+// of room, so the lossless room bound (a lower bound of the fullest mailbox's room) stays valid without an update.
+static int slot_reset(cpbus* b, const std::vector<SlotResetOp>& ops, const std::vector<uint2>& rows) {
+  if (ops.empty()) return CPBUS_OK;
+  const size_t head = ops.size() * sizeof(SlotResetOp), bytes = head + rows.size() * sizeof(uint2);
+  std::vector<unsigned char> list(bytes);
+  memcpy(list.data(), ops.data(), head);
+  if (!rows.empty()) memcpy(list.data() + head, rows.data(), rows.size() * sizeof(uint2));
+  CK(b->d_reset.grow(bytes, 4096));   // (every call ends in a synchronisation: no kernel reads the old list)
+  // (pageable source: the call returns once the list has been taken, and the copy runs in stream order)
+  CK(cudaMemcpyAsync(b->d_reset, list.data(), bytes, cudaMemcpyHostToDevice, b->stream));
+  slot_reset_kernel<<<(uint32_t)((ops.size() + kThreads - 1) / kThreads), kThreads, 0, b->stream>>>(
+      b->d_ctl, b->d_taken.get(), b->d_pairs.get(), b->K ? b->d_timers.get() : nullptr,
+      reinterpret_cast<const SlotResetOp*>(b->d_reset.get()), (uint32_t)ops.size(),
+      reinterpret_cast<const uint2*>(b->d_reset.get() + head), b->K);
+  CK(cudaGetLastError());
+  b->st.kernel_launches++;
+  CK(cudaStreamSynchronize(b->stream));
+  return CPBUS_OK;
+}
+
+// cpbus_release_many's refusal of element sub_id before its flush: CPBUS_ENOENT (never handed out, or released), CPBUS_EINVAL
+// (still subscribed) or CPBUS_OK
+static int release_check(const cpbus* b, uint32_t sub_id) {
+  uint32_t l = 0;
+  if (!sub_index(b, sub_id, &l)) return CPBUS_ENOENT;
+  return b->h_active[l] ? CPBUS_EINVAL : CPBUS_OK;
+}
+
+// The host half of a release: mailbox l (unsubscribed) goes back to the state of a slot never handed out, and its id to the
+// free set; its exact cases go to *touched for the call's one purge of the case lists (SubIndex::purge_released).  Unsubscribing already took it out of the registry's counts, the code lists, the due index and the timer table;
+// the timer slots keep their generations, so an old occupant's timer ids stay stale.
+static void release_host(cpbus* b, uint32_t l, std::vector<uint64_t>* touched) {
+  b->h_released[l] = 1;
+  b->free_ids.push_back(l);
+  std::push_heap(b->free_ids.begin(), b->free_ids.end(), std::greater<uint32_t>());
+  b->h_mask[l] = 0;
+  if (!b->h_npairs.empty()) b->h_npairs[l] = 0;
+  if (b->sparse_records) b->rec_index.release_cases(l, touched);
+  if (b->K && !b->h_timers.empty())
+    for (uint32_t k = 0; k < b->K; k++) {
+      HostTimer& t = b->h_timers[(size_t)l * b->K + k];
+      const uint8_t gen = t.gen;
+      t = HostTimer{};
+      t.gen = gen;
+      if (b->sparse) b->due.drop(l * b->K + k);
+    }
+  b->order_dirty = true;
+}
+
+int cpbus_release_many(cpbus_t* b, const uint32_t* sub_ids, uint32_t n, int* status, uint32_t* applied) try {
+  if (!b || (!sub_ids && n)) return CPBUS_EINVAL;
+  std::vector<int> st(n);
+  bool any = false;
+  for (uint32_t i = 0; i < n; i++) any |= (st[i] = release_check(b, sub_ids[i])) == CPBUS_OK;
+  std::vector<SlotResetOp> ops;
+  if (any) {
+    int rc = enter(b); if (rc) return rc;
+    if ((rc = flush_staged(b, b->now))) return rc;   // ordered with publishes, like Unsubscribe
+    std::vector<uint64_t> touched;   // the released subscribers' exact cases (sparse records)
+    for (uint32_t i = 0; i < n; i++) {
+      if (st[i] != CPBUS_OK) continue;
+      const uint32_t l = sub_ids[i] - b->cfg.sub_id_base;
+      if (b->h_released[l]) { st[i] = CPBUS_ENOENT; continue; }   // an earlier element released it
+      release_host(b, l, &touched);
+      ops.push_back(SlotResetOp{l, 0u, kResetNoRow, 0u});
+    }
+    if (!touched.empty()) b->rec_index.purge_released(touched, b->h_released.data());
+  }
+  const int rc = slot_reset(b, ops, {});
+  if (rc) return rc;
+  if (status && n) memcpy(status, st.data(), (size_t)n * sizeof(int));
+  if (applied) *applied = (uint32_t)ops.size();
+  return CPBUS_OK;
+} CPBUS_CATCH
+
+// The argument checks of cpbus_subscribe_pairs_many, with pairs / n_pairs NULL meaning no cases
+static int subscribe_list_check(const uint32_t* n_pairs, const cpbus_pair* pairs, uint32_t n) {
+  if (!n_pairs) return CPBUS_OK;
+  if (!pairs) return CPBUS_EINVAL;
+  for (uint32_t i = 0; i < n; i++) {
+    if (n_pairs[i] > CPBUS_MAX_PAIRS) return CPBUS_EINVAL;
+    for (uint32_t j = 0; j < n_pairs[i]; j++) if (pairs[(size_t)i * CPBUS_MAX_PAIRS + j].code >= CPBUS_N_CODES) return CPBUS_EINVAL;
+  }
+  return CPBUS_OK;
+}
+
+int cpbus_subscribe_list(cpbus_t* b, const uint32_t* code_masks, const cpbus_pair* pairs, const uint32_t* n_pairs, uint32_t n,
+                         uint32_t* sub_ids) try {
+  if (!b || !n || !sub_ids || subscribe_list_check(n_pairs, pairs, n)) return CPBUS_EINVAL;
+  if (b->free_ids.size() + (uint64_t)(b->N - b->n_next) < n) return CPBUS_ENOSPC;
+  int rc = enter(b); if (rc) return rc;
+  if ((rc = flush_staged(b, b->now))) return rc;   // ordered with publishes
+  bool cases = false;   // some subscriber keeps a case its mask does not cover: it needs the pair tables
+  for (uint32_t i = 0; n_pairs && !cases && i < n; i++) {
+    const uint32_t m = code_masks ? code_masks[i] : CPBUS_MASK_ALL;
+    for (uint32_t j = 0; j < n_pairs[i]; j++) cases |= !((m >> pairs[(size_t)i * CPBUS_MAX_PAIRS + j].code) & 1u);
+  }
+  if (cases && (rc = pair_tables(b))) return rc;
+  std::vector<SlotResetOp> ops(n);
+  std::vector<uint2> rows;
+  uint2 row[CPBUS_MAX_PAIRS];
+  for (uint32_t i = 0; i < n; i++) {   // lowest free id first: the released ones ascending, then fresh ones
+    uint32_t l = b->n_next;
+    if (!b->free_ids.empty()) {
+      l = b->free_ids.front();
+      std::pop_heap(b->free_ids.begin(), b->free_ids.end(), std::greater<uint32_t>());
+      b->free_ids.pop_back();
+      b->h_released[l] = 0;
+    } else {
+      b->n_next++;
+    }
+    subscribe_host(b, l, code_masks ? code_masks[i] : CPBUS_MASK_ALL);
+    ops[i] = SlotResetOp{l, 0u, kResetNoRow, 0u};
+    if (n_pairs && b->d_pairs) {
+      for (uint2& r : row) r = make_uint2(kPairNone, kPairNone);
+      if (pairs_host(b, l, pairs + (size_t)i * CPBUS_MAX_PAIRS, n_pairs[i], row)) {
+        ops[i].row = (uint32_t)(rows.size() / CPBUS_MAX_PAIRS);
+        rows.insert(rows.end(), row, row + CPBUS_MAX_PAIRS);
+      }
+    }
+    ops[i].mask_word = mask_word(b, l);
+    sub_ids[i] = b->cfg.sub_id_base + l;
+  }
+  b->n_active += n; b->order_dirty = true;
+  return slot_reset(b, ops, rows);
+} CPBUS_CATCH
+
 int cpbus_publish(cpbus_t* b, const cpbus_event* ev, size_t n) try {
   if (!b || (!ev && n)) return CPBUS_EINVAL;
   int rc = enter(b); if (rc) return rc;
@@ -2137,7 +2317,7 @@ int cpbus_publish(cpbus_t* b, const cpbus_event* ev, size_t n) try {
 int cpbus_send(cpbus_t* b, uint32_t sub_id, const cpbus_event* ev) try {
   if (!b || !ev || ev->code >= CPBUS_N_CODES) return CPBUS_EINVAL;
   uint32_t l = 0;
-  if (!id_range(b->cfg.sub_id_base, b->n_next, sub_id, 1, &l)) return CPBUS_ENOENT;
+  if (!sub_index(b, sub_id, &l)) return CPBUS_ENOENT;
   if (!b->h_active[l]) return CPBUS_ECLOSED;   // the mailbox is gone (Go: send on a closed channel panics)
   int rc = enter(b); if (rc) return rc;
   if ((rc = stage_one(b, ev->code, ev->source_id, sub_id, CPBUS_F_UNICAST))) return rc;
@@ -2876,7 +3056,7 @@ static int copy_slots(cpbus* b, uint32_t l, uint64_t from, size_t n, cpbus_event
 int cpbus_drain(cpbus_t* b, uint32_t sub_id, cpbus_event* out, size_t cap, size_t* n, uint64_t* lost) try {
   if (!b || !n || (!out && cap)) return CPBUS_EINVAL;
   uint32_t l = 0;
-  if (!id_range(b->cfg.sub_id_base, b->n_next, sub_id, 1, &l)) return CPBUS_ENOENT;
+  if (!sub_index(b, sub_id, &l)) return CPBUS_ENOENT;
   std::lock_guard<std::mutex> g(b->mu);
   int rc = enter(b); if (rc) return rc;
   uint64_t tail = 0, head = 0;
@@ -3007,7 +3187,7 @@ static int ack_many_impl(cpbus* b, const uint32_t* sub_ids, const uint32_t* coun
   std::vector<uint64_t> el;   // mailbox << 32 | element index: sorted, each mailbox's elements stay in array order
   for (uint32_t i = 0; i < n; i++) {
     uint32_t l = 0;
-    if (!id_range(b->cfg.sub_id_base, b->n_next, sub_ids[i], 1, &l)) st[i] = CPBUS_ENOENT;
+    if (!sub_index(b, sub_ids[i], &l)) st[i] = CPBUS_ENOENT;
     else if (counts[i] == 0) st[i] = CPBUS_OK;
     else if (!b->d_taken) st[i] = CPBUS_EINVAL;
     else el.push_back((uint64_t)l << 32 | i);
@@ -3199,7 +3379,7 @@ int cpbus_consume_all(cpbus_t* b) try {
 int cpbus_peek_window(cpbus_t* b, uint32_t sub_id, cpbus_event* out, size_t cap, size_t* n) try {
   if (!b || !n || (!out && cap)) return CPBUS_EINVAL;
   uint32_t l = 0;
-  if (!id_range(b->cfg.sub_id_base, b->n_next, sub_id, 1, &l)) return CPBUS_ENOENT;
+  if (!sub_index(b, sub_id, &l)) return CPBUS_ENOENT;
   std::lock_guard<std::mutex> g(b->mu);
   int rc = enter(b); if (rc) return rc;
   uint64_t tail = 0, head = 0;
@@ -3382,13 +3562,14 @@ static void group_retire(cpbus_group* g) {
   for (cpbus* s : g->shards) if (!s->h_timers.empty()) retire_oneshots(s, s->last_watermark);
 }
 
-// the owning shard of global id `sub_id` and its local index; false: not a subscribed-so-far id
+// the owning shard of global id `sub_id` and its local index; false: not a subscribed-so-far id, or a released one (*s and
+// *l are still set when the id is below n_next)
 static bool group_locate(const cpbus_group* g, uint32_t sub_id, cpbus** s, uint32_t* l) {
   uint32_t i = 0;
   if (!id_range(g->base, g->n_next, sub_id, 1, &i)) return false;
   const uint32_t k = group_shard_of(g, i);
   *s = g->shards[k]; *l = i - g->first[k];
-  return true;
+  return !(*s)->h_released[*l];   // a released id is refused as one never handed out
 }
 
 // Arm timers on shard s: a shard without timers takes the group clock first (cpbus_advance launches nothing there).
@@ -3590,6 +3771,10 @@ int cpbus_group_timer_add_many(cpbus_group_t* g, uint32_t first_sub, uint32_t n,
   if (!g->K) return CPBUS_ENOSPC;
   uint32_t i0 = 0;
   if (!id_range(g->base, g->n_next, first_sub, n, &i0)) return CPBUS_ENOENT;
+  for (uint32_t i = 0; i < n; i++) {   // a released id: as one never handed out
+    cpbus* s = nullptr; uint32_t l = 0;
+    if (!group_locate(g, first_sub + i, &s, &l)) return CPBUS_ENOENT;
+  }
   int rc = flush_staged(g, g->now); if (rc) return rc;
   if (g->h_timers.empty()) g->h_timers.resize((size_t)g->N * g->K);
   group_retire(g);
@@ -3770,6 +3955,64 @@ int cpbus_group_timer_add_list(cpbus_group_t* g, const cpbus_timer_spec* specs, 
   if (timer_ids)
     for (uint32_t i = 0; i < n; i++) if (st[i] == CPBUS_OK) timer_ids[i] = ids[i];
   if (status && n) memcpy(status, st.data(), (size_t)n * sizeof(int));
+  return CPBUS_OK;
+} CPBUS_CATCH
+
+// subscriber id reuse: each shard with work takes its elements, in array order, in one cpbus_release_many call; the group
+// keeps the released global indices in its own free set
+int cpbus_group_release_many(cpbus_group_t* g, const uint32_t* sub_ids, uint32_t n, int* status, uint32_t* applied) try {
+  if (!g || (!sub_ids && n)) return CPBUS_EINVAL;
+  std::vector<uint32_t> ids;
+  return group_membership_many(g, n, status, applied,
+      [&](uint32_t i, uint32_t* k) {
+        cpbus* s = nullptr; uint32_t l = 0;
+        if (!group_locate(g, sub_ids[i], &s, &l)) return CPBUS_ENOENT;
+        if (s->h_active[l]) return CPBUS_EINVAL;
+        *k = group_shard_of(g, sub_ids[i] - g->base);
+        return CPBUS_OK;
+      },
+      [] {},
+      [&](uint32_t k, const std::vector<uint32_t>& el, int* st) -> int {
+        ids.resize(el.size());
+        for (size_t j = 0; j < el.size(); j++) ids[j] = sub_ids[el[j]];
+        const int rc = cpbus_release_many(g->shards[k], ids.data(), (uint32_t)ids.size(), st, nullptr);
+        if (rc) return rc;
+        for (size_t j = 0; j < el.size(); j++)
+          if (st[j] == CPBUS_OK) {
+            g->free_ids.push_back(ids[j] - g->base);
+            std::push_heap(g->free_ids.begin(), g->free_ids.end(), std::greater<uint32_t>());
+          }
+        return CPBUS_OK;
+      });
+} CPBUS_CATCH
+
+// The group hands out the lowest free global ids.  The shards fill in order, so the free ids of shard k's range are its own
+// released ids and its own fresh ones, and the lowest of them are the ones shard k's cpbus_subscribe_list hands out: each
+// shard with work takes its run of elements in one call.
+int cpbus_group_subscribe_list(cpbus_group_t* g, const uint32_t* code_masks, const cpbus_pair* pairs, const uint32_t* n_pairs,
+                               uint32_t n, uint32_t* sub_ids) try {
+  if (!g || !n || !sub_ids || subscribe_list_check(n_pairs, pairs, n)) return CPBUS_EINVAL;
+  if (g->free_ids.size() + (uint64_t)(g->N - g->n_next) < n) return CPBUS_ENOSPC;
+  int rc = flush_staged(g, g->now); if (rc) return rc;
+  std::vector<uint32_t> idx(n);   // global indices, ascending
+  for (uint32_t i = 0; i < n; i++) {
+    if (g->free_ids.empty()) { idx[i] = g->n_next++; continue; }
+    idx[i] = g->free_ids.front();
+    std::pop_heap(g->free_ids.begin(), g->free_ids.end(), std::greater<uint32_t>());
+    g->free_ids.pop_back();
+  }
+  g->n_active += n;
+  for (uint32_t i = 0; i < n;) {
+    const uint32_t k = group_shard_of(g, idx[i]);
+    uint32_t cnt = 1;
+    while (i + cnt < n && idx[i + cnt] < g->first[k + 1]) cnt++;
+    rc = cpbus_subscribe_list(g->shards[k], code_masks ? code_masks + i : nullptr, n_pairs ? pairs + (size_t)i * CPBUS_MAX_PAIRS : nullptr,
+                              n_pairs ? n_pairs + i : nullptr, cnt, sub_ids + i);
+    if (rc) return rc;
+    for (uint32_t j = i; j < i + cnt; j++)
+      if (sub_ids[j] != g->base + idx[j]) return CPBUS_ECUDA;   // cannot happen: the shard's lowest free ids are the group's
+    i += cnt;
+  }
   return CPBUS_OK;
 } CPBUS_CATCH
 

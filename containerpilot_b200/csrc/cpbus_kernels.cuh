@@ -1227,6 +1227,43 @@ __global__ void __launch_bounds__(kThreads) timer_arm_kernel(SubCtl* __restrict_
   ctl[hi.z].mask = hi.w;
 }
 
+// Subscriber id reuse (cpbus_release_many, cpbus_subscribe_list): one entry per mailbox, the state a fresh subscription finds
+// in a slot that was never handed out, with the new occupant's mask word (0 for a release).  The pair-table rows of the
+// entries with cases follow the entries in the same list, CPBUS_MAX_PAIRS per row.
+constexpr uint32_t kResetNoRow = 0xFFFFFFFFu;
+struct __align__(16) SlotResetOp {
+  uint32_t local;       // mailbox (shard-local index)
+  uint32_t mask_word;   // its control block's mask word, as mask_word() leaves it
+  uint32_t row;         // its cases in `rows` (kResetNoRow: none, every pair slot unused)
+  uint32_t pad;
+};
+
+// One thread per entry: the whole control block (tail, head, digest 0: the ring's records are unreachable, and no read goes
+// behind head or below tail - ring_cap), the take cursor, the pair-table row and the K timer slots (idle, every byte 0xFF).
+// The ring itself is not touched.  taken / pairs / timers are null when the bus has none.
+__global__ void __launch_bounds__(kThreads) slot_reset_kernel(SubCtl* __restrict__ ctl, unsigned long long* __restrict__ taken,
+                                                              uint2* __restrict__ pairs, DevTimer* __restrict__ timers,
+                                                              const SlotResetOp* __restrict__ ops, uint32_t n,
+                                                              const uint2* __restrict__ rows, uint32_t K) {
+  const uint32_t i = blockIdx.x * kThreads + threadIdx.x;
+  if (i >= n) return;
+  const SlotResetOp op = ops[i];
+  uint4* c = reinterpret_cast<uint4*>(ctl + op.local);
+  c[0] = make_uint4(0u, 0u, 0u, 0u);
+  c[1] = make_uint4(0u, 0u, op.mask_word, 0u);
+  if (taken) taken[op.local] = 0ull;
+  if (pairs) {
+    uint2* dst = pairs + (size_t)op.local * CPBUS_MAX_PAIRS;
+    for (uint32_t j = 0; j < CPBUS_MAX_PAIRS; j++)
+      dst[j] = op.row == kResetNoRow ? make_uint2(kPairNone, kPairNone) : rows[(size_t)op.row * CPBUS_MAX_PAIRS + j];
+  }
+  const uint4 idle = make_uint4(~0u, ~0u, ~0u, ~0u);
+  for (uint32_t k = 0; k < K; k++) {
+    uint4* tp = reinterpret_cast<uint4*>(timers + (size_t)op.local * K + k);
+    tp[0] = idle; tp[1] = idle;
+  }
+}
+
 // Acknowledged drains (cpbus_ack_many): one entry per mailbox, holding the index range [first, first + n) of its elements
 // in `elems` (in the call's array order).  An element is {records to release, its index in the call}.  The host builds one
 // entry per mailbox, so no two threads touch one mailbox.

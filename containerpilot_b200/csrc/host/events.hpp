@@ -194,7 +194,7 @@ EVENTS_CPBUS_CALL(publish) EVENTS_CPBUS_CALL(send) EVENTS_CPBUS_CALL(advance) EV
 EVENTS_CPBUS_CALL(timer_add) EVENTS_CPBUS_CALL(timer_cancel) EVENTS_CPBUS_CALL(drain) EVENTS_CPBUS_CALL(drain_ready)
 EVENTS_CPBUS_CALL(debug_events) EVENTS_CPBUS_CALL(intern) EVENTS_CPBUS_CALL(intern_ephemeral) EVENTS_CPBUS_CALL(source)
 EVENTS_CPBUS_CALL(lagging) EVENTS_CPBUS_CALL(blockers) EVENTS_CPBUS_CALL(unsubscribe_many)
-EVENTS_CPBUS_CALL(take_ready) EVENTS_CPBUS_CALL(ack_many)
+EVENTS_CPBUS_CALL(take_ready) EVENTS_CPBUS_CALL(ack_many) EVENTS_CPBUS_CALL(release_many) EVENTS_CPBUS_CALL(subscribe_list)
 #undef EVENTS_CPBUS_CALL
 
 namespace detail {
@@ -280,6 +280,12 @@ class EventBus {   // events/bus.go:12-22
       if (!sub->pending_.empty()) pending_subs_.insert(sub);
       registry_.erase(old);
       implicit_.erase(imp);
+    } else if (reuse_) {
+      const uint32_t np = (uint32_t)pairs.size();
+      if (np > CPBUS_MAX_PAIRS) Check(CPBUS_EINVAL, "cpbus_subscribe_list");
+      pairs.resize(CPBUS_MAX_PAIRS);
+      Retry([&] { return cpbus_subscribe_list(h_, &mask, pairs.data(), np ? &np : (const uint32_t*)nullptr, 1u, &id); },
+            "cpbus_subscribe_list");
     } else {
       Retry([&] { return cpbus_subscribe_pairs(h_, mask, pairs.data(), (uint32_t)pairs.size(), &id); }, "cpbus_subscribe_pairs");
     }
@@ -299,6 +305,7 @@ class EventBus {   // events/bus.go:12-22
       FlushLocked();
       DrainOne(sub, /*blocking=*/false);   // what was published before the unsubscribe still reaches Rx
       Retry([&] { return cpbus_unsubscribe(h_, it->second); }, "cpbus_unsubscribe");
+      if (reuse_) Release(&it->second, 1);
       by_id_.erase(it->second);
       pending_subs_.erase(sub);
       registry_.erase(it);
@@ -331,6 +338,7 @@ class EventBus {   // events/bus.go:12-22
     if (!ids.empty()) {
       Retry([&] { return cpbus_unsubscribe_many(h_, ids.data(), (uint32_t)ids.size(), (int*)nullptr, (uint32_t*)nullptr); },
             "cpbus_unsubscribe_many");
+      if (reuse_) Release(ids.data(), ids.size());
       for (Subscriber* sub : subs) {
         auto it = registry_.find(sub);
         if (it == registry_.end()) continue;
@@ -443,6 +451,14 @@ class EventBus {   // events/bus.go:12-22
     if (!pending_subs_.empty()) throw std::logic_error("AckOnDelivery: the pump holds undelivered records");
     ack_ = on;
   }
+  // Subscriber id reuse (off by default).  Off, every Subscribe takes a fresh id, and a bus subscribes n_max_subs times in
+  // its life at most.  On, Unsubscribe releases the mailbox (cpbus_release_many) once the records it owed the channel have
+  // left it, so that n_max_subs bounds the live subscribers only: Subscribe and the timer-only channels' mailboxes take the
+  // lowest free id (cpbus_subscribe_list), a released one first.  Switch it before the first Subscribe.
+  void ReuseIds(bool on) {
+    std::lock_guard<std::recursive_mutex> l(lock_);
+    reuse_ = on;
+  }
   // Records the pump holds on the host for `sub` (taken or drained from its mailbox, not yet accepted by its channel).
   size_t Buffered(const Subscriber* sub) {
     std::lock_guard<std::recursive_mutex> l(lock_);
@@ -503,7 +519,12 @@ class EventBus {   // events/bus.go:12-22
     auto sub = std::make_unique<Subscriber>();
     sub->Rx = rx; sub->Bus = this; sub->implicit_ = true;
     uint32_t id = 0;
-    Retry([&] { return cpbus_subscribe(h_, 0u, &id); }, "cpbus_subscribe");
+    const uint32_t mask = 0;
+    if (reuse_)
+      Retry([&] { return cpbus_subscribe_list(h_, &mask, (const cpbus_pair*)nullptr, (const uint32_t*)nullptr, 1u, &id); },
+            "cpbus_subscribe_list");
+    else
+      Retry([&] { return cpbus_subscribe(h_, mask, &id); }, "cpbus_subscribe");
     sub->id_ = id;
     registry_[sub.get()] = id;
     by_id_[id] = sub.get();
@@ -515,12 +536,17 @@ class EventBus {   // events/bus.go:12-22
   // close(rx) on a timer-only channel: the Go timer goroutine panics on its next send, recovers and exits
   // (events/timer.go:26-30,50-54) — release the mailbox and with it the timers
   void ReleaseImplicit(Subscriber* sub) {
-    cpbus_unsubscribe(h_, sub->id_);
+    if (cpbus_unsubscribe(h_, sub->id_) == CPBUS_OK && reuse_) Release(&sub->id_, 1);
     by_id_.erase(sub->id_);
     pending_subs_.erase(sub);
     registry_.erase(sub);
     detail::RxRegistry().erase(sub->Rx.get());
     implicit_.erase(sub->Rx.get());
+  }
+
+  // ReuseIds: give unsubscribed ids back (their mailboxes owe their channels nothing any more)
+  void Release(const uint32_t* ids, size_t n) {
+    Retry([&] { return cpbus_release_many(h_, ids, (uint32_t)n, (int*)nullptr, (uint32_t*)nullptr); }, "cpbus_release_many");
   }
 
   static void Check(int rc, const char* where) {
@@ -638,6 +664,7 @@ class EventBus {   // events/bus.go:12-22
   static constexpr size_t kDrainCap = 1 << 16, kReadyCap = 4096;
   size_t drain_cap_ = kDrainCap;               // records per cpbus_drain_ready call (at least one mailbox's capacity)
   bool ack_ = false;                           // AckOnDelivery
+  bool reuse_ = false;                         // ReuseIds
   std::vector<cpbus_event> drain_buf_;
   std::vector<cpbus_ready> drain_ready_;
   detail::Handle h_;

@@ -121,14 +121,18 @@ class EventBus:
     """EventBus — events/bus.go:12-22.  NewEventBus() == EventBus()."""
 
     def __init__(self, n_max_subs: int = 64, ring_cap: int = 1024, batch_cap: int = 256, timers_per_sub: int = 4,
-                 lossless: bool = True, devices=None, sparse_records: bool = False, drop_missed_ticks: bool = False, **kw):
+                 lossless: bool = True, devices=None, sparse_records: bool = False, drop_missed_ticks: bool = False,
+                 reuse_ids: bool = False, **kw):
         """`devices`: run on a group of shards, shard g on devices[g] (GroupBus); the answers are the single bus's.
         The single bus is created with sparse timer delivery (CPBUS_CFG_SPARSE_TICKS): a pump step with nothing due
         launches nothing.  A group does not take that flag.
         `sparse_records` (single bus only): CPBUS_CFG_SPARSE_RECORDS, a Publish whose events reach few mailboxes
         launches only over them.
         `drop_missed_ticks`: CPBUS_CFG_DROP_MISSED_TICKS, a clock step across several periods of a NewEventTimer delivers
-        one tick, not one per period, as the Go ticker does (timer.go; its channel holds one tick)."""
+        one tick, not one per period, as the Go ticker does (timer.go; its channel holds one tick).
+        `reuse_ids`: Unsubscribe releases the mailbox (cpbus_release_many) once the records it owed the channel have left
+        it, and Subscribe and the timer-only channels' mailboxes take the lowest free id (cpbus_subscribe_list), so that
+        `n_max_subs` bounds the live subscribers rather than the subscriptions over the bus's life."""
         if sparse_records and devices is not None:
             raise ValueError("sparse_records: a group of shards does not take CPBUS_CFG_SPARSE_RECORDS")
         if devices is not None:
@@ -139,6 +143,7 @@ class EventBus:
                             lossless=lossless, digest=True, sparse_ticks=True, sparse_records=sparse_records,
                             drop_missed_ticks=drop_missed_ticks, **kw)
         self.reload = False
+        self._reuse = reuse_ids
         self._done = 0              # sync.WaitGroup counter (bus.go:16)
         self._subs = {}             # Subscriber -> sub_id  (registry, bus.go:13)
         self._implicit = {}         # Chan -> implicit Subscriber (timer-only channels; NOT in the registry or the WaitGroup)
@@ -162,6 +167,9 @@ class EventBus:
             # the channel already carries timer ticks (NewEventTimer came first): keep that mailbox and its timers, open the mask
             self._bus.set_mask(imp._id, mask)
             subscriber._id, subscriber._tail = imp._id, imp._tail
+        elif self._reuse:
+            pairs = [[(e.Code, self._bus.intern(e.Source)) for e in cases]] if cases else None
+            subscriber._id = int(self._bus.subscribe_list([mask], pairs)[0])
         elif cases:
             subscriber._id = self._bus.subscribe_pairs(mask, [(e.Code, self._bus.intern(e.Source)) for e in cases])
         else:
@@ -177,6 +185,8 @@ class EventBus:
         if subscriber in self._subs:
             subscriber._tail = self._drain(subscriber)       # keep what was delivered before the unsubscribe
             self._bus.unsubscribe(self._subs.pop(subscriber))
+            if self._reuse:
+                self._bus.release_many([subscriber._id])
             subscriber._id = None
         self._done -= 1
         if self._done < 0:
@@ -280,7 +290,8 @@ class EventBus:
         if sub is None:
             sub = Subscriber(rx)
             sub.Bus, sub._implicit = self, True
-            sub._id = self._bus.subscribe(0)          # empty mask: broadcasts never land here, ticks and direct sends do
+            # empty mask: broadcasts never land here, ticks and direct sends do
+            sub._id = int(self._bus.subscribe_list([0])[0]) if self._reuse else self._bus.subscribe(0)
             self._implicit[rx] = sub
         return sub
 
@@ -288,6 +299,8 @@ class EventBus:
         self._implicit.pop(sub.Rx, None)
         try:
             self._bus.unsubscribe(sub._id)            # disarms its timers too
+            if self._reuse:
+                self._bus.release_many([sub._id])
         except nat.CpbusError:
             pass
         sub._id = None

@@ -307,6 +307,35 @@ typedef struct cpbus_timer_spec {
 int cpbus_timer_add_list(cpbus_t* bus, const cpbus_timer_spec* specs, uint32_t n, uint32_t* timer_ids, int* status,
                          uint32_t* applied);
 
+/* ---- subscriber id reuse: ids behave like file descriptors.  An unsubscribed mailbox stays readable until it is released;
+ * a released id goes back to a free set, and cpbus_subscribe_list hands free ids out again, lowest first.  The caller must not
+ * use an id after releasing it: the next subscriber may already hold it.  cpbus_subscribe, _many, _pairs and _pairs_many
+ * hand out fresh ids only and never reuse one; a program that never releases sees no difference anywhere.
+ * cpbus_release_many: each element in array order; status[i] (status may be NULL): CPBUS_ENOENT (never handed out, or
+ * already released, by an earlier element of the same call too), CPBUS_EINVAL (still subscribed: unsubscribe it first) or
+ * CPBUS_OK; the call goes on past refused elements and *applied (may be NULL) = how many got CPBUS_OK.  Ordered with
+ * publishes: one flush runs where the first element that passes these checks would run it (none passes: no flush); in
+ * lossless mode its CPBUS_EAGAIN is returned with nothing applied and status / applied not written.  CPBUS_EINVAL (checked
+ * first): bus NULL, or sub_ids NULL with n > 0.  n == 0: CPBUS_OK, the bus is not read.
+ * A released id is in the state of an id never handed out: cpbus_send, _unsubscribe[_many], _set_mask[_many],
+ * _timer_add[_list], _timer_add_many (a range that holds one), _drain, _peek_window and _ack_many refuse it with
+ * CPBUS_ENOENT.  Range calls (drain_many, drain_ready, take_ready, lagging, digest, digest_fold) still take ranges up to
+ * the highest id ever handed out and see a released mailbox as empty: count and digest 0, nothing to return, never lagging.  Its records are discarded (taken and not yet
+ * acked ones too), and so are its take cursor and its exact cases.  Its timer slots keep their generations, and the next
+ * arming advances them, so a timer id of the old occupant stays stale (CPBUS_ENOENT) and never cancels a new occupant's.
+ * cpbus_subscribe_list: subscriber i gets code_masks[i] (code_masks NULL: CPBUS_MASK_ALL for all) and the first n_pairs[i]
+ * cases of row i of `pairs`, laid out as for cpbus_subscribe_pairs_many (n_pairs NULL: no cases).  Ids are the lowest free
+ * ones: released ids ascending, then fresh ones; sub_ids[i] receives subscriber i's id.  Each new subscriber starts as a
+ * fresh cpbus_subscribe_pairs leaves it: empty mailbox with ring_cap slots of room, count and digest 0, no timers, its mask
+ * and cases.  All or nothing: CPBUS_EINVAL (bus or sub_ids NULL, n == 0, n_pairs non-NULL with pairs NULL, n_pairs[i] >
+ * CPBUS_MAX_PAIRS or a case's code >= CPBUS_N_CODES), CPBUS_ENOSPC (fewer than n ids free), and one flush first, ordered
+ * with publishes, whose lossless CPBUS_EAGAIN applies nothing.
+ * The device work of either call is one H2D copy of one entry per mailbox (plus the rows of new cases), one kernel launch and
+ * one stream synchronisation; none when nothing is applied. ---- */
+int cpbus_release_many(cpbus_t* bus, const uint32_t* sub_ids, uint32_t n, int* status, uint32_t* applied);
+int cpbus_subscribe_list(cpbus_t* bus, const uint32_t* code_masks, const cpbus_pair* pairs, const uint32_t* n_pairs, uint32_t n,
+                         uint32_t* sub_ids);
+
 /* ---- the hot path: EventBus.Publish (events/bus.go:125-140) ---- */
 /* Stages n events; only code/source_id are read from ev (seq, ts, target, flags
  * are stamped by the bus).  Flushes automatically whenever batch_cap is reached.
@@ -702,6 +731,11 @@ int cpbus_group_timer_cancel_many(cpbus_group_t* g, const uint32_t* timer_ids, u
  * are global slots with their generation, as cpbus_group_timer_add returns them */
 int cpbus_group_timer_add_list(cpbus_group_t* g, const cpbus_timer_spec* specs, uint32_t n, uint32_t* timer_ids, int* status,
                                uint32_t* applied);
+/* subscriber id reuse: the group keeps the free set over global ids; each shard with work takes its elements, in array
+ * order, in one cpbus_release_many / cpbus_subscribe_list call */
+int cpbus_group_release_many(cpbus_group_t* g, const uint32_t* sub_ids, uint32_t n, int* status, uint32_t* applied);
+int cpbus_group_subscribe_list(cpbus_group_t* g, const uint32_t* code_masks, const cpbus_pair* pairs, const uint32_t* n_pairs,
+                               uint32_t n, uint32_t* sub_ids);
 int cpbus_group_publish(cpbus_group_t* g, const cpbus_event* ev, size_t n);
 int cpbus_group_send(cpbus_group_t* g, uint32_t sub_id, const cpbus_event* ev);
 int cpbus_group_advance(cpbus_group_t* g, uint64_t now_ns);
