@@ -172,7 +172,8 @@ SYMBOLS = {
 # the group (one handle over several shards): cpbus_group_<name> takes the arguments of cpbus_<name>
 GROUP_CALLS = ("intern", "intern_ephemeral", "source", "subscribe", "subscribe_many", "subscribe_pairs", "subscribe_pairs_many",
                "unsubscribe", "set_mask", "timer_add", "timer_add_many", "timer_cancel", "unsubscribe_many", "set_mask_many",
-               "timer_cancel_many", "timer_add_list", "release_many", "subscribe_list", "publish", "send", "advance", "flush",
+               "timer_cancel_many", "timer_add_list", "release_many", "subscribe_list", "publish", "send", "publish_device",
+               "publish_device_staged", "advance", "flush",
                "sync", "drain", "drain_ready", "take_ready", "ack_many", "lagging", "blockers", "consume_all", "peek_window", "digest", "digest_fold",
                "debug_events", "stats", "publish_counts")
 SYMBOLS["cpbus_group_create"] = (C.c_int, [_P(Config), C.c_void_p, C.c_uint32, _P(C.c_void_p)])

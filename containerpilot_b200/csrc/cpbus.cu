@@ -598,7 +598,15 @@ struct cpbus_group : HostFront {
   uint32_t n_next = 0, n_active = 0;
   std::vector<uint32_t> free_ids;       // released global indices, a min-heap (cpbus_group_subscribe_list)
   std::vector<cpbus_event> staged;      // B records
+  bool dev_counted = false;             // shard 0 has accounted a device batch (cpbus_group_publish_device)
 };
+
+// (defined with the stream below) the put of a batch into the next slot, from host or device memory, and a consumer's
+// launch of the next m records, with or without the accounting of a device-published batch
+extern "C" {
+static int stream_put(cpbus_stream* st, const cpbus_event* ev, size_t n, uint64_t now_ns, uint32_t flags, bool device_src);
+static int stream_fanout_prefix(cpbus_stream* st, size_t n, uint64_t now_ns, size_t m, bool account);
+}
 
 namespace {
 
@@ -641,7 +649,7 @@ void dbg_ring_put(HostFront* f, const cpbus_event& e) {   // events/bus.go:24-31
 
 // While the broadcast events of a device-published batch are still unknown to the host (a marker is pending), later
 // enqueues queue up behind it so that the ring keeps the global publish order; cpbus_debug_events resolves them.  (A group
-// queues no markers: for it this is a put.)
+// marks the device batches it launches, cpbus_group_publish_device, and resolves them against shard 0's accounting.)
 void dbg_enqueue(HostFront* f, const cpbus_event& e) {
   if (f->dbg_pending.empty()) { dbg_ring_put(f, e); return; }
   f->dbg_pending.push_back(DbgItem{false, 0ull, e});
@@ -664,9 +672,9 @@ size_t dbg_read(HostFront* f, cpbus_event* out, size_t cap) {
   return k;
 }
 
-void dbg_mark_device_batch(cpbus* b, unsigned long long launch) {
-  b->dbg_pending.push_back(DbgItem{true, launch, cpbus_event{}});
-  if (b->dbg_pending.size() > (size_t)kAcctDbgRing) b->dbg_pending.pop_front();
+void dbg_mark_device_batch(HostFront* f, unsigned long long launch) {
+  f->dbg_pending.push_back(DbgItem{true, launch, cpbus_event{}});
+  if (f->dbg_pending.size() > (size_t)kAcctDbgRing) f->dbg_pending.pop_front();
 }
 
 // The mask order of the ORDERED build, host-only (exported as cpbus_mask_order so that it can be tested without a GPU).
@@ -1181,25 +1189,30 @@ int flush_staged(cpbus* b, uint64_t w) {
 }
 
 // One launch of the single bus: the same early returns as launch_fanout, otherwise one stream batch on every shard.
-int group_launch(cpbus_group* g, const cpbus_event* ev, uint32_t n, uint64_t w) {
+// `device`: ev is a batch in device memory (cpbus_group_publish_device), which shard 0's put stream copies into the slot.
+// The group's host records hold every record it staged itself; a device batch is accounted where the single bus accounts
+// it, by the kernel — by shard 0's launch alone, marked in the group's debug ring in call order.
+int group_launch(cpbus_group* g, const cpbus_event* ev, uint32_t n, uint64_t w, bool device = false) {
   if (g->n_next == 0) return CPBUS_OK;
   if (n == 0 && g->n_timers == 0) return CPBUS_OK;
-  int rc = cpbus_stream_put(g->streams[0], ev, n, w, CPBUS_PUT_RAW);
+  int rc = stream_put(g->streams[0], ev, n, w, CPBUS_PUT_RAW, device);
   if (rc) return rc;
-  for (cpbus_stream* st : g->streams)   // the whole batch: already admitted on every shard, so it completes in one launch
-    if ((rc = cpbus_stream_fanout_prefix(st, n, w, n))) return rc;
+  for (size_t k = 0; k < g->streams.size(); k++)   // the whole batch: already admitted on every shard, so it completes in one launch
+    if ((rc = stream_fanout_prefix(g->streams[k], n, w, n, device && k == 0))) return rc;
   g->last_watermark = w;
+  if (device && n) { dbg_mark_device_batch(g, g->shards[0]->launch_seq); g->dev_counted = true; }
   return CPBUS_OK;
 }
 
-// Lossless admission of the staged records on every shard (admit), the single bus's verdict being the conjunction and its
-// prefix the minimum.  The records reach a shard's device only when its room bound cannot prove the fit.
-int group_admit(cpbus_group* g, uint32_t n, uint64_t w, bool* ok, uint32_t* m) {
+// Lossless admission of n records at src (the staged records, or a device batch) on every shard (admit), the single bus's
+// verdict being the conjunction and its prefix the minimum.  The records reach a shard's device only when its room bound
+// cannot prove the fit.
+int group_admit(cpbus_group* g, const cpbus_event* src, uint32_t n, uint64_t w, bool* ok, uint32_t* m) {
   *ok = true; *m = n;
   for (cpbus* s : g->shards) {
     if (admit_fits(s, n, w)) continue;
     int rc = dev_guard(s); if (rc) return rc;
-    if (n) CK(cudaMemcpyAsync(s->d_admit_batch, g->staged.data(), (size_t)n * sizeof(cpbus_event), cudaMemcpyHostToDevice, s->stream));
+    if (n) CK(cudaMemcpyAsync(s->d_admit_batch, src, (size_t)n * sizeof(cpbus_event), cudaMemcpyDefault, s->stream));
     bool ok_s = true;
     uint32_t m_s = n;
     if ((rc = admit_pass(s, s->d_admit_batch, n, w, &ok_s, &m_s))) return rc;
@@ -1216,7 +1229,7 @@ int flush_staged(cpbus_group* g, uint64_t w) {
   bool ok = true;
   uint32_t m = n;
   int rc;
-  if (g->lossless && (rc = group_admit(g, n, w, &ok, &m))) return rc;
+  if (g->lossless && (rc = group_admit(g, g->staged.data(), n, w, &ok, &m))) return rc;
   if (!ok) {
     if (m == 0) return CPBUS_EAGAIN;
     if ((rc = group_launch(g, g->staged.data(), m, g->staged[m - 1].ts_ns))) return rc;
@@ -2657,9 +2670,9 @@ int cpbus_stream_status(cpbus_stream_t* st) try {
   return stream_error(st->bus);
 } CPBUS_CATCH
 
-// Publisher: copy the batch into the next slot, then release it (header after payload, same stream).
-int cpbus_stream_put(cpbus_stream_t* st, const cpbus_event* ev, size_t n, uint64_t now_ns, uint32_t flags) try {
-  if (!st || !st->owner || (!ev && n) || n > st->B) return CPBUS_EINVAL;
+// Publisher: copy the batch into the next slot, then release it (header after payload, same stream).  `device_src`: ev
+// holds complete records in device memory (this GPU's or a peer's), copied into the slot as they are (CPBUS_PUT_RAW).
+static int stream_put(cpbus_stream* st, const cpbus_event* ev, size_t n, uint64_t now_ns, uint32_t flags, bool device_src) {
   cpbus* b = st->bus;
   int rc = dev_guard(b); if (rc) return rc;
   const unsigned long long q = st->put_seq + 1;
@@ -2682,7 +2695,9 @@ int cpbus_stream_put(cpbus_stream_t* st, const cpbus_event* ev, size_t n, uint64
   const int s = (int)(q % cpbus_stream::kStage);
   CK(cudaEventSynchronize(st->staged_done[s]));   // the pinned buffers of batch q - kStage have left the host
   cpbus_event* dst = st->h_stage[s];
-  if (flags & CPBUS_PUT_RAW) { if (n) memcpy(dst, ev, n * sizeof(cpbus_event)); }
+  const cpbus_event* src = dst;
+  if (device_src) src = ev;
+  else if (flags & CPBUS_PUT_RAW) { if (n) memcpy(dst, ev, n * sizeof(cpbus_event)); }
   else {
     for (size_t i = 0; i < n; i++) {
       const uint32_t code = ev[i].code;
@@ -2692,7 +2707,8 @@ int cpbus_stream_put(cpbus_stream_t* st, const cpbus_event* ev, size_t n, uint64
     }
   }
   const uint32_t slot = (uint32_t)(q % st->n_slots);
-  if (n) CK(cudaMemcpyAsync(st->payload + (size_t)slot * st->B, dst, n * sizeof(cpbus_event), cudaMemcpyHostToDevice, st->put_stream));
+  if (n) CK(cudaMemcpyAsync(st->payload + (size_t)slot * st->B, src, n * sizeof(cpbus_event),
+                            device_src ? cudaMemcpyDefault : cudaMemcpyHostToDevice, st->put_stream));
   StreamHdr* hh = &st->h_hdr[s];
   memset(hh, 0, sizeof(*hh));
   hh->seq = q; hh->watermark = now_ns; hh->n = (uint32_t)n;
@@ -2701,6 +2717,11 @@ int cpbus_stream_put(cpbus_stream_t* st, const cpbus_event* ev, size_t n, uint64
   CK(cudaEventRecord(st->staged_done[s], st->put_stream));
   st->put_seq = q;
   return CPBUS_OK;
+}
+
+int cpbus_stream_put(cpbus_stream_t* st, const cpbus_event* ev, size_t n, uint64_t now_ns, uint32_t flags) try {
+  if (!st || !st->owner || (!ev && n) || n > st->B) return CPBUS_EINVAL;
+  return stream_put(st, ev, n, now_ns, flags, false);
 } CPBUS_CATCH
 
 // Consumers that are NOT told n / now_ns by their driver: look at the next slot's header (one 32-byte copy across the link).
@@ -2809,7 +2830,8 @@ static void stream_delivered(cpbus* b, cpbus_stream* st, uint32_t m, uint64_t w,
 }
 
 // Fan out the next m undelivered records of the current batch (throughput mode: m = the whole batch, in one launch).
-static int stream_fanout_prefix(cpbus_stream* st, size_t n, uint64_t now_ns, size_t m) {
+// `account`: the lead CTA accounts the records as a device-published batch (a group's shards: see group_launch).
+static int stream_fanout_prefix(cpbus_stream* st, size_t n, uint64_t now_ns, size_t m, bool account) {
   cpbus* b = st->bus;
   int rc = stream_enter(st, now_ns); if (rc) return rc;
   const bool final = m == n - st->get_off;
@@ -2818,6 +2840,7 @@ static int stream_fanout_prefix(cpbus_stream* st, size_t n, uint64_t now_ns, siz
   StreamArgs sa;
   LaunchOpts o;
   const cpbus_event* src = stream_launch(st, q, st->get_off, final, sa, o);
+  o.account = account;
   uint64_t w = now_ns;
   if (!final) {
     // Like a partial cpbus_flush: the watermark is the last delivered record's timestamp, so the ticks due after it go with
@@ -2839,14 +2862,14 @@ static int stream_fanout_prefix(cpbus_stream* st, size_t n, uint64_t now_ns, siz
 
 int cpbus_stream_fanout_prefix(cpbus_stream_t* st, size_t n, uint64_t now_ns, size_t m) try {
   if (!st || n > st->B || st->get_off > n || m > n - st->get_off) return CPBUS_EINVAL;
-  return stream_fanout_prefix(st, n, now_ns, m);
+  return stream_fanout_prefix(st, n, now_ns, m, true);
 } CPBUS_CATCH
 
 // Every rank (the publisher's included): fan out the next batch of the stream to this GPU's shard.
 int cpbus_stream_fanout(cpbus_stream_t* st, size_t n, uint64_t now_ns) try {
   if (!st || n > st->B || st->get_off > n) return CPBUS_EINVAL;
   if (st->bus->lossless) return CPBUS_EINVAL;   // without admission this shard could deliver more than another one does
-  return stream_fanout_prefix(st, n, now_ns, n - st->get_off);
+  return stream_fanout_prefix(st, n, now_ns, n - st->get_off, true);
 } CPBUS_CATCH
 
 // Outstanding follower launches and lossless rounds: one wait on the last of them, then their records in launch order.  A
@@ -3470,30 +3493,31 @@ int cpbus_step_result_end(cpbus_t* b, uint32_t ticket, uint64_t out[4]) try {
 
 // DebugEvents — events/bus.go:34-54
 // Broadcast events of device-published batches join the debug ring here, in publish order (the kernel's lead CTA kept
-// the last 10 of each such batch; launches older than kAcctDbgRing are no longer resolvable and are skipped).
-static int dbg_resolve(cpbus* b) {
-  if (b->dbg_pending.empty()) return CPBUS_OK;
+// the last 10 of each such batch; launches older than kAcctDbgRing are no longer resolvable and are skipped).  f's markers
+// name launches of bus b (f = b, or a group and its shard 0).
+static int dbg_resolve(HostFront* f, cpbus* b) {
+  if (f->dbg_pending.empty()) return CPBUS_OK;
   bool any_marker = false;
-  for (const DbgItem& it : b->dbg_pending) any_marker |= it.marker;
+  for (const DbgItem& it : f->dbg_pending) any_marker |= it.marker;
   if (any_marker) {
     int rc = dev_guard(b); if (rc) return rc;
     CK(cudaMemcpyAsync(b->host_acct()->tail, b->d_acct->tail, sizeof(b->host_acct()->tail), cudaMemcpyDeviceToHost, b->stream));
     CK(cudaStreamSynchronize(b->stream));
   }
-  for (const DbgItem& it : b->dbg_pending) {
-    if (!it.marker) { dbg_ring_put(b, it.ev); continue; }
+  for (const DbgItem& it : f->dbg_pending) {
+    if (!it.marker) { dbg_ring_put(f, it.ev); continue; }
     const DevDbgTail& t = b->host_acct()->tail[it.launch % kAcctDbgRing];
     if (t.launch_seq != it.launch) continue;
-    for (uint32_t j = 0; j < t.n_kept && j < (uint32_t)kAcctDbgKeep; j++) dbg_ring_put(b, t.ev[j]);
+    for (uint32_t j = 0; j < t.n_kept && j < (uint32_t)kAcctDbgKeep; j++) dbg_ring_put(f, t.ev[j]);
   }
-  b->dbg_pending.clear();
+  f->dbg_pending.clear();
   return CPBUS_OK;
 }
 
 int cpbus_debug_events(cpbus_t* b, cpbus_event* out, size_t cap, size_t* n) try {
   if (!b || !n || (!out && cap)) return CPBUS_EINVAL;
   { const int rc = follow_resolve(b); if (rc) return rc; }
-  { const int rc = dbg_resolve(b); if (rc) return rc; }
+  { const int rc = dbg_resolve(b, b); if (rc) return rc; }
   *n = dbg_read(b, out, cap);
   return CPBUS_OK;
 } CPBUS_CATCH
@@ -3526,6 +3550,15 @@ int cpbus_stats(cpbus_t* b, cpbus_stats_t* out) try {
   return CPBUS_OK;
 } CPBUS_CATCH
 
+// The {code, source} table of bus b's device-published batches (DevPubAcct), read back behind b's launches.
+static int device_pairs(cpbus* b, std::vector<unsigned long long>& keys, std::vector<unsigned long long>& cnts) {
+  keys.resize(kAcctPairSlots); cnts.resize(kAcctPairSlots);
+  CK(cudaMemcpyAsync(keys.data(), b->d_acct->pair_key, sizeof(unsigned long long) * kAcctPairSlots, cudaMemcpyDeviceToHost, b->stream));
+  CK(cudaMemcpyAsync(cnts.data(), b->d_acct->pair_cnt, sizeof(unsigned long long) * kAcctPairSlots, cudaMemcpyDeviceToHost, b->stream));
+  CK(cudaStreamSynchronize(b->stream));
+  return CPBUS_OK;
+}
+
 // containerpilot_events{code, source} (events/bus.go:60-68,130-132): host publishes are counted in cpbus_publish, batches
 // that arrive in device memory by the fan-out kernel's lead CTA (DevPubAcct).
 int cpbus_publish_counts(cpbus_t* b, cpbus_pair_count* out, size_t cap, size_t* n) try {
@@ -3533,12 +3566,7 @@ int cpbus_publish_counts(cpbus_t* b, cpbus_pair_count* out, size_t cap, size_t* 
   std::lock_guard<std::mutex> g(b->mu);
   int rc = enter(b); if (rc) return rc;
   std::vector<unsigned long long> keys, cnts;
-  if (b->launch_seq) {
-    keys.resize(kAcctPairSlots); cnts.resize(kAcctPairSlots);
-    CK(cudaMemcpyAsync(keys.data(), b->d_acct->pair_key, sizeof(unsigned long long) * kAcctPairSlots, cudaMemcpyDeviceToHost, b->stream));
-    CK(cudaMemcpyAsync(cnts.data(), b->d_acct->pair_cnt, sizeof(unsigned long long) * kAcctPairSlots, cudaMemcpyDeviceToHost, b->stream));
-    CK(cudaStreamSynchronize(b->stream));
-  }
+  if (b->launch_seq && (rc = device_pairs(b, keys, cnts))) return rc;
   pair_counts(b, keys.data(), cnts.data(), keys.size(), out, cap, n);
   return CPBUS_OK;
 } CPBUS_CATCH
@@ -3623,6 +3651,18 @@ int cpbus_group_create(const cpbus_config* cfg, const int32_t* devices, uint32_t
     if ((rc = cpbus_stream_attach(g->shards[k], st0, k, &st))) return fail(rc);
     g->streams.push_back(st);
   }
+  // a device batch (cpbus_group_publish_device) may live on any GPU of the group: peer access between every two of them
+  // where the hardware has it, as cpbus_stream_attach enables it towards shard 0
+  for (cpbus* a : g->shards)
+    for (cpbus* b : g->shards) {
+      if (a->device == b->device) continue;
+      int can = 0;
+      if (cudaSetDevice(a->device) != cudaSuccess || cudaDeviceCanAccessPeer(&can, a->device, b->device) != cudaSuccess) return fail(CPBUS_ECUDA);
+      if (!can) continue;
+      const cudaError_t e = cudaDeviceEnablePeerAccess(b->device, 0);
+      if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) return fail(CPBUS_ECUDA);
+      cudaGetLastError();   // clear "already enabled"
+    }
   *out = g;
   return CPBUS_OK;
 } CPBUS_CATCH
@@ -4021,6 +4061,73 @@ int cpbus_group_publish(cpbus_group_t* g, const cpbus_event* ev, size_t n) try {
   return publish_burst(g, ev, n);
 } CPBUS_CATCH
 
+// Device batches on the group: publish_device_impl's rules on the group's host front (flush first, the order and argument
+// checks, lossless all-or-nothing admission on every shard, the single bus's split), each launch one stream batch whose
+// payload shard 0's put stream copies from d_events (group_launch).  The prefetch hints are checked as the single bus checks
+// them; the fan-out kernels read shard 0's stream slot, and throughput-mode stream launches already pull the slot after
+// next, so there is nothing for the hints to add.
+static int group_publish_device(cpbus_group* g, const cpbus_event* d_events, size_t n, uint64_t watermark_ns, bool staged,
+                                const void* d_next, size_t n_next);
+
+// publish_device_split on the group: the records' timestamps are read on the stream of a shard on the batch's GPU
+static int group_publish_device_split(cpbus_group* g, const cpbus_event* d_events, size_t n, uint64_t watermark_ns, bool staged,
+                                      const void* d_next, size_t n_next) {
+  std::vector<uint64_t> ts(n), wm;
+  std::vector<size_t> end;
+  cpbus* s = g->shards[0];
+  if (n) {
+    cudaPointerAttributes a{};
+    CK(cudaPointerGetAttributes(&a, d_events));
+    for (cpbus* x : g->shards) if (x->device == a.device) { s = x; break; }
+    int rc = dev_guard(s); if (rc) return rc;
+    CK(cudaMemcpy2DAsync(ts.data(), 8, reinterpret_cast<const unsigned char*>(d_events) + offsetof(cpbus_event, ts_ns), sizeof(cpbus_event),
+                         8, n, cudaMemcpyDefault, s->stream));
+    CK(cudaStreamSynchronize(s->stream));
+  }
+  int rc = split_plan(ts.data(), n, g->B, g->now, watermark_ns, max_window(g), end, wm);
+  if (rc) return rc;
+  size_t i = 0;
+  for (size_t k = 0; k < end.size(); k++) {
+    const bool last = k + 1 == end.size();
+    rc = group_publish_device(g, d_events + i, end[k] - i, wm[k], staged, last ? d_next : nullptr, last ? n_next : 0);
+    if (rc) return rc;
+    g->shards[0]->st.device_splits++;
+    i = end[k];
+  }
+  return CPBUS_OK;
+}
+
+static int group_publish_device(cpbus_group* g, const cpbus_event* d_events, size_t n, uint64_t watermark_ns, bool staged,
+                                const void* d_next, size_t n_next) {
+  if (!g || (!d_events && n) || ((uintptr_t)d_events & 31u) || n_next > g->B || ((uintptr_t)d_next & 31u)) return CPBUS_EINVAL;
+  int rc = flush_staged(g, g->now); if (rc) return rc;
+  if (watermark_ns < g->now) return CPBUS_EORDER;
+  if (staged && g->lossless) return CPBUS_EINVAL;
+  if (n > g->B || watermark_ns - g->last_watermark > max_window(g)) {
+    if (g->lossless) return n > g->B ? CPBUS_EINVAL : CPBUS_EORDER;
+    return group_publish_device_split(g, d_events, n, watermark_ns, staged, d_next, n_next);
+  }
+  bool ok = true;
+  uint32_t m = (uint32_t)n;
+  if (g->lossless && (rc = group_admit(g, d_events, (uint32_t)n, watermark_ns, &ok, &m))) return rc;
+  if (!ok) return CPBUS_EAGAIN;   // (refused on some shard: nothing was put)
+  g->now = watermark_ns;
+  if ((rc = group_launch(g, d_events, (uint32_t)n, watermark_ns, true))) return rc;
+  g->publishes += n; g->seq += n;
+  return CPBUS_OK;
+}
+
+int cpbus_group_publish_device(cpbus_group_t* g, const void* d_events, size_t n, uint64_t watermark_ns) try {
+  if (g && g->drop_missed) return CPBUS_EINVAL;
+  return group_publish_device(g, (const cpbus_event*)d_events, n, watermark_ns, false, nullptr, 0);
+} CPBUS_CATCH
+
+int cpbus_group_publish_device_staged(cpbus_group_t* g, const void* d_events, size_t n, uint64_t watermark_ns, const void* d_next,
+                                      size_t n_next) try {
+  if (g && g->drop_missed) return CPBUS_EINVAL;
+  return group_publish_device(g, (const cpbus_event*)d_events, n, watermark_ns, true, d_next, n_next);
+} CPBUS_CATCH
+
 int cpbus_group_send(cpbus_group_t* g, uint32_t sub_id, const cpbus_event* ev) try {
   if (!g || !ev || ev->code >= CPBUS_N_CODES) return CPBUS_EINVAL;
   cpbus* s = nullptr; uint32_t l = 0;
@@ -4235,6 +4342,7 @@ int cpbus_group_digest_fold(cpbus_group_t* g, uint32_t first_sub, uint32_t n, ui
 
 int cpbus_group_debug_events(cpbus_group_t* g, cpbus_event* out, size_t cap, size_t* n) try {   // cpbus_debug_events
   if (!g || !n || (!out && cap)) return CPBUS_EINVAL;
+  const int rc = dbg_resolve(g, g->shards[0]); if (rc) return rc;
   *n = dbg_read(g, out, cap);
   return CPBUS_OK;
 } CPBUS_CATCH
@@ -4252,7 +4360,8 @@ int cpbus_group_stats(cpbus_group_t* g, cpbus_stats_t* out) try {
   }
   group_retire(g);
   sum.publishes = g->publishes;
-  for (int c = 0; c < CPBUS_N_CODES; c++) sum.published_by_code[c] = g->published_by_code[c];
+  for (int c = 0; c < CPBUS_N_CODES; c++)   // + device batches, accounted by shard 0's launches alone (group_launch)
+    sum.published_by_code[c] = g->published_by_code[c] + s0.published_by_code[c];
   sum.n_subs = g->n_active; sum.n_timers = g->n_timers; sum.now_ns = g->now;
   sum.intern_entries = s0.intern_entries; sum.intern_bytes = s0.intern_bytes;
   sum.ephemeral_live = s0.ephemeral_live; sum.ephemeral_recycled = s0.ephemeral_recycled;
@@ -4262,7 +4371,12 @@ int cpbus_group_stats(cpbus_group_t* g, cpbus_stats_t* out) try {
 
 int cpbus_group_publish_counts(cpbus_group_t* g, cpbus_pair_count* out, size_t cap, size_t* n) try {
   if (!g || !n || (!out && cap)) return CPBUS_EINVAL;
-  pair_counts(g, nullptr, nullptr, 0, out, cap, n);
+  std::vector<unsigned long long> keys, cnts;
+  if (g->dev_counted) {
+    int rc = dev_guard(g->shards[0]);
+    if (rc || (rc = device_pairs(g->shards[0], keys, cnts))) return rc;
+  }
+  pair_counts(g, keys.data(), cnts.data(), keys.size(), out, cap, n);
   return CPBUS_OK;
 } CPBUS_CATCH
 

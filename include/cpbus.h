@@ -704,7 +704,14 @@ int cpbus_device_ptrs(cpbus_t* bus, void** ring, void** ctl);
  * clock steps and cuts lossless prefixes where the single bus does, and admits each flush on every shard before it puts
  * the part every shard can take into the stream.
  * The intern table is shard 0's; the other shards only ever see source ids.  debug_events, publish_counts and
- * published_by_code are the group's own host records; deliveries, ticks and overwritten are sums over the shards. */
+ * published_by_code are the group's own host records, merged with what shard 0's kernel accounted of the device batches
+ * (cpbus_group_publish_device*); deliveries, ticks and overwritten are sums over the shards.
+ * Device batches: cpbus_group_publish_device and _staged keep every rule of the single-bus calls (flush first, the order
+ * and argument checks, all-or-nothing in lossless mode, the same cut of a batch one launch cannot take, CPBUS_EINVAL on a
+ * CPBUS_CFG_DROP_MISSED_TICKS group).  d_events may live in the HBM of any GPU in the group's device list (the group
+ * enables peer access between them); each launch copies the batch into shard 0's stream slot on the device and every
+ * shard fans it out, so d_events must stay unchanged until cpbus_group_sync returns.  d_next / n_next are checked as on
+ * the single bus and otherwise have no effect: the shards read the stream slot, not d_events. */
 typedef struct cpbus_group cpbus_group_t;
 int cpbus_group_create(const cpbus_config* cfg, const int32_t* devices, uint32_t n_devices, cpbus_group_t** out);
 int cpbus_group_destroy(cpbus_group_t* g);
@@ -738,6 +745,9 @@ int cpbus_group_subscribe_list(cpbus_group_t* g, const uint32_t* code_masks, con
                                uint32_t n, uint32_t* sub_ids);
 int cpbus_group_publish(cpbus_group_t* g, const cpbus_event* ev, size_t n);
 int cpbus_group_send(cpbus_group_t* g, uint32_t sub_id, const cpbus_event* ev);
+int cpbus_group_publish_device(cpbus_group_t* g, const void* d_events, size_t n, uint64_t watermark_ns);
+int cpbus_group_publish_device_staged(cpbus_group_t* g, const void* d_events, size_t n, uint64_t watermark_ns,
+                                      const void* d_next, size_t n_next);
 int cpbus_group_advance(cpbus_group_t* g, uint64_t now_ns);
 int cpbus_group_flush(cpbus_group_t* g);
 int cpbus_group_sync(cpbus_group_t* g);
