@@ -215,6 +215,8 @@
         dst[i] = v;
         if (lead) loc[i] = v;
       }
+      // the bulk store path reads s_batch through the async proxy (cp.async.bulk): order these generic writes before it
+      if constexpr (STORE == CPBUS_STORE_BULK) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     }
     mbar_wait(&s_sum->mbar, 0);
     __syncthreads();

@@ -43,15 +43,23 @@ def test_pair_filter_semantics_and_errors():
         assert bus.subscribe_pairs(1 << 5, [(5, 3)]) == 0          # pair already covered by the mask: plain subscription
 
 
-@pytest.mark.parametrize("seed,K,batch_cap", [(1, 0, 32), (2, 1, 64), (3, 2, 128), (4, 4, 256), (5, 8, 512), (6, 0, 512),
-                                              (7, 0, 256), (8, 2, 32)])
-def test_pair_filter_random_traces(seed, K, batch_cap):
-    """pairs mixed with plain masks, unicast sends, membership changes, clock advances and timers"""
-    ops, n_total = tr.random_ops(seed + 900, 24, 4000, timers_per_sub=K, max_subs=40, p_filter=0.8, p_send=0.04,
+PAIR_TRACES = [(1, 0, 32, 0), (2, 1, 64, 0), (3, 2, 128, 0), (4, 4, 256, 0), (5, 8, 512, 0), (6, 0, 512, 0), (7, 0, 256, 0),
+               (8, 2, 32, 0), (9, 0, 64, 1), (10, 2, 256, 1), (11, 1, 128, 3), (12, 4, 512, 3)]
+
+
+@pytest.mark.parametrize("seed,K,batch_cap,grid_ctas", PAIR_TRACES,
+                         ids=[f"{s}-{k}-{b}" + (f"-grid{g}" if g else "") for s, k, b, g in PAIR_TRACES])
+def test_pair_filter_random_traces(seed, K, batch_cap, grid_ctas):
+    """pairs mixed with plain masks, unicast sends, membership changes, clock advances and timers.  A fixed grid
+    (grid_ctas) over ~1,000 subscribers makes every warp walk several blocks of 32 mailboxes in the triage loop, which the
+    default grid does only above 540,672 subscribers on an H100"""
+    n0 = 900 if grid_ctas else 24
+    ops, n_total = tr.random_ops(seed + 900, n0, 4000, timers_per_sub=K, max_subs=n0 + 16, p_filter=0.8, p_send=0.04,
                                  n_sources=5, p_pairs=0.6)
     assert any(len(op) > 2 for op in ops if op[0] == "sub")
-    orc = tr.run_oracle(ops, 40, timers_per_sub=K)
-    with Bus(40, ring_cap=4096, batch_cap=batch_cap, timers_per_sub=K) as bus:
+    assert not grid_ctas or (n_total + 31) // 32 > 8 * grid_ctas            # more triage blocks than warps
+    orc = tr.run_oracle(ops, n0 + 16, timers_per_sub=K)
+    with Bus(n0 + 16, ring_cap=4096, batch_cap=batch_cap, timers_per_sub=K, grid_ctas=grid_ctas) as bus:
         tr.run_bus(bus, ops)
         tr.compare(bus, orc, n_total, window=4096)
 

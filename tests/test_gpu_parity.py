@@ -5,6 +5,7 @@ import numpy as np
 import pytest
 
 import oracle_binding as ob
+import ring_check as rc
 import trace as tr
 from containerpilot_b200 import _native as nat
 from containerpilot_b200.bus import Bus, EVENT_DTYPE
@@ -210,8 +211,13 @@ def test_full_size_config2_properties():
         want = orc.mailbox(0).tobytes()
         for s in (0, 1, 7, 4095, 32_768, 65_535):
             assert bus.peek_window(s).tobytes() == want
-        # the ring memory itself: every mailbox identical (encode -> compare, no sampling)
+        # the ring memory itself: every mailbox's tail and ring against the fleet reference (no sampling)
         ptrs = bus.device_ptrs()
+        model = rc.FleetModel(n_subs, 1024, ev, [(i, i + B, 0) for i in range(0, n_events, B)],
+                              np.full(n_subs, nat.MASK_ALL, dtype=np.uint32))
+        model.pin((0, 65_535))
+        with rc.fleet_views(ptrs, n_subs, 1024) as views:
+            assert rc.check(views, model) == n_subs * 1024
         st = bus.stats()
         assert st["deliveries"] == n_subs * n_events
 
