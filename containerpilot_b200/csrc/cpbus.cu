@@ -5,17 +5,17 @@
 // table, the virtual clock, staging of published events into pinned batches.
 // There is NO CPU data path: without a CUDA device cpbus_create fails with
 // CPBUS_ENODEV, and nothing here touches oracle/.
-#include "cpbus_kernels.cuh"
-#include "cuda_owned.hpp"
+//
+// This file holds the single bus and its streams, and every kernel launch of the library; the group is
+// cpbus_group.cpp, the host-only planners and exports cpbus_host.cpp, and what they share cpbus_internal.hpp.
+#include "cpbus_internal.hpp"
 
 #include <algorithm>
 #include <chrono>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
-#include <deque>
 #include <functional>
-#include <map>
 #include <mutex>
 #include <new>
 #include <string>
@@ -23,614 +23,24 @@
 #include <unordered_map>
 #include <vector>
 
-using namespace cpbus_dev;
-using namespace cuda_owned;
-
-namespace {
-
-thread_local char g_cuda_err[256] = "";
-
-#define CK(call)                                                                                   \
-  do {                                                                                             \
-    cudaError_t e_ = (call);                                                                       \
-    if (e_ != cudaSuccess) {                                                                       \
-      snprintf(g_cuda_err, sizeof(g_cuda_err), "%s:%d %s: %s", __FILE__, __LINE__, #call,          \
-               cudaGetErrorString(e_));                                                            \
-      return CPBUS_ECUDA;                                                                          \
-    }                                                                                              \
-  } while (0)
-
-// debug ring entry awaiting enqueue: a concrete event, or "the broadcast events of device launch `launch`"
-struct DbgItem { bool marker; unsigned long long launch; cpbus_event ev; };
-
-// publish counts by (code << 32 | source_id): the label set of `containerpilot_events` (events/bus.go:131).  Flat
-// open-addressing table (key + 1 stored, 0 = empty): an increment is one probe in the common case, and a burst of n
-// events is counted in two passes (slots prefetched, then incremented) so that cache misses of a high-cardinality
-// source set overlap instead of adding up (a std::unordered_map here cost ~40 ns per published event).
-struct PairCounter {
-  std::vector<uint64_t> keys, cnts;
-  size_t used = 0;
-  static uint64_t mix(uint64_t k) { k ^= k >> 33; k *= 0xff51afd7ed558ccdull; k ^= k >> 33; return k; }
-  void grow() {
-    std::vector<uint64_t> ok, oc;
-    ok.swap(keys); oc.swap(cnts);
-    const size_t cap = ok.empty() ? 1024 : ok.size() * 2;
-    keys.assign(cap, 0); cnts.assign(cap, 0); used = 0;
-    for (size_t i = 0; i < ok.size(); i++) if (ok[i]) add(ok[i] - 1, oc[i]);
-  }
-  void add(uint64_t key, uint64_t by) {
-    if ((used + 1) * 2 > keys.size()) grow();
-    const size_t mask = keys.size() - 1;
-    for (size_t i = mix(key) & mask;; i = (i + 1) & mask) {
-      if (keys[i] == key + 1) { cnts[i] += by; return; }
-      if (!keys[i]) { keys[i] = key + 1; cnts[i] = by; used++; return; }
-    }
-  }
-  void prefetch(uint64_t key) const { if (!keys.empty()) { const size_t i = mix(key) & (keys.size() - 1); __builtin_prefetch(&keys[i]); __builtin_prefetch(&cnts[i]); } }
-};
-
-struct HostTimer { bool active = false, oneshot = false; uint8_t gen = 0; uint64_t period = 0, next_due = 0; uint32_t source_id = 0; };
-// Due times saturate: one that would pass UINT64_MAX - 1 is kTimerIdle, "never".  The slot stays armed (it counts in
-// n_timers and can be cancelled); the kernel never fires a tick due at kTimerIdle.
-inline uint64_t due_after(uint64_t t, uint64_t period) { return period >= kTimerIdle - t ? kTimerIdle : t + period; }
-// a one-shot due by watermark w has fired on the device and disarmed itself
-inline bool oneshot_fired(uint64_t next_due, uint64_t w) { return next_due <= w && next_due != kTimerIdle; }
-// timer id = slot index (subscriber * K + k) | generation << 26: a late cancel from an old context cannot disarm a re-armed slot
-constexpr uint32_t kTimerSlotBits = 26, kTimerSlotMask = (1u << kTimerSlotBits) - 1u;
-
-// The due index of a CPBUS_CFG_SPARSE_TICKS bus: every armed slot whose next due time is not kTimerIdle, as {due, slot}
-// entries in buckets of 2^kDueShift ns of due time (a calendar queue: a std::map from bucket to an unsorted vector of
-// entries, with a lower bound of the bucket's due times).  Arming appends to one bucket, O(1) after the bucket's lookup;
-// a launch to w takes the buckets wholly at or before w and scans the one that w falls in.  Nothing is removed from the
-// middle of a bucket: a cancel, an unsubscribe or a re-arm bumps the slot's version, and an entry whose version is not the
-// slot's any more is stale and skipped (32-bit versions, so a stale entry never passes for a live one the way a 6-bit
-// timer-id generation could).  The whole index is rebuilt when stale entries outnumber the live ones.  A live slot's due
-// time is also its HostTimer::next_due.  (A binary heap was measured first: at 10^6 slots each pop costs ~20 cache misses,
-// ~2 us per due slot on the host; DESIGN.md §4.6.)
-struct DueIndex {
-  static constexpr int kDueShift = 20;   // ~1 ms of due time per bucket: the pump's step
-  struct Entry { uint64_t due; uint32_t slot, ver; };
-  struct Bucket { uint64_t lo = kTimerIdle; std::vector<Entry> e; };   // lo <= every live due in e
-  std::map<uint64_t, Bucket> buckets;
-  std::vector<uint32_t> ver;      // per slot
-  std::vector<uint8_t> live;      // per slot: its current entry is in a bucket
-  size_t n_live = 0, n_entries = 0;
-  bool stale(const Entry& e) const { return ver[e.slot] != e.ver; }
-  void init(size_t n_slots) { buckets.clear(); hot = nullptr; ver.assign(n_slots, 0); live.assign(n_slots, 0); n_live = n_entries = 0; }
-  void drop(uint32_t slot) {
-    ver[slot]++;
-    if (live[slot]) { live[slot] = 0; n_live--; }
-  }
-  Bucket* hot = nullptr;          // the bucket the last insert went to (re-arms of one launch mostly share one)
-  uint64_t hot_key = 0;
-  void insert(const Entry& e) {
-    const uint64_t k = e.due >> kDueShift;
-    if (!hot || hot_key != k) { hot = &buckets[k]; hot_key = k; }
-    hot->e.push_back(e); hot->lo = std::min(hot->lo, e.due);
-    n_entries++;
-  }
-  void put(uint32_t slot, uint64_t due) {
-    drop(slot);
-    if (due == kTimerIdle) return;   // "never": not indexed, though the slot stays armed
-    live[slot] = 1; n_live++;
-    insert(Entry{due, slot, ver[slot]});
-    if (n_entries > 2 * n_live + 64) compact();
-  }
-  void compact() {
-    std::map<uint64_t, Bucket> old;
-    old.swap(buckets);
-    hot = nullptr; n_entries = 0;
-    for (auto& kv : old) for (const Entry& e : kv.second.e) if (!stale(e)) insert(e);
-  }
-  // a lower bound of the earliest due time (kTimerIdle: nothing indexed); exact unless the first bucket holds stale entries
-  uint64_t min_due() const { return buckets.empty() ? kTimerIdle : buckets.begin()->second.lo; }
-  // The live slots due at or before w, appended to *out in no particular order, when there are at most cap of them (true);
-  // false as soon as there are more.  Reads only the buckets that begin at or before w.
-  bool collect(uint64_t w, size_t cap, std::vector<uint32_t>* out) const {
-    size_t found = 0;
-    for (auto it = buckets.begin(); it != buckets.end() && it->first <= (w >> kDueShift); ++it)
-      for (const Entry& e : it->second.e)
-        if (e.due <= w && !stale(e)) {
-          if (++found > cap) return false;
-          out->push_back(e.slot);
-        }
-    return true;
-  }
-};
-
-// Firings of a periodic slot due at `due` <= w in one launch to w, as the kernel counts them: the candidates due + j *
-// period <= w that do not reach kTimerIdle.  And the due time after k firings, saturating like the kernel's re-arm.
-inline uint64_t due_ticks(uint64_t due, uint64_t period, uint64_t w) { return (std::min(w, kTimerIdle - 1) - due) / period + 1; }
-inline uint64_t due_rearm(uint64_t due, uint64_t period, uint64_t k) {
-  uint64_t step = 0;
-  return (__builtin_mul_overflow(k, period, &step) || step >= kTimerIdle - due) ? kTimerIdle : due + step;
-}
-
-// After a launch to watermark w (any kernel that fires timers): every live slot due at or before w has fired on the device.
-// A one-shot is done and leaves the index (retire_oneshots retires it in the host table as before); a periodic slot moves on
-// by k = (w - due) / period + 1 periods into a later bucket.  on_fire(slot, ticks, next due) is told about each.  Each bucket
-// that begins at or before w is taken out whole and its entries are fired, dropped as stale, or (only in the bucket w falls
-// in) put back: O(due slots + that bucket), at most one pass over the table when every slot is due.
-template <class F>
-void due_fire(DueIndex& x, std::vector<HostTimer>& tm, uint64_t w, F&& on_fire) {
-  const uint64_t last = w >> DueIndex::kDueShift;
-  for (auto it = x.buckets.begin(); it != x.buckets.end() && it->first <= last;) {
-    std::vector<DueIndex::Entry> v;
-    v.swap(it->second.e);
-    it = x.buckets.erase(it);   // (re-arms land after w, so in this bucket at the earliest: never in front of `it`)
-    x.hot = nullptr;
-    x.n_entries -= v.size();
-    for (const DueIndex::Entry& e : v) {
-      if (x.stale(e)) continue;
-      if (e.due > w) { x.insert(e); continue; }
-      HostTimer& t = tm[e.slot];
-      if (t.oneshot) { x.drop(e.slot); on_fire(e.slot, (uint64_t)1, kTimerIdle); continue; }
-      const uint64_t k = due_ticks(t.next_due, t.period, w);
-      t.next_due = due_rearm(t.next_due, t.period, k);
-      on_fire(e.slot, k, t.next_due);
-      if (t.next_due == kTimerIdle) { x.drop(e.slot); continue; }
-      x.ver[e.slot]++;   // a new entry for the slot, still live
-      x.insert(DueIndex::Entry{t.next_due, e.slot, x.ver[e.slot]});
-    }
-  }
-}
-
-// CPBUS_CFG_DROP_MISSED_TICKS: the catch-up of a clock step to `now` in the due index, as timer_catchup_kernel does it on the
-// device.  Every live periodic slot due at d <= now whose next firing is also <= now moves to d + k * period, k = (now - d) /
-// period (below kTimerIdle: the kernel's candidates stop there too), under a new version; the slots that move are appended
-// to *moved.  Reads the buckets that begin at or before now: O(entries due by now).
-inline void due_catchup(DueIndex& x, std::vector<HostTimer>& tm, uint64_t now, std::vector<uint32_t>* moved) {
-  const uint64_t w = std::min(now, kTimerIdle - 1);
-  const size_t first = moved->size();
-  for (auto it = x.buckets.begin(); it != x.buckets.end() && it->first <= (w >> DueIndex::kDueShift); ++it)
-    for (const DueIndex::Entry& e : it->second.e) {
-      if (x.stale(e) || e.due > w) continue;
-      const HostTimer& t = tm[e.slot];
-      if (!t.oneshot && w - e.due >= t.period) moved->push_back(e.slot);
-    }
-  for (size_t i = first; i < moved->size(); i++) {   // (put may rebuild the buckets: not while they are walked)
-    HostTimer& t = tm[(*moved)[i]];
-    t.next_due += (w - t.next_due) / t.period * t.period;
-    x.put((*moved)[i], t.next_due);
-  }
-}
-
-// The subscription index of a CPBUS_CFG_SPARSE_RECORDS bus: who takes a broadcast record, by code and by exact case.
-//  * Per code: the count of subscribed mailboxes whose mask has the code's bit, and their list while the count is at most
-//    `keep`.  A code past `keep` drops its list and keeps only the count: planning ends at once on such a code (it reaches
-//    more mailboxes than the plan may), so an all-ones fleet holds 17 counts, not 17 N entries.  The list comes back by a scan
-//    of the table when the plan next meets the code with few enough subscribers.  Entries are removed lazily: an entry is
-//    live while its subscriber is subscribed and has the bit; `listed` (one word per subscriber) says which lists hold an
-//    entry for it, so a bit that comes back revives the old entry instead of adding a second one, and a list is compacted
-//    when its stale entries outnumber the live ones by 64.  Bound per code: 2 * min(count, keep) + 64 entries.
-//  * Per exact case {code, source}: the subscribers with that case.  Cases are set at subscription and never change, so an
-//    entry is live while its subscriber is subscribed; every subscriber's cases are kept (8 bytes each, the device table
-//    keeps 8 too) so that an unsubscribe can find its lists, and a list is compacted when half of it is stale (+ 64).
-//    A subscriber's cases sit in a segment of case_keys that a later occupant of its slot reuses when its cases fit, and
-//    otherwise replaces by a segment of CPBUS_MAX_PAIRS: with slot reuse, at most n + CPBUS_MAX_PAIRS keys per slot.
-//    Bound: 8 bytes per case subscribed so far, at most 8 * (n + CPBUS_MAX_PAIRS) per slot, and 2 * live + 64 entries per case.
-// Maintenance is O(mask bits + cases) per subscriber and call, amortized.  `slot` (one word per subscriber, all UINT32_MAX
-// between plans) maps a mailbox to its plan entry while a plan is built.  A CPBUS_CFG_SPARSE_TICKS bus without the records
-// flag plans due ticks alone: it sizes `slot` and nothing else.
-struct SubIndex {
-  size_t keep = 0;
-  uint32_t cnt[CPBUS_N_CODES] = {}, stale[CPBUS_N_CODES] = {};
-  bool ok[CPBUS_N_CODES] = {};                       // list[c] is kept
-  std::vector<uint32_t> list[CPBUS_N_CODES];
-  std::vector<uint32_t> listed;                      // per subscriber: bit c <=> list[c] holds an entry for it
-  struct Case { std::vector<uint32_t> subs; size_t stale = 0; };
-  std::unordered_map<uint64_t, Case> cases;          // (code << 32 | source) -> subscribers
-  std::vector<uint64_t> case_keys;                   // every subscriber's cases, in subscription order
-  std::vector<uint32_t> case_first;                  // per subscriber (allocated with the first case): its cases in case_keys
-  std::vector<uint8_t> case_n, case_cap;             // per subscriber: its cases, and the size of its segment
-  std::vector<uint32_t> slot;                        // per subscriber: its entry in the plan being built (UINT32_MAX: none)
-
-  static bool takes(const uint32_t* mask, const uint8_t* active, uint32_t l, uint32_t c) {
-    return active[l] && ((mask[l] >> c) & 1u);
-  }
-  void init(size_t n, size_t keep_n) {
-    keep = keep_n;
-    listed.assign(n, 0); slot.assign(n, UINT32_MAX);
-    for (uint32_t c = 0; c < CPBUS_N_CODES; c++) { cnt[c] = stale[c] = 0; ok[c] = true; list[c].clear(); }
-    cases.clear(); case_keys.clear(); case_first.clear(); case_n.clear(); case_cap.clear();
-  }
-  void drop(uint32_t c) {
-    for (uint32_t l : list[c]) listed[l] &= ~(1u << c);
-    std::vector<uint32_t>().swap(list[c]);
-    ok[c] = false; stale[c] = 0;
-  }
-  void compact(uint32_t c, const uint32_t* mask, const uint8_t* active) {
-    size_t o = 0;
-    for (uint32_t l : list[c]) {
-      if (takes(mask, active, l, c)) list[c][o++] = l;
-      else listed[l] &= ~(1u << c);
-    }
-    list[c].resize(o); stale[c] = 0;
-  }
-  void rebuild(uint32_t c, const uint32_t* mask, const uint8_t* active, uint32_t n) {
-    list[c].clear();
-    for (uint32_t l = 0; l < n; l++)
-      if (takes(mask, active, l, c)) { list[c].push_back(l); listed[l] |= 1u << c; }
-    ok[c] = true; stale[c] = 0;
-  }
-  // subscriber l has gained the codes in `bits` (it is subscribed and its mask has them)
-  void add_codes(uint32_t l, uint32_t bits) {
-    for (uint32_t c = 0; c < CPBUS_N_CODES; c++) {
-      if (!((bits >> c) & 1u)) continue;
-      cnt[c]++;
-      if (!ok[c]) continue;
-      if (cnt[c] > keep) { drop(c); continue; }
-      if ((listed[l] >> c) & 1u) stale[c]--;   // its old entry is live again
-      else { list[c].push_back(l); listed[l] |= 1u << c; }
-    }
-  }
-  // subscriber l has lost the codes in `bits` (mask / active already say so)
-  void remove_codes(uint32_t l, uint32_t bits, const uint32_t* mask, const uint8_t* active) {
-    for (uint32_t c = 0; c < CPBUS_N_CODES; c++) {
-      if (!((bits >> c) & 1u)) continue;
-      cnt[c]--;
-      if (!ok[c] || !((listed[l] >> c) & 1u)) continue;
-      if (++stale[c] > cnt[c] + 64) compact(c, mask, active);
-    }
-  }
-  // subscriber l (just subscribed) has the exact cases keys[0..n)
-  void add_cases(uint32_t l, const uint64_t* keys, uint32_t n) {
-    if (!n) return;
-    if (case_first.empty()) { case_first.assign(listed.size(), 0); case_n.assign(listed.size(), 0); case_cap.assign(listed.size(), 0); }
-    if (case_cap[l] < n) {   // a new segment: n keys for a slot's first subscriber with cases, the most a reused slot can need
-      const uint32_t cap = case_cap[l] ? (uint32_t)CPBUS_MAX_PAIRS : n;
-      case_first[l] = (uint32_t)case_keys.size(); case_cap[l] = (uint8_t)cap;
-      case_keys.resize(case_keys.size() + cap);
-    }
-    case_n[l] = (uint8_t)n;
-    for (uint32_t j = 0; j < n; j++) {
-      case_keys[case_first[l] + j] = keys[j];
-      Case& k = cases[keys[j]];
-      if (k.subs.empty() || k.subs.back() != l) k.subs.push_back(l);   // (a case listed twice: one entry)
-    }
-  }
-  // subscriber l has been unsubscribed (its cases stay recorded for release_cases)
-  void remove_cases(uint32_t l, const uint8_t* active) {
-    if (case_n.empty() || !case_n[l]) return;
-    const uint64_t* keys = case_keys.data() + case_first[l];
-    for (uint32_t j = 0; j < case_n[l]; j++) {
-      if (std::find(keys, keys + j, keys[j]) != keys + j) continue;
-      auto it = cases.find(keys[j]);
-      Case& k = it->second;
-      if (++k.stale * 2 <= k.subs.size() + 64) continue;
-      size_t o = 0;
-      for (uint32_t s : k.subs) if (active[s]) k.subs[o++] = s;
-      k.subs.resize(o); k.stale = 0;
-      if (!o) cases.erase(it);
-    }
-  }
-  // subscriber l, unsubscribed, is being released (cpbus_release_many): its cases go to *touched, and purge_released then
-  // takes the released subscribers' stale entries out of those lists, so that a later occupant of l with one of the same
-  // cases is listed once
-  void release_cases(uint32_t l, std::vector<uint64_t>* touched) {
-    if (case_n.empty() || !case_n[l]) return;
-    touched->insert(touched->end(), case_keys.begin() + case_first[l], case_keys.begin() + case_first[l] + case_n[l]);
-    case_n[l] = 0;
-  }
-  // once per call: each touched list is filtered once, O(the touched lists' lengths) whatever number of its subscribers
-  // the call released
-  void purge_released(std::vector<uint64_t>& touched, const uint8_t* released) {
-    std::sort(touched.begin(), touched.end());
-    touched.erase(std::unique(touched.begin(), touched.end()), touched.end());
-    for (uint64_t key : touched) {
-      auto it = cases.find(key);
-      if (it == cases.end()) continue;   // (compacted away)
-      Case& k = it->second;
-      size_t o = 0;
-      for (uint32_t s : k.subs) if (!released[s]) k.subs[o++] = s;
-      const size_t gone = k.subs.size() - o;   // stale entries: a released subscriber was unsubscribed
-      k.subs.resize(o); k.stale = k.stale > gone ? k.stale - gone : 0;
-      if (!o) cases.erase(it);
-    }
-  }
-};
-
-// The plan of a sparse record flush (cpbus_sparse_plan is this function over an index built from its arguments).  For each
-// record: a unicast record goes to its target if subscribed; a broadcast record to the live entries of its code's list and to
-// the subscribers with its exact case whose mask lacks the code (the fan-out's rule: mask bit or case).  A code with more
-// than max_m subscribers ends the planning at once, so a dense fleet costs O(records).  Each mailbox gets a plan entry the
-// first time it turns up (x.slot maps it there), so the planning also ends as soon as a (max_m + 1)-th one does; the
-// {mailbox, record} pairs are appended in record order.  The entries (at most max_m) are then sorted and the record indices
-// scattered to them in that order: O(records planned + max_m log max_m), each entry's indices ascending.  False: the flush
-// takes the full fan-out (more than max_m due slots or candidates, or more than max_d records planned).
-bool sparse_plan(SubIndex& x, const uint32_t* mask, const uint8_t* active, uint32_t n_subs, uint32_t base,
-                 const cpbus_event* rec, size_t n, const std::vector<uint32_t>& due, uint32_t K, size_t max_m, size_t max_d,
-                 std::vector<uint64_t>& pairs, std::vector<cpbus_plan_entry>& out, std::vector<uint32_t>& idx) {
-  out.clear(); idx.clear(); pairs.clear();
-  struct Reset {   // x.slot goes back to all UINT32_MAX whichever way the planning ends
-    SubIndex& x; std::vector<cpbus_plan_entry>& out;
-    ~Reset() { for (const cpbus_plan_entry& e : out) x.slot[e.local] = UINT32_MAX; }
-  } reset{x, out};
-  auto entry = [&](uint32_t l) -> cpbus_plan_entry* {   // nullptr: one mailbox too many
-    uint32_t& s = x.slot[l];
-    if (s == UINT32_MAX) {
-      if (out.size() == max_m) return nullptr;
-      s = (uint32_t)out.size();
-      out.push_back(cpbus_plan_entry{l, 0u, 0u, 0u});
-    }
-    return &out[s];
-  };
-  if (due.size() > max_m) return false;
-  for (uint32_t d : due) entry(d / K)->due_bits |= 1u << (d % K);
-  auto take = [&](uint32_t l, size_t i) -> bool {
-    cpbus_plan_entry* e = entry(l);
-    if (!e) return false;
-    e->count++;
-    pairs.push_back((uint64_t)l << 32 | i);
-    return true;
-  };
-  for (size_t i = 0; i < n; i++) {
-    const cpbus_event& r = rec[i];
-    if (r.target != CPBUS_TARGET_ALL) {
-      const uint32_t l = r.target - base;
-      if (r.target >= base && l < n_subs && active[l] && !take(l, i)) return false;
-    } else if (r.code < CPBUS_N_CODES) {
-      const uint32_t c = r.code;
-      if (x.cnt[c] > max_m) return false;
-      if (!x.ok[c]) x.rebuild(c, mask, active, n_subs);
-      for (uint32_t l : x.list[c])
-        if (SubIndex::takes(mask, active, l, c) && !take(l, i)) return false;
-      if (!x.cases.empty()) {
-        auto it = x.cases.find((uint64_t)c << 32 | r.source_id);
-        if (it != x.cases.end())
-          for (uint32_t l : it->second.subs)
-            if (active[l] && !((mask[l] >> c) & 1u) && !take(l, i)) return false;
-      }
-    }
-    if (pairs.size() > max_d) return false;
-  }
-  std::sort(out.begin(), out.end(), [](const cpbus_plan_entry& a, const cpbus_plan_entry& b) { return a.local < b.local; });
-  uint32_t first = 0;
-  for (uint32_t s = 0; s < out.size(); s++) {
-    x.slot[out[s].local] = s;
-    out[s].first = first; first += out[s].count; out[s].count = 0;
-  }
-  idx.resize(pairs.size());
-  for (uint64_t p : pairs) {
-    cpbus_plan_entry& e = out[x.slot[(uint32_t)(p >> 32)]];
-    idx[e.first + e.count++] = (uint32_t)p;
-  }
-  return true;
-}
-
-// The host front end: what the single bus (cpbus) and the group (cpbus_group) keep over their whole id space, and what the
-// rules below share — the clock window (max_window), timer arming and retirement, staging (stage_one), the publish loop
-// (publish_burst), the clock's advance (advance_clock), the debug ring and the publish counts.
-struct HostFront {
-  uint32_t B = 0, K = 0;                  // batch_cap, timers per subscriber
-  // clock and ordinals
-  uint64_t now = 0, last_watermark = 0, seq = 0;
-  size_t n_staged = 0;
-  std::vector<HostTimer> h_timers;        // N*K, allocated on first timer
-  std::vector<size_t> oneshot_idx;        // armed one-shot timers (index into h_timers)
-  uint32_t n_timers = 0;
-  uint64_t min_period = UINT64_MAX;       // conservative lower bound over armed periodic timers
-  bool drop_missed = false;               // CPBUS_CFG_DROP_MISSED_TICKS: a long clock step drops missed periodic ticks
-  // DebugEvents ring (events/bus.go:18-21, 24-54)
-  int dbg_head = -1, dbg_tail = 0;
-  cpbus_event dbg[10]{};
-  std::deque<DbgItem> dbg_pending;        // debug-ring entries not yet enqueued (events, or markers of device batches)
-  PairCounter pub_pairs;                  // host publishes by (code << 32 | source_id), Metric excluded (bus.go:130-132)
-  uint64_t publishes = 0, published_by_code[CPBUS_N_CODES] = {};   // host publishes and sends; by code (Metric excluded)
-};
-
-}  // namespace
-
-struct cpbus_stream;
-
-struct cpbus : HostFront {
-  cpbus_config cfg{};
-  int device = 0, sm_count = 132;
-  size_t smem_per_sm = 228 * 1024, smem_reserved = 1024;   // shared memory per SM, and what the system keeps per CTA
-  cudaStream_t stream = nullptr;
-  bool own_stream = false;
-  uint32_t N = 0, R = 0;
-  int store = CPBUS_STORE_V8;
-  bool lossless = false, use_digest = false;
-
-  // HBM-resident state (SoA, one entry per subscriber of this shard)
-  DeviceBuf<cpbus_event> d_ring;          // N * R records: each mailbox is one contiguous 32*R-byte ring
-  DeviceBuf<SubCtl> d_ctl;                // N control blocks: {tail, head, digest, mask}, one sector each
-  DeviceBuf<DevTimer> d_timers;           // N * K
-  DeviceBuf<DevStats> d_stats;
-  DeviceBuf<uint64_t> d_pow;              // P^0..: digest multiplier powers, TMA-loaded by every CTA
-  DeviceBuf<unsigned char> d_desc;        // per-launch batch descriptor (CTA 0 writes, the others read)
-  DeviceBuf<unsigned long long> d_desc_ready;
-  unsigned long long launch_seq = 0;
-  DeviceBuf<cpbus_event> d_batch_local;    // staged ingest: CTA 0's local copy of a peer batch
-  DeviceBuf<cpbus_event> d_admit_batch;    // lossless stream: local copy of a slot's undelivered records for the admission pass
-  static constexpr int kPrefetch = 3;      // fused ingest: later batches pulled over NVLink by earlier launches
-  DeviceBuf<cpbus_event> d_prefetch[kPrefetch];
-  const void* pf_ptr[kPrefetch] = {};      // which peer batch sits in d_prefetch[i] ...
-  size_t pf_n[kPrefetch] = {};
-  unsigned long long pf_seq[kPrefetch] = {};   // ... and which launch wrote it
-  int pf_next = 0;
-  std::vector<void*> shared_owned, shared_mapped;   // cpbus_shared_alloc / cpbus_shared_open
-  // stream mode (cpbus_stream_*): device-managed prefetch of later stream batches + sticky error word
-  DeviceBuf<unsigned long long> d_pf_state;   // [kStreamPrefetch]: which stream batch sits in d_prefetch[i]
-  DeviceBuf<cpbus_event> d_pf_buf;            // kStreamPrefetch x batch_cap records (one allocation)
-  MappedBuf<unsigned int> h_err;              // kErr* bits written by the fan-out kernel
-  uint32_t stream_spin_us = 0;                // bound of the in-kernel wait for a stream batch (0 = 2 s)
-  // follower launches (cpbus_stream_fanout_next): enqueued without the batch's shape, resolved lazily (follow_resolve)
-  static constexpr int kFollowMax = 8;        // outstanding at most; the next one resolves first
-  // kind: a follower, a lossless round (cpbus_stream_round_next: rec indexes h_round) or a cpbus_consume_all issued
-  // behind outstanding rounds (no record: it resets the room bound in order)
-  enum FollowKind { kFollower, kRound, kConsumeAll };
-  struct FollowPending { cpbus_stream* st; unsigned long long launch_seq; int rec; FollowKind kind; };
-  std::vector<FollowPending> follow_q;        // outstanding, in launch order
-  MappedBuf<RoundRec> h_round;                // kFollowMax records written by the round agree kernels
-  DeviceBuf<RoundDev> d_round;                // lossless rounds: the device copy of the room bound and clock, round scratch
-  MappedBuf<FollowRec> h_follow;              // kFollowMax records written by the lead CTAs
-  DeviceBuf<unsigned long long> d_follow_clock;   // 4 words: {watermark, launch ordinal} by launch parity
-  int follow_next = 0;
-  CudaEvent follow_done;
-  std::recursive_mutex follow_mu;              // the queue, when stats or drains on another thread resolve it
-  // accounting of device-published batches (cpbus_publish_device*, cpbus_stream_fanout): done by the kernel's lead CTA
-  DeviceBuf<DevPubAcct> d_acct;
-  // pinned staging for cpbus_stats / cpbus_debug_events / cpbus_publish_counts: the fields of a DevPubAcct before pair_key
-  PinnedBuf<unsigned char> h_acct;
-  DevPubAcct* host_acct() const { return reinterpret_cast<DevPubAcct*>(h_acct.get()); }
-  DeviceBuf<cpbus_event> d_drain;             // cpbus_drain_many staging (grown)
-  DeviceBuf<uint2> d_drain_idx;
-  // cpbus_drain_ready staging (records go to d_drain; grown): header + tile counter + tile status, ready list, ring
-  // slot of each run, and the header the gather kernel hands to the host
-  DeviceBuf<unsigned long long> d_ready_lb;
-  DeviceBuf<cpbus_ready> d_ready; DeviceBuf<uint32_t> d_ready_slot;
-  MappedBuf<unsigned long long> h_ready_hdr;
-  // cpbus_lagging / cpbus_blockers: look-back and summary words sized for every subscriber, the header the scans hand to the
-  // host, the blocker ids (lossless buses) and the lagging entries (grown)
-  DeviceBuf<unsigned long long> d_lag_lb;
-  MappedBuf<unsigned long long> h_lag_hdr;
-  MappedBuf<uint32_t> h_block;
-  MappedBuf<cpbus_lag> h_lag;
-  uint32_t subs_per_warp = 0;             // 0 = auto
-  uint32_t order_block = 0;               // mask order is built per block of this many consecutive subscribers (0 = one global order)
-  bool pdl = true;                        // programmatic dependent launch of consecutive fan-outs
-  CudaEvent launched;                     // recorded after the latest fan-out (step results are read on the copy stream)
-  int hints = -1;                         // -1 auto; bit0: control blocks / timer slots evict_last in L2
-  static constexpr int kFoldSlots = 8;
-  DeviceBuf<unsigned long long> d_fold;   // kFoldSlots x 4 words
-  CudaEvent fold_done[kFoldSlots];
-  uint32_t fold_next = 0;
-  static constexpr int kStage = 8;         // staging ring: the host may run several flushes ahead of the GPU
-  static constexpr int kDevSlots = 64, kDevEpoch = 16;
-  DeviceBuf<cpbus_event> d_stage;          // kDevSlots x batch_cap records: device side of the staging ring
-  CudaEvent epoch_done[kDevSlots / kDevEpoch];   // on the bus stream, after the last fan-out of each epoch of slots
-  uint32_t dev_slot = 0;
-  PinnedBuf<cpbus_event> h_batch[kStage];  // staging
-  CudaEvent h2d_done[kStage];              // on copy_stream: batch c has reached HBM
-  CudaStream copy_stream;                  // H2D of batch i+1 overlaps the fan-out of batch i
-  CudaStream result_stream;                // D2H of step results: must not queue in front of the next batch's H2D
-  // per-launch results written by the fan-out kernel itself (no extra kernel to read a step's result)
-  DeviceBuf<DevResultSlot> d_result;       // kResultRing x kResultSub slots
-  PinnedBuf<DevResultSlot> h_result;       // kFoldSlots tickets x kResultSub
-  CudaEvent result_done[8];
-  uint32_t result_next = 0;
-  PinnedBuf<DevStats> h_stats;
-  PinnedBuf<unsigned long long> h_fold;
-  int cur = 0;
-
-  // registry mirror (events/bus.go:13 `registry map[*Subscriber]bool`)
-  std::vector<uint32_t> h_mask;
-  std::vector<uint8_t> h_active;
-  std::vector<uint8_t> h_npairs;          // second-level filter: exact {code, source} cases per subscriber (empty until first use)
-  DeviceBuf<uint2> d_pairs;               // N x CPBUS_MAX_PAIRS, allocated by the first cpbus_subscribe_pairs (pair_tables)
-  uint32_t n_paired = 0;                  // active subscribers with a pair table
-  DeviceBuf<uint32_t> d_order;            // active subscribers sorted by code mask (ORDERED fan-out)
-  uint32_t n_order = 0, n_filtered = 0;   // n_filtered: active subscribers whose mask is not CPBUS_MASK_ALL
-  bool order_dirty = true;
-  uint32_t n_next = 0, n_active = 0;
-  // subscriber id reuse (cpbus_release_many / cpbus_subscribe_list): released mailboxes below n_next, and the same ids as
-  // a min-heap that cpbus_subscribe_list hands out lowest first; the device copy of the slot-reset list (grown)
-  std::vector<uint8_t> h_released;
-  std::vector<uint32_t> free_ids;
-  DeviceBuf<unsigned char> d_reset;
-
-  // lossless mode: a lower bound of the free slots of the FULLEST mailbox.  While a batch provably fits (bound >= what it
-  // can append to one mailbox) the admission pass and its host sync are skipped; the bound is refreshed exactly whenever
-  // the admission kernel does run, and reset by cpbus_consume_all.
-  uint64_t room_lb = 0;
-
-  // CPBUS_CFG_SPARSE_TICKS: the armed slots by due time, and the plan of a sparse flush (entries, record indices, and the
-  // {mailbox, record} pairs it is sorted from), staged in pinned memory as [entries | indices] and copied on the copy stream
-  // into a device buffer (both grown).  CPBUS_CFG_SPARSE_RECORDS: records are planned too, from the subscription
-  // index.
-  bool sparse = false, sparse_records = false;
-  DueIndex due;
-  std::vector<uint32_t> due_slots;
-  SubIndex rec_index;
-  std::vector<cpbus_plan_entry> plan;
-  std::vector<uint32_t> plan_idx;
-  std::vector<uint64_t> plan_pairs;
-  PinnedBuf<unsigned char> h_plan; DeviceBuf<unsigned char> d_plan;
-  CudaEvent plan_done;                    // on copy_stream: the plan (and the batch in front of it) has reached HBM
-  CudaEvent records_done;                 // on the bus stream: the record kernel is done with the plan
-  // CPBUS_CFG_DROP_MISSED_TICKS on a sparse bus: the slots a catch-up moves (host index), and their device copy (grown)
-  std::vector<uint32_t> catchup_slots;
-  DeviceBuf<uint32_t> d_catchup;
-  // the bulk membership calls (cpbus_unsubscribe_many, ...): device copy of the coalesced per-mailbox list (grown)
-  DeviceBuf<MemberOp> d_member;
-  // cpbus_timer_add_list: device copy of the armed slots' list (grown)
-  DeviceBuf<TimerArmOp> d_arm;
-  // acknowledged drains (cpbus_take_ready / cpbus_ack_many): the take cursor of every mailbox, allocated (zero) by the first
-  // take; the ack list ([entries | elements], pinned staging and its device copy, grown) and the statuses (grown)
-  DeviceBuf<unsigned long long> d_taken;
-  PinnedBuf<unsigned char> h_ack; DeviceBuf<unsigned char> d_ack;
-  MappedBuf<int> h_ack_status;
-
-  // intern table (Event.Source string <-> u32)
-  std::unordered_map<std::string, uint32_t> intern;
-  std::vector<std::string> sources;
-  size_t intern_bytes = 0;
-  // bounded region for payload strings (Metric "key|value"): recycled oldest-first
-  struct EphSlot { std::string s; uint32_t gen = 0; bool live = false; };
-  std::vector<EphSlot> eph;
-  std::unordered_map<std::string, uint32_t> eph_map;
-  uint32_t eph_next = 0;
-  uint64_t eph_live = 0, eph_recycled = 0;
-  std::vector<cpbus_stream*> streams;     // open streams (closed by cpbus_destroy if the caller did not)
-
-  cpbus_stats_t st{};
-  std::mutex mu;   // drain/stats from a second thread
-};
-
-// The group: one bus handle over the GPUs of a box (include/cpbus.h: cpbus_group_*).  Its host front end is the single
-// bus's, over the whole id space, and so are the rules that run on it (stage_one, publish_burst, advance_clock, the timer
-// table that sets the clock window, the debug ring and publish counts); only its flush differs (flush_staged of a group).
-// A flush becomes one RAW stream batch that every shard fans out in full: in lossless mode the group first runs the single
-// bus's admission (admit) on every shard and puts only the prefix every shard can take, with the single bus's partial
-// watermark.  (cpbus_stream_admit would hold a batch back until the ticks due by its watermark fit too, where a partial
-// cpbus_flush delivers the records and stalls on the ticks alone.)
-// Shard clocks: a shard's clock is its last launched watermark; a shard without timers is moved to the group clock with
-// cpbus_advance right before a timer is armed on it (no launch: it has no timer window), so every shard's `now + period`
-// is the single bus's.  A shard with timers already has the group clock there (the group has just flushed at `now`).
-struct cpbus_group : HostFront {
-  std::vector<cpbus*> shards;
-  std::vector<cpbus_stream*> streams;   // streams[0] owns the ring (shard 0), the others are attached
-  std::vector<uint32_t> first;          // global index (sub_id_base not applied) of each shard's subscriber 0; + a sentinel
-  uint32_t base = 0, N = 0;
-  bool lossless = false;
-  uint32_t n_next = 0, n_active = 0;
-  std::vector<uint32_t> free_ids;       // released global indices, a min-heap (cpbus_group_subscribe_list)
-  std::vector<cpbus_event> staged;      // B records
-  bool dev_counted = false;             // shard 0 has accounted a device batch (cpbus_group_publish_device)
-};
-
-// (defined with the stream below) the put of a batch into the next slot, from host or device memory, and a consumer's
-// launch of the next m records, with or without the accounting of a device-published batch
-extern "C" {
-static int stream_put(cpbus_stream* st, const cpbus_event* ev, size_t n, uint64_t now_ns, uint32_t flags, bool device_src);
-static int stream_fanout_prefix(cpbus_stream* st, size_t n, uint64_t now_ns, size_t m, bool account);
-}
-
-namespace {
-
-// counting sort of the active subscribers by their 17-bit code mask (stable: ids ascending inside a mask)
-int rebuild_order(cpbus* b);
-
-int dev_guard(cpbus* b) {
+int cpbus_host::dev_guard(cpbus* b) {
   CK(cudaSetDevice(b->device));
   return CPBUS_OK;
 }
 
 // How long the host waits for a stream's consumers or publisher (cpbus_stream_set_timeout; 0 = 2 s).
-std::chrono::microseconds stream_budget(const cpbus* b) {
+static std::chrono::microseconds stream_budget(const cpbus* b) {
   return std::chrono::microseconds(b->stream_spin_us ? b->stream_spin_us : 2000000u);
 }
 
 // The sticky stream error of this bus: a followed batch out of order (CPBUS_EORDER), otherwise a batch that never arrived or
 // did not match its header (CPBUS_ETIMEDOUT).
-int stream_error(const cpbus* b) {
+static int stream_error(const cpbus* b) {
   const unsigned int e = *(volatile const unsigned int*)b->h_err;
   return (e & kErrFollowOrder) ? CPBUS_EORDER : (e ? CPBUS_ETIMEDOUT : CPBUS_OK);
 }
 
-uint32_t mask_word(const cpbus* b, uint32_t local) {
+static uint32_t mask_word(const cpbus* b, uint32_t local) {
   uint32_t hint = 0;
   if (b->K && !b->h_timers.empty())
     for (uint32_t k = 0; k < b->K; k++)
@@ -640,7 +50,7 @@ uint32_t mask_word(const cpbus* b, uint32_t local) {
   return (b->h_mask[local] & CPBUS_MASK_ALL) | (hint << kTimerHintShift) | pair_bit | kActiveBit;
 }
 
-void dbg_ring_put(HostFront* f, const cpbus_event& e) {   // events/bus.go:24-31
+static void dbg_ring_put(HostFront* f, const cpbus_event& e) {   // events/bus.go:24-31
   f->dbg[(f->dbg_head + 1) % 10] = e;
   int old = f->dbg_head;
   f->dbg_head = (f->dbg_head + 1) % 10;
@@ -650,7 +60,7 @@ void dbg_ring_put(HostFront* f, const cpbus_event& e) {   // events/bus.go:24-31
 // While the broadcast events of a device-published batch are still unknown to the host (a marker is pending), later
 // enqueues queue up behind it so that the ring keeps the global publish order; cpbus_debug_events resolves them.  (A group
 // marks the device batches it launches, cpbus_group_publish_device, and resolves them against shard 0's accounting.)
-void dbg_enqueue(HostFront* f, const cpbus_event& e) {
+void cpbus_host::dbg_enqueue(HostFront* f, const cpbus_event& e) {
   if (f->dbg_pending.empty()) { dbg_ring_put(f, e); return; }
   f->dbg_pending.push_back(DbgItem{false, 0ull, e});
   if (f->dbg_pending.size() > (size_t)kAcctDbgRing) f->dbg_pending.pop_front();
@@ -658,7 +68,7 @@ void dbg_enqueue(HostFront* f, const cpbus_event& e) {
 
 // DebugEvents (events/bus.go:34-54): empties the ring oldest first, up to a NonEvent; returns how many it read (the first
 // cap of them go to out)
-size_t dbg_read(HostFront* f, cpbus_event* out, size_t cap) {
+size_t cpbus_host::dbg_read(HostFront* f, cpbus_event* out, size_t cap) {
   size_t k = 0;
   for (;;) {
     if (f->dbg_head == -1) break;
@@ -672,50 +82,13 @@ size_t dbg_read(HostFront* f, cpbus_event* out, size_t cap) {
   return k;
 }
 
-void dbg_mark_device_batch(HostFront* f, unsigned long long launch) {
+void cpbus_host::dbg_mark_device_batch(HostFront* f, unsigned long long launch) {
   f->dbg_pending.push_back(DbgItem{true, launch, cpbus_event{}});
   if (f->dbg_pending.size() > (size_t)kAcctDbgRing) f->dbg_pending.pop_front();
 }
 
-// The mask order of the ORDERED build, host-only (exported as cpbus_mask_order so that it can be tested without a GPU).
-// Equal masks become neighbours, so a warp's consecutive mailboxes share one filter pass.
-//  * Blocks.  A GLOBAL order scatters the mailboxes that are written at the same time over the whole ring area (1,048,576
-//    rings = 32 GiB = 16,384 2-MiB pages, all live at once); ordering block by block of consecutive subscribers keeps the
-//    concurrently written rings within a few hundred pages, at the price of shorter runs.  Policy (block == 0): one global
-//    order up to 16 GiB of rings, blocks of 8 GiB beyond.
-//  * Heavy first.  Within a block a second, stable pass by the number of codes in the mask, most first: CTAs are dispatched
-//    in block order, so the mailboxes that take the most records start first and the launch's last wave is made of the light
-//    ones (shorter tail before the next launch may start); equal masks stay neighbours.
-static void mask_order(const uint32_t* masks, const uint8_t* active, uint32_t n, uint32_t ring_cap, uint32_t block, bool heavy_first,
-                       std::vector<uint32_t>& order) {
-  order.clear();
-  order.reserve(n);
-  const uint64_t ring_bytes = (uint64_t)ring_cap * sizeof(cpbus_event);
-  uint32_t blk = block;
-  if (!blk) blk = (uint64_t)n * ring_bytes <= (16ull << 30) ? std::max(1u, n) : (uint32_t)std::max<uint64_t>(4096, (8ull << 30) / ring_bytes);
-  if (block == 0xFFFFFFFFu) blk = std::max(1u, n);   // one global order (A/B)
-  std::vector<uint32_t> count((size_t)CPBUS_MASK_ALL + 2), tmp;
-  for (uint32_t lo = 0; lo < n; lo += blk) {
-    const uint32_t hi = (uint32_t)std::min<uint64_t>((uint64_t)lo + blk, n);
-    std::fill(count.begin(), count.end(), 0u);
-    for (uint32_t i = lo; i < hi; i++) if (!active || active[i]) count[(masks[i] & CPBUS_MASK_ALL) + 1]++;
-    for (size_t k = 1; k < count.size(); k++) count[k] += count[k - 1];
-    const size_t base = order.size();
-    order.resize(base + count.back());
-    for (uint32_t i = lo; i < hi; i++) if (!active || active[i]) order[base + count[masks[i] & CPBUS_MASK_ALL]++] = i;
-    if (heavy_first) {
-      const size_t nb = order.size() - base;
-      uint32_t pc_count[34] = {};
-      for (size_t k = 0; k < nb; k++) pc_count[32 - __builtin_popcount(masks[order[base + k]] & CPBUS_MASK_ALL) + 1]++;
-      for (int k = 1; k < 34; k++) pc_count[k] += pc_count[k - 1];
-      tmp.resize(nb);
-      for (size_t k = 0; k < nb; k++) tmp[pc_count[32 - __builtin_popcount(masks[order[base + k]] & CPBUS_MASK_ALL)]++] = order[base + k];
-      std::copy(tmp.begin(), tmp.end(), order.begin() + base);
-    }
-  }
-}
-
-int rebuild_order(cpbus* b) {
+// counting sort of the active subscribers by their 17-bit code mask (stable: ids ascending inside a mask)
+static int rebuild_order(cpbus* b) {
   std::vector<uint32_t> order;
   static_assert(sizeof(b->h_active[0]) == 1, "h_active is a byte vector");
   mask_order(b->h_mask.data(), reinterpret_cast<const uint8_t*>(b->h_active.data()), b->n_next, b->R, b->order_block, /*heavy_first=*/true, order);
@@ -733,7 +106,7 @@ constexpr int kFanoutMaxSmem = 200 * 1024;
 enum { kLaunchPlain = 0, kLaunchFollow = 1, kLaunchRound = 2 };
 
 template <int STORE, bool TIMERS, bool DIGEST, bool ORDERED, bool PAIRS = false>
-int launch_fanout_t(cpbus* b, const FanoutParams& p, uint32_t grid, size_t smem, int kind) {
+static int launch_fanout_t(cpbus* b, const FanoutParams& p, uint32_t grid, size_t smem, int kind) {
   static bool attr_done[3][64] = {};   // per instantiation AND per device: function attributes are per-device state
   void (*kernel)(FanoutParams) = kind == kLaunchRound  ? fanout_round_kernel<STORE, TIMERS, DIGEST, ORDERED, PAIRS>
                                : kind == kLaunchFollow ? fanout_follow_kernel<STORE, TIMERS, DIGEST, ORDERED, PAIRS>
@@ -755,15 +128,13 @@ int launch_fanout_t(cpbus* b, const FanoutParams& p, uint32_t grid, size_t smem,
   return CPBUS_OK;
 }
 
-uint64_t max_window(const HostFront* f);
-
 // Lossless rounds wait in the kernel: for the publisher's header (decide) and for the other shards' offers (agree).  With
 // CUDA's lazy module loading, the first launch of a kernel loads it, and a load may wait for the kernels already running on
 // the device — such as a round waiting for a batch that this very thread has yet to put, or for an offer that another shard
 // of this thread has yet to queue.  So every kernel a lossless bus may launch while its rounds wait is loaded up front, once
 // per device, when the bus is created.
 template <int ST>
-int preload_round_fanouts() {
+static int preload_round_fanouts() {
   void (*ks[])(FanoutParams) = {
       fanout_round_kernel<ST, false, false, false>, fanout_round_kernel<ST, false, true, false>,
       fanout_round_kernel<ST, true, false, false>, fanout_round_kernel<ST, true, true, false>,
@@ -773,7 +144,7 @@ int preload_round_fanouts() {
   return CPBUS_OK;
 }
 
-int preload_round_kernels(cpbus* b) {
+static int preload_round_kernels(cpbus* b) {
   static bool done[64] = {};
   static std::mutex mu;
   std::lock_guard<std::mutex> g(mu);
@@ -815,17 +186,17 @@ struct LaunchOpts {
 };
 
 // The step-result sub-slots of launch ordinal `seq`: a launch adds into its own and zeroes its successor's.
-DevResultSlot* result_slot(const cpbus* b, unsigned long long seq) {
+static DevResultSlot* result_slot(const cpbus* b, unsigned long long seq) {
   return b->d_result + (size_t)(seq % kResultRing) * kResultSub;
 }
 
 // A launch (or a flush with nothing to launch) has reached watermark w: the clock, and the due index, follow it.
-void launched_to(cpbus* b, uint64_t w) {
+static void launched_to(cpbus* b, uint64_t w) {
   b->last_watermark = w;
   if (b->sparse) due_fire(b->due, b->h_timers, w, [](uint32_t, uint64_t, uint64_t) {});
 }
 
-int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, const LaunchOpts& o = {}) {
+static int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, const LaunchOpts& o = {}) {
   const StreamArgs* sa = o.stream;
   if (b->n_next == 0 && !sa) return CPBUS_OK;
   if (n == 0 && b->n_timers == 0 && !sa) return CPBUS_OK;   // (a stream batch is always consumed: its slot must be acknowledged)
@@ -940,7 +311,7 @@ int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, co
 }
 
 // The host timer table, allocated by the first timer, and with it the due index.
-void timer_table(cpbus* b) {
+static void timer_table(cpbus* b) {
   b->h_timers.resize((size_t)b->N * b->K);
   if (b->sparse) b->due.init(b->h_timers.size());
 }
@@ -950,7 +321,7 @@ void timer_table(cpbus* b) {
 // host-side check once per epoch of kDevEpoch slots (almost always already satisfied).  stage_batch takes the next slot
 // (*d_dst) and puts the n records of the current pinned buffer on their way into it; retire_slot follows the launch that
 // reads the slot.
-int stage_batch(cpbus* b, uint32_t n, cpbus_event** d_dst) {
+static int stage_batch(cpbus* b, uint32_t n, cpbus_event** d_dst) {
   const uint32_t slot = b->dev_slot;
   *d_dst = b->d_stage + (size_t)slot * b->B;
   if (slot % cpbus::kDevEpoch == 0) CK(cudaEventSynchronize(b->epoch_done[slot / cpbus::kDevEpoch]));   // last round's users of this epoch are done
@@ -961,7 +332,7 @@ int stage_batch(cpbus* b, uint32_t n, cpbus_event** d_dst) {
   return CPBUS_OK;
 }
 
-int retire_slot(cpbus* b) {
+static int retire_slot(cpbus* b) {
   const uint32_t slot = b->dev_slot;
   if (slot % cpbus::kDevEpoch == cpbus::kDevEpoch - 1) CK(cudaEventRecord(b->epoch_done[slot / cpbus::kDevEpoch], b->stream));
   b->dev_slot = (slot + 1) % cpbus::kDevSlots;
@@ -970,7 +341,7 @@ int retire_slot(cpbus* b) {
 
 // Give the 8-16 KiB copy that `copied` marks up to 30 us to land.  If it has, the bus stream needs no wait node, consecutive
 // fan-outs stay adjacent in the stream and the next launch's prologue overlaps this one's tail (programmatic dependent launch).
-int await_copy(cpbus* b, cudaEvent_t copied) {
+static int await_copy(cpbus* b, cudaEvent_t copied) {
   const auto t_spin = std::chrono::steady_clock::now();
   do {
     const cudaError_t q = cudaEventQuery(copied);
@@ -982,7 +353,7 @@ int await_copy(cpbus* b, cudaEvent_t copied) {
 }
 
 // The staged batch has been launched whole: staging moves on to the next pinned buffer.
-int next_buffer(cpbus* b) {
+static int next_buffer(cpbus* b) {
   b->cur = (b->cur + 1) % cpbus::kStage;
   CK(cudaEventSynchronize(b->h2d_done[b->cur]));   // the pinned buffer we are about to overwrite has left the host
   return CPBUS_OK;
@@ -992,12 +363,12 @@ int next_buffer(cpbus* b) {
 // takes the full fan-out.  Measured on an H100 (DESIGN.md §4.6, §4.7): at 1,048,576 subscribers a dedicated tick kernel won
 // at N/1,024 due slots and lost at N/128; the record kernel on timer-only plans costs the same as that kernel at N/1,024
 // (the rows re-measured in §4.6), so the cap stays.
-size_t sparse_max(const cpbus* b) { return std::max<size_t>(32, b->n_next / 1024); }
-size_t sparse_max_deliveries(const cpbus* b) { return std::max<size_t>(1024, b->n_next / 256); }
+static size_t sparse_max(const cpbus* b) { return std::max<size_t>(32, b->n_next / 1024); }
+static size_t sparse_max_deliveries(const cpbus* b) { return std::max<size_t>(1024, b->n_next / 256); }
 
 // The pinned plan buffer is free for `bytes`: the previous plan has left it, or both buffers are regrown (behind every
 // kernel that may still read the old device buffer).
-int plan_room(cpbus* b, size_t bytes) {
+static int plan_room(cpbus* b, size_t bytes) {
   if (bytes <= b->d_plan.size() && bytes <= b->h_plan.size()) { CK(cudaEventSynchronize(b->plan_done)); return CPBUS_OK; }
   CK(cudaStreamSynchronize(b->stream)); CK(cudaStreamSynchronize(b->copy_stream));
   CK(b->d_plan.grow(bytes, 64 << 10));
@@ -1011,7 +382,7 @@ int plan_room(cpbus* b, size_t bytes) {
 // spin waits for both, and the staging buffer moves on.  A flush of due ticks alone has no batch: the bus stream waits for
 // the plan.  A plan without a mailbox launches nothing and copies nothing.  The clock and the due index follow, as after a
 // fan-out.
-int launch_sparse(cpbus* b, uint64_t w) {
+static int launch_sparse(cpbus* b, uint64_t w) {
   const size_t n_list = b->plan.size(), n_idx = b->plan_idx.size();
   const uint32_t n = (uint32_t)b->n_staged;
   if (n_list) {
@@ -1051,7 +422,7 @@ int launch_sparse(cpbus* b, uint64_t w) {
 // by w and the staged records are planned, and a plan within the caps launches the record kernel over its mailboxes (none:
 // no launch).  False: the full fan-out follows, with admission and the partial prefix as before — past a cap, or (lossless)
 // when the room bound cannot prove that the most one mailbox takes, records and ticks, fits.
-bool sparse_flush(cpbus* b, uint64_t w, int* rc) {
+static bool sparse_flush(cpbus* b, uint64_t w, int* rc) {
   *rc = CPBUS_OK;
   const bool ticks = b->due.min_due() <= w;
   if (!ticks && !b->n_staged) { b->last_watermark = w; return true; }
@@ -1083,7 +454,7 @@ bool sparse_flush(cpbus* b, uint64_t w, int* rc) {
 
 // lossless admission (reference: the sender blocks on a full channel, events/subscriber.go:30-32)
 // Fast path: true when n records with watermark w provably fit (or nothing has to be admitted) — no kernel, no sync.
-bool admit_fits(cpbus* b, uint32_t n, uint64_t w) {
+bool cpbus_host::admit_fits(cpbus* b, uint32_t n, uint64_t w) {
   if (!b->lossless || b->n_next == 0) return true;
   const uint64_t need = admit_need(n, w, b->last_watermark, b->min_period, b->K, b->n_timers && b->K);
   if (b->room_lb >= need) { b->room_lb -= need; b->st.admit_skipped++; return true; }
@@ -1091,7 +462,7 @@ bool admit_fits(cpbus* b, uint32_t n, uint64_t w) {
 }
 
 // The admission pass (after admit_fits said no): one kernel over every mailbox of the shard, then a host sync.
-int admit_pass(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, bool* ok, uint32_t* prefix) {
+int cpbus_host::admit_pass(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, bool* ok, uint32_t* prefix) {
   CK(cudaMemsetAsync(&b->d_stats->admit_overflow, 0, 4 * sizeof(unsigned long long), b->stream));   // overflow, overwritten, max_used, deficit
   const uint32_t threads = 256, grid = (b->n_next + threads - 1) / threads;
   admit_kernel<<<grid, threads, 0, b->stream>>>(d_src, n, w, b->d_ctl, b->d_timers, b->n_next, b->R, b->K,
@@ -1111,7 +482,7 @@ int admit_pass(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, bool*
   return CPBUS_OK;
 }
 
-int admit(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, bool* ok, uint32_t* prefix = nullptr) {
+static int admit(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, bool* ok, uint32_t* prefix = nullptr) {
   *ok = true;
   if (prefix) *prefix = n;
   if (admit_fits(b, n, w)) return CPBUS_OK;
@@ -1120,7 +491,7 @@ int admit(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_t w, bool* ok, 
 
 // host mirror of one-shot timers that have fired on the device (events/timer.go:19-33):
 // a one-shot whose due time is <= the last launched watermark has disarmed itself.
-void retire_oneshots(HostFront* f, uint64_t w) {
+void cpbus_host::retire_oneshots(HostFront* f, uint64_t w) {
   size_t keep = 0;
   for (size_t i = 0; i < f->oneshot_idx.size(); i++) {
     HostTimer& t = f->h_timers[f->oneshot_idx[i]];
@@ -1133,7 +504,7 @@ void retire_oneshots(HostFront* f, uint64_t w) {
 
 // Arm table slot `slot` (subscriber * K + k) at the clock: periodic timers bound the clock window, one-shots wait for
 // retirement.
-HostTimer& timer_arm(HostFront* f, size_t slot, uint64_t period, uint32_t source_id, bool oneshot) {
+HostTimer& cpbus_host::timer_arm(HostFront* f, size_t slot, uint64_t period, uint32_t source_id, bool oneshot) {
   HostTimer& t = f->h_timers[slot];
   t.active = true; t.oneshot = oneshot; t.period = period; t.next_due = due_after(f->now, period); t.source_id = source_id;
   f->n_timers++;
@@ -1144,7 +515,7 @@ HostTimer& timer_arm(HostFront* f, size_t slot, uint64_t period, uint32_t source
 
 // Disarm table slot `slot` if it is armed.  A cancel (reset_bound) lets the window's bound go with the last timer; an
 // unsubscribe keeps the stale bound, which narrows the window (and so the launch grid) until a cancel or a retirement.
-void timer_disarm(HostFront* f, size_t slot, bool reset_bound) {
+void cpbus_host::timer_disarm(HostFront* f, size_t slot, bool reset_bound) {
   HostTimer& t = f->h_timers[slot];
   if (t.active) { t.active = false; f->n_timers--; }
   if (reset_bound && f->n_timers == 0) f->min_period = UINT64_MAX;
@@ -1152,13 +523,13 @@ void timer_disarm(HostFront* f, size_t slot, bool reset_bound) {
 
 // True when a flush to watermark w launches nothing: no record is staged, and no timer is armed (the watermark then
 // follows the clock) or the clock has not moved since the last launch.
-bool flush_idle(HostFront* f, uint64_t w) {
+bool cpbus_host::flush_idle(HostFront* f, uint64_t w) {
   if (f->n_staged) return false;
   if (f->n_timers == 0) { f->last_watermark = std::max(f->last_watermark, w); return true; }
   return w == f->last_watermark;
 }
 
-int flush_staged(cpbus* b, uint64_t w) {
+int cpbus_host::flush_staged(cpbus* b, uint64_t w) {
   if (flush_idle(b, w)) return CPBUS_OK;
   int rc;
   if (b->sparse && (!b->n_staged || b->sparse_records) && sparse_flush(b, w, &rc)) return rc;
@@ -1188,115 +559,18 @@ int flush_staged(cpbus* b, uint64_t w) {
   return next_buffer(b);
 }
 
-// One launch of the single bus: the same early returns as launch_fanout, otherwise one stream batch on every shard.
-// `device`: ev is a batch in device memory (cpbus_group_publish_device), which shard 0's put stream copies into the slot.
-// The group's host records hold every record it staged itself; a device batch is accounted where the single bus accounts
-// it, by the kernel — by shard 0's launch alone, marked in the group's debug ring in call order.
-int group_launch(cpbus_group* g, const cpbus_event* ev, uint32_t n, uint64_t w, bool device = false) {
-  if (g->n_next == 0) return CPBUS_OK;
-  if (n == 0 && g->n_timers == 0) return CPBUS_OK;
-  int rc = stream_put(g->streams[0], ev, n, w, CPBUS_PUT_RAW, device);
-  if (rc) return rc;
-  for (size_t k = 0; k < g->streams.size(); k++)   // the whole batch: already admitted on every shard, so it completes in one launch
-    if ((rc = stream_fanout_prefix(g->streams[k], n, w, n, device && k == 0))) return rc;
-  g->last_watermark = w;
-  if (device && n) { dbg_mark_device_batch(g, g->shards[0]->launch_seq); g->dev_counted = true; }
-  return CPBUS_OK;
-}
+cpbus_event* cpbus_host::staging(cpbus* b) { return b->h_batch[b->cur]; }
 
-// Lossless admission of n records at src (the staged records, or a device batch) on every shard (admit), the single bus's
-// verdict being the conjunction and its prefix the minimum.  The records reach a shard's device only when its room bound
-// cannot prove the fit.
-int group_admit(cpbus_group* g, const cpbus_event* src, uint32_t n, uint64_t w, bool* ok, uint32_t* m) {
-  *ok = true; *m = n;
-  for (cpbus* s : g->shards) {
-    if (admit_fits(s, n, w)) continue;
-    int rc = dev_guard(s); if (rc) return rc;
-    if (n) CK(cudaMemcpyAsync(s->d_admit_batch, src, (size_t)n * sizeof(cpbus_event), cudaMemcpyDefault, s->stream));
-    bool ok_s = true;
-    uint32_t m_s = n;
-    if ((rc = admit_pass(s, s->d_admit_batch, n, w, &ok_s, &m_s))) return rc;
-    if (!ok_s) { *ok = false; *m = std::min(*m, m_s); }
-  }
-  return CPBUS_OK;
-}
-
-// The group's flush: the single bus's outcome (the whole staged batch, or in lossless mode the prefix every shard can take
-// with the partial watermark), as one stream batch
-int flush_staged(cpbus_group* g, uint64_t w) {
-  if (flush_idle(g, w)) return CPBUS_OK;
-  const uint32_t n = (uint32_t)g->n_staged;
-  bool ok = true;
-  uint32_t m = n;
-  int rc;
-  if (g->lossless && (rc = group_admit(g, g->staged.data(), n, w, &ok, &m))) return rc;
-  if (!ok) {
-    if (m == 0) return CPBUS_EAGAIN;
-    if ((rc = group_launch(g, g->staged.data(), m, g->staged[m - 1].ts_ns))) return rc;
-    std::copy(g->staged.begin() + m, g->staged.begin() + n, g->staged.begin());
-    g->n_staged = n - m;
-    for (cpbus* s : g->shards) { s->room_lb = 0; s->st.admit_partial++; }
-    return CPBUS_EAGAIN;
-  }
-  if ((rc = group_launch(g, g->staged.data(), n, w))) return rc;
-  g->n_staged = 0;
-  return CPBUS_OK;
-}
-
-// where the next staged record goes
-cpbus_event* staging(cpbus* b) { return b->h_batch[b->cur]; }
-cpbus_event* staging(cpbus_group* g) { return g->staged.data(); }
-
-uint64_t max_window(const HostFront* f) {
+uint64_t cpbus_host::max_window(const HostFront* f) {
   if (!f->K || f->n_timers == 0 || f->min_period == UINT64_MAX) return UINT64_MAX;
   const uint64_t J = 32u / f->K;
   return f->min_period > UINT64_MAX / J ? UINT64_MAX : f->min_period * J;
 }
 
-// stage_one, publish_burst and advance_clock run on the single bus and on the group alike (Owner = cpbus or cpbus_group):
-// one body each, with the owner's own flush.
-template <class Owner>
-int stage_one(Owner* o, uint32_t code, uint32_t source_id, uint32_t target, uint32_t flags) {
-  if (o->n_staged == o->B) { int rc = flush_staged(o, o->now); if (rc) return rc; }
-  cpbus_event& e = staging(o)[o->n_staged++];
-  e.seq = o->seq++; e.ts_ns = o->now; e.code = code; e.source_id = source_id; e.target = target; e.flags = flags;
-  return CPBUS_OK;
-}
-
-// Publish a burst (events/bus.go:126-139): nothing of a burst with an invalid code is published.
-template <class Owner>
-int publish_burst(Owner* o, const cpbus_event* ev, size_t n) {
-  for (size_t i = 0; i < n; i++) {   // counter slots of the whole burst: requested up front, touched in the loop below
-    if (ev[i].code < CPBUS_N_CODES && ev[i].code != CPBUS_METRIC) o->pub_pairs.prefetch(((uint64_t)ev[i].code << 32) | ev[i].source_id);
-  }
-  // The debug ring holds 10 entries (events/bus.go:24-31): of a burst only the last 10 published can ever be seen, so only
-  // those are enqueued — including when the call stops early (CPBUS_EAGAIN from an automatic flush in lossless mode).
-  auto dbg_tail = [&](size_t published) {
-    for (size_t j = published > 10 ? published - 10 : 0; j < published; j++) {
-      cpbus_event e{};
-      e.seq = o->seq - (published - j); e.ts_ns = o->now; e.code = ev[j].code; e.source_id = ev[j].source_id; e.target = CPBUS_TARGET_ALL;
-      dbg_enqueue(o, e);
-    }
-  };
-  for (size_t i = 0; i < n; i++) if (ev[i].code >= CPBUS_N_CODES) return CPBUS_EINVAL;
-  for (size_t i = 0; i < n; i++) {
-    const uint32_t code = ev[i].code;
-    const int rc = stage_one(o, code, ev[i].source_id, CPBUS_TARGET_ALL, 0);
-    if (rc) { dbg_tail(i); return rc; }
-    if (code != CPBUS_METRIC) {                                  // events/bus.go:130-132
-      o->published_by_code[code]++;
-      o->pub_pairs.add(((uint64_t)code << 32) | ev[i].source_id, 1);
-    }
-    o->publishes++;
-  }
-  dbg_tail(n);                                                   // events/bus.go:139
-  return CPBUS_OK;
-}
-
 // CPBUS_CFG_DROP_MISSED_TICKS: the catch-up of a clock step to `now`, after a flush to the old clock.  timer_catchup_kernel
 // runs on the bus stream behind every earlier launch: over the whole slot table of a dense bus, and over exactly the slots
 // that the due index moved (due_catchup) on a sparse one, where no slot moving means no launch.
-int catch_up(cpbus* b, uint64_t now) {
+int cpbus_host::catch_up(cpbus* b, uint64_t now) {
   if (!b->K || b->n_timers == 0 || b->h_timers.empty() || b->n_next == 0) return CPBUS_OK;
   const uint32_t* list = nullptr;
   size_t n = (size_t)b->n_next * b->K;
@@ -1319,55 +593,23 @@ int catch_up(cpbus* b, uint64_t now) {
   return CPBUS_OK;
 }
 
-// The group: the same catch-up on every shard that has timers (its shards are dense buses).
-int catch_up(cpbus_group* g, uint64_t now) {
-  for (cpbus* s : g->shards) {
-    if (!s->K || s->n_timers == 0) continue;
-    int rc = dev_guard(s);
-    if (rc || (rc = catch_up(s, now))) return rc;
-  }
-  return CPBUS_OK;
-}
-
-// Move the clock to now_ns.  The kernel looks at <= 32/K candidate firings per timer slot per launch: every flush window is
-// kept within that many periods of the fastest periodic timer (for a group, a stream batch never steps past a shard's window).
-// CPBUS_CFG_DROP_MISSED_TICKS: only a step longer than the shortest period can hold two firings of one timer.  On such a
-// step, what is due by the old clock is delivered on its own first (the previous step's window split keeps that flush within
-// the window; CPBUS_EAGAIN leaves the clock where it was), then every periodic timer with missed firings moves to its last
-// one, so the window split below launches at most one firing per slot.
-template <class Owner>
-int advance_clock(Owner* o, uint64_t now_ns) {
-  if (now_ns < o->now) return CPBUS_EORDER;
-  if (now_ns == o->now) return CPBUS_OK;
-  if (o->drop_missed && o->n_timers && o->min_period != UINT64_MAX && now_ns - o->now > o->min_period) {
-    int rc = flush_staged(o, o->now);
-    if (rc || (rc = catch_up(o, now_ns))) return rc;
-  }
-  const uint64_t win = max_window(o);
-  while (win != UINT64_MAX && now_ns - o->last_watermark > win) {
-    o->now = o->last_watermark + win;
-    const int rc = flush_staged(o, o->now); if (rc) return rc;
-  }
-  o->now = now_ns;
-  return CPBUS_OK;
-}
 
 // Whether ids [first, first + n) lie in [base, base + n_next), the ids subscribed so far; *index = first - base.
-bool id_range(uint32_t base, uint32_t n_next, uint32_t first, uint64_t n, uint32_t* index) {
+bool cpbus_host::id_range(uint32_t base, uint32_t n_next, uint32_t first, uint64_t n, uint32_t* index) {
   *index = first - base;
   return first >= base && (uint64_t)*index + n <= n_next;
 }
 
 // Whether sub_id names a mailbox of this bus that was handed out and not released since; *l = its index.  A released id
 // is refused as one never handed out; range calls keep n_next as their bound and see a released mailbox as empty.
-bool sub_index(const cpbus* b, uint32_t sub_id, uint32_t* l) {
+static bool sub_index(const cpbus* b, uint32_t sub_id, uint32_t* l) {
   return id_range(b->cfg.sub_id_base, b->n_next, sub_id, 1, l) && !b->h_released[*l];
 }
 
 // cpbus_publish_counts: the host publish counts of f and n_dev device-counted pairs (key + 1 per slot, 0 = empty), merged by
 // {code, source} and sorted; *n = how many pairs there are, the first cap of them go to out.
-void pair_counts(const HostFront* f, const unsigned long long* dev_keys, const unsigned long long* dev_cnts, size_t n_dev,
-                 cpbus_pair_count* out, size_t cap, size_t* n) {
+void cpbus_host::pair_counts(const HostFront* f, const unsigned long long* dev_keys, const unsigned long long* dev_cnts, size_t n_dev,
+                             cpbus_pair_count* out, size_t cap, size_t* n) {
   std::unordered_map<uint64_t, uint64_t> merged;
   for (size_t i = 0; i < f->pub_pairs.keys.size(); i++) if (f->pub_pairs.keys[i]) merged[f->pub_pairs.keys[i] - 1] += f->pub_pairs.cnts[i];
   for (size_t i = 0; i < n_dev; i++) if (dev_keys[i]) merged[dev_keys[i] - 1] += dev_cnts[i];
@@ -1377,9 +619,7 @@ void pair_counts(const HostFront* f, const unsigned long long* dev_keys, const u
   *n = v.size();
 }
 
-bool is_pow2(uint32_t x) { return x && !(x & (x - 1)); }
-
-}  // namespace
+static bool is_pow2(uint32_t x) { return x && !(x & (x - 1)); }
 
 // outstanding followers and rounds that hold one of the kFollowMax records
 static int follow_records(const cpbus* b) {
@@ -1388,187 +628,16 @@ static int follow_records(const cpbus* b) {
   return n;
 }
 
-extern "C" {
 static int follow_resolve(cpbus* b);
 // The opening of the entry points that read or change host-side bus state: this bus's device, then the outstanding
 // followers and rounds folded in (DESIGN.md §8, lazy resolution).
-static int enter(cpbus* b) {
+int cpbus_host::enter(cpbus* b) {
   const int rc = dev_guard(b);
   return rc ? rc : follow_resolve(b);
 }
-// Nothing may unwind through the C boundary (cgo, ctypes): every status-returning entry point is a function-try-block.
-#define CPBUS_CATCH                                                                                   \
-  catch (const std::bad_alloc&) { return CPBUS_ENOMEM; }                                              \
-  catch (...) { snprintf(g_cuda_err, sizeof(g_cuda_err), "unexpected C++ exception"); return CPBUS_ECUDA; }
-
-uint32_t cpbus_abi_version(void) { return 2; }
-static int split_plan(const uint64_t* ts, size_t n, uint32_t batch_cap, uint64_t now, uint64_t watermark, uint64_t window,
-                      std::vector<size_t>& end, std::vector<uint64_t>& wm);
-int cpbus_split_plan(const uint64_t* ts, size_t n, uint32_t batch_cap, uint64_t now_ns, uint64_t watermark_ns, uint64_t window_ns,
-                     size_t* ends, uint64_t* watermarks, size_t cap, size_t* n_slices) try {
-  if ((!ts && n) || !n_slices || (cap && (!ends || !watermarks))) return CPBUS_EINVAL;
-  std::vector<size_t> end; std::vector<uint64_t> wm;
-  const int rc = split_plan(ts, n, batch_cap, now_ns, watermark_ns, window_ns, end, wm);
-  if (rc) return rc;
-  *n_slices = end.size();
-  for (size_t k = 0; k < end.size() && k < cap; k++) { ends[k] = end[k]; watermarks[k] = wm[k]; }
-  return CPBUS_OK;
-} CPBUS_CATCH
-size_t cpbus_mask_order(const uint32_t* masks, const uint8_t* active, uint32_t n, uint32_t ring_cap, uint32_t block, int heavy_first, uint32_t* out) {
-  if (!masks || !out || !ring_cap) return 0;
-  try {
-    std::vector<uint32_t> order;
-    mask_order(masks, active, n, ring_cap, block, heavy_first != 0, order);
-    std::copy(order.begin(), order.end(), out);
-    return order.size();
-  } catch (const std::bad_alloc&) { return 0; }
-}
-// The due index of a sparse-ticks bus over a table of n_slots slots, driven by ops instead of the bus's entry points (arms
-// start at the clock as timer_arm does; a launch fires what due_fire fires after a launch of the bus).
-int cpbus_due_trace(const cpbus_due_op* ops, size_t n_ops, uint32_t n_slots, uint32_t K, cpbus_due_fire* out, size_t cap,
-                    size_t* n_out) try {
-  if ((!ops && n_ops) || !n_out || (cap && !out) || !(K == 1 || K == 2 || K == 4 || K == 8)) return CPBUS_EINVAL;
-  std::vector<HostTimer> tm(n_slots);
-  DueIndex x;
-  x.init(n_slots);
-  uint64_t clock = 0, last = 0, launches = 0;
-  size_t n = 0;
-  std::vector<cpbus_due_fire> fired;
-  for (size_t i = 0; i < n_ops; i++) {
-    const cpbus_due_op& op = ops[i];
-    switch (op.kind) {
-      case CPBUS_DUE_CLOCK: clock = op.value; break;
-      case CPBUS_DUE_ARM:
-      case CPBUS_DUE_ONESHOT: {
-        if (op.slot >= n_slots || !op.value) return CPBUS_EINVAL;
-        HostTimer& t = tm[op.slot];
-        t.active = true; t.oneshot = op.kind == CPBUS_DUE_ONESHOT; t.period = op.value; t.next_due = due_after(clock, op.value);
-        x.put(op.slot, t.next_due);
-        break;
-      }
-      case CPBUS_DUE_DISARM:
-        if (op.slot >= n_slots) return CPBUS_EINVAL;
-        tm[op.slot].active = false; x.drop(op.slot);
-        break;
-      case CPBUS_DUE_UNSUB:
-        if ((uint64_t)op.slot * K + K > n_slots) return CPBUS_EINVAL;
-        for (uint32_t k = 0; k < K; k++) { tm[op.slot * K + k].active = false; x.drop(op.slot * K + k); }
-        break;
-      case CPBUS_DUE_CATCHUP: {
-        if (op.value < last) return CPBUS_EINVAL;
-        std::vector<uint32_t> moved;
-        due_catchup(x, tm, op.value, &moved);
-        clock = op.value;
-        break;
-      }
-      case CPBUS_DUE_LAUNCH:
-        if (op.value < last) return CPBUS_EINVAL;
-        last = op.value;
-        fired.clear();
-        due_fire(x, tm, op.value, [&](uint32_t s, uint64_t ticks, uint64_t nd) {
-          fired.push_back(cpbus_due_fire{launches, s, 0u, ticks, nd});
-        });
-        std::sort(fired.begin(), fired.end(), [](const cpbus_due_fire& a, const cpbus_due_fire& b) { return a.slot < b.slot; });
-        for (const cpbus_due_fire& f : fired) { if (n < cap) out[n] = f; n++; }
-        launches++;
-        break;
-      default: return CPBUS_EINVAL;
-    }
-  }
-  *n_out = n;
-  return CPBUS_OK;
-} CPBUS_CATCH
-// The plan of a sparse-records flush over an index built from the arguments, with the bus's own planning code (keep =
-// max_mailboxes: a code with more subscribers keeps only its count, as on a bus).
-int cpbus_sparse_plan(const uint32_t* masks, const uint8_t* active, uint32_t n_subs, const cpbus_pair* pairs,
-                      const uint32_t* n_pairs, uint32_t sub_id_base, const cpbus_event* records, size_t n_records,
-                      const uint32_t* due_slots, size_t n_due, uint32_t K, size_t max_mailboxes, size_t max_deliveries,
-                      cpbus_plan_entry* out, size_t cap, uint32_t* rec_idx, size_t idx_cap, size_t* n_out, size_t* n_idx) try {
-  if ((!masks && n_subs) || (!records && n_records) || (!due_slots && n_due) || (pairs && !n_pairs) || !n_out || !n_idx ||
-      (cap && !out) || (idx_cap && !rec_idx) || !(K == 0 || K == 1 || K == 2 || K == 4 || K == 8) || (!K && n_due))
-    return CPBUS_EINVAL;
-  for (size_t d = 0; d < n_due; d++) if (due_slots[d] / K >= n_subs) return CPBUS_EINVAL;
-  if (pairs) for (uint32_t l = 0; l < n_subs; l++) if (n_pairs[l] > CPBUS_MAX_PAIRS) return CPBUS_EINVAL;
-  std::vector<uint32_t> mask(n_subs);
-  std::vector<uint8_t> act(n_subs, 1);
-  for (uint32_t l = 0; l < n_subs; l++) { mask[l] = masks[l] & CPBUS_MASK_ALL; if (active) act[l] = active[l] ? 1 : 0; }
-  SubIndex x;
-  x.init(n_subs, max_mailboxes);
-  for (uint32_t l = 0; l < n_subs; l++) {
-    if (!act[l]) continue;
-    x.add_codes(l, mask[l]);
-    if (!pairs) continue;
-    uint64_t keys[CPBUS_MAX_PAIRS];
-    for (uint32_t j = 0; j < n_pairs[l]; j++) {
-      const cpbus_pair& pr = pairs[(size_t)l * CPBUS_MAX_PAIRS + j];
-      keys[j] = (uint64_t)pr.code << 32 | pr.source_id;
-    }
-    x.add_cases(l, keys, n_pairs[l]);
-  }
-  std::vector<uint32_t> due(due_slots, due_slots + n_due);
-  std::sort(due.begin(), due.end());
-  due.erase(std::unique(due.begin(), due.end()), due.end());
-  std::vector<uint64_t> scratch;
-  std::vector<cpbus_plan_entry> plan;
-  std::vector<uint32_t> idx;
-  if (!sparse_plan(x, mask.data(), act.data(), n_subs, sub_id_base, records, n_records, due, K, max_mailboxes, max_deliveries,
-                   scratch, plan, idx))
-    return CPBUS_ENOSPC;
-  std::copy(plan.begin(), plan.begin() + std::min(cap, plan.size()), out);
-  std::copy(idx.begin(), idx.begin() + std::min(idx_cap, idx.size()), rec_idx);
-  *n_out = plan.size(); *n_idx = idx.size();
-  return CPBUS_OK;
-} CPBUS_CATCH
-
-const char* cpbus_last_cuda_error(void) { return g_cuda_err; }
-
-const char* cpbus_strerror(int s) {
-  switch (s) {
-    case CPBUS_OK: return "ok";
-    case CPBUS_EINVAL: return "invalid argument";
-    case CPBUS_ENOMEM: return "out of memory";
-    case CPBUS_ECUDA: return "CUDA error";
-    case CPBUS_EAGAIN: return "mailbox full (lossless mode): drain and retry";
-    case CPBUS_ENOSPC: return "capacity exhausted";
-    case CPBUS_ENOENT: return "no such subscriber or timer";
-    case CPBUS_ECLOSED: return "subscriber already unsubscribed";
-    case CPBUS_ENODEV: return "no CUDA device (libcpbus has no CPU fallback)";
-    case CPBUS_EORDER: return "clock moved backwards, batch unsorted or timer window exceeded";
-    case CPBUS_ETIMEDOUT: return "stream batch never arrived (publisher stalled or consumer a whole ring behind)";
-    default: return "unknown status";
-  }
-}
-
-// EventCode.String — events/eventcode_string.go:5-15
-const char* cpbus_code_name(int code) {
-  static const char* const names[CPBUS_N_CODES] = {
-      "None", "ExitSuccess", "ExitFailed", "Stopping", "Stopped", "StatusHealthy", "StatusUnhealthy", "StatusChanged",
-      "TimerExpired", "EnterMaintenance", "ExitMaintenance", "Error", "Quit", "Metric", "Startup", "Shutdown", "Signal"};
-  return (code < 0 || code >= CPBUS_N_CODES) ? nullptr : names[code];
-}
-
-// FromString — events/events.go:52-86
-int cpbus_code_from_string(const char* name) try {
-  if (!name) return -1;
-  static const std::unordered_map<std::string, int> table = {
-      {"exitSuccess", CPBUS_EXIT_SUCCESS}, {"exitFailed", CPBUS_EXIT_FAILED}, {"stopping", CPBUS_STOPPING},
-      {"stopped", CPBUS_STOPPED}, {"healthy", CPBUS_STATUS_HEALTHY}, {"unhealthy", CPBUS_STATUS_UNHEALTHY},
-      {"changed", CPBUS_STATUS_CHANGED}, {"timerExpired", CPBUS_TIMER_EXPIRED},
-      {"enterMaintenance", CPBUS_ENTER_MAINTENANCE}, {"exitMaintenance", CPBUS_EXIT_MAINTENANCE},
-      {"error", CPBUS_ERROR}, {"quit", CPBUS_QUIT}, {"startup", CPBUS_STARTUP}, {"shutdown", CPBUS_SHUTDOWN},
-      {"SIGHUP", CPBUS_SIGNAL}, {"SIGUSR2", CPBUS_SIGNAL}};
-  auto it = table.find(name);
-  return it == table.end() ? -1 : it->second;
-} CPBUS_CATCH
-
-uint64_t cpbus_record_hash(const cpbus_event* e) {
-  return record_hash_words(e->seq, e->ts_ns, (uint64_t)e->code | ((uint64_t)e->source_id << 32),
-                           (uint64_t)e->target | ((uint64_t)e->flags << 32));
-}
-uint64_t cpbus_digest_multiplier(void) { return kDigestP; }
 
 // The checks cpbus_create makes of a config (cpbus_group_create makes them of the total); R and B get the defaults applied.
-static int config_check(const cpbus_config* cfg, uint32_t* R_out, uint32_t* B_out) {
+int cpbus_host::config_check(const cpbus_config* cfg, uint32_t* R_out, uint32_t* B_out) {
   const uint32_t R = cfg->ring_cap ? cfg->ring_cap : 1024;
   const uint32_t B = cfg->batch_cap ? cfg->batch_cap : std::min(256u, R / 2);
   const uint32_t K = cfg->timers_per_sub;
@@ -1818,7 +887,13 @@ int cpbus_subscribe_many(cpbus_t* b, const uint32_t* masks, uint32_t n, uint32_t
 
 int cpbus_subscribe(cpbus_t* b, uint32_t mask, uint32_t* sub_id) { return cpbus_subscribe_many(b, &mask, 1, sub_id); }
 
-static int push_mask_words(cpbus* b, uint32_t first, uint32_t n);
+static int push_mask_words(cpbus* b, uint32_t first, uint32_t n) {
+  std::vector<uint32_t> words(n);
+  for (uint32_t i = 0; i < n; i++) words[i] = mask_word(b, first + i);
+  CK(cudaMemcpy2DAsync(&b->d_ctl[first].mask, sizeof(SubCtl), words.data(), 4, 4, n, cudaMemcpyHostToDevice, b->stream));
+  CK(cudaStreamSynchronize(b->stream));
+  return CPBUS_OK;
+}
 
 // The pair tables of every subscriber, allocated by the first subscription with pairs.
 static int pair_tables(cpbus* b) {
@@ -1951,14 +1026,6 @@ int cpbus_set_mask(cpbus_t* b, uint32_t sub_id, uint32_t mask) try {
   return push_mask_words(b, l, 1);
 } CPBUS_CATCH
 
-static int push_mask_words(cpbus* b, uint32_t first, uint32_t n) {
-  std::vector<uint32_t> words(n);
-  for (uint32_t i = 0; i < n; i++) words[i] = mask_word(b, first + i);
-  CK(cudaMemcpy2DAsync(&b->d_ctl[first].mask, sizeof(SubCtl), words.data(), 4, 4, n, cudaMemcpyHostToDevice, b->stream));
-  CK(cudaStreamSynchronize(b->stream));
-  return CPBUS_OK;
-}
-
 int cpbus_timer_add(cpbus_t* b, uint32_t sub_id, uint64_t period_ns, uint32_t source_id, int oneshot, uint32_t* timer_id) try {
   if (!b || !period_ns) return CPBUS_EINVAL;
   if (!b->K) return CPBUS_ENOSPC;
@@ -2051,7 +1118,6 @@ int cpbus_timer_cancel(cpbus_t* b, uint32_t timer_id) try {
 // refusal.  The flush's CPBUS_EAGAIN (or an error) is returned with nothing applied and status / applied not written.
 // Every mailbox an applied element touched then gets one membership_kernel entry with its final mask word: one H2D copy,
 // one launch and one synchronisation, where the single calls take one synchronised round trip each.
-extern "C++" {
 template <class Check, class AfterFlush, class Apply>
 static int membership_many(cpbus* b, uint32_t n, int* status, uint32_t* applied, Check&& check, AfterFlush&& after_flush,
                            Apply&& apply) {
@@ -2093,7 +1159,6 @@ static int membership_many(cpbus* b, uint32_t n, int* status, uint32_t* applied,
   if (applied) *applied = ok;
   return CPBUS_OK;
 }
-}
 
 int cpbus_unsubscribe_many(cpbus_t* b, const uint32_t* sub_ids, uint32_t n, int* status, uint32_t* applied) try {
   if (!b || (!sub_ids && n)) return CPBUS_EINVAL;
@@ -2130,7 +1195,6 @@ int cpbus_timer_cancel_many(cpbus_t* b, const uint32_t* timer_ids, uint32_t n, i
 } CPBUS_CATCH
 
 static_assert(sizeof(cpbus_timer_spec) == 24, "cpbus_timer_spec is part of the ABI");
-static_assert(sizeof(TimerArmOp) == 32, "timer_arm_kernel reads an entry as two 16-byte words");
 
 // cpbus_timer_add's refusals before its flush: CPBUS_EINVAL, CPBUS_ENOSPC (no timer slots at all), CPBUS_ENOENT
 static int timer_add_check(const cpbus* b, const cpbus_timer_spec& s) {
@@ -2270,7 +1334,7 @@ int cpbus_release_many(cpbus_t* b, const uint32_t* sub_ids, uint32_t n, int* sta
 } CPBUS_CATCH
 
 // The argument checks of cpbus_subscribe_pairs_many, with pairs / n_pairs NULL meaning no cases
-static int subscribe_list_check(const uint32_t* n_pairs, const cpbus_pair* pairs, uint32_t n) {
+int cpbus_host::subscribe_list_check(const uint32_t* n_pairs, const cpbus_pair* pairs, uint32_t n) {
   if (!n_pairs) return CPBUS_OK;
   if (!pairs) return CPBUS_EINVAL;
   for (uint32_t i = 0; i < n; i++) {
@@ -2369,27 +1433,6 @@ static int publish_device_impl(cpbus_t* b, const void* d_events, size_t n, uint6
 // a tick is ordered in front of every event with ts >= its due time and such events are either in this slice behind it or
 // in a later one.  The host path does the same at cpbus_advance.  (events/timer.go:40-71 has no such limit: a Go timer
 // that fell behind fires late, never "not at all".)
-// The cut itself, host-only (exported as cpbus_split_plan so that it can be tested without a GPU): slice k = records
-// [end[k-1], end[k]) launched with watermark wm[k].  `now` = the bus clock (= the last launched watermark once staged events
-// are flushed), `window` = the widest watermark step one launch may take (UINT64_MAX: no timer armed).
-static int split_plan(const uint64_t* ts, size_t n, uint32_t batch_cap, uint64_t now, uint64_t watermark, uint64_t window,
-                      std::vector<size_t>& end, std::vector<uint64_t>& wm) {
-  for (size_t i = 1; i < n; i++) if (ts[i] < ts[i - 1]) return CPBUS_EORDER;
-  if (!batch_cap || !window) return CPBUS_EINVAL;
-  if (watermark < now || (n && ts[n - 1] > watermark)) return CPBUS_EORDER;
-  size_t i = 0;
-  uint64_t lw = now;
-  for (;;) {
-    const uint64_t edge = (window == UINT64_MAX || watermark - lw <= window) ? watermark : lw + window;
-    size_t j = std::upper_bound(ts + i, ts + n, edge) - ts;
-    uint64_t w = edge;
-    if (j - i > batch_cap) { j = i + batch_cap; w = std::max(ts[j - 1], lw); }   // (records older than the clock ride with it)
-    end.push_back(j); wm.push_back(w);
-    i = j; lw = w;
-    if (j == n && w == watermark) return CPBUS_OK;
-  }
-}
-
 static int publish_device_split(cpbus_t* b, const cpbus_event* d_events, size_t n, uint64_t watermark_ns, bool staged,
                                 const void* d_next, size_t n_next) {
   std::vector<uint64_t> ts, wm;
@@ -2672,7 +1715,7 @@ int cpbus_stream_status(cpbus_stream_t* st) try {
 
 // Publisher: copy the batch into the next slot, then release it (header after payload, same stream).  `device_src`: ev
 // holds complete records in device memory (this GPU's or a peer's), copied into the slot as they are (CPBUS_PUT_RAW).
-static int stream_put(cpbus_stream* st, const cpbus_event* ev, size_t n, uint64_t now_ns, uint32_t flags, bool device_src) {
+int cpbus_host::stream_put(cpbus_stream* st, const cpbus_event* ev, size_t n, uint64_t now_ns, uint32_t flags, bool device_src) {
   cpbus* b = st->bus;
   int rc = dev_guard(b); if (rc) return rc;
   const unsigned long long q = st->put_seq + 1;
@@ -2831,7 +1874,7 @@ static void stream_delivered(cpbus* b, cpbus_stream* st, uint32_t m, uint64_t w,
 
 // Fan out the next m undelivered records of the current batch (throughput mode: m = the whole batch, in one launch).
 // `account`: the lead CTA accounts the records as a device-published batch (a group's shards: see group_launch).
-static int stream_fanout_prefix(cpbus_stream* st, size_t n, uint64_t now_ns, size_t m, bool account) {
+int cpbus_host::stream_fanout_prefix(cpbus_stream* st, size_t n, uint64_t now_ns, size_t m, bool account) {
   cpbus* b = st->bus;
   int rc = stream_enter(st, now_ns); if (rc) return rc;
   const bool final = m == n - st->get_off;
@@ -3130,13 +2173,6 @@ int cpbus_drain_many(cpbus_t* b, uint32_t first_sub, uint32_t n, cpbus_event* ou
 // Sparse drain: only the mailboxes that hold records.  The scan kernel reads each control block of the range once and
 // writes the ready list of the taken prefix; the gather kernel copies their runs and hands the 3-word header to the host
 // through mapped pinned memory.  One sync reads the header; a second one follows the two copies sized by it.
-// The body of cpbus_drain_ready, without its cap >= ring_cap check: a group hands each shard the cap its earlier shards
-// left, which can be smaller.  *all_taken: every ready mailbox of the range was taken (then *next_sub = start_sub).
-// take: cpbus_take_ready's scan (the caller has checked that the bus is lossless).
-static int drain_ready_impl(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start_sub, cpbus_event* out, size_t cap,
-                            cpbus_ready* ready, size_t ready_cap, size_t* n_ready, size_t* total, uint32_t* next_sub,
-                            bool* all_taken, bool take = false);
-
 int cpbus_drain_ready(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start_sub, cpbus_event* out, size_t cap,
                       cpbus_ready* ready, size_t ready_cap, size_t* n_ready, size_t* total, uint32_t* next_sub) try {
   if (!b || !out || !ready || !n_ready || !total || !next_sub || !n || !ready_cap) return CPBUS_EINVAL;
@@ -3153,9 +2189,12 @@ int cpbus_take_ready(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start_
   return drain_ready_impl(b, first_sub, n, start_sub, out, cap, ready, ready_cap, n_ready, total, next_sub, &all_taken, true);
 } CPBUS_CATCH
 
-static int drain_ready_impl(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start_sub, cpbus_event* out, size_t cap,
-                            cpbus_ready* ready, size_t ready_cap, size_t* n_ready, size_t* total, uint32_t* next_sub,
-                            bool* all_taken, bool take) {
+// The body of cpbus_drain_ready, without its cap >= ring_cap check: a group hands each shard the cap its earlier shards
+// left, which can be smaller.  *all_taken: every ready mailbox of the range was taken (then *next_sub = start_sub).
+// take: cpbus_take_ready's scan (the caller has checked that the bus is lossless).
+int cpbus_host::drain_ready_impl(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start_sub, cpbus_event* out, size_t cap,
+                                 cpbus_ready* ready, size_t ready_cap, size_t* n_ready, size_t* total, uint32_t* next_sub,
+                                 bool* all_taken, bool take) {
   if (start_sub < first_sub || start_sub - first_sub >= n) return CPBUS_EINVAL;
   uint32_t l = 0;
   if (!id_range(b->cfg.sub_id_base, b->n_next, first_sub, n, &l)) return CPBUS_ENOENT;
@@ -3206,7 +2245,7 @@ static int drain_ready_impl(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t
 // cpbus_ack_many on one bus (the caller has checked the arguments and that the bus is lossless): st[i] for every element.
 // Unknown ids get CPBUS_ENOENT and count 0 gets CPBUS_OK on the host; the others go to ack_kernel, one entry per mailbox
 // with its elements in array order.  Before the first take nothing is held, so they are refused without a launch.
-static int ack_many_impl(cpbus* b, const uint32_t* sub_ids, const uint32_t* counts, uint32_t n, int* st) {
+int cpbus_host::ack_many_impl(cpbus* b, const uint32_t* sub_ids, const uint32_t* counts, uint32_t n, int* st) {
   std::vector<uint64_t> el;   // mailbox << 32 | element index: sorted, each mailbox's elements stay in array order
   for (uint32_t i = 0; i < n; i++) {
     uint32_t l = 0;
@@ -3247,7 +2286,7 @@ static int ack_many_impl(cpbus* b, const uint32_t* sub_ids, const uint32_t* coun
 }
 
 // status (may be NULL) = st, *applied (may be NULL) = how many are CPBUS_OK
-static void ack_statuses(const std::vector<int>& st, int* status, uint32_t* applied) {
+void cpbus_host::ack_statuses(const std::vector<int>& st, int* status, uint32_t* applied) {
   if (status) memcpy(status, st.data(), st.size() * sizeof(int));
   if (applied) *applied = (uint32_t)std::count(st.begin(), st.end(), CPBUS_OK);
 }
@@ -3268,8 +2307,8 @@ int cpbus_ack_many(cpbus_t* b, const uint32_t* sub_ids, const uint32_t* counts, 
 
 // Consumer backlog: one read-only scan of the range's control blocks; the entries and the header {selected, cut position,
 // summary} arrive in mapped pinned memory, so one sync is the only wait.  *all_returned: every lagging mailbox was returned.
-static int lagging_impl(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start_sub, uint32_t min_backlog, cpbus_lag* out,
-                        size_t cap, size_t* n_out, uint32_t* next_sub, cpbus_lag_summary* sum, bool* all_returned) {
+int cpbus_host::lagging_impl(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start_sub, uint32_t min_backlog, cpbus_lag* out,
+                             size_t cap, size_t* n_out, uint32_t* next_sub, cpbus_lag_summary* sum, bool* all_returned) {
   static_assert(sizeof(cpbus_lag) == 16 && sizeof(cpbus_lag_summary) == kLagSumWords * sizeof(unsigned long long), "C-ABI layout");
   if (start_sub < first_sub || start_sub - first_sub >= n) return CPBUS_EINVAL;
   uint32_t l = 0;
@@ -3311,7 +2350,7 @@ int cpbus_lagging(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start_sub
 // The subscribed mailboxes of this shard that refuse the next unit U of a lossless flush: the record `rec` (NULL: ticks
 // only) with the ticks due by t.  The caller holds b->mu and has resolved.  No kernel when the room bound proves that U fits
 // (admit_fits without taking anything from the bound).
-static int blockers_impl(cpbus* b, const cpbus_event* rec, uint64_t t, uint32_t* out, size_t cap, size_t* n) {
+int cpbus_host::blockers_impl(cpbus* b, const cpbus_event* rec, uint64_t t, uint32_t* out, size_t cap, size_t* n) {
   *n = 0;
   const bool timers_on = b->n_timers > 0 && b->K > 0;
   if (b->n_next == 0 || b->room_lb >= admit_need(rec ? 1 : 0, t, b->last_watermark, b->min_period, b->K, timers_on)) return CPBUS_OK;
@@ -3495,7 +2534,7 @@ int cpbus_step_result_end(cpbus_t* b, uint32_t ticket, uint64_t out[4]) try {
 // Broadcast events of device-published batches join the debug ring here, in publish order (the kernel's lead CTA kept
 // the last 10 of each such batch; launches older than kAcctDbgRing are no longer resolvable and are skipped).  f's markers
 // name launches of bus b (f = b, or a group and its shard 0).
-static int dbg_resolve(HostFront* f, cpbus* b) {
+int cpbus_host::dbg_resolve(HostFront* f, cpbus* b) {
   if (f->dbg_pending.empty()) return CPBUS_OK;
   bool any_marker = false;
   for (const DbgItem& it : f->dbg_pending) any_marker |= it.marker;
@@ -3551,7 +2590,7 @@ int cpbus_stats(cpbus_t* b, cpbus_stats_t* out) try {
 } CPBUS_CATCH
 
 // The {code, source} table of bus b's device-published batches (DevPubAcct), read back behind b's launches.
-static int device_pairs(cpbus* b, std::vector<unsigned long long>& keys, std::vector<unsigned long long>& cnts) {
+int cpbus_host::device_pairs(cpbus* b, std::vector<unsigned long long>& keys, std::vector<unsigned long long>& cnts) {
   keys.resize(kAcctPairSlots); cnts.resize(kAcctPairSlots);
   CK(cudaMemcpyAsync(keys.data(), b->d_acct->pair_key, sizeof(unsigned long long) * kAcctPairSlots, cudaMemcpyDeviceToHost, b->stream));
   CK(cudaMemcpyAsync(cnts.data(), b->d_acct->pair_cnt, sizeof(unsigned long long) * kAcctPairSlots, cudaMemcpyDeviceToHost, b->stream));
@@ -3577,807 +2616,3 @@ int cpbus_device_ptrs(cpbus_t* b, void** ring, void** ctl) try {
   if (ctl) *ctl = b->d_ctl;
   return CPBUS_OK;
 } CPBUS_CATCH
-
-// ---- the group: one bus handle over the GPUs of a box (include/cpbus.h: cpbus_group_*; struct cpbus_group) ---------------
-static uint32_t group_shard_of(const cpbus_group* g, uint32_t index) {   // index < N
-  return (uint32_t)(std::upper_bound(g->first.begin(), g->first.end(), index) - g->first.begin()) - 1;
-}
-
-// retire_oneshots for the group's table and, at the same moment, every shard's own: a shard's timer count (and so its
-// window) then never lags the group's
-static void group_retire(cpbus_group* g) {
-  retire_oneshots(g, g->last_watermark);
-  for (cpbus* s : g->shards) if (!s->h_timers.empty()) retire_oneshots(s, s->last_watermark);
-}
-
-// the owning shard of global id `sub_id` and its local index; false: not a subscribed-so-far id, or a released one (*s and
-// *l are still set when the id is below n_next)
-static bool group_locate(const cpbus_group* g, uint32_t sub_id, cpbus** s, uint32_t* l) {
-  uint32_t i = 0;
-  if (!id_range(g->base, g->n_next, sub_id, 1, &i)) return false;
-  const uint32_t k = group_shard_of(g, i);
-  *s = g->shards[k]; *l = i - g->first[k];
-  return !(*s)->h_released[*l];   // a released id is refused as one never handed out
-}
-
-// Arm timers on shard s: a shard without timers takes the group clock first (cpbus_advance launches nothing there).
-static int group_shard_clock(cpbus_group* g, cpbus* s) {
-  if (s->now == g->now) return CPBUS_OK;
-  if (s->n_timers) return CPBUS_ECUDA;   // cannot happen: the group has just flushed at now, which moved this shard there
-  return cpbus_advance(s, g->now);
-}
-
-int cpbus_group_destroy(cpbus_group_t* g) try {
-  if (!g) return CPBUS_EINVAL;
-  for (size_t i = g->streams.size(); i-- > 0;) if (g->streams[i]) cpbus_stream_close(g->streams[i]);   // importers first
-  for (cpbus* s : g->shards) if (s) cpbus_destroy(s);
-  delete g;
-  return CPBUS_OK;
-} CPBUS_CATCH
-
-int cpbus_group_create(const cpbus_config* cfg, const int32_t* devices, uint32_t n_devices, cpbus_group_t** out) try {
-  if (!cfg || !devices || !n_devices || !out || cfg->stream || n_devices > kStreamMaxConsumers) return CPBUS_EINVAL;
-  *out = nullptr;
-  if (cfg->flags & CPBUS_CFG_SPARSE_TICKS) return CPBUS_EINVAL;   // the group's flush is a stream batch (see cpbus_stream_create)
-  if (cfg->flags & CPBUS_CFG_SPARSE_RECORDS) return CPBUS_EINVAL;
-  uint32_t R = 0, B = 0;
-  if (config_check(cfg, &R, &B) || cfg->n_max_subs < n_devices) return CPBUS_EINVAL;
-  cpbus_group* g = new (std::nothrow) cpbus_group();
-  if (!g) return CPBUS_ENOMEM;
-  g->base = cfg->sub_id_base; g->N = cfg->n_max_subs; g->B = B; g->K = cfg->timers_per_sub;
-  g->lossless = cfg->flags & CPBUS_CFG_LOSSLESS;
-  g->drop_missed = cfg->flags & CPBUS_CFG_DROP_MISSED_TICKS;   // the group catches its shards up itself (catch_up)
-  g->staged.resize(B);
-  auto fail = [&](int code) { cpbus_group_destroy(g); return code; };
-  const uint32_t each = g->N / n_devices, extra = g->N % n_devices;   // sharding.shard_range
-  for (uint32_t k = 0; k < n_devices; k++) {
-    const uint32_t first = k * each + std::min(k, extra), count = each + (k < extra ? 1u : 0u);
-    cpbus_config c = *cfg;
-    c.n_max_subs = count; c.device = devices[k]; c.sub_id_base = g->base + first;
-    c.flags &= ~CPBUS_CFG_DROP_MISSED_TICKS;   // (a flagged shard would refuse the group's streams)
-    cpbus* s = nullptr;
-    const int rc = cpbus_create(&c, &s);
-    if (rc) return fail(rc);
-    g->shards.push_back(s); g->first.push_back(first);
-  }
-  g->first.push_back(g->N);
-  unsigned char handle[64];
-  cpbus_stream* st0 = nullptr;
-  int rc = cpbus_stream_create(g->shards[0], 8, n_devices, &st0, handle);
-  if (rc) return fail(rc);
-  g->streams.push_back(st0);
-  for (uint32_t k = 1; k < n_devices; k++) {
-    cpbus_stream* st = nullptr;
-    if ((rc = cpbus_stream_attach(g->shards[k], st0, k, &st))) return fail(rc);
-    g->streams.push_back(st);
-  }
-  // a device batch (cpbus_group_publish_device) may live on any GPU of the group: peer access between every two of them
-  // where the hardware has it, as cpbus_stream_attach enables it towards shard 0
-  for (cpbus* a : g->shards)
-    for (cpbus* b : g->shards) {
-      if (a->device == b->device) continue;
-      int can = 0;
-      if (cudaSetDevice(a->device) != cudaSuccess || cudaDeviceCanAccessPeer(&can, a->device, b->device) != cudaSuccess) return fail(CPBUS_ECUDA);
-      if (!can) continue;
-      const cudaError_t e = cudaDeviceEnablePeerAccess(b->device, 0);
-      if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) return fail(CPBUS_ECUDA);
-      cudaGetLastError();   // clear "already enabled"
-    }
-  *out = g;
-  return CPBUS_OK;
-} CPBUS_CATCH
-
-int cpbus_group_intern(cpbus_group_t* g, const char* s, size_t len, uint32_t* source_id) try {
-  return g ? cpbus_intern(g->shards[0], s, len, source_id) : CPBUS_EINVAL;
-} CPBUS_CATCH
-int cpbus_group_intern_ephemeral(cpbus_group_t* g, const char* s, size_t len, uint32_t* source_id) try {
-  return g ? cpbus_intern_ephemeral(g->shards[0], s, len, source_id) : CPBUS_EINVAL;
-} CPBUS_CATCH
-int cpbus_group_source(cpbus_group_t* g, uint32_t source_id, char* out, size_t cap, size_t* len) try {
-  return g ? cpbus_source(g->shards[0], source_id, out, cap, len) : CPBUS_EINVAL;
-} CPBUS_CATCH
-
-// Subscribers [n_next, n_next + n) across the shards that own them; fn(shard, offset into the caller's arrays, count).
-extern "C++" {
-template <class Fn>
-static int group_each_range(cpbus_group* g, uint32_t first_index, uint32_t n, Fn&& fn) {
-  for (uint32_t done = 0; done < n;) {
-    const uint32_t i = first_index + done, k = group_shard_of(g, i);
-    const uint32_t cnt = std::min(n - done, g->first[k + 1] - i);
-    const int rc = fn(g->shards[k], i - g->first[k], done, cnt);
-    if (rc) return rc;
-    done += cnt;
-  }
-  return CPBUS_OK;
-}
-
-// The cyclic walk of a paged query (cpbus_drain_ready, cpbus_lagging) over ids [first_sub, first_sub + n) from start_sub, in
-// pieces that each lie on one shard: fn(shard, local index, id, count) returns CPBUS_OK to go on, kWalkEnd to end the walk,
-// or an error.  The checks are the single call's; *next_sub is set to start_sub (the walk found no cut) before the first piece.
-constexpr int kWalkEnd = 1;
-template <class Fn>
-static int group_walk(cpbus_group* g, uint32_t first_sub, uint32_t n, uint32_t start_sub, uint32_t* next_sub, Fn&& fn) {
-  if (start_sub < first_sub || start_sub - first_sub >= n) return CPBUS_EINVAL;
-  uint32_t i0 = 0;
-  if (!id_range(g->base, g->n_next, first_sub, n, &i0)) return CPBUS_ENOENT;
-  const uint32_t rot = start_sub - first_sub;
-  *next_sub = start_sub;
-  for (uint32_t done = 0; done < n;) {
-    const uint32_t i = i0 + (rot + done) % n;                       // global index of the walk's next mailbox
-    const uint32_t k = group_shard_of(g, i);
-    const uint32_t wrap = i0 + n - i;                               // the walk wraps to first_sub after this many
-    const uint32_t cnt = std::min({n - done, g->first[k + 1] - i, wrap});
-    const int rc = fn(g->shards[k], i - g->first[k], g->base + i, cnt);
-    if (rc) return rc == kWalkEnd ? CPBUS_OK : rc;
-    done += cnt;
-  }
-  return CPBUS_OK;
-}
-}
-
-int cpbus_group_subscribe_many(cpbus_group_t* g, const uint32_t* masks, uint32_t n, uint32_t* first_sub_id) try {
-  if (!g || !n) return CPBUS_EINVAL;
-  if ((uint64_t)g->n_next + n > g->N) return CPBUS_ENOSPC;
-  int rc = flush_staged(g, g->now); if (rc) return rc;
-  const uint32_t first = g->n_next;
-  rc = group_each_range(g, first, n, [&](cpbus* s, uint32_t, uint32_t off, uint32_t cnt) -> int {
-    uint32_t id = 0;
-    return cpbus_subscribe_many(s, masks ? masks + off : nullptr, cnt, &id);
-  });
-  if (rc) return rc;
-  g->n_next += n; g->n_active += n;
-  if (first_sub_id) *first_sub_id = g->base + first;
-  return CPBUS_OK;
-} CPBUS_CATCH
-
-int cpbus_group_subscribe(cpbus_group_t* g, uint32_t mask, uint32_t* sub_id) { return cpbus_group_subscribe_many(g, &mask, 1, sub_id); }
-
-int cpbus_group_subscribe_pairs(cpbus_group_t* g, uint32_t mask, const cpbus_pair* pairs, uint32_t n_pairs, uint32_t* sub_id) try {
-  if (!g || n_pairs > CPBUS_MAX_PAIRS || (n_pairs && !pairs)) return CPBUS_EINVAL;
-  for (uint32_t j = 0; j < n_pairs; j++) if (pairs[j].code >= CPBUS_N_CODES) return CPBUS_EINVAL;
-  if (g->n_next >= g->N) return CPBUS_ENOSPC;
-  int rc = flush_staged(g, g->now); if (rc) return rc;
-  const uint32_t k = group_shard_of(g, g->n_next);
-  uint32_t id = 0;
-  if ((rc = cpbus_subscribe_pairs(g->shards[k], mask, pairs, n_pairs, &id))) return rc;
-  g->n_next++; g->n_active++;
-  if (sub_id) *sub_id = id;
-  return CPBUS_OK;
-} CPBUS_CATCH
-
-int cpbus_group_subscribe_pairs_many(cpbus_group_t* g, const uint32_t* masks, const cpbus_pair* pairs, const uint32_t* n_pairs,
-                                     uint32_t n, uint32_t* first_sub_id) try {
-  if (!g || !n || !masks || !pairs || !n_pairs) return CPBUS_EINVAL;
-  for (uint32_t i = 0; i < n; i++) {
-    if (n_pairs[i] > CPBUS_MAX_PAIRS) return CPBUS_EINVAL;
-    for (uint32_t j = 0; j < n_pairs[i]; j++) if (pairs[(size_t)i * CPBUS_MAX_PAIRS + j].code >= CPBUS_N_CODES) return CPBUS_EINVAL;
-  }
-  if ((uint64_t)g->n_next + n > g->N) return CPBUS_ENOSPC;
-  int rc = flush_staged(g, g->now); if (rc) return rc;
-  const uint32_t first = g->n_next;
-  rc = group_each_range(g, first, n, [&](cpbus* s, uint32_t, uint32_t off, uint32_t cnt) -> int {
-    uint32_t id = 0;
-    return cpbus_subscribe_pairs_many(s, masks + off, pairs + (size_t)off * CPBUS_MAX_PAIRS, n_pairs + off, cnt, &id);
-  });
-  if (rc) return rc;
-  g->n_next += n; g->n_active += n;
-  if (first_sub_id) *first_sub_id = g->base + first;
-  return CPBUS_OK;
-} CPBUS_CATCH
-
-int cpbus_group_unsubscribe(cpbus_group_t* g, uint32_t sub_id) try {
-  if (!g) return CPBUS_EINVAL;
-  cpbus* s = nullptr; uint32_t l = 0;
-  if (!group_locate(g, sub_id, &s, &l)) return CPBUS_ENOENT;
-  int rc = flush_staged(g, g->now); if (rc) return rc;
-  if ((rc = cpbus_unsubscribe(s, sub_id))) return rc;
-  if (g->K && !g->h_timers.empty())
-    for (uint32_t k = 0; k < g->K; k++) timer_disarm(g, (size_t)(sub_id - g->base) * g->K + k, /*reset_bound=*/false);
-  g->n_active--;
-  return CPBUS_OK;
-} CPBUS_CATCH
-
-int cpbus_group_set_mask(cpbus_group_t* g, uint32_t sub_id, uint32_t mask) try {
-  if (!g) return CPBUS_EINVAL;
-  cpbus* s = nullptr; uint32_t l = 0;
-  if (!group_locate(g, sub_id, &s, &l)) return CPBUS_ENOENT;
-  if (!s->h_active[l]) return CPBUS_ECLOSED;
-  const int rc = flush_staged(g, g->now); if (rc) return rc;
-  return cpbus_set_mask(s, sub_id, mask);
-} CPBUS_CATCH
-
-int cpbus_group_timer_add(cpbus_group_t* g, uint32_t sub_id, uint64_t period_ns, uint32_t source_id, int oneshot, uint32_t* timer_id) try {
-  if (!g || !period_ns) return CPBUS_EINVAL;
-  if (!g->K) return CPBUS_ENOSPC;
-  cpbus* s = nullptr; uint32_t l = 0;
-  if (!group_locate(g, sub_id, &s, &l)) return CPBUS_ENOENT;
-  int rc = flush_staged(g, g->now); if (rc) return rc;
-  if (g->h_timers.empty()) g->h_timers.resize((size_t)g->N * g->K);
-  group_retire(g);
-  if (!s->h_active[l]) return CPBUS_ECLOSED;
-  if ((rc = group_shard_clock(g, s))) return rc;
-  uint32_t id = 0;
-  if ((rc = cpbus_timer_add(s, sub_id, period_ns, source_id, oneshot, &id))) return rc;
-  const uint32_t shard_base_slot = (sub_id - l - g->base) * g->K;   // global slot of the shard's slot 0
-  const size_t slot = (size_t)(id & kTimerSlotMask) + shard_base_slot;
-  timer_arm(g, slot, period_ns, source_id, oneshot != 0);
-  if (timer_id) *timer_id = (uint32_t)slot | (id & ~kTimerSlotMask);
-  return CPBUS_OK;
-} CPBUS_CATCH
-
-int cpbus_group_timer_add_many(cpbus_group_t* g, uint32_t first_sub, uint32_t n, uint64_t period_ns, const uint32_t* source_ids,
-                               uint32_t source_id0, int oneshot) try {
-  if (!g || !period_ns || !n) return CPBUS_EINVAL;
-  if (!g->K) return CPBUS_ENOSPC;
-  uint32_t i0 = 0;
-  if (!id_range(g->base, g->n_next, first_sub, n, &i0)) return CPBUS_ENOENT;
-  for (uint32_t i = 0; i < n; i++) {   // a released id: as one never handed out
-    cpbus* s = nullptr; uint32_t l = 0;
-    if (!group_locate(g, first_sub + i, &s, &l)) return CPBUS_ENOENT;
-  }
-  int rc = flush_staged(g, g->now); if (rc) return rc;
-  if (g->h_timers.empty()) g->h_timers.resize((size_t)g->N * g->K);
-  group_retire(g);
-  // the single bus checks every subscriber before it arms any
-  for (uint32_t i = 0; i < n; i++) {
-    cpbus* s = nullptr; uint32_t l = 0;
-    group_locate(g, first_sub + i, &s, &l);
-    if (!s->h_active[l]) return CPBUS_ECLOSED;
-    if (g->h_timers[(size_t)(i0 + i) * g->K].active) return CPBUS_ENOSPC;
-  }
-  rc = group_each_range(g, i0, n, [&](cpbus* s, uint32_t l, uint32_t off, uint32_t cnt) -> int {
-    const int rc_clock = group_shard_clock(g, s);
-    if (rc_clock) return rc_clock;
-    return cpbus_timer_add_many(s, s->cfg.sub_id_base + l, cnt, period_ns, source_ids ? source_ids + off : nullptr,
-                                source_id0 + off, oneshot);
-  });
-  if (rc) return rc;
-  for (uint32_t i = 0; i < n; i++)
-    timer_arm(g, (size_t)(i0 + i) * g->K, period_ns, source_ids ? source_ids[i] : source_id0 + i, oneshot != 0);
-  return CPBUS_OK;
-} CPBUS_CATCH
-
-int cpbus_group_timer_cancel(cpbus_group_t* g, uint32_t timer_id) try {
-  if (!g) return CPBUS_EINVAL;
-  if (!g->K || g->h_timers.empty()) return CPBUS_ENOENT;
-  const uint32_t slot = timer_id & kTimerSlotMask, i = slot / g->K;
-  if (i >= g->n_next) return CPBUS_ENOENT;
-  int rc = flush_staged(g, g->now); if (rc) return rc;
-  group_retire(g);
-  const uint32_t k = group_shard_of(g, i);
-  const uint32_t local = (slot - g->first[k] * g->K) | (timer_id & ~kTimerSlotMask);
-  if ((rc = cpbus_timer_cancel(g->shards[k], local))) return rc;
-  timer_disarm(g, slot, /*reset_bound=*/true);
-  return CPBUS_OK;
-} CPBUS_CATCH
-
-// The group's bulk membership calls: the single group calls' loop.  check(i, &k) is element i's refusal before the group's
-// flush (CPBUS_OK: none, and k = its shard); the group flushes once, where the first element that passes would, then
-// after_flush(); then each shard with work takes its elements, in array order, in one call of the shard's bulk call:
-// run(k, elements, their statuses), which also keeps the group's own records of the elements the shard applied.  Shards
-// are independent, and the group's records of these calls (n_active, n_timers, min_period) end where the interleaved loop
-// leaves them.
-extern "C++" {
-template <class Check, class AfterFlush, class Run>
-static int group_membership_many(cpbus_group* g, uint32_t n, int* status, uint32_t* applied, Check&& check,
-                                 AfterFlush&& after_flush, Run&& run) {
-  std::vector<int> st(n);
-  std::vector<std::vector<uint32_t>> work(g->shards.size());
-  bool any = false;
-  for (uint32_t i = 0; i < n; i++) {
-    uint32_t k = 0;
-    if ((st[i] = check(i, &k)) == CPBUS_OK) { work[k].push_back(i); any = true; }
-  }
-  if (any) {
-    int rc = flush_staged(g, g->now); if (rc) return rc;
-    after_flush();
-    std::vector<int> st_k;
-    for (uint32_t k = 0; k < g->shards.size(); k++) {
-      if (work[k].empty()) continue;
-      st_k.assign(work[k].size(), CPBUS_OK);
-      if ((rc = run(k, work[k], st_k.data()))) return rc;
-      for (size_t j = 0; j < work[k].size(); j++) st[work[k][j]] = st_k[j];
-    }
-  }
-  uint32_t ok = 0;
-  for (uint32_t i = 0; i < n; i++) ok += st[i] == CPBUS_OK ? 1u : 0u;
-  if (status && n) memcpy(status, st.data(), (size_t)n * sizeof(int));
-  if (applied) *applied = ok;
-  return CPBUS_OK;
-}
-}
-
-int cpbus_group_unsubscribe_many(cpbus_group_t* g, const uint32_t* sub_ids, uint32_t n, int* status, uint32_t* applied) try {
-  if (!g || (!sub_ids && n)) return CPBUS_EINVAL;
-  std::vector<uint32_t> ids;
-  return group_membership_many(g, n, status, applied,
-      [&](uint32_t i, uint32_t* k) {
-        cpbus* s = nullptr; uint32_t l = 0;
-        if (!group_locate(g, sub_ids[i], &s, &l)) return CPBUS_ENOENT;
-        *k = group_shard_of(g, sub_ids[i] - g->base);
-        return CPBUS_OK;
-      },
-      [] {},
-      [&](uint32_t k, const std::vector<uint32_t>& el, int* st) -> int {
-        ids.resize(el.size());
-        for (size_t j = 0; j < el.size(); j++) ids[j] = sub_ids[el[j]];
-        const int rc = cpbus_unsubscribe_many(g->shards[k], ids.data(), (uint32_t)ids.size(), st, nullptr);
-        if (rc) return rc;
-        for (size_t j = 0; j < el.size(); j++) {
-          if (st[j] != CPBUS_OK) continue;
-          if (g->K && !g->h_timers.empty())
-            for (uint32_t t = 0; t < g->K; t++) timer_disarm(g, (size_t)(ids[j] - g->base) * g->K + t, /*reset_bound=*/false);
-          g->n_active--;
-        }
-        return CPBUS_OK;
-      });
-} CPBUS_CATCH
-
-int cpbus_group_set_mask_many(cpbus_group_t* g, const uint32_t* sub_ids, const uint32_t* code_masks, uint32_t n, int* status,
-                              uint32_t* applied) try {
-  if (!g || ((!sub_ids || !code_masks) && n)) return CPBUS_EINVAL;
-  std::vector<uint32_t> ids, masks;
-  return group_membership_many(g, n, status, applied,
-      [&](uint32_t i, uint32_t* k) {
-        cpbus* s = nullptr; uint32_t l = 0;
-        if (!group_locate(g, sub_ids[i], &s, &l)) return CPBUS_ENOENT;
-        if (!s->h_active[l]) return CPBUS_ECLOSED;
-        *k = group_shard_of(g, sub_ids[i] - g->base);
-        return CPBUS_OK;
-      },
-      [] {},
-      [&](uint32_t k, const std::vector<uint32_t>& el, int* st) -> int {
-        ids.resize(el.size()); masks.resize(el.size());
-        for (size_t j = 0; j < el.size(); j++) { ids[j] = sub_ids[el[j]]; masks[j] = code_masks[el[j]]; }
-        return cpbus_set_mask_many(g->shards[k], ids.data(), masks.data(), (uint32_t)ids.size(), st, nullptr);
-      });
-} CPBUS_CATCH
-
-int cpbus_group_timer_cancel_many(cpbus_group_t* g, const uint32_t* timer_ids, uint32_t n, int* status, uint32_t* applied) try {
-  if (!g || (!timer_ids && n)) return CPBUS_EINVAL;
-  std::vector<uint32_t> ids;
-  return group_membership_many(g, n, status, applied,
-      [&](uint32_t i, uint32_t* k) {
-        if (!g->K || g->h_timers.empty()) return CPBUS_ENOENT;
-        const uint32_t slot = timer_ids[i] & kTimerSlotMask;
-        if (slot / g->K >= g->n_next) return CPBUS_ENOENT;
-        *k = group_shard_of(g, slot / g->K);
-        return CPBUS_OK;
-      },
-      [&] { group_retire(g); },
-      [&](uint32_t k, const std::vector<uint32_t>& el, int* st) -> int {
-        ids.resize(el.size());   // the shard's own timer ids, as cpbus_group_timer_cancel maps them
-        for (size_t j = 0; j < el.size(); j++)
-          ids[j] = ((timer_ids[el[j]] & kTimerSlotMask) - g->first[k] * g->K) | (timer_ids[el[j]] & ~kTimerSlotMask);
-        const int rc = cpbus_timer_cancel_many(g->shards[k], ids.data(), (uint32_t)ids.size(), st, nullptr);
-        if (rc) return rc;
-        for (size_t j = 0; j < el.size(); j++)
-          if (st[j] == CPBUS_OK) timer_disarm(g, timer_ids[el[j]] & kTimerSlotMask, /*reset_bound=*/true);
-        return CPBUS_OK;
-      });
-} CPBUS_CATCH
-
-int cpbus_group_timer_add_list(cpbus_group_t* g, const cpbus_timer_spec* specs, uint32_t n, uint32_t* timer_ids, int* status,
-                               uint32_t* applied) try {
-  if (!g || (!specs && n)) return CPBUS_EINVAL;
-  std::vector<int> st(n);
-  std::vector<uint32_t> ids(n), shard_ids;
-  std::vector<cpbus_timer_spec> shard_specs;
-  const int rc = group_membership_many(g, n, st.data(), applied,
-      [&](uint32_t i, uint32_t* k) {
-        if (!specs[i].period_ns) return CPBUS_EINVAL;
-        if (!g->K) return CPBUS_ENOSPC;
-        cpbus* s = nullptr; uint32_t l = 0;
-        if (!group_locate(g, specs[i].sub_id, &s, &l)) return CPBUS_ENOENT;
-        *k = group_shard_of(g, specs[i].sub_id - g->base);
-        return CPBUS_OK;
-      },
-      [&] {
-        if (g->h_timers.empty()) g->h_timers.resize((size_t)g->N * g->K);
-        group_retire(g);
-      },
-      [&](uint32_t k, const std::vector<uint32_t>& el, int* st_k) -> int {
-        int rc_k = group_shard_clock(g, g->shards[k]); if (rc_k) return rc_k;
-        shard_specs.resize(el.size()); shard_ids.resize(el.size());
-        for (size_t j = 0; j < el.size(); j++) shard_specs[j] = specs[el[j]];
-        rc_k = cpbus_timer_add_list(g->shards[k], shard_specs.data(), (uint32_t)el.size(), shard_ids.data(), st_k, nullptr);
-        if (rc_k) return rc_k;
-        for (size_t j = 0; j < el.size(); j++) {   // the group's slot and id, as cpbus_group_timer_add maps them
-          if (st_k[j] != CPBUS_OK) continue;
-          const cpbus_timer_spec& s = shard_specs[j];
-          const size_t slot = (size_t)(shard_ids[j] & kTimerSlotMask) + (size_t)g->first[k] * g->K;
-          timer_arm(g, slot, s.period_ns, s.source_id, s.oneshot != 0);
-          ids[el[j]] = (uint32_t)slot | (shard_ids[j] & ~kTimerSlotMask);
-        }
-        return CPBUS_OK;
-      });
-  if (rc) return rc;
-  if (timer_ids)
-    for (uint32_t i = 0; i < n; i++) if (st[i] == CPBUS_OK) timer_ids[i] = ids[i];
-  if (status && n) memcpy(status, st.data(), (size_t)n * sizeof(int));
-  return CPBUS_OK;
-} CPBUS_CATCH
-
-// subscriber id reuse: each shard with work takes its elements, in array order, in one cpbus_release_many call; the group
-// keeps the released global indices in its own free set
-int cpbus_group_release_many(cpbus_group_t* g, const uint32_t* sub_ids, uint32_t n, int* status, uint32_t* applied) try {
-  if (!g || (!sub_ids && n)) return CPBUS_EINVAL;
-  std::vector<uint32_t> ids;
-  return group_membership_many(g, n, status, applied,
-      [&](uint32_t i, uint32_t* k) {
-        cpbus* s = nullptr; uint32_t l = 0;
-        if (!group_locate(g, sub_ids[i], &s, &l)) return CPBUS_ENOENT;
-        if (s->h_active[l]) return CPBUS_EINVAL;
-        *k = group_shard_of(g, sub_ids[i] - g->base);
-        return CPBUS_OK;
-      },
-      [] {},
-      [&](uint32_t k, const std::vector<uint32_t>& el, int* st) -> int {
-        ids.resize(el.size());
-        for (size_t j = 0; j < el.size(); j++) ids[j] = sub_ids[el[j]];
-        const int rc = cpbus_release_many(g->shards[k], ids.data(), (uint32_t)ids.size(), st, nullptr);
-        if (rc) return rc;
-        for (size_t j = 0; j < el.size(); j++)
-          if (st[j] == CPBUS_OK) {
-            g->free_ids.push_back(ids[j] - g->base);
-            std::push_heap(g->free_ids.begin(), g->free_ids.end(), std::greater<uint32_t>());
-          }
-        return CPBUS_OK;
-      });
-} CPBUS_CATCH
-
-// The group hands out the lowest free global ids.  The shards fill in order, so the free ids of shard k's range are its own
-// released ids and its own fresh ones, and the lowest of them are the ones shard k's cpbus_subscribe_list hands out: each
-// shard with work takes its run of elements in one call.
-int cpbus_group_subscribe_list(cpbus_group_t* g, const uint32_t* code_masks, const cpbus_pair* pairs, const uint32_t* n_pairs,
-                               uint32_t n, uint32_t* sub_ids) try {
-  if (!g || !n || !sub_ids || subscribe_list_check(n_pairs, pairs, n)) return CPBUS_EINVAL;
-  if (g->free_ids.size() + (uint64_t)(g->N - g->n_next) < n) return CPBUS_ENOSPC;
-  int rc = flush_staged(g, g->now); if (rc) return rc;
-  std::vector<uint32_t> idx(n);   // global indices, ascending
-  for (uint32_t i = 0; i < n; i++) {
-    if (g->free_ids.empty()) { idx[i] = g->n_next++; continue; }
-    idx[i] = g->free_ids.front();
-    std::pop_heap(g->free_ids.begin(), g->free_ids.end(), std::greater<uint32_t>());
-    g->free_ids.pop_back();
-  }
-  g->n_active += n;
-  for (uint32_t i = 0; i < n;) {
-    const uint32_t k = group_shard_of(g, idx[i]);
-    uint32_t cnt = 1;
-    while (i + cnt < n && idx[i + cnt] < g->first[k + 1]) cnt++;
-    rc = cpbus_subscribe_list(g->shards[k], code_masks ? code_masks + i : nullptr, n_pairs ? pairs + (size_t)i * CPBUS_MAX_PAIRS : nullptr,
-                              n_pairs ? n_pairs + i : nullptr, cnt, sub_ids + i);
-    if (rc) return rc;
-    for (uint32_t j = i; j < i + cnt; j++)
-      if (sub_ids[j] != g->base + idx[j]) return CPBUS_ECUDA;   // cannot happen: the shard's lowest free ids are the group's
-    i += cnt;
-  }
-  return CPBUS_OK;
-} CPBUS_CATCH
-
-int cpbus_group_publish(cpbus_group_t* g, const cpbus_event* ev, size_t n) try {
-  if (!g || (!ev && n)) return CPBUS_EINVAL;
-  return publish_burst(g, ev, n);
-} CPBUS_CATCH
-
-// Device batches on the group: publish_device_impl's rules on the group's host front (flush first, the order and argument
-// checks, lossless all-or-nothing admission on every shard, the single bus's split), each launch one stream batch whose
-// payload shard 0's put stream copies from d_events (group_launch).  The prefetch hints are checked as the single bus checks
-// them; the fan-out kernels read shard 0's stream slot, and throughput-mode stream launches already pull the slot after
-// next, so there is nothing for the hints to add.
-static int group_publish_device(cpbus_group* g, const cpbus_event* d_events, size_t n, uint64_t watermark_ns, bool staged,
-                                const void* d_next, size_t n_next);
-
-// publish_device_split on the group: the records' timestamps are read on the stream of a shard on the batch's GPU
-static int group_publish_device_split(cpbus_group* g, const cpbus_event* d_events, size_t n, uint64_t watermark_ns, bool staged,
-                                      const void* d_next, size_t n_next) {
-  std::vector<uint64_t> ts(n), wm;
-  std::vector<size_t> end;
-  cpbus* s = g->shards[0];
-  if (n) {
-    cudaPointerAttributes a{};
-    CK(cudaPointerGetAttributes(&a, d_events));
-    for (cpbus* x : g->shards) if (x->device == a.device) { s = x; break; }
-    int rc = dev_guard(s); if (rc) return rc;
-    CK(cudaMemcpy2DAsync(ts.data(), 8, reinterpret_cast<const unsigned char*>(d_events) + offsetof(cpbus_event, ts_ns), sizeof(cpbus_event),
-                         8, n, cudaMemcpyDefault, s->stream));
-    CK(cudaStreamSynchronize(s->stream));
-  }
-  int rc = split_plan(ts.data(), n, g->B, g->now, watermark_ns, max_window(g), end, wm);
-  if (rc) return rc;
-  size_t i = 0;
-  for (size_t k = 0; k < end.size(); k++) {
-    const bool last = k + 1 == end.size();
-    rc = group_publish_device(g, d_events + i, end[k] - i, wm[k], staged, last ? d_next : nullptr, last ? n_next : 0);
-    if (rc) return rc;
-    g->shards[0]->st.device_splits++;
-    i = end[k];
-  }
-  return CPBUS_OK;
-}
-
-static int group_publish_device(cpbus_group* g, const cpbus_event* d_events, size_t n, uint64_t watermark_ns, bool staged,
-                                const void* d_next, size_t n_next) {
-  if (!g || (!d_events && n) || ((uintptr_t)d_events & 31u) || n_next > g->B || ((uintptr_t)d_next & 31u)) return CPBUS_EINVAL;
-  int rc = flush_staged(g, g->now); if (rc) return rc;
-  if (watermark_ns < g->now) return CPBUS_EORDER;
-  if (staged && g->lossless) return CPBUS_EINVAL;
-  if (n > g->B || watermark_ns - g->last_watermark > max_window(g)) {
-    if (g->lossless) return n > g->B ? CPBUS_EINVAL : CPBUS_EORDER;
-    return group_publish_device_split(g, d_events, n, watermark_ns, staged, d_next, n_next);
-  }
-  bool ok = true;
-  uint32_t m = (uint32_t)n;
-  if (g->lossless && (rc = group_admit(g, d_events, (uint32_t)n, watermark_ns, &ok, &m))) return rc;
-  if (!ok) return CPBUS_EAGAIN;   // (refused on some shard: nothing was put)
-  g->now = watermark_ns;
-  if ((rc = group_launch(g, d_events, (uint32_t)n, watermark_ns, true))) return rc;
-  g->publishes += n; g->seq += n;
-  return CPBUS_OK;
-}
-
-int cpbus_group_publish_device(cpbus_group_t* g, const void* d_events, size_t n, uint64_t watermark_ns) try {
-  if (g && g->drop_missed) return CPBUS_EINVAL;
-  return group_publish_device(g, (const cpbus_event*)d_events, n, watermark_ns, false, nullptr, 0);
-} CPBUS_CATCH
-
-int cpbus_group_publish_device_staged(cpbus_group_t* g, const void* d_events, size_t n, uint64_t watermark_ns, const void* d_next,
-                                      size_t n_next) try {
-  if (g && g->drop_missed) return CPBUS_EINVAL;
-  return group_publish_device(g, (const cpbus_event*)d_events, n, watermark_ns, true, d_next, n_next);
-} CPBUS_CATCH
-
-int cpbus_group_send(cpbus_group_t* g, uint32_t sub_id, const cpbus_event* ev) try {
-  if (!g || !ev || ev->code >= CPBUS_N_CODES) return CPBUS_EINVAL;
-  cpbus* s = nullptr; uint32_t l = 0;
-  if (!group_locate(g, sub_id, &s, &l)) return CPBUS_ENOENT;
-  if (!s->h_active[l]) return CPBUS_ECLOSED;
-  const int rc = stage_one(g, ev->code, ev->source_id, sub_id, CPBUS_F_UNICAST);
-  if (rc) return rc;
-  g->publishes++;
-  return CPBUS_OK;
-} CPBUS_CATCH
-
-int cpbus_group_advance(cpbus_group_t* g, uint64_t now_ns) try {
-  return g ? advance_clock(g, now_ns) : CPBUS_EINVAL;
-} CPBUS_CATCH
-
-int cpbus_group_flush(cpbus_group_t* g) try {
-  return g ? flush_staged(g, g->now) : CPBUS_EINVAL;
-} CPBUS_CATCH
-
-int cpbus_group_sync(cpbus_group_t* g) try {
-  if (!g) return CPBUS_EINVAL;
-  for (cpbus* s : g->shards) { const int rc = cpbus_sync(s); if (rc) return rc; }
-  return CPBUS_OK;
-} CPBUS_CATCH
-
-int cpbus_group_drain(cpbus_group_t* g, uint32_t sub_id, cpbus_event* out, size_t cap, size_t* n, uint64_t* lost) try {
-  if (!g || !n || (!out && cap)) return CPBUS_EINVAL;
-  cpbus* s = nullptr; uint32_t l = 0;
-  if (!group_locate(g, sub_id, &s, &l)) return CPBUS_ENOENT;
-  return cpbus_drain(s, sub_id, out, cap, n, lost);
-} CPBUS_CATCH
-
-// The first ready mailbox of [a, a + cnt) on shard s (cnt when none): where a walk with no room left stops.
-// take: ready as cpbus_take_ready sees it (records past the take cursor).
-static int group_first_ready(cpbus* s, uint32_t l, uint32_t cnt, uint32_t* at, bool take = false) {
-  std::vector<SubCtl> c(cnt);
-  std::vector<unsigned long long> tk(cnt, 0ull);
-  int rc = dev_guard(s); if (rc) return rc;
-  CK(cudaMemcpyAsync(c.data(), s->d_ctl + l, (size_t)cnt * sizeof(SubCtl), cudaMemcpyDeviceToHost, s->stream));
-  if (take && s->d_taken)
-    CK(cudaMemcpyAsync(tk.data(), s->d_taken + l, (size_t)cnt * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s->stream));
-  CK(cudaStreamSynchronize(s->stream));
-  *at = cnt;
-  for (uint32_t i = 0; i < cnt; i++) if (c[i].tail > std::max<uint64_t>(c[i].head, tk[i])) { *at = i; break; }
-  return CPBUS_OK;
-}
-
-// The cyclic walk of cpbus_drain_ready (take: cpbus_take_ready) over the shards: each piece of the walk that lies on one
-// shard is drained there with the cap and ready entries still left, and the walk stops at the first mailbox that does not
-// fit, as the single call does.  The caller has checked the arguments.
-static int group_drain_ready(cpbus_group* g, uint32_t first_sub, uint32_t n, uint32_t start_sub, cpbus_event* out, size_t cap,
-                             cpbus_ready* ready, size_t ready_cap, size_t* n_ready, size_t* total, uint32_t* next_sub, bool take) {
-  size_t nr = 0, tot = 0, ready_left = std::min<size_t>(ready_cap, n);
-  const int rc = group_walk(g, first_sub, n, start_sub, next_sub, [&](cpbus* s, uint32_t l, uint32_t a, uint32_t cnt) -> int {
-    if (ready_left == 0 || tot == cap) {                           // no room: the next ready mailbox ends the walk
-      uint32_t at = cnt;
-      const int rc_s = group_first_ready(s, l, cnt, &at, take); if (rc_s) return rc_s;
-      if (at == cnt) return CPBUS_OK;
-      *next_sub = a + at;
-      return kWalkEnd;
-    }
-    size_t nr_s = 0, tot_s = 0;
-    uint32_t next_s = a;
-    bool all = false;
-    const int rc_s = drain_ready_impl(s, a, cnt, a, out + tot, cap - tot, ready + nr, ready_left, &nr_s, &tot_s, &next_s, &all,
-                                      take);
-    if (rc_s) return rc_s;
-    for (size_t j = 0; j < nr_s; j++) ready[nr + j].offset += (uint32_t)tot;
-    nr += nr_s; tot += tot_s; ready_left -= nr_s;
-    if (all) return CPBUS_OK;
-    *next_sub = next_s;
-    return kWalkEnd;
-  });
-  if (rc) return rc;
-  *n_ready = nr; *total = tot;
-  return CPBUS_OK;
-}
-
-int cpbus_group_drain_ready(cpbus_group_t* g, uint32_t first_sub, uint32_t n, uint32_t start_sub, cpbus_event* out, size_t cap,
-                            cpbus_ready* ready, size_t ready_cap, size_t* n_ready, size_t* total, uint32_t* next_sub) try {
-  if (!g || !out || !ready || !n_ready || !total || !next_sub || !n || !ready_cap) return CPBUS_EINVAL;
-  if (cap < g->shards[0]->R || cap > 0xFFFFFFFFull) return CPBUS_EINVAL;
-  return group_drain_ready(g, first_sub, n, start_sub, out, cap, ready, ready_cap, n_ready, total, next_sub, false);
-} CPBUS_CATCH
-
-int cpbus_group_take_ready(cpbus_group_t* g, uint32_t first_sub, uint32_t n, uint32_t start_sub, cpbus_event* out, size_t cap,
-                           cpbus_ready* ready, size_t ready_cap, size_t* n_ready, size_t* total, uint32_t* next_sub) try {
-  if (!g || !out || !ready || !n_ready || !total || !next_sub || !n || !ready_cap) return CPBUS_EINVAL;
-  if (cap < g->shards[0]->R || cap > 0xFFFFFFFFull || !g->lossless) return CPBUS_EINVAL;
-  return group_drain_ready(g, first_sub, n, start_sub, out, cap, ready, ready_cap, n_ready, total, next_sub, true);
-} CPBUS_CATCH
-
-// Each shard with work takes its elements, in array order, in one cpbus_ack_many call; shards hold disjoint mailboxes, so
-// the statuses are the single bus's.
-int cpbus_group_ack_many(cpbus_group_t* g, const uint32_t* sub_ids, const uint32_t* counts, uint32_t n, int* status,
-                         uint32_t* applied) try {
-  if (!g || ((!sub_ids || !counts) && n)) return CPBUS_EINVAL;
-  if (n == 0) {
-    if (applied) *applied = 0;
-    return CPBUS_OK;
-  }
-  if (!g->lossless) return CPBUS_EINVAL;
-  std::vector<int> st(n);
-  std::vector<std::vector<uint32_t>> work(g->shards.size());
-  for (uint32_t i = 0; i < n; i++) {
-    cpbus* s = nullptr; uint32_t l = 0;
-    if (!group_locate(g, sub_ids[i], &s, &l)) st[i] = CPBUS_ENOENT;
-    else work[group_shard_of(g, sub_ids[i] - g->base)].push_back(i);
-  }
-  std::vector<uint32_t> ids, cnts;
-  std::vector<int> st_k;
-  for (uint32_t k = 0; k < g->shards.size(); k++) {
-    if (work[k].empty()) continue;
-    ids.resize(work[k].size()); cnts.resize(work[k].size()); st_k.resize(work[k].size());
-    for (size_t j = 0; j < work[k].size(); j++) { ids[j] = sub_ids[work[k][j]]; cnts[j] = counts[work[k][j]]; }
-    const int rc = ack_many_impl(g->shards[k], ids.data(), cnts.data(), (uint32_t)ids.size(), st_k.data());
-    if (rc) return rc;
-    for (size_t j = 0; j < work[k].size(); j++) st[work[k][j]] = st_k[j];
-  }
-  ack_statuses(st, status, applied);
-  return CPBUS_OK;
-} CPBUS_CATCH
-
-// The cyclic walk of cpbus_lagging over the shards: each piece on one shard is scanned with the cap still left; the first
-// piece that could not return all of its lagging mailboxes sets next_sub, and every piece adds to the summary.
-int cpbus_group_lagging(cpbus_group_t* g, uint32_t first_sub, uint32_t n, uint32_t start_sub, uint32_t min_backlog, cpbus_lag* out,
-                        size_t cap, size_t* n_out, uint32_t* next_sub, cpbus_lag_summary* sum) try {
-  if (!g || !n_out || !next_sub || !n || (!out && cap)) return CPBUS_EINVAL;
-  cpbus_lag_summary acc{};
-  size_t got = 0;
-  bool cut = false;
-  const int rc = group_walk(g, first_sub, n, start_sub, next_sub, [&](cpbus* s, uint32_t, uint32_t a, uint32_t cnt) -> int {
-    cpbus_lag_summary part{};
-    size_t n_s = 0;
-    uint32_t next_s = a;
-    bool all = false;
-    const int rc_s = lagging_impl(s, a, cnt, a, min_backlog, out ? out + got : nullptr, cap - got, &n_s, &next_s, &part, &all);
-    if (rc_s) return rc_s;
-    got += n_s;
-    if (!all && !cut) { *next_sub = next_s; cut = true; }
-    acc.active += part.active; acc.lagging += part.lagging; acc.backlog_total += part.backlog_total;
-    acc.backlog_max = std::max(acc.backlog_max, part.backlog_max); acc.lost_total += part.lost_total;
-    for (int h = 0; h < 33; h++) acc.hist[h] += part.hist[h];
-    return CPBUS_OK;
-  });
-  if (rc) return rc;
-  *n_out = got;
-  if (sum) *sum = acc;
-  return CPBUS_OK;
-} CPBUS_CATCH
-
-// The group's next unit (its staged remainder and clock, as cpbus_blockers reads the single bus's) on every shard; the
-// shards own ascending id ranges, so their lists concatenate in ascending order.
-int cpbus_group_blockers(cpbus_group_t* g, uint32_t* out, size_t cap, size_t* n) try {
-  if (!g || !n || (!out && cap)) return CPBUS_EINVAL;
-  *n = 0;
-  if (!g->lossless) return CPBUS_OK;
-  const cpbus_event* rec = g->n_staged ? &g->staged[0] : nullptr;
-  if (!rec && (g->n_timers == 0 || g->now == g->last_watermark)) return CPBUS_OK;   // the next flush launches nothing
-  const uint64_t t = rec ? rec->ts_ns : g->now;
-  size_t tot = 0;
-  for (cpbus* s : g->shards) {
-    std::lock_guard<std::mutex> lk(s->mu);
-    int rc = enter(s); if (rc) return rc;
-    const size_t used = std::min(tot, cap);
-    size_t n_s = 0;
-    if ((rc = blockers_impl(s, rec, t, out ? out + used : nullptr, cap - used, &n_s))) return rc;
-    tot += n_s;
-  }
-  *n = tot;
-  return CPBUS_OK;
-} CPBUS_CATCH
-
-int cpbus_group_consume_all(cpbus_group_t* g) try {
-  if (!g) return CPBUS_EINVAL;
-  for (cpbus* s : g->shards) { const int rc = cpbus_consume_all(s); if (rc) return rc; }
-  return CPBUS_OK;
-} CPBUS_CATCH
-
-int cpbus_group_peek_window(cpbus_group_t* g, uint32_t sub_id, cpbus_event* out, size_t cap, size_t* n) try {
-  if (!g || !n || (!out && cap)) return CPBUS_EINVAL;
-  cpbus* s = nullptr; uint32_t l = 0;
-  if (!group_locate(g, sub_id, &s, &l)) return CPBUS_ENOENT;
-  return cpbus_peek_window(s, sub_id, out, cap, n);
-} CPBUS_CATCH
-
-int cpbus_group_digest(cpbus_group_t* g, uint32_t first_sub, uint32_t n, cpbus_digest_t* out) try {
-  if (!g || !out || !n) return CPBUS_EINVAL;
-  uint32_t i0 = 0;
-  if (!id_range(g->base, g->n_next, first_sub, n, &i0)) return CPBUS_ENOENT;
-  return group_each_range(g, i0, n, [&](cpbus* s, uint32_t l, uint32_t off, uint32_t cnt) -> int {
-    return cpbus_digest(s, s->cfg.sub_id_base + l, cnt, out + off);
-  });
-} CPBUS_CATCH
-
-int cpbus_group_digest_fold(cpbus_group_t* g, uint32_t first_sub, uint32_t n, uint64_t out[4]) try {
-  if (!g || !out || !n) return CPBUS_EINVAL;
-  uint32_t i0 = 0;
-  if (!id_range(g->base, g->n_next, first_sub, n, &i0)) return CPBUS_ENOENT;
-  uint64_t acc[4] = {0, 0, 0, 0};
-  const int rc = group_each_range(g, i0, n, [&](cpbus* s, uint32_t l, uint32_t, uint32_t cnt) -> int {
-    uint64_t part[4];
-    const int rc_s = cpbus_digest_fold(s, s->cfg.sub_id_base + l, cnt, part);
-    if (rc_s) return rc_s;
-    acc[0] += part[0]; acc[1] += part[1]; acc[2] ^= part[2]; acc[3] += part[3];   // sums add, the hash term XORs
-    return CPBUS_OK;
-  });
-  if (rc) return rc;
-  for (int j = 0; j < 4; j++) out[j] = acc[j];
-  return CPBUS_OK;
-} CPBUS_CATCH
-
-int cpbus_group_debug_events(cpbus_group_t* g, cpbus_event* out, size_t cap, size_t* n) try {   // cpbus_debug_events
-  if (!g || !n || (!out && cap)) return CPBUS_EINVAL;
-  const int rc = dbg_resolve(g, g->shards[0]); if (rc) return rc;
-  *n = dbg_read(g, out, cap);
-  return CPBUS_OK;
-} CPBUS_CATCH
-
-int cpbus_group_stats(cpbus_group_t* g, cpbus_stats_t* out) try {
-  if (!g || !out) return CPBUS_EINVAL;
-  cpbus_stats_t sum{}, s0{};
-  for (cpbus* s : g->shards) {
-    cpbus_stats_t x{};
-    const int rc = cpbus_stats(s, &x); if (rc) return rc;
-    if (s == g->shards[0]) s0 = x;   // the intern table's figures
-    sum.deliveries += x.deliveries; sum.ticks += x.ticks; sum.overwritten += x.overwritten;
-    sum.batches += x.batches; sum.kernel_launches += x.kernel_launches; sum.device_splits += x.device_splits;
-    sum.admit_passes += x.admit_passes; sum.admit_skipped += x.admit_skipped; sum.admit_partial += x.admit_partial;
-  }
-  group_retire(g);
-  sum.publishes = g->publishes;
-  for (int c = 0; c < CPBUS_N_CODES; c++)   // + device batches, accounted by shard 0's launches alone (group_launch)
-    sum.published_by_code[c] = g->published_by_code[c] + s0.published_by_code[c];
-  sum.n_subs = g->n_active; sum.n_timers = g->n_timers; sum.now_ns = g->now;
-  sum.intern_entries = s0.intern_entries; sum.intern_bytes = s0.intern_bytes;
-  sum.ephemeral_live = s0.ephemeral_live; sum.ephemeral_recycled = s0.ephemeral_recycled;
-  *out = sum;
-  return CPBUS_OK;
-} CPBUS_CATCH
-
-int cpbus_group_publish_counts(cpbus_group_t* g, cpbus_pair_count* out, size_t cap, size_t* n) try {
-  if (!g || !n || (!out && cap)) return CPBUS_EINVAL;
-  std::vector<unsigned long long> keys, cnts;
-  if (g->dev_counted) {
-    int rc = dev_guard(g->shards[0]);
-    if (rc || (rc = device_pairs(g->shards[0], keys, cnts))) return rc;
-  }
-  pair_counts(g, keys.data(), cnts.data(), keys.size(), out, cap, n);
-  return CPBUS_OK;
-} CPBUS_CATCH
-
-}  // extern "C"

@@ -266,6 +266,40 @@ __host__ __device__ inline uint64_t pow_p(uint32_t e) {
   return r;
 }
 
+// ---- the op lists the host fills for a membership, arming or slot-reset kernel ----
+// The bulk membership calls (cpbus_unsubscribe_many, cpbus_set_mask_many, cpbus_timer_cancel_many): one entry per mailbox,
+// its final state after the call.  The host coalesces every element that touches a mailbox into one entry, so no two threads
+// write one mailbox.
+struct __align__(16) MemberOp {
+  uint32_t local;        // mailbox (shard-local index)
+  uint32_t mask_word;    // its control block's mask word, as mask_word() leaves it
+  uint32_t clear_slots;  // bit k: timer slot k is disarmed (every byte 0xFF, as cpbus_create leaves an idle slot)
+  uint32_t pad;
+};
+
+// Bulk timer arming (cpbus_timer_add_list): one entry per armed slot.  A slot appears at most once per call (an arm list
+// holds no cancels, and nothing fires between its elements), and the entries of one mailbox carry the same final mask word.
+struct __align__(16) TimerArmOp {
+  uint64_t next_due;     // the slot's first due time, as timer_arm sets it
+  uint64_t period;       // 0 for a one-shot
+  uint32_t source_id;
+  uint32_t slot;         // shard-local timer slot (mailbox * K + k)
+  uint32_t local;        // its mailbox
+  uint32_t mask_word;    // the mailbox's control-block mask word after the whole call, as mask_word() leaves it
+};
+static_assert(sizeof(TimerArmOp) == 32, "timer_arm_kernel reads an entry as two 16-byte words");
+
+// Subscriber id reuse (cpbus_release_many, cpbus_subscribe_list): one entry per mailbox, the state a fresh subscription finds
+// in a slot that was never handed out, with the new occupant's mask word (0 for a release).  The pair-table rows of the
+// entries with cases follow the entries in the same list, CPBUS_MAX_PAIRS per row.
+constexpr uint32_t kResetNoRow = 0xFFFFFFFFu;
+struct __align__(16) SlotResetOp {
+  uint32_t local;       // mailbox (shard-local index)
+  uint32_t mask_word;   // its control block's mask word, as mask_word() leaves it
+  uint32_t row;         // its cases in `rows` (kResetNoRow: none, every pair slot unused)
+  uint32_t pad;
+};
+
 #ifdef __CUDACC__
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ uint64_t shfl64(uint64_t v, int src) {
@@ -1177,16 +1211,6 @@ __global__ void __launch_bounds__(kThreads) timer_catchup_kernel(DevTimer* __res
   tp->fired += (uint32_t)k;
 }
 
-// The bulk membership calls (cpbus_unsubscribe_many, cpbus_set_mask_many, cpbus_timer_cancel_many): one entry per mailbox,
-// its final state after the call.  The host coalesces every element that touches a mailbox into one entry, so no two threads
-// write one mailbox.
-struct __align__(16) MemberOp {
-  uint32_t local;        // mailbox (shard-local index)
-  uint32_t mask_word;    // its control block's mask word, as mask_word() leaves it
-  uint32_t clear_slots;  // bit k: timer slot k is disarmed (every byte 0xFF, as cpbus_create leaves an idle slot)
-  uint32_t pad;
-};
-
 // One thread per entry: the mask word, then the cleared timer slots.  The ring, tail, head and digest are not touched.
 __global__ void __launch_bounds__(kThreads) membership_kernel(SubCtl* __restrict__ ctl, DevTimer* __restrict__ timers,
                                                               const MemberOp* __restrict__ ops, uint32_t n, uint32_t K) {
@@ -1202,17 +1226,6 @@ __global__ void __launch_bounds__(kThreads) membership_kernel(SubCtl* __restrict
     }
 }
 
-// Bulk timer arming (cpbus_timer_add_list): one entry per armed slot.  A slot appears at most once per call (an arm list
-// holds no cancels, and nothing fires between its elements), and the entries of one mailbox carry the same final mask word.
-struct __align__(16) TimerArmOp {
-  uint64_t next_due;     // the slot's first due time, as timer_arm sets it
-  uint64_t period;       // 0 for a one-shot
-  uint32_t source_id;
-  uint32_t slot;         // shard-local timer slot (mailbox * K + k)
-  uint32_t local;        // its mailbox
-  uint32_t mask_word;    // the mailbox's control-block mask word after the whole call, as mask_word() leaves it
-};
-
 // One thread per entry: the slot's whole DevTimer image (what cpbus_timer_add copies: fired and pad 0) in two 16-byte
 // stores, then the mailbox's mask word.  The ring, tail, head and digest are not touched.
 __global__ void __launch_bounds__(kThreads) timer_arm_kernel(SubCtl* __restrict__ ctl, DevTimer* __restrict__ timers,
@@ -1226,17 +1239,6 @@ __global__ void __launch_bounds__(kThreads) timer_arm_kernel(SubCtl* __restrict_
   tp[1] = make_uint4(hi.x, 0u, 0u, 0u);
   ctl[hi.z].mask = hi.w;
 }
-
-// Subscriber id reuse (cpbus_release_many, cpbus_subscribe_list): one entry per mailbox, the state a fresh subscription finds
-// in a slot that was never handed out, with the new occupant's mask word (0 for a release).  The pair-table rows of the
-// entries with cases follow the entries in the same list, CPBUS_MAX_PAIRS per row.
-constexpr uint32_t kResetNoRow = 0xFFFFFFFFu;
-struct __align__(16) SlotResetOp {
-  uint32_t local;       // mailbox (shard-local index)
-  uint32_t mask_word;   // its control block's mask word, as mask_word() leaves it
-  uint32_t row;         // its cases in `rows` (kResetNoRow: none, every pair slot unused)
-  uint32_t pad;
-};
 
 // One thread per entry: the whole control block (tail, head, digest 0: the ring's records are unreachable, and no read goes
 // behind head or below tail - ring_cap), the take cursor, the pair-table row and the K timer slots (idle, every byte 0xFF).
