@@ -139,6 +139,10 @@ SYMBOLS = {
     "cpbus_take_ready": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p,
                                    C.c_size_t, _P(C.c_size_t), _P(C.c_size_t), _P(C.c_uint32)]),
     "cpbus_ack_many": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, _P(C.c_uint32)]),
+    "cpbus_drain_ready_begin": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_size_t, C.c_size_t, _P(C.c_uint32)]),
+    "cpbus_take_ready_begin": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_size_t, C.c_size_t, _P(C.c_uint32)]),
+    "cpbus_drain_ready_end": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, _P(C.c_size_t),
+                                        _P(C.c_size_t), _P(C.c_uint32)]),
     "cpbus_lagging": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t,
                                 _P(C.c_size_t), _P(C.c_uint32), _P(LagSummary)]),
     "cpbus_blockers": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, _P(C.c_size_t)]),

@@ -19,6 +19,20 @@ READY_DTYPE = np.dtype([("sub_id", "<u4"), ("count", "<u4"), ("offset", "<u4"), 
 assert READY_DTYPE.itemsize == 24
 
 
+class _SingleBusOnly:
+    """A `Bus` method that `GroupBus` does not have (the group has no C twin of it): on a class that sets `_GROUP`, and
+    its instances, the name does not exist."""
+
+    def __init__(self, fn):
+        self._fn = fn
+        self.__doc__, self.__name__ = fn.__doc__, fn.__name__
+
+    def __get__(self, obj, owner=None):
+        if getattr(owner if owner is not None else type(obj), "_GROUP", False):
+            raise AttributeError(f"{self.__name__} has no cpbus_group_* counterpart")
+        return self._fn if obj is None else self._fn.__get__(obj, owner)
+
+
 class Bus:
     def __init__(self, n_max_subs: int, ring_cap: int = 1024, batch_cap: int = 256, timers_per_sub: int = 0,
                  lossless: bool = False, digest: bool = True, device: int = -1, sub_id_base: int = 0,
@@ -379,6 +393,41 @@ class Bus:
         n_ready, total, next_sub = C.c_size_t(), C.c_size_t(), C.c_uint32()
         nat.check(getattr(self._lib, name)(self._h, first_sub, n, start_sub, out.ctypes.data, cap, ready.ctypes.data,
                                            ready_cap, C.byref(n_ready), C.byref(total), C.byref(next_sub)), name)
+        return out[: total.value], ready[: n_ready.value], next_sub.value
+
+    @_SingleBusOnly
+    def drain_ready_begin(self, first_sub: int, n: int, start_sub: int, cap: int, ready_cap: int) -> int:
+        """drain_ready enqueued on the bus stream: returns a ticket for drain_ready_end, which returns what drain_ready
+        would have returned here.  At most 8 tickets are outstanding (a 9th begin raises with ENOSPC)."""
+        return self._ready_begin("cpbus_drain_ready_begin", first_sub, n, start_sub, cap, ready_cap)
+
+    @_SingleBusOnly
+    def take_ready_begin(self, first_sub: int, n: int, start_sub: int, cap: int, ready_cap: int) -> int:
+        """Lossless mode: take_ready enqueued on the bus stream; collect it with drain_ready_end."""
+        return self._ready_begin("cpbus_take_ready_begin", first_sub, n, start_sub, cap, ready_cap)
+
+    def _ready_begin(self, name: str, first_sub: int, n: int, start_sub: int, cap: int, ready_cap: int) -> int:
+        t = C.c_uint32()
+        nat.check(getattr(self._lib, name)(self._h, first_sub, n, start_sub, cap, ready_cap, C.byref(t)), name)
+        # the entries _end can return: min(ready_cap, n), as drain_ready sizes its list
+        self.__dict__.setdefault("_ticket_rows", {})[t.value] = min(ready_cap, n)
+        return t.value
+
+    @_SingleBusOnly
+    def drain_ready_end(self, ticket: int, cap: int, ready_cap: int, out=None):
+        """Waits for the ticket of drain_ready_begin or take_ready_begin and returns (records, ready, next_sub), as
+        drain_ready does; cap and ready_cap are at least the begin's.  `out`: a preallocated EVENT_DTYPE array of at least
+        `cap` records; records is a view of it."""
+        if out is None:
+            out = np.zeros(cap, dtype=EVENT_DTYPE)
+        if len(out) < cap:
+            raise ValueError("out holds fewer than cap records")
+        rows = self.__dict__.get("_ticket_rows", {})
+        ready = np.zeros(max(1, min(ready_cap, rows.get(ticket, ready_cap))), dtype=READY_DTYPE)
+        n_ready, total, next_sub = C.c_size_t(), C.c_size_t(), C.c_uint32()
+        nat.check(self._lib.cpbus_drain_ready_end(self._h, ticket, out.ctypes.data, cap, ready.ctypes.data, ready_cap,
+                                                  C.byref(n_ready), C.byref(total), C.byref(next_sub)), "cpbus_drain_ready_end")
+        rows.pop(ticket, None)
         return out[: total.value], ready[: n_ready.value], next_sub.value
 
     def ack_many(self, sub_ids, counts) -> np.ndarray:

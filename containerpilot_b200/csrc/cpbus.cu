@@ -2189,28 +2189,27 @@ int cpbus_take_ready(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start_
   return drain_ready_impl(b, first_sub, n, start_sub, out, cap, ready, ready_cap, n_ready, total, next_sub, &all_taken, true);
 } CPBUS_CATCH
 
-// The body of cpbus_drain_ready, without its cap >= ring_cap check: a group hands each shard the cap its earlier shards
-// left, which can be smaller.  *all_taken: every ready mailbox of the range was taken (then *next_sub = start_sub).
-// take: cpbus_take_ready's scan (the caller has checked that the bus is lossless).
-int cpbus_host::drain_ready_impl(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start_sub, cpbus_event* out, size_t cap,
-                                 cpbus_ready* ready, size_t ready_cap, size_t* n_ready, size_t* total, uint32_t* next_sub,
-                                 bool* all_taken, bool take) {
+// The checks every sparse drain makes after its own: start_sub within the range (CPBUS_EINVAL), and the range within this
+// shard (CPBUS_ENOENT); *l = the range's first mailbox.
+static int ready_range(const cpbus* b, uint32_t first_sub, uint32_t n, uint32_t start_sub, uint32_t* l) {
   if (start_sub < first_sub || start_sub - first_sub >= n) return CPBUS_EINVAL;
-  uint32_t l = 0;
-  if (!id_range(b->cfg.sub_id_base, b->n_next, first_sub, n, &l)) return CPBUS_ENOENT;
-  std::lock_guard<std::mutex> g(b->mu);
+  return id_range(b->cfg.sub_id_base, b->n_next, first_sub, n, l) ? CPBUS_OK : CPBUS_ENOENT;
+}
+
+// The host part of every sparse drain, synchronous or ticketed, up to its gather (the caller holds b->mu): resolution, the
+// device scratch and the scan of mailboxes [l, l + n) from position rot, with at most rcap entries.  The gathers of
+// outstanding tickets may still read the scratch on the bus stream, so a scratch buffer that has to grow while a ticket is
+// outstanding waits for the stream first.
+static int ready_scan_enqueue(cpbus* b, uint32_t l, uint32_t n, uint32_t rot, size_t cap, size_t rcap, bool take) {
   int rc = enter(b); if (rc) return rc;
-  const size_t rcap = std::min<size_t>(ready_cap, n);   // never more entries than mailboxes
   const uint32_t tiles = (n + kReadyTile - 1) / kReadyTile;
-  // the records share cpbus_drain_many's buffer
-  CK(b->d_drain.grow(cap));
+  const size_t lb_words = kReadyLbOffset + (size_t)tiles;
+  if (b->drain_tk_busy && (rcap > b->d_ready.size() || rcap > b->d_ready_slot.size() || lb_words > b->d_ready_lb.size()))
+    CK(cudaStreamSynchronize(b->stream));
   CK(b->d_ready.grow(rcap));
   CK(b->d_ready_slot.grow(rcap));
-  CK(b->d_ready_lb.grow(kReadyLbOffset + (size_t)tiles));
-  CK(b->h_ready_hdr.grow(8));
-  CK(cudaMemsetAsync(b->d_ready_lb + kReadyHdrWords, 0, (kReadyLbOffset - kReadyHdrWords + (size_t)tiles) * sizeof(unsigned long long),
-                     b->stream));
-  const uint32_t rot = start_sub - first_sub;
+  CK(b->d_ready_lb.grow(lb_words));
+  CK(cudaMemsetAsync(b->d_ready_lb + kReadyHdrWords, 0, (lb_words - kReadyHdrWords) * sizeof(unsigned long long), b->stream));
   if (take) {
     if (!b->d_taken) {   // every cursor 0: max(0, head) = head, so nothing is held
       CK(b->d_taken.alloc(b->N));
@@ -2223,6 +2222,25 @@ int cpbus_host::drain_ready_impl(cpbus_t* b, uint32_t first_sub, uint32_t n, uin
                                                                 cap, rcap, b->d_ready_lb, b->d_ready, b->d_ready_slot);
   }
   CK(cudaGetLastError());
+  return CPBUS_OK;
+}
+
+// The body of cpbus_drain_ready, without its cap >= ring_cap check: a group hands each shard the cap its earlier shards
+// left, which can be smaller.  *all_taken: every ready mailbox of the range was taken (then *next_sub = start_sub).
+// take: cpbus_take_ready's scan (the caller has checked that the bus is lossless).
+int cpbus_host::drain_ready_impl(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start_sub, cpbus_event* out, size_t cap,
+                                 cpbus_ready* ready, size_t ready_cap, size_t* n_ready, size_t* total, uint32_t* next_sub,
+                                 bool* all_taken, bool take) {
+  uint32_t l = 0;
+  int rc = ready_range(b, first_sub, n, start_sub, &l); if (rc) return rc;
+  std::lock_guard<std::mutex> g(b->mu);
+  const size_t rcap = std::min<size_t>(ready_cap, n);   // never more entries than mailboxes
+  const uint32_t rot = start_sub - first_sub;
+  // the records share cpbus_drain_many's buffer; allocated before the scan, so that a refusal leaves every mailbox as it was
+  if ((rc = dev_guard(b))) return rc;
+  CK(b->d_drain.grow(cap));
+  CK(b->h_ready_hdr.grow(8));
+  if ((rc = ready_scan_enqueue(b, l, n, rot, cap, rcap, take))) return rc;
   const uint32_t gather_grid = (uint32_t)std::min<size_t>((size_t)b->sm_count * 4, (rcap + kWarpsPerCta - 1) / kWarpsPerCta);
   drain_ready_gather_kernel<<<gather_grid, kThreads, 0, b->stream>>>(b->d_ring, b->R, b->cfg.sub_id_base, b->d_ready,
                                                                       b->d_ready_slot, b->d_ready_lb, b->d_drain, b->h_ready_hdr.dev());
@@ -2241,6 +2259,80 @@ int cpbus_host::drain_ready_impl(cpbus_t* b, uint32_t first_sub, uint32_t n, uin
   *next_sub = cut >= n ? start_sub : first_sub + (uint32_t)((rot + cut) % n);
   return CPBUS_OK;
 }
+
+// Drain tickets: the scan of the synchronous call, then a gather that writes the records, the ready list and the header
+// into the ticket's mapped host buffer; _end waits for the ticket's event and copies them out.
+constexpr size_t kTicketHdrBytes = 128;   // the records start on a 128-byte line of the buffer
+
+static int drain_ready_begin(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start_sub, size_t cap, size_t ready_cap,
+                             uint32_t* ticket, bool take) {
+  if (!b || !ticket || !n || !ready_cap) return CPBUS_EINVAL;
+  if (cap < b->R || cap > 0xFFFFFFFFull || (take && !b->lossless)) return CPBUS_EINVAL;
+  uint32_t l = 0;
+  int rc = ready_range(b, first_sub, n, start_sub, &l); if (rc) return rc;
+  std::lock_guard<std::mutex> g(b->mu);
+  if (b->drain_tk_busy == (uint32_t)cpbus::kDrainTickets) return CPBUS_ENOSPC;   // no result is ever overwritten
+  uint32_t i = 0;
+  while (b->drain_tk[i].busy) i++;
+  cpbus::DrainTicket& t = b->drain_tk[i];
+  const size_t rcap = std::min<size_t>(ready_cap, n);
+  const size_t rec_bytes = cap * sizeof(cpbus_event);
+  // the slot is free: no kernel writes its buffer, which may be replaced
+  if ((rc = dev_guard(b))) return rc;
+  CK(t.buf.grow(kTicketHdrBytes + rec_bytes + rcap * sizeof(cpbus_ready)));
+  if (!(cudaEvent_t)t.done) CK(t.done.create());
+  const uint32_t rot = start_sub - first_sub;
+  if ((rc = ready_scan_enqueue(b, l, n, rot, cap, rcap, take))) return rc;
+  unsigned char* d = t.buf.dev();
+  const uint32_t grid = (uint32_t)std::min<size_t>((size_t)b->sm_count * 4, ((cap + 15) / 16 + kWarpsPerCta - 1) / kWarpsPerCta);
+  drain_ready_ticket_gather_kernel<<<grid, kThreads, 0, b->stream>>>(
+      b->d_ring, b->R, b->cfg.sub_id_base, b->d_ready, b->d_ready_slot, b->d_ready_lb,
+      reinterpret_cast<unsigned long long*>(d), reinterpret_cast<uint4*>(d + kTicketHdrBytes),
+      reinterpret_cast<uint2*>(d + kTicketHdrBytes + rec_bytes));
+  CK(cudaGetLastError());
+  b->st.kernel_launches += 2;
+  CK(cudaEventRecord(t.done, b->stream));
+  t.busy = true;
+  b->drain_tk_busy++;
+  t.ticket = (b->drain_tk_gen++ & 0x1FFFFFFFu) << 3 | i;
+  t.first = first_sub; t.n = n; t.start = start_sub; t.cap = cap; t.ready_cap = ready_cap;
+  *ticket = t.ticket;
+  return CPBUS_OK;
+}
+
+int cpbus_drain_ready_begin(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start_sub, size_t cap, size_t ready_cap,
+                            uint32_t* ticket) try {
+  return drain_ready_begin(b, first_sub, n, start_sub, cap, ready_cap, ticket, false);
+} CPBUS_CATCH
+
+int cpbus_take_ready_begin(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start_sub, size_t cap, size_t ready_cap,
+                           uint32_t* ticket) try {
+  return drain_ready_begin(b, first_sub, n, start_sub, cap, ready_cap, ticket, true);
+} CPBUS_CATCH
+
+int cpbus_drain_ready_end(cpbus_t* b, uint32_t ticket, cpbus_event* out, size_t cap, cpbus_ready* ready, size_t ready_cap,
+                          size_t* n_ready, size_t* total, uint32_t* next_sub) try {
+  if (!b || !out || !ready || !n_ready || !total || !next_sub) return CPBUS_EINVAL;
+  std::lock_guard<std::mutex> g(b->mu);
+  cpbus::DrainTicket& t = b->drain_tk[ticket % cpbus::kDrainTickets];
+  if (!t.busy || t.ticket != ticket) return CPBUS_ENOENT;
+  if (cap < t.cap || ready_cap < t.ready_cap) return CPBUS_EINVAL;   // the ticket stays outstanding
+  int rc = dev_guard(b); if (rc) return rc;
+  CK(cudaEventSynchronize(t.done));
+  const unsigned char* h = t.buf.get();
+  const volatile unsigned long long* hdr = reinterpret_cast<const volatile unsigned long long*>(h);
+  const size_t nr = (size_t)hdr[0], tot = (size_t)hdr[1];
+  const uint64_t cut = hdr[2];
+  if (nr) {
+    memcpy(ready, h + kTicketHdrBytes + t.cap * sizeof(cpbus_event), nr * sizeof(cpbus_ready));
+    memcpy(out, h + kTicketHdrBytes, tot * sizeof(cpbus_event));
+  }
+  *n_ready = nr; *total = tot;
+  *next_sub = cut >= t.n ? t.start : t.first + (uint32_t)(((uint64_t)(t.start - t.first) + cut) % t.n);
+  t.busy = false;
+  b->drain_tk_busy--;
+  return CPBUS_OK;
+} CPBUS_CATCH
 
 // cpbus_ack_many on one bus (the caller has checked the arguments and that the bus is lossless): st[i] for every element.
 // Unknown ids get CPBUS_ENOENT and count 0 gets CPBUS_OK on the host; the others go to ack_kernel, one entry per mailbox

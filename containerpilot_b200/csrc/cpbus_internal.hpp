@@ -163,10 +163,23 @@ struct cpbus : HostFront {
   DeviceBuf<cpbus_event> d_drain;             // cpbus_drain_many staging (grown)
   DeviceBuf<uint2> d_drain_idx;
   // cpbus_drain_ready staging (records go to d_drain; grown): header + tile counter + tile status, ready list, ring
-  // slot of each run, and the header the gather kernel hands to the host
+  // slot of each run, and the header the gather kernel hands to the host.  Drain tickets share the first three.
   DeviceBuf<unsigned long long> d_ready_lb;
   DeviceBuf<cpbus_ready> d_ready; DeviceBuf<uint32_t> d_ready_slot;
   MappedBuf<unsigned long long> h_ready_hdr;
+  // drain tickets (cpbus_drain_ready_begin, cpbus_take_ready_begin, cpbus_drain_ready_end): per slot, the mapped host buffer
+  // the ticket gather kernel writes ([header, 128 bytes | cap records | min(ready_cap, n) entries], grown only while the
+  // slot is free), the event recorded behind that kernel, and what _end needs.  ticket = generation << 3 | slot.
+  static constexpr int kDrainTickets = 8;
+  struct DrainTicket {
+    MappedBuf<unsigned char> buf;
+    CudaEvent done;
+    bool busy = false;
+    uint32_t ticket = 0, first = 0, n = 0, start = 0;
+    size_t cap = 0, ready_cap = 0;
+  };
+  DrainTicket drain_tk[kDrainTickets];
+  uint32_t drain_tk_gen = 0, drain_tk_busy = 0;
   // cpbus_lagging / cpbus_blockers: look-back and summary words sized for every subscriber, the header the scans hand to the
   // host, the blocker ids (lossless buses) and the lagging entries (grown)
   DeviceBuf<unsigned long long> d_lag_lb;

@@ -809,6 +809,56 @@ __global__ void __launch_bounds__(kThreads) drain_ready_gather_kernel(const cpbu
   }
 }
 
+// The gather of a drain ticket (cpbus_drain_ready_begin, cpbus_take_ready_begin): the taken runs, the ready list and the
+// header go straight into the ticket's mapped host buffer, so every store crosses the host link.  The records are cut
+// into chunks of 16 (512 bytes: four whole 128-byte lines of the output, which starts on a line), and each warp stores a
+// contiguous range of chunks, whatever the runs' lengths: lane pair p stores record 16c + p of chunk c.  A chunk's
+// records lie in at most 16 consecutive entries (every run holds one record or more), so the warp loads that window of
+// entries once per chunk and each lane finds its own entry among them with shuffles.  The next chunk starts in the entry
+// of this chunk's last record, or in the one after it when that run ends with the chunk.  The ready list is copied as
+// flat 8-byte words, and the header {taken mailboxes, records, cut} by the first threads.
+__global__ void __launch_bounds__(kThreads) drain_ready_ticket_gather_kernel(const cpbus_event* __restrict__ ring,
+                                                                             uint32_t ring_cap, uint32_t sub_base,
+                                                                             const cpbus_ready* __restrict__ ready,
+                                                                             const uint32_t* __restrict__ slot,
+                                                                             const unsigned long long* __restrict__ hdr,
+                                                                             unsigned long long* h_hdr, uint4* h_rec,
+                                                                             uint2* h_ent) {
+  const uint32_t n_ready = (uint32_t)hdr[0], total = (uint32_t)hdr[1];   // both below 2^32: at most n and cap
+  const uint32_t tid = blockIdx.x * blockDim.x + threadIdx.x, nt = gridDim.x * blockDim.x;
+  if (tid < 3) h_hdr[tid] = hdr[tid];
+  const uint2* ent = reinterpret_cast<const uint2*>(ready);
+  for (uint32_t i = tid; i < 3 * n_ready; i += nt) h_ent[i] = ent[i];
+  const uint32_t lane = threadIdx.x & 31, half = lane & 1, nw = nt >> 5;
+  const uint32_t chunks = (total + 15) >> 4, per = (chunks + nw - 1) / nw;
+  uint32_t c = (tid >> 5) * per;
+  const uint32_t c_end = min(c + per, chunks);
+  if (c >= c_end) return;
+  uint32_t e = 0, hi = n_ready - 1;   // the entry that holds record 16c: the last one whose offset is at most 16c
+  while (e < hi) {
+    const uint32_t mid = (e + hi + 1) >> 1;
+    if (ready[mid].offset <= 16 * c) e = mid; else hi = mid - 1;
+  }
+  const uint4* src = reinterpret_cast<const uint4*>(ring);
+  for (; c < c_end; c++) {
+    const uint32_t r = 16 * c + (lane >> 1), k = e + (lane & 15);
+    uint32_t w_off = 0xFFFFFFFFu, w_end = 0xFFFFFFFFu, w_sub = 0, w_slot = 0;   // w_end: one past the entry's run
+    if (k < n_ready) {
+      const cpbus_ready rd = ready[k];
+      w_off = rd.offset; w_end = rd.offset + rd.count; w_sub = rd.sub_id - sub_base; w_slot = slot[k];
+    }
+    uint32_t j = 0;   // this lane's entry in the window: the last one whose offset is at most r (entry e always is)
+#pragma unroll
+    for (uint32_t q = 1; q < 16; q++) j += __shfl_sync(0xffffffffu, w_off, q) <= r ? 1u : 0u;
+    const uint32_t off = __shfl_sync(0xffffffffu, w_off, j), sub = __shfl_sync(0xffffffffu, w_sub, j),
+                   s0 = __shfl_sync(0xffffffffu, w_slot, j);
+    if (r < total) h_rec[2 * r + half] = src[2 * ((size_t)sub * ring_cap + ((s0 + (r - off)) & (ring_cap - 1))) + half];
+    // record 16c + 16 is in the entry of record 16c + 15 (lane 31's), or in the next one when that run ends at 16c + 16
+    const uint32_t j31 = __shfl_sync(0xffffffffu, j, 31), end31 = __shfl_sync(0xffffffffu, w_end, j31);
+    e += j31 + (end31 <= 16 * c + 16 ? 1u : 0u);
+  }
+}
+
 // ---- consumer backlog (cpbus_lagging) and the mailboxes a lossless flush waits on (cpbus_blockers) ----------------------
 // Read-only scans over the control blocks.  Each numbers the mailboxes it selects in position order with the single-pass
 // decoupled look-back of drain_ready_scan_kernel, reduced to one count per tile: flag (bits 62-63, kLbAgg / kLbIncl) |

@@ -27,6 +27,8 @@ class _GroupCalls:
 
 
 class GroupBus(Bus):
+    _GROUP = True   # hides the single-bus-only methods (the drain tickets)
+
     def __init__(self, n_max_subs: int, devices, ring_cap: int = 1024, batch_cap: int = 256, timers_per_sub: int = 0,
                  lossless: bool = False, digest: bool = True, sub_id_base: int = 0, store_path: int = nat.STORE_AUTO,
                  grid_ctas: int = 0, drop_missed_ticks: bool = False):

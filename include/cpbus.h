@@ -591,6 +591,39 @@ int cpbus_take_ready(cpbus_t* bus, uint32_t first_sub, uint32_t n, uint32_t star
                      cpbus_event* out, size_t cap, cpbus_ready* ready, size_t ready_cap,
                      size_t* n_ready, size_t* total, uint32_t* next_sub);
 int cpbus_ack_many(cpbus_t* bus, const uint32_t* sub_ids, const uint32_t* counts, uint32_t n, int* status, uint32_t* applied);
+/* ---- drain tickets: cpbus_drain_ready and cpbus_take_ready split in two, so that a pump hands one step's records to its
+ * channels while the next step's drain runs on the GPU.
+ *  - _begin enqueues the call on the bus stream and returns a ticket: it sees every launch queued before it and none
+ *    queued after.  Like the synchronous calls it resolves outstanding followers first and does not flush staged events.
+ *    It never waits for the GPU, except to allocate or grow a ticket's host buffer while that ticket is free, or the
+ *    bus's scan scratch while other tickets are outstanding (a larger n or ready_cap than before).  Cost: a memset, two
+ *    launches, and no host<->device copy issued by the host: the gather kernel writes the records, the ready list and the
+ *    header into the bus's pinned, mapped memory (the library keeps no caller pointer past a call).
+ *  - _end(ticket, ...) waits for that ticket only, writes out, ready, *n_ready, *total and *next_sub and frees the ticket.
+ *    They are byte-identical to what the synchronous call with the begin's arguments would have returned at the begin's
+ *    place in stream order, whatever was called in between (publishes, flushes, advances, membership changes, acks, other
+ *    drains and begins).  A bus that replaces each cpbus_drain_ready / cpbus_take_ready with _begin + _end, and one that
+ *    does not, give the same results afterwards: every later return code, drain, window, digest, fold, lagging, blockers
+ *    and debug event, and every cpbus_stats field but kernel_launches.  Cost: one event wait and host memcpys of
+ *    24*n_ready + 32*total bytes.
+ *  - One _end serves both begins; the tickets share one space.  At most 8 are outstanding: a 9th _begin returns
+ *    CPBUS_ENOSPC and enqueues nothing (a drain's records have left their mailboxes, so no result is ever overwritten).
+ *    Tickets may be ended in any order.  cpbus_destroy releases outstanding tickets: their records are lost, as records
+ *    drained into a buffer nobody reads.
+ *  - Memory: each of the 8 ticket slots keeps a pinned host buffer of 128 + 32*cap + 24*min(ready_cap, n) bytes for the
+ *    largest call it has served; buffers never shrink and are freed by cpbus_destroy (eight tickets with cap = 2^22 hold
+ *    about 1 GiB).
+ * CPBUS_EINVAL (_begin): as the synchronous call — a NULL bus or ticket, n == 0, ready_cap == 0, cap < ring_cap,
+ * cap > 0xFFFFFFFF, start_sub outside the range; cpbus_take_ready_begin also on a throughput-mode bus.  CPBUS_ENOENT
+ * (_begin): the range is not within this shard's subscribers.
+ * CPBUS_EINVAL (_end): a NULL pointer, or cap / ready_cap below the begin's (the ticket stays outstanding).  CPBUS_ENOENT
+ * (_end): a ticket that is not outstanding (never begun, or already ended). */
+int cpbus_drain_ready_begin(cpbus_t* bus, uint32_t first_sub, uint32_t n, uint32_t start_sub,
+                            size_t cap, size_t ready_cap, uint32_t* ticket);
+int cpbus_take_ready_begin(cpbus_t* bus, uint32_t first_sub, uint32_t n, uint32_t start_sub,
+                           size_t cap, size_t ready_cap, uint32_t* ticket);
+int cpbus_drain_ready_end(cpbus_t* bus, uint32_t ticket, cpbus_event* out, size_t cap,
+                          cpbus_ready* ready, size_t ready_cap, size_t* n_ready, size_t* total, uint32_t* next_sub);
 /* Consumer backlog, read-only: which subscribed mailboxes fall behind and by how much, without consuming anything (head never
  * moves; a drain after this call returns exactly what it would have returned without it).  Mailboxes [first_sub,
  * first_sub+n) are visited in cyclic id order from start_sub, as by cpbus_drain_ready; only subscribed ones count (the implicit
