@@ -19,7 +19,7 @@ MASK_ALL = 0x0001FFFF
 TARGET_ALL = 0xFFFFFFFF
 F_TICK, F_UNICAST = 0x1, 0x2
 CFG_LOSSLESS, CFG_DIGEST, CFG_SPARSE_TICKS, CFG_SPARSE_RECORDS = 0x1, 0x2, 0x4, 0x8
-CFG_DROP_MISSED_TICKS = 0x10
+CFG_DROP_MISSED_TICKS, CFG_SPARSE_DRAINS = 0x10, 0x20
 STORE_AUTO, STORE_V4, STORE_V8, STORE_BULK = 0, 1, 2, 3
 
 OK, EINVAL, ENOMEM, ECUDA, EAGAIN, ENOSPC, ENOENT, ECLOSED, ENODEV, EORDER, ETIMEDOUT = 0, -1, -2, -3, -4, -5, -6, -7, -8, -9, -10
@@ -27,6 +27,7 @@ PUT_STAMP, PUT_RAW, PUT_NOWAIT = 0, 1, 2
 EPHEMERAL_BIT, EPHEMERAL_SLOTS = 0x80000000, 65536
 DUE_CLOCK, DUE_ARM, DUE_ONESHOT, DUE_DISARM, DUE_UNSUB, DUE_LAUNCH = 0, 1, 2, 3, 4, 5
 DUE_CATCHUP = 6
+READY_SPARSE, READY_FULL, READY_DRAIN, READY_TAKE, READY_END, READY_CONSUME_ALL, READY_RELEASE = 0, 1, 2, 3, 4, 5, 6
 
 
 class Event(C.Structure):
@@ -82,6 +83,10 @@ assert PLAN_ENTRY_DTYPE.itemsize == 16
 # cpbus_timer_spec: one timer of cpbus_timer_add_list's list
 TIMER_SPEC_DTYPE = np.dtype([("period_ns", "<u8"), ("sub_id", "<u4"), ("source_id", "<u4"), ("oneshot", "<u4"), ("pad", "<u4")])
 assert TIMER_SPEC_DTYPE.itemsize == 24
+# cpbus_ready_op: one op of cpbus_ready_trace
+READY_OP_DTYPE = np.dtype([("kind", "<u4"), ("ticket", "<u4"), ("first", "<u4"), ("n", "<u4"), ("ids", "<u4"), ("n_ids", "<u4"),
+                           ("cut", "<u8")])
+assert READY_OP_DTYPE.itemsize == 32
 
 # every symbol include/cpbus.h declares: (restype, argtypes)
 _P = C.POINTER
@@ -170,6 +175,8 @@ SYMBOLS = {
     "cpbus_sparse_plan": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p,
                                     C.c_size_t, C.c_void_p, C.c_size_t, C.c_uint32, C.c_size_t, C.c_size_t, C.c_void_p,
                                     C.c_size_t, C.c_void_p, C.c_size_t, _P(C.c_size_t), _P(C.c_size_t)]),
+    "cpbus_ready_trace": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_uint32, C.c_size_t, C.c_void_p,
+                                    C.c_size_t, C.c_void_p, _P(C.c_size_t)]),
     "cpbus_record_hash": (C.c_uint64, [_P(Event)]),
     "cpbus_digest_multiplier": (C.c_uint64, []),
 }

@@ -37,18 +37,21 @@ class Bus:
     def __init__(self, n_max_subs: int, ring_cap: int = 1024, batch_cap: int = 256, timers_per_sub: int = 0,
                  lossless: bool = False, digest: bool = True, device: int = -1, sub_id_base: int = 0,
                  store_path: int = nat.STORE_AUTO, stream: int | None = None, grid_ctas: int = 0, sparse_ticks: bool = False,
-                 sparse_records: bool = False, drop_missed_ticks: bool = False):
+                 sparse_records: bool = False, drop_missed_ticks: bool = False, sparse_drains: bool = False):
         """`sparse_ticks`: CPBUS_CFG_SPARSE_TICKS, a flush with no staged event costs what is due (no streams on such a bus).
         `sparse_records`: CPBUS_CFG_SPARSE_RECORDS (implies sparse_ticks), a flush whose events reach few mailboxes
         launches only over them.
+        `sparse_drains`: CPBUS_CFG_SPARSE_DRAINS (implies sparse_ticks), a ready drain whose range holds no candidate
+        launches nothing, and one with few scans only them.
         `drop_missed_ticks`: CPBUS_CFG_DROP_MISSED_TICKS, a clock step that crosses several periods of a periodic timer
         delivers only its last tick, like Go's time.Ticker (no streams or device batches on such a bus)"""
         self._lib = nat.load()
         cfg = nat.Config()
         cfg.n_max_subs, cfg.ring_cap, cfg.batch_cap, cfg.timers_per_sub = n_max_subs, ring_cap, batch_cap, timers_per_sub
         cfg.flags = ((nat.CFG_LOSSLESS if lossless else 0) | (nat.CFG_DIGEST if digest else 0)
-                     | (nat.CFG_SPARSE_TICKS if sparse_ticks or sparse_records else 0)
+                     | (nat.CFG_SPARSE_TICKS if sparse_ticks or sparse_records or sparse_drains else 0)
                      | (nat.CFG_SPARSE_RECORDS if sparse_records else 0)
+                     | (nat.CFG_SPARSE_DRAINS if sparse_drains else 0)
                      | (nat.CFG_DROP_MISSED_TICKS if drop_missed_ticks else 0))
         cfg.device, cfg.sub_id_base, cfg.store_path, cfg.grid_ctas = device, sub_id_base, store_path, grid_ctas
         cfg.stream = C.c_void_p(stream) if stream else None

@@ -284,7 +284,10 @@ static int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_
     smem = off + p.stage_subs * per_sub;
   }
   const int variant = pairs_on ? (p.use_digest ? 7 : 6) : (p.timers_on ? 2 : 0) | (p.use_digest ? 1 : 0) | (p.order ? 4 : 0);
-#define CPBUS_DISPATCH(ST)                                                                \
+  // CPBUS_CFG_SPARSE_DRAINS: a drain on another thread sees the launch and the candidate index's update together
+  std::unique_lock<std::mutex> ready_lock(b->mu, std::defer_lock);
+  if (b->sparse_drains) ready_lock.lock();
+#define CPBUS_DISPATCH(ST)                                                              \
   switch (variant) {                                                                     \
     case 0: rc = launch_fanout_t<ST, false, false, false>(b, p, grid, smem, kind); break;      \
     case 1: rc = launch_fanout_t<ST, false, true, false>(b, p, grid, smem, kind); break;       \
@@ -301,6 +304,7 @@ static int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_
     default: CPBUS_DISPATCH(CPBUS_STORE_V8); break;
   }
 #undef CPBUS_DISPATCH
+  if (b->sparse_drains) b->ready_ix.full();   // any mailbox may have taken a record
   if (rc) return rc;
   b->st.kernel_launches++;
   if (!round) b->st.batches++;   // (a round's batch counts when it is resolved, if it delivered)
@@ -365,6 +369,10 @@ static int next_buffer(cpbus* b) {
 // (the rows re-measured in §4.6), so the cap stays.
 static size_t sparse_max(const cpbus* b) { return std::max<size_t>(32, b->n_next / 1024); }
 static size_t sparse_max_deliveries(const cpbus* b) { return std::max<size_t>(1024, b->n_next / 256); }
+// CPBUS_CFG_SPARSE_DRAINS: candidates in a drain's range beyond which it takes the dense scan, and a quarter of what the
+// index keeps per set for a bus of n mailboxes.  Measured on an H100 at 1,048,576 mailboxes (DESIGN.md §4.13): the list
+// scan beat the dense one up to 64 candidates, tied at 256 and lost from 1,024 on; the dense scan's cost grows with n.
+static size_t ready_list_max(size_t n) { return std::max<size_t>(256, n / 4096); }
 
 // The pinned plan buffer is free for `bytes`: the previous plan has left it, or both buffers are regrown (behind every
 // kernel that may still read the old device buffer).
@@ -404,7 +412,13 @@ static int launch_sparse(cpbus* b, uint64_t w) {
     p.launch_seq = ++b->launch_seq;
     p.result = result_slot(b, p.launch_seq); p.result_next = result_slot(b, p.launch_seq + 1);
     p.w_now = w; p.ring_cap = b->R; p.K = b->K; p.sub_base = b->cfg.sub_id_base; p.use_digest = b->use_digest ? 1u : 0u;
-    record_scatter_kernel<<<(uint32_t)((n_list + kWarpsPerCta - 1) / kWarpsPerCta), kThreads, 0, b->stream>>>(p);
+    {
+      // CPBUS_CFG_SPARSE_DRAINS: a drain on another thread sees the launch and its mailboxes in the index together
+      std::unique_lock<std::mutex> ready_lock(b->mu, std::defer_lock);
+      if (b->sparse_drains) ready_lock.lock();
+      record_scatter_kernel<<<(uint32_t)((n_list + kWarpsPerCta - 1) / kWarpsPerCta), kThreads, 0, b->stream>>>(p);
+      if (b->sparse_drains) b->ready_ix.add(&b->plan[0].local, n_list, sizeof(cpbus_plan_entry) / sizeof(uint32_t));
+    }
     CK(cudaGetLastError());
     CK(cudaEventRecord(b->records_done, b->stream));
     b->st.kernel_launches++;
@@ -656,6 +670,7 @@ int cpbus_create(const cpbus_config* cfg, cpbus_t** out) try {
   uint32_t R = 0, B = 0;
   if (config_check(cfg, &R, &B)) return CPBUS_EINVAL;
   if ((cfg->flags & CPBUS_CFG_SPARSE_RECORDS) && !(cfg->flags & CPBUS_CFG_SPARSE_TICKS)) return CPBUS_EINVAL;   // the due index finds the ticks
+  if ((cfg->flags & CPBUS_CFG_SPARSE_DRAINS) && !(cfg->flags & CPBUS_CFG_SPARSE_TICKS)) return CPBUS_EINVAL;    // launches that know their mailboxes
   const uint32_t K = cfg->timers_per_sub;
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
@@ -669,6 +684,7 @@ int cpbus_create(const cpbus_config* cfg, cpbus_t** out) try {
   b->lossless = cfg->flags & CPBUS_CFG_LOSSLESS; b->use_digest = cfg->flags & CPBUS_CFG_DIGEST;
   b->sparse = cfg->flags & CPBUS_CFG_SPARSE_TICKS;
   b->sparse_records = cfg->flags & CPBUS_CFG_SPARSE_RECORDS;
+  b->sparse_drains = cfg->flags & CPBUS_CFG_SPARSE_DRAINS;
   b->drop_missed = cfg->flags & CPBUS_CFG_DROP_MISSED_TICKS;
   b->room_lb = R;
   b->store = cfg->store_path == CPBUS_STORE_AUTO ? CPBUS_STORE_V8 : (int)cfg->store_path;
@@ -763,6 +779,7 @@ int cpbus_create(const cpbus_config* cfg, cpbus_t** out) try {
   b->h_released.assign(N, 0);
   if (b->sparse_records) b->rec_index.init(N, 2 * std::max<size_t>(32, N / 1024));   // lists of up to twice the largest cap
   else if (b->sparse) b->rec_index.slot.assign(N, UINT32_MAX);
+  if (b->sparse_drains) b->ready_ix.init(N, 4 * ready_list_max(N));
   b->intern.emplace(std::string(), 0u);   // "" -> 0 so that NonEvent == {None, 0} (events/events.go:45)
   b->sources.emplace_back();
   *out = b;
@@ -1328,6 +1345,10 @@ int cpbus_release_many(cpbus_t* b, const uint32_t* sub_ids, uint32_t n, int* sta
   }
   const int rc = slot_reset(b, ops, {});
   if (rc) return rc;
+  if (b->sparse_drains && !ops.empty()) {   // (after the reset: a drain between the two sees a superset)
+    std::lock_guard<std::mutex> g(b->mu);
+    b->ready_ix.released(&ops[0].local, ops.size(), sizeof(SlotResetOp) / sizeof(uint32_t));
+  }
   if (status && n) memcpy(status, st.data(), (size_t)n * sizeof(int));
   if (applied) *applied = (uint32_t)ops.size();
   return CPBUS_OK;
@@ -2196,12 +2217,48 @@ static int ready_range(const cpbus* b, uint32_t first_sub, uint32_t n, uint32_t 
   return id_range(b->cfg.sub_id_base, b->n_next, first_sub, n, l) ? CPBUS_OK : CPBUS_ENOENT;
 }
 
+// CPBUS_CFG_SPARSE_DRAINS: b->ready_list = the candidates of b->ready_cand (ascending, in [l, l + n)) with their positions
+// in the walk from rot, in position order: those at or after the start, then the ones before it.
+static void ready_walk(cpbus* b, uint32_t l, uint32_t n, uint32_t rot) {
+  const std::vector<uint32_t>& c = b->ready_cand;
+  const size_t split = std::lower_bound(c.begin(), c.end(), l + rot) - c.begin();
+  b->ready_list.clear();
+  for (size_t i = split; i < c.size(); i++) b->ready_list.push_back(make_uint2(c[i], c[i] - l - rot));
+  for (size_t i = 0; i < split; i++) b->ready_list.push_back(make_uint2(c[i], c[i] - l + (n - rot)));
+}
+
 // The host part of every sparse drain, synchronous or ticketed, up to its gather (the caller holds b->mu): resolution, the
 // device scratch and the scan of mailboxes [l, l + n) from position rot, with at most rcap entries.  The gathers of
 // outstanding tickets may still read the scratch on the bus stream, so a scratch buffer that has to grow while a ticket is
-// outstanding waits for the stream first.
-static int ready_scan_enqueue(cpbus* b, uint32_t l, uint32_t n, uint32_t rot, size_t cap, size_t rcap, bool take) {
+// outstanding waits for the stream first.  CPBUS_CFG_SPARSE_DRAINS: with no candidate in the range nothing is enqueued
+// (*none = true); with few, the list scan reads only them; otherwise the dense scan runs.
+static int ready_scan_enqueue(cpbus* b, uint32_t l, uint32_t n, uint32_t rot, size_t cap, size_t rcap, bool take, bool* none) {
   int rc = enter(b); if (rc) return rc;
+  *none = false;
+  if (take && !b->d_taken) {   // every cursor 0: max(0, head) = head, so nothing is held
+    CK(b->d_taken.alloc(b->N));
+    CK(cudaMemsetAsync(b->d_taken, 0, (size_t)b->N * sizeof(unsigned long long), b->stream));
+  }
+  if (b->sparse_drains && b->ready_ix.candidates(take, l, n, ready_list_max(b->n_next), &b->ready_cand)) {
+    if (b->ready_cand.empty()) { *none = true; return CPBUS_OK; }
+    ready_walk(b, l, n, rot);
+    const size_t m = b->ready_list.size();
+    if (b->drain_tk_busy && (rcap > b->d_ready.size() || rcap > b->d_ready_slot.size() || kReadyLbOffset > b->d_ready_lb.size() ||
+                             m > b->d_ready_list.size()))
+      CK(cudaStreamSynchronize(b->stream));
+    CK(b->d_ready.grow(rcap));
+    CK(b->d_ready_slot.grow(rcap));
+    CK(b->d_ready_lb.grow(kReadyLbOffset));
+    CK(b->d_ready_list.grow(m, 1024));
+    // (pageable source: the call returns once the list has been taken, and the copy runs in stream order)
+    CK(cudaMemcpyAsync(b->d_ready_list, b->ready_list.data(), m * sizeof(uint2), cudaMemcpyHostToDevice, b->stream));
+    ready_list_scan_kernel<<<1, kThreads, 0, b->stream>>>(b->d_ctl, take ? b->d_taken.get() : nullptr, b->d_ready_list,
+                                                           (uint32_t)m, n, b->R, b->lossless ? 1u : 0u, take ? 1u : 0u,
+                                                           b->cfg.sub_id_base, cap, rcap, b->d_ready_lb, b->d_ready,
+                                                           b->d_ready_slot);
+    CK(cudaGetLastError());
+    return CPBUS_OK;
+  }
   const uint32_t tiles = (n + kReadyTile - 1) / kReadyTile;
   const size_t lb_words = kReadyLbOffset + (size_t)tiles;
   if (b->drain_tk_busy && (rcap > b->d_ready.size() || rcap > b->d_ready_slot.size() || lb_words > b->d_ready_lb.size()))
@@ -2211,10 +2268,6 @@ static int ready_scan_enqueue(cpbus* b, uint32_t l, uint32_t n, uint32_t rot, si
   CK(b->d_ready_lb.grow(lb_words));
   CK(cudaMemsetAsync(b->d_ready_lb + kReadyHdrWords, 0, (lb_words - kReadyHdrWords) * sizeof(unsigned long long), b->stream));
   if (take) {
-    if (!b->d_taken) {   // every cursor 0: max(0, head) = head, so nothing is held
-      CK(b->d_taken.alloc(b->N));
-      CK(cudaMemsetAsync(b->d_taken, 0, (size_t)b->N * sizeof(unsigned long long), b->stream));
-    }
     take_ready_scan_kernel<<<tiles, kThreads, 0, b->stream>>>(b->d_ctl, b->d_taken, l, n, rot, b->R, b->cfg.sub_id_base, cap,
                                                                rcap, b->d_ready_lb, b->d_ready, b->d_ready_slot);
   } else {
@@ -2223,6 +2276,21 @@ static int ready_scan_enqueue(cpbus* b, uint32_t l, uint32_t n, uint32_t rot, si
   }
   CK(cudaGetLastError());
   return CPBUS_OK;
+}
+
+// CPBUS_CFG_SPARSE_DRAINS: whether [first_sub, first_sub + n) is every mailbox subscribed so far
+static bool ready_whole(const cpbus* b, uint32_t first_sub, uint32_t n) {
+  return first_sub == b->cfg.sub_id_base && n == b->n_next;
+}
+
+// CPBUS_CFG_SPARSE_DRAINS: the drain placed at `place` (take: a take_ready) has taken the mailboxes of ready[0..nr); all:
+// every ready mailbox of its range, which covers every subscribed mailbox when whole.  The caller holds b->mu.
+static void ready_drained(cpbus* b, bool take, uint64_t place, const cpbus_ready* ready, size_t nr, bool whole, bool all) {
+  if (!b->sparse_drains) return;
+  std::vector<uint32_t>& ids = b->ready_cand;
+  ids.resize(nr);
+  for (size_t i = 0; i < nr; i++) ids[i] = ready[i].sub_id - b->cfg.sub_id_base;
+  b->ready_ix.drained(take, place, ids.data(), nr, 1, whole && all);
 }
 
 // The body of cpbus_drain_ready, without its cap >= ring_cap check: a group hands each shard the cap its earlier shards
@@ -2240,7 +2308,14 @@ int cpbus_host::drain_ready_impl(cpbus_t* b, uint32_t first_sub, uint32_t n, uin
   if ((rc = dev_guard(b))) return rc;
   CK(b->d_drain.grow(cap));
   CK(b->h_ready_hdr.grow(8));
-  if ((rc = ready_scan_enqueue(b, l, n, rot, cap, rcap, take))) return rc;
+  const uint64_t place = b->ready_ix.place();
+  bool none = false;
+  if ((rc = ready_scan_enqueue(b, l, n, rot, cap, rcap, take, &none))) return rc;
+  if (none) {
+    ready_drained(b, take, place, nullptr, 0, ready_whole(b, first_sub, n), true);
+    *n_ready = 0; *total = 0; *all_taken = true; *next_sub = start_sub;
+    return CPBUS_OK;
+  }
   const uint32_t gather_grid = (uint32_t)std::min<size_t>((size_t)b->sm_count * 4, (rcap + kWarpsPerCta - 1) / kWarpsPerCta);
   drain_ready_gather_kernel<<<gather_grid, kThreads, 0, b->stream>>>(b->d_ring, b->R, b->cfg.sub_id_base, b->d_ready,
                                                                       b->d_ready_slot, b->d_ready_lb, b->d_drain, b->h_ready_hdr.dev());
@@ -2254,6 +2329,7 @@ int cpbus_host::drain_ready_impl(cpbus_t* b, uint32_t first_sub, uint32_t n, uin
     CK(cudaMemcpyAsync(out, b->d_drain, tot * sizeof(cpbus_event), cudaMemcpyDeviceToHost, b->stream));
     CK(cudaStreamSynchronize(b->stream));
   }
+  ready_drained(b, take, place, ready, nr, ready_whole(b, first_sub, n), cut >= n);
   *n_ready = nr; *total = tot;
   *all_taken = cut >= n;
   *next_sub = cut >= n ? start_sub : first_sub + (uint32_t)((rot + cut) % n);
@@ -2282,16 +2358,21 @@ static int drain_ready_begin(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_
   CK(t.buf.grow(kTicketHdrBytes + rec_bytes + rcap * sizeof(cpbus_ready)));
   if (!(cudaEvent_t)t.done) CK(t.done.create());
   const uint32_t rot = start_sub - first_sub;
-  if ((rc = ready_scan_enqueue(b, l, n, rot, cap, rcap, take))) return rc;
-  unsigned char* d = t.buf.dev();
-  const uint32_t grid = (uint32_t)std::min<size_t>((size_t)b->sm_count * 4, ((cap + 15) / 16 + kWarpsPerCta - 1) / kWarpsPerCta);
-  drain_ready_ticket_gather_kernel<<<grid, kThreads, 0, b->stream>>>(
-      b->d_ring, b->R, b->cfg.sub_id_base, b->d_ready, b->d_ready_slot, b->d_ready_lb,
-      reinterpret_cast<unsigned long long*>(d), reinterpret_cast<uint4*>(d + kTicketHdrBytes),
-      reinterpret_cast<uint2*>(d + kTicketHdrBytes + rec_bytes));
-  CK(cudaGetLastError());
-  b->st.kernel_launches += 2;
-  CK(cudaEventRecord(t.done, b->stream));
+  const uint64_t place = b->ready_ix.place();
+  bool none = false;
+  if ((rc = ready_scan_enqueue(b, l, n, rot, cap, rcap, take, &none))) return rc;
+  if (!none) {
+    unsigned char* d = t.buf.dev();
+    const uint32_t grid = (uint32_t)std::min<size_t>((size_t)b->sm_count * 4, ((cap + 15) / 16 + kWarpsPerCta - 1) / kWarpsPerCta);
+    drain_ready_ticket_gather_kernel<<<grid, kThreads, 0, b->stream>>>(
+        b->d_ring, b->R, b->cfg.sub_id_base, b->d_ready, b->d_ready_slot, b->d_ready_lb,
+        reinterpret_cast<unsigned long long*>(d), reinterpret_cast<uint4*>(d + kTicketHdrBytes),
+        reinterpret_cast<uint2*>(d + kTicketHdrBytes + rec_bytes));
+    CK(cudaGetLastError());
+    b->st.kernel_launches += 2;
+    CK(cudaEventRecord(t.done, b->stream));
+  }
+  t.place = place; t.take = take; t.whole = ready_whole(b, first_sub, n); t.none = none;
   t.busy = true;
   b->drain_tk_busy++;
   t.ticket = (b->drain_tk_gen++ & 0x1FFFFFFFu) << 3 | i;
@@ -2318,15 +2399,19 @@ int cpbus_drain_ready_end(cpbus_t* b, uint32_t ticket, cpbus_event* out, size_t 
   if (!t.busy || t.ticket != ticket) return CPBUS_ENOENT;
   if (cap < t.cap || ready_cap < t.ready_cap) return CPBUS_EINVAL;   // the ticket stays outstanding
   int rc = dev_guard(b); if (rc) return rc;
-  CK(cudaEventSynchronize(t.done));
-  const unsigned char* h = t.buf.get();
-  const volatile unsigned long long* hdr = reinterpret_cast<const volatile unsigned long long*>(h);
-  const size_t nr = (size_t)hdr[0], tot = (size_t)hdr[1];
-  const uint64_t cut = hdr[2];
-  if (nr) {
-    memcpy(ready, h + kTicketHdrBytes + t.cap * sizeof(cpbus_event), nr * sizeof(cpbus_ready));
-    memcpy(out, h + kTicketHdrBytes, tot * sizeof(cpbus_event));
+  size_t nr = 0, tot = 0;
+  uint64_t cut = t.n;   // a ticket that enqueued nothing: its range held no candidate
+  if (!t.none) {
+    CK(cudaEventSynchronize(t.done));
+    const unsigned char* h = t.buf.get();
+    const volatile unsigned long long* hdr = reinterpret_cast<const volatile unsigned long long*>(h);
+    nr = (size_t)hdr[0]; tot = (size_t)hdr[1]; cut = hdr[2];
+    if (nr) {
+      memcpy(ready, h + kTicketHdrBytes + t.cap * sizeof(cpbus_event), nr * sizeof(cpbus_ready));
+      memcpy(out, h + kTicketHdrBytes, tot * sizeof(cpbus_event));
+    }
   }
+  ready_drained(b, t.take, t.place, ready, nr, t.whole, cut >= t.n);
   *n_ready = nr; *total = tot;
   *next_sub = cut >= t.n ? t.start : t.first + (uint32_t)(((uint64_t)(t.start - t.first) + cut) % t.n);
   t.busy = false;
@@ -2527,6 +2612,7 @@ int cpbus_consume_all(cpbus_t* b) try {
     b->follow_q.push_back(cpbus::FollowPending{nullptr, 0ull, -1, cpbus::kConsumeAll});
   }
   b->room_lb = b->R;   // stream-ordered behind every earlier fan-out: from here on every mailbox is empty
+  if (b->sparse_drains) b->ready_ix.consumed();
   return CPBUS_OK;
 } CPBUS_CATCH
 

@@ -117,6 +117,7 @@ int cpbus_group_create(const cpbus_config* cfg, const int32_t* devices, uint32_t
   *out = nullptr;
   if (cfg->flags & CPBUS_CFG_SPARSE_TICKS) return CPBUS_EINVAL;   // the group's flush is a stream batch (see cpbus_stream_create)
   if (cfg->flags & CPBUS_CFG_SPARSE_RECORDS) return CPBUS_EINVAL;
+  if (cfg->flags & CPBUS_CFG_SPARSE_DRAINS) return CPBUS_EINVAL;
   uint32_t R = 0, B = 0;
   if (config_check(cfg, &R, &B) || cfg->n_max_subs < n_devices) return CPBUS_EINVAL;
   cpbus_group* g = new (std::nothrow) cpbus_group();

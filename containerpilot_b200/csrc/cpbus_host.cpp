@@ -213,6 +213,52 @@ int cpbus_due_trace(const cpbus_due_op* ops, size_t n_ops, uint32_t n_slots, uin
   *n_out = n;
   return CPBUS_OK;
 } CPBUS_CATCH
+// The candidate index of a sparse-drains bus over n_subs subscribed mailboxes, driven by ops instead of the bus's launches
+// and drains (the bus's own list cap is max(256, subscribers / 4096), and its bound 4 times that).
+int cpbus_ready_trace(const cpbus_ready_op* ops, size_t n_ops, const uint32_t* ids, size_t n_ids_total, uint32_t n_subs,
+                      size_t list_cap, uint32_t* out, size_t cap, int64_t* counts, size_t* n_out) try {
+  if ((!ops && n_ops) || (!ids && n_ids_total) || !n_out || (cap && !out) || (!counts && n_ops) || !list_cap) return CPBUS_EINVAL;
+  ReadyIndex x;
+  x.init(n_subs, 4 * list_cap);
+  struct Open { uint64_t place; uint32_t first, n; bool take; };
+  std::unordered_map<uint32_t, Open> open;
+  std::vector<uint32_t> cand;
+  size_t n = 0;
+  for (size_t i = 0; i < n_ops; i++) {
+    const cpbus_ready_op& op = ops[i];
+    counts[i] = 0;
+    if ((uint64_t)op.ids + op.n_ids > n_ids_total) return CPBUS_EINVAL;
+    const uint32_t* list = ids + op.ids;
+    for (uint32_t j = 0; j < op.n_ids; j++) if (list[j] >= n_subs) return CPBUS_EINVAL;
+    switch (op.kind) {
+      case CPBUS_READY_SPARSE: x.add(list, op.n_ids); break;
+      case CPBUS_READY_FULL: x.full(); break;
+      case CPBUS_READY_DRAIN:
+      case CPBUS_READY_TAKE: {
+        const bool take = op.kind == CPBUS_READY_TAKE;
+        if (!op.n || (uint64_t)op.first + op.n > n_subs || open.count(op.ticket)) return CPBUS_EINVAL;
+        open[op.ticket] = Open{x.place(), op.first, op.n, take};
+        if (!x.candidates(take, op.first, op.n, list_cap, &cand)) { counts[i] = -1; break; }
+        counts[i] = (int64_t)cand.size();
+        for (uint32_t l : cand) { if (n < cap) out[n] = l; n++; }
+        break;
+      }
+      case CPBUS_READY_END: {
+        auto it = open.find(op.ticket);
+        if (it == open.end()) return CPBUS_ENOENT;
+        const Open o = it->second;
+        open.erase(it);
+        x.drained(o.take, o.place, list, op.n_ids, 1, op.cut >= o.n && o.first == 0 && o.n == n_subs);
+        break;
+      }
+      case CPBUS_READY_CONSUME_ALL: x.consumed(); break;
+      case CPBUS_READY_RELEASE: x.released(list, op.n_ids); break;
+      default: return CPBUS_EINVAL;
+    }
+  }
+  *n_out = n;
+  return CPBUS_OK;
+} CPBUS_CATCH
 // The plan of a sparse-records flush over an index built from the arguments, with the bus's own planning code (keep =
 // max_mailboxes: a code with more subscribers keeps only its count, as on a bus).
 int cpbus_sparse_plan(const uint32_t* masks, const uint8_t* active, uint32_t n_subs, const cpbus_pair* pairs,

@@ -177,6 +177,10 @@ struct cpbus : HostFront {
     bool busy = false;
     uint32_t ticket = 0, first = 0, n = 0, start = 0;
     size_t cap = 0, ready_cap = 0;
+    // CPBUS_CFG_SPARSE_DRAINS: the drain's place in the candidate index, its kind, whether it covers every subscribed
+    // mailbox, and whether its range held no candidate (nothing was enqueued: _end returns the empty result)
+    uint64_t place = 0;
+    bool take = false, whole = false, none = false;
   };
   DrainTicket drain_tk[kDrainTickets];
   uint32_t drain_tk_gen = 0, drain_tk_busy = 0;
@@ -260,6 +264,14 @@ struct cpbus : HostFront {
   DeviceBuf<unsigned long long> d_taken;
   PinnedBuf<unsigned char> h_ack; DeviceBuf<unsigned char> d_ack;
   MappedBuf<int> h_ack_status;
+  // CPBUS_CFG_SPARSE_DRAINS: the candidate index (read and written under mu, like the drains' scratch: launches take mu to
+  // update it), the candidates of one drain, and the list the list scan reads ({mailbox, walk position}; host copy and
+  // device copy, grown)
+  bool sparse_drains = false;
+  ReadyIndex ready_ix;
+  std::vector<uint32_t> ready_cand;
+  std::vector<uint2> ready_list;
+  DeviceBuf<uint2> d_ready_list;
 
   // intern table (Event.Source string <-> u32)
   std::unordered_map<std::string, uint32_t> intern;

@@ -784,6 +784,98 @@ __global__ void __launch_bounds__(kThreads) take_ready_scan_kernel(SubCtl* __res
   ready_scan<true>(ctl, taken, first, n, rot, ring_cap, 1u, sub_base, cap, ready_cap, lb, ready, slot);
 }
 
+// CPBUS_CFG_SPARSE_DRAINS: the scan of drain_ready_scan_kernel (take = 0) or take_ready_scan_kernel (take = 1) over a
+// candidate list instead of the whole range.  list[i] = {mailbox, its position in the range's cyclic walk}, in ascending
+// position.  One CTA walks the list in tiles of kReadyTile candidates; each tile is numbered as a tile of the dense scan,
+// offset by the totals of the tiles before it, and the tile that holds the first ready candidate that does not fit ends the
+// walk.  A mailbox outside the list holds nothing for the predicate, so the entries, the cursors moved and the header
+// {taken, records, position of the first ready mailbox that did not fit (n: none)} are the dense scan's.
+__global__ void __launch_bounds__(kThreads) ready_list_scan_kernel(SubCtl* __restrict__ ctl,
+                                                                   unsigned long long* __restrict__ taken,
+                                                                   const uint2* __restrict__ list, uint32_t m, uint32_t n,
+                                                                   uint32_t ring_cap, uint32_t lossless, uint32_t take,
+                                                                   uint32_t sub_base, unsigned long long cap,
+                                                                   unsigned long long ready_cap, unsigned long long* hdr,
+                                                                   cpbus_ready* __restrict__ ready, uint32_t* __restrict__ slot) {
+  __shared__ uint32_t s_wr[32];              // per (item, warp) chunk: ready mailboxes, then their exclusive prefix in the tile
+  __shared__ unsigned long long s_wc[32];    // ... and records
+  __shared__ unsigned long long s_base_r, s_base_c, s_tile_r, s_tile_c;
+  __shared__ uint32_t s_stop;
+  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (threadIdx.x == 0) { s_base_r = 0; s_base_c = 0; s_stop = 0; }
+  for (uint32_t t0 = 0; t0 < m; t0 += kReadyTile) {
+    uint32_t loc[kReadyItems], pos[kReadyItems], r_in[kReadyItems];
+    unsigned long long tl[kReadyItems], cur[kReadyItems], hd[kReadyItems], c_in[kReadyItems];
+#pragma unroll
+    for (uint32_t k = 0; k < kReadyItems; k++) {
+      const uint32_t i = t0 + k * kThreads + threadIdx.x;
+      unsigned long long t = 0, h = 0, c = 0;
+      uint32_t l = 0, p = 0;
+      if (i < m) {
+        const uint2 e = list[i];
+        l = e.x; p = e.y;
+        const ulonglong2 th = *reinterpret_cast<const ulonglong2*>(ctl + l);   // {tail, head}
+        t = th.x; h = th.y; c = h;
+        if (take) {
+          const unsigned long long tk = taken[l];
+          if (tk > c) c = tk;
+        } else if (!lossless && t > ring_cap && t - ring_cap > c) {
+          c = t - ring_cap;   // overwritten before being taken
+        }
+      }
+      loc[k] = l; pos[k] = p; tl[k] = t; hd[k] = h; cur[k] = c;
+      uint32_t r = t != c ? 1u : 0u;
+      unsigned long long s = t - c;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t ro = __shfl_up_sync(0xffffffffu, r, o);
+        const unsigned long long so = shfl64(s, (int)lane - o);
+        if ((int)lane >= o) { r += ro; s += so; }
+      }
+      r_in[k] = r; c_in[k] = s;
+      if (lane == 31) { s_wr[k * kWarpsPerCta + warp] = r; s_wc[k * kWarpsPerCta + warp] = s; }
+    }
+    __syncthreads();
+    if (warp == 0) {
+      const uint32_t r0 = s_wr[lane];
+      const unsigned long long c0 = s_wc[lane];
+      uint32_t r = r0;
+      unsigned long long c = c0;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t ro = __shfl_up_sync(0xffffffffu, r, o);
+        const unsigned long long co = shfl64(c, (int)lane - o);
+        if ((int)lane >= o) { r += ro; c += co; }
+      }
+      s_wr[lane] = r - r0; s_wc[lane] = c - c0;
+      if (lane == 31) { s_tile_r = r; s_tile_c = c; }
+    }
+    __syncthreads();
+    const unsigned long long base_r = s_base_r, base_c = s_base_c;
+#pragma unroll
+    for (uint32_t k = 0; k < kReadyItems; k++) {
+      const unsigned long long cnt = tl[k] - cur[k];
+      if (!cnt) continue;
+      const uint32_t chunk = k * kWarpsPerCta + warp;
+      const unsigned long long r = base_r + s_wr[chunk] + r_in[k] - 1;        // entry index among the ready mailboxes
+      const unsigned long long o = base_c + s_wc[chunk] + c_in[k] - cnt;      // first record of the run in `out`
+      if (r < ready_cap && o + cnt <= cap) {
+        ready[r] = cpbus_ready{sub_base + loc[k], (uint32_t)cnt, (uint32_t)o, 0u, take ? 0ull : cur[k] - hd[k]};
+        slot[r] = (uint32_t)(cur[k] & (ring_cap - 1));
+        if (take) taken[loc[k]] = tl[k];
+        else ctl[loc[k]].head = tl[k];
+      } else if (r == 0 || (r - 1 < ready_cap && o <= cap)) {   // its predecessor was taken: this one ends the call
+        hdr[0] = r; hdr[1] = o; hdr[2] = pos[k];
+        s_stop = 1;
+      }
+    }
+    __syncthreads();
+    if (s_stop) return;
+    if (threadIdx.x == 0) { s_base_r += s_tile_r; s_base_c += s_tile_c; }
+  }
+  if (threadIdx.x == 0) { hdr[0] = s_base_r; hdr[1] = s_base_c; hdr[2] = n; }
+}
+
 // Copies the taken runs: one warp per ready entry, lane pairs per record (each pair writes one whole 32-byte sector), and
 // hands the header to the host through mapped pinned memory.
 __global__ void __launch_bounds__(kThreads) drain_ready_gather_kernel(const cpbus_event* __restrict__ ring, uint32_t ring_cap,

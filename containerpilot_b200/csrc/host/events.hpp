@@ -212,18 +212,21 @@ class EventBus {   // events/bus.go:12-22
   // sparse_records: CPBUS_CFG_SPARSE_RECORDS, a Publish whose events reach few mailboxes launches only over them (one bus only).
   // drop_missed_ticks: CPBUS_CFG_DROP_MISSED_TICKS, a clock step across several periods of a timer delivers its last tick
   // only, as Go's time.Ticker does.
+  // sparse_drains: CPBUS_CFG_SPARSE_DRAINS, the pump's drain of a step that delivered nothing launches nothing, and one
+  // after a few deliveries scans only their mailboxes (one bus only).
   explicit EventBus(Clock clock = Clock::Monotonic, uint32_t n_max_subs = 256, uint32_t mailbox_cap = 1024,
-                    bool sparse_records = false, bool drop_missed_ticks = false)
-      : EventBus(std::vector<int32_t>{}, clock, n_max_subs, mailbox_cap, sparse_records, drop_missed_ticks) {}
+                    bool sparse_records = false, bool drop_missed_ticks = false, bool sparse_drains = false)
+      : EventBus(std::vector<int32_t>{}, clock, n_max_subs, mailbox_cap, sparse_records, drop_missed_ticks, sparse_drains) {}
   // The same bus on a group of shards, shard g on devices[g] (cpbus_group_create; devices may repeat).  Empty: one bus on
-  // the current device.  A group refuses sparse_records (std::runtime_error).
+  // the current device.  A group refuses sparse_records and sparse_drains (std::runtime_error).
   EventBus(const std::vector<int32_t>& devices, Clock clock, uint32_t n_max_subs = 256, uint32_t mailbox_cap = 1024,
-           bool sparse_records = false, bool drop_missed_ticks = false) : clock_(clock) {
+           bool sparse_records = false, bool drop_missed_ticks = false, bool sparse_drains = false) : clock_(clock) {
     cpbus_config cfg{};
     cfg.n_max_subs = n_max_subs; cfg.ring_cap = mailbox_cap; cfg.batch_cap = mailbox_cap >= 512 ? 256 : mailbox_cap / 2;
     cfg.timers_per_sub = 4; cfg.flags = CPBUS_CFG_LOSSLESS | CPBUS_CFG_DIGEST; cfg.device = -1;
     if (devices.empty()) cfg.flags |= CPBUS_CFG_SPARSE_TICKS;   // the 1 ms pump launches only for due ticks (a group has no such mode)
     if (sparse_records) cfg.flags |= CPBUS_CFG_SPARSE_RECORDS;
+    if (sparse_drains) cfg.flags |= CPBUS_CFG_SPARSE_DRAINS;
     if (drop_missed_ticks) cfg.flags |= CPBUS_CFG_DROP_MISSED_TICKS;
     batch_cap_ = cfg.batch_cap;
     drain_cap_ = std::max<size_t>(kDrainCap, mailbox_cap);

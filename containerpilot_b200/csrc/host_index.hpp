@@ -1,8 +1,9 @@
 // host_index.hpp — the host-only indexes of a bus and the planners that read them: the timer table's due-time
 // arithmetic and the due index of a CPBUS_CFG_SPARSE_TICKS bus (DueIndex), the subscription index of a
-// CPBUS_CFG_SPARSE_RECORDS bus (SubIndex), and the declarations of sparse_plan, split_plan and mask_order, which
-// cpbus_host.cpp defines.  Plain C++17 with no device code: cpbus_due_trace, cpbus_sparse_plan, cpbus_split_plan and
-// cpbus_mask_order export this code so that it can be tested without a GPU.
+// CPBUS_CFG_SPARSE_RECORDS bus (SubIndex), the drain candidates of a CPBUS_CFG_SPARSE_DRAINS bus (ReadyIndex), and the
+// declarations of sparse_plan, split_plan and mask_order, which cpbus_host.cpp defines.  Plain C++17 with no device code:
+// cpbus_due_trace, cpbus_sparse_plan, cpbus_ready_trace, cpbus_split_plan and cpbus_mask_order export this code so that it
+// can be tested without a GPU.
 #pragma once
 #include <algorithm>
 #include <cstddef>
@@ -274,6 +275,105 @@ struct SubIndex {
       k.subs.resize(o); k.stale = k.stale > gone ? k.stale - gone : 0;
       if (!o) cases.erase(it);
     }
+  }
+};
+
+// The candidate index of a CPBUS_CFG_SPARSE_DRAINS bus: for each drain predicate a set of mailboxes that may hold records
+// for it, or "unknown".  Set 0 (C_unread) serves cpbus_drain_ready: every mailbox that may have tail > head.  Set 1
+// (C_untaken) serves cpbus_take_ready: every mailbox that may have tail > max(take cursor, head).  The invariant: at every
+// point in stream order each mailbox with records for the predicate is in its set, or the set is unknown.
+//  * Launches that append are numbered (`ord`).  A sparse launch stamps its mailboxes with its ordinal in both sets; any
+//    other launch makes both unknown and records its ordinal as `blind`.
+//  * A drain's place is the ordinal of the last launch in front of it in stream order (taken when it is enqueued).  When its
+//    result is known it removes the mailboxes it took whose stamp is at most its place (a later launch may have refilled
+//    the others).  A drain that took every ready mailbox of the whole subscribed range, with no blind launch after its
+//    place, makes the set known: what holds records now was appended after its place, so it is the members stamped later.
+//  * While unknown a set keeps stamping what sparse launches add, so that such a drain can make it known again.  A set of
+//    more than `bound` members is emptied and made unknown (blind at the current ordinal).
+// Drains of both kinds empty C_untaken; only cpbus_drain_ready empties C_unread.
+struct ReadyIndex {
+  // A set: per mailbox the ordinal of the launch that last added it (0: not a member), and the list of members, which may
+  // also hold mailboxes removed since the list was last compacted (`listed`: in the list).  O(1) per added or removed
+  // mailbox; a drain's candidates cost one pass over the list.
+  struct Set {
+    bool known = true;                               // a new bus: every mailbox is empty
+    uint64_t blind = 0;                              // the last launch whose mailboxes may be missing from the set
+    size_t live = 0;
+    std::vector<uint64_t> stamp;
+    std::vector<uint8_t> listed;
+    std::vector<uint32_t> list;
+    void put(uint32_t l, uint64_t o) {
+      if (!stamp[l]) live++;
+      stamp[l] = o;
+      if (!listed[l]) { listed[l] = 1; list.push_back(l); }
+    }
+    void drop(uint32_t l) { if (stamp[l]) { stamp[l] = 0; live--; } }
+    void clear() { for (uint32_t l : list) { stamp[l] = 0; listed[l] = 0; } list.clear(); live = 0; }
+    void compact() {
+      size_t o = 0;
+      for (uint32_t l : list) { if (stamp[l]) list[o++] = l; else listed[l] = 0; }
+      list.resize(o);
+    }
+    void tidy() { if (list.size() > 2 * live + 64) compact(); }
+  };
+  Set set[2];
+  uint64_t ord = 0;
+  size_t bound = 0;
+
+  void init(size_t n, size_t bound_n) {
+    bound = bound_n; ord = 0;
+    for (Set& s : set) { s = Set{}; s.stamp.assign(n, 0); s.listed.assign(n, 0); }
+  }
+  uint64_t place() const { return ord; }
+  void add(const uint32_t* ids, size_t n, size_t stride = 1) {
+    ord++;
+    for (Set& s : set) {
+      for (size_t i = 0; i < n; i++) s.put(ids[i * stride], ord);
+      if (s.live > bound) { s.clear(); s.known = false; s.blind = ord; }
+    }
+  }
+  void full() {
+    ord++;
+    for (Set& s : set) { s.clear(); s.known = false; s.blind = ord; }
+  }
+  // a drain (take: a take_ready) placed at p took ids[0..n) (local indices, every `stride` words); complete: it took every
+  // ready mailbox of the whole subscribed range
+  void drained(bool take, uint64_t p, const uint32_t* ids, size_t n, size_t stride, bool complete) {
+    for (int k = take ? 1 : 0; k < 2; k++) {
+      Set& s = set[k];
+      for (size_t i = 0; s.live && i < n; i++) {
+        const uint32_t l = ids[i * stride];
+        if (s.stamp[l] <= p) s.drop(l);
+      }
+      if (complete && s.blind <= p) {
+        s.known = true;
+        for (uint32_t l : s.list) if (s.stamp[l] <= p) s.drop(l);
+        s.compact();
+      } else {
+        s.tidy();
+      }
+    }
+  }
+  void consumed() { for (Set& s : set) { s.clear(); s.known = true; } }
+  void released(const uint32_t* ids, size_t n, size_t stride = 1) {
+    for (Set& s : set) {
+      for (size_t i = 0; i < n; i++) s.drop(ids[i * stride]);
+      s.tidy();
+    }
+  }
+  // The candidates of set `take` in [l, l + n), ascending, into *out: true when the set is known and holds at most cap of
+  // them there; false for the dense scan.
+  bool candidates(bool take, uint32_t l, uint32_t n, size_t cap, std::vector<uint32_t>* out) const {
+    out->clear();
+    const Set& s = set[take ? 1 : 0];
+    if (!s.known) return false;
+    for (uint32_t m : s.list)
+      if (s.stamp[m] && m - l < n) {
+        if (out->size() == cap) return false;
+        out->push_back(m);
+      }
+    std::sort(out->begin(), out->end());
+    return true;
   }
 };
 

@@ -122,12 +122,14 @@ class EventBus:
 
     def __init__(self, n_max_subs: int = 64, ring_cap: int = 1024, batch_cap: int = 256, timers_per_sub: int = 4,
                  lossless: bool = True, devices=None, sparse_records: bool = False, drop_missed_ticks: bool = False,
-                 reuse_ids: bool = False, **kw):
+                 reuse_ids: bool = False, sparse_drains: bool = False, **kw):
         """`devices`: run on a group of shards, shard g on devices[g] (GroupBus); the answers are the single bus's.
         The single bus is created with sparse timer delivery (CPBUS_CFG_SPARSE_TICKS): a pump step with nothing due
         launches nothing.  A group does not take that flag.
         `sparse_records` (single bus only): CPBUS_CFG_SPARSE_RECORDS, a Publish whose events reach few mailboxes
         launches only over them.
+        `sparse_drains` (single bus only): CPBUS_CFG_SPARSE_DRAINS, the pump's drain of a step in which nothing was
+        delivered launches nothing, and one after a few deliveries scans only their mailboxes.
         `drop_missed_ticks`: CPBUS_CFG_DROP_MISSED_TICKS, a clock step across several periods of a NewEventTimer delivers
         one tick, not one per period, as the Go ticker does (timer.go; its channel holds one tick).
         `reuse_ids`: Unsubscribe releases the mailbox (cpbus_release_many) once the records it owed the channel have left
@@ -135,13 +137,15 @@ class EventBus:
         `n_max_subs` bounds the live subscribers rather than the subscriptions over the bus's life."""
         if sparse_records and devices is not None:
             raise ValueError("sparse_records: a group of shards does not take CPBUS_CFG_SPARSE_RECORDS")
+        if sparse_drains and devices is not None:
+            raise ValueError("sparse_drains: a group of shards does not take CPBUS_CFG_SPARSE_DRAINS")
         if devices is not None:
             self._bus = GroupBus(n_max_subs, devices, ring_cap=ring_cap, batch_cap=batch_cap, timers_per_sub=timers_per_sub,
                                  lossless=lossless, digest=True, drop_missed_ticks=drop_missed_ticks, **kw)
         else:
             self._bus = Bus(n_max_subs, ring_cap=ring_cap, batch_cap=batch_cap, timers_per_sub=timers_per_sub,
                             lossless=lossless, digest=True, sparse_ticks=True, sparse_records=sparse_records,
-                            drop_missed_ticks=drop_missed_ticks, **kw)
+                            sparse_drains=sparse_drains, drop_missed_ticks=drop_missed_ticks, **kw)
         self.reload = False
         self._reuse = reuse_ids
         self._done = 0              # sync.WaitGroup counter (bus.go:16)

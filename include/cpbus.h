@@ -147,6 +147,22 @@ enum {
                                    cpbus_stream_create/_open/_attach and cpbus_publish_device
                                    /_staged return CPBUS_EINVAL on a flagged bus (the group's own
                                    internal streams excepted); lifting that is future work. */
+#define CPBUS_CFG_SPARSE_DRAINS 0x20u /* cpbus_drain_ready / cpbus_take_ready (and their
+                                   tickets) cost what the range can hold: the host keeps the
+                                   mailboxes each sparse launch appended to and each drain
+                                   emptied, and a ready call whose range holds no candidate
+                                   launches nothing, copies nothing and does not synchronise
+                                   (n_ready = total = 0, next_sub = start_sub; a _begin still
+                                   takes a ticket slot), one with at most max(256,
+                                   subscribers/4096) candidates scans only those, and otherwise
+                                   the dense scan runs.  A full fan-out, a lossless partial
+                                   flush or a device batch makes the candidates unknown (dense
+                                   scans) until a drain that takes every ready mailbox of the
+                                   whole subscribed range.  Results are those of a bus without
+                                   the flag making the same calls, except
+                                   cpbus_stats.kernel_launches.  Requires
+                                   CPBUS_CFG_SPARSE_TICKS (CPBUS_EINVAL otherwise); not
+                                   supported on a group: CPBUS_EINVAL. */
 
 /* cpbus_config.store_path: how records reach the rings (all are bit-identical) */
 enum {
@@ -872,6 +888,28 @@ int cpbus_sparse_plan(const uint32_t* masks, const uint8_t* active, uint32_t n_s
                       const uint32_t* n_pairs, uint32_t sub_id_base, const cpbus_event* records, size_t n_records,
                       const uint32_t* due_slots, size_t n_due, uint32_t K, size_t max_mailboxes, size_t max_deliveries,
                       cpbus_plan_entry* out, size_t cap, uint32_t* rec_idx, size_t idx_cap, size_t* n_out, size_t* n_idx);
+/* The candidate index of a CPBUS_CFG_SPARSE_DRAINS bus, as a pure host function (no device needed; the bus runs the same
+ * code): ops[0..n_ops) run in order over mailboxes [0, n_subs), all subscribed and empty at the start.  Each op is {kind,
+ * ticket, first, n, ids, n_ids, cut}; ids[ids .. ids + n_ids) is the op's mailbox list (local indices):
+ *   CPBUS_READY_SPARSE       a sparse launch that appends to the listed mailboxes
+ *   CPBUS_READY_FULL         a launch that may append to any mailbox (fan-out, lossless partial flush, device batch)
+ *   CPBUS_READY_DRAIN        a cpbus_drain_ready over [first, first + n), begun under `ticket` (any value not outstanding)
+ *   CPBUS_READY_TAKE         the same for cpbus_take_ready
+ *   CPBUS_READY_END          the end of `ticket`: the drain took the listed mailboxes, and cut >= its n when it took every
+ *                            ready mailbox of its range
+ *   CPBUS_READY_CONSUME_ALL  cpbus_consume_all
+ *   CPBUS_READY_RELEASE      cpbus_release_many of the listed mailboxes
+ * counts[i] is, for a DRAIN or TAKE op, the number of candidates its scan visits (0: no launch) or -1 for the dense scan
+ * (unknown candidates, or more than list_cap of them in the range), and 0 for every other op.  The candidate lists, each
+ * in ascending order, go to out one after the other; *n_out = their total length (the first cap are written).  A set
+ * that grows past 4 * list_cap becomes unknown.  CPBUS_EINVAL: an unknown kind, a range or id outside [0, n_subs), an id
+ * list outside ids[0 .. n_ids_total), list_cap == 0, or a DRAIN / TAKE under an outstanding ticket; CPBUS_ENOENT: an END
+ * of a ticket not outstanding. */
+enum { CPBUS_READY_SPARSE = 0, CPBUS_READY_FULL = 1, CPBUS_READY_DRAIN = 2, CPBUS_READY_TAKE = 3, CPBUS_READY_END = 4,
+       CPBUS_READY_CONSUME_ALL = 5, CPBUS_READY_RELEASE = 6 };
+typedef struct cpbus_ready_op { uint32_t kind, ticket, first, n, ids, n_ids; uint64_t cut; } cpbus_ready_op;   /* sizeof == 32 */
+int cpbus_ready_trace(const cpbus_ready_op* ops, size_t n_ops, const uint32_t* ids, size_t n_ids_total, uint32_t n_subs,
+                      size_t list_cap, uint32_t* out, size_t cap, int64_t* counts, size_t* n_out);
 
 #ifdef __cplusplus
 }
