@@ -2197,7 +2197,7 @@ int cpbus_drain_many(cpbus_t* b, uint32_t first_sub, uint32_t n, cpbus_event* ou
 int cpbus_drain_ready(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start_sub, cpbus_event* out, size_t cap,
                       cpbus_ready* ready, size_t ready_cap, size_t* n_ready, size_t* total, uint32_t* next_sub) try {
   if (!b || !out || !ready || !n_ready || !total || !next_sub || !n || !ready_cap) return CPBUS_EINVAL;
-  if (cap < b->R || cap > 0xFFFFFFFFull) return CPBUS_EINVAL;   // cap >= ring_cap: a ready mailbox always fits an empty call
+  if (!ready_cap_ok(cap, b->R, false, b->lossless)) return CPBUS_EINVAL;
   bool all_taken = false;
   return drain_ready_impl(b, first_sub, n, start_sub, out, cap, ready, ready_cap, n_ready, total, next_sub, &all_taken);
 } CPBUS_CATCH
@@ -2205,16 +2205,21 @@ int cpbus_drain_ready(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start
 int cpbus_take_ready(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start_sub, cpbus_event* out, size_t cap,
                      cpbus_ready* ready, size_t ready_cap, size_t* n_ready, size_t* total, uint32_t* next_sub) try {
   if (!b || !out || !ready || !n_ready || !total || !next_sub || !n || !ready_cap) return CPBUS_EINVAL;
-  if (cap < b->R || cap > 0xFFFFFFFFull || !b->lossless) return CPBUS_EINVAL;
+  if (!ready_cap_ok(cap, b->R, true, b->lossless)) return CPBUS_EINVAL;
   bool all_taken = false;
   return drain_ready_impl(b, first_sub, n, start_sub, out, cap, ready, ready_cap, n_ready, total, next_sub, &all_taken, true);
 } CPBUS_CATCH
 
-// The checks every sparse drain makes after its own: start_sub within the range (CPBUS_EINVAL), and the range within this
-// shard (CPBUS_ENOENT); *l = the range's first mailbox.
-static int ready_range(const cpbus* b, uint32_t first_sub, uint32_t n, uint32_t start_sub, uint32_t* l) {
+// The range checks of a paged walk over ids [first_sub, first_sub + n) from start_sub (the sparse drains, cpbus_lagging):
+// start_sub within the range (CPBUS_EINVAL), and the range within this shard (CPBUS_ENOENT); *l = the range's first mailbox.
+static int walk_range(const cpbus* b, uint32_t first_sub, uint32_t n, uint32_t start_sub, uint32_t* l) {
   if (start_sub < first_sub || start_sub - first_sub >= n) return CPBUS_EINVAL;
   return id_range(b->cfg.sub_id_base, b->n_next, first_sub, n, l) ? CPBUS_OK : CPBUS_ENOENT;
+}
+
+// Where that walk goes on after a call that stopped at position `cut` (n or more: it did not stop, so at start_sub again)
+static uint32_t walk_next(uint32_t first_sub, uint32_t n, uint32_t start_sub, uint64_t cut) {
+  return cut >= n ? start_sub : first_sub + (uint32_t)(((uint64_t)(start_sub - first_sub) + cut) % n);
 }
 
 // CPBUS_CFG_SPARSE_DRAINS: b->ready_list = the candidates of b->ready_cand (ascending, in [l, l + n)) with their positions
@@ -2239,40 +2244,28 @@ static int ready_scan_enqueue(cpbus* b, uint32_t l, uint32_t n, uint32_t rot, si
     CK(b->d_taken.alloc(b->N));
     CK(cudaMemsetAsync(b->d_taken, 0, (size_t)b->N * sizeof(unsigned long long), b->stream));
   }
-  if (b->sparse_drains && b->ready_ix.candidates(take, l, n, ready_list_max(b->n_next), &b->ready_cand)) {
-    if (b->ready_cand.empty()) { *none = true; return CPBUS_OK; }
-    ready_walk(b, l, n, rot);
-    const size_t m = b->ready_list.size();
-    if (b->drain_tk_busy && (rcap > b->d_ready.size() || rcap > b->d_ready_slot.size() || kReadyLbOffset > b->d_ready_lb.size() ||
-                             m > b->d_ready_list.size()))
-      CK(cudaStreamSynchronize(b->stream));
-    CK(b->d_ready.grow(rcap));
-    CK(b->d_ready_slot.grow(rcap));
-    CK(b->d_ready_lb.grow(kReadyLbOffset));
-    CK(b->d_ready_list.grow(m, 1024));
-    // (pageable source: the call returns once the list has been taken, and the copy runs in stream order)
-    CK(cudaMemcpyAsync(b->d_ready_list, b->ready_list.data(), m * sizeof(uint2), cudaMemcpyHostToDevice, b->stream));
-    ready_list_scan_kernel<<<1, kThreads, 0, b->stream>>>(b->d_ctl, take ? b->d_taken.get() : nullptr, b->d_ready_list,
-                                                           (uint32_t)m, n, b->R, b->lossless ? 1u : 0u, take ? 1u : 0u,
-                                                           b->cfg.sub_id_base, cap, rcap, b->d_ready_lb, b->d_ready,
-                                                           b->d_ready_slot);
-    CK(cudaGetLastError());
-    return CPBUS_OK;
-  }
-  const uint32_t tiles = (n + kReadyTile - 1) / kReadyTile;
-  const size_t lb_words = kReadyLbOffset + (size_t)tiles;
-  if (b->drain_tk_busy && (rcap > b->d_ready.size() || rcap > b->d_ready_slot.size() || lb_words > b->d_ready_lb.size()))
+  const bool list = b->sparse_drains && b->ready_ix.candidates(take, l, n, ready_list_max(b->n_next), &b->ready_cand);
+  if (list && b->ready_cand.empty()) { *none = true; return CPBUS_OK; }
+  if (list) ready_walk(b, l, n, rot);
+  const uint32_t tiles = list ? 1u : (n + kReadyTile - 1) / kReadyTile;
+  const size_t m = list ? b->ready_list.size() : 0, lb_words = kReadyLbOffset + (list ? 0 : (size_t)tiles);
+  if (b->drain_tk_busy && (rcap > b->d_ready.size() || rcap > b->d_ready_slot.size() || lb_words > b->d_ready_lb.size() ||
+                           m > b->d_ready_list.size()))
     CK(cudaStreamSynchronize(b->stream));
   CK(b->d_ready.grow(rcap));
   CK(b->d_ready_slot.grow(rcap));
   CK(b->d_ready_lb.grow(lb_words));
-  CK(cudaMemsetAsync(b->d_ready_lb + kReadyHdrWords, 0, (lb_words - kReadyHdrWords) * sizeof(unsigned long long), b->stream));
-  if (take) {
-    take_ready_scan_kernel<<<tiles, kThreads, 0, b->stream>>>(b->d_ctl, b->d_taken, l, n, rot, b->R, b->cfg.sub_id_base, cap,
-                                                               rcap, b->d_ready_lb, b->d_ready, b->d_ready_slot);
+  CK(b->d_ready_list.grow(m, 1024));
+  const ReadyScan a{b->d_ctl, take ? b->d_taken.get() : nullptr, n, b->R, b->lossless ? 1u : 0u, b->cfg.sub_id_base, cap, rcap,
+                    b->d_ready_lb, b->d_ready, b->d_ready_slot};
+  if (list) {
+    // (pageable source: the call returns once the list has been taken, and the copy runs in stream order)
+    CK(cudaMemcpyAsync(b->d_ready_list, b->ready_list.data(), m * sizeof(uint2), cudaMemcpyHostToDevice, b->stream));
+    (take ? ready_list_scan_kernel<true> : ready_list_scan_kernel<false>)<<<1, kThreads, 0, b->stream>>>(a, b->d_ready_list,
+                                                                                                       (uint32_t)m);
   } else {
-    drain_ready_scan_kernel<<<tiles, kThreads, 0, b->stream>>>(b->d_ctl, l, n, rot, b->R, b->lossless ? 1u : 0u, b->cfg.sub_id_base,
-                                                                cap, rcap, b->d_ready_lb, b->d_ready, b->d_ready_slot);
+    CK(cudaMemsetAsync(b->d_ready_lb + kReadyHdrWords, 0, (lb_words - kReadyHdrWords) * sizeof(unsigned long long), b->stream));
+    (take ? ready_scan_kernel<true> : ready_scan_kernel<false>)<<<tiles, kThreads, 0, b->stream>>>(a, l, rot);
   }
   CK(cudaGetLastError());
   return CPBUS_OK;
@@ -2300,7 +2293,7 @@ int cpbus_host::drain_ready_impl(cpbus_t* b, uint32_t first_sub, uint32_t n, uin
                                  cpbus_ready* ready, size_t ready_cap, size_t* n_ready, size_t* total, uint32_t* next_sub,
                                  bool* all_taken, bool take) {
   uint32_t l = 0;
-  int rc = ready_range(b, first_sub, n, start_sub, &l); if (rc) return rc;
+  int rc = walk_range(b, first_sub, n, start_sub, &l); if (rc) return rc;
   std::lock_guard<std::mutex> g(b->mu);
   const size_t rcap = std::min<size_t>(ready_cap, n);   // never more entries than mailboxes
   const uint32_t rot = start_sub - first_sub;
@@ -2332,7 +2325,7 @@ int cpbus_host::drain_ready_impl(cpbus_t* b, uint32_t first_sub, uint32_t n, uin
   ready_drained(b, take, place, ready, nr, ready_whole(b, first_sub, n), cut >= n);
   *n_ready = nr; *total = tot;
   *all_taken = cut >= n;
-  *next_sub = cut >= n ? start_sub : first_sub + (uint32_t)((rot + cut) % n);
+  *next_sub = walk_next(first_sub, n, start_sub, cut);
   return CPBUS_OK;
 }
 
@@ -2342,10 +2335,9 @@ constexpr size_t kTicketHdrBytes = 128;   // the records start on a 128-byte lin
 
 static int drain_ready_begin(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start_sub, size_t cap, size_t ready_cap,
                              uint32_t* ticket, bool take) {
-  if (!b || !ticket || !n || !ready_cap) return CPBUS_EINVAL;
-  if (cap < b->R || cap > 0xFFFFFFFFull || (take && !b->lossless)) return CPBUS_EINVAL;
+  if (!b || !ticket || !n || !ready_cap || !ready_cap_ok(cap, b->R, take, b->lossless)) return CPBUS_EINVAL;
   uint32_t l = 0;
-  int rc = ready_range(b, first_sub, n, start_sub, &l); if (rc) return rc;
+  int rc = walk_range(b, first_sub, n, start_sub, &l); if (rc) return rc;
   std::lock_guard<std::mutex> g(b->mu);
   if (b->drain_tk_busy == (uint32_t)cpbus::kDrainTickets) return CPBUS_ENOSPC;   // no result is ever overwritten
   uint32_t i = 0;
@@ -2413,7 +2405,7 @@ int cpbus_drain_ready_end(cpbus_t* b, uint32_t ticket, cpbus_event* out, size_t 
   }
   ready_drained(b, t.take, t.place, ready, nr, t.whole, cut >= t.n);
   *n_ready = nr; *total = tot;
-  *next_sub = cut >= t.n ? t.start : t.first + (uint32_t)(((uint64_t)(t.start - t.first) + cut) % t.n);
+  *next_sub = walk_next(t.first, t.n, t.start, cut);
   t.busy = false;
   b->drain_tk_busy--;
   return CPBUS_OK;
@@ -2482,20 +2474,26 @@ int cpbus_ack_many(cpbus_t* b, const uint32_t* sub_ids, const uint32_t* counts, 
   return CPBUS_OK;
 } CPBUS_CATCH
 
+// The look-back scans of cpbus_lagging and cpbus_blockers over n mailboxes: their work buffer's counters and tile status are
+// zeroed on the bus stream, and *tiles = the grid, one tile per kReadyTile mailboxes.
+static cudaError_t lag_scan_reset(cpbus* b, uint32_t n, uint32_t* tiles) {
+  *tiles = (n + kReadyTile - 1) / kReadyTile;
+  return cudaMemsetAsync(b->d_lag_lb, 0, (kLagLbOffset + (size_t)*tiles) * sizeof(unsigned long long), b->stream);
+}
+
 // Consumer backlog: one read-only scan of the range's control blocks; the entries and the header {selected, cut position,
 // summary} arrive in mapped pinned memory, so one sync is the only wait.  *all_returned: every lagging mailbox was returned.
 int cpbus_host::lagging_impl(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start_sub, uint32_t min_backlog, cpbus_lag* out,
                              size_t cap, size_t* n_out, uint32_t* next_sub, cpbus_lag_summary* sum, bool* all_returned) {
   static_assert(sizeof(cpbus_lag) == 16 && sizeof(cpbus_lag_summary) == kLagSumWords * sizeof(unsigned long long), "C-ABI layout");
-  if (start_sub < first_sub || start_sub - first_sub >= n) return CPBUS_EINVAL;
   uint32_t l = 0;
-  if (!id_range(b->cfg.sub_id_base, b->n_next, first_sub, n, &l)) return CPBUS_ENOENT;
+  int rc = walk_range(b, first_sub, n, start_sub, &l); if (rc) return rc;
   std::lock_guard<std::mutex> g(b->mu);
-  int rc = enter(b); if (rc) return rc;
+  if ((rc = enter(b))) return rc;
   const size_t ecap = std::min<size_t>(cap, n);   // never more entries than mailboxes
   CK(b->h_lag.grow(ecap));
-  const uint32_t tiles = (n + kReadyTile - 1) / kReadyTile;
-  CK(cudaMemsetAsync(b->d_lag_lb, 0, (kLagLbOffset + (size_t)tiles) * sizeof(unsigned long long), b->stream));
+  uint32_t tiles = 0;
+  CK(lag_scan_reset(b, n, &tiles));
   const uint32_t rot = start_sub - first_sub;
   lagging_scan_kernel<<<tiles, kThreads, 0, b->stream>>>(b->d_ctl, l, n, rot, b->R, b->lossless ? 1u : 0u, b->cfg.sub_id_base,
                                                           min_backlog, ecap, b->d_lag_lb, b->h_lag.dev(), b->h_lag_hdr.dev());
@@ -2512,8 +2510,8 @@ int cpbus_host::lagging_impl(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_
     memcpy(sum, w, sizeof(w));
   }
   *n_out = got;
-  *all_returned = total <= ecap;
-  *next_sub = *all_returned ? start_sub : first_sub + (uint32_t)((rot + cut) % n);
+  *all_returned = total <= ecap;   // (then the cut position is n)
+  *next_sub = walk_next(first_sub, n, start_sub, cut);
   return CPBUS_OK;
 }
 
@@ -2531,8 +2529,8 @@ int cpbus_host::blockers_impl(cpbus* b, const cpbus_event* rec, uint64_t t, uint
   *n = 0;
   const bool timers_on = b->n_timers > 0 && b->K > 0;
   if (b->n_next == 0 || b->room_lb >= admit_need(rec ? 1 : 0, t, b->last_watermark, b->min_period, b->K, timers_on)) return CPBUS_OK;
-  const uint32_t tiles = (b->n_next + kReadyTile - 1) / kReadyTile;
-  CK(cudaMemsetAsync(b->d_lag_lb, 0, (kLagLbOffset + (size_t)tiles) * sizeof(unsigned long long), b->stream));
+  uint32_t tiles = 0;
+  CK(lag_scan_reset(b, b->n_next, &tiles));
   const size_t ecap = std::min<size_t>(cap, b->n_next);
   blockers_scan_kernel<<<tiles, kThreads, 0, b->stream>>>(b->d_ctl, b->d_timers, b->n_paired > 0 ? b->d_pairs.get() : nullptr, b->n_next,
                                                            b->R, b->K, b->cfg.sub_id_base, timers_on ? 1u : 0u, rec ? 1u : 0u,

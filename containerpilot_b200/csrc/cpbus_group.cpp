@@ -703,14 +703,14 @@ static int group_drain_ready(cpbus_group* g, uint32_t first_sub, uint32_t n, uin
 int cpbus_group_drain_ready(cpbus_group_t* g, uint32_t first_sub, uint32_t n, uint32_t start_sub, cpbus_event* out, size_t cap,
                             cpbus_ready* ready, size_t ready_cap, size_t* n_ready, size_t* total, uint32_t* next_sub) try {
   if (!g || !out || !ready || !n_ready || !total || !next_sub || !n || !ready_cap) return CPBUS_EINVAL;
-  if (cap < g->shards[0]->R || cap > 0xFFFFFFFFull) return CPBUS_EINVAL;
+  if (!ready_cap_ok(cap, g->shards[0]->R, false, g->lossless)) return CPBUS_EINVAL;
   return group_drain_ready(g, first_sub, n, start_sub, out, cap, ready, ready_cap, n_ready, total, next_sub, false);
 } CPBUS_CATCH
 
 int cpbus_group_take_ready(cpbus_group_t* g, uint32_t first_sub, uint32_t n, uint32_t start_sub, cpbus_event* out, size_t cap,
                            cpbus_ready* ready, size_t ready_cap, size_t* n_ready, size_t* total, uint32_t* next_sub) try {
   if (!g || !out || !ready || !n_ready || !total || !next_sub || !n || !ready_cap) return CPBUS_EINVAL;
-  if (cap < g->shards[0]->R || cap > 0xFFFFFFFFull || !g->lossless) return CPBUS_EINVAL;
+  if (!ready_cap_ok(cap, g->shards[0]->R, true, g->lossless)) return CPBUS_EINVAL;
   return group_drain_ready(g, first_sub, n, start_sub, out, cap, ready, ready_cap, n_ready, total, next_sub, true);
 } CPBUS_CATCH
 

@@ -346,6 +346,11 @@ void pair_counts(const HostFront* f, const unsigned long long* dev_keys, const u
 int drain_ready_impl(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start_sub, cpbus_event* out, size_t cap,
                      cpbus_ready* ready, size_t ready_cap, size_t* n_ready, size_t* total, uint32_t* next_sub,
                      bool* all_taken, bool take = false);
+// The cap check of every sparse drain (single bus, ticket or group; take: cpbus_take_ready's): a ready mailbox always fits
+// an empty call (cap >= ring_cap), record offsets are 32-bit, and only a lossless bus holds records back for acks.
+inline bool ready_cap_ok(size_t cap, uint32_t ring_cap, bool take, bool lossless) {
+  return cap >= ring_cap && cap <= 0xFFFFFFFFull && (!take || lossless);
+}
 int ack_many_impl(cpbus* b, const uint32_t* sub_ids, const uint32_t* counts, uint32_t n, int* st);
 void ack_statuses(const std::vector<int>& st, int* status, uint32_t* applied);
 int lagging_impl(cpbus_t* b, uint32_t first_sub, uint32_t n, uint32_t start_sub, uint32_t min_backlog, cpbus_lag* out,

@@ -648,49 +648,93 @@ __device__ __forceinline__ unsigned long long lb_pack(unsigned long long flag, u
   return flag | (ready << 33) | (rec < kLbRecMax ? rec : kLbRecMax);
 }
 
-// hdr[0..2] = {mailboxes taken, records taken, position of the first ready mailbox that did not fit (n: none)}; exactly one
-// thread writes it: the one holding that mailbox, or the last tile when everything fits.
-// kTake (cpbus_take_ready, lossless only): a mailbox's cursor is max(take cursor, head), and taking it moves the take
-// cursor to tail instead of head.
+// Mailbox first + (rot + p) mod n, for position p < n
+__device__ __forceinline__ uint32_t walk_mailbox(uint32_t first, uint32_t n, uint32_t rot, uint32_t p) {
+  unsigned long long q = (unsigned long long)rot + p;
+  if (q >= n) q -= n;
+  return first + (uint32_t)q;
+}
+
+// A mailbox's consumer cursor: its records are [cur, tail).  Drain: head, or in throughput mode max(head, tail - ring_cap)
+// (records overwritten before being taken).  kTake (cpbus_take_ready, lossless only): max(head, take cursor).
+struct MailboxCursor { unsigned long long tail, head, cur; };
 template <bool kTake>
-__device__ __forceinline__ void ready_scan(SubCtl* __restrict__ ctl, unsigned long long* __restrict__ taken, uint32_t first,
-                                           uint32_t n, uint32_t rot, uint32_t ring_cap, uint32_t lossless, uint32_t sub_base,
-                                           unsigned long long cap, unsigned long long ready_cap, unsigned long long* lb,
-                                           cpbus_ready* __restrict__ ready, uint32_t* __restrict__ slot) {
-  __shared__ uint32_t s_tile;
+__device__ __forceinline__ MailboxCursor mailbox_cursor(const SubCtl* __restrict__ ctl, const unsigned long long* __restrict__ taken,
+                                                        uint32_t l, uint32_t ring_cap, uint32_t lossless) {
+  const ulonglong2 th = *reinterpret_cast<const ulonglong2*>(ctl + l);   // {tail, head}
+  MailboxCursor c{th.x, th.y, th.y};
+  if constexpr (kTake) {
+    const unsigned long long tk = taken[l];
+    if (tk > c.cur) c.cur = tk;
+  } else if (!lossless && c.tail > ring_cap && c.tail - ring_cap > c.cur) {
+    c.cur = c.tail - ring_cap;
+  }
+  return c;
+}
+
+// The decoupled look-back of tile `tile` (warp 0 of its CTA): publishes the tile's totals, adds up its predecessors' words
+// back to the nearest inclusive prefix, publishes its own inclusive prefix and returns the totals before the tile.  Tiles
+// are numbered in the order the CTAs start, so every predecessor a tile waits for is running or done.
+struct LbCount { unsigned long long ready, rec; };
+__device__ __forceinline__ LbCount lookback(unsigned long long* status, uint32_t tile, LbCount agg) {
+  volatile unsigned long long* st = status;
+  const uint32_t lane = threadIdx.x & 31;
+  LbCount ex{0, 0};
+  if (tile == 0) {
+    if (lane == 0) st[0] = lb_pack(kLbIncl, agg.ready, agg.rec);
+    return ex;
+  }
+  if (lane == 0) st[tile] = lb_pack(kLbAgg, agg.ready, agg.rec);
+  // look back over windows of 32 predecessors until one has published its inclusive prefix (tile 0 always does)
+  for (int pred = (int)tile - 1;; pred -= 32) {
+    const int j = pred - (int)lane;
+    unsigned long long v = kLbIncl;   // before tile 0: an empty inclusive prefix (never summed, tile 0 stops the walk)
+    do {
+      if (j >= 0) v = st[j];
+    } while (__any_sync(0xffffffffu, (v >> 62) == 0));
+    const uint32_t incl = __ballot_sync(0xffffffffu, (v >> 62) == 2);
+    const uint32_t stop = incl ? (uint32_t)(__ffs(incl) - 1) : 31u;   // the nearest inclusive predecessor ends the walk
+    ex.ready += warp_sum64(lane <= stop ? (v >> 33) & ((1ull << 29) - 1) : 0ull);
+    ex.rec += warp_sum64(lane <= stop ? v & kLbRecMax : 0ull);
+    ex.rec = ex.rec < kLbRecMax ? ex.rec : kLbRecMax;
+    if (incl) break;
+  }
+  if (lane == 0) st[tile] = lb_pack(kLbIncl, ex.ready + agg.ready, ex.rec + agg.rec);
+  return ex;
+}
+
+// What both ready scans pass to their kernel.  hdr[0..2] = {mailboxes taken, records taken, position of the first ready
+// mailbox that did not fit (n: none)}, written by exactly one thread: the one holding that mailbox, or the last tile when
+// everything fits.  kTake reads and moves the take cursors `taken` instead of head (which it reads, never writes).
+struct ReadyScan {
+  SubCtl* ctl;
+  unsigned long long* taken;         // kTake only
+  uint32_t n, ring_cap, lossless, sub_base;
+  unsigned long long cap, ready_cap;
+  unsigned long long* hdr;           // the header, then (dense scan) the tile counter and the tile status
+  cpbus_ready* ready;
+  uint32_t* slot;
+};
+
+// One tile of a ready scan.  item(k, l, p) names item k of this thread (false: none): mailbox l at walk position p.
+// base(agg) runs on warp 0 with the tile's totals and returns the totals of the tiles before it.  last: the final tile,
+// which writes the header when everything fits.  Returns whether this thread wrote the cut header.
+template <bool kTake, class Item, class Base>
+__device__ __forceinline__ bool ready_tile(const ReadyScan& a, bool last, Item item, Base base) {
   __shared__ uint32_t s_wr[32];              // per (item, warp) chunk: ready mailboxes, then their exclusive prefix in the tile
   __shared__ unsigned long long s_wc[32];    // ... and records
-  __shared__ unsigned long long s_base_r, s_base_c;
-  unsigned long long* hdr = lb;
-  unsigned long long* status = lb + kReadyLbOffset;
+  __shared__ LbCount s_base;
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  // tiles are numbered in the order the CTAs start, so every predecessor a tile waits for is running or done
-  if (threadIdx.x == 0) s_tile = atomicAdd(reinterpret_cast<unsigned int*>(lb + kReadyHdrWords), 1u);
-  __syncthreads();
-  const uint32_t tile = s_tile;
-  uint32_t loc[kReadyItems], r_in[kReadyItems];
+  uint32_t loc[kReadyItems], pos[kReadyItems], r_in[kReadyItems];
   unsigned long long tl[kReadyItems], cur[kReadyItems], hd[kReadyItems], c_in[kReadyItems];
 #pragma unroll
-  for (uint32_t k = 0; k < kReadyItems; k++) {   // item k of the tile = positions k*kThreads .. +kThreads: coalesced loads
-    const uint32_t p = tile * kReadyTile + k * kThreads + threadIdx.x;
-    unsigned long long t = 0, h = 0, c = 0;
-    uint32_t l = 0;
-    if (p < n) {
-      unsigned long long q = (unsigned long long)rot + p;
-      if (q >= n) q -= n;
-      l = first + (uint32_t)q;
-      const ulonglong2 th = *reinterpret_cast<const ulonglong2*>(ctl + l);   // {tail, head}
-      t = th.x; h = th.y; c = h;
-      if constexpr (kTake) {
-        const unsigned long long tk = taken[l];
-        if (tk > c) c = tk;
-      } else {
-        if (!lossless && t > ring_cap && t - ring_cap > c) c = t - ring_cap;   // overwritten before being taken
-      }
-    }
-    loc[k] = l; tl[k] = t; hd[k] = h; cur[k] = c;
-    uint32_t r = t != c ? 1u : 0u;
-    unsigned long long s = t - c;
+  for (uint32_t k = 0; k < kReadyItems; k++) {
+    uint32_t l = 0, p = 0;
+    MailboxCursor c{0, 0, 0};
+    if (item(k, l, p)) c = mailbox_cursor<kTake>(a.ctl, a.taken, l, a.ring_cap, a.lossless);
+    loc[k] = l; pos[k] = p; tl[k] = c.tail; hd[k] = c.head; cur[k] = c.cur;
+    uint32_t r = c.tail != c.cur ? 1u : 0u;
+    unsigned long long s = c.tail - c.cur;
 #pragma unroll
     for (int o = 1; o < 32; o <<= 1) {
       const uint32_t ro = __shfl_up_sync(0xffffffffu, r, o);
@@ -713,167 +757,83 @@ __device__ __forceinline__ void ready_scan(SubCtl* __restrict__ ctl, unsigned lo
       if ((int)lane >= o) { r += ro; c += co; }
     }
     s_wr[lane] = r - r0; s_wc[lane] = c - c0;
-    const unsigned long long agg_r = __shfl_sync(0xffffffffu, r, 31), agg_c = shfl64(c, 31);
-    unsigned long long ex_r = 0, ex_c = 0;
-    if (tile == 0) {
-      if (lane == 0) *reinterpret_cast<volatile unsigned long long*>(status) = lb_pack(kLbIncl, agg_r, agg_c);
-    } else {
-      if (lane == 0) *reinterpret_cast<volatile unsigned long long*>(status + tile) = lb_pack(kLbAgg, agg_r, agg_c);
-      // look back over windows of 32 predecessors until one has published its inclusive prefix (tile 0 always does)
-      for (int pred = (int)tile - 1;; pred -= 32) {
-        const int j = pred - (int)lane;
-        unsigned long long v = kLbIncl;   // before tile 0: an empty inclusive prefix (never summed, tile 0 stops the walk)
-        do {
-          if (j >= 0) v = *reinterpret_cast<volatile unsigned long long*>(status + j);
-        } while (__any_sync(0xffffffffu, (v >> 62) == 0));
-        const uint32_t incl = __ballot_sync(0xffffffffu, (v >> 62) == 2);
-        const uint32_t stop = incl ? (uint32_t)(__ffs(incl) - 1) : 31u;   // the nearest inclusive predecessor ends the walk
-        ex_r += warp_sum64(lane <= stop ? (v >> 33) & ((1ull << 29) - 1) : 0ull);
-        ex_c += warp_sum64(lane <= stop ? v & kLbRecMax : 0ull);
-        ex_c = ex_c < kLbRecMax ? ex_c : kLbRecMax;
-        if (incl) break;
-      }
-      if (lane == 0) *reinterpret_cast<volatile unsigned long long*>(status + tile) = lb_pack(kLbIncl, ex_r + agg_r, ex_c + agg_c);
-    }
+    const LbCount agg{__shfl_sync(0xffffffffu, r, 31), shfl64(c, 31)};
+    const LbCount ex = base(agg);
     if (lane == 0) {
-      s_base_r = ex_r; s_base_c = ex_c;
-      const unsigned long long all_r = ex_r + agg_r, all_c = ex_c + agg_c;
-      if (tile == gridDim.x - 1 && all_r <= ready_cap && all_c <= cap) { hdr[0] = all_r; hdr[1] = all_c; hdr[2] = n; }
+      s_base = ex;
+      const unsigned long long all_r = ex.ready + agg.ready, all_c = ex.rec + agg.rec;
+      if (last && all_r <= a.ready_cap && all_c <= a.cap) { a.hdr[0] = all_r; a.hdr[1] = all_c; a.hdr[2] = a.n; }
     }
   }
   __syncthreads();
+  bool cut = false;
 #pragma unroll
   for (uint32_t k = 0; k < kReadyItems; k++) {
     const unsigned long long cnt = tl[k] - cur[k];
     if (!cnt) continue;
     const uint32_t chunk = k * kWarpsPerCta + warp;
-    const unsigned long long r = s_base_r + s_wr[chunk] + r_in[k] - 1;        // entry index among the ready mailboxes
-    const unsigned long long o = s_base_c + s_wc[chunk] + c_in[k] - cnt;      // first record of the run in `out`
-    if (r < ready_cap && o + cnt <= cap) {
-      if constexpr (kTake) {
-        ready[r] = cpbus_ready{sub_base + loc[k], (uint32_t)cnt, (uint32_t)o, 0u, 0ull};
-        slot[r] = (uint32_t)(cur[k] & (ring_cap - 1));
-        taken[loc[k]] = tl[k];
-      } else {
-        ready[r] = cpbus_ready{sub_base + loc[k], (uint32_t)cnt, (uint32_t)o, 0u, cur[k] - hd[k]};
-        slot[r] = (uint32_t)(cur[k] & (ring_cap - 1));
-        ctl[loc[k]].head = tl[k];
-      }
-    } else if (r == 0 || (r - 1 < ready_cap && o <= cap)) {   // its predecessor was taken: this one ends the call
-      hdr[0] = r; hdr[1] = o; hdr[2] = tile * kReadyTile + k * kThreads + threadIdx.x;
+    const unsigned long long r = s_base.ready + s_wr[chunk] + r_in[k] - 1;   // entry index among the ready mailboxes
+    const unsigned long long o = s_base.rec + s_wc[chunk] + c_in[k] - cnt;   // first record of the run in `out`
+    if (r < a.ready_cap && o + cnt <= a.cap) {
+      a.ready[r] = cpbus_ready{a.sub_base + loc[k], (uint32_t)cnt, (uint32_t)o, 0u, kTake ? 0ull : cur[k] - hd[k]};
+      a.slot[r] = (uint32_t)(cur[k] & (a.ring_cap - 1));
+      if constexpr (kTake) a.taken[loc[k]] = tl[k];
+      else a.ctl[loc[k]].head = tl[k];
+    } else if (r == 0 || (r - 1 < a.ready_cap && o <= a.cap)) {   // its predecessor was taken: this one ends the call
+      a.hdr[0] = r; a.hdr[1] = o; a.hdr[2] = pos[k];
+      cut = true;
     }
   }
+  return cut;
 }
 
-__global__ void __launch_bounds__(kThreads) drain_ready_scan_kernel(SubCtl* __restrict__ ctl, uint32_t first, uint32_t n,
-                                                                    uint32_t rot, uint32_t ring_cap, uint32_t lossless,
-                                                                    uint32_t sub_base, unsigned long long cap,
-                                                                    unsigned long long ready_cap, unsigned long long* lb,
-                                                                    cpbus_ready* __restrict__ ready, uint32_t* __restrict__ slot) {
-  ready_scan<false>(ctl, nullptr, first, n, rot, ring_cap, lossless, sub_base, cap, ready_cap, lb, ready, slot);
+// The dense scan (cpbus_drain_ready; kTake: cpbus_take_ready over a lossless bus): mailboxes [first, first + n) from
+// position rot, one tile per CTA, numbered by the look-back over a.hdr's tile status.  Item k of a tile is positions
+// k * kThreads .. + kThreads: coalesced loads.  The taken runs are copied by a gather kernel.
+template <bool kTake>
+__global__ void __launch_bounds__(kThreads) ready_scan_kernel(const ReadyScan a, uint32_t first, uint32_t rot) {
+  __shared__ uint32_t s_tile;
+  if (threadIdx.x == 0) s_tile = atomicAdd(reinterpret_cast<unsigned int*>(a.hdr + kReadyHdrWords), 1u);
+  __syncthreads();
+  const uint32_t tile = s_tile;
+  ready_tile<kTake>(
+      a, tile == gridDim.x - 1,
+      [&](uint32_t k, uint32_t& l, uint32_t& p) {
+        p = tile * kReadyTile + k * kThreads + threadIdx.x;
+        if (p >= a.n) return false;
+        l = walk_mailbox(first, a.n, rot, p);
+        return true;
+      },
+      [&](LbCount agg) { return lookback(a.hdr + kReadyLbOffset, tile, agg); });
 }
 
-// cpbus_take_ready: the same scan over a lossless bus, reading and moving the take cursors `taken` (one per mailbox); head
-// is read, never written.  The taken runs are copied by drain_ready_gather_kernel.
-__global__ void __launch_bounds__(kThreads) take_ready_scan_kernel(SubCtl* __restrict__ ctl,
-                                                                   unsigned long long* __restrict__ taken, uint32_t first,
-                                                                   uint32_t n, uint32_t rot, uint32_t ring_cap,
-                                                                   uint32_t sub_base, unsigned long long cap,
-                                                                   unsigned long long ready_cap, unsigned long long* lb,
-                                                                   cpbus_ready* __restrict__ ready, uint32_t* __restrict__ slot) {
-  ready_scan<true>(ctl, taken, first, n, rot, ring_cap, 1u, sub_base, cap, ready_cap, lb, ready, slot);
-}
-
-// CPBUS_CFG_SPARSE_DRAINS: the scan of drain_ready_scan_kernel (take = 0) or take_ready_scan_kernel (take = 1) over a
-// candidate list instead of the whole range.  list[i] = {mailbox, its position in the range's cyclic walk}, in ascending
-// position.  One CTA walks the list in tiles of kReadyTile candidates; each tile is numbered as a tile of the dense scan,
-// offset by the totals of the tiles before it, and the tile that holds the first ready candidate that does not fit ends the
-// walk.  A mailbox outside the list holds nothing for the predicate, so the entries, the cursors moved and the header
-// {taken, records, position of the first ready mailbox that did not fit (n: none)} are the dense scan's.
-__global__ void __launch_bounds__(kThreads) ready_list_scan_kernel(SubCtl* __restrict__ ctl,
-                                                                   unsigned long long* __restrict__ taken,
-                                                                   const uint2* __restrict__ list, uint32_t m, uint32_t n,
-                                                                   uint32_t ring_cap, uint32_t lossless, uint32_t take,
-                                                                   uint32_t sub_base, unsigned long long cap,
-                                                                   unsigned long long ready_cap, unsigned long long* hdr,
-                                                                   cpbus_ready* __restrict__ ready, uint32_t* __restrict__ slot) {
-  __shared__ uint32_t s_wr[32];              // per (item, warp) chunk: ready mailboxes, then their exclusive prefix in the tile
-  __shared__ unsigned long long s_wc[32];    // ... and records
-  __shared__ unsigned long long s_base_r, s_base_c, s_tile_r, s_tile_c;
-  __shared__ uint32_t s_stop;
-  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (threadIdx.x == 0) { s_base_r = 0; s_base_c = 0; s_stop = 0; }
+// CPBUS_CFG_SPARSE_DRAINS: the dense scan over a candidate list instead of the whole range.  list[i] = {mailbox, its
+// position in the range's cyclic walk}, in ascending position, m >= 1.  One CTA walks the list in tiles of kReadyTile
+// candidates; each tile is numbered as a tile of the dense scan, offset by the totals of the tiles before it, and the tile
+// that holds the first ready candidate that does not fit ends the walk.  A mailbox outside the list holds nothing for the
+// predicate, so the entries, the cursors moved and the header are the dense scan's.
+template <bool kTake>
+__global__ void __launch_bounds__(kThreads) ready_list_scan_kernel(const ReadyScan a, const uint2* __restrict__ list, uint32_t m) {
+  __shared__ LbCount s_run;                  // the totals of the tiles walked so far
+  if (threadIdx.x == 0) s_run = LbCount{0, 0};
   for (uint32_t t0 = 0; t0 < m; t0 += kReadyTile) {
-    uint32_t loc[kReadyItems], pos[kReadyItems], r_in[kReadyItems];
-    unsigned long long tl[kReadyItems], cur[kReadyItems], hd[kReadyItems], c_in[kReadyItems];
-#pragma unroll
-    for (uint32_t k = 0; k < kReadyItems; k++) {
-      const uint32_t i = t0 + k * kThreads + threadIdx.x;
-      unsigned long long t = 0, h = 0, c = 0;
-      uint32_t l = 0, p = 0;
-      if (i < m) {
-        const uint2 e = list[i];
-        l = e.x; p = e.y;
-        const ulonglong2 th = *reinterpret_cast<const ulonglong2*>(ctl + l);   // {tail, head}
-        t = th.x; h = th.y; c = h;
-        if (take) {
-          const unsigned long long tk = taken[l];
-          if (tk > c) c = tk;
-        } else if (!lossless && t > ring_cap && t - ring_cap > c) {
-          c = t - ring_cap;   // overwritten before being taken
-        }
-      }
-      loc[k] = l; pos[k] = p; tl[k] = t; hd[k] = h; cur[k] = c;
-      uint32_t r = t != c ? 1u : 0u;
-      unsigned long long s = t - c;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t ro = __shfl_up_sync(0xffffffffu, r, o);
-        const unsigned long long so = shfl64(s, (int)lane - o);
-        if ((int)lane >= o) { r += ro; s += so; }
-      }
-      r_in[k] = r; c_in[k] = s;
-      if (lane == 31) { s_wr[k * kWarpsPerCta + warp] = r; s_wc[k * kWarpsPerCta + warp] = s; }
-    }
-    __syncthreads();
-    if (warp == 0) {
-      const uint32_t r0 = s_wr[lane];
-      const unsigned long long c0 = s_wc[lane];
-      uint32_t r = r0;
-      unsigned long long c = c0;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t ro = __shfl_up_sync(0xffffffffu, r, o);
-        const unsigned long long co = shfl64(c, (int)lane - o);
-        if ((int)lane >= o) { r += ro; c += co; }
-      }
-      s_wr[lane] = r - r0; s_wc[lane] = c - c0;
-      if (lane == 31) { s_tile_r = r; s_tile_c = c; }
-    }
-    __syncthreads();
-    const unsigned long long base_r = s_base_r, base_c = s_base_c;
-#pragma unroll
-    for (uint32_t k = 0; k < kReadyItems; k++) {
-      const unsigned long long cnt = tl[k] - cur[k];
-      if (!cnt) continue;
-      const uint32_t chunk = k * kWarpsPerCta + warp;
-      const unsigned long long r = base_r + s_wr[chunk] + r_in[k] - 1;        // entry index among the ready mailboxes
-      const unsigned long long o = base_c + s_wc[chunk] + c_in[k] - cnt;      // first record of the run in `out`
-      if (r < ready_cap && o + cnt <= cap) {
-        ready[r] = cpbus_ready{sub_base + loc[k], (uint32_t)cnt, (uint32_t)o, 0u, take ? 0ull : cur[k] - hd[k]};
-        slot[r] = (uint32_t)(cur[k] & (ring_cap - 1));
-        if (take) taken[loc[k]] = tl[k];
-        else ctl[loc[k]].head = tl[k];
-      } else if (r == 0 || (r - 1 < ready_cap && o <= cap)) {   // its predecessor was taken: this one ends the call
-        hdr[0] = r; hdr[1] = o; hdr[2] = pos[k];
-        s_stop = 1;
-      }
-    }
-    __syncthreads();
-    if (s_stop) return;
-    if (threadIdx.x == 0) { s_base_r += s_tile_r; s_base_c += s_tile_c; }
+    const bool cut = ready_tile<kTake>(
+        a, t0 + kReadyTile >= m,
+        [&](uint32_t k, uint32_t& l, uint32_t& p) {
+          const uint32_t i = t0 + k * kThreads + threadIdx.x;
+          if (i >= m) return false;
+          const uint2 e = list[i];
+          l = e.x; p = e.y;
+          return true;
+        },
+        [&](LbCount agg) {
+          const LbCount ex = s_run;
+          __syncwarp();
+          if ((threadIdx.x & 31) == 0) s_run = LbCount{ex.ready + agg.ready, ex.rec + agg.rec};
+          return ex;
+        });
+    if (__syncthreads_or(cut)) return;
   }
-  if (threadIdx.x == 0) { hdr[0] = s_base_r; hdr[1] = s_base_c; hdr[2] = n; }
 }
 
 // Copies the taken runs: one warp per ready entry, lane pairs per record (each pair writes one whole 32-byte sector), and
@@ -952,16 +912,15 @@ __global__ void __launch_bounds__(kThreads) drain_ready_ticket_gather_kernel(con
 }
 
 // ---- consumer backlog (cpbus_lagging) and the mailboxes a lossless flush waits on (cpbus_blockers) ----------------------
-// Read-only scans over the control blocks.  Each numbers the mailboxes it selects in position order with the single-pass
-// decoupled look-back of drain_ready_scan_kernel, reduced to one count per tile: flag (bits 62-63, kLbAgg / kLbIncl) |
-// selected mailboxes (bits 0-61).  Work buffer `lb`: [0] tile counter, [1] CTAs done, [2] selected mailboxes, [3] position
-// of the first selected mailbox not returned, [kLagSumOffset ..) summary (cpbus_lag_summary), [kLagLbOffset ..) tile status.
+// Read-only scans over the control blocks.  Each numbers the mailboxes it selects in position order with the ready scans'
+// look-back, its count in the ready-mailbox field and none in the record field.  Work buffer `lb`: [0] tile counter, [1]
+// CTAs done, [2] selected mailboxes, [3] position of the first selected mailbox not returned, [kLagSumOffset ..) summary
+// (cpbus_lag_summary), [kLagLbOffset ..) tile status.
 constexpr uint32_t kLagHist = 33;
 constexpr uint32_t kLagSumWords = 5 + kLagHist;   // active, lagging, backlog_total, backlog_max, lost_total, hist[33]
 constexpr uint32_t kLagSumOffset = 8, kLagLbOffset = 48;
 constexpr uint32_t kLagHdrWords = 2 + kLagSumWords;   // handed to the host: {selected, cut position, summary}
 static_assert(kLagSumOffset + kLagSumWords <= kLagLbOffset, "summary words overlap the tile status");
-constexpr unsigned long long kLbCountMask = (1ull << 62) - 1;
 
 // Position order index of every selected item of this thread's kReadyItems items (item k = position
 // tile * kReadyTile + k * kThreads + threadIdx.x).  The last tile writes the total to *total.
@@ -989,24 +948,7 @@ __device__ __forceinline__ void select_compact(const bool (&sel)[kReadyItems], u
     }
     s_cnt[lane] = c - c0;
     const unsigned long long agg = __shfl_sync(0xffffffffu, c, 31);
-    unsigned long long ex = 0;
-    if (tile == 0) {
-      if (lane == 0) *reinterpret_cast<volatile unsigned long long*>(status) = kLbIncl | agg;
-    } else {
-      if (lane == 0) *reinterpret_cast<volatile unsigned long long*>(status + tile) = kLbAgg | agg;
-      for (int pred = (int)tile - 1;; pred -= 32) {
-        const int j = pred - (int)lane;
-        unsigned long long v = kLbIncl;   // before tile 0: an empty inclusive prefix (never summed, tile 0 stops the walk)
-        do {
-          if (j >= 0) v = *reinterpret_cast<volatile unsigned long long*>(status + j);
-        } while (__any_sync(0xffffffffu, (v >> 62) == 0));
-        const uint32_t incl = __ballot_sync(0xffffffffu, (v >> 62) == 2);
-        const uint32_t stop = incl ? (uint32_t)(__ffs(incl) - 1) : 31u;
-        ex += warp_sum64(lane <= stop ? v & kLbCountMask : 0ull);
-        if (incl) break;
-      }
-      if (lane == 0) *reinterpret_cast<volatile unsigned long long*>(status + tile) = kLbIncl | (ex + agg);
-    }
+    const unsigned long long ex = lookback(status, tile, LbCount{agg, 0}).ready;
     if (lane == 0) {
       s_base = ex;
       if (tile == gridDim.x - 1) *total = ex + agg;
@@ -1017,7 +959,7 @@ __device__ __forceinline__ void select_compact(const bool (&sel)[kReadyItems], u
   for (uint32_t k = 0; k < kReadyItems; k++) idx[k] = s_base + s_cnt[k * kWarpsPerCta + warp] + before[k];
 }
 
-// Mailboxes [first, first + n) in cyclic position order from rot (as drain_ready_scan_kernel).  A subscribed mailbox holds
+// Mailboxes [first, first + n) in cyclic position order from rot (as ready_scan_kernel).  A subscribed mailbox holds
 // backlog = tail - cursor records (cursor = head, or in throughput mode max(head, tail - ring_cap)) and has lost cursor -
 // head; it is listed when backlog >= min_backlog.  Entries [0, cap) go straight to the host's mapped buffer `out`; the
 // summary is gathered per CTA in shared memory, added into lb with one atomic per field, and the last CTA to finish hands
@@ -1045,18 +987,14 @@ __global__ void __launch_bounds__(kThreads) lagging_scan_kernel(const SubCtl* __
     const uint32_t p = tile * kReadyTile + k * kThreads + threadIdx.x;
     sel[k] = false; loc[k] = 0; bl[k] = 0; lost[k] = 0;
     if (p < n) {
-      unsigned long long q = (unsigned long long)rot + p;
-      if (q >= n) q -= n;
-      const uint32_t l = first + (uint32_t)q;
-      const ulonglong2 th = *reinterpret_cast<const ulonglong2*>(ctl + l);   // {tail, head}
+      const uint32_t l = walk_mailbox(first, n, rot, p);
+      const MailboxCursor c = mailbox_cursor<false>(ctl, nullptr, l, ring_cap, lossless);
       const uint32_t m = ctl[l].mask;
       if (m & kActiveBit) {
-        unsigned long long c = th.y;
-        if (!lossless && th.x > ring_cap && th.x - ring_cap > c) c = th.x - ring_cap;   // overwritten before being taken
-        const uint32_t b = (uint32_t)(th.x - c);
-        loc[k] = l; bl[k] = b; lost[k] = c - th.y;
+        const uint32_t b = (uint32_t)(c.tail - c.cur);
+        loc[k] = l; bl[k] = b; lost[k] = c.cur - c.head;
         sel[k] = b >= min_backlog;
-        act++; lag += sel[k] ? 1u : 0u; btot += b; ltot += c - th.y; bmax = b > bmax ? b : bmax;
+        act++; lag += sel[k] ? 1u : 0u; btot += b; ltot += c.cur - c.head; bmax = b > bmax ? b : bmax;
         atomicAdd(&s_hist[b ? 32 - __clz(b) : 0], 1u);   // [0] = 0, [k] = [2^(k-1), 2^k)
       }
     }
