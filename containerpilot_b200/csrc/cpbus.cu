@@ -101,6 +101,11 @@ static int rebuild_order(cpbus* b) {
   return CPBUS_OK;
 }
 
+// The ORDERED build (no timer armed, no pair table, at least one filtered subscriber) walks the mask order rebuild_order keeps
+static bool ordered_build(const cpbus* b) {
+  return !(b->n_paired > 0 && b->d_pairs) && !(b->n_timers > 0 && b->K > 0) && b->n_filtered > 0;
+}
+
 constexpr int kFanoutMaxSmem = 200 * 1024;
 
 enum { kLaunchPlain = 0, kLaunchFollow = 1, kLaunchRound = 2 };
@@ -240,7 +245,7 @@ static int launch_fanout(cpbus* b, const cpbus_event* d_src, uint32_t n, uint64_
   const bool pairs_on = b->n_paired > 0 && b->d_pairs;
   p.pairs = pairs_on ? b->d_pairs.get() : nullptr;
   size_t smem = fanout_smem_bytes(p.smem_cap) + (pairs_on ? kPairFilterBytes : 0);   // + the batch's {code, source} presence filter
-  if (!pairs_on && !p.timers_on && b->n_filtered > 0) {
+  if (ordered_build(b)) {
     if (b->order_dirty) { const int rc_order = rebuild_order(b); if (rc_order) return rc_order; }
     if (b->n_order) {
       const uint32_t scale = std::max(1u, (p.n_ev + 128u) / 256u);
@@ -2031,6 +2036,11 @@ int cpbus_stream_round_next(cpbus_stream_t* st) try {
   std::lock_guard<std::recursive_mutex> g(b->follow_mu);
   int ri = 0; bool seed_bus = false;
   int rc = follow_begin(b, cpbus::kRound, &ri, &seed_bus); if (rc) return rc;
+  // The ORDERED build rebuilds its mask order, with a sync of the bus stream, at the first fan-out after a membership
+  // change.  That sync must come before this round's kernels are queued: behind the agree kernel it would wait for offers
+  // that other shards driven by this thread have not queued yet, until the stream timeout.  (A membership change resolves
+  // every outstanding round, so nothing of this bus is waiting here when the order is stale.)
+  if (b->order_dirty && ordered_build(b) && (rc = rebuild_order(b))) return rc;
   const bool seed_cur = st->follow_out == 0;   // likewise the stream's cursor, while none of this stream's rounds is queued
   RoundParams P{};
   P.dev = b->d_round; P.cur = st->d_cursor; P.rec = b->h_round.dev() + ri;

@@ -440,7 +440,8 @@ class LocalShardedBus:
     in the publisher's memory and the agree kernel — the protocol `ShardedBus(lossless=True)` runs across processes."""
 
     def __init__(self, n_subs_total: int, devices, ring_cap: int = 1024, batch_cap: int = 512, timers_per_sub: int = 0,
-                 digest: bool = True, stream_slots: int = 64, lossless: bool = False, agree: str = "host"):
+                 digest: bool = True, stream_slots: int = 64, lossless: bool = False, agree: str = "host",
+                 store_path: int = nat.STORE_AUTO, grid_ctas: int = 0):
         if agree not in ("host", "device"):
             raise ValueError(f"agree must be 'host' or 'device', not {agree!r}")
         self.world = len(devices)
@@ -450,7 +451,8 @@ class LocalShardedBus:
         for g, dev in enumerate(devices):
             first, count = shard_range(n_subs_total, self.world, g)
             self.shards.append((first, count, Bus(max(count, 1), ring_cap=ring_cap, batch_cap=batch_cap, timers_per_sub=timers_per_sub,
-                                                  lossless=lossless, digest=digest, device=dev, sub_id_base=first)))
+                                                  lossless=lossless, digest=digest, device=dev, sub_id_base=first,
+                                                  store_path=store_path, grid_ctas=grid_ctas)))
         pub = self.shards[0][2]
         st0, _ = pub.stream_create(stream_slots, self.world)
         self._st = [st0] + [self.shards[g][2].stream_attach(st0, g) for g in range(1, self.world)]

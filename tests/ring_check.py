@@ -44,6 +44,7 @@ def fleet_views(ptrs: dict, n_subs: int, ring_cap: int):
 
 class FleetModel:
     """What a fresh bus (tails at 0, subscribers 0..n_subs-1 subscribed in order, never unsubscribed) was given.
+    Mailbox i holds global id sub_id_base + i (a shard of a sharded bus): unicast records and tick targets use that id.
 
     records: EVENT_DTYPE array in publish order, as the rings hold them (seq, ts, code, source_id, target, flags), ts
         non-decreasing; batches: [(first, end, watermark)] in order, how they reached the bus (for the oracle).
@@ -52,8 +53,8 @@ class FleetModel:
     timers: one dict per timer slot, in slot order: period (uint64 [n]), source (uint32 [n]), oneshot (bool); every timer
         armed at clock 0 on every subscriber."""
 
-    def __init__(self, n_subs, ring_cap, records, batches, masks, pair_shapes=None, shape_of=None, timers=()):
-        self.n, self.R = n_subs, ring_cap
+    def __init__(self, n_subs, ring_cap, records, batches, masks, pair_shapes=None, shape_of=None, timers=(), sub_id_base=0):
+        self.n, self.R, self.base = n_subs, ring_cap, sub_id_base
         self.records, self.batches = np.ascontiguousarray(records), list(batches)
         assert (np.diff(self.records["ts_ns"].astype(np.int64)) >= 0).all(), "records must be in clock order"
         self.watermark = max([int(w) for _, _, w in self.batches] + [int(self.records["ts_ns"].max(initial=0))])
@@ -86,10 +87,10 @@ class FleetModel:
         return max(1, min(self.n, 1 << max(0, (2 ** 25 // max(1, len(self.records))).bit_length() - 1)))
 
     def expected(self, g0: int, g1: int, device):
-        """(count [C], image int64 [C * R, 4], written bool [C * R]) of mailboxes [g0, g1)"""
+        """(count [C], image int64 [C * R, 4], written bool [C * R]) of mailboxes [g0, g1) (indices, not global ids)"""
         d, R, C = self._on(device), self.R, g1 - g0
         rec, E = d["rec"], len(self.records)
-        gid = torch.arange(g0, g1, device=device, dtype=torch.int64)
+        gid = torch.arange(self.base + g0, self.base + g1, device=device, dtype=torch.int64)
         ts = rec[:, 1].contiguous()
         match = (((d["masks"][g0:g1, None] >> d["mask_bit"][None, :]) & 1) != 0) & d["bcast"][None, :]
         if "shape_match" in d:
@@ -135,40 +136,43 @@ class FleetModel:
             written[at] = True
         return count, image, written
 
-    def window(self, gid: int, device="cpu") -> np.ndarray:
-        """the reference's last min(count, R) records of one mailbox, oldest first"""
-        count, image, _ = self.expected(gid, gid + 1, device)
+    def window(self, i: int, device="cpu") -> np.ndarray:
+        """the reference's last min(count, R) records of mailbox i, oldest first"""
+        count, image, _ = self.expected(i, i + 1, device)
         c = int(count[0])
         slots = torch.arange(max(0, c - self.R), c, device=device) & (self.R - 1)
         return image[slots].cpu().numpy().view(ob.EVENT_DTYPE).reshape(-1)
 
-    def oracle_for_one(self, gid: int) -> ob.Oracle:
-        """the C oracle's view of ONE mailbox: a 1-subscriber oracle at sub_id_base = gid, fed the same batches"""
+    def oracle_for_one(self, i: int) -> ob.Oracle:
+        """the C oracle's view of mailbox i alone: a 1-subscriber oracle at sub_id_base = its global id, fed the same
+        batches"""
+        gid = self.base + i
         orc = ob.Oracle(1, timers_per_sub=len(self.timers), keep_window=self.R, sub_id_base=gid)
         pairs = None
         if self.pair_shapes is not None:
-            rows = self.pair_shapes[self.shape_of[gid]]
+            rows = self.pair_shapes[self.shape_of[i]]
             pairs = [(int(c), int(s)) for c, s in rows if c != 0xFFFFFFFF]
-        orc.subscribe(int(self.masks[gid]), pairs)
+        orc.subscribe(int(self.masks[i]), pairs)
         for tm in self.timers:
-            orc.timer_add(gid, int(tm["period"][gid]), int(tm["source"][gid]), bool(tm["oneshot"]))
+            orc.timer_add(gid, int(tm["period"][i]), int(tm["source"][i]), bool(tm["oneshot"]))
         for a, b, w in self.batches:
             assert orc.publish_records(self.records[a:b], int(w)) == 0
         return orc
 
-    def pin(self, gids):
-        """the reference against the C oracle on sampled mailboxes: it is not a second unchecked implementation"""
-        for gid in gids:
-            orc = self.oracle_for_one(int(gid))
-            want = orc.mailbox(int(gid))
-            got = self.window(int(gid))
-            assert len(got) == min(orc.count(int(gid)), self.R), f"reference count at mailbox {gid}"
+    def pin(self, mailboxes):
+        """the reference against the C oracle on sampled mailboxes (indices): it is not a second unchecked implementation"""
+        for i in mailboxes:
+            i, gid = int(i), self.base + int(i)
+            orc = self.oracle_for_one(i)
+            want = orc.mailbox(gid)
+            got = self.window(i)
+            assert len(got) == min(orc.count(gid), self.R), f"reference count at mailbox {gid}"
             assert got.tobytes() == want.tobytes(), f"reference window differs from the oracle at mailbox {gid}"
 
 
 def check(views, model: FleetModel) -> int:
     """Every mailbox: tail == expected count, and every slot the reference writes equals the ring word for word.
-    Raises AssertionError naming the first mailbox, slot and word that differ.  Returns the slots compared."""
+    Raises AssertionError naming the first mailbox (by global id), slot and word that differ.  Returns the slots compared."""
     ring, ctl = views
     R, C, compared = model.R, model.chunk(), 0
     for g0 in range(0, model.n, C):
@@ -178,12 +182,12 @@ def check(views, model: FleetModel) -> int:
         bad = (tail != count).nonzero()
         if len(bad):
             i = int(bad[0])
-            raise AssertionError(f"mailbox {g0 + i}: tail {int(tail[i])}, expected count {int(count[i])}")
+            raise AssertionError(f"mailbox {model.base + g0 + i}: tail {int(tail[i])}, expected count {int(count[i])}")
         diff = (ring[g0:g1].reshape(-1, 4) != image) & written[:, None]
         if bool(diff.any()):
             at, w = (int(x) for x in diff.nonzero()[0])
             got = int(ring[g0:g1].reshape(-1, 4)[at, w])
-            raise AssertionError(f"mailbox {g0 + at // R} slot {at % R} word {w}: ring {got & (2**64 - 1):#018x}, "
+            raise AssertionError(f"mailbox {model.base + g0 + at // R} slot {at % R} word {w}: ring {got & (2**64 - 1):#018x}, "
                                  f"expected {int(image[at, w]) & (2**64 - 1):#018x}")
         compared += int(written.sum())
         free = torch.cuda.mem_get_info()[0]
